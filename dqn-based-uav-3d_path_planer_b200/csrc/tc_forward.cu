@@ -118,7 +118,8 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
 // FUSE_ENV: after a tile's actions are written, the same CTA steps those R envs (env_block.cuh) -- the act -> step
 // dependency is per env, so no grid-wide boundary is needed between Trainer.get_action and BaseEnv.Move_Agent.
 // ACT (a.mode == kTcAct) and DUELING are compile-time: the kernel a pass runs carries no code of the other modes.
-template <bool FUSE_ENV, bool ACT, bool DUELING>
+// FIXED: every layer product is one unbroken compile-time wgmma chain (wgmma.cuh mma_fixed; tc_fixed_chains).
+template <bool FUSE_ENV, bool ACT, bool DUELING, bool FIXED>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, TcArgs a, EnvFuse ef)
 {
     TC_TRACE(0);
@@ -236,7 +237,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
 
         for (int l = 0; l < tc.n_layers; ++l) {
             const TcLayer T = tc.L[l];
-            mma_3xtf32(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
+            mma_3xtf32<kMmaFwd, FIXED>(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
             TC_TRACE(5 + 3 * l);
             if (!w2ready) { if (w_split < (uint32_t)tc.img_bytes) mbar_wait(&wbar2, 0); w2ready = true; }   // biases + the next layers' weights
             TC_TRACE(6 + 3 * l);
@@ -244,21 +245,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
             const int row = quad * 32 + lane;
             const bool live = quad * 32 < R;                       // this warp's rows are real rows
             if (l + 1 < tc.n_layers) {
-                // hidden layer epilogue: bias + ReLU, re-split, write the next A operand (K_next = N_pad)
+                // hidden layer epilogue on every thread (EpiSlice): bias + ReLU, re-split, write the next A operand (K_next = N_pad)
                 const uint32_t sbon = mma_sbo(T.N_pad);
-                for (int c0 = half * 32; live && c0 < T.N_pad; c0 += 64) {
-                    float v[32];
-                    acc_ld32(acc, tc.acc_ld, row, c0, v);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float4 h, lo4;
-                        float x0 = fmaxf(v[4 * j + 0] + bias[c0 + 4 * j + 0], 0.f), x1 = fmaxf(v[4 * j + 1] + bias[c0 + 4 * j + 1], 0.f);
-                        float x2 = fmaxf(v[4 * j + 2] + bias[c0 + 4 * j + 2], 0.f), x3 = fmaxf(v[4 * j + 3] + bias[c0 + 4 * j + 3], 0.f);
-                        tf32_split(x0, h.x, lo4.x); tf32_split(x1, h.y, lo4.y); tf32_split(x2, h.z, lo4.z); tf32_split(x3, h.w, lo4.w);
-                        const uint32_t off = mma_off(row, c0 + 4 * j, sbon);
-                        *reinterpret_cast<float4 *>(Ahi + off) = h;
-                        *reinterpret_cast<float4 *>(Alo + off) = lo4;
-                    }
+                const EpiSlice e(R, kTcThreads);
+                for (int c = e.c0; c < T.N_pad; c += e.step) {
+                    const float4 v = e.ld(acc, tc.acc_ld, c);
+                    float4 h, lo4;
+                    const float x0 = fmaxf(v.x + bias[c + 0], 0.f), x1 = fmaxf(v.y + bias[c + 1], 0.f);
+                    const float x2 = fmaxf(v.z + bias[c + 2], 0.f), x3 = fmaxf(v.w + bias[c + 3], 0.f);
+                    tf32_split(x0, h.x, lo4.x); tf32_split(x1, h.y, lo4.y); tf32_split(x2, h.z, lo4.z); tf32_split(x3, h.w, lo4.w);
+                    const uint32_t off = mma_off(e.row, c, sbon);
+                    *reinterpret_cast<float4 *>(Ahi + off) = h;
+                    *reinterpret_cast<float4 *>(Alo + off) = lo4;
                 }
                 fence_proxy_async();
                 __syncthreads();
@@ -330,14 +328,26 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
     TC_TRACE(20);
 }
 
-typedef void (*ForwardKernel)(TcNet, TcArgs, EnvFuse);
-template <bool F, bool A>
-static ForwardKernel pick_fwd_d(bool dueling) { return dueling ? tc_forward_kernel_t<F, A, true> : tc_forward_kernel_t<F, A, false>; }
-// the fused act + env step variant exists for the act mode only
-static ForwardKernel pick_forward_kernel(bool fuse_env, bool act, bool dueling)
+bool tc_fixed_chains(const TcNet &tc, bool train)
 {
-    if (fuse_env) return pick_fwd_d<true, true>(dueling);
-    return act ? pick_fwd_d<false, true>(dueling) : pick_fwd_d<false, false>(dueling);
+    for (int l = 0; l < tc.n_layers; ++l) {
+        const TcLayer &T = tc.L[l];
+        if (!mma_fixed_product(kMmaFwd, T.N_pad, T.K_pad / 8)) return false;
+        if (train && l > 0 && !mma_fixed_product(kMmaDx, T.K_pad, T.N_pad / 8)) return false;
+    }
+    return true;
+}
+
+typedef void (*ForwardKernel)(TcNet, TcArgs, EnvFuse);
+template <bool F, bool A, bool D>
+static ForwardKernel pick_fwd_x(bool fixed) { return fixed ? tc_forward_kernel_t<F, A, D, true> : tc_forward_kernel_t<F, A, D, false>; }
+template <bool F, bool A>
+static ForwardKernel pick_fwd_d(bool dueling, bool fixed) { return dueling ? pick_fwd_x<F, A, true>(fixed) : pick_fwd_x<F, A, false>(fixed); }
+// the fused act + env step variant exists for the act mode only
+static ForwardKernel pick_forward_kernel(bool fuse_env, bool act, bool dueling, bool fixed)
+{
+    if (fuse_env) return pick_fwd_d<true, true>(dueling, fixed);
+    return act ? pick_fwd_d<false, true>(dueling, fixed) : pick_fwd_d<false, false>(dueling, fixed);
 }
 
 int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st, const EnvFuse *fuse)
@@ -366,10 +376,10 @@ int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st, con
     memset(&ef, 0, sizeof(ef));
     if (fuse) {
         ef = *fuse;
-        UAVRL_CUDA(launch_kernel(pick_forward_kernel(true, a.mode == kTcAct, l->tc.dueling != 0), dim3(grid), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
+        UAVRL_CUDA(launch_kernel(pick_forward_kernel(true, a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
         l->pdl_prev = l->pdl_chain ? kPdlEnv : kPdlNone;
     } else {
-        UAVRL_CUDA(launch_kernel(pick_forward_kernel(false, a.mode == kTcAct, l->tc.dueling != 0), dim3(grid), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
+        UAVRL_CUDA(launch_kernel(pick_forward_kernel(false, a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
         l->pdl_prev = l->pdl_chain ? (a.mode == kTcAct ? kPdlAct : kPdlTd) : kPdlNone;
     }
     UAVRL_LAUNCHED();
@@ -405,20 +415,21 @@ int tc_init(uavrl_learner *l)
     }
     UAVRL_CUDA(cudaMalloc((void **)&l->y_buf, (size_t)l->cfg.batch_size * 4));
     UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->cfg.batch_size * 4));
+    const bool fixed = tc_fixed_chains(l->tc, false);
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du)
-            UAVRL_CUDA(cudaFuncSetAttribute(pick_forward_kernel(false, ac != 0, du != 0), cudaFuncAttributeMaxDynamicSharedMemorySize,
+            UAVRL_CUDA(cudaFuncSetAttribute(pick_forward_kernel(false, ac != 0, du != 0, fixed), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             (int)tc_smem_bytes(l->tc)));
     {   // the fused act+step variant carries the env scratch as static shared memory on top: it must still fit one CTA
         l->fuse_ok = true;
         for (int du = 0; du < 2; ++du) {
             cudaFuncAttributes fa;
-            UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_forward_kernel(true, true, du != 0)));
+            UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_forward_kernel(true, true, du != 0, fixed)));
             if (fa.sharedSizeBytes + tc_smem_bytes(l->tc) > (size_t)227 * 1024) l->fuse_ok = false;
         }
         if (l->fuse_ok)
             for (int du = 0; du < 2; ++du)
-                UAVRL_CUDA(cudaFuncSetAttribute(pick_forward_kernel(true, true, du != 0), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                UAVRL_CUDA(cudaFuncSetAttribute(pick_forward_kernel(true, true, du != 0, fixed), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                 (int)tc_smem_bytes(l->tc)));
     }
     l->y_cap = l->cfg.batch_size;

@@ -7,7 +7,7 @@
 
 namespace uavrl {
 
-constexpr int kTcThreads = 256;        // 2 warpgroups (m64 each); in the epilogues warp w owns rows 32*(w%4).., two warps share them
+constexpr int kTcThreads = 256;        // 2 warpgroups (m64 each); the head epilogue: warp w owns rows 32*(w%4).. (warps 0-3)
 constexpr int kTcTile = 128;           // samples per CTA tile (two m64 warpgroup MMAs)
 
 enum TcMode { kTcAct = 0, kTcArgmax = 1, kTcTdMax = 2, kTcTdGather = 3 };
@@ -39,6 +39,9 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
 // the TD-target pass(es) can run inside the training kernel (one tile per CTA): no separate launch_tc_forward TD calls
 bool tc_train_can_fuse_td(const uavrl_learner *l, int B);
 size_t tc_smem_bytes(const TcNet &tc);
+// every layer product (train: also those of the dX chain) has a compile-time wgmma chain (wgmma.cuh mma_fixed): the kernels'
+// FIXED variants apply
+bool tc_fixed_chains(const TcNet &tc, bool train);
 // the env step fused behind the act pass (tc_forward.cu): env batch + where the step writes
 struct EnvFuse { EnvDev d; float *obs_next; float *reward; uint8_t *done; };
 int launch_tc_forward(uavrl_learner *l, const TcArgs &a, cudaStream_t st, const EnvFuse *fuse = nullptr);

@@ -152,7 +152,8 @@ __device__ __forceinline__ uint32_t nl_split(const TcNet &tc) { return tc.n_laye
 // NPRE / DUELING are compile-time so that the kernel a configuration runs carries no code of the others: a third of the
 // live warps' stall samples of the generic kernel were instruction-fetch stalls (143 KB of code, executed once per CTA).
 // NPRE = forward-only TD passes ahead of the training chain (0: y comes from stand-alone passes, 1: DQN, 2: double DQN).
-template <int NPRE, bool DUELING>
+// FIXED: every layer product, forward and dX, is one unbroken compile-time wgmma chain (wgmma.cuh mma_fixed; tc_fixed_chains).
+template <int NPRE, bool DUELING, bool FIXED>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTrainArgs a)
 {
     TR_TRACE(0);
@@ -206,10 +207,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
     Philox::gen(a.src.key, a.src.epoch, 0x5A17ull, pkey);
     bool wready = false;
     const int nl = tc.n_layers;
-    const int row = quad * 32 + lane;
+    const int row = quad * 32 + lane;                        // the head epilogues: one sample row per thread of warps 0-3
     const bool live = quad * 32 < R;
-    // ReLU' for the dX chain: bit j of hmK = (H_K[row][half * 32 + j] > 0), kept from the forward epilogue of the same thread
-    // (hidden layers are at most 64 wide here: one 32-column chunk per thread) -- no reload of H from global memory
+    // the hidden-layer and dX epilogues run on every thread: row e.row, 4-column groups e.c0 + i * e.step (i = 0, 1, ...)
+    const EpiSlice e(R, kTcThreads);
+    // ReLU' for the dX chain: bit 4i + j of hmK = (H_K[e.row][e.c0 + i * e.step + j] > 0), kept from the forward epilogue of the
+    // same thread (hidden layers are at most 64 wide and R <= 64 here: at most 16 elements per thread) -- no reload of H
     uint32_t hm1 = 0u, hm2 = 0u, hm3 = 0u, hm4 = 0u;
 
     for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
@@ -259,23 +262,19 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
             const bool td_pass = (pass == n_pre - 1);
             for (int l = 0; l < nl; ++l) {
                 const TcLayer T = tc.L[l];
-                mma_3xtf32(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
+                mma_3xtf32<kMmaFwd, FIXED>(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
                 const float *bias = bias_all + T.bias_off;
                 if (l + 1 < nl) {
                     const uint32_t sbon = mma_sbo(T.N_pad);
-                    for (int c0 = half * 32; live && c0 < T.N_pad; c0 += 64) {
-                        float v[32];
-                        acc_ld32(acc, tc.acc_ld, row, c0, v);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            float4 x, h, lo4;
-                            x.x = fmaxf(v[4 * j + 0] + bias[c0 + 4 * j + 0], 0.f); x.y = fmaxf(v[4 * j + 1] + bias[c0 + 4 * j + 1], 0.f);
-                            x.z = fmaxf(v[4 * j + 2] + bias[c0 + 4 * j + 2], 0.f); x.w = fmaxf(v[4 * j + 3] + bias[c0 + 4 * j + 3], 0.f);
-                            tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
-                            const uint32_t off = mma_off(row, c0 + 4 * j, sbon);
-                            *reinterpret_cast<float4 *>(Ahi + off) = h;
-                            *reinterpret_cast<float4 *>(Alo + off) = lo4;
-                        }
+                    for (int c = e.c0; c < T.N_pad; c += e.step) {
+                        const float4 v = e.ld(acc, tc.acc_ld, c);
+                        float4 x, h, lo4;
+                        x.x = fmaxf(v.x + bias[c + 0], 0.f); x.y = fmaxf(v.y + bias[c + 1], 0.f);
+                        x.z = fmaxf(v.z + bias[c + 2], 0.f); x.w = fmaxf(v.w + bias[c + 3], 0.f);
+                        tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
+                        const uint32_t off = mma_off(e.row, c, sbon);
+                        *reinterpret_cast<float4 *>(Ahi + off) = h;
+                        *reinterpret_cast<float4 *>(Alo + off) = lo4;
                     }
                 } else if (half == 0 && live) {
                     float q[32];
@@ -327,38 +326,36 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         fence_proxy_async();
         __syncthreads();
         TR_TRACE(10);
-        const int gb = base + row;                          // this thread's sample (valid when live && gb < B)
+        const int gb = base + row;                          // this thread's sample in the head epilogue (valid when live && gb < B)
         const bool mine = live && gb < a.B;
+        const int egb = base + e.row;                       // ... and in the hidden-layer / dX epilogues
+        const bool emine = egb < a.B;
 
         // ---------------- forward chain
         for (int l = 0; l < nl; ++l) {
             const TcLayer T = tc.L[l];
-            mma_3xtf32(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
+            mma_3xtf32<kMmaFwd, FIXED>(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
             if (fused && l == 0 && w_split < (uint32_t)tc.img_bytes) mbar_wait(&wbar2, 0);     // biases + the later layers' weights
             if (l < 4) TR_TRACE(27 + l);
             const float *bias = bias_all + T.bias_off;
             if (l + 1 < nl) {
                 const uint32_t sbon = mma_sbo(T.N_pad);
-                float *act_row = a.act_buf + (size_t)gb * tc.act_stride + tc.L[l + 1].act_off;
-                for (int c0 = half * 32; live && c0 < T.N_pad; c0 += 64) {
-                    float v[32];
-                    acc_ld32(acc, tc.acc_ld, row, c0, v);
-                    uint32_t mk = 0u;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float4 x, h, lo4;
-                        x.x = fmaxf(v[4 * j + 0] + bias[c0 + 4 * j + 0], 0.f); x.y = fmaxf(v[4 * j + 1] + bias[c0 + 4 * j + 1], 0.f);
-                        x.z = fmaxf(v[4 * j + 2] + bias[c0 + 4 * j + 2], 0.f); x.w = fmaxf(v[4 * j + 3] + bias[c0 + 4 * j + 3], 0.f);
-                        tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
-                        const uint32_t off = mma_off(row, c0 + 4 * j, sbon);
-                        *reinterpret_cast<float4 *>(Ahi + off) = h;
-                        *reinterpret_cast<float4 *>(Alo + off) = lo4;
-                        if (mine) *reinterpret_cast<float4 *>(act_row + c0 + 4 * j) = x;      // kept for dW
-                        mk |= ((x.x > 0.f ? 1u : 0u) | (x.y > 0.f ? 2u : 0u) | (x.z > 0.f ? 4u : 0u) | (x.w > 0.f ? 8u : 0u)) << (4 * j);
-                    }
-                    if (!mine) mk = 0u;
-                    if (l == 0) hm1 = mk; else if (l == 1) hm2 = mk; else if (l == 2) hm3 = mk; else hm4 = mk;
+                float *act_row = a.act_buf + (size_t)egb * tc.act_stride + tc.L[l + 1].act_off;
+                uint32_t mk = 0u;
+                for (int c = e.c0, sh = 0; c < T.N_pad; c += e.step, sh += 4) {
+                    const float4 v = e.ld(acc, tc.acc_ld, c);
+                    float4 x, h, lo4;
+                    x.x = fmaxf(v.x + bias[c + 0], 0.f); x.y = fmaxf(v.y + bias[c + 1], 0.f);
+                    x.z = fmaxf(v.z + bias[c + 2], 0.f); x.w = fmaxf(v.w + bias[c + 3], 0.f);
+                    tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
+                    const uint32_t off = mma_off(e.row, c, sbon);
+                    *reinterpret_cast<float4 *>(Ahi + off) = h;
+                    *reinterpret_cast<float4 *>(Alo + off) = lo4;
+                    if (emine) *reinterpret_cast<float4 *>(act_row + c) = x;      // kept for dW
+                    mk |= ((x.x > 0.f ? 1u : 0u) | (x.y > 0.f ? 2u : 0u) | (x.z > 0.f ? 4u : 0u) | (x.w > 0.f ? 8u : 0u)) << sh;
                 }
+                if (!emine) mk = 0u;
+                if (l == 0) hm1 = mk; else if (l == 1) hm2 = mk; else if (l == 2) hm3 = mk; else hm4 = mk;
             } else {
                 // head: Q(s, .), loss, dLoss/dHead -> next A operand (K = 32) and the dz scratch
                 const uint32_t sbon = mma_sbo(T.N_pad);
@@ -435,30 +432,23 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         // ---------------- dX chain: dZ_{l-1} = (dZ_l * W_l) .* (H_l > 0), l = nl-1 .. 1
         for (int l = nl - 1; l >= 1; --l) {
             const TcLayer T = tc.L[l];
-            mma_3xtf32(acc, tc.acc_ld, Ahi, Alo, W + T.t_hi_off, W + T.t_lo_off, mma_sbo(T.N_pad), T.K_pad, T.N_pad / 8, R);
-            // ReLU'(H_l): the sign mask this thread kept in the forward epilogue (K_pad <= 64: one 32-column chunk per thread)
+            mma_3xtf32<kMmaDx, FIXED>(acc, tc.acc_ld, Ahi, Alo, W + T.t_hi_off, W + T.t_lo_off, mma_sbo(T.N_pad), T.K_pad, T.N_pad / 8, R);
+            // ReLU'(H_l): the sign mask this thread kept in the forward epilogue of the same columns (K_pad(l) = N_pad(l - 1))
             const uint32_t hmask = (l == 1) ? hm1 : (l == 2) ? hm2 : (l == 3) ? hm3 : hm4;
             const uint32_t sbon = mma_sbo(T.K_pad);
-            float *dz_row = a.dz_buf + (size_t)gb * tc.dz_stride + tc.L[l - 1].dz_off;
-            {
-                const int c0 = half * 32;
-                if (live && c0 < T.K_pad) {
-                    float v[32];
-                    acc_ld32(acc, tc.acc_ld, row, c0, v);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const uint32_t m4 = hmask >> (4 * j);
-                        float4 x, h, lo4;
-                        x.x = (m4 & 1u) ? v[4 * j + 0] : 0.f; x.y = (m4 & 2u) ? v[4 * j + 1] : 0.f;
-                        x.z = (m4 & 4u) ? v[4 * j + 2] : 0.f; x.w = (m4 & 8u) ? v[4 * j + 3] : 0.f;
-                        if (mine) *reinterpret_cast<float4 *>(dz_row + c0 + 4 * j) = x;
-                        if (l > 1) {
-                            tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
-                            const uint32_t off = mma_off(row, c0 + 4 * j, sbon);
-                            *reinterpret_cast<float4 *>(Ahi + off) = h;
-                            *reinterpret_cast<float4 *>(Alo + off) = lo4;
-                        }
-                    }
+            float *dz_row = a.dz_buf + (size_t)egb * tc.dz_stride + tc.L[l - 1].dz_off;
+            for (int c = e.c0, sh = 0; c < T.K_pad; c += e.step, sh += 4) {
+                const float4 v = e.ld(acc, tc.acc_ld, c);
+                const uint32_t m4 = hmask >> sh;
+                float4 x, h, lo4;
+                x.x = (m4 & 1u) ? v.x : 0.f; x.y = (m4 & 2u) ? v.y : 0.f;
+                x.z = (m4 & 4u) ? v.z : 0.f; x.w = (m4 & 8u) ? v.w : 0.f;
+                if (emine) *reinterpret_cast<float4 *>(dz_row + c) = x;
+                if (l > 1) {
+                    tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
+                    const uint32_t off = mma_off(e.row, c, sbon);
+                    *reinterpret_cast<float4 *>(Ahi + off) = h;
+                    *reinterpret_cast<float4 *>(Alo + off) = lo4;
                 }
             }
             fence_proxy_async();
@@ -722,9 +712,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
 }
 
 typedef void (*TrainKernel)(TcNet, TcTrainArgs);
+template <int N, bool D>
+static TrainKernel pick_train_x(bool fixed) { return fixed ? tc_train_kernel<N, D, true> : tc_train_kernel<N, D, false>; }
 template <int N>
-static TrainKernel pick_train_d(bool dueling) { return dueling ? tc_train_kernel<N, true> : tc_train_kernel<N, false>; }
-static TrainKernel pick_train_kernel(int npre, bool dueling) { return npre == 0 ? pick_train_d<0>(dueling) : npre == 1 ? pick_train_d<1>(dueling) : pick_train_d<2>(dueling); }
+static TrainKernel pick_train_d(bool dueling, bool fixed) { return dueling ? pick_train_x<N, true>(fixed) : pick_train_x<N, false>(fixed); }
+static TrainKernel pick_train_kernel(int npre, bool dueling, bool fixed)
+{
+    return npre == 0 ? pick_train_d<0>(dueling, fixed) : npre == 1 ? pick_train_d<1>(dueling, fixed) : pick_train_d<2>(dueling, fixed);
+}
 
 static size_t train_smem_bytes(const TcNet &tc, int R)
 {
@@ -749,7 +744,7 @@ int tc_train_init(uavrl_learner *l)
     if (train_smem_bytes(tc, 32) < (size_t)(32 / 8) * mma_sbo(tc.max_k) + (size_t)8 * mma_sbo(tc.max_k)) return 0;
     for (int np = 0; np < 3; ++np)
         for (int du = 0; du < 2; ++du)
-            UAVRL_CUDA(cudaFuncSetAttribute(pick_train_kernel(np, du != 0), cudaFuncAttributeMaxDynamicSharedMemorySize,
+            UAVRL_CUDA(cudaFuncSetAttribute(pick_train_kernel(np, du != 0, tc_fixed_chains(tc, true)), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             (int)(train_smem_bytes(tc, 64) <= 227 * 1024 ? train_smem_bytes(tc, 64) : train_smem_bytes(tc, 32))));
     UAVRL_CUDA(cudaFuncSetAttribute(tc_dw_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dw_smem_bytes(tc)));
     UAVRL_CUDA(cudaFuncSetAttribute(tc_dw_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dw_smem_bytes(tc)));
@@ -799,7 +794,7 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     if (trace_on) { UAVRL_CUDA(cudaMalloc((void **)&tr, 48 * sizeof(long long))); UAVRL_CUDA(cudaMemset(tr, 0, 48 * sizeof(long long))); a.trace = tr + 16; }
     const bool use_pdl = chain && (fused_td ? (l->pdl_prev == kPdlEnv) : (l->pdl_prev == kPdlTd));
     const int npre = fused_td ? (l->cfg.algo != UAVRL_ALGO_DQN ? 2 : 1) : 0;
-    auto train_fn = pick_train_kernel(npre, tc.dueling != 0);
+    auto train_fn = pick_train_kernel(npre, tc.dueling != 0, tc_fixed_chains(tc, true));
     UAVRL_CUDA(launch_kernel(train_fn, dim3(grid), dim3(kTcThreads), train_smem_bytes(tc, a.R), st, use_pdl, tc, a));
     // experiment (with UAVRL_TC_TRACE): the same launch again, back to back -- the kernel is idempotent, the second run finds
     // its code in the instruction caches, and the stage trace printed below is the second run's

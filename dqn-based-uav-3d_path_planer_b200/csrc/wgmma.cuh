@@ -9,7 +9,8 @@
 // wgmma reads tf32 operands from shared memory K-major only, so every product contracts over the operands' fast index.
 //
 // Accumulators: a warpgroup (128 threads) owns an m64 x N fp32 tile in registers; mma_3xtf32 stages it through a
-// row-major shared-memory tile so that the epilogues read one sample row (32 consecutive columns) per thread.
+// row-major shared-memory tile; the elementwise epilogues read it in 4-column groups spread over every thread (EpiSlice), the
+// head epilogues one sample row (32 consecutive columns) per thread.
 #pragma once
 #include <stdint.h>
 
@@ -88,6 +89,9 @@ template <> __device__ __forceinline__ void wgmma_tf32<64>(float *d, uint64_t a,
 
 // The three TF32 products hi*hi + hi*lo + lo*hi of one K extent (K = 8 * ksteps) into the warpgroup's registers.
 // accumulate == 0: the first product overwrites d.  The next K step is +2*LBO bytes = +16 in the descriptor's address field.
+// With a runtime ksteps ptxas closes the wgmma group every few instructions and re-opens it (C7519: warpgroup.arrive injected),
+// so the layer products of the shipped networks use wgmma_3xtf32_k below; this one serves compile-time K (tc_dw_kernel)
+// and every other network shape.
 template <int N>
 __device__ __forceinline__ void wgmma_3xtf32(float *d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, int ksteps,
                                              uint32_t accumulate)
@@ -103,6 +107,52 @@ __device__ __forceinline__ void wgmma_3xtf32(float *d, uint64_t a_hi, uint64_t a
     fence_operands<N>(d);
 }
 
+// The same products for a compile-time K extent (K = 8 * KS): all 3 * KS wgmma back to back behind one fence, one commit,
+// one wait -- one unbroken chain.
+template <int N, int KS>
+__device__ __forceinline__ void wgmma_3xtf32_k(float *d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo)
+{
+    const uint64_t kStep = (uint64_t)((2 * kMmaLBO) >> 4);
+    fence_operands<N>(d);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KS; ++k) wgmma_tf32<N>(d, a_hi + k * kStep, b_hi + k * kStep, k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int k = 0; k < KS; ++k) wgmma_tf32<N>(d, a_hi + k * kStep, b_lo + k * kStep, 1u);
+#pragma unroll
+    for (int k = 0; k < KS; ++k) wgmma_tf32<N>(d, a_lo + k * kStep, b_hi + k * kStep, 1u);
+    wgmma_commit();
+    wgmma_wait0();
+    fence_operands<N>(d);
+}
+
+// Which layer product a call site issues: the forward chain (A = activations, B = W) or the dX chain (A = dZ, B = W^T).
+enum MmaKind { kMmaFwd = 0, kMmaDx = 1 };
+
+// The (chunk width, k-steps) pairs of the shipped networks (input 100, hidden 64 / 128, head 27 / 28 padded to 32), which the
+// kernels issue as compile-time chains: forward 64-column chunks over the input (13) or a 64 / 128-wide hidden layer (8 / 16)
+// and the 32-column head over a 64-wide hidden layer (8); dX 64-column chunks over the head's 32 or a hidden layer's 64
+// gradients (4 / 8).  Only these pairs, so that each call site carries a few chains and not every combination.
+__host__ __device__ constexpr bool mma_fixed(int kind, int n, int ksteps)
+{
+    return kind == kMmaFwd ? (n == 64 && (ksteps == 13 || ksteps == 8 || ksteps == 16)) || (n == 32 && ksteps == 8)
+                           : n == 64 && (ksteps == 4 || ksteps == 8);
+}
+// every chunk of an N-wide product (64-column chunks, then 32, then 16) is one of the pairs above
+__host__ __device__ constexpr bool mma_fixed_product(int kind, int n, int ksteps)
+{
+    return (n < 64 || mma_fixed(kind, 64, ksteps)) && (n % 64 < 32 || mma_fixed(kind, 32, ksteps)) && n % 32 == 0;
+}
+
+template <int N, int KIND>
+__device__ __forceinline__ void wgmma_3xtf32_fixed(float *d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, int ksteps)
+{
+    if constexpr (mma_fixed(KIND, N, 4)) if (ksteps == 4) wgmma_3xtf32_k<N, 4>(d, a_hi, a_lo, b_hi, b_lo);
+    if constexpr (mma_fixed(KIND, N, 8)) if (ksteps == 8) wgmma_3xtf32_k<N, 8>(d, a_hi, a_lo, b_hi, b_lo);
+    if constexpr (mma_fixed(KIND, N, 13)) if (ksteps == 13) wgmma_3xtf32_k<N, 13>(d, a_hi, a_lo, b_hi, b_lo);
+    if constexpr (mma_fixed(KIND, N, 16)) if (ksteps == 16) wgmma_3xtf32_k<N, 16>(d, a_hi, a_lo, b_hi, b_lo);
+}
+
 // the warpgroup's fragment -> acc[row][col0 + c] (row-major, ld floats per row); rows >= R are not stored
 template <int N>
 __device__ __forceinline__ void store_frag(const float *d, float *acc, int ld, int row0, int col0, int R)
@@ -115,13 +165,18 @@ __device__ __forceinline__ void store_frag(const float *d, float *acc, int ld, i
     }
 }
 
-template <int N>
+// FIXED: the product is one of the pairs above (mma_fixed_product), issued as one unbroken chain.  Otherwise the runtime-K
+// chain; a kernel that has it anywhere gets every chain broken up by ptxas, so the kernels come in both variants
+// and the host picks the FIXED one whenever the network's shape allows.
+template <int N, int KIND, bool FIXED>
 __device__ __forceinline__ void mma_chunk(float *acc, int ld, int row0, int n0, uint64_t a_hi, uint64_t a_lo, const unsigned char *b_hi,
                                           const unsigned char *b_lo, uint32_t sbo, int ksteps, int R)
 {
     float d[N / 2];
     const uint32_t boff = (uint32_t)(n0 >> 3) * sbo;
-    wgmma_3xtf32<N>(d, a_hi, a_lo, mma_desc(b_hi + boff, sbo), mma_desc(b_lo + boff, sbo), ksteps, 0u);
+    const uint64_t bh = mma_desc(b_hi + boff, sbo), bl = mma_desc(b_lo + boff, sbo);
+    if (FIXED) wgmma_3xtf32_fixed<N, KIND>(d, a_hi, a_lo, bh, bl, ksteps);
+    else wgmma_3xtf32<N>(d, a_hi, a_lo, bh, bl, ksteps, 0u);
     store_frag<N>(d, acc, ld, row0, n0, R);
 }
 
@@ -129,6 +184,7 @@ __device__ __forceinline__ void mma_chunk(float *acc, int ld, int row0, int n0, 
 // K extent and so the SBO.  Called by every thread of the CTA (256 = two warpgroups, warpgroup g computes rows [64g, 64g + 64),
 // and only where they hold real rows); ends with a CTA barrier behind which acc is complete.  The operands' generic-proxy
 // writes must have been fenced (fence_proxy_async) and published by a barrier before the call.
+template <int KIND, bool FIXED>
 __device__ __forceinline__ void mma_3xtf32(float *acc, int ld, const unsigned char *a_hi, const unsigned char *a_lo,
                                            const unsigned char *b_hi, const unsigned char *b_lo, uint32_t sbo, int N, int ksteps, int R)
 {
@@ -136,9 +192,9 @@ __device__ __forceinline__ void mma_3xtf32(float *acc, int ld, const unsigned ch
     if (row0 < R) {
         const uint64_t ah = mma_desc(a_hi + (row0 >> 3) * sbo, sbo), al = mma_desc(a_lo + (row0 >> 3) * sbo, sbo);
         int n0 = 0;
-        for (; n0 + 64 <= N; n0 += 64) mma_chunk<64>(acc, ld, row0, n0, ah, al, b_hi, b_lo, sbo, ksteps, R);
-        if (n0 + 32 <= N) { mma_chunk<32>(acc, ld, row0, n0, ah, al, b_hi, b_lo, sbo, ksteps, R); n0 += 32; }
-        if (n0 < N) mma_chunk<16>(acc, ld, row0, n0, ah, al, b_hi, b_lo, sbo, ksteps, R);
+        for (; n0 + 64 <= N; n0 += 64) mma_chunk<64, KIND, FIXED>(acc, ld, row0, n0, ah, al, b_hi, b_lo, sbo, ksteps, R);
+        if (n0 + 32 <= N) { mma_chunk<32, KIND, FIXED>(acc, ld, row0, n0, ah, al, b_hi, b_lo, sbo, ksteps, R); n0 += 32; }
+        if (!FIXED && n0 < N) mma_chunk<16, KIND, FIXED>(acc, ld, row0, n0, ah, al, b_hi, b_lo, sbo, ksteps, R);
     }
     __syncthreads();
 }
@@ -153,5 +209,22 @@ __device__ __forceinline__ void acc_ld32(const float *acc, int ld, int row, int 
         v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
     }
 }
+
+// One thread's share of an elementwise epilogue over the staged R x N accumulator (R = 32 / 64 / 128 rows, nt threads): row
+// t % R, 4-column groups c0, c0 + step, ... (c0 = 4 * (t / R), step = 4 * nt / R).  Every warp of the CTA, on all four
+// scheduler sub-partitions, takes part whatever R is.  Eight consecutive lanes read eight rows of one group (ld = 4 mod 32
+// words: no bank conflict) and write one whole core matrix of the next A operand (128 contiguous bytes).
+struct EpiSlice {
+    int row, c0, step;
+    __device__ __forceinline__ EpiSlice(int R, int nt)
+    {
+        const int lgR = 31 - __clz(R);
+        row = threadIdx.x & (R - 1); c0 = 4 * (threadIdx.x >> lgR); step = 4 * (nt >> lgR);
+    }
+    __device__ __forceinline__ float4 ld(const float *acc, int ld, int c) const
+    {
+        return *reinterpret_cast<const float4 *>(acc + (size_t)row * ld + c);
+    }
+};
 
 }  // namespace uavrl
