@@ -81,6 +81,7 @@ SIGNATURES = {
     "uavrl_set_fuse_dw_adam": (C.c_int, [C.c_int32]),
     "uavrl_set_fuse_td": (C.c_int, [C.c_int32]),
     "uavrl_learner_td_fused": (C.c_int, [C.c_void_p, C.c_int32]),
+    "uavrl_learner_tc_route": (C.c_int, [VP, C.c_int32, VP]),
     "uavrl_env_set_extras": (C.c_int, [VP, VP]),
     "uavrl_env_get_energy": (C.c_int, [VP, VP]),
     "uavrl_env_get_energy_total": (C.c_int, [VP, C.POINTER(C.c_double)]),

@@ -887,6 +887,12 @@ int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out)
     l->cfg = *cfg;
     int rc = build_net(*cfg, l->net);
     if (rc) { delete l; return rc; }
+    // the fp32 kernels hold the whole network in shared memory: refuse a network that does not fit before allocating anything
+    l->dual_weights = upd_smem_bytes(l->net, 1) <= kMaxDynSmem ? 1 : 0;
+    if (upd_smem_bytes(l->net, l->dual_weights) > kMaxDynSmem || act_smem_bytes(l->net) > kMaxDynSmem) {
+        delete l;
+        return fail(UAVRL_ERR_INVALID, "network too large for the shared-memory resident kernels");
+    }
     const size_t P = (size_t)l->net.P;
     l->max_ctas = 4 * num_sms();
     if ((rc = dev_alloc(&l->local, P)) || (rc = dev_alloc(&l->target, P)) || (rc = dev_alloc(&l->m, P)) ||
@@ -900,9 +906,6 @@ int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out)
         std::vector<int32_t> map;
         build_image_map(l->net, map);
         UAVRL_CUDA(cudaMemcpy(l->img_map, map.data(), P * sizeof(int32_t), cudaMemcpyHostToDevice));
-        l->dual_weights = upd_smem_bytes(l->net, 1) <= kMaxDynSmem ? 1 : 0;
-        if (upd_smem_bytes(l->net, l->dual_weights) > kMaxDynSmem || act_smem_bytes(l->net) > kMaxDynSmem)
-            return fail(UAVRL_ERR_INVALID, "network too large for the shared-memory resident kernels");
     }
     if ((rc = tc_init(l))) return rc;
     const size_t in = (size_t)cfg->in_dim;

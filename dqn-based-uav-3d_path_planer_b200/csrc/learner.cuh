@@ -72,6 +72,7 @@ struct TcNet {
     int32_t bias_base;                 // byte offset of the bias area
     int32_t train_img_bytes;           // forward image + transposed blocks (training chain)
     int32_t max_rows;                  // rows of the largest forward tile: 128, or 64 when 128 rows do not fit shared memory
+    int32_t train_max_rows;            // rows of the largest training tile: 64, or 32 when 64 rows do not fit (tc_train_init)
     int32_t a_bytes;                   // bytes of ONE A-operand buffer (hi or lo): max_rows x max K_pad
     int32_t max_k;                     // max K_pad over layers
     int32_t act_stride, dz_stride;     // floats per sample in the activation / derivative scratch

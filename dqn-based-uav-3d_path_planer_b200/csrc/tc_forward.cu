@@ -350,11 +350,17 @@ static ForwardKernel pick_forward_kernel(bool fuse_env, bool act, bool dueling, 
     return act ? pick_fwd_d<false, true>(dueling, fixed) : pick_fwd_d<false, false>(dueling, fixed);
 }
 
+int tc_forward_rows_per_tile(const TcNet &tc, int n)
+{
+    const int n_sm = num_sms();
+    return (n >= 128 * n_sm && tc.max_rows == 128) ? 128 : (n >= 64 * n_sm) ? 64 : 32;
+}
+
 int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st, const EnvFuse *fuse)
 {
     TcArgs a = a_in;
     const int n_sm = num_sms();
-    a.rows_per_tile = (a.n >= 128 * n_sm && l->tc.max_rows == 128) ? 128 : (a.n >= 64 * n_sm) ? 64 : 32;
+    a.rows_per_tile = tc_forward_rows_per_tile(l->tc, a.n);
     a.n_tiles = (a.n + a.rows_per_tile - 1) / a.rows_per_tile;
     const int grid = a.n_tiles < n_sm ? a.n_tiles : n_sm;
     static const bool trace_on = getenv("UAVRL_TC_TRACE") != nullptr;
@@ -400,7 +406,15 @@ int tc_init(uavrl_learner *l)
     std::vector<int32_t> hi, lo, hi2, lo2;
     l->tc_ok = false; l->tc_train_ok = false;
     if (tc_build(l->cfg, l->net, l->tc, hi, lo, hi2, lo2) != 0) return 0;
-    if (tc_smem_bytes(l->tc) > 227 * 1024) return 0;
+    const bool fixed = tc_fixed_chains(l->tc, false);
+    size_t fwd_static = 0;                                       // the kernels' static shared memory (row table, barriers)
+    for (int ac = 0; ac < 2; ++ac)
+        for (int du = 0; du < 2; ++du) {
+            cudaFuncAttributes fa;
+            UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_forward_kernel(false, ac != 0, du != 0, fixed)));
+            if (fa.sharedSizeBytes > fwd_static) fwd_static = fa.sharedSizeBytes;
+        }
+    if (tc_smem_bytes(l->tc) + fwd_static > 227 * 1024) return 0;
     const size_t P = (size_t)l->net.P;
     const size_t img = (size_t)l->tc.train_img_bytes;
     UAVRL_CUDA(cudaMalloc((void **)&l->tc_img_local, img));
@@ -415,7 +429,6 @@ int tc_init(uavrl_learner *l)
     }
     UAVRL_CUDA(cudaMalloc((void **)&l->y_buf, (size_t)l->cfg.batch_size * 4));
     UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->cfg.batch_size * 4));
-    const bool fixed = tc_fixed_chains(l->tc, false);
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du)
             UAVRL_CUDA(cudaFuncSetAttribute(pick_forward_kernel(false, ac != 0, du != 0, fixed), cudaFuncAttributeMaxDynamicSharedMemorySize,

@@ -38,6 +38,9 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
                     float *loss_out = nullptr, bool *adam_done = nullptr, bool fused_td = false);
 // the TD-target pass(es) can run inside the training kernel (one tile per CTA): no separate launch_tc_forward TD calls
 bool tc_train_can_fuse_td(const uavrl_learner *l, int B);
+// rows per tile of an act / TD pass over n samples (launch_tc_forward) and of the training kernel for a batch of B
+int tc_forward_rows_per_tile(const TcNet &tc, int n);
+int train_rows_per_tile(const TcNet &tc, int B);
 size_t tc_smem_bytes(const TcNet &tc);
 // every layer product (train: also those of the dX chain) has a compile-time wgmma chain (wgmma.cuh mma_fixed): the kernels'
 // FIXED variants apply

@@ -735,17 +735,34 @@ static size_t dw_smem_bytes(const TcNet &tc)
 int tc_train_init(uavrl_learner *l)
 {
     l->tc_train_ok = false;
-    const TcNet &tc = l->tc;
+    TcNet &tc = l->tc;
+    tc.train_max_rows = 0;
     for (int i = 0; i < tc.n_layers; ++i)
         if (tc.L[i].K_real + 1 > 128 || tc.L[i].K_real % 4 != 0 || (tc.L[i].N_pad != 32 && tc.L[i].N_pad != 64)) return 0;   // ones column / float4 chunks / 1-2 blocks
+    // a block's 227 KB hold the kernels' static shared memory (sample tables, barriers) as well as the dynamic allocation
+    const bool fixed = tc_fixed_chains(tc, true);
+    size_t train_static = 0, dw_static = 0;
+    for (int np = 0; np < 3; ++np)
+        for (int du = 0; du < 2; ++du) {
+            cudaFuncAttributes fa;
+            UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_train_kernel(np, du != 0, fixed)));
+            if (fa.sharedSizeBytes > train_static) train_static = fa.sharedSizeBytes;
+        }
+    for (int fu = 0; fu < 2; ++fu) {
+        cudaFuncAttributes fa;
+        UAVRL_CUDA(cudaFuncGetAttributes(&fa, fu ? tc_dw_kernel<true> : tc_dw_kernel<false>));
+        if (fa.sharedSizeBytes > dw_static) dw_static = fa.sharedSizeBytes;
+    }
+    const size_t train_budget = (size_t)227 * 1024 - train_static;
     // the m64 MMA reads 8 row groups from each A buffer: with fewer real rows it runs into the next buffers,
     // which must still be inside the CTA's allocation
-    if (train_smem_bytes(tc, 32) > 227 * 1024 || dw_smem_bytes(tc) > 227 * 1024) return 0;
+    if (train_smem_bytes(tc, 32) > train_budget || dw_smem_bytes(tc) + dw_static > (size_t)227 * 1024) return 0;
     if (train_smem_bytes(tc, 32) < (size_t)(32 / 8) * mma_sbo(tc.max_k) + (size_t)8 * mma_sbo(tc.max_k)) return 0;
+    tc.train_max_rows = train_smem_bytes(tc, 64) <= train_budget ? 64 : 32;
     for (int np = 0; np < 3; ++np)
         for (int du = 0; du < 2; ++du)
-            UAVRL_CUDA(cudaFuncSetAttribute(pick_train_kernel(np, du != 0, tc_fixed_chains(tc, true)), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)(train_smem_bytes(tc, 64) <= 227 * 1024 ? train_smem_bytes(tc, 64) : train_smem_bytes(tc, 32))));
+            UAVRL_CUDA(cudaFuncSetAttribute(pick_train_kernel(np, du != 0, fixed), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)train_smem_bytes(tc, tc.train_max_rows)));
     UAVRL_CUDA(cudaFuncSetAttribute(tc_dw_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dw_smem_bytes(tc)));
     UAVRL_CUDA(cudaFuncSetAttribute(tc_dw_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dw_smem_bytes(tc)));
     const size_t cap = (size_t)l->cfg.batch_size;
@@ -758,9 +775,9 @@ int tc_train_init(uavrl_learner *l)
 
 std::atomic<int> g_fuse_td{1};               // uavrl_set_fuse_td(); default on
 // rows per tile of the training kernel: 32 while the batch fits one wave of 32-row tiles, else 64 (when the 64-row operands fit)
-static int train_rows_per_tile(const TcNet &tc, int B)
+int train_rows_per_tile(const TcNet &tc, int B)
 {
-    return (B > 32 * num_sms() && train_smem_bytes(tc, 64) <= 227 * 1024) ? 64 : 32;
+    return (B > 32 * num_sms() && tc.train_max_rows == 64) ? 64 : 32;
 }
 bool tc_train_can_fuse_td(const uavrl_learner *l, int B)
 {
@@ -860,3 +877,16 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
 extern "C" int uavrl_set_fuse_dw_adam(int32_t on) { uavrl::g_fuse_dw_adam.store(on ? 1 : 0); return 0; }
 extern "C" int uavrl_set_fuse_td(int32_t on) { uavrl::g_fuse_td.store(on ? 1 : 0); return 0; }
 extern "C" int uavrl_learner_td_fused(const uavrl_learner *l, int32_t batch) { return (l && l->tc_ok && l->use_tc && uavrl::tc_train_can_fuse_td(l, batch)) ? 1 : 0; }
+// the same decisions launch_act / launch_update_impl take (uavrl.h)
+extern "C" int uavrl_learner_tc_route(const uavrl_learner *l, int32_t n, int32_t *out)
+{
+    if (!l || !out || n <= 0) return uavrl::fail(UAVRL_ERR_INVALID, "bad argument");
+    const bool fwd = l->tc_ok && l->use_tc, train = fwd && l->tc_train_ok;
+    out[0] = fwd ? (uavrl::tc_fixed_chains(l->tc, false) ? 2 : 1) : 0;
+    out[1] = train ? (uavrl::tc_fixed_chains(l->tc, true) ? 2 : 1) : 0;
+    out[2] = fwd ? uavrl::tc_forward_rows_per_tile(l->tc, n) : 0;
+    out[3] = train ? uavrl::train_rows_per_tile(l->tc, n) : 0;
+    out[4] = (train && uavrl::tc_train_can_fuse_td(l, n)) ? 1 : 0;
+    out[5] = l->dual_weights;
+    return 0;
+}

@@ -406,6 +406,18 @@ class Learner:
         """True when an update of `batch` transitions runs its TD-target pass(es) inside the training kernel."""
         return bool(_lib.lib().uavrl_learner_td_fused(self.h, int(self.cfg.batch_size if batch is None else batch)))
 
+    def route(self, n):
+        """Which kernels an act / TD pass over n samples and an update of a batch of n run, with the current
+        set_tensor_cores setting: tc_fwd / tc_train = "fixed" (compile-time wgmma chains), "generic" (runtime k-step
+        chains) or None (the fp32 CUDA-core kernel); fwd_rows / train_rows = rows per tile of those tensor-core kernels
+        (None when not used); td_fused = the TD-target pass(es) run inside the training kernel; fp32_dual = the fp32 update
+        kernel keeps both networks' weights in shared memory at once."""
+        out = (C.c_int32 * 6)()
+        check(_lib.lib().uavrl_learner_tc_route(self.h, int(n), out))
+        variant = {0: None, 1: "generic", 2: "fixed"}
+        return dict(tc_fwd=variant[out[0]], tc_train=variant[out[1]], fwd_rows=out[2] or None, train_rows=out[3] or None,
+                    td_fused=bool(out[4]), fp32_dual=bool(out[5]))
+
     def lockstep_restart(self):
         check(_lib.lib().uavrl_learner_lockstep_restart(self.h))
 

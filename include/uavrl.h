@@ -377,6 +377,12 @@ int uavrl_set_fuse_dw_adam(int32_t on);
 int uavrl_set_fuse_td(int32_t on);
 /* 1 if an update of `batch` transitions on this learner runs the TD-target pass(es) inside the training kernel (see above). */
 int uavrl_learner_td_fused(const uavrl_learner *l, int32_t batch);
+/* Which kernels an act / TD pass over n samples and an update of a batch of n run on this learner, with its current
+ * tensor-core setting.  out[6]: [0] tensor-core act / TD pass, [1] tensor-core training kernel (0 = not used, the fp32
+ * CUDA-core kernel runs; 1 = generic variant, runtime k-step chains; 2 = FIXED variant, compile-time chains); [2] rows per
+ * tile of that act / TD pass, [3] rows per tile of that training kernel (0 when not used); [4] the TD-target pass(es) run
+ * inside the training kernel; [5] the fp32 update kernel keeps both networks' weights in shared memory at once. */
+int uavrl_learner_tc_route(const uavrl_learner *l, int32_t n, int32_t *out);
 
 #ifdef __cplusplus
 }

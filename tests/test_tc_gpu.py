@@ -83,8 +83,11 @@ def test_tc_td_targets_keep_update_parity(dqn_golden, name):
 # ---------------------------------------------------------------------------------------------------------------------
 # The tile variants the large BASELINE configs select (launch_tc_forward: R = 64 rows per tile from n >= 64 x 132,
 # R = 128 from n >= 128 x 132 when 128-row tiles fit shared memory; tc_train: R = 64 from B >= 32 x 132) compared with the oracle by VALUE, ragged last tiles.
-def big_inputs(g, n, rng):
+def big_inputs(g, n, rng, in_dim=100):
+    """n rows of the golden observations (columns cropped or tiled to in_dim) plus noise: occupancy bits and real-valued
+    entries at the scales the learner sees."""
     base = np.concatenate([g["batch_s"].reshape(-1, 100), g["batch_s2"].reshape(-1, 100)])
+    base = np.tile(base, (1, -(-in_dim // 100)))[:, :in_dim]
     x = np.tile(base, (n // base.shape[0] + 1, 1))[:n]
     return (x + rng.normal(0, 0.02, x.shape)).astype(np.float32)
 
@@ -111,29 +114,44 @@ def test_tc_act_large_tiles_vs_oracle(dqn_golden, n, hidden, dueling):
     L.close()
 
 
+def net_layers(in_dim, hidden, n_actions, dueling):
+    """(out, in) of every Linear in state_dict order: the trunk, then fc_A (or the Q head) and fc_V."""
+    dims = [in_dim] + list(hidden)
+    head = [(n_actions, hidden[-1]), (1, hidden[-1])] if dueling else [(n_actions, hidden[-1])]
+    return [(dims[i + 1], dims[i]) for i in range(len(hidden))] + head
+
+
+def f64_unpack(layers, flat):
+    out, off = [], 0
+    for (o, i) in layers:
+        W = flat[off:off + o * i].reshape(o, i).astype(np.float64); off += o * i
+        b = flat[off:off + o].astype(np.float64); off += o
+        out.append((W, b))
+    assert off == flat.size
+    return out
+
+
+def f64_forward(P, dueling, x):
+    """Q(x) of the unpacked float64 network P, and the activations [x, H1, ..] kept for the backward pass."""
+    x = np.asarray(x, np.float64)
+    acts, h = [x], x
+    nt = len(P) - (2 if dueling else 1)
+    for W, b in P[:nt]:
+        h = np.maximum(h @ W.T + b, 0.0); acts.append(h)
+    if dueling:
+        (WA, bA), (WV, bV) = P[nt], P[nt + 1]
+        A = h @ WA.T + bA; V = h @ WV.T + bV
+        return V + A - A.mean(1, keepdims=True), acts
+    W, b = P[nt]
+    return h @ W.T + b, acts
+
+
 def f64_update(layers, algo, dueling, local, target, s, a, r, s2, d, gamma=0.99):
     """The TD update's loss and gradient in float64 numpy (the arbiter between two fp32 implementations whose summation
     orders differ): DQN_Trainer.py:107-124 / DDQN_Trainer.py:93-107 / DuelingDQN_Trainer.py:164-180."""
-    def unpack(flat):
-        out, off = [], 0
-        for (o, i) in layers:
-            W = flat[off:off + o * i].reshape(o, i).astype(np.float64); off += o * i
-            b = flat[off:off + o].astype(np.float64); off += o
-            out.append((W, b))
-        return out
-
     def fwd(P, x):
-        acts, h = [x], x
-        nt = len(P) - (2 if dueling else 1)
-        for W, b in P[:nt]:
-            h = np.maximum(h @ W.T + b, 0.0); acts.append(h)
-        if dueling:
-            (WA, bA), (WV, bV) = P[nt], P[nt + 1]
-            A = h @ WA.T + bA; V = h @ WV.T + bV
-            return V + A - A.mean(1, keepdims=True), acts
-        W, b = P[nt]
-        return h @ W.T + b, acts
-    PL, PT = unpack(local), unpack(target)
+        return f64_forward(P, dueling, x)
+    PL, PT = f64_unpack(layers, local), f64_unpack(layers, target)
     s, s2 = s.astype(np.float64), s2.astype(np.float64)
     B = s.shape[0]
     qt, _ = fwd(PT, s2)
@@ -184,8 +202,7 @@ def test_tc_update_large_batch_vs_oracle(dqn_golden, name, B):
     L.set_params(g[name + "_local0"], 0); L.set_params(g[name + "_target0"], 1)
     OL = O.OracleLearner(net, algo, g[name + "_local0"], update_loop=3)
     OL.target[:] = g[name + "_target0"]
-    dims = [100] + list(hidden)
-    layers = [(dims[i + 1], dims[i]) for i in range(len(hidden))] + ([(27, hidden[-1]), (1, hidden[-1])] if dueling else [(27, hidden[-1])])
+    layers = net_layers(100, hidden, 27, dueling)
     loss = torch.zeros(1, device="cuda")
     noisy = np.zeros(L.P, bool)
     for step in range(4):
