@@ -102,6 +102,8 @@ SIGNATURES = {
     "uavrl_env_set_state": (C.c_int, [VP, C.POINTER(EnvStateHost)]),
     "uavrl_env_threaten_rate": (C.c_int, [VP, C.c_int32, VP, VP]),
     "uavrl_learner_create": (C.c_int, [C.POINTER(LearnerConfig), C.POINTER(VP)]),
+    "uavrl_learner_create_trainers": (C.c_int, [C.POINTER(LearnerConfig), C.c_int32, C.POINTER(VP)]),
+    "uavrl_learner_trainer_count": (C.c_int32, [VP]),
     "uavrl_learner_destroy": (C.c_int, [VP]),
     "uavrl_learner_param_count": (C.c_int64, [VP]),
     "uavrl_learner_set_params": (C.c_int, [VP, C.c_int32, VP]),

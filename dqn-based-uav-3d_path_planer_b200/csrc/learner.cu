@@ -21,6 +21,7 @@
 #include <math.h>
 #include <string.h>
 
+#include <string>
 #include <vector>
 
 namespace uavrl {
@@ -79,9 +80,19 @@ __global__ void __launch_bounds__(kNetThreads)
 act_kernel(NetDev net, const float *__restrict__ params, const float *__restrict__ obs, int n, float eps,
            int is_train, const float *__restrict__ u_tape, const int32_t *__restrict__ rand_tape,
            uint64_t key, uint64_t call, int32_t *__restrict__ actions, int32_t *__restrict__ actions2,
-           float *__restrict__ q_out, int n_tiles)
+           float *__restrict__ q_out, int n_tiles, int img_floats)
 {
     extern __shared__ __align__(16) float smem[];
+    {   // trainer blockIdx.y of a grouped learner: its weight image, its n rows and its eps-greedy key
+        const int g = blockIdx.y;
+        const size_t r0 = (size_t)g * (size_t)n;
+        params += (size_t)g * img_floats; obs += r0 * net.in_dim; actions += r0;
+        if (actions2) actions2 += r0;
+        if (q_out) q_out += r0 * net.n_actions;
+        if (u_tape) u_tape += r0;
+        if (rand_tape) rand_tape += r0;
+        key = trainer_key(key, kActSalt, g);
+    }
     float *sw = smem;
     float *sA = smem + net.smem_total_floats;
     float *sB = sA + kTile * kMaxDim;
@@ -127,6 +138,7 @@ struct UpdateArgs {
     const float *img_local, *img_target;
     float *partials, *loss_partials;
     int B, n_tiles, algo, dual, loss_kind;
+    int img_floats;                    // grouped learner: per-trainer stride of the weight images
     float gamma, inv_global_b;
     const float *y_in;                 // non-null: TD targets already computed (tensor-core pass); skip the target net
 };
@@ -154,7 +166,16 @@ update_kernel(NetDev net, BatchSrc src, UpdateArgs ua)
     __shared__ float s_rew[kTile], s_done[kTile], s_loss[kTile];
     __shared__ uint64_t barL, barT;
 
-    float *gpart = ua.partials + (size_t)blockIdx.x * net.P;
+    // trainer blockIdx.y of a grouped learner: its B samples, weight images and partial slots [G][gridDim.x]
+    const int grp = blockIdx.y;
+    src = trainer_src(src, grp, ua.B, net.in_dim);
+    {
+        const size_t wo = (size_t)grp * ua.img_floats;
+        ua.img_local += wo; ua.img_target += wo;
+        if (ua.y_in) ua.y_in += (size_t)grp * ua.B;
+    }
+    const size_t part = (size_t)grp * gridDim.x + blockIdx.x;
+    float *gpart = ua.partials + part * net.P;
     float loss_acc = 0.f;
     int iter = 0;
     uint32_t pkey[4];
@@ -266,7 +287,7 @@ update_kernel(NetDev net, BatchSrc src, UpdateArgs ua)
             float *tmp = dY; dY = dXb; dXb = tmp;
         }
     }
-    if (threadIdx.x == 0) ua.loss_partials[blockIdx.x] = loss_acc;
+    if (threadIdx.x == 0) ua.loss_partials[part] = loss_acc;
 }
 
 // ------------------------------------------------------------------ reduce partials + Adam + target copy
@@ -284,6 +305,14 @@ reduce_adam_kernel(AdamArgs a, const float *__restrict__ partials, const float *
     __shared__ float red[4][64];
     const int ix = threadIdx.x & 63, cg = threadIdx.x >> 6;
     const int i = blockIdx.x * 64 + ix;
+    {   // trainer blockIdx.y of a grouped learner: its partials [nparts][P], vectors [P], images and loss
+        const size_t g = blockIdx.y, gp = g * (size_t)a.P;
+        partials += gp * (size_t)a.nparts; loss_partials += g * (size_t)a.n_loss_parts;
+        grad += gp; local += gp; m += gp; v += gp; target += gp;
+        img_local += g * (size_t)a.img_floats; img_target += g * (size_t)a.img_floats;
+        if (tc_local) { tc_local += g * (size_t)a.tc_floats; tc_target += g * (size_t)a.tc_floats; }
+        if (loss_out) loss_out += g;
+    }
     AdamPtrs q;
     q.partials = partials; q.loss_partials = loss_partials; q.grad = grad; q.local = local; q.m = m; q.v = v; q.target = target;
     q.img_local = img_local; q.img_target = img_target; q.img_map = img_map; q.tc_local = tc_local; q.tc_target = tc_target;
@@ -553,10 +582,14 @@ __global__ void gather_kernel(int n, int in, BatchSrc src, const int64_t *__rest
     }
 }
 
-__global__ void copy_kernel(int n, const float *__restrict__ src, float *__restrict__ dst)
+__global__ void copy_kernel(size_t n, const float *__restrict__ src, float *__restrict__ dst)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dst[i] = src[i];
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = src[i];
+}
+static void launch_copy(size_t n, const float *src, float *dst, cudaStream_t st)
+{
+    const size_t blocks = (n + 255) / 256;
+    copy_kernel<<<(unsigned)(blocks < 65536 ? blocks : 65536), 256, 0, st>>>(n, src, dst);
 }
 
 // generic replay push (paired rows)
@@ -585,22 +618,23 @@ static size_t upd_smem_bytes(const NetDev &n, int dual)
 }
 static const size_t kMaxDynSmem = 227 * 1024;
 
-int launch_act(uavrl_learner *l, const float *obs, int n, float eps, int is_train, const float *u_tape,
+int launch_act(uavrl_learner *l, const float *obs, int n_all, float eps, int is_train, const float *u_tape,
                const int32_t *rand_tape, int32_t *actions, float *q_out, cudaStream_t st)
 {
+    const int n = n_all / l->G;                          // rows per trainer (grouped learner: G equal blocks)
     if (l->tc_ok && l->use_tc) {                         // tensor-core forward chain (tc_forward.cu)
         TcArgs a;
         memset(&a, 0, sizeof(a));
         a.img = l->tc_img_local; a.obs = obs; a.n = n; a.n_tiles = (n + kTcTile - 1) / kTcTile; a.mode = kTcAct;
         a.eps = eps; a.is_train = is_train; a.u_tape = u_tape; a.rand_tape = rand_tape;
-        a.key = l->cfg.seed ^ 0xAC7ull; a.call = l->act_calls++; a.actions = actions; a.q_out = q_out;
+        a.key = l->cfg.seed ^ kActSalt; a.call = l->act_calls++; a.actions = actions; a.q_out = q_out;
         return launch_tc_forward(l, a, st);
     }
     const int n_tiles = (n + kTile - 1) / kTile;
     const int grid = n_tiles < 4 * num_sms() ? n_tiles : 4 * num_sms();
-    act_kernel<<<grid, kNetThreads, act_smem_bytes(l->net), st>>>(l->net, l->img_local, obs, n, eps, is_train, u_tape,
-                                                                rand_tape, l->cfg.seed ^ 0xAC7ull, l->act_calls++,
-                                                                actions, nullptr, q_out, n_tiles);
+    act_kernel<<<dim3(grid, l->G), kNetThreads, act_smem_bytes(l->net), st>>>(l->net, l->img_local, obs, n, eps, is_train, u_tape,
+                                                                             rand_tape, l->cfg.seed ^ kActSalt, l->act_calls++,
+                                                                             actions, nullptr, q_out, n_tiles, l->net.smem_w_floats);
     l->pdl_prev = kPdlNone;
     UAVRL_LAUNCHED();
     return 0;
@@ -615,12 +649,12 @@ std::atomic<int> g_fuse_act_env{0};
 int launch_act_env(uavrl_learner *l, const EnvDev &d, const float *obs, float eps, int32_t *actions, float *obs_next, float *rew,
                    uint8_t *done, cudaStream_t st)
 {
-    if (!(l->tc_ok && l->use_tc && l->fuse_ok) || !g_fuse_act_env.load()) return 1;
+    if (!(l->tc_ok && l->use_tc && l->fuse_ok) || !g_fuse_act_env.load() || l->G > 1) return 1;
     TcArgs a;
     memset(&a, 0, sizeof(a));
     a.img = l->tc_img_local; a.obs = obs; a.n = d.n; a.n_tiles = (d.n + kTcTile - 1) / kTcTile; a.mode = kTcAct;
     a.eps = eps; a.is_train = l->is_train;
-    a.key = l->cfg.seed ^ 0xAC7ull; a.call = l->act_calls++; a.actions = actions;
+    a.key = l->cfg.seed ^ kActSalt; a.call = l->act_calls++; a.actions = actions;
     EnvFuse ef;
     ef.d = d; ef.obs_next = obs_next; ef.reward = rew; ef.done = done;
     return launch_tc_forward(l, a, st, &ef);
@@ -655,6 +689,15 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
     }
     const int n_tiles = (B + kTile - 1) / kTile;
     const int grid = n_tiles < l->max_ctas ? n_tiles : l->max_ctas;
+    if (grid > l->parts_cap) {                           // grouped learner, batch larger than batch_size: more partial slots
+        UAVRL_CUDA(cudaStreamSynchronize(st));
+        cudaFree(l->partials); cudaFree(l->loss_partials);
+        l->partials = nullptr; l->loss_partials = nullptr;
+        int rc;
+        if ((rc = dev_alloc(&l->partials, (size_t)l->G * grid * l->net.P)) || (rc = dev_alloc(&l->loss_partials, (size_t)l->G * grid)))
+            return rc;
+        l->parts_cap = grid;
+    }
     const float *y_in = nullptr;
     const bool fuse_td = l->tc_ok && l->use_tc && tc_train_can_fuse_td(l, B);
     if (l->tc_ok && l->use_tc && fuse_td) {
@@ -665,8 +708,8 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
         if (B > l->y_cap) {
             UAVRL_CUDA(cudaStreamSynchronize(st));
             cudaFree(l->y_buf); cudaFree(l->astar_buf);
-            UAVRL_CUDA(cudaMalloc((void **)&l->y_buf, (size_t)B * 4));
-            UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)B * 4));
+            UAVRL_CUDA(cudaMalloc((void **)&l->y_buf, (size_t)l->G * B * 4));
+            UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->G * B * 4));
             l->y_cap = B;
         }
         TcArgs a;
@@ -691,6 +734,7 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
     AdamArgs a;
     memset(&a, 0, sizeof(a));
     a.P = l->net.P; a.apply = apply ? 1 : 0; a.world = l->world;
+    a.img_floats = l->net.smem_w_floats; a.tc_floats = l->tc.train_img_bytes / 4;
     a.inv_b = 1.0f / (float)global_batch;
     if (apply && !partials_only) {
         l->adam_t += 1;
@@ -707,8 +751,8 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
         if (B > l->train_cap) {
             UAVRL_CUDA(cudaStreamSynchronize(st));
             cudaFree(l->act_buf); cudaFree(l->dz_buf);
-            UAVRL_CUDA(cudaMalloc((void **)&l->act_buf, (size_t)B * (size_t)(l->tc.act_stride > 0 ? l->tc.act_stride : 4) * 4));
-            UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, (size_t)B * (size_t)l->tc.dz_stride * 4));
+            UAVRL_CUDA(cudaMalloc((void **)&l->act_buf, (size_t)l->G * B * (size_t)(l->tc.act_stride > 0 ? l->tc.act_stride : 4) * 4));
+            UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, (size_t)l->G * B * (size_t)l->tc.dz_stride * 4));
             l->train_cap = B;
         }
         const bool may_fuse = apply && !partials_only && !per_batch;
@@ -719,10 +763,10 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
     UpdateArgs ua;
     ua.img_local = l->img_local; ua.img_target = l->img_target; ua.partials = l->partials; ua.loss_partials = l->loss_partials;
     ua.B = B; ua.n_tiles = n_tiles; ua.algo = l->cfg.algo; ua.gamma = l->cfg.gamma; ua.dual = l->dual_weights;
-    ua.loss_kind = l->cfg.loss_kind;
+    ua.loss_kind = l->cfg.loss_kind; ua.img_floats = l->net.smem_w_floats;
     ua.inv_global_b = 1.0f / (float)global_batch;
     ua.y_in = y_in;
-    update_kernel<<<grid, kNetThreads, upd_smem_bytes(l->net, l->dual_weights), st>>>(l->net, src, ua);
+    update_kernel<<<dim3(grid, l->G), kNetThreads, upd_smem_bytes(l->net, l->dual_weights), st>>>(l->net, src, ua);
     l->pdl_prev = kPdlNone;
     UAVRL_LAUNCHED();
     if (mid) UAVRL_CUDA(cudaEventRecord(mid[1], st));
@@ -738,7 +782,7 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
     if (adam_done) return 0;                                    // the weight-gradient kernel applied the optimiser step itself
     a.nparts = nparts; a.n_loss_parts = n_loss_parts;
     const bool chain = l->pdl_chain && g_pdl.load();
-    UAVRL_CUDA(launch_kernel(reduce_adam_kernel, dim3((a.P + 63) / 64), dim3(256), 0, st, chain && l->pdl_prev == kPdlDw && !mid, a,
+    UAVRL_CUDA(launch_kernel(reduce_adam_kernel, dim3((a.P + 63) / 64, l->G), dim3(256), 0, st, chain && l->pdl_prev == kPdlDw && !mid, a,
                              l->partials, l->loss_partials, l->grad, l->local, l->m, l->v, l->target, l->img_local, l->img_target,
                              l->img_map, (float *)l->tc_img_local, (float *)l->tc_img_target, l->tc_hi_map, l->tc_lo_map,
                              l->tc_hi2_map, l->tc_lo2_map, loss_out ? loss_out : l->loss_dev));
@@ -750,17 +794,19 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
 
 static int repack_images(uavrl_learner *l, cudaStream_t st)
 {
-    const int threads = 256, blocks = (l->net.P + threads - 1) / threads;
-    pack_image_kernel<<<blocks, threads, 0, st>>>(l->net.P, l->local, l->img_map, l->img_local);
+    const int threads = 256;
+    const dim3 blocks((l->net.P + threads - 1) / threads, l->G);          // y: trainer
+    const int wf = l->net.smem_w_floats, tf = l->tc.train_img_bytes / 4;
+    pack_image_kernel<<<blocks, threads, 0, st>>>(l->net.P, l->local, l->img_map, l->img_local, wf);
     UAVRL_LAUNCHED();
-    pack_image_kernel<<<blocks, threads, 0, st>>>(l->net.P, l->target, l->img_map, l->img_target);
+    pack_image_kernel<<<blocks, threads, 0, st>>>(l->net.P, l->target, l->img_map, l->img_target, wf);
     UAVRL_LAUNCHED();
     if (l->tc_ok) {
         pack_tc_kernel<<<blocks, threads, 0, st>>>(l->net.P, l->local, l->tc_hi_map, l->tc_lo_map, l->tc_hi2_map, l->tc_lo2_map,
-                                                   (float *)l->tc_img_local);
+                                                   (float *)l->tc_img_local, tf);
         UAVRL_LAUNCHED();
         pack_tc_kernel<<<blocks, threads, 0, st>>>(l->net.P, l->target, l->tc_hi_map, l->tc_lo_map, l->tc_hi2_map, l->tc_lo2_map,
-                                                   (float *)l->tc_img_target);
+                                                   (float *)l->tc_img_target, tf);
         UAVRL_LAUNCHED();
     }
     return 0;
@@ -832,8 +878,10 @@ BatchSrc replay_source(uavrl_learner *l, const int32_t *idx_tape)
     s.idx_tape = idx_tape; s.count = l->count;
     s.key = l->cfg.seed ^ 0x5EEDull; s.epoch = (uint64_t)l->epoch;
     if (l->mode == kReplayLockstep) {
+        // grouped learner: every trainer samples its own block of N / G envs (trainer_src), count = its transitions
         const int64_t N = l->cfg.lockstep_envs, nf = l->count / N;
-        s.cap = l->ring_frames; s.n_envs = (int32_t)N;
+        s.cap = l->ring_frames; s.n_envs = (int32_t)(N / l->G); s.row_stride = (int32_t)N;
+        s.count = l->count / l->G;
         s.oldest = ((l->head - nf) % l->ring_frames + l->ring_frames) % l->ring_frames;
     } else {
         s.cap = l->slots;
@@ -875,7 +923,18 @@ extern "C" {
 
 int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out)
 {
+    return uavrl_learner_create_trainers(cfg, 1, out);
+}
+
+int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_trainers, uavrl_learner **out)
+{
     if (!cfg || !out) return fail(UAVRL_ERR_INVALID, "uavrl_learner_create: null argument");
+    if (n_trainers < 1 || n_trainers > 65535)        // every grouped kernel runs one grid row per trainer: gridDim.y <= 65535
+        return fail(UAVRL_ERR_INVALID, "n_trainers must be in [1, 65535]");
+    if (n_trainers > 1 && (cfg->lockstep_envs < 0 || cfg->lockstep_envs % n_trainers != 0))
+        return fail(UAVRL_ERR_INVALID, "lockstep_envs must be a multiple of n_trainers (every trainer owns lockstep_envs / n_trainers envs)");
+    if (n_trainers > 1 && cfg->replay_capacity / n_trainers <= 0)
+        return fail(UAVRL_ERR_INVALID, "replay_capacity / n_trainers must be > 0");
     if (cfg->batch_size <= 0 || cfg->replay_capacity <= 0) return fail(UAVRL_ERR_INVALID, "batch_size and replay_capacity must be > 0");
     if (cfg->algo < 0 || cfg->algo > 2) return fail(UAVRL_ERR_INVALID, "unknown algo");
     if (cfg->loss_kind < 0 || cfg->loss_kind > 1) return fail(UAVRL_ERR_INVALID, "loss_kind must be 0 (MSE) or 1 (Huber)");
@@ -885,6 +944,7 @@ int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out)
     UAVRL_CUDA(cudaSetDevice(cfg->device));
     uavrl_learner *l = new uavrl_learner();
     l->cfg = *cfg;
+    l->G = n_trainers;
     int rc = build_net(*cfg, l->net);
     if (rc) { delete l; return rc; }
     // the fp32 kernels hold the whole network in shared memory: refuse a network that does not fit before allocating anything
@@ -893,16 +953,22 @@ int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out)
         delete l;
         return fail(UAVRL_ERR_INVALID, "network too large for the shared-memory resident kernels");
     }
-    const size_t P = (size_t)l->net.P;
+    const size_t G = (size_t)n_trainers, P = (size_t)l->net.P;
     l->max_ctas = 4 * num_sms();
-    if ((rc = dev_alloc(&l->local, P)) || (rc = dev_alloc(&l->target, P)) || (rc = dev_alloc(&l->m, P)) ||
-        (rc = dev_alloc(&l->v, P)) || (rc = dev_alloc(&l->grad, P)) ||
-        (rc = dev_alloc(&l->partials, P * (size_t)l->max_ctas)) || (rc = dev_alloc(&l->loss_partials, (size_t)l->max_ctas)) ||
-        (rc = dev_alloc(&l->loss_dev, 1)))
+    // gradient / loss partial slots per trainer: one learner keeps max_ctas (any batch); a grouped learner sizes them from the
+    // per-trainer batch (the fp32 update kernel's grid, the largest of the update routes) and grows them for larger batches
+    {
+        const int tiles = (cfg->batch_size + kTile - 1) / kTile;
+        l->parts_cap = (G == 1 || tiles > l->max_ctas) ? l->max_ctas : tiles;
+    }
+    if ((rc = dev_alloc(&l->local, G * P)) || (rc = dev_alloc(&l->target, G * P)) || (rc = dev_alloc(&l->m, G * P)) ||
+        (rc = dev_alloc(&l->v, G * P)) || (rc = dev_alloc(&l->grad, G * P)) ||
+        (rc = dev_alloc(&l->partials, G * P * (size_t)l->parts_cap)) || (rc = dev_alloc(&l->loss_partials, G * (size_t)l->parts_cap)) ||
+        (rc = dev_alloc(&l->loss_dev, G)))
         return rc;
     {
         const size_t wf = (size_t)l->net.smem_w_floats;
-        if ((rc = dev_alloc(&l->img_local, wf)) || (rc = dev_alloc(&l->img_target, wf)) || (rc = dev_alloc(&l->img_map, P))) return rc;
+        if ((rc = dev_alloc(&l->img_local, G * wf)) || (rc = dev_alloc(&l->img_target, G * wf)) || (rc = dev_alloc(&l->img_map, P))) return rc;
         std::vector<int32_t> map;
         build_image_map(l->net, map);
         UAVRL_CUDA(cudaMemcpy(l->img_map, map.data(), P * sizeof(int32_t), cudaMemcpyHostToDevice));
@@ -910,8 +976,10 @@ int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out)
     if ((rc = tc_init(l))) return rc;
     const size_t in = (size_t)cfg->in_dim;
     if (cfg->lockstep_envs > 0) {
-        const int64_t N = cfg->lockstep_envs;
-        int64_t cap_frames = (cfg->replay_capacity + N - 1) / N;
+        // a grouped learner's ring holds, for every trainer, the frames a stand-alone learner with replay_capacity / G
+        // transitions over N / G envs would keep
+        const int64_t N = cfg->lockstep_envs, cap_g = cfg->replay_capacity / n_trainers, Ng = N / n_trainers;
+        int64_t cap_frames = (cap_g + Ng - 1) / Ng;
         if (cap_frames < 2) cap_frames = 2;
         l->mode = kReplayLockstep;
         l->ring_frames = cap_frames + 1;
@@ -959,6 +1027,15 @@ int uavrl_learner_destroy(uavrl_learner *l)
 }
 
 int64_t uavrl_learner_param_count(const uavrl_learner *l) { return l ? l->net.P : 0; }
+int32_t uavrl_learner_trainer_count(const uavrl_learner *l) { return l ? l->G : 0; }
+
+// entry points a grouped learner does not offer: refused before anything is enqueued or allocated
+static int refuse_grouped(const uavrl_learner *l, const char *what)
+{
+    if (l && l->G > 1)
+        return fail(UAVRL_ERR_INVALID, std::string(what) + " is not available on a learner with " + std::to_string(l->G) + " trainers");
+    return 0;
+}
 
 static float *which_buf(uavrl_learner *l, int which)
 {
@@ -973,7 +1050,7 @@ int uavrl_learner_set_params(uavrl_learner *l, int32_t which, const float *h)
     if (!l || !h || !which_buf(l, which)) return fail(UAVRL_ERR_INVALID, "bad argument");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     UAVRL_CUDA(cudaDeviceSynchronize());
-    UAVRL_CUDA(cudaMemcpy(which_buf(l, which), h, (size_t)l->net.P * 4, cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(which_buf(l, which), h, (size_t)l->G * l->net.P * 4, cudaMemcpyHostToDevice));
     if (which <= 1) { int rc = repack_images(l, 0); if (rc) return rc; UAVRL_CUDA(cudaDeviceSynchronize()); }
     return 0;
 }
@@ -983,7 +1060,7 @@ int uavrl_learner_get_params(uavrl_learner *l, int32_t which, float *h)
     if (!l || !h || !which_buf(l, which)) return fail(UAVRL_ERR_INVALID, "bad argument");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     UAVRL_CUDA(cudaDeviceSynchronize());
-    UAVRL_CUDA(cudaMemcpy(h, which_buf(l, which), (size_t)l->net.P * 4, cudaMemcpyDeviceToHost));
+    UAVRL_CUDA(cudaMemcpy(h, which_buf(l, which), (size_t)l->G * l->net.P * 4, cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -1007,6 +1084,7 @@ int uavrl_learner_act(uavrl_learner *l, const float *obs_dev, int32_t n, float e
                       void *stream)
 {
     if (!l || !obs_dev || !actions_dev || n <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (n % l->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_learner_act: n must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     return launch_act(l, obs_dev, n, eps, is_train, u_tape_dev, rand_tape_dev, actions_dev, q_out_dev, (cudaStream_t)stream);
 }
@@ -1015,6 +1093,7 @@ int uavrl_replay_push(uavrl_learner *l, int32_t n, const float *obs, const int32
                       const float *next_obs, const uint8_t *done, void *stream)
 {
     if (!l || n <= 0 || !obs || !act || !rew || !next_obs || !done) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_grouped(l, "uavrl_replay_push (grouped learners take the lockstep ring or explicit batches)")) return rc;
     if (l->mode != kReplayPaired) return fail(UAVRL_ERR_STATE, "uavrl_replay_push needs lockstep_envs == 0 (the lockstep ring is fed by uavrl_train_run)");
     if (n > l->slots) return fail(UAVRL_ERR_INVALID, "push larger than the replay capacity");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
@@ -1046,7 +1125,8 @@ int uavrl_replay_gather(uavrl_learner *l, int32_t n, const int64_t *idx, float *
     for (int i = 0; i < n; ++i)
         if (idx[i] < 0 || idx[i] >= l->count) return fail(UAVRL_ERR_INVALID, "logical index out of range");
     UAVRL_CUDA(cudaDeviceSynchronize());
-    const BatchSrc src = replay_source(l, nullptr);
+    BatchSrc src = replay_source(l, nullptr);
+    if (src.mode == kReplayLockstep) src.n_envs = src.row_stride;    // whole-ring logical indices, whatever the trainer count
     const size_t in = (size_t)l->net.in_dim;
     // one gather kernel into a packed staging block, then one device->host copy per output array (round 1 issued 5 n
     // synchronous cudaMemcpy calls)
@@ -1086,7 +1166,7 @@ int uavrl_learner_update(uavrl_learner *l, const int32_t *idx_tape_dev, float *l
 {
     if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
     l->epoch += 1;                                              // DuelingDQN_Trainer.py:152
-    if (l->count <= l->cfg.batch_size) return 0;                // PathPlan_City.py:383: nothing sampled yet
+    if (l->count / l->G <= l->cfg.batch_size) return 0;         // PathPlan_City.py:383: nothing sampled yet (per trainer)
     BatchSrc src = replay_source(l, idx_tape_dev);
     return do_update(l, src, l->cfg.batch_size, l->cfg.batch_size, loss_dev, true, stream);
 }
@@ -1095,17 +1175,20 @@ int uavrl_learner_update_batch(uavrl_learner *l, int32_t B, const float *s, cons
                                const float *s2, const float *d, float *loss_dev, void *stream)
 {
     if (!l || B <= 0 || !s || !a || !r || !s2 || !d) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (B % l->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_learner_update_batch: B must be a multiple of the trainer count");
     l->epoch += 1;
     BatchSrc src;
     memset(&src, 0, sizeof(src));
     src.mode = kBatchExplicit; src.frames = s; src.s2_rows = s2; src.act = a; src.rew = r; src.done_f32 = d;
-    return do_update(l, src, B, B, loss_dev, true, stream);
+    const int Bg = B / l->G;                                    // block g of the rows belongs to trainer g
+    return do_update(l, src, Bg, Bg, loss_dev, true, stream);
 }
 
 int uavrl_learner_update_batch_per(uavrl_learner *l, int32_t B, const float *s, const int32_t *a, const float *r, const float *s2,
                                    const float *d, const float *is_weights, float *abs_err_out, float *loss_dev, void *stream)
 {
     if (!l || B <= 0 || !s || !a || !r || !s2 || !d) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_grouped(l, "uavrl_learner_update_batch_per (prioritised replay)")) return rc;
     l->epoch += 1;
     BatchSrc src;
     memset(&src, 0, sizeof(src));
@@ -1118,6 +1201,7 @@ int uavrl_learner_compute_grads(uavrl_learner *l, const int32_t *idx_tape_dev, i
                                 void *stream)
 {
     if (!l || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_grouped(l, "uavrl_learner_compute_grads (data-parallel training)")) return rc;
     l->epoch += 1;
     if (l->count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
     BatchSrc src = replay_source(l, idx_tape_dev);
@@ -1129,6 +1213,7 @@ float *uavrl_learner_grad_ptr(uavrl_learner *l) { return l ? l->grad : nullptr; 
 int uavrl_learner_apply_grads(uavrl_learner *l, void *stream)
 {
     if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
+    if (int rc = refuse_grouped(l, "uavrl_learner_apply_grads (data-parallel training)")) return rc;
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     AdamArgs a;
     memset(&a, 0, sizeof(a));
@@ -1152,16 +1237,15 @@ int uavrl_learner_hard_update(uavrl_learner *l, void *stream)
 {
     if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    const int threads = 256, blocks = (l->net.P + threads - 1) / threads;
-    copy_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(l->net.P, l->local, l->target);
+    // every trainer's vectors and images are contiguous ([G][...]): one copy each covers all trainers
+    const size_t G = (size_t)l->G;
+    const cudaStream_t st = (cudaStream_t)stream;
+    launch_copy(G * l->net.P, l->local, l->target, st);
     UAVRL_LAUNCHED();
-    const int wf = l->net.smem_w_floats;
-    copy_kernel<<<(wf + threads - 1) / threads, threads, 0, (cudaStream_t)stream>>>(wf, l->img_local, l->img_target);
+    launch_copy(G * l->net.smem_w_floats, l->img_local, l->img_target, st);
     UAVRL_LAUNCHED();
     if (l->tc_ok) {
-        const int nf = l->tc.train_img_bytes / 4;
-        copy_kernel<<<(nf + threads - 1) / threads, threads, 0, (cudaStream_t)stream>>>(nf, (const float *)l->tc_img_local,
-                                                                                       (float *)l->tc_img_target);
+        launch_copy(G * (size_t)(l->tc.train_img_bytes / 4), (const float *)l->tc_img_local, (float *)l->tc_img_target, st);
         UAVRL_LAUNCHED();
     }
     return 0;
@@ -1202,6 +1286,7 @@ int uavrl_learner_comm_init(uavrl_learner *l, int32_t rank, int32_t world, void 
 {
     if (!l || world < 1 || world > 64 || rank < 0 || rank >= world || !grad_handle_out || !flag_handle_out)
         return fail(UAVRL_ERR_INVALID, "bad rank/world/handle pointer");
+    if (int rc = refuse_grouped(l, "uavrl_learner_comm_init (data-parallel training)")) return rc;
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     l->rank = rank; l->world = world;
     if (l->comm_grad && l->comm_world != world) {                // re-initialised with another world size
@@ -1232,6 +1317,7 @@ int uavrl_learner_comm_init(uavrl_learner *l, int32_t rank, int32_t world, void 
 
 int uavrl_learner_comm_connect(uavrl_learner *l, const void *grad_handles, const void *flag_handles)
 {
+    if (int rc = refuse_grouped(l, "uavrl_learner_comm_connect (data-parallel training)")) return rc;
     if (!l || !grad_handles || !flag_handles || !l->comm_grad) return fail(UAVRL_ERR_STATE, "uavrl_learner_comm_connect before comm_init");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     for (int q = 0; q < l->world; ++q) {
@@ -1254,6 +1340,7 @@ int uavrl_learner_comm_connect(uavrl_learner *l, const void *grad_handles, const
 int uavrl_learner_update_dp(uavrl_learner *l, const int32_t *idx_tape_dev, int32_t global_batch, float *loss_dev, void *stream)
 {
     if (!l || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_grouped(l, "uavrl_learner_update_dp (data-parallel training)")) return rc;
     if (!l->comm_ready) return fail(UAVRL_ERR_STATE, "uavrl_learner_update_dp before uavrl_learner_comm_connect");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     l->epoch += 1;

@@ -48,9 +48,16 @@ struct BatchSrc {
     float *abs_err;                   // optional out: |Q - y| per sample (ReplayTree.batch_update input)
     int64_t count, oldest;            // valid transitions, logical index of the oldest
     int64_t cap;                      // paired: slots ; lockstep: frames in the ring
-    int32_t n_envs;                   // lockstep only
+    int32_t n_envs;                   // lockstep only: envs one trainer samples (count = frames x n_envs)
+    int32_t row_stride;               // lockstep only: envs per ring frame (0 = n_envs); > n_envs for a grouped learner
+    int32_t env_base;                 // lockstep only: first env sampled (trainer_src sets g x n_envs)
     uint64_t key, epoch;              // Philox key / counter for sampling
 };
+
+// Philox key salts of a learner seeded with `seed`: the eps-greedy draws use seed ^ kActSalt, replay sampling seed ^ kSampleSalt.
+// Trainer g of a grouped learner draws exactly what a stand-alone learner seeded with seed + g draws.
+constexpr uint64_t kActSalt = 0xAC7ull, kSampleSalt = 0x5EEDull;
+__host__ __device__ __forceinline__ uint64_t trainer_key(uint64_t key, uint64_t salt, int g) { return ((key ^ salt) + (uint64_t)g) ^ salt; }
 
 // ---- tensor-core (wgmma) forward path: one dense layer as a B operand [N_pad][K_pad], K-major canonical
 // layout (wgmma.cuh), hi and lo images of the 3xTF32 split
@@ -109,8 +116,12 @@ struct uavrl_learner {
     int32_t train_cap = 0;
     float *partials = nullptr;        // [max_ctas][P] per-CTA gradient partials
     float *loss_partials = nullptr;   // [max_ctas]
-    float *loss_dev = nullptr;        // [1]
+    float *loss_dev = nullptr;        // [G]
     int32_t max_ctas = 0;
+    int32_t parts_cap = 0;            // gradient / loss partial slots per trainer (partials: [G][parts_cap][P])
+    // grouped learner (uavrl_learner_create_trainers): G independent trainers of the same network.  Every per-network vector
+    // and weight image is [G][...], trainer g acts for envs [g Ng, (g + 1) Ng) and samples only their transitions
+    int32_t G = 1;
     int64_t epoch = 0, adam_t = 0;
     // replay
     int32_t mode = 0;
@@ -189,6 +200,24 @@ struct Transition { const float *s, *s2; int a; float r, d, ax, ay; };
 // transition's action / reward / done, which the env step of the same iteration may just have written
 // fresh: the next-state row lies in the frame the env step of the SAME iteration writes (lockstep ring: the frame behind the
 // newest transition group) -- the only sampled row a kernel launched programmatically behind that env step must not read early
+// Trainer g's view of a batch source (grouped learner: gridDim.y = G trainers, B rows each).  Explicit batches: block g of the
+// G x B rows.  Lockstep ring: env block [g n_envs, (g + 1) n_envs), trainer g's sampling key and row g of a [G][B] index tape.
+__device__ __forceinline__ BatchSrc trainer_src(BatchSrc s, int g, int B, int in_dim)
+{
+    if (g == 0) return s;
+    const size_t r0 = (size_t)g * (size_t)B;
+    if (s.mode == kBatchExplicit) {
+        s.frames += r0 * in_dim; s.s2_rows += r0 * in_dim; s.rew += r0; s.done_f32 += r0;
+        if (s.act) s.act += r0;
+        if (s.act2) s.act2 += 2 * r0;
+        return s;
+    }
+    s.env_base = g * s.n_envs;
+    s.key = trainer_key(s.key, kSampleSalt, g);
+    if (s.idx_tape) s.idx_tape += r0;
+    return s;
+}
+
 __device__ __forceinline__ int64_t resolve_rows(const BatchSrc &src, int gb, int in_dim, const uint32_t pkey[4], const float *&s, const float *&s2,
                                                 bool *fresh = nullptr)
 {
@@ -200,10 +229,11 @@ __device__ __forceinline__ int64_t resolve_rows(const BatchSrc &src, int gb, int
     const uint64_t j = src.idx_tape ? (uint64_t)src.idx_tape[gb] : perm_index((uint64_t)gb, (uint64_t)src.count, pkey);
     int64_t slot, row, row2;
     if (src.mode == kReplayLockstep) {
+        const int64_t N = src.row_stride ? src.row_stride : src.n_envs;
         const int64_t f = src.idx_is_slot ? (int64_t)(j / src.n_envs) : (src.oldest + (int64_t)(j / src.n_envs)) % src.cap;
-        const int64_t e = (int64_t)(j % src.n_envs);
-        slot = f * src.n_envs + e; row = slot;
-        row2 = ((f + 1) % src.cap) * src.n_envs + e;
+        const int64_t e = src.env_base + (int64_t)(j % src.n_envs);
+        slot = f * N + e; row = slot;
+        row2 = ((f + 1) % src.cap) * N + e;
         if (fresh) *fresh = ((f + 1) % src.cap) == (src.oldest + src.count / src.n_envs) % src.cap;
     } else {
         slot = src.idx_is_slot ? (int64_t)j : (src.oldest + (int64_t)j) % src.cap; row = 2 * slot; row2 = 2 * slot + 1;
@@ -229,10 +259,11 @@ __device__ __forceinline__ Transition resolve_transition(const BatchSrc &src, in
     const uint64_t j = src.idx_tape ? (uint64_t)src.idx_tape[gb] : perm_index((uint64_t)gb, (uint64_t)src.count, pkey);
     int64_t slot, row, row2;
     if (src.mode == kReplayLockstep) {
+        const int64_t N = src.row_stride ? src.row_stride : src.n_envs;
         const int64_t f = src.idx_is_slot ? (int64_t)(j / src.n_envs) : (src.oldest + (int64_t)(j / src.n_envs)) % src.cap;
-        const int64_t e = (int64_t)(j % src.n_envs);
-        slot = f * src.n_envs + e; row = slot;
-        row2 = ((f + 1) % src.cap) * src.n_envs + e;
+        const int64_t e = src.env_base + (int64_t)(j % src.n_envs);
+        slot = f * N + e; row = slot;
+        row2 = ((f + 1) % src.cap) * N + e;
     } else {
         slot = src.idx_is_slot ? (int64_t)j : (src.oldest + (int64_t)j) % src.cap; row = 2 * slot; row2 = 2 * slot + 1;
     }
@@ -247,6 +278,7 @@ __device__ __forceinline__ Transition resolve_transition(const BatchSrc &src, in
 // optimiser kernel arguments (reduce_adam_kernel, learner.cu; also launched by sac.cu)
 struct AdamArgs {
     int P, nparts, apply, hard, world, n_loss_parts;
+    int img_floats, tc_floats;        // grouped learner (gridDim.y = G): per-trainer strides of the fp32 / tensor-core weight images
     float step_size, beta1_c, beta2, beta2_c, eps, bc2_sqrt, inv_b;
 };
 

@@ -30,18 +30,22 @@ inline void build_image_map(const NetDev &net, std::vector<int32_t> &map)
     }
 }
 
-static __global__ void pack_image_kernel(int P, const float *__restrict__ flat, const int32_t *__restrict__ map, float *__restrict__ img)
+// blockIdx.y: network y of a stack of networks ([y][P] parameters, images img_stride floats apart)
+static __global__ void pack_image_kernel(int P, const float *__restrict__ flat, const int32_t *__restrict__ map, float *__restrict__ img,
+                                         int img_stride)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    flat += (size_t)blockIdx.y * P; img += (size_t)blockIdx.y * img_stride;
     if (i < P) img[map[i]] = flat[i];
 }
 
 static __global__ void pack_tc_kernel(int P, const float *__restrict__ flat, const int32_t *__restrict__ hi_map,
                                const int32_t *__restrict__ lo_map, const int32_t *__restrict__ hi2_map,
-                               const int32_t *__restrict__ lo2_map, float *__restrict__ img)
+                               const int32_t *__restrict__ lo2_map, float *__restrict__ img, int img_stride)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
+    flat += (size_t)blockIdx.y * P; img += (size_t)blockIdx.y * img_stride;
     const float p = flat[i];
     if (lo_map[i] >= 0) {
         float hi, lo; tf32_split(p, hi, lo);

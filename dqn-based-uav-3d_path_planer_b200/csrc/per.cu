@@ -208,6 +208,7 @@ extern "C" {
 int uavrl_per_enable(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
 {
     if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
+    if (l->G > 1) return fail(UAVRL_ERR_INVALID, "prioritised replay is not available on a learner with several trainers");
     if (l->per.enabled) return fail(UAVRL_ERR_STATE, "prioritised replay is already enabled");
     if (l->count != 0) return fail(UAVRL_ERR_STATE, "enable prioritised replay before the first transition is stored");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));

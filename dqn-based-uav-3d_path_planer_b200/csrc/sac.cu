@@ -452,7 +452,7 @@ static size_t smem_act(const uavrl_sac *s) { return (size_t)(s->actor.smem_total
 static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
 {
     const NetDev &n = role == 0 ? s->actor : s->critic;
-    pack_image_kernel<<<(n.P + 255) / 256, 256, 0, st>>>(n.P, s->p[role], role == 0 ? s->map_a : s->map_c, s->img[role]);
+    pack_image_kernel<<<(n.P + 255) / 256, 256, 0, st>>>(n.P, s->p[role], role == 0 ? s->map_a : s->map_c, s->img[role], 0);
     UAVRL_LAUNCHED();
     return 0;
 }

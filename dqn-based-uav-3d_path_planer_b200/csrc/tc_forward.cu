@@ -113,7 +113,7 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
 }
 
 
-#define TC_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
+#define TC_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
 
 // FUSE_ENV: after a tile's actions are written, the same CTA steps those R envs (env_block.cuh) -- the act -> step
 // dependency is per env, so no grid-wide boundary is needed between Trainer.get_action and BaseEnv.Move_Agent.
@@ -131,6 +131,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
     __shared__ float s_rew[kTcTile], s_done[kTcTile];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = warp & 3, half = warp >> 2;
+    // trainer blockIdx.y of a grouped learner: its weight image, rows [r0, r0 + n) of the inputs / outputs, its keys
+    const int grp = blockIdx.y;
+    const size_t r0 = (size_t)grp * (size_t)a.n;
+    const unsigned char *img = a.img + (size_t)grp * (size_t)a.img_stride;
     // The first thread of the last warp initialises the two mbarriers and issues the weight copies while the other warps
     // already gather the first tile; the CTA-wide barrier in front of the first weight wait publishes the barriers.
     constexpr int kCtl = kTcThreads - 32;
@@ -141,8 +145,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
     const uint32_t w_split = tc.n_layers > 1 ? (uint32_t)tc.L[1].hi_off : (uint32_t)tc.img_bytes;
     auto stage_image = [&]() {
         fence_proxy_async();
-        bulk_g2s_chunked(W, a.img, w_split, &wbar);
-        if (w_split < (uint32_t)tc.img_bytes) bulk_g2s_chunked(W + w_split, a.img + w_split, (uint32_t)tc.img_bytes - w_split, &wbar2);
+        bulk_g2s_chunked(W, img, w_split, &wbar);
+        if (w_split < (uint32_t)tc.img_bytes) bulk_g2s_chunked(W + w_split, img + w_split, (uint32_t)tc.img_bytes - w_split, &wbar2);
     };
     if (tid == kCtl) {
         mbar_init(&wbar, 1); mbar_init(&wbar2, 1); fence_barrier_init();
@@ -163,7 +167,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
     // act mode: row b of the tile is simply obs[base + b] -- no replay sampling (Philox), no pointer table, no barrier
     constexpr bool direct = ACT;
     uint32_t pkey[4] = {0u, 0u, 0u, 0u};
-    if (!direct) Philox::gen(a.src.key, a.src.epoch, 0x5A17ull, pkey);
+    const BatchSrc src = direct ? a.src : trainer_src(a.src, grp, a.n, tc.in_dim);
+    if (!direct) Philox::gen(src.key, src.epoch, 0x5A17ull, pkey);
     bool wready = false, w2ready = false;
 
     // R = real rows per tile (32 / 64 / 128, at most tc.max_rows).  A warpgroup's m64 MMA runs when its rows hold real
@@ -178,7 +183,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
                 const float *p = nullptr;
                 float r = 0.f, d = 0.f;
                 if (b < a.n) {
-                    const Transition t = resolve_transition(a.src, b, tc.in_dim, pkey);
+                    const Transition t = resolve_transition(src, b, tc.in_dim, pkey);
                     p = a.use_next ? t.s2 : t.s; r = t.r; d = t.d;
                 }
                 rows[tid] = p; s_rew[tid] = r; s_done[tid] = d;
@@ -200,7 +205,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
                     v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
                     if (i < total) {
                         const int r = i & (R - 1), j = i >> lgR;
-                        const float *rp = direct ? ((base + r < a.n) ? a.obs + (size_t)(base + r) * tc.in_dim : nullptr) : rows[r];
+                        const float *rp = direct ? ((base + r < a.n) ? a.obs + (r0 + base + r) * tc.in_dim : nullptr) : rows[r];
                         if (rp && 4 * j < tc.in_dim) v[u] = __ldg(reinterpret_cast<const float4 *>(rp) + j);
                     }
                 }
@@ -283,33 +288,34 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
                     int best = 0; float bv = q[0];
 #pragma unroll
                     for (int j = 1; j < 32; ++j) if (j < nA && q[j] > bv) { bv = q[j]; best = j; }
-                    const int b = base + row;
+                    const int b = base + row;                               // trainer-local row
+                    const size_t ob = r0 + b;                               // its row in the [G][n] inputs / outputs
                     if (b < a.n) {
                         if (a.q_out) {
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) if (j < nA) a.q_out[(size_t)b * nA + j] = q[j];
+                            for (int j = 0; j < 32; ++j) if (j < nA) a.q_out[ob * nA + j] = q[j];
                         }
                         if (ACT) {
                             float u; int ra;
-                            if (a.u_tape) { u = a.u_tape[b]; ra = a.rand_tape ? a.rand_tape[b] : 0; }
+                            if (a.u_tape) { u = a.u_tape[ob]; ra = a.rand_tape ? a.rand_tape[ob] : 0; }
                             else {
                                 uint32_t rr[4];
-                                Philox::gen(a.key, a.call, (uint64_t)b, rr);
+                                Philox::gen(trainer_key(a.key, kActSalt, grp), a.call, (uint64_t)b, rr);
                                 u = Philox::u01(rr[0]);
                                 ra = (int)(((uint64_t)rr[1] * (uint64_t)nA) >> 32);
                             }
-                            a.actions[b] = (u > a.eps || !a.is_train) ? best : ra;      // DuelingDQN_Trainer.py:89-97
+                            a.actions[ob] = (u > a.eps || !a.is_train) ? best : ra;     // DuelingDQN_Trainer.py:89-97
                         } else if (!ACT && a.mode == kTcArgmax) {
-                            a.actions[b] = best;                                        // DDQN_Trainer.py:94
+                            a.actions[ob] = best;                                       // DDQN_Trainer.py:94
                         } else {
                             float nq = bv;                                              // DQN_Trainer.py:109
                             if (a.mode == kTcTdGather) {                                // DDQN_Trainer.py:95
-                                const int as = a.actions[b];
+                                const int as = a.actions[ob];
                                 nq = 0.f;
 #pragma unroll
                                 for (int j = 0; j < 32; ++j) if (j == as) nq = q[j];
                             }
-                            a.y_out[b] = s_rew[row] + (a.gamma * nq * (1.f - s_done[row]));   // :99 / :114 / :171
+                            a.y_out[ob] = s_rew[row] + (a.gamma * nq * (1.f - s_done[row]));  // :99 / :114 / :171
                         }
                     }
                 }
@@ -359,6 +365,7 @@ int tc_forward_rows_per_tile(const TcNet &tc, int n)
 int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st, const EnvFuse *fuse)
 {
     TcArgs a = a_in;
+    a.img_stride = l->tc.train_img_bytes;
     const int n_sm = num_sms();
     a.rows_per_tile = tc_forward_rows_per_tile(l->tc, a.n);
     a.n_tiles = (a.n + a.rows_per_tile - 1) / a.rows_per_tile;
@@ -385,7 +392,7 @@ int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st, con
         UAVRL_CUDA(launch_kernel(pick_forward_kernel(true, a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
         l->pdl_prev = l->pdl_chain ? kPdlEnv : kPdlNone;
     } else {
-        UAVRL_CUDA(launch_kernel(pick_forward_kernel(false, a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
+        UAVRL_CUDA(launch_kernel(pick_forward_kernel(false, a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid, l->G), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
         l->pdl_prev = l->pdl_chain ? (a.mode == kTcAct ? kPdlAct : kPdlTd) : kPdlNone;
     }
     UAVRL_LAUNCHED();
@@ -417,18 +424,19 @@ int tc_init(uavrl_learner *l)
     if (tc_smem_bytes(l->tc) + fwd_static > 227 * 1024) return 0;
     const size_t P = (size_t)l->net.P;
     const size_t img = (size_t)l->tc.train_img_bytes;
-    UAVRL_CUDA(cudaMalloc((void **)&l->tc_img_local, img));
-    UAVRL_CUDA(cudaMalloc((void **)&l->tc_img_target, img));
-    UAVRL_CUDA(cudaMemset(l->tc_img_local, 0, img));
-    UAVRL_CUDA(cudaMemset(l->tc_img_target, 0, img));
+    const size_t img_all = (size_t)l->G * img;                  // [G] images of a grouped learner
+    UAVRL_CUDA(cudaMalloc((void **)&l->tc_img_local, img_all));
+    UAVRL_CUDA(cudaMalloc((void **)&l->tc_img_target, img_all));
+    UAVRL_CUDA(cudaMemset(l->tc_img_local, 0, img_all));
+    UAVRL_CUDA(cudaMemset(l->tc_img_target, 0, img_all));
     int32_t **maps[] = { &l->tc_hi_map, &l->tc_lo_map, &l->tc_hi2_map, &l->tc_lo2_map };
     std::vector<int32_t> *src[] = { &hi, &lo, &hi2, &lo2 };
     for (int i = 0; i < 4; ++i) {
         UAVRL_CUDA(cudaMalloc((void **)maps[i], P * 4));
         UAVRL_CUDA(cudaMemcpy(*maps[i], src[i]->data(), P * 4, cudaMemcpyHostToDevice));
     }
-    UAVRL_CUDA(cudaMalloc((void **)&l->y_buf, (size_t)l->cfg.batch_size * 4));
-    UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->cfg.batch_size * 4));
+    UAVRL_CUDA(cudaMalloc((void **)&l->y_buf, (size_t)l->G * l->cfg.batch_size * 4));
+    UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->G * l->cfg.batch_size * 4));
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du)
             UAVRL_CUDA(cudaFuncSetAttribute(pick_forward_kernel(false, ac != 0, du != 0, fixed), cudaFuncAttributeMaxDynamicSharedMemorySize,

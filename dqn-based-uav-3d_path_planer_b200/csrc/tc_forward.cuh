@@ -14,6 +14,8 @@ enum TcMode { kTcAct = 0, kTcArgmax = 1, kTcTdMax = 2, kTcTdGather = 3 };
 
 struct TcArgs {
     const unsigned char *img;          // TC weight image of the network to evaluate
+    int64_t img_stride;                // grouped learner (gridDim.y = G): bytes between two trainers' images; every [n] input /
+                                       // output above and below is [G][n], trainer g's block at row g n
     BatchSrc src;                      // row source for the TD modes (next-state rows); unused for kTcAct
     const float *obs;                  // kTcAct: [n][in_dim]
     int32_t n, n_tiles, mode, use_next, rows_per_tile;
@@ -25,7 +27,7 @@ struct TcArgs {
     float *y_out;                      // TD modes: y[b] = r + gamma * next_q * (1 - d)
     float gamma;
     int32_t pdl;                       // kPdlOn | kPdlEarlyWeights | kPdlEarlyRows (set by launch_tc_forward)
-    long long *trace;                  // debug: CTA 0 / thread 0 writes clock64() at stage boundaries (UAVRL_TC_TRACE=1)
+    long long *trace;                  // debug: CTA (0, 0) / thread 0 writes clock64() at stage boundaries (UAVRL_TC_TRACE=1)
 };
 
 int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::vector<int32_t> &hi_map, std::vector<int32_t> &lo_map,

@@ -44,9 +44,11 @@ struct TcTrainArgs {
     int32_t fused_td, algo;
     float gamma;
     const unsigned char *img_target;   // target network, forward image
-    long long *trace;                  // debug (UAVRL_TC_TRACE): CTA 0 / thread 0 stage timestamps
+    int64_t img_stride;                // grouped learner (gridDim.y = G): bytes between two trainers' images; y, the scratch rows
+                                       // and the batch are [G][B], the loss partials [G][gridDim.x]
+    long long *trace;                  // debug (UAVRL_TC_TRACE): CTA (0, 0) / thread 0 stage timestamps
 };
-#define TR_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
+#define TR_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
 
 struct TcDwArgs {
     BatchSrc src;
@@ -54,7 +56,7 @@ struct TcDwArgs {
     int32_t n_slices;                  // CTAs per layer; slice i accumulates chunks i, i + n_slices, ... into partial i
     const float *act_buf, *dz_buf;
     float *partials;                   // [n_slices][P]
-    long long *trace;                  // debug (UAVRL_TC_TRACE): CTA 0 / thread 0 stage timestamps
+    long long *trace;                  // debug (UAVRL_TC_TRACE): CTA (0, 0) / thread 0 stage timestamps
     // fused optimiser tail (fuse_adam = 1, only when every CTA of the grid is resident at once): the partials travel as 8-byte
     // words {epoch : value} (part64 [n_slices][P]); a reader polls the word itself -- no grid barrier, no fence, no flag
     int32_t fuse_adam;
@@ -63,7 +65,7 @@ struct TcDwArgs {
     AdamArgs adam;
     AdamPtrs ptrs;
 };
-#define DW_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
+#define DW_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
 
 // Gather R rows (pointers in rows[]) into the layer-0 A operand.  All of a thread's loads are issued before any
 // is consumed (4 in flight), so the gather costs one L2 round trip instead of one per chunk.  Item i = (chunk j = i / R,
@@ -172,6 +174,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
     __shared__ float s_loss;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = warp & 3, half = warp >> 2;
+    // trainer blockIdx.y of a grouped learner: its images, batch, TD targets and scratch rows
+    const int grp = blockIdx.y;
+    const unsigned char *img = a.img + (size_t)grp * (size_t)a.img_stride, *img_t = a.img_target + (size_t)grp * (size_t)a.img_stride;
+    const BatchSrc src = trainer_src(a.src, grp, a.B, tc.in_dim);
+    const size_t r0 = (size_t)grp * (size_t)a.B;
+    float *act_buf = a.act_buf + r0 * tc.act_stride, *dz_buf = a.dz_buf + r0 * tc.dz_stride;
+    const float *y_in = a.y ? a.y + r0 : nullptr;
     // control thread (first of the last warp): barrier init and weight copies -- concurrently with warp 0 resolving the tile's
     // samples; the first CTA-wide barrier (behind the sample table) publishes the barriers (tc_forward.cu)
     constexpr int kCtl = kTcThreads - 32;
@@ -187,13 +196,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
     if (tid == kCtl) {
         mbar_init(&wbar, 1); mbar_init(&wbar2, 1); mbar_init(&wbar3, 1); fence_barrier_init();
         fence_proxy_async();
-        if (!fused) bulk_g2s_chunked(W, a.img, (uint32_t)tc.train_img_bytes, &wbar);
+        if (!fused) bulk_g2s_chunked(W, img, (uint32_t)tc.train_img_bytes, &wbar);
         else {
-            bulk_g2s_chunked(W, (n_pre == 2) ? a.img : a.img_target, (uint32_t)tc.img_bytes, &wbar);
+            bulk_g2s_chunked(W, (n_pre == 2) ? img : img_t, (uint32_t)tc.img_bytes, &wbar);
             // the transposed blocks of the training image (dX chain) lie behind the forward image the TD passes use: they are
             // fetched now (written by the optimiser step, >= 2 kernels back) and first waited for in front of the dX chain
             if (tc.train_img_bytes > tc.img_bytes)
-                bulk_g2s_chunked(W + tc.img_bytes, a.img + tc.img_bytes, (uint32_t)(tc.train_img_bytes - tc.img_bytes), &wbar3);
+                bulk_g2s_chunked(W + tc.img_bytes, img + tc.img_bytes, (uint32_t)(tc.train_img_bytes - tc.img_bytes), &wbar3);
         }
     }
     // fused: after the TD passes the forward part of the training image comes in two pieces -- layer 0's block on wbar (all the
@@ -204,7 +213,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
     const float *bias_all = reinterpret_cast<const float *>(W + tc.bias_base);
 
     uint32_t pkey[4];
-    Philox::gen(a.src.key, a.src.epoch, 0x5A17ull, pkey);
+    Philox::gen(src.key, src.epoch, 0x5A17ull, pkey);
     bool wready = false;
     const int nl = tc.n_layers;
     const int row = quad * 32 + lane;                        // the head epilogues: one sample row per thread of warps 0-3
@@ -225,7 +234,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
             const int b = base + tid;
             const float *p = nullptr, *p2 = nullptr;
             bool fr = false;
-            if (b < a.B) my_slot = resolve_rows(a.src, b, tc.in_dim, pkey, p, p2, &fr);
+            if (b < a.B) my_slot = resolve_rows(src, b, tc.in_dim, pkey, p, p2, &fr);
             rows[tid] = p;
             if (fused) { rows2[tid] = p2; s_astar[tid] = 0; s_fresh[tid] = fr ? 1 : 0; }
         }
@@ -242,7 +251,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         }
         if (fused && !waited) { pdl_wait(); pdl_trigger(); waited = true; }
         int m_act = 0; float m_rew = 0.f, m_done = 0.f;
-        if (my_slot >= 0) load_meta(a.src, my_slot, m_act, m_rew, m_done);
+        if (my_slot >= 0) load_meta(src, my_slot, m_act, m_rew, m_done);
         if (early_rows) a0_load_sel(rows2, s_fresh, true, R, tc.in_dim, tc.L[0].K_pad, vnext);
         auto park_meta = [&]() { if (tid < R) { s_act[tid] = m_act; if (fused) { s_rew[tid] = m_rew; s_done[tid] = m_done; } } };
         TR_TRACE(2);
@@ -250,7 +259,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         for (int pass = 0; pass < n_pre; ++pass) {
             if (pass > 0 && tid == kTcThreads - 32) {                          // the target image replaces the local one (all its readers are done)
                 fence_proxy_async();
-                bulk_g2s_chunked(W, a.img_target, (uint32_t)tc.img_bytes, &wbar);
+                bulk_g2s_chunked(W, img_t, (uint32_t)tc.img_bytes, &wbar);
             }
             if (pass == 0 && early_rows) a0_store(vnext, R, tc.L[0].K_pad, Ahi, Alo);
             else build_a0(rows2, R, tc.in_dim, tc.L[0].K_pad, Ahi, Alo);
@@ -312,15 +321,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         }
         if (fused && tid == kTcThreads - 32) {                                  // the training image (every reader of the TD image is done)
             fence_proxy_async();
-            bulk_g2s_chunked(W, a.img, w_split, &wbar);
-            if (w_split < (uint32_t)tc.img_bytes) bulk_g2s_chunked(W + w_split, a.img + w_split, (uint32_t)tc.img_bytes - w_split, &wbar2);
+            bulk_g2s_chunked(W, img, w_split, &wbar);
+            if (w_split < (uint32_t)tc.img_bytes) bulk_g2s_chunked(W + w_split, img + w_split, (uint32_t)tc.img_bytes - w_split, &wbar2);
         }
         if (early_rows) a0_store(vmain, R, tc.L[0].K_pad, Ahi, Alo);
         else build_a0(rows, R, tc.in_dim, tc.L[0].K_pad, Ahi, Alo);
         TR_TRACE(9);
         if (!waited) { pdl_wait(); pdl_trigger(); waited = true; }
         if (n_pre == 0) park_meta();
-        if (!fused && tid < R) s_y[tid] = (base + tid < a.B) ? a.y[base + tid] : 0.f;      // visible after the barrier below
+        if (!fused && tid < R) s_y[tid] = (base + tid < a.B) ? y_in[base + tid] : 0.f;      // visible after the barrier below
         if (fused) { mbar_wait(&wbar, wphase); wphase ^= 1; }
         else if (!wready) { mbar_wait(&wbar, 0); wready = true; }
         fence_proxy_async();
@@ -340,7 +349,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
             const float *bias = bias_all + T.bias_off;
             if (l + 1 < nl) {
                 const uint32_t sbon = mma_sbo(T.N_pad);
-                float *act_row = a.act_buf + (size_t)egb * tc.act_stride + tc.L[l + 1].act_off;
+                float *act_row = act_buf + (size_t)egb * tc.act_stride + tc.L[l + 1].act_off;
                 uint32_t mk = 0u;
                 for (int c = e.c0, sh = 0; c < T.N_pad; c += e.step, sh += 4) {
                     const float4 v = e.ld(acc, tc.acc_ld, c);
@@ -382,8 +391,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
                     float gq = 0.f, lterm = 0.f;
                     if (mine) {
                         const float diff = qa - s_y[row];
-                        const float wb = a.src.is_w ? a.src.is_w[gb] : 1.f;
-                        if (a.src.abs_err) a.src.abs_err[gb] = fabsf(diff);
+                        const float wb = src.is_w ? src.is_w[gb] : 1.f;
+                        if (src.abs_err) src.abs_err[gb] = fabsf(diff);
                         if (a.loss_kind == 0) {                       // MSELoss (BaseTrainer.py:40)
                             lterm = wb * (diff * diff);
                             gq = (2.f * diff * wb) * a.inv_global_b;
@@ -410,7 +419,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
                         g[j] = gj;
                     }
                     TR_TRACE(25);
-                    float *dz_row = a.dz_buf + (size_t)gb * tc.dz_stride + T.dz_off;
+                    float *dz_row = dz_buf + (size_t)gb * tc.dz_stride + T.dz_off;
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
                         float4 x = make_float4(g[4 * j], g[4 * j + 1], g[4 * j + 2], g[4 * j + 3]), h, lo4;
@@ -436,7 +445,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
             // ReLU'(H_l): the sign mask this thread kept in the forward epilogue of the same columns (K_pad(l) = N_pad(l - 1))
             const uint32_t hmask = (l == 1) ? hm1 : (l == 2) ? hm2 : (l == 3) ? hm3 : hm4;
             const uint32_t sbon = mma_sbo(T.K_pad);
-            float *dz_row = a.dz_buf + (size_t)egb * tc.dz_stride + tc.L[l - 1].dz_off;
+            float *dz_row = dz_buf + (size_t)egb * tc.dz_stride + tc.L[l - 1].dz_off;
             for (int c = e.c0, sh = 0; c < T.K_pad; c += e.step, sh += 4) {
                 const float4 v = e.ld(acc, tc.acc_ld, c);
                 const uint32_t m4 = hmask >> sh;
@@ -457,7 +466,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         }
     }
     TR_TRACE(20);
-    if (tid == 0) a.loss_partials[blockIdx.x] = s_loss;
+    if (tid == 0) a.loss_partials[(size_t)grp * gridDim.x + blockIdx.x] = s_loss;
 }
 
 // ------------------------------------------------------------------ split-K weight gradients
@@ -515,6 +524,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     extern __shared__ __align__(1024) unsigned char smem[];
     const int l = blockIdx.x % tc.n_layers, slice = blockIdx.x / tc.n_layers;
     const int chunk = slice;                                  // partial index
+    // trainer blockIdx.y of a grouped learner: its batch, scratch rows and partials [n_slices][P]
+    const int grp = blockIdx.y;
+    const BatchSrc src = trainer_src(a.src, grp, a.B, tc.in_dim);
+    const float *act_buf = a.act_buf + (size_t)grp * a.B * tc.act_stride, *dz_buf = a.dz_buf + (size_t)grp * a.B * tc.dz_stride;
     const TcLayer T = tc.L[l];
     const int rowsA = T.K_real + 1;                           // input features + the all-ones column (bias gradient)
     // A = [act ; 1]^T as [feature][sample] (rows past rowsA are zero), B = dZ^T as [out][sample]; hi and lo images of each
@@ -526,14 +539,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = warp & 3, half = warp >> 2;
     DW_TRACE(0);
     uint32_t pkey[4];
-    Philox::gen(a.src.key, a.src.epoch, 0x5A17ull, pkey);
+    Philox::gen(src.key, src.epoch, 0x5A17ull, pkey);
     auto resolve_chunk = [&](int c, int buf) {                // row pointers of chunk c (128 samples)
         if (tid < kDwChunk) {
             const int b = c * kDwChunk + tid;
             const float *p = nullptr, *dzp = nullptr;
             if (c < a.n_chunks && b < a.B) {
-                p = (l == 0) ? resolve_transition(a.src, b, tc.in_dim, pkey).s : a.act_buf + (size_t)b * tc.act_stride + T.act_off;
-                dzp = a.dz_buf + (size_t)b * tc.dz_stride + T.dz_off;
+                p = (l == 0) ? resolve_transition(src, b, tc.in_dim, pkey).s : act_buf + (size_t)b * tc.act_stride + T.act_off;
+                dzp = dz_buf + (size_t)b * tc.dz_stride + T.dz_off;
             }
             rows[buf][tid] = p; drows[buf][tid] = dzp;
         }
@@ -610,7 +623,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     // Partial slice `chunk`: plain floats for the separate optimiser kernel, or 8-byte words {epoch : value} for the fused tail.
     // Lanes hold consecutive f, so every store instruction writes 32 consecutive elements of one weight row; the 32 columns of a
     // thread walk the rows with a pointer increment and a predicate each (the address arithmetic used to dominate this epilogue).
-    float *part = a.partials + (size_t)chunk * a.P;
+    float *part = a.partials + ((size_t)grp * a.n_slices + chunk) * a.P;
     unsigned long long *part64 = FUSE_ADAM ? a.part64 + (size_t)chunk * a.P : nullptr;
     const unsigned long long tag = (unsigned long long)a.ll_epoch << 32;
     const int f = quad * 32 + lane;
@@ -765,9 +778,9 @@ int tc_train_init(uavrl_learner *l)
                                             (int)train_smem_bytes(tc, tc.train_max_rows)));
     UAVRL_CUDA(cudaFuncSetAttribute(tc_dw_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dw_smem_bytes(tc)));
     UAVRL_CUDA(cudaFuncSetAttribute(tc_dw_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dw_smem_bytes(tc)));
-    const size_t cap = (size_t)l->cfg.batch_size;
-    UAVRL_CUDA(cudaMalloc((void **)&l->act_buf, cap * (size_t)(tc.act_stride > 0 ? tc.act_stride : 4) * 4));
-    UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, cap * (size_t)tc.dz_stride * 4));
+    const size_t cap = (size_t)l->cfg.batch_size, G = (size_t)l->G;
+    UAVRL_CUDA(cudaMalloc((void **)&l->act_buf, G * cap * (size_t)(tc.act_stride > 0 ? tc.act_stride : 4) * 4));
+    UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, G * cap * (size_t)tc.dz_stride * 4));
     l->train_cap = (int32_t)cap;
     l->tc_train_ok = true;
     return 0;
@@ -801,6 +814,7 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     a.act_buf = l->act_buf; a.dz_buf = l->dz_buf; a.loss_partials = l->loss_partials;
     a.loss_kind = l->cfg.loss_kind;
     a.fused_td = fused_td ? 1 : 0; a.algo = l->cfg.algo; a.gamma = l->cfg.gamma; a.img_target = l->tc_img_target;
+    a.img_stride = tc.train_img_bytes;
     a.R = train_rows_per_tile(tc, B);
     a.n_tiles = (B + a.R - 1) / a.R;
     const int grid = a.n_tiles < num_sms() ? a.n_tiles : num_sms();
@@ -812,11 +826,11 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     const bool use_pdl = chain && (fused_td ? (l->pdl_prev == kPdlEnv) : (l->pdl_prev == kPdlTd));
     const int npre = fused_td ? (l->cfg.algo != UAVRL_ALGO_DQN ? 2 : 1) : 0;
     auto train_fn = pick_train_kernel(npre, tc.dueling != 0, tc_fixed_chains(tc, true));
-    UAVRL_CUDA(launch_kernel(train_fn, dim3(grid), dim3(kTcThreads), train_smem_bytes(tc, a.R), st, use_pdl, tc, a));
+    UAVRL_CUDA(launch_kernel(train_fn, dim3(grid, l->G), dim3(kTcThreads), train_smem_bytes(tc, a.R), st, use_pdl, tc, a));
     // experiment (with UAVRL_TC_TRACE): the same launch again, back to back -- the kernel is idempotent, the second run finds
     // its code in the instruction caches, and the stage trace printed below is the second run's
     static const bool twice = trace_on && getenv("UAVRL_TRAIN_TWICE") != nullptr;
-    if (twice) UAVRL_CUDA(launch_kernel(train_fn, dim3(grid), dim3(kTcThreads), train_smem_bytes(tc, a.R), st, false, tc, a));
+    if (twice) UAVRL_CUDA(launch_kernel(train_fn, dim3(grid, l->G), dim3(kTcThreads), train_smem_bytes(tc, a.R), st, false, tc, a));
     l->pdl_prev = chain ? kPdlTrain : kPdlNone;
     UAVRL_LAUNCHED();
     if (after_chain) UAVRL_CUDA(cudaEventRecord(after_chain, st));
@@ -831,7 +845,7 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     const int dw_grid = d.n_slices * tc.n_layers;
     // Fused optimiser tail: the kernel's grid barrier needs every CTA resident at once -- one CTA per SM (193 KB of shared
     // memory each), so only when the grid fits the SMs; larger batches keep the separate reduce_adam_kernel.
-    const bool fuse = adam != nullptr && g_fuse_dw_adam.load() && dw_grid <= n_sm;
+    const bool fuse = adam != nullptr && g_fuse_dw_adam.load() && dw_grid <= n_sm && l->G == 1;
     if (adam_done) *adam_done = fuse;
     if (fuse) {
         if (!l->dw_bar) {                                        // the {epoch : value} partial buffer [max_slices][P], zeroed once
@@ -851,7 +865,7 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
         q.tc_hi2 = l->tc_hi2_map; q.tc_lo2 = l->tc_lo2_map; q.loss_out = loss_out;
     }
     if (trace_on) d.trace = tr;
-    UAVRL_CUDA(launch_kernel(fuse ? tc_dw_kernel<true> : tc_dw_kernel<false>, dim3(dw_grid), dim3(kTcThreads), dw_smem_bytes(tc), st,
+    UAVRL_CUDA(launch_kernel(fuse ? tc_dw_kernel<true> : tc_dw_kernel<false>, dim3(dw_grid, l->G), dim3(kTcThreads), dw_smem_bytes(tc), st,
                              chain && !after_chain, tc, d));
     l->pdl_prev = chain ? (fuse ? kPdlAdam : kPdlDw) : kPdlNone;
     UAVRL_LAUNCHED();

@@ -55,7 +55,7 @@ extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters
         if (do_update) {
             for (int u = 0; u < updates_per_iter; ++u) {  // PathPlan_City.update -> Trainer.update (:757-776)
                 l->epoch += 1;
-                if (l->count <= l->cfg.batch_size) continue;
+                if (l->count / l->G <= l->cfg.batch_size) continue;      // per trainer
                 BatchSrc src = replay_source(l, nullptr);
                 if ((rc = launch_update(l, src, l->cfg.batch_size, l->cfg.batch_size, l->loss_dev, true, st))) return rc;
                 ++updates;
@@ -67,7 +67,11 @@ extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters
         unsigned long long c1[8]; double r1; float loss;
         UAVRL_CUDA(cudaMemcpy(c1, env->d.stat_counts, sizeof(c1), cudaMemcpyDeviceToHost));
         UAVRL_CUDA(cudaMemcpy(&r1, env->d.stat_reward, sizeof(r1), cudaMemcpyDeviceToHost));
-        UAVRL_CUDA(cudaMemcpy(&loss, l->loss_dev, sizeof(loss), cudaMemcpyDeviceToHost));
+        std::vector<float> losses((size_t)l->G);                // grouped learner: the mean over trainers
+        UAVRL_CUDA(cudaMemcpy(losses.data(), l->loss_dev, losses.size() * sizeof(float), cudaMemcpyDeviceToHost));
+        double lsum = 0.0;
+        for (float x : losses) lsum += x;
+        loss = (float)(lsum / (double)l->G);
         stats_host->env_steps = (int64_t)(c1[0] - c0[0]);
         stats_host->episodes_ended = (int64_t)(c1[1] - c0[1]);
         stats_host->collisions = (int64_t)(c1[2] - c0[2]);
@@ -83,6 +87,7 @@ extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters
 extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, int32_t global_batch, void *stream)
 {
     if (!env || !l || n_iters < 0 || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (l->G > 1) return fail(UAVRL_ERR_INVALID, "uavrl_train_run_dp is not available on a learner with several trainers");
     if (l->mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n)
         return fail(UAVRL_ERR_INVALID, "learner.lockstep_envs must equal env.n_envs");
     if (!l->comm_ready) return fail(UAVRL_ERR_STATE, "uavrl_train_run_dp before uavrl_learner_comm_connect");
@@ -142,7 +147,7 @@ extern "C" int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_i
         UAVRL_CUDA(cudaEventRecord(e[2], st));
         lockstep_commit(l, st);
         l->epoch += 1;
-        if (l->count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay not warmed up");
+        if (l->count / l->G <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay not warmed up");
         BatchSrc src = replay_source(l, nullptr);
         if ((rc = launch_update_split(l, src, l->cfg.batch_size, st, &e[3]))) return rc;   // records e[3], e[4], e[5]
         UAVRL_CUDA(cudaEventRecord(e[6], st));

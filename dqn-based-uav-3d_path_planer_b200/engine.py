@@ -230,10 +230,17 @@ NET_KINDS = {                       # BaseClass/BaseCNN.py class name -> (hidden
 
 
 class Learner:
-    """Q-network + Adam + replay on one GPU (DQN / DDQN / DuelingDQN trainers of the reference)."""
+    """Q-network + Adam + replay on one GPU (DQN / DDQN / DuelingDQN trainers of the reference).
+
+    trainers = G > 1: G independent trainers of this network in one handle (one Trainer per UAV group, PathPlan_City.py:59-69).
+    The lockstep envs split into G blocks of lockstep_envs / G, trainer g learns from its block only and computes what a
+    stand-alone Learner(seed=seed + g, replay_capacity=replay_capacity // G, lockstep_envs=lockstep_envs // G) computes.
+    Parameters are then (G, P) arrays, act / update_batch take G equal row blocks and loss tensors are [G]
+    (include/uavrl.h, uavrl_learner_create_trainers)."""
 
     def __init__(self, in_dim=OBS_DIM, hidden=(64, 64), n_actions=27, dueling=False, algo=ALGO_DDQN, lr=5e-4,
-                 gamma=0.99, batch_size=64, update_loop=3, replay_capacity=10000, lockstep_envs=0, seed=42, device=0, loss="mse"):
+                 gamma=0.99, batch_size=64, update_loop=3, replay_capacity=10000, lockstep_envs=0, seed=42, device=0, loss="mse",
+                 trainers=1):
         self.device = torch.device("cuda", device)
         c = _lib.LearnerConfig()
         c.loss_kind = {"mse": 0, "huber": 1}[loss]
@@ -245,8 +252,9 @@ class Learner:
         self.cfg = c
         self.in_dim, self.hidden, self.n_actions, self.dueling = in_dim, list(hidden), n_actions, bool(dueling)
         self.h = C.c_void_p()
-        check(_lib.lib().uavrl_learner_create(C.byref(c), C.byref(self.h)))
+        check(_lib.lib().uavrl_learner_create_trainers(C.byref(c), int(trainers), C.byref(self.h)))
         self.P = int(_lib.lib().uavrl_learner_param_count(self.h))
+        self.G = int(_lib.lib().uavrl_learner_trainer_count(self.h))
 
     def close(self):
         if self.h:
@@ -262,7 +270,14 @@ class Learner:
     # -- parameters (flat, state_dict order)
     def init_params(self, seed=0):
         """torch.nn.Linear default init (kaiming_uniform(a=sqrt(5)) == U(+-1/sqrt(fan_in)) for W and b),
-        independent draws for q_local and q_target like the reference's two Create_Network calls."""
+        independent draws for q_local and q_target like the reference's two Create_Network calls.
+        Trainer g of a grouped learner draws with seed + g."""
+        draws = [self._init_draw(seed + g) for g in range(self.G)]
+        for which in (0, 1):
+            flat = draws[0][which] if self.G == 1 else np.stack([d[which] for d in draws])
+            self.set_params(flat, which)
+
+    def _init_draw(self, seed):
         g = torch.Generator().manual_seed(seed)
         outs = []
         for _ in range(2):
@@ -277,18 +292,24 @@ class Learner:
                     fan_in = out
             outs.append(torch.cat(parts).numpy().astype(np.float32))
         assert outs[0].size == self.P
-        self.set_params(outs[0], 0)
-        self.set_params(outs[1], 1)
+        return outs
+
+    def _param_shape(self):
+        return (self.P,) if self.G == 1 else (self.G, self.P)
 
     def set_params(self, flat, which=0):
+        """which: 0 q_local, 1 q_target, 2 / 3 Adam exp_avg / exp_avg_sq, 4 gradient; (P,) or, with trainers > 1, (G, P)."""
         flat = np.ascontiguousarray(flat, np.float32)
-        assert flat.size == self.P, (flat.size, self.P)
+        assert flat.size == self.G * self.P, (flat.shape, self._param_shape())
         check(_lib.lib().uavrl_learner_set_params(self.h, which, _ptr(flat)))
 
     def get_params(self, which=0):
-        out = np.zeros(self.P, np.float32)
+        out = np.zeros(self._param_shape(), np.float32)
         check(_lib.lib().uavrl_learner_get_params(self.h, which, _ptr(out)))
         return out
+
+    def trainer_count(self):
+        return self.G
 
     def counters(self):
         e, t = C.c_int64(), C.c_int64()
@@ -322,12 +343,18 @@ class Learner:
         check(_lib.lib().uavrl_replay_gather(self.h, n, _ptr(idx), _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d)))
         return s, a, r, s2, d
 
+    def _loss(self, loss):
+        """A caller's loss tensor: the update writes one loss per trainer, so it must hold at least G floats."""
+        if loss is not None and loss.numel() < self.G:
+            raise ValueError("loss holds %d elements; a learner with %d trainers writes %d losses" % (loss.numel(), self.G, self.G))
+        return _ptr(loss)
+
     def update(self, idx_tape=None, loss=None):
-        check(_lib.lib().uavrl_learner_update(self.h, _ptr(idx_tape), _ptr(loss), _stream(self.device)))
+        check(_lib.lib().uavrl_learner_update(self.h, _ptr(idx_tape), self._loss(loss), _stream(self.device)))
 
     def update_batch(self, s, a, r, s2, d, loss=None):
         check(_lib.lib().uavrl_learner_update_batch(self.h, s.shape[0], _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d),
-                                                    _ptr(loss), _stream(self.device)))
+                                                    self._loss(loss), _stream(self.device)))
 
     def update_batch_per(self, s, a, r, s2, d, is_weights=None, abs_err_out=None, loss=None):
         """update_batch with per-sample importance weights in the loss and |Q - y| written back (prioritised replay)."""

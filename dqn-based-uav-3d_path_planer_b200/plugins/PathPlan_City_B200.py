@@ -1,6 +1,7 @@
 """Env plug-in: the reference's PathPlan_City (Envs/PathPlan_City.py) with `num_UAV` UAV instances
-stepped in lockstep on a H100 and ONE shared Q-network trainer (the north-star design; the
-reference keeps one trainer per UAV -- with num_UAV = 1 both coincide).
+stepped in lockstep on a H100.  <num_trainers> (default 1) independent Q-network trainers share them: trainer g learns
+from UAVs [g num_UAV / num_trainers, (g + 1) num_UAV / num_trainers) and is named UAV_<g num_UAV / num_trainers>.
+num_trainers = num_UAV is the reference's one trainer per UAV (PathPlan_City.py:59-69); 1 is one shared trainer.
 
 Constructor takes the same parsed-XML dict the reference's EnvFactory passes
 (config/PathPlan_City.xml <env> ... </env>): len/width/h, num_UAV, Agent.xml_path_agent,
@@ -119,6 +120,9 @@ class PathPlan_City_B200:
         self.city = engine.City(self.len, self.width, self.h, self.buildings_table)
         # agents (PathPlan_City.py:54-69)
         self.num_UAV = int(param.get('num_UAV'))
+        self.num_trainers = int(None2Value(param.get('num_trainers'), 1))
+        if self.num_trainers < 1 or self.num_UAV % self.num_trainers != 0:
+            raise ValueError("num_UAV (%d) must be a multiple of num_trainers (%d)" % (self.num_UAV, self.num_trainers))
         agents_params = param.get('Agent')
         self.uav_dict = XML2Dict(os.path.normpath(agents_params['xml_path_agent'])).get('Agent')
         self.uav_params = uav_params_from_dict(self.uav_dict)
@@ -144,7 +148,7 @@ class PathPlan_City_B200:
         if power is not None or self.record_csv:
             self.batch.set_extras(power=power, track_envs=(1 if self.record_csv else 0),
                                   track_capacity=(64 * self.uav_params.max_step if self.record_csv else 0))
-        # trainer (one, shared)
+        # trainer(s): one handle holding num_trainers independent trainers
         tpath = os.path.normpath(agents_params['Trainer']['Trainer_path'])
         tdict = XML2Dict(tpath).get('Trainer')
         tdict['name'] = 'UAV_0'
@@ -152,6 +156,9 @@ class PathPlan_City_B200:
         # HOST arrays across every boundary like the reference's own objects, and the trainer keeps the generic replay store;
         # 0 (default): run_eposide drives the device-resident lockstep loop (observations go straight into the replay ring)
         self.host_driven = int(None2Value(param.get('host_driven'), 0))
+        if self.host_driven and self.num_trainers > 1:
+            raise ValueError("host_driven = 1 drives one trainer: it needs num_trainers = 1")
+        tdict['n_trainers'] = str(self.num_trainers)
         tdict['lockstep_envs'] = '0' if self.host_driven else str(self.num_UAV)
         tdict['device'] = str(self.device_index)
         ttype = tdict.get('Trainer_Type')

@@ -89,13 +89,18 @@ class TrainerB200:
         self.network = net
         self.device_index = int(None2Value(param.get('device'), 0))
         self.lockstep_envs = int(None2Value(param.get('lockstep_envs'), 0))
+        # n_trainers = G > 1: one independent trainer per block of lockstep_envs / G UAVs (the reference's Trainer per UAV,
+        # PathPlan_City.py:59-69), each with its own replay_size transitions; trainer g is named UAV_<g * lockstep_envs / G>
+        self.n_trainers = int(None2Value(param.get('n_trainers'), 1))
+        G = self.n_trainers
+        self.names = [self.name] if G == 1 else ['UAV_%d' % (g * (self.lockstep_envs // G)) for g in range(G)]
         self._learner = engine.Learner(self.w, hidden_fn(hid), self.output, dueling, self.ALGO, lr=self.LEARNING_RATE,
                                        gamma=self.gamma, batch_size=self.Batch_Size, update_loop=self.Update_loop,
-                                       replay_capacity=self.replay_size, lockstep_envs=self.lockstep_envs,
-                                       seed=int(None2Value(param.get('seed'), 42)), device=self.device_index)
+                                       replay_capacity=self.replay_size * G, lockstep_envs=self.lockstep_envs,
+                                       seed=int(None2Value(param.get('seed'), 42)), device=self.device_index, trainers=G)
         self._learner.init_params(int(None2Value(param.get('seed'), 42)))
         self._dev = self._learner.device
-        self._loss = torch.zeros(1, device=self._dev)
+        self._loss = torch.zeros(G, device=self._dev)
         self.loss = 0
         self._rng = np.random.default_rng([int(None2Value(param.get('seed'), 42)), sum(map(ord, str(self.name)))])
         self._learner.set_is_train(self.Is_Train)        # the lockstep loops read it (get_action greedy when 0)
@@ -248,78 +253,131 @@ class TrainerB200:
         names += ["fc_A", "fc_V"] if self._learner.dueling else ["fc%d" % (len(self._learner.hidden) + 1)]
         return names
 
-    def state_dict(self, which=0):
-        flat = self._learner.get_params(which)
-        sd, off, fan_in = collections.OrderedDict(), 0, self.w
+    def _param_shapes(self):
+        """(state_dict key, shape) of every tensor, in state_dict order -- from the network description, no device read."""
+        out, fan_in = [], self.w
         widths = self._learner.hidden + [self.output] + ([1] if self._learner.dueling else [])
-        for i, (nm, out) in enumerate(zip(self._names(), widths)):
+        for i, (nm, o) in enumerate(zip(self._names(), widths)):
             fi = fan_in if i <= len(self._learner.hidden) else self._learner.hidden[-1]
-            sd[nm + ".weight"] = torch.from_numpy(flat[off:off + out * fi].reshape(out, fi).copy()); off += out * fi
-            sd[nm + ".bias"] = torch.from_numpy(flat[off:off + out].copy()); off += out
+            out += [(nm + ".weight", (o, fi)), (nm + ".bias", (o,))]
             if i < len(self._learner.hidden):
-                fan_in = out
+                fan_in = o
+        return out
+
+    def _rows(self, which):
+        """Vector `which` of every trainer, (G, P), in ONE device read: checkpoints of many trainers slice these rows
+        instead of reading the whole [G][P] vector once per trainer."""
+        return self._learner.get_params(which).reshape(self.n_trainers, -1)
+
+    @staticmethod
+    def _flat_of(tensors):
+        return np.concatenate([np.asarray(v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v, np.float32).ravel()
+                               for v in tensors])
+
+    def state_dict(self, which=0, g=0, flat=None):
+        """Trainer g's network `which` (0 q_local, 1 q_target) as a state_dict; `flat` = its row when already on the host."""
+        flat = self._rows(which)[g] if flat is None else flat
+        sd, off = collections.OrderedDict(), 0
+        for nm, shape in self._param_shapes():
+            k = int(np.prod(shape))
+            sd[nm] = torch.from_numpy(flat[off:off + k].reshape(shape).copy())
+            off += k
         return sd
 
-    def load_state_dict(self, sd, which=0):
-        flat = np.concatenate([np.asarray(v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v,
-                                          np.float32).ravel() for v in sd.values()])
+    def load_state_dict(self, sd, which=0, g=0):
+        flat = self._flat_of(sd.values())
+        if self.n_trainers > 1:                 # trainer g's row of the [G][P] parameters
+            rows = self._rows(which)
+            rows[g] = flat
+            flat = rows
         self._learner.set_params(flat, which)
 
-    def optimizer_state_dict(self):
-        n = len(self.state_dict())
-        e, t = self._learner.counters()
-        m, v = self._learner.get_params(2), self._learner.get_params(3)
+    def optimizer_state_dict(self, g=0, m=None, v=None):
+        """torch.optim.Adam state_dict of trainer g; m / v = its exp_avg / exp_avg_sq rows when already on the host."""
+        shapes = self._param_shapes()
+        t = self._learner.counters()[1]
+        m = self._rows(2)[g] if m is None else m
+        v = self._rows(3)[g] if v is None else v
         state, off = {}, 0
-        for i, p in enumerate(self.state_dict().values()):
-            k = p.numel()
-            state[i] = {'step': torch.tensor(float(t)), 'exp_avg': torch.from_numpy(m[off:off + k].reshape(p.shape).copy()),
-                        'exp_avg_sq': torch.from_numpy(v[off:off + k].reshape(p.shape).copy())}
+        for i, (_, shape) in enumerate(shapes):
+            k = int(np.prod(shape))
+            state[i] = {'step': torch.tensor(float(t)), 'exp_avg': torch.from_numpy(m[off:off + k].reshape(shape).copy()),
+                        'exp_avg_sq': torch.from_numpy(v[off:off + k].reshape(shape).copy())}
             off += k
         group = {'lr': self.LEARNING_RATE, 'betas': (0.9, 0.999), 'eps': 1e-08, 'weight_decay': 0, 'amsgrad': False,
-                 'params': list(range(n))}
+                 'params': list(range(len(shapes)))}
         return {'state': state, 'param_groups': [group]}
 
-    def load_optimizer_state_dict(self, osd):
+    @classmethod
+    def _adam_rows(cls, osd):
+        """(exp_avg, exp_avg_sq, step) of an optimizer state_dict, or None when it holds no state."""
         st = osd.get('state', {})
         if not st:
-            return
+            return None
         keys = sorted(st.keys())
-        m = np.concatenate([st[k]['exp_avg'].detach().cpu().numpy().ravel() for k in keys]).astype(np.float32)
-        v = np.concatenate([st[k]['exp_avg_sq'].detach().cpu().numpy().ravel() for k in keys]).astype(np.float32)
-        self._learner.set_params(m, 2)
-        self._learner.set_params(v, 3)
-        step = int(float(st[keys[0]]['step']))
-        self._learner.set_counters(self._learner.counters()[0], step)
+        return (cls._flat_of(st[k]['exp_avg'] for k in keys), cls._flat_of(st[k]['exp_avg_sq'] for k in keys),
+                int(float(st[keys[0]]['step'])))
 
-    def _paths(self, directory):
-        return (os.path.join(directory, 'q_target_%s%s.pth' % (self.TAG, self.name)),
-                os.path.join(directory, 'q_local_%s%s.pth' % (self.TAG, self.name)))
+    def load_optimizer_state_dict(self, osd, g=0):
+        mvs = self._adam_rows(osd)
+        if mvs is None:
+            return
+        for which, x in ((2, mvs[0]), (3, mvs[1])):
+            rows = self._rows(which)
+            rows[g] = x
+            self._learner.set_params(rows, which)
+        self._learner.set_counters(self._learner.counters()[0], mvs[2])
+
+    def _paths(self, directory, g=0):
+        return (os.path.join(directory, 'q_target_%s%s.pth' % (self.TAG, self.names[g])),
+                os.path.join(directory, 'q_local_%s%s.pth' % (self.TAG, self.names[g])))
 
     def save(self, directory=None):
+        """One q_target / q_local file pair per trainer, named after the trainer (the reference's per-UAV files).  Each of the
+        four vectors is read from the device once for all trainers."""
         directory = directory or self.model_dir or os.path.join(os.getcwd(), 'Mod')
         os.makedirs(directory, exist_ok=True)
-        pt, pl = self._paths(directory)
-        osd = self.optimizer_state_dict()
-        torch.save({'model': self.state_dict(1), 'optimizer': osd, 'epoch': self.epoch}, pt)
-        torch.save({'model': self.state_dict(0), 'optimizer': osd, 'epoch': self.epoch}, pl)
+        local, target, m, v = (self._rows(w) for w in range(4))
+        epoch = self.epoch
+        for g in range(self.n_trainers):
+            pt, pl = self._paths(directory, g)
+            osd = self.optimizer_state_dict(g, m[g], v[g])
+            torch.save({'model': self.state_dict(1, g, target[g]), 'optimizer': osd, 'epoch': epoch}, pt)
+            torch.save({'model': self.state_dict(0, g, local[g]), 'optimizer': osd, 'epoch': epoch}, pl)
 
     def Load_Mod(self, Mod_path=None):
         """DuelingDQN_Trainer.Load_Mod (:40-69): <root>/Mod by default; a given Mod_path is tried as written and, like the
-        reference's `root + Mod_path`, relative to the working directory."""
+        reference's `root + Mod_path`, relative to the working directory.  Every trainer whose file pair exists is restored
+        into host copies of the four vectors, which go to the device once each."""
         directory = Mod_path or os.path.join(os.getcwd(), 'Mod')
         if Mod_path and not os.path.isdir(directory) and os.path.isdir(os.path.join(os.getcwd(), Mod_path.lstrip('/'))):
             directory = os.path.join(os.getcwd(), Mod_path.lstrip('/'))
-        pt, pl = self._paths(directory)
-        if os.path.exists(pt) and os.path.exists(pl):
+        rows, epoch, step = None, None, None
+        for g in range(self.n_trainers):
+            pt, pl = self._paths(directory, g)
+            if not (os.path.exists(pt) and os.path.exists(pl)):
+                continue
             try:
                 mt = torch.load(pt, weights_only=False, map_location='cpu')
                 ml = torch.load(pl, weights_only=False, map_location='cpu')
-                self.load_state_dict(mt['model'], 1)
-                self.load_state_dict(ml['model'], 0)
-                self.load_optimizer_state_dict(ml['optimizer'])
-                self._learner.set_counters(int(ml['epoch']), self._learner.counters()[1])
+                tgt, loc = self._flat_of(mt['model'].values()), self._flat_of(ml['model'].values())
+                mvs = self._adam_rows(ml['optimizer'])
+                ep = int(ml['epoch'])
             except Exception as e:          # the reference prints and carries on (:56-57)
                 print(e.args)
+                continue
+            if rows is None:
+                rows = [self._rows(w) for w in range(4)]
+            rows[0][g], rows[1][g] = loc, tgt
+            if mvs is not None:
+                rows[2][g], rows[3][g], step = mvs
+            epoch = ep
+        if rows is None:
+            return
+        for w in range(4):
+            self._learner.set_params(rows[w], w)
+        e, t = self._learner.counters()
+        self._learner.set_counters(epoch, t if step is None else step)
 
     def _maybe_save(self):
         if self.save_loop > 0 and self.epoch % self.save_loop == 0:

@@ -188,6 +188,28 @@ int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out);
 int uavrl_learner_destroy(uavrl_learner *l);
 int64_t uavrl_learner_param_count(const uavrl_learner *l);
 
+/* G independent trainers of the same network and hyper-parameters in one handle (PathPlan_City.py:59-69 builds one Trainer per
+ * UAV; several seeds or replicas trained side by side).  uavrl_learner_create is n_trainers = 1.  The lockstep envs are split
+ * into G contiguous blocks of Ng = lockstep_envs / G: trainer g acts for envs [g Ng, (g + 1) Ng), samples only their
+ * transitions and owns its local and target parameters, Adam moments, gradient and loss.  epoch, adam_step and the
+ * hard-update schedule are shared (the trainers step in lockstep).  Trainer g computes bit for bit what a stand-alone learner
+ * with its parameters, seed + g, replay_capacity / G and Ng envs computes.  With G > 1:
+ *   - set/get_params move [G][P] floats;
+ *   - uavrl_learner_act takes n rows in G equal blocks (block g -> trainer g);
+ *   - uavrl_learner_update_batch takes G B rows, block g for trainer g (B = rows / G);
+ *   - uavrl_learner_update: idx_tape_dev is [G][batch_size] trainer-local logical indices; the k-th oldest transition of
+ *     trainer g is the ring's logical index (k / Ng) N + g Ng + k % Ng (uavrl_replay_gather keeps whole-ring indices);
+ *   - loss_dev receives [G] losses; uavrl_train_stats.last_loss is their mean;
+ *   - replay_capacity is the total over trainers, and an update runs once every trainer holds more than batch_size
+ *     transitions (replay size / G > batch_size);
+ *   - uavrl_learner_tc_route describes one trainer's kernels for a per-trainer size n;
+ *   - refused with UAVRL_ERR_INVALID: n_trainers outside [1, 65535] (one grid row per trainer), lockstep_envs % n_trainers != 0, uavrl_per_enable,
+ *     uavrl_learner_update_batch_per, uavrl_replay_push, uavrl_learner_comm_init / comm_connect / update_dp / compute_grads /
+ *     apply_grads, uavrl_train_run_dp, and act / update_batch sizes that are not multiples of G;
+ *   - the process-wide fused act + step and fused weight-gradient + optimiser paths are not taken (the separate kernels run). */
+int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_trainers, uavrl_learner **out);
+int32_t uavrl_learner_trainer_count(const uavrl_learner *l);
+
 /* state_dict()-ordered flat fp32 parameters (fc1.weight [out][in], fc1.bias, ..., for dueling nets
  * ..., fc_A.weight, fc_A.bias, fc_V.weight, fc_V.bias) -- what torch.save({'model': ...}) holds
  * (DuelingDQN_Trainer.py:79-84).  which: 0 = q_local, 1 = q_target, 2 = Adam exp_avg,
