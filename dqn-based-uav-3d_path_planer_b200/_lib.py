@@ -137,6 +137,10 @@ SIGNATURES = {
     "uavrl_sac_act": (C.c_int, [VP, VP, C.c_int32, VP, VP, VP]),
     "uavrl_sac_update_batch": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP, VP, VP, VP, VP, VP]),
     "uavrl_sac_train_run": (C.c_int, [VP, VP, C.c_int32, C.c_int32, C.POINTER(TrainStats), VP]),
+    "uavrl_sac_smem_bytes": (C.c_int, [C.POINTER(SacConfig), VP]),
+    "uavrl_sac_replay_size": (C.c_int64, [VP]),
+    "uavrl_sac_replay_gather": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP, VP, VP]),
+    "uavrl_sac_update_replay": (C.c_int, [VP, VP, VP, VP, VP, VP]),
     "uavrl_train_run_dp": (C.c_int, [VP, VP, C.c_int32, C.c_float, C.c_int32, VP]),
     "uavrl_train_profile": (C.c_int, [VP, VP, C.c_int32, C.c_float, VP, VP]),
     "uavrl_last_error": (C.c_char_p, []),

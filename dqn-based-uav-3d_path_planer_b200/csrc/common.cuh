@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <atomic>
+#include <mutex>
 #include <string>
 
 #include "../../include/uavrl.h"
@@ -84,6 +85,21 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
 enum PdlPrev { kPdlNone = 0, kPdlAct, kPdlEnv, kPdlTd, kPdlTrain, kPdlDw, kPdlAdam };
 // TcArgs.pdl / kernel flags
 constexpr int kPdlOn = 1, kPdlEarlyWeights = 2, kPdlEarlyRows = 4;
+
+// cudaFuncAttributeMaxDynamicSharedMemorySize belongs to the kernel (process-wide, per device), not to the learner that sets
+// it: raise it to what this instance launches with, never lower it.  Setting it to a smaller instance's size would make every
+// launch of a larger instance that is still alive fail.
+template <class K>
+inline int raise_dyn_smem(K *kernel, size_t bytes)
+{
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lock(mu);
+    cudaFuncAttributes fa;
+    UAVRL_CUDA(cudaFuncGetAttributes(&fa, kernel));
+    if ((size_t)fa.maxDynamicSharedSizeBytes < bytes)
+        UAVRL_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    return 0;
+}
 
 template <class T>
 inline int dev_alloc(T **p, size_t n)

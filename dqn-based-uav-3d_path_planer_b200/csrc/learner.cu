@@ -993,8 +993,8 @@ int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_tra
     if ((rc = dev_alloc(&l->r_act, (size_t)l->slots)) || (rc = dev_alloc(&l->r_rew, (size_t)l->slots)) ||
         (rc = dev_alloc(&l->r_done, (size_t)l->slots)))
         return rc;
-    UAVRL_CUDA(cudaFuncSetAttribute(act_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)act_smem_bytes(l->net)));
-    UAVRL_CUDA(cudaFuncSetAttribute(update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(l->net, l->dual_weights)));
+    if ((rc = raise_dyn_smem(act_kernel, act_smem_bytes(l->net))) || (rc = raise_dyn_smem(update_kernel, upd_smem_bytes(l->net, l->dual_weights))))
+        return rc;
     *out = l;
     return 0;
 }

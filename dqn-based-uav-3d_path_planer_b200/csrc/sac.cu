@@ -26,7 +26,9 @@
 namespace uavrl {
 
 constexpr int kSacA = 2;                 // action_dim of the reference's UAV task (config/Trainer.xml:8,21)
-constexpr int kGld = 64;                 // row stride of the gradient ping-pong planes
+// row stride of the gradient ping-pong planes: a learner's sac_gld() = max(64, round_up(hidden, 32)), the columns
+// layer_backward_dw reads.  The critic kernel also stages s rows across both planes at stride 2 gld (obs_dim <= 124 <= 2 x 64)
+__host__ __device__ inline int sac_gld(int hidden) { const int w = round_up(hidden, 32); return w > 64 ? w : 64; }
 
 struct SacHyper { float actor_lr, critic_lr, alpha_lr, target_entropy, gamma, tau, bound; };
 
@@ -34,6 +36,7 @@ struct SacArgs {
     NetDev actor, critic;
     BatchSrc src;
     int32_t B, n_tiles;
+    int32_t gld;                         // row stride of the gradient planes (sac_gld)
     const float *img_actor, *img_c1, *img_c2, *img_t1, *img_t2;
     const float *eps;                    // [B][A] injected noise (nullptr -> Philox Box-Muller)
     uint64_t key, ctr;
@@ -98,18 +101,22 @@ __device__ void build_critic_input(const float *S, int lds, int obs_dim, float *
     }
 }
 
-// backward of one critic for the tile: dY (head gradient plane, [32][kGld], zero beyond the 2 outputs) -> optional parameter
+// backward of one critic for the tile: dY (head gradient plane, [32][gld], zero beyond the 2 outputs) -> optional parameter
 // gradients into gpart, optional action-input gradient dA[32][A].  Planes of the critic live at rc + act_off.
-__device__ void critic_backward_tile(const NetDev &cn, const float *sw, const float *rc, float *dY, float *dX, float *gpart,
+__device__ void critic_backward_tile(const NetDev &cn, const float *sw, const float *rc, float *dY, float *dX, int gld, float *gpart,
                                      bool accumulate, float (*dA)[kSacA], int obs_dim)
 {
     for (int l = cn.n_layers - 1; l >= 0; --l) {
         const LayerDev &L = cn.L[l];
         const float *Xin = rc + cn.act_off[l];
         const int ldx = cn.act_ld[l];
-        if (gpart) layer_backward_dw(dY, kGld, Xin, ldx, gpart, L, accumulate);
+        if (gpart) layer_backward_dw(dY, gld, Xin, ldx, gpart, L, accumulate);
         if (l > 0) {
-            layer_backward_dx(dY, kGld, sw + L.smem_w, Xin, ldx, dX, kGld, L.in, L.out);
+            layer_backward_dx(dY, gld, sw + L.smem_w, Xin, ldx, dX, gld, L.in, L.out);
+            // the next layer_backward_dx reads dX up to round_up(in, 4) and multiplies the pad by zero weights: the pad must be
+            // zero, not whatever the plane held (0 x NaN is NaN)
+            const int pad = round_up(L.in, 4) - L.in;
+            if (pad && threadIdx.x < kTile * pad) dX[(threadIdx.x / pad) * gld + L.in + threadIdx.x % pad] = 0.f;
             __syncthreads();
             float *tmp = dY; dY = dX; dX = tmp;
         } else if (dA) {
@@ -120,7 +127,7 @@ __device__ void critic_backward_tile(const NetDev &cn, const float *sw, const fl
                 const int ldw = ldw_of(L.out);
                 const float *w = sw + L.smem_w + (obs_dim + j) * ldw;
                 float s = 0.f;
-                for (int o = 0; o < L.out; ++o) s += dY[b * kGld + o] * w[o];
+                for (int o = 0; o < L.out; ++o) s += dY[b * gld + o] * w[o];
                 dA[b][j] = s;
             }
         }
@@ -189,7 +196,8 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
     extern __shared__ __align__(16) float smem[];
     const NetDev &cn = a.critic;
     float *RC = smem, *WC2 = RC + cn.smem_total_floats;
-    float *dYa = WC2 + cn.smem_w_floats, *dYb = dYa + kTile * kGld, *Q = dYb + kTile * kGld;
+    const int gld = a.gld;
+    float *dYa = WC2 + cn.smem_w_floats, *dYb = dYa + kTile * gld, *Q = dYb + kTile * gld;
     __shared__ uint64_t bar[2];
     __shared__ const float *rows[kTile];
     __shared__ float s_act[kTile][kSacA], s_sq[kTile];
@@ -210,9 +218,9 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
             rows[threadIdx.x] = (gb < a.B) ? tr.s : nullptr; s_act[threadIdx.x][0] = tr.ax; s_act[threadIdx.x][1] = tr.ay;
         }
         __syncthreads();
-        load_rows(rows, dYa, kGld * 2, cn.in_dim - kSacA);                  // stage s in the (still unused) gradient planes: 32 x 128
+        load_rows(rows, dYa, gld * 2, cn.in_dim - kSacA);                   // stage s in the (still unused) gradient planes: 32 x 2 gld
         __syncthreads();
-        build_critic_input(dYa, kGld * 2, cn.in_dim - kSacA, RC + cn.act_off[0], cn.act_ld[0], s_act);
+        build_critic_input(dYa, gld * 2, cn.in_dim - kSacA, RC + cn.act_off[0], cn.act_ld[0], s_act);
         if (!ready) { mbar_wait(&bar[0], 0); mbar_wait(&bar[1], 0); ready = true; }
         __syncthreads();
         for (int which = 0; which < 2; ++which) {
@@ -220,7 +228,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
             net_forward(cn, sw, RC + cn.act_off[0], cn.act_ld[0], RC, true, nullptr, nullptr, Q);
             if (threadIdx.x < kTile) {
                 const int b = threadIdx.x, gb = t * kTile + b;
-                float *g = dYa + b * kGld;
+                float *g = dYa + b * gld;
                 for (int o = 0; o < 32; ++o) g[o] = 0.f;
                 float e2 = 0.f;
                 if (gb < a.B)
@@ -233,7 +241,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
             }
             __syncthreads();
             if (threadIdx.x == 0) { float s = 0.f; for (int b = 0; b < kTile; ++b) s += s_sq[b]; sq[which] += s; }
-            critic_backward_tile(cn, sw, RC, dYa, dYb, (which ? a.part_c2 : a.part_c1) + (size_t)blockIdx.x * cn.P, iter > 0, nullptr, 0);
+            critic_backward_tile(cn, sw, RC, dYa, dYb, gld, (which ? a.part_c2 : a.part_c1) + (size_t)blockIdx.x * cn.P, iter > 0, nullptr, 0);
         }
     }
     if (threadIdx.x == 0) { a.stat[blockIdx.x * 4 + 0] = sq[0]; a.stat[blockIdx.x * 4 + 1] = sq[1]; }
@@ -245,7 +253,8 @@ __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
     extern __shared__ __align__(16) float smem[];
     const NetDev &an = a.actor, &cn = a.critic;
     float *RA = smem, *RC = RA + an.smem_total_floats, *WC2 = RC + cn.smem_total_floats;
-    float *dYa = WC2 + cn.smem_w_floats, *dYb = dYa + kTile * kGld, *head = dYb + kTile * kGld, *q1 = head + kTile * 32, *q2 = q1 + kTile * 32;
+    const int gld = a.gld;
+    float *dYa = WC2 + cn.smem_w_floats, *dYb = dYa + kTile * gld, *head = dYb + kTile * gld, *q1 = head + kTile * 32, *q2 = q1 + kTile * 32;
     __shared__ uint64_t bar[3];
     __shared__ const float *rows[kTile];
     __shared__ ActorOut s_o[kTile][kSacA];
@@ -292,7 +301,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
         if (threadIdx.x < kTile) {
             const int b = threadIdx.x, gb = t * kTile + b;
             float l = 0.f, en = 0.f;
-            float *g = dYa + b * kGld;
+            float *g = dYa + b * gld;
             for (int o = 0; o < 32; ++o) g[o] = 0.f;
             for (int j = 0; j < kSacA; ++j) {
                 const float v1 = q1[b * 32 + j], v2 = q2[b * 32 + j];
@@ -306,19 +315,19 @@ __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
         }
         __syncthreads();
         if (threadIdx.x == 0) { float s = 0.f, e = 0.f; for (int b = 0; b < kTile; ++b) { s += s_l[b]; e += s_e[b]; } loss_acc += s; ent_acc += e; }
-        critic_backward_tile(cn, WC2, RC, dYa, dYb, nullptr, false, s_dA2, an.in_dim);              // d/d a through critic 2
+        critic_backward_tile(cn, WC2, RC, dYa, dYb, gld, nullptr, false, s_dA2, an.in_dim);              // d/d a through critic 2
         net_forward(cn, RC, RC + cn.act_off[0], cn.act_ld[0], RC, true, nullptr, nullptr, q1);      // planes back to critic 1
         if (threadIdx.x < kTile) {
-            float *g = dYa + threadIdx.x * kGld;
+            float *g = dYa + threadIdx.x * gld;
             for (int o = 0; o < 32; ++o) g[o] = 0.f;
             for (int j = 0; j < kSacA; ++j) g[j] = s_dq1[threadIdx.x][j];
         }
         __syncthreads();
-        critic_backward_tile(cn, RC, RC, dYa, dYb, nullptr, false, s_dA1, an.in_dim);               // d/d a through critic 1
+        critic_backward_tile(cn, RC, RC, dYa, dYb, gld, nullptr, false, s_dA1, an.in_dim);               // d/d a through critic 1
         // through tanh squash, reparameterisation, tanh / softplus heads to the head pre-activations
         if (threadIdx.x < kTile) {
             const int b = threadIdx.x;
-            float *g = dYa + b * kGld;
+            float *g = dYa + b * gld;
             for (int o = 0; o < 32; ++o) g[o] = 0.f;
             const bool valid = (t * kTile + b) < a.B;
             for (int j = 0; j < kSacA; ++j) {
@@ -335,10 +344,10 @@ __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
         // actor backward: head (dW, dX), trunk (dW)
         {
             const LayerDev &L1 = an.L[1], &L0 = an.L[0];
-            layer_backward_dw(dYa, kGld, RA + an.act_off[1], an.act_ld[1], gpart, L1, iter > 0);
-            layer_backward_dx(dYa, kGld, RA + L1.smem_w, RA + an.act_off[1], an.act_ld[1], dYb, kGld, L1.in, L1.out);
+            layer_backward_dw(dYa, gld, RA + an.act_off[1], an.act_ld[1], gpart, L1, iter > 0);
+            layer_backward_dx(dYa, gld, RA + L1.smem_w, RA + an.act_off[1], an.act_ld[1], dYb, gld, L1.in, L1.out);
             __syncthreads();
-            layer_backward_dw(dYb, kGld, RA + an.act_off[0], an.act_ld[0], gpart, L0, iter > 0);
+            layer_backward_dw(dYb, gld, RA + an.act_off[0], an.act_ld[0], gpart, L0, iter > 0);
             __syncthreads();
         }
     }
@@ -421,14 +430,72 @@ __global__ void __launch_bounds__(kNetThreads) sac_act_kernel(SacArgs a, const f
     }
 }
 
+// uavrl_sac_replay_gather: logical indices of the lockstep ring -> packed rows (one warp per transition)
+__global__ void sac_gather_kernel(int n, int in, BatchSrc src, const int64_t *__restrict__ idx, float *__restrict__ s, float *__restrict__ s2,
+                                  float *__restrict__ a, float *__restrict__ r, uint8_t *__restrict__ d)
+{
+    const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (i >= n) return;
+    const int64_t j = idx[i];
+    const int64_t f = (src.oldest + j / src.n_envs) % src.cap, e = j % src.n_envs;
+    const int64_t slot = f * src.n_envs + e, slot2 = ((f + 1) % src.cap) * src.n_envs + e;
+    for (int k = lane; k < in; k += 32) {
+        if (s) s[(size_t)i * in + k] = src.frames[(size_t)slot * in + k];
+        if (s2) s2[(size_t)i * in + k] = src.frames[(size_t)slot2 * in + k];
+    }
+    if (lane == 0) {
+        if (a) { a[2 * i] = src.act2[2 * slot]; a[2 * i + 1] = src.act2[2 * slot + 1]; }
+        if (r) r[i] = src.rew[slot];
+        if (d) d[i] = src.done_u8[slot];
+    }
+}
+
 }  // namespace uavrl
 
 using namespace uavrl;
 
 // ------------------------------------------------------------------ host handle
+// the two networks of a SAC learner and the stride of its gradient planes: everything the kernels' shared memory follows from
+struct SacShape { NetDev actor, critic; int32_t gld; };
+
+constexpr size_t kSacMaxSmem = 227 * 1024;     // shared memory one block may use on sm_90
+
+// refuses a configuration before anything is allocated
+static int sac_shape(const uavrl_sac_config &c, SacShape &sh)
+{
+    if (c.act_dim != kSacA) return fail(UAVRL_ERR_INVALID, "act_dim must be 2 (the reference's UAV task)");
+    if (c.obs_dim <= 0 || c.obs_dim % 4 != 0) return fail(UAVRL_ERR_INVALID, "obs_dim must be a multiple of 4");
+    if (c.obs_dim > kMaxDim - kSacA) return fail(UAVRL_ERR_INVALID, "obs_dim must be at most 124 (the critic input obs_dim + 2 is at most 128)");
+    if (c.hidden < 1 || c.hidden > kMaxDim) return fail(UAVRL_ERR_INVALID, "hidden must be in [1, 128]");
+    int rc;
+    const int32_t ha[1] = { c.hidden }, hc[2] = { c.hidden, c.hidden };
+    if ((rc = build_mlp(c.obs_dim, 1, ha, kSacA, kSacA, sh.actor))) return rc;              // fc1 -> {fc_mu ; fc_std}
+    if ((rc = build_mlp(c.obs_dim + kSacA, 2, hc, kSacA, 0, sh.critic))) return rc;          // fc1 -> fc2 -> fc_out
+    sh.gld = sac_gld(c.hidden);
+    return 0;
+}
+
+static size_t smem_target(const SacShape &s) { return (size_t)(s.actor.smem_total_floats + s.critic.smem_total_floats + s.critic.smem_w_floats + 3 * kTile * 32) * 4; }
+static size_t smem_critic(const SacShape &s) { return (size_t)(s.critic.smem_total_floats + s.critic.smem_w_floats + 2 * kTile * s.gld + kTile * 32) * 4; }
+static size_t smem_actor(const SacShape &s) { return (size_t)(s.actor.smem_total_floats + s.critic.smem_total_floats + s.critic.smem_w_floats + 2 * kTile * s.gld + 3 * kTile * 32) * 4; }
+static size_t smem_act(const SacShape &s) { return (size_t)(s.actor.smem_total_floats + kTile * 32) * 4; }
+
+// dynamic and static shared memory of one CTA of each kernel: target, critic, actor, act
+static int sac_smem_total(const SacShape &s, size_t out[4])
+{
+    const void *k[4] = { (const void *)sac_target_kernel, (const void *)sac_critic_kernel, (const void *)sac_actor_kernel, (const void *)sac_act_kernel };
+    const size_t dyn[4] = { smem_target(s), smem_critic(s), smem_actor(s), smem_act(s) };
+    for (int i = 0; i < 4; ++i) {
+        cudaFuncAttributes fa;
+        UAVRL_CUDA(cudaFuncGetAttributes(&fa, k[i]));
+        out[i] = dyn[i] + fa.sharedSizeBytes;
+    }
+    return 0;
+}
+
 struct uavrl_sac {
     uavrl_sac_config cfg;
-    NetDev actor, critic;
+    SacShape sh;
     float *p[5] = { nullptr }, *img[5] = { nullptr };      // actor, c1, c2, t1, t2
     float *m[3] = { nullptr }, *v[3] = { nullptr }, *grad[3] = { nullptr };
     int32_t *map_a = nullptr, *map_c = nullptr;
@@ -444,14 +511,9 @@ struct uavrl_sac {
     bool frame0_valid = false;
 };
 
-static size_t smem_target(const uavrl_sac *s) { return (size_t)(s->actor.smem_total_floats + s->critic.smem_total_floats + s->critic.smem_w_floats + 3 * kTile * 32) * 4; }
-static size_t smem_critic(const uavrl_sac *s) { return (size_t)(s->critic.smem_total_floats + s->critic.smem_w_floats + 2 * kTile * kGld + kTile * 32) * 4; }
-static size_t smem_actor(const uavrl_sac *s) { return (size_t)(s->actor.smem_total_floats + s->critic.smem_total_floats + s->critic.smem_w_floats + 2 * kTile * kGld + 3 * kTile * 32) * 4; }
-static size_t smem_act(const uavrl_sac *s) { return (size_t)(s->actor.smem_total_floats + kTile * 32) * 4; }
-
 static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
 {
-    const NetDev &n = role == 0 ? s->actor : s->critic;
+    const NetDev &n = role == 0 ? s->sh.actor : s->sh.critic;
     pack_image_kernel<<<(n.P + 255) / 256, 256, 0, st>>>(n.P, s->p[role], role == 0 ? s->map_a : s->map_c, s->img[role], 0);
     UAVRL_LAUNCHED();
     return 0;
@@ -460,7 +522,7 @@ static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
 static void sac_fill_args(uavrl_sac *s, SacArgs &a, const BatchSrc &src, int B, const float *eps, uint64_t ctr)
 {
     memset(&a, 0, sizeof(a));
-    a.actor = s->actor; a.critic = s->critic; a.src = src; a.B = B; a.n_tiles = (B + kTile - 1) / kTile;
+    a.actor = s->sh.actor; a.critic = s->sh.critic; a.src = src; a.B = B; a.n_tiles = (B + kTile - 1) / kTile; a.gld = s->sh.gld;
     a.img_actor = s->img[0]; a.img_c1 = s->img[1]; a.img_c2 = s->img[2]; a.img_t1 = s->img[3]; a.img_t2 = s->img[4];
     a.eps = eps; a.key = s->cfg.seed ^ 0x5AC5ull; a.ctr = ctr; a.log_alpha = s->scal; a.td = s->td;
     a.part_a = s->part[0]; a.part_c1 = s->part[1]; a.part_c2 = s->part[2]; a.stat = s->stat;
@@ -492,27 +554,27 @@ static int sac_update_impl(uavrl_sac *s, const BatchSrc &src, int B, const float
     const int grid = n_tiles < s->max_ctas ? n_tiles : s->max_ctas;
     s->adam_t += 1;
     sac_fill_args(s, a, src, B, eps_next, 2 * (uint64_t)s->epoch);
-    sac_target_kernel<<<grid, kNetThreads, smem_target(s), st>>>(a);
+    sac_target_kernel<<<grid, kNetThreads, smem_target(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
-    sac_critic_kernel<<<grid, kNetThreads, smem_critic(s), st>>>(a);
+    sac_critic_kernel<<<grid, kNetThreads, smem_critic(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
     AdamArgs aa;
     for (int c = 1; c <= 2; ++c) {
-        adam_args(aa, s->critic.P, grid, s->cfg.critic_lr, s->adam_t);
+        adam_args(aa, s->sh.critic.P, grid, s->cfg.critic_lr, s->adam_t);
         reduce_adam_kernel<<<(aa.P + 63) / 64, 256, 0, st>>>(aa, s->part[c], s->lossbuf, s->grad[c], s->p[c], s->m[c], s->v[c], nullptr, s->img[c],
                                                              nullptr, s->map_c, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
         UAVRL_LAUNCHED();
     }
     sac_fill_args(s, a, src, B, eps_cur, 2 * (uint64_t)s->epoch + 1);
-    sac_actor_kernel<<<grid, kNetThreads, smem_actor(s), st>>>(a);
+    sac_actor_kernel<<<grid, kNetThreads, smem_actor(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
-    adam_args(aa, s->actor.P, grid, s->cfg.actor_lr, s->adam_t);
+    adam_args(aa, s->sh.actor.P, grid, s->cfg.actor_lr, s->adam_t);
     reduce_adam_kernel<<<(aa.P + 63) / 64, 256, 0, st>>>(aa, s->part[0], s->lossbuf, s->grad[0], s->p[0], s->m[0], s->v[0], nullptr, s->img[0], nullptr,
                                                          s->map_a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     UAVRL_LAUNCHED();
     SacFinishArgs f;
     memset(&f, 0, sizeof(f));
-    f.Pc = s->critic.P; f.nparts = grid; f.tau = s->cfg.tau; f.alpha_lr = s->cfg.alpha_lr; f.target_entropy = s->cfg.target_entropy;
+    f.Pc = s->sh.critic.P; f.nparts = grid; f.tau = s->cfg.tau; f.alpha_lr = s->cfg.alpha_lr; f.target_entropy = s->cfg.target_entropy;
     f.inv_n = 1.f / ((float)B * (float)kSacA); f.do_alpha = 1;
     const double bc1 = 1.0 - pow(0.9, (double)s->adam_t), bc2 = 1.0 - pow(0.999, (double)s->adam_t);
     f.step_size_scale = (float)((double)s->cfg.alpha_lr / bc1); f.bc2_sqrt = (float)sqrt(bc2);
@@ -522,42 +584,24 @@ static int sac_update_impl(uavrl_sac *s, const BatchSrc &src, int B, const float
     return 0;
 }
 
-extern "C" {
 
-int uavrl_sac_create(const uavrl_sac_config *cfg, uavrl_sac **out)
+// everything a learner allocates; on failure the caller destroys the half-built handle
+static int sac_alloc(uavrl_sac *s)
 {
-    if (!cfg || !out) return fail(UAVRL_ERR_INVALID, "uavrl_sac_create: null argument");
-    if (cfg->act_dim != kSacA) return fail(UAVRL_ERR_INVALID, "act_dim must be 2 (the reference's UAV task)");
-    if (cfg->batch_size <= 0 || cfg->replay_capacity <= 0) return fail(UAVRL_ERR_INVALID, "batch_size and replay_capacity must be > 0");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(UAVRL_ERR_CUDA, "no CUDA device: the SAC learner has no CPU fallback");
-    UAVRL_CUDA(cudaSetDevice(cfg->device));
-    uavrl_sac *s = new uavrl_sac();
-    s->cfg = *cfg;
-    {   // grid cap of the tile kernels: 4 CTAs per SM's worth of tiles, i.e. one tile per CTA up to batch 4 x SMs x 32.  (One CTA
-        // per SM looping over its tiles would accumulate ONE partial, at the price of a read-modify-write of the global partial
-        // per tile.)
-        const char *ov = getenv("UAVRL_SAC_MAX_CTAS");            // tests: force the multi-tile (accumulating) path on a small batch
-        if (ov && atoi(ov) > 0) s->max_ctas = atoi(ov);
-    }
+    const uavrl_sac_config *cfg = &s->cfg;
     int rc;
-    const int32_t ha[1] = { cfg->hidden }, hc[2] = { cfg->hidden, cfg->hidden };
-    if ((rc = build_mlp(cfg->obs_dim, 1, ha, kSacA, kSacA, s->actor))) return rc;              // fc1 -> {fc_mu ; fc_std}
-    if ((rc = build_mlp(cfg->obs_dim + kSacA, 2, hc, kSacA, 0, s->critic))) return rc;          // fc1 -> fc2 -> fc_out
-    if (cfg->obs_dim % 4 != 0) return fail(UAVRL_ERR_INVALID, "obs_dim must be a multiple of 4");
-    if (smem_target(s) > 227 * 1024 || smem_actor(s) > 227 * 1024) return fail(UAVRL_ERR_INVALID, "networks too large for the SMEM-resident SAC kernels");
     for (int r = 0; r < 5; ++r) {
-        const NetDev &n = r == 0 ? s->actor : s->critic;
+        const NetDev &n = r == 0 ? s->sh.actor : s->sh.critic;
         if ((rc = dev_alloc(&s->p[r], (size_t)n.P)) || (rc = dev_alloc(&s->img[r], (size_t)n.smem_w_floats))) return rc;
     }
     for (int r = 0; r < 3; ++r) {
-        const NetDev &n = r == 0 ? s->actor : s->critic;
+        const NetDev &n = r == 0 ? s->sh.actor : s->sh.critic;
         if ((rc = dev_alloc(&s->m[r], (size_t)n.P)) || (rc = dev_alloc(&s->v[r], (size_t)n.P)) || (rc = dev_alloc(&s->grad[r], (size_t)n.P)) ||
             (rc = dev_alloc(&s->part[r], (size_t)n.P * s->max_ctas)))
             return rc;
     }
     std::vector<int32_t> ma, mc;
-    build_image_map(s->actor, ma); build_image_map(s->critic, mc);
+    build_image_map(s->sh.actor, ma); build_image_map(s->sh.critic, mc);
     if ((rc = dev_alloc(&s->map_a, ma.size())) || (rc = dev_alloc(&s->map_c, mc.size()))) return rc;
     UAVRL_CUDA(cudaMemcpy(s->map_a, ma.data(), ma.size() * 4, cudaMemcpyHostToDevice));
     UAVRL_CUDA(cudaMemcpy(s->map_c, mc.data(), mc.size() * 4, cudaMemcpyHostToDevice));
@@ -577,10 +621,59 @@ int uavrl_sac_create(const uavrl_sac_config *cfg, uavrl_sac **out)
             (rc = dev_alloc(&s->r_done, slots)))
             return rc;
     }
-    UAVRL_CUDA(cudaFuncSetAttribute(sac_target_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_target(s)));
-    UAVRL_CUDA(cudaFuncSetAttribute(sac_critic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_critic(s)));
-    UAVRL_CUDA(cudaFuncSetAttribute(sac_actor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_actor(s)));
-    UAVRL_CUDA(cudaFuncSetAttribute(sac_act_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_act(s)));
+    if ((rc = raise_dyn_smem(sac_target_kernel, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel, smem_critic(s->sh))) ||
+        (rc = raise_dyn_smem(sac_actor_kernel, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel, smem_act(s->sh))))
+        return rc;
+    return 0;
+}
+
+extern "C" {
+
+int uavrl_sac_smem_bytes(const uavrl_sac_config *cfg, int64_t *bytes_out)
+{
+    if (!cfg || !bytes_out) return fail(UAVRL_ERR_INVALID, "uavrl_sac_smem_bytes: null argument");
+    SacShape sh;
+    int rc = sac_shape(*cfg, sh);
+    if (rc) return rc;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(UAVRL_ERR_CUDA, "no CUDA device: the SAC learner has no CPU fallback");
+    UAVRL_CUDA(cudaSetDevice(cfg->device));
+    size_t b[4];
+    if ((rc = sac_smem_total(sh, b))) return rc;
+    for (int i = 0; i < 4; ++i) bytes_out[i] = (int64_t)b[i];
+    return 0;
+}
+
+int uavrl_sac_create(const uavrl_sac_config *cfg, uavrl_sac **out)
+{
+    if (!cfg || !out) return fail(UAVRL_ERR_INVALID, "uavrl_sac_create: null argument");
+    if (cfg->batch_size <= 0 || cfg->replay_capacity <= 0) return fail(UAVRL_ERR_INVALID, "batch_size and replay_capacity must be > 0");
+    SacShape sh;
+    int rc = sac_shape(*cfg, sh);
+    if (rc) return rc;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(UAVRL_ERR_CUDA, "no CUDA device: the SAC learner has no CPU fallback");
+    UAVRL_CUDA(cudaSetDevice(cfg->device));
+    size_t smem[4];
+    if ((rc = sac_smem_total(sh, smem))) return rc;
+    for (int i = 0; i < 4; ++i)
+        if (smem[i] > kSacMaxSmem)
+            return fail(UAVRL_ERR_INVALID, "networks too large for the SMEM-resident SAC kernels: " + std::to_string(smem[i]) +
+                                               " B of shared memory per block, at most " + std::to_string(kSacMaxSmem));
+    uavrl_sac *s = new uavrl_sac();
+    s->cfg = *cfg;
+    s->sh = sh;
+    {   // grid cap of the tile kernels: 4 CTAs per SM's worth of tiles, i.e. one tile per CTA up to batch 4 x SMs x 32.  (One CTA
+        // per SM looping over its tiles would accumulate ONE partial, at the price of a read-modify-write of the global partial
+        // per tile.)
+        const char *ov = getenv("UAVRL_SAC_MAX_CTAS");            // tests: force the multi-tile (accumulating) path on a small batch
+        if (ov && atoi(ov) > 0) s->max_ctas = atoi(ov);
+    }
+    if ((rc = sac_alloc(s))) {
+        uavrl_sac_destroy(s);
+        cudaGetLastError();                                  // a failed cudaMalloc must not surface at the next launch check
+        return rc;
+    }
     *out = s;
     return 0;
 }
@@ -598,23 +691,25 @@ int uavrl_sac_destroy(uavrl_sac *s)
     return 0;
 }
 
-int64_t uavrl_sac_param_count(const uavrl_sac *s, int32_t role) { return !s ? 0 : (role == 0 ? s->actor.P : s->critic.P); }
+int64_t uavrl_sac_param_count(const uavrl_sac *s, int32_t role) { return !s ? 0 : (role == 0 ? s->sh.actor.P : s->sh.critic.P); }
 
 static float *sac_buf(uavrl_sac *s, int role)
 {
     if (role >= 0 && role < 5) return s->p[role];
     if (role >= 5 && role < 8) return s->m[role - 5];
     if (role >= 8 && role < 11) return s->v[role - 8];
+    if (role >= 11 && role < 14) return s->grad[role - 11];        // last reduced gradients: read-only
     return nullptr;
 }
 
 int uavrl_sac_set_params(uavrl_sac *s, int32_t role, const float *h)
 {
     if (!s || !h || !sac_buf(s, role)) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (role >= 11) return fail(UAVRL_ERR_INVALID, "roles 11-13 (the last reduced gradients) are read-only");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     UAVRL_CUDA(cudaDeviceSynchronize());
     const int rr = role < 5 ? role : (role - 5) % 3;
-    const int P = rr == 0 ? s->actor.P : s->critic.P;
+    const int P = rr == 0 ? s->sh.actor.P : s->sh.critic.P;
     UAVRL_CUDA(cudaMemcpy(sac_buf(s, role), h, (size_t)P * 4, cudaMemcpyHostToDevice));
     if (role < 5) { int rc = sac_pack(s, role, 0); if (rc) return rc; UAVRL_CUDA(cudaDeviceSynchronize()); }
     return 0;
@@ -626,7 +721,7 @@ int uavrl_sac_get_params(uavrl_sac *s, int32_t role, float *h)
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     UAVRL_CUDA(cudaDeviceSynchronize());
     const int rr = role < 5 ? role : (role - 5) % 3;
-    const int P = rr == 0 ? s->actor.P : s->critic.P;
+    const int P = rr == 0 ? s->sh.actor.P : s->sh.critic.P;
     UAVRL_CUDA(cudaMemcpy(h, sac_buf(s, role), (size_t)P * 4, cudaMemcpyDeviceToHost));
     return 0;
 }
@@ -666,7 +761,7 @@ int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *ep
     memset(&none, 0, sizeof(none));
     sac_fill_args(s, a, none, n, eps_dev, 0x8000000000000000ull | s->calls++);
     const int grid = a.n_tiles < s->max_ctas ? a.n_tiles : s->max_ctas;
-    sac_act_kernel<<<grid, kNetThreads, smem_act(s), (cudaStream_t)stream>>>(a, obs_dev, n, actions_dev);
+    sac_act_kernel<<<grid, kNetThreads, smem_act(s->sh), (cudaStream_t)stream>>>(a, obs_dev, n, actions_dev);
     UAVRL_LAUNCHED();
     return 0;
 }
@@ -681,6 +776,65 @@ int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const fl
     memset(&src, 0, sizeof(src));
     src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.act2 = a_dev; src.rew = r_dev; src.done_f32 = d_dev;
     return sac_update_impl(s, src, B, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
+}
+
+// the lockstep ring as a batch source: idx_tape (device, [batch_size] logical indices, 0 = oldest) or Philox sampling keyed
+// by the epoch
+static BatchSrc sac_ring_source(const uavrl_sac *s, const int32_t *idx_tape)
+{
+    const int64_t N = s->cfg.lockstep_envs, R = s->ring_frames;
+    BatchSrc src;
+    memset(&src, 0, sizeof(src));
+    src.mode = kReplayLockstep; src.frames = s->frames; src.act2 = s->r_act2; src.rew = s->r_rew; src.done_u8 = s->r_done;
+    src.count = s->count; src.cap = R; src.n_envs = (int32_t)N;
+    src.oldest = ((s->head - s->count / N) % R + R) % R;
+    src.key = s->cfg.seed ^ 0x5EEDull; src.epoch = (uint64_t)s->epoch;
+    src.idx_tape = idx_tape;
+    return src;
+}
+
+int64_t uavrl_sac_replay_size(const uavrl_sac *s) { return s ? s->count : 0; }
+
+int uavrl_sac_replay_gather(uavrl_sac *s, int32_t n, const int64_t *idx, float *s_host, float *a_host, float *r_host, float *s2_host,
+                            uint8_t *d_host)
+{
+    if (!s || n <= 0 || !idx) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (!s->frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
+    for (int i = 0; i < n; ++i)
+        if (idx[i] < 0 || idx[i] >= s->count) return fail(UAVRL_ERR_INVALID, "logical index out of range");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    UAVRL_CUDA(cudaDeviceSynchronize());
+    const BatchSrc src = sac_ring_source(s, nullptr);
+    const size_t in = (size_t)s->cfg.obs_dim;
+    int64_t *d_idx = nullptr; float *d_s = nullptr, *d_s2 = nullptr, *d_a = nullptr, *d_r = nullptr; uint8_t *d_d = nullptr;
+    struct Free { void **p[6]; ~Free() { for (auto q : p) if (*q) cudaFree(*q); } } guard{ { (void **)&d_idx, (void **)&d_s, (void **)&d_s2,
+                                                                                             (void **)&d_a, (void **)&d_r, (void **)&d_d } };
+    UAVRL_CUDA(cudaMalloc((void **)&d_idx, (size_t)n * 8));
+    UAVRL_CUDA(cudaMemcpy(d_idx, idx, (size_t)n * 8, cudaMemcpyHostToDevice));
+    if (s_host) UAVRL_CUDA(cudaMalloc((void **)&d_s, (size_t)n * in * 4));
+    if (s2_host) UAVRL_CUDA(cudaMalloc((void **)&d_s2, (size_t)n * in * 4));
+    if (a_host) UAVRL_CUDA(cudaMalloc((void **)&d_a, (size_t)n * kSacA * 4));
+    if (r_host) UAVRL_CUDA(cudaMalloc((void **)&d_r, (size_t)n * 4));
+    if (d_host) UAVRL_CUDA(cudaMalloc((void **)&d_d, (size_t)n));
+    sac_gather_kernel<<<(n + 7) / 8, 256>>>(n, (int)in, src, d_idx, d_s, d_s2, d_a, d_r, d_d);
+    UAVRL_CUDA(cudaGetLastError());
+    if (s_host) UAVRL_CUDA(cudaMemcpy(s_host, d_s, (size_t)n * in * 4, cudaMemcpyDeviceToHost));
+    if (s2_host) UAVRL_CUDA(cudaMemcpy(s2_host, d_s2, (size_t)n * in * 4, cudaMemcpyDeviceToHost));
+    if (a_host) UAVRL_CUDA(cudaMemcpy(a_host, d_a, (size_t)n * kSacA * 4, cudaMemcpyDeviceToHost));
+    if (r_host) UAVRL_CUDA(cudaMemcpy(r_host, d_r, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    if (d_host) UAVRL_CUDA(cudaMemcpy(d_host, d_d, (size_t)n, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const float *eps_next_dev, const float *eps_cur_dev, float *losses_dev,
+                            void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (!s->frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    s->epoch += 1;                                             // SAC_Trainer.py:320
+    if (s->count <= s->cfg.batch_size) return 0;               // PathPlan_City.py:383: nothing sampled yet
+    return sac_update_impl(s, sac_ring_source(s, idx_tape_dev), s->cfg.batch_size, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
 }
 
 // lockstep loop with the continuous env step: state -> actor sample -> Move_Agent -> replay add -> update
@@ -712,13 +866,7 @@ int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t d
         if (do_update) {
             s->epoch += 1;
             if (s->count <= s->cfg.batch_size) continue;
-            BatchSrc src;
-            memset(&src, 0, sizeof(src));
-            src.mode = kReplayLockstep; src.frames = s->frames; src.act2 = s->r_act2; src.rew = s->r_rew; src.done_u8 = s->r_done;
-            src.count = s->count; src.cap = R; src.n_envs = (int32_t)N;
-            src.oldest = ((s->head - s->count / N) % R + R) % R;
-            src.key = s->cfg.seed ^ 0x5EEDull; src.epoch = (uint64_t)s->epoch;
-            if ((rc = sac_update_impl(s, src, s->cfg.batch_size, nullptr, nullptr, nullptr, st))) return rc;
+            if ((rc = sac_update_impl(s, sac_ring_source(s, nullptr), s->cfg.batch_size, nullptr, nullptr, nullptr, st))) return rc;
             ++updates;
         }
     }

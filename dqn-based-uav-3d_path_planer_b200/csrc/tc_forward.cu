@@ -439,8 +439,7 @@ int tc_init(uavrl_learner *l)
     UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->G * l->cfg.batch_size * 4));
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du)
-            UAVRL_CUDA(cudaFuncSetAttribute(pick_forward_kernel(false, ac != 0, du != 0, fixed), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)tc_smem_bytes(l->tc)));
+            if (int rc = raise_dyn_smem(pick_forward_kernel(false, ac != 0, du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
     {   // the fused act+step variant carries the env scratch as static shared memory on top: it must still fit one CTA
         l->fuse_ok = true;
         for (int du = 0; du < 2; ++du) {
@@ -450,8 +449,7 @@ int tc_init(uavrl_learner *l)
         }
         if (l->fuse_ok)
             for (int du = 0; du < 2; ++du)
-                UAVRL_CUDA(cudaFuncSetAttribute(pick_forward_kernel(true, true, du != 0, fixed), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                (int)tc_smem_bytes(l->tc)));
+                if (int rc = raise_dyn_smem(pick_forward_kernel(true, true, du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
     }
     l->y_cap = l->cfg.batch_size;
     l->tc_ok = true;

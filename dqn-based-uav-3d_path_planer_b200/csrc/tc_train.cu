@@ -774,10 +774,9 @@ int tc_train_init(uavrl_learner *l)
     tc.train_max_rows = train_smem_bytes(tc, 64) <= train_budget ? 64 : 32;
     for (int np = 0; np < 3; ++np)
         for (int du = 0; du < 2; ++du)
-            UAVRL_CUDA(cudaFuncSetAttribute(pick_train_kernel(np, du != 0, fixed), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)train_smem_bytes(tc, tc.train_max_rows)));
-    UAVRL_CUDA(cudaFuncSetAttribute(tc_dw_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dw_smem_bytes(tc)));
-    UAVRL_CUDA(cudaFuncSetAttribute(tc_dw_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dw_smem_bytes(tc)));
+            if (int rc = raise_dyn_smem(pick_train_kernel(np, du != 0, fixed), train_smem_bytes(tc, tc.train_max_rows))) return rc;
+    if (int rc = raise_dyn_smem(tc_dw_kernel<false>, dw_smem_bytes(tc))) return rc;
+    if (int rc = raise_dyn_smem(tc_dw_kernel<true>, dw_smem_bytes(tc))) return rc;
     const size_t cap = (size_t)l->cfg.batch_size, G = (size_t)l->G;
     UAVRL_CUDA(cudaMalloc((void **)&l->act_buf, G * cap * (size_t)(tc.act_stride > 0 ? tc.act_stride : 4) * 4));
     UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, G * cap * (size_t)tc.dz_stride * 4));

@@ -486,7 +486,9 @@ def train_run_dp(env, learner, n_iters, eps, global_batch):
 
 
 class SacLearner:
-    """SAC continuous (the reference's shipped trainer, config/Trainer.xml) on one GPU."""
+    """SAC continuous (the reference's shipped trainer, config/Trainer.xml) on one GPU.  obs_dim must be a multiple of 4 in
+    [4, 124], hidden in [1, 128], and the networks must fit the kernels' shared memory (sac_smem_bytes).  Parameter roles:
+    0-4 actor, critic_1, critic_2 and their targets, 5-7 / 8-10 Adam moments, 11-13 the last reduced gradients (read-only)."""
     ROLES = ("actor", "critic_1", "critic_2", "target_critic_1", "target_critic_2")
 
     def __init__(self, obs_dim=OBS_DIM, hidden=64, act_dim=2, action_bound=1.0, actor_lr=1e-4, critic_lr=1e-3, alpha_lr=1e-4,
@@ -551,6 +553,41 @@ class SacLearner:
     def update_batch(self, s, a, r, s2, d, eps_next=None, eps_cur=None, losses=None):
         check(_lib.lib().uavrl_sac_update_batch(self.h, s.shape[0], _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d), _ptr(eps_next),
                                                 _ptr(eps_cur), _ptr(losses), _stream(self.device)))
+
+    def grads(self, role):
+        """The gradient of network `role` (0 actor, 1 critic_1, 2 critic_2) that the last update reduced and fed to Adam."""
+        return self.get_params(11 + role)
+
+    def smem_bytes(self):
+        """Shared memory per block of the target, critic, actor and get_action kernels (see sac_smem_bytes)."""
+        return sac_smem_bytes(self.cfg.obs_dim, self.cfg.hidden, self.cfg.device)
+
+    def replay_size(self):
+        return int(_lib.lib().uavrl_sac_replay_size(self.h))
+
+    def gather(self, logical_idx):
+        """Transitions of the lockstep ring by logical index (0 = oldest): s, a [n, 2], r, s2, d."""
+        idx = np.ascontiguousarray(logical_idx, np.int64)
+        n, o = idx.size, self.cfg.obs_dim
+        s = np.zeros((n, o), np.float32); s2 = np.zeros((n, o), np.float32)
+        a = np.zeros((n, 2), np.float32); r = np.zeros(n, np.float32); d = np.zeros(n, np.uint8)
+        check(_lib.lib().uavrl_sac_replay_gather(self.h, n, _ptr(idx), _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d)))
+        return s, a, r, s2, d
+
+    def update_replay(self, idx_tape=None, eps_next=None, eps_cur=None, losses=None):
+        """One update sampled from the lockstep ring (idx_tape: device int32 [batch_size] logical indices, None = Philox)."""
+        check(_lib.lib().uavrl_sac_update_replay(self.h, _ptr(idx_tape), _ptr(eps_next), _ptr(eps_cur), _ptr(losses),
+                                                 _stream(self.device)))
+
+
+def sac_smem_bytes(obs_dim, hidden, device=0):
+    """Shared memory (dynamic + static bytes) one block of each SAC kernel takes for these networks: [target, critic update,
+    actor update, get_action].  SacLearner refuses the shape when any exceeds 227 KB (232 448 B)."""
+    c = _lib.SacConfig()
+    c.obs_dim, c.hidden, c.act_dim, c.device = int(obs_dim), int(hidden), 2, int(device)
+    out = np.zeros(4, np.int64)
+    check(_lib.lib().uavrl_sac_smem_bytes(C.byref(c), _ptr(out)))
+    return [int(x) for x in out]
 
 
 def sac_train_run(env, sac, n_iters, do_update=True, want_stats=True):

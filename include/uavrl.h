@@ -317,10 +317,17 @@ typedef struct {
     int32_t device;
 } uavrl_sac_config;
 
+/* Limits: obs_dim a multiple of 4 in [4, 124] (the critic input obs_dim + 2 is at most 128), hidden in [1, 128], and every
+ * SAC kernel's shared memory (the networks are resident in it) at most 227 KB per block.  Refused with UAVRL_ERR_INVALID before
+ * anything is allocated. */
 int uavrl_sac_create(const uavrl_sac_config *cfg, uavrl_sac **out);
 int uavrl_sac_destroy(uavrl_sac *s);
+/* Shared memory (dynamic + static bytes) one block of each SAC kernel would take for cfg's networks: bytes_out[4] = target,
+ * critic update, actor update, get_action.  uavrl_sac_create refuses cfg when any exceeds 227 KB (232 448 B). */
+int uavrl_sac_smem_bytes(const uavrl_sac_config *cfg, int64_t *bytes_out);
 /* role: 0 actor, 1 critic_1, 2 critic_2, 3 target_critic_1, 4 target_critic_2 (flat state_dict order:
- * actor = fc1, fc_mu, fc_std; critic = fc1, fc2, fc_out); 5..7 Adam exp_avg of actor/critic_1/critic_2, 8..10 exp_avg_sq */
+ * actor = fc1, fc_mu, fc_std; critic = fc1, fc2, fc_out); 5..7 Adam exp_avg of actor/critic_1/critic_2, 8..10 exp_avg_sq;
+ * 11..13 the gradients of actor/critic_1/critic_2 the last update reduced over its batch and fed to Adam (get only) */
 int64_t uavrl_sac_param_count(const uavrl_sac *s, int32_t role);
 int uavrl_sac_set_params(uavrl_sac *s, int32_t role, const float *params_host);
 int uavrl_sac_get_params(uavrl_sac *s, int32_t role, float *params_host);
@@ -334,6 +341,16 @@ int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *ep
  * {actor_loss, critic_1_loss, critic_2_loss, d alpha_loss / d log_alpha}. */
 int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev,
                            const float *d_dev, const float *eps_next_dev, const float *eps_cur_dev, float *losses_dev, void *stream);
+/* The lockstep replay ring (lockstep_envs > 0): uavrl_sac_replay_size = transitions held; uavrl_sac_replay_gather reads n of
+ * them back by logical index (0 = oldest; k -> frame k / N, env k % N) into host arrays s/s2 [n][obs], a [n][2], r [n], d [n]. */
+int64_t uavrl_sac_replay_size(const uavrl_sac *s);
+int uavrl_sac_replay_gather(uavrl_sac *s, int32_t n, const int64_t *logical_idx_host, float *s_host, float *a_host, float *r_host,
+                            float *s2_host, uint8_t *d_host);
+/* One SAC_Trainer.update sampled from the lockstep ring, as uavrl_sac_train_run performs it: epoch += 1, skipped while the ring
+ * holds <= batch_size transitions.  idx_tape_dev [batch_size] injects logical indices (NULL = Philox sampling); eps_next / eps_cur
+ * and losses_dev as in uavrl_sac_update_batch. */
+int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const float *eps_next_dev, const float *eps_cur_dev, float *losses_dev,
+                            void *stream);
 /* PathPlan_City.run_thread_OffPolicy + update with the SAC trainer and the reference's continuous step, N envs in lockstep */
 int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t do_update, uavrl_train_stats *stats_host, void *stream);
 
