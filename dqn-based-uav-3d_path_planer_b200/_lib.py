@@ -104,6 +104,7 @@ SIGNATURES = {
     "uavrl_learner_create": (C.c_int, [C.POINTER(LearnerConfig), C.POINTER(VP)]),
     "uavrl_learner_create_trainers": (C.c_int, [C.POINTER(LearnerConfig), C.c_int32, C.POINTER(VP)]),
     "uavrl_learner_trainer_count": (C.c_int32, [VP]),
+    "uavrl_learner_federate": (C.c_int, [VP, VP, VP, VP, VP, VP, VP]),
     "uavrl_learner_destroy": (C.c_int, [VP]),
     "uavrl_learner_param_count": (C.c_int64, [VP]),
     "uavrl_learner_set_params": (C.c_int, [VP, C.c_int32, VP]),

@@ -1,0 +1,197 @@
+// federate.cu -- selective federated aggregation across the trainers of a grouped learner, sm_90a.
+//
+// Replaces Envs/PathPlan_City.py:644-684 (Federated_Learning_choice), the reference's aggregation for DQN-family trainers.
+// Round p = 0 .. G-1, in this order and in place:
+//   1. probe states: 10 distinct transitions of trainer p's own replay (random.sample), their state rows;
+//   2. q_value = Q_p(probes) with trainer p's parameters as they stand (they change only in round p);
+//   3. loss_q = mse(q_value, Q_q(probes)) for every q != p with trainer q's CURRENT parameters (already replaced for q < p);
+//   4. the stable sort by loss (equal losses keep ascending q), the first k = (G - 1) / 2;
+//   5. theta_p <- (theta_p + theta_c0 + theta_c1 + ...) / (k + 1): float32, left to right, one division;
+//   6. only q_local is written (replace_param); q_target, the Adam moments and the counters stay.
+//
+// Schedule (every launch on the caller's stream, no host synchronisation):
+//   probe rows (ring: one gather kernel)          -> probes [G][10][in]
+//   the act pass on the probes                    -> q_ref [G][10][A]          (block g of rows -> trainer g)
+//   loss variant of the act pass, G weight sets   -> M[p][q], q > p, initial parameters (stay valid until round p)
+//   per round p: rank (M row p) -> average -> refresh trainer p's fp32 / tensor-core images -> loss variant with the new
+//                theta_p on the probes of every p' > p -> column p of M
+// so the forwards evaluate G (G - 1) 10 rows in all, and a call makes 5 G + 2 kernel launches (4 G + 2 without tensor cores;
+// one fewer with explicit probe states) plus three memsets.
+#include "learner.cuh"
+#include "mlp_tile.cuh"
+#include "tc_forward.cuh"
+
+#include <string.h>
+
+namespace uavrl {
+
+// probe states of every trainer from the lockstep ring: 10 distinct trainer-local logical indices (perm_index keyed by
+// seed + g and the call counter, or row g of a [G][10] tape), their state rows copied to probes[g]
+__global__ void fed_probe_kernel(BatchSrc src, int in_dim, uint64_t fed_key, uint64_t call, float *__restrict__ probes,
+                                 int32_t *__restrict__ idx_out)
+{
+    __shared__ const float *rows[kFedProbes];
+    const int g = blockIdx.x;
+    if (threadIdx.x < kFedProbes) {
+        BatchSrc sg = trainer_src(src, g, kFedProbes, in_dim);
+        sg.key = trainer_key(fed_key, kFedSalt, g);
+        uint32_t pkey[4];
+        Philox::gen(sg.key, call, 0xFEDull, pkey);
+        const int s = threadIdx.x;
+        const int64_t j = sg.idx_tape ? (int64_t)sg.idx_tape[s] : (int64_t)perm_index((uint64_t)s, (uint64_t)sg.count, pkey);
+        const float *sp, *s2p;
+        resolve_rows(sg, s, in_dim, pkey, sp, s2p);
+        rows[s] = sp;
+        if (idx_out) idx_out[(size_t)g * kFedProbes + s] = (int32_t)j;
+    }
+    __syncthreads();
+    float *out = probes + (size_t)g * kFedProbes * in_dim;
+    for (int i = threadIdx.x; i < kFedProbes * in_dim; i += blockDim.x) out[i] = rows[i / in_dim][i % in_dim];
+}
+
+// loss -> an unsigned key with the order of the floats (NaN last)
+__device__ __forceinline__ uint32_t loss_key(float x)
+{
+    const uint32_t u = __float_as_uint(x);
+    if (x != x) return 0xFFFFFFFFu;
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// round p's selection: candidate q's rank among q' != p under (loss, index); rank < k -> chosen[p][rank] = q.  One thread per
+// candidate over any number of CTAs; row p of M is staged through shared memory in chunks.
+constexpr int kRankChunk = 2048;
+__global__ void __launch_bounds__(256) fed_rank_kernel(int G, int p, int k, int kk, const float *__restrict__ M, int32_t *__restrict__ chosen)
+{
+    __shared__ uint32_t keys[kRankChunk];
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    const float *row = M + (size_t)p * G;
+    const uint32_t kq = q < G ? loss_key(row[q]) : 0u;
+    int rank = 0;
+    for (int c0 = 0; c0 < G; c0 += kRankChunk) {
+        const int n = G - c0 < kRankChunk ? G - c0 : kRankChunk;
+        __syncthreads();
+        for (int i = threadIdx.x; i < n; i += blockDim.x) keys[i] = loss_key(row[c0 + i]);
+        __syncthreads();
+        if (q < G && q != p)
+            for (int i = 0; i < n; ++i) {
+                const int q2 = c0 + i;
+                const uint32_t k2 = keys[i];
+                rank += (q2 != p) && (k2 < kq || (k2 == kq && q2 < q));
+            }
+    }
+    if (q < G && q != p && rank < k) chosen[(size_t)p * kk + rank] = q;
+}
+
+// theta_p <- (theta_p + theta_c0 + ... + theta_c{k-1}) / (k + 1): every addition and the division individually rounded (no FMA
+// contraction, no reassociation); the loads of 8 chosen rows are issued ahead of their additions
+__global__ void __launch_bounds__(256) fed_average_kernel(int P, int p, int k, const int32_t *__restrict__ chosen, float *__restrict__ local)
+{
+    __shared__ int32_t c[256];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    float s = i < P ? local[(size_t)p * P + i] : 0.f;
+    for (int j0 = 0; j0 < k; j0 += 256) {
+        const int n = k - j0 < 256 ? k - j0 : 256;
+        __syncthreads();
+        if ((int)threadIdx.x < n) c[threadIdx.x] = chosen[j0 + threadIdx.x];
+        __syncthreads();
+        if (i < P) {
+            int j = 0;
+            for (; j + 8 <= n; j += 8) {
+                float v[8];
+#pragma unroll
+                for (int u = 0; u < 8; ++u) v[u] = local[(size_t)c[j + u] * P + i];
+#pragma unroll
+                for (int u = 0; u < 8; ++u) s = __fadd_rn(s, v[u]);
+            }
+            for (; j < n; ++j) s = __fadd_rn(s, local[(size_t)c[j] * P + i]);
+        }
+    }
+    if (i < P) local[(size_t)p * P + i] = __fdiv_rn(s, (float)(k + 1));
+}
+
+}  // namespace uavrl
+
+using namespace uavrl;
+
+extern "C" {
+
+int uavrl_learner_federate(uavrl_learner *l, const float *probe_states_dev, const int32_t *probe_tape_dev, int32_t *probe_idx_out_dev,
+                           float *loss_out_dev, int32_t *chosen_out_dev, void *stream)
+{
+    if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
+    if (probe_states_dev && probe_tape_dev)
+        return fail(UAVRL_ERR_INVALID, "uavrl_learner_federate: give probe states or a probe tape, not both");
+    const int G = l->G;
+    if (G == 1) return 0;
+    const bool ring = probe_states_dev == nullptr;
+    if (ring && (l->mode != kReplayLockstep || l->count / G < kFedProbes))
+        return fail(UAVRL_ERR_INVALID, "uavrl_learner_federate: every trainer needs at least 10 transitions in the ring to draw probe states from");
+    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int k = (G - 1) / 2, kk = k > 0 ? k : 1, in = l->net.in_dim, A = l->net.n_actions, P = l->net.P;
+    const size_t rows = (size_t)G * kFedProbes;
+    // per-call scratch, stream-ordered
+    float *probes = nullptr, *q_ref = nullptr, *M = loss_out_dev;
+    int32_t *acts = nullptr, *chosen = chosen_out_dev;
+    bool ok = true;
+    auto alloc = [&](void **p, size_t bytes) { if (ok && cudaMallocAsync(p, bytes, st) != cudaSuccess) ok = false; };
+    if (ring) alloc((void **)&probes, rows * in * 4);
+    alloc((void **)&q_ref, rows * A * 4);
+    alloc((void **)&acts, rows * 4);
+    if (!M) alloc((void **)&M, (size_t)G * G * 4);
+    if (!chosen) alloc((void **)&chosen, (size_t)G * kk * 4);
+    int rc = 0;
+    auto done = [&](int code) {
+        if (probes) cudaFreeAsync(probes, st);
+        if (q_ref) cudaFreeAsync(q_ref, st);
+        if (acts) cudaFreeAsync(acts, st);
+        if (M && M != loss_out_dev) cudaFreeAsync(M, st);
+        if (chosen && chosen != chosen_out_dev) cudaFreeAsync(chosen, st);
+        return code;
+    };
+    if (!ok) { cudaGetLastError(); return done(fail(UAVRL_ERR_CUDA, "uavrl_learner_federate: out of device memory for the scratch")); }
+    // 1. probe rows
+    if (ring) {
+        BatchSrc src = replay_source(l, probe_tape_dev);
+        fed_probe_kernel<<<G, 256, 0, st>>>(src, in, l->cfg.seed ^ kFedSalt, l->fed_calls++, probes, probe_idx_out_dev);
+        UAVRL_LAUNCHED();
+    } else if (probe_idx_out_dev) {
+        if (cudaMemsetAsync(probe_idx_out_dev, 0xFF, rows * 4, st) != cudaSuccess)             // no replay indices: -1
+            return done(fail(UAVRL_ERR_CUDA, "uavrl_learner_federate: cudaMemsetAsync failed"));
+    }
+    const float *pr = ring ? probes : probe_states_dev;
+    // 2. own Q of every trainer on its probes: the grouped act pass (greedy; not an act call, so its Philox counter stays)
+    const uint64_t calls = l->act_calls;
+    if ((rc = launch_act(l, pr, (int)rows, 0.f, 0, nullptr, nullptr, acts, q_ref, st))) return done(rc);
+    l->act_calls = calls;
+    // 3. losses of the initial parameters: M[p][q], q > p; [p][p] = 0
+    if (cudaMemsetAsync(M, 0, (size_t)G * G * 4, st) != cudaSuccess || cudaMemsetAsync(chosen, 0xFF, (size_t)G * kk * 4, st) != cudaSuccess)
+        return done(fail(UAVRL_ERR_CUDA, "uavrl_learner_federate: cudaMemsetAsync failed"));
+    if ((rc = launch_fed_loss(l, pr, q_ref, M, 0, G, true, st))) return done(rc);
+    if (k == 0) {                                                    // G = 2: nothing is averaged, M[1][0] from the same parameters
+        if ((rc = launch_fed_loss(l, pr, q_ref, M, 0, G, false, st))) return done(rc);
+        return done(0);
+    }
+    const int tf = l->tc.train_img_bytes / 4, wf = l->net.smem_w_floats;
+    const int pb = (P + 255) / 256;
+    for (int p = 0; p < G; ++p) {
+        fed_rank_kernel<<<(G + 255) / 256, 256, 0, st>>>(G, p, k, kk, M, chosen);
+        UAVRL_LAUNCHED();
+        fed_average_kernel<<<pb, 256, 0, st>>>(P, p, k, chosen + (size_t)p * kk, l->local);
+        UAVRL_LAUNCHED();
+        // trainer p's kernel-layout images of q_local (the target images are not touched)
+        pack_image_kernel<<<pb, 256, 0, st>>>(P, l->local + (size_t)p * P, l->img_map, l->img_local + (size_t)p * wf, wf);
+        UAVRL_LAUNCHED();
+        if (l->tc_ok) {
+            pack_tc_kernel<<<pb, 256, 0, st>>>(P, l->local + (size_t)p * P, l->tc_hi_map, l->tc_lo_map, l->tc_hi2_map, l->tc_lo2_map,
+                                               (float *)l->tc_img_local + (size_t)p * tf, tf);
+            UAVRL_LAUNCHED();
+        }
+        // the new theta_p on the probes of every later round: column p of M
+        if (p + 1 < G && (rc = launch_fed_loss(l, pr, q_ref, M, p, 1, false, st))) return done(rc);
+    }
+    l->pdl_prev = kPdlNone;
+    return done(0);
+}
+
+}  // extern "C"

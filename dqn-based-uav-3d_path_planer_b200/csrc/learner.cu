@@ -76,14 +76,31 @@ static int build_net(const uavrl_learner_config &c, NetDev &n)
 }
 
 // ------------------------------------------------------------------ eps-greedy action kernel
+// LOSS (federation, launch_fed_loss): grid row y evaluates weight set w = fl.w0 + y on probe rows [0, S w) (fl.tri) or
+// [S (w + 1), n) of obs = [G][S][in_dim], S = kFedProbes; a tile takes 3 whole probe groups (30 rows) and writes
+// fl.loss_out[p][w] = sum over trainer p's rows of sum_a (fl.q_ref - Q_w)^2 / (S A).  The same reduction as the tensor-core
+// loss variant (tc_forward.cu).
+struct FedLossArgs { const float *q_ref; float *loss_out; int w0, tri; };
+
+template <bool LOSS>
 __global__ void __launch_bounds__(kNetThreads)
-act_kernel(NetDev net, const float *__restrict__ params, const float *__restrict__ obs, int n, float eps,
-           int is_train, const float *__restrict__ u_tape, const int32_t *__restrict__ rand_tape,
-           uint64_t key, uint64_t call, int32_t *__restrict__ actions, int32_t *__restrict__ actions2,
-           float *__restrict__ q_out, int n_tiles, int img_floats)
+act_kernel_t(NetDev net, const float *__restrict__ params, const float *__restrict__ obs, int n, float eps,
+             int is_train, const float *__restrict__ u_tape, const int32_t *__restrict__ rand_tape,
+             uint64_t key, uint64_t call, int32_t *__restrict__ actions, int32_t *__restrict__ actions2,
+             float *__restrict__ q_out, int n_tiles, int img_floats, FedLossArgs fl)
 {
     extern __shared__ __align__(16) float smem[];
-    {   // trainer blockIdx.y of a grouped learner: its weight image, its n rows and its eps-greedy key
+    constexpr int kStep = LOSS ? (kTile / kFedProbes) * kFedProbes : kTile;      // rows a tile advances by
+    int w_set = 0, n_rows = n;
+    size_t row0 = 0;
+    if (LOSS) {
+        w_set = fl.w0 + blockIdx.y;
+        const int lo = fl.tri ? 0 : kFedProbes * (w_set + 1), hi = fl.tri ? kFedProbes * w_set : n;
+        row0 = (size_t)lo; n_rows = hi - lo;
+        n_tiles = (n_rows + kStep - 1) / kStep;
+        if ((int)blockIdx.x >= n_tiles) return;
+        params += (size_t)w_set * img_floats; obs += row0 * net.in_dim;
+    } else {   // trainer blockIdx.y of a grouped learner: its weight image, its n rows and its eps-greedy key
         const int g = blockIdx.y;
         const size_t r0 = (size_t)g * (size_t)n;
         params += (size_t)g * img_floats; obs += r0 * net.in_dim; actions += r0;
@@ -104,15 +121,32 @@ act_kernel(NetDev net, const float *__restrict__ params, const float *__restrict
     if (threadIdx.x == 0) stage_weights(net, params, sw, &wbar);      // params = the network's smem image
     bool weights_ready = false;
     for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        const int e0 = t * kTile;
-        if (threadIdx.x < kTile) rows[threadIdx.x] = (e0 + threadIdx.x < n) ? obs + (size_t)(e0 + threadIdx.x) * net.in_dim : nullptr;
+        const int e0 = t * kStep;
+        if (threadIdx.x < kTile)
+            rows[threadIdx.x] = (threadIdx.x < kStep && e0 + threadIdx.x < n_rows) ? obs + (size_t)(e0 + threadIdx.x) * net.in_dim : nullptr;
         __syncthreads();
         if (net.in_dim % 4 == 0) load_rows(rows, smem + net.act_off[0], net.act_ld[0], net.in_dim);
         else load_rows_scalar(rows, smem + net.act_off[0], net.act_ld[0], net.in_dim);
         if (!weights_ready) { mbar_wait(&wbar, 0); weights_ready = true; }
         __syncthreads();
         net_forward(net, sw, smem + net.act_off[0], net.act_ld[0], smem, false, sA, sB, head);
-        if (threadIdx.x < kTile && e0 + threadIdx.x < n) {
+        if (LOSS) {
+            if (threadIdx.x < kTile) {
+                float d2 = 0.f;
+                if (threadIdx.x < kStep && e0 + threadIdx.x < n_rows) {
+                    const float *row = head + threadIdx.x * 32, *ref = fl.q_ref + (row0 + e0 + threadIdx.x) * net.n_actions;
+                    for (int k = 0; k < net.n_actions; ++k) { const float d = ref[k] - row[k]; d2 += d * d; }
+                }
+                sA[threadIdx.x] = d2;                     // sA: free scratch once the forward is done
+            }
+            __syncthreads();
+            if (threadIdx.x * kFedProbes < kStep && e0 + (int)threadIdx.x * kFedProbes < n_rows) {
+                float s2 = 0.f;
+                for (int r = 0; r < kFedProbes; ++r) s2 += sA[threadIdx.x * kFedProbes + r];
+                const size_t p = (row0 + e0 + threadIdx.x * kFedProbes) / kFedProbes;
+                fl.loss_out[p * (size_t)(n / kFedProbes) + w_set] = s2 / (float)(kFedProbes * net.n_actions);
+            }
+        } else if (threadIdx.x < kTile && e0 + threadIdx.x < n) {
             const int e = e0 + threadIdx.x;
             const float *row = head + threadIdx.x * 32;
             float u; int ra;
@@ -632,9 +666,34 @@ int launch_act(uavrl_learner *l, const float *obs, int n_all, float eps, int is_
     }
     const int n_tiles = (n + kTile - 1) / kTile;
     const int grid = n_tiles < 4 * num_sms() ? n_tiles : 4 * num_sms();
-    act_kernel<<<dim3(grid, l->G), kNetThreads, act_smem_bytes(l->net), st>>>(l->net, l->img_local, obs, n, eps, is_train, u_tape,
-                                                                             rand_tape, l->cfg.seed ^ kActSalt, l->act_calls++,
-                                                                             actions, nullptr, q_out, n_tiles, l->net.smem_w_floats);
+    act_kernel_t<false><<<dim3(grid, l->G), kNetThreads, act_smem_bytes(l->net), st>>>(l->net, l->img_local, obs, n, eps, is_train, u_tape,
+                                                                                      rand_tape, l->cfg.seed ^ kActSalt, l->act_calls++,
+                                                                                      actions, nullptr, q_out, n_tiles, l->net.smem_w_floats,
+                                                                                      FedLossArgs{});
+    l->pdl_prev = kPdlNone;
+    UAVRL_LAUNCHED();
+    return 0;
+}
+
+int launch_fed_loss(uavrl_learner *l, const float *probes, const float *q_ref, float *loss_out, int w0, int n_weights, bool tri,
+                    cudaStream_t st)
+{
+    const int n = l->G * kFedProbes;                     // every probe row; a weight set evaluates at most n - S of them
+    const int max_rows = n - kFedProbes;
+    if (max_rows <= 0 || n_weights <= 0) return 0;
+    if (l->tc_ok && l->use_tc) {
+        TcArgs a;
+        memset(&a, 0, sizeof(a));
+        a.img = l->tc_img_local; a.obs = probes; a.n = n; a.mode = kTcAct;
+        a.q_ref = q_ref; a.loss_out = loss_out; a.loss_w0 = w0; a.loss_tri = tri ? 1 : 0;
+        return launch_tc_loss(l, a, n_weights, max_rows, st);
+    }
+    constexpr int step = (kTile / kFedProbes) * kFedProbes;
+    const int n_tiles = (max_rows + step - 1) / step;
+    const int grid = n_tiles < 4 * num_sms() ? n_tiles : 4 * num_sms();
+    act_kernel_t<true><<<dim3(grid, n_weights), kNetThreads, act_smem_bytes(l->net), st>>>(l->net, l->img_local, probes, n, 0.f, 0, nullptr,
+                                                                                          nullptr, 0, 0, nullptr, nullptr, nullptr, n_tiles,
+                                                                                          l->net.smem_w_floats, FedLossArgs{ q_ref, loss_out, w0, tri ? 1 : 0 });
     l->pdl_prev = kPdlNone;
     UAVRL_LAUNCHED();
     return 0;
@@ -993,7 +1052,7 @@ int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_tra
     if ((rc = dev_alloc(&l->r_act, (size_t)l->slots)) || (rc = dev_alloc(&l->r_rew, (size_t)l->slots)) ||
         (rc = dev_alloc(&l->r_done, (size_t)l->slots)))
         return rc;
-    if ((rc = raise_dyn_smem(act_kernel, act_smem_bytes(l->net))) || (rc = raise_dyn_smem(update_kernel, upd_smem_bytes(l->net, l->dual_weights))))
+    if ((rc = raise_dyn_smem(act_kernel_t<false>, act_smem_bytes(l->net))) || (rc = raise_dyn_smem(act_kernel_t<true>, act_smem_bytes(l->net))) || (rc = raise_dyn_smem(update_kernel, upd_smem_bytes(l->net, l->dual_weights))))
         return rc;
     *out = l;
     return 0;

@@ -9,6 +9,7 @@ constexpr int kTile = 32;             // samples per CTA tile
 constexpr int kNetThreads = 256;      // 8 warps: lane -> output unit, warp -> 4 samples
 constexpr int kMaxDim = 128;          // every layer width (and in_dim) <= 128
 constexpr int kMaxLayers = UAVRL_MAX_HIDDEN + 1;   // trunk layers + (combined) head
+constexpr int kFedProbes = 10;        // probe states per trainer of a federation round (PathPlan_City.py:658)
 
 // One dense layer as the kernels see it.  Weights live in smem transposed: Wt[k][o], ld = out+1
 // (odd when out is even -> conflict-free whether lanes walk o or k).
@@ -56,7 +57,8 @@ struct BatchSrc {
 
 // Philox key salts of a learner seeded with `seed`: the eps-greedy draws use seed ^ kActSalt, replay sampling seed ^ kSampleSalt.
 // Trainer g of a grouped learner draws exactly what a stand-alone learner seeded with seed + g draws.
-constexpr uint64_t kActSalt = 0xAC7ull, kSampleSalt = 0x5EEDull;
+// Federation probe draws (federate.cu) use seed ^ kFedSalt.
+constexpr uint64_t kActSalt = 0xAC7ull, kSampleSalt = 0x5EEDull, kFedSalt = 0xFEDull;
 __host__ __device__ __forceinline__ uint64_t trainer_key(uint64_t key, uint64_t salt, int g) { return ((key ^ salt) + (uint64_t)g) ^ salt; }
 
 // ---- tensor-core (wgmma) forward path: one dense layer as a B operand [N_pad][K_pad], K-major canonical
@@ -142,6 +144,7 @@ struct uavrl_learner {
     uavrl::PerDev per = {};
     uint64_t per_calls = 0;
     uint64_t act_calls = 0;
+    uint64_t fed_calls = 0;           // ring-sampled federation calls: the Philox counter of their probe draws (federate.cu)
     // data-parallel: one-shot NVLink all-reduce fused with Adam (symmetric buffers exchanged through CUDA IPC)
     int32_t rank = 0, world = 1;
     float *comm_grad = nullptr;       // own receive buffer recv[2][world][P+1]: slot q is written by rank q (remote stores)
@@ -379,6 +382,10 @@ int launch_act_env(uavrl_learner *l, const EnvDev &d, const float *obs, float ep
                    uint8_t *done, cudaStream_t st);
 int launch_act(uavrl_learner *l, const float *obs, int n, float eps, int is_train, const float *u_tape,
                const int32_t *rand_tape, int32_t *actions, float *q_out, cudaStream_t st);
+// the loss variant of the act pass (federation): weight sets w0 .. w0 + n_weights - 1 on the probe rows [G][kFedProbes][in_dim]
+// (tc_forward.cuh TcArgs::loss_* for the row ranges), losses into loss_out[G][G]
+int launch_fed_loss(uavrl_learner *l, const float *probes, const float *q_ref, float *loss_out, int w0, int n_weights, bool tri,
+                    cudaStream_t st);
 int launch_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out,
                   bool apply, cudaStream_t st);
 int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, cudaStream_t st);

@@ -119,8 +119,11 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
 // dependency is per env, so no grid-wide boundary is needed between Trainer.get_action and BaseEnv.Move_Agent.
 // ACT (a.mode == kTcAct) and DUELING are compile-time: the kernel a pass runs carries no code of the other modes.
 // FIXED: every layer product is one unbroken compile-time wgmma chain (wgmma.cuh mma_fixed; tc_fixed_chains).
-template <bool FUSE_ENV, bool ACT, bool DUELING, bool FIXED>
-__global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, TcArgs a, EnvFuse ef)
+// LOSS (with ACT, federation): grid row y evaluates weight set loss_w0 + y on a probe-row range (TcArgs::loss_*); a tile
+// takes whole groups of kFedProbes rows, and its head epilogue reduces each group to one loss entry.
+// The kernels below are thin entry points over this body: tc_forward_kernel_t (LOSS = false) and tc_loss_kernel_t.
+template <bool FUSE_ENV, bool ACT, bool DUELING, bool FIXED, bool LOSS>
+__device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a, const EnvFuse &ef)
 {
     TC_TRACE(0);
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -133,8 +136,20 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = warp & 3, half = warp >> 2;
     // trainer blockIdx.y of a grouped learner: its weight image, rows [r0, r0 + n) of the inputs / outputs, its keys
     const int grp = blockIdx.y;
-    const size_t r0 = (size_t)grp * (size_t)a.n;
+    size_t r0 = (size_t)grp * (size_t)a.n;
     const unsigned char *img = a.img + (size_t)grp * (size_t)a.img_stride;
+    // rows this grid row evaluates, tiles over them and the rows a tile advances by (LOSS: whole probe groups only)
+    int n_rows = a.n, n_tiles = a.n_tiles, tile_step = a.rows_per_tile;
+    int w_set = 0;
+    if (LOSS) {
+        w_set = a.loss_w0 + grp;
+        const int lo = a.loss_tri ? 0 : kFedProbes * (w_set + 1), hi = a.loss_tri ? kFedProbes * w_set : a.n;
+        r0 = (size_t)lo; n_rows = hi - lo;
+        tile_step = (a.rows_per_tile / kFedProbes) * kFedProbes;
+        n_tiles = (n_rows + tile_step - 1) / tile_step;
+        img = a.img + (size_t)w_set * (size_t)a.img_stride;
+        if ((int)blockIdx.x >= n_tiles) return;                  // nothing staged or waited for yet
+    }
     // The first thread of the last warp initialises the two mbarriers and issues the weight copies while the other warps
     // already gather the first tile; the CTA-wide barrier in front of the first weight wait publishes the barriers.
     constexpr int kCtl = kTcThreads - 32;
@@ -175,8 +190,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
     // samples; accumulator rows >= R are computed from whatever SMEM follows the R-row operand (still inside this CTA's allocation) and never stored.
     // Small batches use R = 32 so that 4096 samples spread over 128 CTAs instead of 32.
     const int R = a.rows_per_tile, lgR = 31 - __clz(R);
-    for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
-        const int base = tile * R;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int base = tile * tile_step;
         if (!direct) {
             if (tid < R) {
                 const int b = base + tid;
@@ -205,7 +220,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
                     v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
                     if (i < total) {
                         const int r = i & (R - 1), j = i >> lgR;
-                        const float *rp = direct ? ((base + r < a.n) ? a.obs + (r0 + base + r) * tc.in_dim : nullptr) : rows[r];
+                        const float *rp = direct ? ((base + r < n_rows && r < tile_step) ? a.obs + (r0 + base + r) * tc.in_dim : nullptr) : rows[r];
                         if (rp && 4 * j < tc.in_dim) v[u] = __ldg(reinterpret_cast<const float4 *>(rp) + j);
                     }
                 }
@@ -290,7 +305,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
                     for (int j = 1; j < 32; ++j) if (j < nA && q[j] > bv) { bv = q[j]; best = j; }
                     const int b = base + row;                               // trainer-local row
                     const size_t ob = r0 + b;                               // its row in the [G][n] inputs / outputs
-                    if (b < a.n) {
+                    if (LOSS) {
+                        float d2 = 0.f;
+                        if (b < n_rows && row < tile_step) {
+#pragma unroll
+                            for (int j = 0; j < 32; ++j)
+                                if (j < nA) { const float d = a.q_ref[ob * nA + j] - q[j]; d2 += d * d; }
+                        }
+                        s_rew[row] = d2;
+                    } else if (b < a.n) {
                         if (a.q_out) {
 #pragma unroll
                             for (int j = 0; j < 32; ++j) if (j < nA) a.q_out[ob * nA + j] = q[j];
@@ -320,6 +343,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
                     }
                 }
                 __syncthreads();
+                if (LOSS && tid * kFedProbes < tile_step && base + tid * kFedProbes < n_rows) {
+                    // one probe group (trainer p's rows) per thread: its rows' squared differences in row order
+                    float s2 = 0.f;
+                    for (int r = 0; r < kFedProbes; ++r) s2 += s_rew[tid * kFedProbes + r];
+                    const size_t p = (r0 + base + tid * kFedProbes) / kFedProbes;
+                    a.loss_out[p * (size_t)(a.n / kFedProbes) + w_set] = s2 / (float)(kFedProbes * tc.n_actions);
+                }
             }
         }
         if (FUSE_ENV) {
@@ -332,6 +362,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, T
         }
     }
     TC_TRACE(20);
+}
+
+template <bool FUSE_ENV, bool ACT, bool DUELING, bool FIXED>
+__global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, TcArgs a, EnvFuse ef)
+{
+    tc_forward_body<FUSE_ENV, ACT, DUELING, FIXED, false>(tc, a, ef);
+}
+
+template <bool DUELING, bool FIXED>
+__global__ void __launch_bounds__(kTcThreads, 1) tc_loss_kernel_t(TcNet tc, TcArgs a, EnvFuse ef)
+{
+    tc_forward_body<false, true, DUELING, FIXED, true>(tc, a, ef);
 }
 
 bool tc_fixed_chains(const TcNet &tc, bool train)
@@ -355,6 +397,10 @@ static ForwardKernel pick_forward_kernel(bool fuse_env, bool act, bool dueling, 
     if (fuse_env) return pick_fwd_d<true, true>(dueling, fixed);
     return act ? pick_fwd_d<false, true>(dueling, fixed) : pick_fwd_d<false, false>(dueling, fixed);
 }
+
+template <bool D>
+static ForwardKernel pick_loss_d(bool fixed) { return fixed ? tc_loss_kernel_t<D, true> : tc_loss_kernel_t<D, false>; }
+static ForwardKernel pick_loss_kernel(bool dueling, bool fixed) { return dueling ? pick_loss_d<true>(fixed) : pick_loss_d<false>(fixed); }
 
 int tc_forward_rows_per_tile(const TcNet &tc, int n)
 {
@@ -408,6 +454,24 @@ int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st, con
     return 0;
 }
 
+int launch_tc_loss(uavrl_learner *l, const TcArgs &a_in, int n_weights, int max_rows, cudaStream_t st)
+{
+    TcArgs a = a_in;
+    a.img_stride = l->tc.train_img_bytes;
+    a.rows_per_tile = tc_forward_rows_per_tile(l->tc, max_rows);
+    const int step = (a.rows_per_tile / kFedProbes) * kFedProbes;
+    const int tiles = (max_rows + step - 1) / step, n_sm = num_sms();
+    a.n_tiles = tiles;
+    a.pdl = 0;
+    EnvFuse ef;
+    memset(&ef, 0, sizeof(ef));
+    UAVRL_CUDA(launch_kernel(pick_loss_kernel(l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(tiles < n_sm ? tiles : n_sm, n_weights),
+                             dim3(kTcThreads), tc_smem_bytes(l->tc), st, false, l->tc, a, ef));
+    l->pdl_prev = kPdlNone;
+    UAVRL_LAUNCHED();
+    return 0;
+}
+
 int tc_init(uavrl_learner *l)
 {
     std::vector<int32_t> hi, lo, hi2, lo2;
@@ -440,6 +504,8 @@ int tc_init(uavrl_learner *l)
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du)
             if (int rc = raise_dyn_smem(pick_forward_kernel(false, ac != 0, du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
+    for (int du = 0; du < 2; ++du)                               // the loss variant: the act kernel's static shared memory
+        if (int rc = raise_dyn_smem(pick_loss_kernel(du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
     {   // the fused act+step variant carries the env scratch as static shared memory on top: it must still fit one CTA
         l->fuse_ok = true;
         for (int du = 0; du < 2; ++du) {

@@ -28,6 +28,10 @@ struct TcArgs {
     float gamma;
     int32_t pdl;                       // kPdlOn | kPdlEarlyWeights | kPdlEarlyRows (set by launch_tc_forward)
     long long *trace;                  // debug: CTA (0, 0) / thread 0 writes clock64() at stage boundaries (UAVRL_TC_TRACE=1)
+    // loss variant of the act kernel (launch_tc_loss, federation): grid row y evaluates weight set w = loss_w0 + y on the
+    // probe rows [0, S w) (loss_tri) or [S (w + 1), n) of obs = [G][S][in_dim], S = kFedProbes, and writes
+    // loss_out[p][w] = sum over trainer p's S rows of sum_a (q_ref - Q_w)^2 / (S A), q_ref = [G][S][A]
+    const float *q_ref; float *loss_out; int32_t loss_w0, loss_tri;
 };
 
 int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::vector<int32_t> &hi_map, std::vector<int32_t> &lo_map,
@@ -50,6 +54,8 @@ bool tc_fixed_chains(const TcNet &tc, bool train);
 // the env step fused behind the act pass (tc_forward.cu): env batch + where the step writes
 struct EnvFuse { EnvDev d; float *obs_next; float *reward; uint8_t *done; };
 int launch_tc_forward(uavrl_learner *l, const TcArgs &a, cudaStream_t st, const EnvFuse *fuse = nullptr);
+// the loss variant over n_weights weight sets (grid rows), max_rows = the most probe rows one of them evaluates
+int launch_tc_loss(uavrl_learner *l, const TcArgs &a, int n_weights, int max_rows, cudaStream_t st);
 int tc_init(uavrl_learner *l);        // builds the TC images/maps; leaves l->tc_ok = false when the net does not fit
 
 }  // namespace uavrl

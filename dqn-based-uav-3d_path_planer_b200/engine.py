@@ -352,6 +352,35 @@ class Learner:
     def update(self, idx_tape=None, loss=None):
         check(_lib.lib().uavrl_learner_update(self.h, _ptr(idx_tape), self._loss(loss), _stream(self.device)))
 
+    def federate(self, probe_states=None, probe_tape=None, want_details=False):
+        """Selective federated aggregation across the trainers (PathPlan_City.Federated_Learning_choice, include/uavrl.h
+        uavrl_learner_federate).  probe_states: (G, 10, in_dim) device tensor, or None to draw the probes from the lockstep
+        ring; probe_tape: (G, 10) trainer-local replay indices for the ring draw, a host array (checked, then uploaded) or a
+        device int32 tensor.  want_details: returns device tensors (probe_idx (G, 10), losses (G, G), chosen (G, max(1, k)))."""
+        G = self.G
+        if probe_tape is not None and not isinstance(probe_tape, torch.Tensor):
+            tape = np.ascontiguousarray(probe_tape, np.int64)
+            if tape.shape != (G, 10):
+                raise ValueError("probe_tape must be (%d, 10), got %s" % (G, tape.shape))
+            if any(len(set(row.tolist())) != 10 for row in tape):
+                raise ValueError("probe_tape rows must hold 10 distinct indices")
+            n_g = self.replay_size() // G
+            if (tape < 0).any() or (tape >= n_g).any():
+                raise ValueError("probe_tape indices must lie in [0, %d) (transitions per trainer)" % n_g)
+            probe_tape = torch.from_numpy(tape.astype(np.int32)).to(self.device)
+        if probe_states is not None and tuple(probe_states.shape) != (G, 10, self.in_dim):
+            raise ValueError("probe_states must be (%d, 10, %d)" % (G, self.in_dim))
+        k = (G - 1) // 2
+        idx = losses = chosen = None
+        if want_details:
+            idx = torch.empty((G, 10), dtype=torch.int32, device=self.device)
+            losses = torch.empty((G, G), dtype=torch.float32, device=self.device)
+            chosen = torch.empty((G, max(1, k)), dtype=torch.int32, device=self.device)
+        check(_lib.lib().uavrl_learner_federate(self.h, _ptr(probe_states), _ptr(probe_tape), _ptr(idx), _ptr(losses), _ptr(chosen),
+                                                _stream(self.device)))
+        if want_details:
+            return idx, losses, chosen
+
     def update_batch(self, s, a, r, s2, d, loss=None):
         check(_lib.lib().uavrl_learner_update_batch(self.h, s.shape[0], _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d),
                                                     self._loss(loss), _stream(self.device)))

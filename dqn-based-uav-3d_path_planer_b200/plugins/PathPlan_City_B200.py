@@ -173,7 +173,16 @@ class PathPlan_City_B200:
         self.result = {}
         self.epoch = 0
         self.print_loop = int(None2Value(param.get('print_loop'), 2))
-        self.Is_FL = 0
+        # federated aggregation every FL_Loop episodes (PathPlan_City.py:78-79, :469-475).  With DQN-family trainers it runs the
+        # reference's selective aggregation Federated_Learning_choice (:644-684) across the num_trainers trainers
+        self.Is_FL = int(None2Value(param.get('Is_FL'), 0))
+        self.FL_Loop = int(None2Value(param.get('FL_Loop'), 3))
+        if self.Is_FL:
+            if self.FL_Loop < 1:
+                raise ValueError("FL_Loop must be >= 1 when Is_FL = 1")
+            if self.Is_AC and not isinstance(self.Trainer._learner, engine.SacLearner):
+                raise ValueError("Is_FL = 1 with Is_AC = 1 averages the trainers' actors (Federated_Learning_AC), which DQN-family "
+                                 "trainers do not have: set Is_AC = 0")
         self.executed_time = 0
         self.Scene_Random_Reset()
 
@@ -293,11 +302,23 @@ class PathPlan_City_B200:
                            step=iters, env_steps=steps, updates=updates, collisions=coll, episodes=ended)
         self.epoch += 1
         self.executed_time += dt
+        if self.Is_FL and self.epoch % self.FL_Loop == 0:             # PathPlan_City.py:469-475
+            self.Federated_Learning_choice()
         if self.record_csv:
             self._write_path_csv()
             if self.print_loop > 0 and self.epoch % self.print_loop == 0:
                 ag.record_list()                                   # PathPlan_City.run_eposide :463-468 (every print_loop episodes)
         return self.result
+
+    def Federated_Learning_choice(self):
+        """PathPlan_City.py:644-684 on the device (engine.Learner.federate): every trainer averages itself with the half of
+        the other trainers whose Q-values lie closest to its own on 10 states of its replay.  The reference's run_eposide calls
+        Federated_Learning (:475), which cannot run (sample2 unpacking, trainer methods the reference lacks); this plug-in runs
+        the reference's selective aggregation instead.  One trainer (or the SAC trainer) has nothing to aggregate with."""
+        learner = self.Trainer._learner
+        if isinstance(learner, engine.SacLearner) or learner.trainer_count() < 2:
+            return
+        learner.federate()
 
     def _write_path_csv(self, path="path.csv"):
         """UAV.py:461-464 / :479-482 / :505-508: at a terminal step the reference rewrites path.csv (CWD-relative) with the

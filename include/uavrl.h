@@ -210,6 +210,32 @@ int64_t uavrl_learner_param_count(const uavrl_learner *l);
 int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_trainers, uavrl_learner **out);
 int32_t uavrl_learner_trainer_count(const uavrl_learner *l);
 
+/* Selective federated aggregation across the G trainers (Envs/PathPlan_City.py:644-684, Federated_Learning_choice; Is_FL with
+ * a DQN-family trainer).  Rounds p = 0, 1, ..., G-1, in this order and in place:
+ *   - probes: 10 distinct transitions of trainer p's own replay (random.sample(memory, 10)), their state rows;
+ *   - q_value = Q(theta_p, probes) with theta_p as it stands (it changes only in round p);
+ *   - loss_q = mean((q_value - Q(theta_q, probes))^2) over 10 x A for every q != p, theta_q trainer q's CURRENT q_local:
+ *     for q < p the parameters round q already replaced;
+ *   - the trainers sorted by (loss, index) -- Python's stable sort keeps equal losses in ascending q -- and the first
+ *     k = (G - 1) / 2 kept;
+ *   - theta_p <- (theta_p + theta_c0 + theta_c1 + ...) / (k + 1), per element a float32 left-to-right sum in the sorted
+ *     order and one float32 division (bit-reproducible).
+ * Only q_local and its kernel-layout images change (replace_param, :683; the reference's averaged q_target is discarded):
+ * q_target, the Adam moments, epoch and adam_step are untouched.  G = 1 returns 0 and does nothing; G = 2 has k = 0 and
+ * leaves every parameter as it is.
+ *   probe_states_dev   [G][10][in_dim] explicit probe states (block p for round p), or NULL: draw them from the lockstep ring;
+ *   probe_tape_dev     ring mode only, or NULL: [G][10] trainer-local logical indices (the convention of
+ *                      uavrl_learner_update's tape: in range [0, replay size / G) and distinct within a row -- not checked on
+ *                      the device).  NULL: Philox draws keyed by seed + g and a per-learner federation call counter;
+ *   probe_idx_out_dev  optional [G][10]: the trainer-local indices used (-1 with explicit probe states);
+ *   loss_out_dev       optional [G][G]: row p = the losses round p ranked, [p][p] = 0;
+ *   chosen_out_dev     optional [G][max(1, k)]: round p's chosen trainers in sorted order (-1 when k = 0).
+ * Everything is enqueued on `stream` (about 5 G kernel launches; the cost grows as G^2), with no host synchronisation.
+ * Refused with UAVRL_ERR_INVALID before anything is enqueued: both probe sources given; ring mode on a learner without a
+ * lockstep ring or with fewer than 10 transitions per trainer. */
+int uavrl_learner_federate(uavrl_learner *l, const float *probe_states_dev, const int32_t *probe_tape_dev,
+                           int32_t *probe_idx_out_dev, float *loss_out_dev, int32_t *chosen_out_dev, void *stream);
+
 /* state_dict()-ordered flat fp32 parameters (fc1.weight [out][in], fc1.bias, ..., for dueling nets
  * ..., fc_A.weight, fc_A.bias, fc_V.weight, fc_V.bias) -- what torch.save({'model': ...}) holds
  * (DuelingDQN_Trainer.py:79-84).  which: 0 = q_local, 1 = q_target, 2 = Adam exp_avg,
