@@ -129,6 +129,11 @@ SIGNATURES = {
     "uavrl_learner_update_dp": (C.c_int, [VP, VP, C.c_int32, VP, VP]),
     "uavrl_train_run": (C.c_int, [VP, VP, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.POINTER(TrainStats), VP]),
     "uavrl_sac_create": (C.c_int, [C.POINTER(SacConfig), C.POINTER(VP)]),
+    "uavrl_sac_create_trainers": (C.c_int, [C.POINTER(SacConfig), C.c_int32, C.POINTER(VP)]),
+    "uavrl_sac_trainer_count": (C.c_int32, [VP]),
+    "uavrl_sac_set_alpha": (C.c_int, [VP, VP]),
+    "uavrl_sac_get_alpha": (C.c_int, [VP, VP]),
+    "uavrl_sac_federate_actors": (C.c_int, [VP, VP]),
     "uavrl_sac_destroy": (C.c_int, [VP]),
     "uavrl_sac_param_count": (C.c_int64, [VP, C.c_int32]),
     "uavrl_sac_set_params": (C.c_int, [VP, C.c_int32, VP]),

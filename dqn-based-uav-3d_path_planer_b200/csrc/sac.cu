@@ -14,6 +14,10 @@
 //   sac_actor_kernel    actor forward on s (fresh noise), the UPDATED critics on [s, a_new], loss, backward through the
 //                       critics to the action inputs, through tanh / softplus / the reparameterisation to the actor
 // then reduce_adam_kernel per network and sac_finish_kernel (alpha step, soft target update).
+// A grouped learner (uavrl_sac_create_trainers) holds G independent SAC trainers of one shape: every kernel takes the trainer
+// from blockIdx.y (gridDim.y = G) and offsets its weight images, rows, noise key, log_alpha and scratch by it (sac_g and the
+// helpers after it).
+// sac_federate_kernel is Federated_Learning_AC (Envs/PathPlan_City.py:590-601) across those trainers' actors.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -32,29 +36,45 @@ __host__ __device__ inline int sac_gld(int hidden) { const int w = round_up(hidd
 
 struct SacHyper { float actor_lr, critic_lr, alpha_lr, target_entropy, gamma, tau, bound; };
 
+// Every per-trainer array below is [G][...] (G = gridDim.y); the comments give one trainer's block.
 struct SacArgs {
     NetDev actor, critic;
     BatchSrc src;
-    int32_t B, n_tiles;
+    int32_t B, n_tiles;                  // per trainer
     int32_t gld;                         // row stride of the gradient planes (sac_gld)
-    const float *img_actor, *img_c1, *img_c2, *img_t1, *img_t2;
+    const float *img_actor, *img_c1, *img_c2, *img_t1, *img_t2;   // [G][smem_w_floats] weight images
     const float *eps;                    // [B][A] injected noise (nullptr -> Philox Box-Muller)
-    uint64_t key, ctr;
-    const float *log_alpha;              // device scalar
+    uint64_t key, ctr;                   // noise key of trainer 0 (trainer g: trainer_key(key, kNoiseSalt, g)), counter (shared)
+    const float *log_alpha;              // [3]: log_alpha, its Adam exp_avg, exp_avg_sq
     float *td;                           // [B][A]
     float *part_a, *part_c1, *part_c2;   // gradient partials [grid][P]
     float *stat;                         // [grid][4]: critic-1 sq-err sum, critic-2 sq-err sum, actor-loss sum, entropy sum
     SacHyper h;
 };
 
+constexpr uint64_t kNoiseSalt = 0x5AC5ull;   // reparameterisation noise of a learner seeded `seed`: key seed ^ kNoiseSalt
+
+// The tile kernels are templated on GR (grouped): a one-trainer learner launches GR = false, where the trainer index is the
+// constant 0 and every offset below folds away, so it runs the code of a learner that knows nothing of trainers.
+// Trainer g's share of the launch, evaluated where it is used (kept out of registers across the tile loop): its rows, weight
+// images, noise key and stream, log_alpha, TD targets and partial slots.
+template <bool GR> __device__ __forceinline__ int sac_g() { return GR ? (int)blockIdx.y : 0; }
+template <bool GR> __device__ __forceinline__ BatchSrc sac_src(const SacArgs &a) { return trainer_src(a.src, sac_g<GR>(), a.B, a.actor.in_dim); }
+template <bool GR> __device__ __forceinline__ uint64_t sac_sample_key(const SacArgs &a) { return trainer_key(a.src.key, kSampleSalt, sac_g<GR>()); }
+template <bool GR> __device__ __forceinline__ const float *sac_img(const float *img, const NetDev &n) { return img + (size_t)sac_g<GR>() * n.smem_w_floats; }
+template <bool GR> __device__ __forceinline__ const float *sac_eps(const SacArgs &a) { return a.eps ? a.eps + (size_t)sac_g<GR>() * a.B * kSacA : nullptr; }
+template <bool GR> __device__ __forceinline__ uint64_t sac_noise_key(const SacArgs &a) { return trainer_key(a.key, kNoiseSalt, sac_g<GR>()); }   // (seed + g) ^ salt
+template <bool GR> __device__ __forceinline__ float *sac_td(const SacArgs &a) { return a.td + (size_t)sac_g<GR>() * a.B * kSacA; }
+template <bool GR> __device__ __forceinline__ size_t sac_part() { return (size_t)sac_g<GR>() * gridDim.x + blockIdx.x; }
+
 __device__ __forceinline__ float softplus_f(float x) { return x > 20.f ? x : log1pf(expf(x)); }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
 
-__device__ __forceinline__ void noise2(const SacArgs &a, int gb, float &e0, float &e1)
+__device__ __forceinline__ void noise2(const float *eps, uint64_t key, uint64_t ctr, int gb, float &e0, float &e1)
 {
-    if (a.eps) { e0 = a.eps[2 * gb]; e1 = a.eps[2 * gb + 1]; return; }
+    if (eps) { e0 = eps[2 * gb]; e1 = eps[2 * gb + 1]; return; }
     uint32_t r[4];
-    Philox::gen(a.key, a.ctr, (uint64_t)gb, r);
+    Philox::gen(key, ctr, (uint64_t)gb, r);
     const float u0 = ((float)(r[0] >> 8) + 0.5f) * (1.0f / 16777216.0f), u1 = Philox::u01(r[1]);
     const float rad = sqrtf(-2.f * logf(u0));
     e0 = rad * cospif(2.f * u1); e1 = rad * sinpif(2.f * u1);
@@ -136,6 +156,7 @@ __device__ void critic_backward_tile(const NetDev &cn, const float *sw, const fl
 }
 
 // ------------------------------------------------------------------ TD target (calc_target, :122-131)
+template <bool GR>
 __global__ void __launch_bounds__(kNetThreads) sac_target_kernel(SacArgs a)
 {
     extern __shared__ __align__(16) float smem[];
@@ -147,16 +168,19 @@ __global__ void __launch_bounds__(kNetThreads) sac_target_kernel(SacArgs a)
     __shared__ float s_r[kTile], s_d[kTile], s_logp[kTile][kSacA], s_act[kTile][kSacA];
     if (threadIdx.x == 0) { for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1); fence_barrier_init(); }
     __syncthreads();
-    if (threadIdx.x == 0) { stage_weights(an, a.img_actor, RA, &bar[0]); stage_weights(cn, a.img_t1, RT1, &bar[1]); stage_weights(cn, a.img_t2, WT2, &bar[2]); }
+    if (threadIdx.x == 0) {
+        stage_weights(an, sac_img<GR>(a.img_actor, an), RA, &bar[0]); stage_weights(cn, sac_img<GR>(a.img_t1, cn), RT1, &bar[1]);
+        stage_weights(cn, sac_img<GR>(a.img_t2, cn), WT2, &bar[2]);
+    }
     uint32_t pkey[4];
-    Philox::gen(a.src.key, a.src.epoch, 0x5A17ull, pkey);
-    const float alpha = expf(*a.log_alpha);
+    Philox::gen(sac_sample_key<GR>(a), a.src.epoch, 0x5A17ull, pkey);
+    const float alpha = expf(a.log_alpha[3 * sac_g<GR>()]);
     bool ready = false;
     for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x) {
         if (threadIdx.x < kTile) {
             const int gb = t * kTile + threadIdx.x;
             Transition tr; tr.s2 = nullptr; tr.r = 0.f; tr.d = 0.f;
-            if (gb < a.B) tr = resolve_transition(a.src, gb, an.in_dim, pkey);
+            if (gb < a.B) tr = resolve_transition(sac_src<GR>(a), gb, an.in_dim, pkey);
             rows[threadIdx.x] = (gb < a.B) ? tr.s2 : nullptr; s_r[threadIdx.x] = tr.r; s_d[threadIdx.x] = tr.d;
         }
         __syncthreads();
@@ -167,7 +191,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_target_kernel(SacArgs a)
         if (threadIdx.x < kTile) {
             const int b = threadIdx.x, gb = t * kTile + b;
             float e[2] = { 0.f, 0.f };
-            if (gb < a.B) noise2(a, gb, e[0], e[1]);
+            if (gb < a.B) noise2(sac_eps<GR>(a), sac_noise_key<GR>(a), a.ctr, gb, e[0], e[1]);
             for (int j = 0; j < kSacA; ++j) {
                 const ActorOut o = actor_point(head[b * 32 + j], head[b * 32 + kSacA + j], e[j]);
                 s_act[b][j] = o.a * a.h.bound; s_logp[b][j] = o.logp;
@@ -183,7 +207,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_target_kernel(SacArgs a)
             if (gb < a.B)
                 for (int j = 0; j < kSacA; ++j) {
                     const float nv = fminf(q1[b * 32 + j], q2[b * 32 + j]) + alpha * (-s_logp[b][j]);
-                    a.td[(size_t)gb * kSacA + j] = s_r[b] + a.h.gamma * nv * (1.f - s_d[b]);
+                    sac_td<GR>(a)[(size_t)gb * kSacA + j] = s_r[b] + a.h.gamma * nv * (1.f - s_d[b]);
                 }
         }
         __syncthreads();
@@ -191,6 +215,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_target_kernel(SacArgs a)
 }
 
 // ------------------------------------------------------------------ critic update (:343-360)
+template <bool GR>
 __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
 {
     extern __shared__ __align__(16) float smem[];
@@ -203,9 +228,9 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
     __shared__ float s_act[kTile][kSacA], s_sq[kTile];
     if (threadIdx.x == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); fence_barrier_init(); }
     __syncthreads();
-    if (threadIdx.x == 0) { stage_weights(cn, a.img_c1, RC, &bar[0]); stage_weights(cn, a.img_c2, WC2, &bar[1]); }
+    if (threadIdx.x == 0) { stage_weights(cn, sac_img<GR>(a.img_c1, cn), RC, &bar[0]); stage_weights(cn, sac_img<GR>(a.img_c2, cn), WC2, &bar[1]); }
     uint32_t pkey[4];
-    Philox::gen(a.src.key, a.src.epoch, 0x5A17ull, pkey);
+    Philox::gen(sac_sample_key<GR>(a), a.src.epoch, 0x5A17ull, pkey);
     const float inv = 1.f / ((float)a.B * (float)kSacA);
     float sq[2] = { 0.f, 0.f };
     bool ready = false;
@@ -214,7 +239,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
         if (threadIdx.x < kTile) {
             const int gb = t * kTile + threadIdx.x;
             Transition tr; tr.s = nullptr; tr.ax = tr.ay = 0.f;
-            if (gb < a.B) tr = resolve_transition(a.src, gb, cn.in_dim - kSacA, pkey);
+            if (gb < a.B) tr = resolve_transition(sac_src<GR>(a), gb, cn.in_dim - kSacA, pkey);
             rows[threadIdx.x] = (gb < a.B) ? tr.s : nullptr; s_act[threadIdx.x][0] = tr.ax; s_act[threadIdx.x][1] = tr.ay;
         }
         __syncthreads();
@@ -233,7 +258,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
                 float e2 = 0.f;
                 if (gb < a.B)
                     for (int j = 0; j < kSacA; ++j) {
-                        const float diff = Q[b * 32 + j] - a.td[(size_t)gb * kSacA + j];
+                        const float diff = Q[b * 32 + j] - sac_td<GR>(a)[(size_t)gb * kSacA + j];
                         e2 += diff * diff;
                         g[j] = 2.f * diff * inv;
                     }
@@ -241,13 +266,14 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
             }
             __syncthreads();
             if (threadIdx.x == 0) { float s = 0.f; for (int b = 0; b < kTile; ++b) s += s_sq[b]; sq[which] += s; }
-            critic_backward_tile(cn, sw, RC, dYa, dYb, gld, (which ? a.part_c2 : a.part_c1) + (size_t)blockIdx.x * cn.P, iter > 0, nullptr, 0);
+            critic_backward_tile(cn, sw, RC, dYa, dYb, gld, (which ? a.part_c2 : a.part_c1) + sac_part<GR>() * cn.P, iter > 0, nullptr, 0);
         }
     }
-    if (threadIdx.x == 0) { a.stat[blockIdx.x * 4 + 0] = sq[0]; a.stat[blockIdx.x * 4 + 1] = sq[1]; }
+    if (threadIdx.x == 0) { a.stat[sac_part<GR>() * 4 + 0] = sq[0]; a.stat[sac_part<GR>() * 4 + 1] = sq[1]; }
 }
 
 // ------------------------------------------------------------------ actor update (:362-376)
+template <bool GR>
 __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
 {
     extern __shared__ __align__(16) float smem[];
@@ -262,20 +288,23 @@ __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
         s_dA2[kTile][kSacA], s_l[kTile], s_e[kTile];
     if (threadIdx.x == 0) { for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1); fence_barrier_init(); }
     __syncthreads();
-    if (threadIdx.x == 0) { stage_weights(an, a.img_actor, RA, &bar[0]); stage_weights(cn, a.img_c1, RC, &bar[1]); stage_weights(cn, a.img_c2, WC2, &bar[2]); }
+    if (threadIdx.x == 0) {
+        stage_weights(an, sac_img<GR>(a.img_actor, an), RA, &bar[0]); stage_weights(cn, sac_img<GR>(a.img_c1, cn), RC, &bar[1]);
+        stage_weights(cn, sac_img<GR>(a.img_c2, cn), WC2, &bar[2]);
+    }
     uint32_t pkey[4];
-    Philox::gen(a.src.key, a.src.epoch, 0x5A17ull, pkey);
-    const float alpha = expf(*a.log_alpha);
+    Philox::gen(sac_sample_key<GR>(a), a.src.epoch, 0x5A17ull, pkey);
+    const float alpha = expf(a.log_alpha[3 * sac_g<GR>()]);
     const float inv = 1.f / ((float)a.B * (float)kSacA);
     float loss_acc = 0.f, ent_acc = 0.f;
     bool ready = false;
     int iter = 0;
-    float *gpart = a.part_a + (size_t)blockIdx.x * an.P;
+    float *gpart = a.part_a + sac_part<GR>() * an.P;
     for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x, ++iter) {
         if (threadIdx.x < kTile) {
             const int gb = t * kTile + threadIdx.x;
             Transition tr; tr.s = nullptr;
-            if (gb < a.B) tr = resolve_transition(a.src, gb, an.in_dim, pkey);
+            if (gb < a.B) tr = resolve_transition(sac_src<GR>(a), gb, an.in_dim, pkey);
             rows[threadIdx.x] = (gb < a.B) ? tr.s : nullptr;
         }
         __syncthreads();
@@ -286,7 +315,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
         if (threadIdx.x < kTile) {
             const int b = threadIdx.x, gb = t * kTile + b;
             float e[2] = { 0.f, 0.f };
-            if (gb < a.B) noise2(a, gb, e[0], e[1]);
+            if (gb < a.B) noise2(sac_eps<GR>(a), sac_noise_key<GR>(a), a.ctr, gb, e[0], e[1]);
             for (int j = 0; j < kSacA; ++j) {
                 s_eps[b][j] = e[j];
                 s_o[b][j] = actor_point(head[b * 32 + j], head[b * 32 + kSacA + j], e[j]);
@@ -351,20 +380,28 @@ __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
             __syncthreads();
         }
     }
-    if (threadIdx.x == 0) { a.stat[blockIdx.x * 4 + 2] = loss_acc; a.stat[blockIdx.x * 4 + 3] = ent_acc; }
+    if (threadIdx.x == 0) { a.stat[sac_part<GR>() * 4 + 2] = loss_acc; a.stat[sac_part<GR>() * 4 + 3] = ent_acc; }
 }
 
 // ------------------------------------------------------------------ alpha step + soft target update + scalar outputs
 struct SacFinishArgs {
     int Pc, nparts;
+    int img_floats;                      // per-trainer stride of the critic weight images
     float tau, alpha_lr, target_entropy, inv_n, step_size_scale, bc2_sqrt;
     int do_alpha;
 };
 
+// blockIdx.y = trainer g: its stat [nparts][4], scal [3], critics and targets [Pc], target images and out [4]
 __global__ void sac_finish_kernel(SacFinishArgs f, const float *__restrict__ stat, float *__restrict__ scal, const float *__restrict__ c1,
                                   const float *__restrict__ c2, float *__restrict__ t1, float *__restrict__ t2, float *__restrict__ img_t1,
                                   float *__restrict__ img_t2, const int32_t *__restrict__ cmap, float *__restrict__ out)
 {
+    {
+        const size_t g = blockIdx.y, gp = g * (size_t)f.Pc, gi = g * (size_t)f.img_floats;
+        stat += g * 4 * (size_t)f.nparts; scal += 3 * g;
+        c1 += gp; c2 += gp; t1 += gp; t2 += gp; img_t1 += gi; img_t2 += gi;
+        if (out) out += 4 * g;
+    }
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < f.Pc) {                                                           // soft_update (:145-147) with the updated critics
         const int im = cmap[i];
@@ -399,7 +436,8 @@ __global__ void sac_finish_kernel(SacFinishArgs f, const float *__restrict__ sta
     }
 }
 
-// get_action (:444-448): action = actor(state)[0] with fresh noise
+// get_action (:444-448): action = actor(state)[0] with fresh noise.  Trainer blockIdx.y acts for rows [g n, (g + 1) n).
+template <bool GR>
 __global__ void __launch_bounds__(kNetThreads) sac_act_kernel(SacArgs a, const float *__restrict__ obs, int n, float *__restrict__ actions)
 {
     extern __shared__ __align__(16) float smem[];
@@ -407,9 +445,13 @@ __global__ void __launch_bounds__(kNetThreads) sac_act_kernel(SacArgs a, const f
     float *RA = smem, *head = RA + an.smem_total_floats;
     __shared__ uint64_t bar;
     __shared__ const float *rows[kTile];
+    const int g = sac_g<GR>();
+    const float *img = sac_img<GR>(a.img_actor, an), *eps = a.eps ? a.eps + (size_t)g * n * kSacA : nullptr;
+    const uint64_t key = sac_noise_key<GR>(a);
+    obs += (size_t)g * n * an.in_dim; actions += (size_t)g * n * kSacA;
     if (threadIdx.x == 0) { mbar_init(&bar, 1); fence_barrier_init(); }
     __syncthreads();
-    if (threadIdx.x == 0) stage_weights(an, a.img_actor, RA, &bar);
+    if (threadIdx.x == 0) stage_weights(an, img, RA, &bar);
     bool ready = false;
     for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x) {
         if (threadIdx.x < kTile) rows[threadIdx.x] = (t * kTile + threadIdx.x < n) ? obs + (size_t)(t * kTile + threadIdx.x) * an.in_dim : nullptr;
@@ -422,12 +464,24 @@ __global__ void __launch_bounds__(kNetThreads) sac_act_kernel(SacArgs a, const f
             const int b = threadIdx.x, gb = t * kTile + b;
             if (gb < n) {
                 float e[2];
-                noise2(a, gb, e[0], e[1]);
+                noise2(eps, key, a.ctr, gb, e[0], e[1]);
                 for (int j = 0; j < kSacA; ++j) actions[(size_t)gb * kSacA + j] = actor_point(head[b * 32 + j], head[b * 32 + kSacA + j], e[j]).a * a.h.bound;
             }
         }
         __syncthreads();
     }
+}
+
+// Federated_Learning_AC (Envs/PathPlan_City.py:590-601): global = deepcopy(actor_0); global[k] += actor_i[k] for i = 1 .. G-1;
+// every actor <- global.  The reference's division assigns into a temporary state_dict and is lost, so every actor becomes the
+// float32 sum theta_0 + theta_1 + ... + theta_{G-1}, added left to right in trainer order.  One thread per actor parameter.
+__global__ void sac_federate_kernel(int P, int G, float *__restrict__ actor)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    float s = actor[i];
+    for (int g = 1; g < G; ++g) s = __fadd_rn(s, actor[(size_t)g * P + i]);
+    for (int g = 0; g < G; ++g) actor[(size_t)g * P + i] = s;
 }
 
 // uavrl_sac_replay_gather: logical indices of the lockstep ring -> packed rows (one warp per transition)
@@ -483,7 +537,8 @@ static size_t smem_act(const SacShape &s) { return (size_t)(s.actor.smem_total_f
 // dynamic and static shared memory of one CTA of each kernel: target, critic, actor, act
 static int sac_smem_total(const SacShape &s, size_t out[4])
 {
-    const void *k[4] = { (const void *)sac_target_kernel, (const void *)sac_critic_kernel, (const void *)sac_actor_kernel, (const void *)sac_act_kernel };
+    const void *k[4] = { (const void *)sac_target_kernel<true>, (const void *)sac_critic_kernel<true>, (const void *)sac_actor_kernel<true>,
+                         (const void *)sac_act_kernel<true> };     // the one-trainer instances declare the same static shared memory
     const size_t dyn[4] = { smem_target(s), smem_critic(s), smem_actor(s), smem_act(s) };
     for (int i = 0; i < 4; ++i) {
         cudaFuncAttributes fa;
@@ -493,15 +548,19 @@ static int sac_smem_total(const SacShape &s, size_t out[4])
     return 0;
 }
 
+// A grouped learner (uavrl_sac_create_trainers) holds G trainers: every per-network vector, weight image and scratch array
+// below is [G][...]; trainer g acts for envs [g Ng, (g + 1) Ng) of the shared ring frames and samples only their transitions.
 struct uavrl_sac {
     uavrl_sac_config cfg;
     SacShape sh;
+    int32_t G = 1;
     float *p[5] = { nullptr }, *img[5] = { nullptr };      // actor, c1, c2, t1, t2
     float *m[3] = { nullptr }, *v[3] = { nullptr }, *grad[3] = { nullptr };
     int32_t *map_a = nullptr, *map_c = nullptr;
-    float *part[3] = { nullptr };                          // gradient partials
-    float *stat = nullptr, *scal = nullptr, *out = nullptr, *td = nullptr, *lossbuf = nullptr;
-    int32_t td_cap = 0, max_ctas = 4 * num_sms();
+    float *part[3] = { nullptr };                          // gradient partials [G][parts_cap][P]
+    float *stat = nullptr, *out = nullptr, *td = nullptr, *lossbuf = nullptr;   // [G][parts_cap][4], [G][4], [G][td_cap][2]
+    float *scal = nullptr;                                 // [G][3]: log_alpha, its Adam exp_avg, exp_avg_sq
+    int32_t td_cap = 0, parts_cap = 0, max_ctas = 4 * num_sms();
     int64_t epoch = 0, adam_t = 0;
     uint64_t calls = 0;
     // lockstep replay ring (continuous actions)
@@ -514,7 +573,8 @@ struct uavrl_sac {
 static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
 {
     const NetDev &n = role == 0 ? s->sh.actor : s->sh.critic;
-    pack_image_kernel<<<(n.P + 255) / 256, 256, 0, st>>>(n.P, s->p[role], role == 0 ? s->map_a : s->map_c, s->img[role], 0);
+    pack_image_kernel<<<dim3((n.P + 255) / 256, s->G), 256, 0, st>>>(n.P, s->p[role], role == 0 ? s->map_a : s->map_c, s->img[role],
+                                                                     n.smem_w_floats);
     UAVRL_LAUNCHED();
     return 0;
 }
@@ -524,15 +584,15 @@ static void sac_fill_args(uavrl_sac *s, SacArgs &a, const BatchSrc &src, int B, 
     memset(&a, 0, sizeof(a));
     a.actor = s->sh.actor; a.critic = s->sh.critic; a.src = src; a.B = B; a.n_tiles = (B + kTile - 1) / kTile; a.gld = s->sh.gld;
     a.img_actor = s->img[0]; a.img_c1 = s->img[1]; a.img_c2 = s->img[2]; a.img_t1 = s->img[3]; a.img_t2 = s->img[4];
-    a.eps = eps; a.key = s->cfg.seed ^ 0x5AC5ull; a.ctr = ctr; a.log_alpha = s->scal; a.td = s->td;
+    a.eps = eps; a.key = s->cfg.seed ^ kNoiseSalt; a.ctr = ctr; a.log_alpha = s->scal; a.td = s->td;
     a.part_a = s->part[0]; a.part_c1 = s->part[1]; a.part_c2 = s->part[2]; a.stat = s->stat;
     a.h = SacHyper{ s->cfg.actor_lr, s->cfg.critic_lr, s->cfg.alpha_lr, s->cfg.target_entropy, s->cfg.gamma, s->cfg.tau, s->cfg.action_bound };
 }
 
-static void adam_args(AdamArgs &a, int P, int nparts, float lr, int64_t t)
+static void adam_args(AdamArgs &a, const NetDev &n, int nparts, float lr, int64_t t)
 {
     memset(&a, 0, sizeof(a));
-    a.P = P; a.nparts = nparts; a.n_loss_parts = 0; a.apply = 1; a.world = 1;
+    a.P = n.P; a.nparts = nparts; a.n_loss_parts = 0; a.apply = 1; a.world = 1; a.img_floats = n.smem_w_floats;
     const double b1 = 0.9, b2 = 0.999;
     const double bc1 = 1.0 - pow(b1, (double)t), bc2 = 1.0 - pow(b2, (double)t);
     a.step_size = (float)((double)lr / bc1);
@@ -540,46 +600,75 @@ static void adam_args(AdamArgs &a, int P, int nparts, float lr, int64_t t)
     a.eps = 1e-8f; a.bc2_sqrt = (float)sqrt(bc2); a.inv_b = 1.f;
 }
 
-// one SAC_Trainer.update on the batch described by src
-static int sac_update_impl(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev, cudaStream_t st)
+// gradient partial / stat slots per trainer for a per-trainer batch B: the tile kernels' grid.  They grow (never shrink) when a
+// larger explicit batch arrives; TD targets likewise
+static int sac_scratch(uavrl_sac *s, int B, int grid, cudaStream_t st)
 {
+    const size_t G = (size_t)s->G;
+    int rc;
+    if (grid > s->parts_cap) {
+        UAVRL_CUDA(cudaStreamSynchronize(st));
+        for (int r = 0; r < 3; ++r) { cudaFree(s->part[r]); s->part[r] = nullptr; }
+        cudaFree(s->stat); s->stat = nullptr;
+        s->parts_cap = 0;
+        for (int r = 0; r < 3; ++r)
+            if ((rc = dev_alloc(&s->part[r], G * grid * (size_t)(r == 0 ? s->sh.actor.P : s->sh.critic.P)))) return rc;
+        if ((rc = dev_alloc(&s->stat, G * grid * 4))) return rc;
+        s->parts_cap = grid;
+    }
     if (B > s->td_cap) {
         UAVRL_CUDA(cudaStreamSynchronize(st));
-        cudaFree(s->td);
-        UAVRL_CUDA(cudaMalloc((void **)&s->td, (size_t)B * kSacA * 4));
+        cudaFree(s->td); s->td = nullptr;
+        s->td_cap = 0;
+        if ((rc = dev_alloc(&s->td, G * B * kSacA))) return rc;
         s->td_cap = B;
     }
-    SacArgs a;
+    return 0;
+}
+
+// one SAC_Trainer.update of every trainer on the batch described by src (B rows per trainer)
+static int sac_update_impl(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev, cudaStream_t st)
+{
     const int n_tiles = (B + kTile - 1) / kTile;
     const int grid = n_tiles < s->max_ctas ? n_tiles : s->max_ctas;
+    int rc = sac_scratch(s, B, grid, st);
+    if (rc) return rc;
+    const dim3 tiles(grid, s->G);                        // y: trainer
+    SacArgs a;
     s->adam_t += 1;
     sac_fill_args(s, a, src, B, eps_next, 2 * (uint64_t)s->epoch);
-    sac_target_kernel<<<grid, kNetThreads, smem_target(s->sh), st>>>(a);
+    if (s->G > 1) sac_target_kernel<true><<<tiles, kNetThreads, smem_target(s->sh), st>>>(a);
+    else sac_target_kernel<false><<<grid, kNetThreads, smem_target(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
-    sac_critic_kernel<<<grid, kNetThreads, smem_critic(s->sh), st>>>(a);
+    if (s->G > 1) sac_critic_kernel<true><<<tiles, kNetThreads, smem_critic(s->sh), st>>>(a);
+    else sac_critic_kernel<false><<<grid, kNetThreads, smem_critic(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
     AdamArgs aa;
     for (int c = 1; c <= 2; ++c) {
-        adam_args(aa, s->sh.critic.P, grid, s->cfg.critic_lr, s->adam_t);
-        reduce_adam_kernel<<<(aa.P + 63) / 64, 256, 0, st>>>(aa, s->part[c], s->lossbuf, s->grad[c], s->p[c], s->m[c], s->v[c], nullptr, s->img[c],
-                                                             nullptr, s->map_c, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        adam_args(aa, s->sh.critic, grid, s->cfg.critic_lr, s->adam_t);
+        reduce_adam_kernel<<<dim3((aa.P + 63) / 64, s->G), 256, 0, st>>>(aa, s->part[c], s->lossbuf, s->grad[c], s->p[c], s->m[c], s->v[c], nullptr,
+                                                                        s->img[c], nullptr, s->map_c, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                                        nullptr, nullptr);
         UAVRL_LAUNCHED();
     }
     sac_fill_args(s, a, src, B, eps_cur, 2 * (uint64_t)s->epoch + 1);
-    sac_actor_kernel<<<grid, kNetThreads, smem_actor(s->sh), st>>>(a);
+    if (s->G > 1) sac_actor_kernel<true><<<tiles, kNetThreads, smem_actor(s->sh), st>>>(a);
+    else sac_actor_kernel<false><<<grid, kNetThreads, smem_actor(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
-    adam_args(aa, s->sh.actor.P, grid, s->cfg.actor_lr, s->adam_t);
-    reduce_adam_kernel<<<(aa.P + 63) / 64, 256, 0, st>>>(aa, s->part[0], s->lossbuf, s->grad[0], s->p[0], s->m[0], s->v[0], nullptr, s->img[0], nullptr,
-                                                         s->map_a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+    adam_args(aa, s->sh.actor, grid, s->cfg.actor_lr, s->adam_t);
+    reduce_adam_kernel<<<dim3((aa.P + 63) / 64, s->G), 256, 0, st>>>(aa, s->part[0], s->lossbuf, s->grad[0], s->p[0], s->m[0], s->v[0], nullptr,
+                                                                    s->img[0], nullptr, s->map_a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                                    nullptr);
     UAVRL_LAUNCHED();
     SacFinishArgs f;
     memset(&f, 0, sizeof(f));
-    f.Pc = s->sh.critic.P; f.nparts = grid; f.tau = s->cfg.tau; f.alpha_lr = s->cfg.alpha_lr; f.target_entropy = s->cfg.target_entropy;
+    f.Pc = s->sh.critic.P; f.nparts = grid; f.img_floats = s->sh.critic.smem_w_floats;
+    f.tau = s->cfg.tau; f.alpha_lr = s->cfg.alpha_lr; f.target_entropy = s->cfg.target_entropy;
     f.inv_n = 1.f / ((float)B * (float)kSacA); f.do_alpha = 1;
     const double bc1 = 1.0 - pow(0.9, (double)s->adam_t), bc2 = 1.0 - pow(0.999, (double)s->adam_t);
     f.step_size_scale = (float)((double)s->cfg.alpha_lr / bc1); f.bc2_sqrt = (float)sqrt(bc2);
-    sac_finish_kernel<<<(f.Pc + 255) / 256, 256, 0, st>>>(f, s->stat, s->scal, s->p[1], s->p[2], s->p[3], s->p[4], s->img[3], s->img[4], s->map_c,
-                                                         losses_dev ? losses_dev : s->out);
+    sac_finish_kernel<<<dim3((f.Pc + 255) / 256, s->G), 256, 0, st>>>(f, s->stat, s->scal, s->p[1], s->p[2], s->p[3], s->p[4], s->img[3],
+                                                                     s->img[4], s->map_c, losses_dev ? losses_dev : s->out);
     UAVRL_LAUNCHED();
     return 0;
 }
@@ -589,31 +678,36 @@ static int sac_update_impl(uavrl_sac *s, const BatchSrc &src, int B, const float
 static int sac_alloc(uavrl_sac *s)
 {
     const uavrl_sac_config *cfg = &s->cfg;
+    const size_t G = (size_t)s->G;
     int rc;
     for (int r = 0; r < 5; ++r) {
         const NetDev &n = r == 0 ? s->sh.actor : s->sh.critic;
-        if ((rc = dev_alloc(&s->p[r], (size_t)n.P)) || (rc = dev_alloc(&s->img[r], (size_t)n.smem_w_floats))) return rc;
+        if ((rc = dev_alloc(&s->p[r], G * n.P)) || (rc = dev_alloc(&s->img[r], G * n.smem_w_floats))) return rc;
     }
     for (int r = 0; r < 3; ++r) {
         const NetDev &n = r == 0 ? s->sh.actor : s->sh.critic;
-        if ((rc = dev_alloc(&s->m[r], (size_t)n.P)) || (rc = dev_alloc(&s->v[r], (size_t)n.P)) || (rc = dev_alloc(&s->grad[r], (size_t)n.P)) ||
-            (rc = dev_alloc(&s->part[r], (size_t)n.P * s->max_ctas)))
-            return rc;
+        if ((rc = dev_alloc(&s->m[r], G * n.P)) || (rc = dev_alloc(&s->v[r], G * n.P)) || (rc = dev_alloc(&s->grad[r], G * n.P))) return rc;
     }
     std::vector<int32_t> ma, mc;
     build_image_map(s->sh.actor, ma); build_image_map(s->sh.critic, mc);
     if ((rc = dev_alloc(&s->map_a, ma.size())) || (rc = dev_alloc(&s->map_c, mc.size()))) return rc;
     UAVRL_CUDA(cudaMemcpy(s->map_a, ma.data(), ma.size() * 4, cudaMemcpyHostToDevice));
     UAVRL_CUDA(cudaMemcpy(s->map_c, mc.data(), mc.size() * 4, cudaMemcpyHostToDevice));
-    if ((rc = dev_alloc(&s->stat, (size_t)4 * s->max_ctas)) || (rc = dev_alloc(&s->scal, 4)) || (rc = dev_alloc(&s->out, 4)) ||
-        (rc = dev_alloc(&s->lossbuf, (size_t)s->max_ctas)) || (rc = dev_alloc(&s->td, (size_t)cfg->batch_size * kSacA)))
-        return rc;
-    s->td_cap = cfg->batch_size;
-    const float la0 = logf(0.01f);                                     // SAC_Trainer.py:53
-    UAVRL_CUDA(cudaMemcpy(s->scal, &la0, 4, cudaMemcpyHostToDevice));
+    {   // gradient partial / stat slots per trainer: one learner keeps max_ctas (any batch); a grouped learner sizes them from the
+        // per-trainer batch and grows them for larger explicit batches (sac_scratch)
+        const int tiles = (cfg->batch_size + kTile - 1) / kTile;
+        const int cap = (G == 1 || tiles > s->max_ctas) ? s->max_ctas : tiles;
+        if ((rc = sac_scratch(s, cfg->batch_size, cap, 0))) return rc;
+    }
+    if ((rc = dev_alloc(&s->scal, 3 * G)) || (rc = dev_alloc(&s->out, 4 * G)) || (rc = dev_alloc(&s->lossbuf, 1))) return rc;
+    std::vector<float> init(3 * G, 0.f);
+    for (size_t g = 0; g < G; ++g) init[3 * g] = logf(0.01f);          // SAC_Trainer.py:53
+    UAVRL_CUDA(cudaMemcpy(s->scal, init.data(), init.size() * 4, cudaMemcpyHostToDevice));
     if (cfg->lockstep_envs > 0) {
-        const int64_t N = cfg->lockstep_envs;
-        int64_t cap_frames = (cfg->replay_capacity + N - 1) / N;
+        // the ring holds, for every trainer, the frames a stand-alone learner with replay_capacity / G transitions over N / G
+        // envs would keep
+        const int64_t N = cfg->lockstep_envs, Ng = N / s->G, cap_g = cfg->replay_capacity / s->G;
+        int64_t cap_frames = (cap_g + Ng - 1) / Ng;
         if (cap_frames < 2) cap_frames = 2;
         s->ring_frames = cap_frames + 1;
         const size_t slots = (size_t)s->ring_frames * N;
@@ -621,8 +715,10 @@ static int sac_alloc(uavrl_sac *s)
             (rc = dev_alloc(&s->r_done, slots)))
             return rc;
     }
-    if ((rc = raise_dyn_smem(sac_target_kernel, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel, smem_critic(s->sh))) ||
-        (rc = raise_dyn_smem(sac_actor_kernel, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel, smem_act(s->sh))))
+    if ((rc = raise_dyn_smem(sac_target_kernel<false>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<false>, smem_critic(s->sh))) ||
+        (rc = raise_dyn_smem(sac_actor_kernel<false>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<false>, smem_act(s->sh))) ||
+        (rc = raise_dyn_smem(sac_target_kernel<true>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true>, smem_critic(s->sh))) ||
+        (rc = raise_dyn_smem(sac_actor_kernel<true>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<true>, smem_act(s->sh))))
         return rc;
     return 0;
 }
@@ -646,7 +742,18 @@ int uavrl_sac_smem_bytes(const uavrl_sac_config *cfg, int64_t *bytes_out)
 
 int uavrl_sac_create(const uavrl_sac_config *cfg, uavrl_sac **out)
 {
+    return uavrl_sac_create_trainers(cfg, 1, out);
+}
+
+int uavrl_sac_create_trainers(const uavrl_sac_config *cfg, int32_t n_trainers, uavrl_sac **out)
+{
     if (!cfg || !out) return fail(UAVRL_ERR_INVALID, "uavrl_sac_create: null argument");
+    if (n_trainers < 1 || n_trainers > 65535)        // every grouped kernel runs one grid row per trainer: gridDim.y <= 65535
+        return fail(UAVRL_ERR_INVALID, "n_trainers must be in [1, 65535]");
+    if (n_trainers > 1 && (cfg->lockstep_envs < 0 || cfg->lockstep_envs % n_trainers != 0))
+        return fail(UAVRL_ERR_INVALID, "lockstep_envs must be a multiple of n_trainers (every trainer owns lockstep_envs / n_trainers envs)");
+    if (n_trainers > 1 && cfg->replay_capacity / n_trainers <= 0)
+        return fail(UAVRL_ERR_INVALID, "replay_capacity / n_trainers must be > 0");
     if (cfg->batch_size <= 0 || cfg->replay_capacity <= 0) return fail(UAVRL_ERR_INVALID, "batch_size and replay_capacity must be > 0");
     SacShape sh;
     int rc = sac_shape(*cfg, sh);
@@ -663,6 +770,7 @@ int uavrl_sac_create(const uavrl_sac_config *cfg, uavrl_sac **out)
     uavrl_sac *s = new uavrl_sac();
     s->cfg = *cfg;
     s->sh = sh;
+    s->G = n_trainers;
     {   // grid cap of the tile kernels: 4 CTAs per SM's worth of tiles, i.e. one tile per CTA up to batch 4 x SMs x 32.  (One CTA
         // per SM looping over its tiles would accumulate ONE partial, at the price of a read-modify-write of the global partial
         // per tile.)
@@ -692,6 +800,7 @@ int uavrl_sac_destroy(uavrl_sac *s)
 }
 
 int64_t uavrl_sac_param_count(const uavrl_sac *s, int32_t role) { return !s ? 0 : (role == 0 ? s->sh.actor.P : s->sh.critic.P); }
+int32_t uavrl_sac_trainer_count(const uavrl_sac *s) { return s ? s->G : 0; }
 
 static float *sac_buf(uavrl_sac *s, int role)
 {
@@ -710,7 +819,7 @@ int uavrl_sac_set_params(uavrl_sac *s, int32_t role, const float *h)
     UAVRL_CUDA(cudaDeviceSynchronize());
     const int rr = role < 5 ? role : (role - 5) % 3;
     const int P = rr == 0 ? s->sh.actor.P : s->sh.critic.P;
-    UAVRL_CUDA(cudaMemcpy(sac_buf(s, role), h, (size_t)P * 4, cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(sac_buf(s, role), h, (size_t)s->G * P * 4, cudaMemcpyHostToDevice));
     if (role < 5) { int rc = sac_pack(s, role, 0); if (rc) return rc; UAVRL_CUDA(cudaDeviceSynchronize()); }
     return 0;
 }
@@ -722,7 +831,25 @@ int uavrl_sac_get_params(uavrl_sac *s, int32_t role, float *h)
     UAVRL_CUDA(cudaDeviceSynchronize());
     const int rr = role < 5 ? role : (role - 5) % 3;
     const int P = rr == 0 ? s->sh.actor.P : s->sh.critic.P;
-    UAVRL_CUDA(cudaMemcpy(h, sac_buf(s, role), (size_t)P * 4, cudaMemcpyDeviceToHost));
+    UAVRL_CUDA(cudaMemcpy(h, sac_buf(s, role), (size_t)s->G * P * 4, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int uavrl_sac_set_alpha(uavrl_sac *s, const float *h)
+{
+    if (!s || !h) return fail(UAVRL_ERR_INVALID, "bad argument");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    UAVRL_CUDA(cudaDeviceSynchronize());
+    UAVRL_CUDA(cudaMemcpy(s->scal, h, (size_t)s->G * 3 * 4, cudaMemcpyHostToDevice));
+    return 0;
+}
+
+int uavrl_sac_get_alpha(uavrl_sac *s, float *h)
+{
+    if (!s || !h) return fail(UAVRL_ERR_INVALID, "bad argument");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    UAVRL_CUDA(cudaDeviceSynchronize());
+    UAVRL_CUDA(cudaMemcpy(h, s->scal, (size_t)s->G * 3 * 4, cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -731,8 +858,9 @@ int uavrl_sac_set_scalars(uavrl_sac *s, float log_alpha, float la_m, float la_v,
     if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     UAVRL_CUDA(cudaDeviceSynchronize());
-    const float v[3] = { log_alpha, la_m, la_v };
-    UAVRL_CUDA(cudaMemcpy(s->scal, v, sizeof(v), cudaMemcpyHostToDevice));
+    std::vector<float> v((size_t)s->G * 3);                    // the same triple for every trainer
+    for (size_t g = 0; g < (size_t)s->G; ++g) { v[3 * g] = log_alpha; v[3 * g + 1] = la_m; v[3 * g + 2] = la_v; }
+    UAVRL_CUDA(cudaMemcpy(s->scal, v.data(), v.size() * 4, cudaMemcpyHostToDevice));
     s->epoch = epoch; s->adam_t = adam_step;
     return 0;
 }
@@ -755,13 +883,16 @@ int uavrl_sac_get_scalars(uavrl_sac *s, float *log_alpha, float *la_m, float *la
 int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *eps_dev, float *actions_dev, void *stream)
 {
     if (!s || !obs_dev || !actions_dev || n <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (n % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_act: n must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     SacArgs a;
     BatchSrc none;
     memset(&none, 0, sizeof(none));
-    sac_fill_args(s, a, none, n, eps_dev, 0x8000000000000000ull | s->calls++);
+    const int ng = n / s->G;                                   // rows per trainer: block g belongs to trainer g
+    sac_fill_args(s, a, none, ng, eps_dev, 0x8000000000000000ull | s->calls++);
     const int grid = a.n_tiles < s->max_ctas ? a.n_tiles : s->max_ctas;
-    sac_act_kernel<<<grid, kNetThreads, smem_act(s->sh), (cudaStream_t)stream>>>(a, obs_dev, n, actions_dev);
+    if (s->G > 1) sac_act_kernel<true><<<dim3(grid, s->G), kNetThreads, smem_act(s->sh), (cudaStream_t)stream>>>(a, obs_dev, ng, actions_dev);
+    else sac_act_kernel<false><<<grid, kNetThreads, smem_act(s->sh), (cudaStream_t)stream>>>(a, obs_dev, ng, actions_dev);
     UAVRL_LAUNCHED();
     return 0;
 }
@@ -770,25 +901,26 @@ int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const fl
                            const float *d_dev, const float *eps_next_dev, const float *eps_cur_dev, float *losses_dev, void *stream)
 {
     if (!s || B <= 0 || !s_dev || !a_dev || !r_dev || !s2_dev || !d_dev) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (B % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_update_batch: B must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;                                             // SAC_Trainer.py:320
     BatchSrc src;
     memset(&src, 0, sizeof(src));
     src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.act2 = a_dev; src.rew = r_dev; src.done_f32 = d_dev;
-    return sac_update_impl(s, src, B, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
+    return sac_update_impl(s, src, B / s->G, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
 }
 
-// the lockstep ring as a batch source: idx_tape (device, [batch_size] logical indices, 0 = oldest) or Philox sampling keyed
-// by the epoch
+// the lockstep ring as a batch source: idx_tape (device, [G][batch_size] trainer-local logical indices, 0 = oldest) or Philox
+// sampling keyed by the epoch.  Every trainer samples its own block of N / G envs (trainer_src), count = its transitions
 static BatchSrc sac_ring_source(const uavrl_sac *s, const int32_t *idx_tape)
 {
     const int64_t N = s->cfg.lockstep_envs, R = s->ring_frames;
     BatchSrc src;
     memset(&src, 0, sizeof(src));
     src.mode = kReplayLockstep; src.frames = s->frames; src.act2 = s->r_act2; src.rew = s->r_rew; src.done_u8 = s->r_done;
-    src.count = s->count; src.cap = R; src.n_envs = (int32_t)N;
+    src.count = s->count / s->G; src.cap = R; src.n_envs = (int32_t)(N / s->G); src.row_stride = (int32_t)N;
     src.oldest = ((s->head - s->count / N) % R + R) % R;
-    src.key = s->cfg.seed ^ 0x5EEDull; src.epoch = (uint64_t)s->epoch;
+    src.key = s->cfg.seed ^ kSampleSalt; src.epoch = (uint64_t)s->epoch;
     src.idx_tape = idx_tape;
     return src;
 }
@@ -804,7 +936,8 @@ int uavrl_sac_replay_gather(uavrl_sac *s, int32_t n, const int64_t *idx, float *
         if (idx[i] < 0 || idx[i] >= s->count) return fail(UAVRL_ERR_INVALID, "logical index out of range");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     UAVRL_CUDA(cudaDeviceSynchronize());
-    const BatchSrc src = sac_ring_source(s, nullptr);
+    BatchSrc src = sac_ring_source(s, nullptr);
+    src.n_envs = src.row_stride;                                // whole-ring logical indices, whatever the trainer count
     const size_t in = (size_t)s->cfg.obs_dim;
     int64_t *d_idx = nullptr; float *d_s = nullptr, *d_s2 = nullptr, *d_a = nullptr, *d_r = nullptr; uint8_t *d_d = nullptr;
     struct Free { void **p[6]; ~Free() { for (auto q : p) if (*q) cudaFree(*q); } } guard{ { (void **)&d_idx, (void **)&d_s, (void **)&d_s2,
@@ -833,8 +966,19 @@ int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const flo
     if (!s->frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;                                             // SAC_Trainer.py:320
-    if (s->count <= s->cfg.batch_size) return 0;               // PathPlan_City.py:383: nothing sampled yet
+    if (s->count / s->G <= s->cfg.batch_size) return 0;        // PathPlan_City.py:383: nothing sampled yet (per trainer)
     return sac_update_impl(s, sac_ring_source(s, idx_tape_dev), s->cfg.batch_size, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
+}
+
+int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int P = s->sh.actor.P;
+    sac_federate_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, s->G, s->p[0]);
+    UAVRL_LAUNCHED();
+    return sac_pack(s, 0, st);                                 // the G actor images
 }
 
 // lockstep loop with the continuous env step: state -> actor sample -> Move_Agent -> replay add -> update
@@ -865,21 +1009,24 @@ int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t d
         s->count = s->count + N > maxc ? maxc : s->count + N;
         if (do_update) {
             s->epoch += 1;
-            if (s->count <= s->cfg.batch_size) continue;
+            if (s->count / s->G <= s->cfg.batch_size) continue;     // per trainer
             if ((rc = sac_update_impl(s, sac_ring_source(s, nullptr), s->cfg.batch_size, nullptr, nullptr, nullptr, st))) return rc;
             ++updates;
         }
     }
     if (stats_host) {
         UAVRL_CUDA(cudaStreamSynchronize(st));
-        unsigned long long c1[8]; double r1; float o[4];
+        unsigned long long c1[8]; double r1;
         UAVRL_CUDA(cudaMemcpy(c1, env->d.stat_counts, sizeof(c1), cudaMemcpyDeviceToHost));
         UAVRL_CUDA(cudaMemcpy(&r1, env->d.stat_reward, sizeof(r1), cudaMemcpyDeviceToHost));
-        UAVRL_CUDA(cudaMemcpy(o, s->out, sizeof(o), cudaMemcpyDeviceToHost));
+        std::vector<float> o((size_t)s->G * 4);                 // [G][4]; last_loss = the mean actor loss over trainers
+        UAVRL_CUDA(cudaMemcpy(o.data(), s->out, o.size() * sizeof(float), cudaMemcpyDeviceToHost));
+        double lsum = 0.0;
+        for (int g = 0; g < s->G; ++g) lsum += o[4 * (size_t)g];
         stats_host->env_steps = (int64_t)(c1[0] - c0[0]); stats_host->episodes_ended = (int64_t)(c1[1] - c0[1]);
         stats_host->collisions = (int64_t)(c1[2] - c0[2]); stats_host->n_success = (int64_t)(c1[3] - c0[3]);
         stats_host->n_lose = (int64_t)(c1[4] - c0[4]); stats_host->sum_reward = r1 - r0; stats_host->updates = updates;
-        stats_host->last_loss = o[0];
+        stats_host->last_loss = (float)(lsum / (double)s->G);
     }
     return 0;
 }

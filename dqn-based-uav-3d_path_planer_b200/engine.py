@@ -517,18 +517,26 @@ def train_run_dp(env, learner, n_iters, eps, global_batch):
 class SacLearner:
     """SAC continuous (the reference's shipped trainer, config/Trainer.xml) on one GPU.  obs_dim must be a multiple of 4 in
     [4, 124], hidden in [1, 128], and the networks must fit the kernels' shared memory (sac_smem_bytes).  Parameter roles:
-    0-4 actor, critic_1, critic_2 and their targets, 5-7 / 8-10 Adam moments, 11-13 the last reduced gradients (read-only)."""
+    0-4 actor, critic_1, critic_2 and their targets, 5-7 / 8-10 Adam moments, 11-13 the last reduced gradients (read-only).
+
+    trainers = G > 1: G independent SAC trainers in one handle (one SAC_Trainer per UAV group, PathPlan_City.py:59-69).  The
+    lockstep envs split into G blocks of lockstep_envs / G, trainer g learns from its block only and computes what a
+    stand-alone SacLearner(seed=seed + g, replay_capacity=replay_capacity // G, lockstep_envs=lockstep_envs // G) computes.
+    Parameters are then (G, P) arrays, alpha() is (G, 3), act / update_batch take G equal row blocks and loss tensors hold
+    [G][4] floats (include/uavrl.h, uavrl_sac_create_trainers)."""
     ROLES = ("actor", "critic_1", "critic_2", "target_critic_1", "target_critic_2")
 
     def __init__(self, obs_dim=OBS_DIM, hidden=64, act_dim=2, action_bound=1.0, actor_lr=1e-4, critic_lr=1e-3, alpha_lr=1e-4,
-                 target_entropy=1.0, gamma=0.99, tau=0.05, batch_size=64, replay_capacity=10000, lockstep_envs=0, seed=42, device=0):
+                 target_entropy=1.0, gamma=0.99, tau=0.05, batch_size=64, replay_capacity=10000, lockstep_envs=0, seed=42, device=0,
+                 trainers=1):
         self.device = torch.device("cuda", device)
         c = _lib.SacConfig(obs_dim, hidden, act_dim, action_bound, actor_lr, critic_lr, alpha_lr, target_entropy, gamma, tau,
                            batch_size, replay_capacity, lockstep_envs, seed, device)
         self.cfg = c
         self.h = C.c_void_p()
-        check(_lib.lib().uavrl_sac_create(C.byref(c), C.byref(self.h)))
+        check(_lib.lib().uavrl_sac_create_trainers(C.byref(c), int(trainers), C.byref(self.h)))
         self.P = [int(_lib.lib().uavrl_sac_param_count(self.h, r)) for r in range(5)]
+        self.G = int(_lib.lib().uavrl_sac_trainer_count(self.h))
 
     def close(self):
         if self.h:
@@ -541,28 +549,66 @@ class SacLearner:
         except Exception:
             pass
 
+    def _param_shape(self, role):
+        n = self.P[role] if role < 5 else self.P[(role - 5) % 3]
+        return (n,) if self.G == 1 else (self.G, n)
+
     def set_params(self, role, flat):
+        """(P,) or, with trainers > 1, (G, P) values of `role` for every trainer."""
         flat = np.ascontiguousarray(flat, np.float32)
+        shape = self._param_shape(role)
+        assert flat.size == int(np.prod(shape)), (flat.shape, shape)
         check(_lib.lib().uavrl_sac_set_params(self.h, role, _ptr(flat)))
 
     def get_params(self, role):
-        n = self.P[role] if role < 5 else self.P[(role - 5) % 3]
-        out = np.zeros(n, np.float32)
+        out = np.zeros(self._param_shape(role), np.float32)
         check(_lib.lib().uavrl_sac_get_params(self.h, role, _ptr(out)))
         return out
 
-    def init_params(self, seed=0):
-        """nn.Linear default init for actor and the two critics; targets copy the critics (SAC_Trainer.py:33-34)."""
-        g = torch.Generator().manual_seed(seed)
-        o, h, a = self.cfg.obs_dim, self.cfg.hidden, self.cfg.act_dim
+    def trainer_count(self):
+        return self.G
 
-        def lin(out, fi):
-            b = 1.0 / np.sqrt(fi)
-            return [(torch.rand(out * fi, generator=g) * 2 - 1) * b, (torch.rand(out, generator=g) * 2 - 1) * b]
-        self.set_params(0, torch.cat(lin(h, o) + lin(a, h) + lin(a, h)).numpy())
-        for r in (1, 2):
-            flat = torch.cat(lin(h, o + a) + lin(h, h) + lin(a, h)).numpy()
-            self.set_params(r, flat); self.set_params(r + 2, flat)
+    def init_params(self, seed=0):
+        """nn.Linear default init for actor and the two critics; targets copy the critics (SAC_Trainer.py:33-34).
+        Trainer g of a grouped learner draws with seed + g."""
+        o, h, a = self.cfg.obs_dim, self.cfg.hidden, self.cfg.act_dim
+        draws = []
+        for t in range(self.G):
+            g = torch.Generator().manual_seed(seed + t)
+
+            def lin(out, fi):
+                b = 1.0 / np.sqrt(fi)
+                return [(torch.rand(out * fi, generator=g) * 2 - 1) * b, (torch.rand(out, generator=g) * 2 - 1) * b]
+            draws.append([torch.cat(lin(h, o) + lin(a, h) + lin(a, h)).numpy()] +
+                         [torch.cat(lin(h, o + a) + lin(h, h) + lin(a, h)).numpy() for _ in (1, 2)])
+        for r in range(3):
+            flat = np.stack([d[r] for d in draws])
+            self.set_params(r, flat)
+            if r > 0:
+                self.set_params(r + 2, flat)
+
+    def alpha(self):
+        """Every trainer's (log_alpha, Adam exp_avg, Adam exp_avg_sq): a (G, 3) array."""
+        out = np.zeros((self.G, 3), np.float32)
+        check(_lib.lib().uavrl_sac_get_alpha(self.h, _ptr(out)))
+        return out
+
+    def set_alpha(self, triples):
+        t = np.ascontiguousarray(triples, np.float32)
+        if t.size != 3 * self.G:
+            raise ValueError("alpha triples must be (%d, 3), got %s" % (self.G, t.shape))
+        check(_lib.lib().uavrl_sac_set_alpha(self.h, _ptr(t)))
+
+    def federate_actors(self):
+        """Federated_Learning_AC (PathPlan_City.py:590-601, include/uavrl.h uavrl_sac_federate_actors): every trainer's actor
+        becomes the float32 sum of all G actors (the reference's division by G is lost); nothing else changes."""
+        check(_lib.lib().uavrl_sac_federate_actors(self.h, _stream(self.device)))
+
+    def _losses(self, losses):
+        """A caller's loss tensor: an update writes 4 losses per trainer, so it must hold at least 4 G floats."""
+        if losses is not None and losses.numel() < 4 * self.G:
+            raise ValueError("losses holds %d elements; a learner with %d trainers writes %d losses" % (losses.numel(), self.G, 4 * self.G))
+        return _ptr(losses)
 
     def scalars(self):
         la, m, v = C.c_float(), C.c_float(), C.c_float()
@@ -581,7 +627,7 @@ class SacLearner:
 
     def update_batch(self, s, a, r, s2, d, eps_next=None, eps_cur=None, losses=None):
         check(_lib.lib().uavrl_sac_update_batch(self.h, s.shape[0], _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d), _ptr(eps_next),
-                                                _ptr(eps_cur), _ptr(losses), _stream(self.device)))
+                                                _ptr(eps_cur), self._losses(losses), _stream(self.device)))
 
     def grads(self, role):
         """The gradient of network `role` (0 actor, 1 critic_1, 2 critic_2) that the last update reduced and fed to Adam."""
@@ -604,8 +650,9 @@ class SacLearner:
         return s, a, r, s2, d
 
     def update_replay(self, idx_tape=None, eps_next=None, eps_cur=None, losses=None):
-        """One update sampled from the lockstep ring (idx_tape: device int32 [batch_size] logical indices, None = Philox)."""
-        check(_lib.lib().uavrl_sac_update_replay(self.h, _ptr(idx_tape), _ptr(eps_next), _ptr(eps_cur), _ptr(losses),
+        """One update sampled from the lockstep ring (idx_tape: device int32 [batch_size] logical indices, or [G][batch_size]
+        trainer-local ones; None = Philox)."""
+        check(_lib.lib().uavrl_sac_update_replay(self.h, _ptr(idx_tape), _ptr(eps_next), _ptr(eps_cur), self._losses(losses),
                                                  _stream(self.device)))
 
 

@@ -174,7 +174,8 @@ class PathPlan_City_B200:
         self.epoch = 0
         self.print_loop = int(None2Value(param.get('print_loop'), 2))
         # federated aggregation every FL_Loop episodes (PathPlan_City.py:78-79, :469-475).  With DQN-family trainers it runs the
-        # reference's selective aggregation Federated_Learning_choice (:644-684) across the num_trainers trainers
+        # reference's selective aggregation Federated_Learning_choice (:644-684) across the num_trainers trainers; with SAC
+        # trainers and Is_AC = 1 the reference's Federated_Learning_AC (:590-601)
         self.Is_FL = int(None2Value(param.get('Is_FL'), 0))
         self.FL_Loop = int(None2Value(param.get('FL_Loop'), 3))
         if self.Is_FL:
@@ -303,7 +304,10 @@ class PathPlan_City_B200:
         self.epoch += 1
         self.executed_time += dt
         if self.Is_FL and self.epoch % self.FL_Loop == 0:             # PathPlan_City.py:469-475
-            self.Federated_Learning_choice()
+            if self.Is_AC and is_sac:
+                self.Federated_Learning_AC()
+            else:
+                self.Federated_Learning_choice()
         if self.record_csv:
             self._write_path_csv()
             if self.print_loop > 0 and self.epoch % self.print_loop == 0:
@@ -319,6 +323,13 @@ class PathPlan_City_B200:
         if isinstance(learner, engine.SacLearner) or learner.trainer_count() < 2:
             return
         learner.federate()
+
+    def Federated_Learning_AC(self):
+        """PathPlan_City.py:590-601 on the device (engine.SacLearner.federate_actors): every SAC trainer's actor is replaced by
+        the sum of all trainers' actors.  The reference divides by the trainer count into a temporary state_dict, so the
+        division is lost and the sum is what it trains on; this plug-in reproduces that.  Critics, targets, Adam moments and
+        alpha are untouched; one trainer keeps its actor."""
+        self.Trainer._learner.federate_actors()
 
     def _write_path_csv(self, path="path.csv"):
         """UAV.py:461-464 / :479-482 / :505-508: at a terminal step the reference rewrites path.csv (CWD-relative) with the

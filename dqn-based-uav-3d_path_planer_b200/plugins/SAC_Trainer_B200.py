@@ -32,14 +32,19 @@ class SAC_Trainer_B200:
         self.w, self.hidden, self.act_dim = int(actor.get('w')), int(actor.get('hiden_dim')), int(actor.get('output'))
         self.lockstep_envs = int(None2Value(param.get('lockstep_envs'), 0))
         self.device_index = int(None2Value(param.get('device'), 0))
+        # n_trainers = G > 1: one independent SAC trainer per block of lockstep_envs / G UAVs (the reference's SAC_Trainer per UAV,
+        # PathPlan_City.py:59-69), each with its own replay_size transitions; trainer g is named UAV_<g * lockstep_envs / G>
+        self.n_trainers = int(None2Value(param.get('n_trainers'), 1))
+        G = self.n_trainers
+        self.names = [self.name] if G == 1 else ['UAV_%d' % (g * (self.lockstep_envs // G)) for g in range(G)]
         self._learner = engine.SacLearner(
             self.w, self.hidden, self.act_dim, float(actor.get('action_bound')), float(actor.get('lr')), float(critic.get('lr')),
             float(sp.get('alpha_lr')), float(sp.get('target_entropy')), float(sp.get('gamma')), float(sp.get('tau')),
-            batch_size=self.Batch_Size, replay_capacity=self.replay_size, lockstep_envs=self.lockstep_envs,
-            seed=int(None2Value(param.get('seed'), 42)), device=self.device_index)
+            batch_size=self.Batch_Size, replay_capacity=self.replay_size * G, lockstep_envs=self.lockstep_envs,
+            seed=int(None2Value(param.get('seed'), 42)), device=self.device_index, trainers=G)
         self._learner.init_params(int(None2Value(param.get('seed'), 42)))
         self._dev = self._learner.device
-        self._losses = torch.zeros(4, device=self._dev)
+        self._losses = torch.zeros(4 * G, device=self._dev)
         self.loss = 0
         self.model_dir = None2Value(param.get('model_path'), None)
         self.Load_Mod()
@@ -53,9 +58,12 @@ class SAC_Trainer_B200:
         return self._learner.scalars()["log_alpha"]
 
     def get_action(self, state, eps=0.0):
-        """SAC_Trainer.get_action (:444-448): [a0, a1] for one state, or an [N, 2] array for a batch."""
+        """SAC_Trainer.get_action (:444-448): [a0, a1] for one state, or an [N, 2] array for a batch (with several trainers the
+        [num_UAV, obs] batch: row block g goes to trainer g)."""
         s = np.ascontiguousarray(state, np.float32)
         single = s.ndim == 1
+        if single and self.n_trainers > 1:
+            raise ValueError("get_action with %d trainers takes the [num_UAV, %d] batch, not one state" % (self.n_trainers, self.w))
         a = self._learner.act(torch.from_numpy(s.reshape(-1, self.w)).to(self._dev)).cpu().numpy()
         return a[0].tolist() if single else a
 
@@ -64,7 +72,7 @@ class SAC_Trainer_B200:
         states = transition_dict['states']
         if all(len(sub) == 0 for sub in states) if isinstance(states, list) else len(states) == 0:      # :322-324
             sc = self._learner.scalars()
-            self._learner.set_scalars(sc["log_alpha"], sc["la_m"], sc["la_v"], sc["epoch"] + 1, sc["adam_step"])
+            self._set_counters(sc["epoch"] + 1, sc["adam_step"])
             return {'sum_epoch': self.epoch, 'loss': self.loss}
         dev = self._dev
         f = lambda x, shape: torch.as_tensor(np.asarray(x, np.float32).reshape(shape)).to(dev)  # noqa: E731
@@ -72,14 +80,17 @@ class SAC_Trainer_B200:
         a = f(transition_dict['actions'], (-1, self.act_dim))
         r = f(transition_dict['rewards'], (-1,)); d = f(transition_dict['dones'], (-1,))
         self._learner.update_batch(s, a, r, s2, d, None, None, self._losses)
-        self.loss = self._losses[0:1]
+        self.loss = self._losses[0::4]                           # every trainer's actor loss (one trainer: a 1-element tensor)
         if self.save_loop > 0 and self.epoch % self.save_loop == 0:
             self.save()
         return {'sum_epoch': self.epoch, 'loss': self.loss}
 
-    # ---- checkpoints in the reference's format: {'model', 'optimizer', 'epoch'} per network
-    def _state_dict(self, role):
-        flat = self._learner.get_params(role)
+    # ---- checkpoints in the reference's format: {'model', 'optimizer', 'epoch'} per network and trainer
+    def _rows(self, role):
+        """Role `role` of every trainer, (G, P), in ONE device read."""
+        return self._learner.get_params(role).reshape(self.n_trainers, -1)
+
+    def _state_dict(self, role, flat):
         o, h, a = self.w, self.hidden, self.act_dim
         if role == 0:
             shapes = [("fc1.weight", (h, o)), ("fc1.bias", (h,)), ("fc_mu.weight", (a, h)), ("fc_mu.bias", (a,)),
@@ -93,10 +104,7 @@ class SAC_Trainer_B200:
             sd[nm] = torch.from_numpy(flat[off:off + n].reshape(shp).copy()); off += n
         return sd
 
-    def _optim_dict(self, role, lr):
-        sd = self._state_dict(role)
-        m, v = self._learner.get_params(5 + role), self._learner.get_params(8 + role)
-        t = self._learner.scalars()["adam_step"]
+    def _optim_dict(self, sd, m, v, t, lr):
         state, off = {}, 0
         for i, p in enumerate(sd.values()):
             k = p.numel()
@@ -106,51 +114,74 @@ class SAC_Trainer_B200:
         return {'state': state, 'param_groups': [{'lr': lr, 'betas': (0.9, 0.999), 'eps': 1e-08, 'weight_decay': 0,
                                                   'amsgrad': False, 'params': list(range(len(sd)))}]}
 
+    def _paths(self, directory, g):
+        return [os.path.join(directory, '%s_SAC_%s.pth' % (nm, self.names[g])) for nm in self.ROLE_FILES]
+
     def save(self, directory=None):
+        """actor_ / critic_1_ / critic_2_SAC_<name>.pth per trainer (SAC_Trainer.save, :109-119).  Each of the nine vectors
+        (three networks, their two Adam moments) is read from the device once for all trainers."""
         directory = directory or self.model_dir or os.path.join(os.getcwd(), 'Mod')
         os.makedirs(directory, exist_ok=True)
         lrs = (self._learner.cfg.actor_lr, self._learner.cfg.critic_lr, self._learner.cfg.critic_lr)
-        for role, nm in enumerate(self.ROLE_FILES):
-            torch.save({'model': self._state_dict(role), 'optimizer': self._optim_dict(role, lrs[role]), 'epoch': self.epoch},
-                       os.path.join(directory, '%s_SAC_%s.pth' % (nm, self.name)))
+        p, m, v = ([self._rows(base + role) for role in range(3)] for base in (0, 5, 8))
+        sc = self._learner.scalars()
+        epoch, t = sc["epoch"], sc["adam_step"]
+        for g in range(self.n_trainers):
+            for role, path in enumerate(self._paths(directory, g)):
+                sd = self._state_dict(role, p[role][g])
+                torch.save({'model': sd, 'optimizer': self._optim_dict(sd, m[role][g], v[role][g], t, lrs[role]), 'epoch': epoch}, path)
 
     def Load_Mod(self, Mod=None):
-        """SAC_Trainer.Load_Mod (:70-106): resume actor / critics (+ their Adam moments); targets copy the critics."""
+        """SAC_Trainer.Load_Mod (:70-106): resume actor / critics (+ their Adam moments) of every trainer whose three files
+        exist; targets copy the critics.  Every file is parsed into host arrays before anything touches the device; a trainer
+        whose files do not parse is left as it is.  Each vector then moves between host and device once for all trainers."""
         directory = self.model_dir or os.path.join(os.getcwd(), 'Mod')
-        paths = [os.path.join(directory, '%s_SAC_%s.pth' % (nm, self.name)) for nm in self.ROLE_FILES]
-        if not all(os.path.exists(p) for p in paths):
+        epoch, step, staged = None, None, {}
+        for g in range(self.n_trainers):
+            paths = self._paths(directory, g)
+            if not all(os.path.exists(p) for p in paths):
+                continue
+            try:
+                mine, ep = [], 0
+                for role, p in enumerate(paths):
+                    ck = torch.load(p, weights_only=False, map_location='cpu')
+                    flat = np.concatenate([v.detach().cpu().numpy().ravel() for v in ck['model'].values()]).astype(np.float32)
+                    if flat.size != self._learner.P[role]:
+                        raise ValueError("%s holds %d parameters, the network has %d" % (p, flat.size, self._learner.P[role]))
+                    m = v = None
+                    st = ck['optimizer'].get('state', {})
+                    if st:
+                        keys = sorted(st.keys())
+                        m = np.concatenate([st[k]['exp_avg'].detach().cpu().numpy().ravel() for k in keys]).astype(np.float32)
+                        v = np.concatenate([st[k]['exp_avg_sq'].detach().cpu().numpy().ravel() for k in keys]).astype(np.float32)
+                        if m.size != flat.size or v.size != flat.size:
+                            raise ValueError("%s: optimizer state does not match the model" % p)
+                        step = int(float(st[keys[0]]['step']))
+                    ep = int(ck['epoch'])
+                    mine.append((flat, m, v))
+            except Exception as e:          # the reference prints and carries on (SAC_Trainer.py:105-106); nothing was applied
+                print(e.args)
+                continue
+            staged[g], epoch = mine, ep
+        if not staged:
             return
-        try:
-            # parse all three checkpoints into host arrays first; only a fully parsed set touches the live learner
-            epoch, step, staged = 0, 0, []
-            for role, p in enumerate(paths):
-                ck = torch.load(p, weights_only=False, map_location='cpu')
-                flat = np.concatenate([v.detach().cpu().numpy().ravel() for v in ck['model'].values()]).astype(np.float32)
-                if flat.size != self._learner.P[role]:
-                    raise ValueError("%s holds %d parameters, the network has %d" % (p, flat.size, self._learner.P[role]))
-                m = v = None
-                st = ck['optimizer'].get('state', {})
-                if st:
-                    keys = sorted(st.keys())
-                    m = np.concatenate([st[k]['exp_avg'].detach().cpu().numpy().ravel() for k in keys]).astype(np.float32)
-                    v = np.concatenate([st[k]['exp_avg_sq'].detach().cpu().numpy().ravel() for k in keys]).astype(np.float32)
-                    if m.size != flat.size or v.size != flat.size:
-                        raise ValueError("%s: optimizer state does not match the model" % p)
-                    step = int(float(st[keys[0]]['step']))
-                epoch = int(ck['epoch'])
-                staged.append((role, flat, m, v))
-        except Exception as e:              # the reference prints and carries on (SAC_Trainer.py:105-106); nothing was applied
-            print(e.args)
-            return
-        for role, flat, m, v in staged:
-            self._learner.set_params(role, flat)
-            if role > 0:
-                self._learner.set_params(role + 2, flat)
-            if m is not None:
-                self._learner.set_params(5 + role, m)
-                self._learner.set_params(8 + role, v)
-        sc = self._learner.scalars()
-        self._learner.set_scalars(sc["log_alpha"], sc["la_m"], sc["la_v"], epoch, step)
+        rows = {r: self._rows(r) for r in (0, 1, 2, 5, 6, 7, 8, 9, 10)}
+        for g, mine in staged.items():
+            for role, (flat, m, v) in enumerate(mine):
+                rows[role][g] = flat
+                if m is not None:
+                    rows[5 + role][g], rows[8 + role][g] = m, v
+        for r in (0, 1, 2, 5, 6, 7, 8, 9, 10):
+            self._learner.set_params(r, rows[r])
+        for r in (1, 2):
+            self._learner.set_params(r + 2, rows[r])
+        self._set_counters(epoch, 0 if step is None else step)
+
+    def _set_counters(self, epoch, adam_step):
+        """epoch and Adam step; every trainer keeps its own alpha (set_scalars alone would give all of them trainer 0's)."""
+        al = self._learner.alpha()
+        self._learner.set_scalars(*(float(x) for x in al[0]), epoch, adam_step)
+        self._learner.set_alpha(al)
 
     def hard_update(self):
         pass

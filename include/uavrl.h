@@ -348,6 +348,33 @@ typedef struct {
  * anything is allocated. */
 int uavrl_sac_create(const uavrl_sac_config *cfg, uavrl_sac **out);
 int uavrl_sac_destroy(uavrl_sac *s);
+/* G independent SAC trainers of the same networks and hyper-parameters in one handle (PathPlan_City.py:59-69 builds one
+ * SAC_Trainer per UAV).  uavrl_sac_create is n_trainers = 1.  The lockstep envs are split into G contiguous blocks of
+ * Ng = lockstep_envs / G: trainer g acts for envs [g Ng, (g + 1) Ng), samples only their transitions and owns its actor, both
+ * critics and both targets, their Adam moments and last gradients, its log_alpha with that scalar's Adam moments, and its
+ * losses.  epoch and adam_step are shared (the trainers step in lockstep).  Trainer g computes bit for bit what a stand-alone
+ * learner with its parameters and alpha, seed + g, replay_capacity / G and Ng envs computes.  With G > 1:
+ *   - uavrl_sac_set/get_params move [G][P] floats for every role;
+ *   - uavrl_sac_set/get_alpha move the [G][3] array {log_alpha, exp_avg, exp_avg_sq} (any G);
+ *   - uavrl_sac_get_scalars reports trainer 0's alpha triple, uavrl_sac_set_scalars writes its triple to every trainer;
+ *   - uavrl_sac_act takes n rows in G equal blocks (block g -> trainer g; eps_dev likewise);
+ *   - uavrl_sac_update_batch takes G B rows, block g for trainer g (B = rows / G; eps_next / eps_cur likewise);
+ *   - uavrl_sac_update_replay: idx_tape_dev is [G][batch_size] trainer-local logical indices; the k-th oldest transition of
+ *     trainer g is the ring's logical index (k / Ng) N + g Ng + k % Ng (uavrl_sac_replay_gather keeps whole-ring indices);
+ *   - losses_dev receives [G][4] losses; uavrl_train_stats.last_loss is the mean of the G actor losses;
+ *   - replay_capacity is the total over trainers, and an update runs once every trainer holds more than batch_size
+ *     transitions (replay size / G > batch_size);
+ *   - refused with UAVRL_ERR_INVALID before anything is allocated: n_trainers outside [1, 65535] (one grid row per trainer),
+ *     lockstep_envs % n_trainers != 0, replay_capacity / n_trainers == 0; and act / update_batch sizes that are not multiples
+ *     of G. */
+int uavrl_sac_create_trainers(const uavrl_sac_config *cfg, int32_t n_trainers, uavrl_sac **out);
+int32_t uavrl_sac_trainer_count(const uavrl_sac *s);
+/* Federated_Learning_AC (Envs/PathPlan_City.py:590-601; Is_FL = 1 with Is_AC = 1 and SAC trainers) across the G trainers.
+ * The reference copies actor 0, adds actors 1 .. G-1 into the copy, and its division by G assigns into a temporary state_dict,
+ * so nothing is divided: every trainer's actor becomes the float32 sum theta_0 + theta_1 + ... + theta_{G-1}, added left to
+ * right in trainer order (bit-reproducible).  G = 1 leaves the actor as it is.  Critics, targets, every Adam moment, alpha,
+ * epoch and adam_step are untouched.  Enqueued on `stream` (two launches), with no host synchronisation. */
+int uavrl_sac_federate_actors(uavrl_sac *s, void *stream);
 /* Shared memory (dynamic + static bytes) one block of each SAC kernel would take for cfg's networks: bytes_out[4] = target,
  * critic update, actor update, get_action.  uavrl_sac_create refuses cfg when any exceeds 227 KB (232 448 B). */
 int uavrl_sac_smem_bytes(const uavrl_sac_config *cfg, int64_t *bytes_out);
@@ -359,6 +386,9 @@ int uavrl_sac_set_params(uavrl_sac *s, int32_t role, const float *params_host);
 int uavrl_sac_get_params(uavrl_sac *s, int32_t role, float *params_host);
 int uavrl_sac_set_scalars(uavrl_sac *s, float log_alpha, float la_exp_avg, float la_exp_avg_sq, int64_t epoch, int64_t adam_step);
 int uavrl_sac_get_scalars(uavrl_sac *s, float *log_alpha, float *la_exp_avg, float *la_exp_avg_sq, int64_t *epoch, int64_t *adam_step);
+/* every trainer's {log_alpha, Adam exp_avg, Adam exp_avg_sq}: [G][3] floats */
+int uavrl_sac_set_alpha(uavrl_sac *s, const float *alpha_host);
+int uavrl_sac_get_alpha(uavrl_sac *s, float *alpha_host);
 /* SAC_Trainer.get_action (:444-448): actions_dev [n][2] = tanh(mu + sigma*eps)*bound; eps_dev [n][2] injects the
  * reparameterisation noise (NULL = Philox Box-Muller) */
 int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *eps_dev, float *actions_dev, void *stream);
