@@ -129,6 +129,32 @@ int launch_env_observe(const EnvDev &d, float *obs, cudaStream_t st)
     return 0;
 }
 
+int EnvStatsMark::begin(const EnvDev &d, cudaStream_t st, const uavrl_train_stats *out)
+{
+    if (!out) return 0;
+    UAVRL_CUDA(cudaStreamSynchronize(st));
+    UAVRL_CUDA(cudaMemcpy(c, d.stat_counts, sizeof(c), cudaMemcpyDeviceToHost));
+    UAVRL_CUDA(cudaMemcpy(&r, d.stat_reward, sizeof(r), cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int EnvStatsMark::end(const EnvDev &d, cudaStream_t st, int64_t updates, uavrl_train_stats *out) const
+{
+    if (!out) return 0;
+    UAVRL_CUDA(cudaStreamSynchronize(st));
+    unsigned long long c1[8]; double r1;
+    UAVRL_CUDA(cudaMemcpy(c1, d.stat_counts, sizeof(c1), cudaMemcpyDeviceToHost));
+    UAVRL_CUDA(cudaMemcpy(&r1, d.stat_reward, sizeof(r1), cudaMemcpyDeviceToHost));
+    out->env_steps = (int64_t)(c1[0] - c[0]);
+    out->episodes_ended = (int64_t)(c1[1] - c[1]);
+    out->collisions = (int64_t)(c1[2] - c[2]);
+    out->n_success = (int64_t)(c1[3] - c[3]);
+    out->n_lose = (int64_t)(c1[4] - c[4]);
+    out->sum_reward = r1 - r;
+    out->updates = updates;
+    return 0;
+}
+
 }  // namespace uavrl
 
 namespace uavrl {

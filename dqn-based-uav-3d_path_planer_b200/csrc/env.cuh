@@ -66,5 +66,14 @@ namespace uavrl {
 int launch_env_step(const EnvDev &d, int action_kind, const void *actions, float *obs, float *reward,
                     uint8_t *done, uint8_t *info, uint8_t *coll, uint8_t *ended, cudaStream_t st, bool pdl = false);
 int launch_env_observe(const EnvDev &d, float *obs, cudaStream_t st);
+// the env counters around a training loop (uavrl_train_run, uavrl_sac_train_run): begin() reads them, end() fills `out` with
+// what the loop added, all but last_loss, which each loop takes from its own losses.  Both synchronise `st`; nothing happens
+// when out is null.
+struct EnvStatsMark {
+    unsigned long long c[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
+    double r = 0.0;
+    int begin(const EnvDev &d, cudaStream_t st, const uavrl_train_stats *out);
+    int end(const EnvDev &d, cudaStream_t st, int64_t updates, uavrl_train_stats *out) const;
+};
 void free_pool(EnvDev &d);            // scenario.cu replaces the pool with a device-generated one
 }  // namespace uavrl

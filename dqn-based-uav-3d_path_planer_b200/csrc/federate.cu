@@ -124,7 +124,7 @@ int uavrl_learner_federate(uavrl_learner *l, const float *probe_states_dev, cons
     const int G = l->G;
     if (G == 1) return 0;
     const bool ring = probe_states_dev == nullptr;
-    if (ring && (l->mode != kReplayLockstep || l->count / G < kFedProbes))
+    if (ring && (l->replay.mode != kReplayLockstep || l->replay.count / G < kFedProbes))
         return fail(UAVRL_ERR_INVALID, "uavrl_learner_federate: every trainer needs at least 10 transitions in the ring to draw probe states from");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     const cudaStream_t st = (cudaStream_t)stream;
@@ -152,7 +152,7 @@ int uavrl_learner_federate(uavrl_learner *l, const float *probe_states_dev, cons
     if (!ok) { cudaGetLastError(); return done(fail(UAVRL_ERR_CUDA, "uavrl_learner_federate: out of device memory for the scratch")); }
     // 1. probe rows
     if (ring) {
-        BatchSrc src = replay_source(l, probe_tape_dev);
+        BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, probe_tape_dev);
         fed_probe_kernel<<<G, 256, 0, st>>>(src, in, l->cfg.seed ^ kFedSalt, l->fed_calls++, probes, probe_idx_out_dev);
         UAVRL_LAUNCHED();
     } else if (probe_idx_out_dev) {

@@ -2,6 +2,7 @@
 #pragma once
 #include "common.cuh"
 #include "per.cuh"
+#include "replay.cuh"
 
 namespace uavrl {
 
@@ -30,36 +31,6 @@ struct NetDev {
     int32_t smem_total_floats;        // whole dynamic smem carve-up for the update kernel
     LayerDev L[kMaxLayers];
 };
-
-enum ReplayMode { kReplayPaired = 0, kReplayLockstep = 1, kBatchExplicit = 2 };
-
-// where the rows of a batch come from
-struct BatchSrc {
-    int32_t mode;
-    const float *frames;              // replay observation rows [rows][in_dim]
-    const int32_t *act;               // [slots] discrete action index (DQN family)
-    const float *act2;                // [slots][2] continuous action (SAC); nullptr otherwise
-    const float *rew;                 // [slots]
-    const uint8_t *done_u8;           // [slots]  (replay)          } one of the two
-    const float *done_f32;            // [B]      (explicit batch)  }
-    const float *s2_rows;             // explicit: next-state rows [B][in]
-    const int32_t *idx_tape;          // optional injected indices [B]: logical (k-th oldest), or physical slots if idx_is_slot
-    int32_t idx_is_slot;
-    const float *is_w;                // optional per-sample importance weights (prioritised replay): loss = mean(w (Q-y)^2)
-    float *abs_err;                   // optional out: |Q - y| per sample (ReplayTree.batch_update input)
-    int64_t count, oldest;            // valid transitions, logical index of the oldest
-    int64_t cap;                      // paired: slots ; lockstep: frames in the ring
-    int32_t n_envs;                   // lockstep only: envs one trainer samples (count = frames x n_envs)
-    int32_t row_stride;               // lockstep only: envs per ring frame (0 = n_envs); > n_envs for a grouped learner
-    int32_t env_base;                 // lockstep only: first env sampled (trainer_src sets g x n_envs)
-    uint64_t key, epoch;              // Philox key / counter for sampling
-};
-
-// Philox key salts of a learner seeded with `seed`: the eps-greedy draws use seed ^ kActSalt, replay sampling seed ^ kSampleSalt.
-// Trainer g of a grouped learner draws exactly what a stand-alone learner seeded with seed + g draws.
-// Federation probe draws (federate.cu) use seed ^ kFedSalt.
-constexpr uint64_t kActSalt = 0xAC7ull, kSampleSalt = 0x5EEDull, kFedSalt = 0xFEDull;
-__host__ __device__ __forceinline__ uint64_t trainer_key(uint64_t key, uint64_t salt, int g) { return ((key ^ salt) + (uint64_t)g) ^ salt; }
 
 // ---- tensor-core (wgmma) forward path: one dense layer as a B operand [N_pad][K_pad], K-major canonical
 // layout (wgmma.cuh), hi and lo images of the 3xTF32 split
@@ -125,17 +96,7 @@ struct uavrl_learner {
     // and weight image is [G][...], trainer g acts for envs [g Ng, (g + 1) Ng) and samples only their transitions
     int32_t G = 1;
     int64_t epoch = 0, adam_t = 0;
-    // replay
-    int32_t mode = 0;
-    float *frames = nullptr;
-    int32_t *r_act = nullptr;
-    float *r_rew = nullptr;
-    uint8_t *r_done = nullptr;
-    int64_t slots = 0;                // paired: capacity ; lockstep: (ring_frames)*N
-    int64_t ring_frames = 0;          // lockstep: frames in the ring (= capacity_frames + 1)
-    int64_t head = 0;                 // paired: next slot to write ; lockstep: frame holding obs_t
-    int64_t count = 0;                // valid transitions
-    bool frame0_valid = false;
+    uavrl::ReplayStore replay;        // int32 actions
     // programmatic dependent launch chain of the lockstep loops (common.cuh)
     bool fuse_ok = false;             // the fused get_action + step kernel fits (tc_forward.cu)
     bool pdl_chain = false;
@@ -164,119 +125,6 @@ struct uavrl_learner {
 };
 
 namespace uavrl {
-
-#if defined(__CUDACC__)
-__device__ __forceinline__ uint32_t mix32(uint32_t x)
-{
-    x ^= x >> 16; x *= 0x7feb352dU; x ^= x >> 15; x *= 0x846ca68bU; x ^= x >> 16;
-    return x;
-}
-
-// i-th element of a keyed pseudo-random permutation of [0, M): 4-round Feistel on 2*h bits with
-// cycle walking.  perm(0..B-1) = B distinct uniform indices = random.sample(range(M), B)
-// (BaseClass/replay_buffer.py:49).
-__device__ __forceinline__ uint64_t perm_index(uint64_t i, uint64_t M, const uint32_t key[4])
-{
-    int bits = 1;
-    while ((1ull << bits) < M) ++bits;
-    const int h = (bits + 1) / 2;
-    const uint32_t mask = (h >= 32) ? 0xffffffffu : ((1u << h) - 1u);
-    uint64_t x = i;
-    do {
-        uint32_t Lh = (uint32_t)(x >> h) & mask, Rh = (uint32_t)x & mask;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const uint32_t f = mix32(Rh ^ key[r]) & mask;
-            const uint32_t nl = Rh;
-            Rh = Lh ^ f;
-            Lh = nl;
-        }
-        x = ((uint64_t)Lh << h) | Rh;
-    } while (x >= M);
-    return x;
-}
-
-// batch position gb -> the transition's state row, next-state row and metadata
-struct Transition { const float *s, *s2; int a; float r, d, ax, ay; };
-// the two halves of resolve_transition: (1) where the rows are -- index arithmetic only, nothing a predecessor kernel writes is
-// read (an index tape, when present, comes from a kernel that is never a programmatic-launch predecessor); (2) the
-// transition's action / reward / done, which the env step of the same iteration may just have written
-// fresh: the next-state row lies in the frame the env step of the SAME iteration writes (lockstep ring: the frame behind the
-// newest transition group) -- the only sampled row a kernel launched programmatically behind that env step must not read early
-// Trainer g's view of a batch source (grouped learner: gridDim.y = G trainers, B rows each).  Explicit batches: block g of the
-// G x B rows.  Lockstep ring: env block [g n_envs, (g + 1) n_envs), trainer g's sampling key and row g of a [G][B] index tape.
-__device__ __forceinline__ BatchSrc trainer_src(BatchSrc s, int g, int B, int in_dim)
-{
-    if (g == 0) return s;
-    const size_t r0 = (size_t)g * (size_t)B;
-    if (s.mode == kBatchExplicit) {
-        s.frames += r0 * in_dim; s.s2_rows += r0 * in_dim; s.rew += r0; s.done_f32 += r0;
-        if (s.act) s.act += r0;
-        if (s.act2) s.act2 += 2 * r0;
-        return s;
-    }
-    s.env_base = g * s.n_envs;
-    s.key = trainer_key(s.key, kSampleSalt, g);
-    if (s.idx_tape) s.idx_tape += r0;
-    return s;
-}
-
-__device__ __forceinline__ int64_t resolve_rows(const BatchSrc &src, int gb, int in_dim, const uint32_t pkey[4], const float *&s, const float *&s2,
-                                                bool *fresh = nullptr)
-{
-    if (fresh) *fresh = false;
-    if (src.mode == kBatchExplicit) {
-        s = src.frames + (size_t)gb * in_dim; s2 = src.s2_rows + (size_t)gb * in_dim;
-        return gb;
-    }
-    const uint64_t j = src.idx_tape ? (uint64_t)src.idx_tape[gb] : perm_index((uint64_t)gb, (uint64_t)src.count, pkey);
-    int64_t slot, row, row2;
-    if (src.mode == kReplayLockstep) {
-        const int64_t N = src.row_stride ? src.row_stride : src.n_envs;
-        const int64_t f = src.idx_is_slot ? (int64_t)(j / src.n_envs) : (src.oldest + (int64_t)(j / src.n_envs)) % src.cap;
-        const int64_t e = src.env_base + (int64_t)(j % src.n_envs);
-        slot = f * N + e; row = slot;
-        row2 = ((f + 1) % src.cap) * N + e;
-        if (fresh) *fresh = ((f + 1) % src.cap) == (src.oldest + src.count / src.n_envs) % src.cap;
-    } else {
-        slot = src.idx_is_slot ? (int64_t)j : (src.oldest + (int64_t)j) % src.cap; row = 2 * slot; row2 = 2 * slot + 1;
-    }
-    s = src.frames + (size_t)row * in_dim; s2 = src.frames + (size_t)row2 * in_dim;
-    return slot;
-}
-__device__ __forceinline__ void load_meta(const BatchSrc &src, int64_t slot, int &a, float &r, float &d)
-{
-    a = src.act ? src.act[slot] : 0; r = src.rew[slot];
-    d = (src.mode == kBatchExplicit) ? src.done_f32[slot] : (src.done_u8[slot] ? 1.f : 0.f);
-}
-__device__ __forceinline__ Transition resolve_transition(const BatchSrc &src, int gb, int in_dim, const uint32_t pkey[4])
-{
-    Transition t;
-    if (src.mode == kBatchExplicit) {
-        t.s = src.frames + (size_t)gb * in_dim;
-        t.s2 = src.s2_rows + (size_t)gb * in_dim;
-        t.a = src.act ? src.act[gb] : 0; t.r = src.rew[gb]; t.d = src.done_f32[gb];
-        t.ax = src.act2 ? src.act2[2 * gb] : 0.f; t.ay = src.act2 ? src.act2[2 * gb + 1] : 0.f;
-        return t;
-    }
-    const uint64_t j = src.idx_tape ? (uint64_t)src.idx_tape[gb] : perm_index((uint64_t)gb, (uint64_t)src.count, pkey);
-    int64_t slot, row, row2;
-    if (src.mode == kReplayLockstep) {
-        const int64_t N = src.row_stride ? src.row_stride : src.n_envs;
-        const int64_t f = src.idx_is_slot ? (int64_t)(j / src.n_envs) : (src.oldest + (int64_t)(j / src.n_envs)) % src.cap;
-        const int64_t e = src.env_base + (int64_t)(j % src.n_envs);
-        slot = f * N + e; row = slot;
-        row2 = ((f + 1) % src.cap) * N + e;
-    } else {
-        slot = src.idx_is_slot ? (int64_t)j : (src.oldest + (int64_t)j) % src.cap; row = 2 * slot; row2 = 2 * slot + 1;
-    }
-    t.s = src.frames + (size_t)row * in_dim;
-    t.s2 = src.frames + (size_t)row2 * in_dim;
-    t.a = src.act ? src.act[slot] : 0; t.r = src.rew[slot]; t.d = src.done_u8[slot] ? 1.f : 0.f;
-    t.ax = src.act2 ? src.act2[2 * slot] : 0.f; t.ay = src.act2 ? src.act2[2 * slot + 1] : 0.f;
-    return t;
-}
-#endif
 
 // optimiser kernel arguments (reduce_adam_kernel, learner.cu; also launched by sac.cu)
 struct AdamArgs {
@@ -366,13 +214,15 @@ __device__ __forceinline__ void adam_update_one(const AdamArgs &a, const AdamPtr
     adam_update_pre(a, q, i, g, adam_prefetch(q, i));
 }
 
-__global__ void reduce_adam_kernel(AdamArgs a, const float *__restrict__ partials, const float *__restrict__ loss_partials,
-                                   float *__restrict__ grad, float *__restrict__ local, float *__restrict__ m, float *__restrict__ v,
-                                   float *__restrict__ target, float *__restrict__ img_local, float *__restrict__ img_target,
-                                   const int32_t *__restrict__ img_map, float *__restrict__ tc_local, float *__restrict__ tc_target,
-                                   const int32_t *__restrict__ tc_hi, const int32_t *__restrict__ tc_lo, const int32_t *__restrict__ tc_hi2,
-                                   const int32_t *__restrict__ tc_lo2, float *__restrict__ loss_out);
 #endif
+// reduce_adam_kernel (learner.cu) on `grid` (y: trainer) with the pointers of q; pdl: programmatic dependent launch
+cudaError_t launch_reduce_adam(dim3 grid, cudaStream_t st, bool pdl, const AdamArgs &a, const AdamPtrs &q);
+
+// torch.optim.Adam (betas 0.9 / 0.999, eps 1e-8) at step t with learning rate lr: the fields of AdamArgs the step computes in
+// double precision on the host (bias corrections, step size)
+void adam_hyper(AdamArgs &a, float lr, int64_t t);
+// every vector and image of a learner's optimiser step (trainer 0; the kernels offset by trainer)
+AdamPtrs learner_adam_ptrs(const uavrl_learner *l, float *loss_out);
 
 // generic MLP description: trunk widths + head = `head_main` rows (+ `head_extra` rows from a second parameter block)
 int build_mlp(int in_dim, int n_hidden, const int32_t *hidden, int head_main, int head_extra, NetDev &n);
@@ -390,7 +240,6 @@ int launch_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch
                   bool apply, cudaStream_t st);
 int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, cudaStream_t st);
 int launch_update_split(uavrl_learner *l, const BatchSrc &src, int B, cudaStream_t st, cudaEvent_t *mid);
-int lockstep_begin(uavrl_learner *l, float **obs_t, float **obs_next, int32_t **act, float **rew, uint8_t **done);
+// the lockstep ring's commit plus, with prioritised replay, the priorities of the frames it makes and drops sampleable
 void lockstep_commit(uavrl_learner *l, cudaStream_t st = nullptr);
-BatchSrc replay_source(uavrl_learner *l, const int32_t *idx_tape);
 }  // namespace uavrl

@@ -181,7 +181,7 @@ int per_sample(uavrl_learner *l, int B, const double *u_tape, int32_t *slot_out,
     UAVRL_CUDA(cudaMemsetAsync(p.wmax_bits, 0, 8, st));
     int grid = (B + 7) / 8;
     if (grid > num_sms() * 4) grid = num_sms() * 4;
-    per_sample_kernel<<<grid, 256, 0, st>>>(p, B, u_tape, l->cfg.seed ^ 0x9E12ull, l->per_calls++, (double)l->count, p.beta,
+    per_sample_kernel<<<grid, 256, 0, st>>>(p, B, u_tape, l->cfg.seed ^ 0x9E12ull, l->per_calls++, (double)l->replay.count, p.beta,
                                           slot_out ? slot_out : p.idx, p.w_raw, p.wmax_bits);
     UAVRL_LAUNCHED();
     per_norm_kernel<<<(B + 255) / 256, 256, 0, st>>>(B, p.w_raw, p.wmax_bits, w_out ? w_out : p.w);
@@ -210,11 +210,11 @@ int uavrl_per_enable(uavrl_learner *l, double alpha, double beta0, double beta_i
     if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
     if (l->G > 1) return fail(UAVRL_ERR_INVALID, "prioritised replay is not available on a learner with several trainers");
     if (l->per.enabled) return fail(UAVRL_ERR_STATE, "prioritised replay is already enabled");
-    if (l->count != 0) return fail(UAVRL_ERR_STATE, "enable prioritised replay before the first transition is stored");
+    if (l->replay.count != 0) return fail(UAVRL_ERR_STATE, "enable prioritised replay before the first transition is stored");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     PerDev &p = l->per;
     memset(&p, 0, sizeof(p));
-    p.cap = l->slots;
+    p.cap = l->replay.slots;
     int64_t pow2 = 1;
     while (pow2 < p.cap) pow2 <<= 1;
     p.rot = pow2 - p.cap;
@@ -247,7 +247,7 @@ int uavrl_per_set_errors(uavrl_learner *l, int32_t n, const int32_t *slots_dev, 
 int uavrl_per_sample(uavrl_learner *l, int32_t B, const double *u_tape_dev, int32_t *slots_out_dev, float *weights_out_dev, void *stream)
 {
     if (!l || !l->per.enabled || B <= 0 || !slots_out_dev || !weights_out_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
-    if (l->count <= 0) return fail(UAVRL_ERR_STATE, "the replay is empty");
+    if (l->replay.count <= 0) return fail(UAVRL_ERR_STATE, "the replay is empty");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     return per_sample(l, B, u_tape_dev, slots_out_dev, weights_out_dev, (cudaStream_t)stream);
 }

@@ -484,26 +484,6 @@ __global__ void sac_federate_kernel(int P, int G, float *__restrict__ actor)
     for (int g = 0; g < G; ++g) actor[(size_t)g * P + i] = s;
 }
 
-// uavrl_sac_replay_gather: logical indices of the lockstep ring -> packed rows (one warp per transition)
-__global__ void sac_gather_kernel(int n, int in, BatchSrc src, const int64_t *__restrict__ idx, float *__restrict__ s, float *__restrict__ s2,
-                                  float *__restrict__ a, float *__restrict__ r, uint8_t *__restrict__ d)
-{
-    const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (i >= n) return;
-    const int64_t j = idx[i];
-    const int64_t f = (src.oldest + j / src.n_envs) % src.cap, e = j % src.n_envs;
-    const int64_t slot = f * src.n_envs + e, slot2 = ((f + 1) % src.cap) * src.n_envs + e;
-    for (int k = lane; k < in; k += 32) {
-        if (s) s[(size_t)i * in + k] = src.frames[(size_t)slot * in + k];
-        if (s2) s2[(size_t)i * in + k] = src.frames[(size_t)slot2 * in + k];
-    }
-    if (lane == 0) {
-        if (a) { a[2 * i] = src.act2[2 * slot]; a[2 * i + 1] = src.act2[2 * slot + 1]; }
-        if (r) r[i] = src.rew[slot];
-        if (d) d[i] = src.done_u8[slot];
-    }
-}
-
 }  // namespace uavrl
 
 using namespace uavrl;
@@ -563,11 +543,7 @@ struct uavrl_sac {
     int32_t td_cap = 0, parts_cap = 0, max_ctas = 4 * num_sms();
     int64_t epoch = 0, adam_t = 0;
     uint64_t calls = 0;
-    // lockstep replay ring (continuous actions)
-    float *frames = nullptr, *r_act2 = nullptr, *r_rew = nullptr;
-    uint8_t *r_done = nullptr;
-    int64_t ring_frames = 0, head = 0, count = 0;
-    bool frame0_valid = false;
+    ReplayStore replay;                                    // lockstep ring (float[2] actions); none when lockstep_envs == 0
 };
 
 static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
@@ -593,11 +569,18 @@ static void adam_args(AdamArgs &a, const NetDev &n, int nparts, float lr, int64_
 {
     memset(&a, 0, sizeof(a));
     a.P = n.P; a.nparts = nparts; a.n_loss_parts = 0; a.apply = 1; a.world = 1; a.img_floats = n.smem_w_floats;
-    const double b1 = 0.9, b2 = 0.999;
-    const double bc1 = 1.0 - pow(b1, (double)t), bc2 = 1.0 - pow(b2, (double)t);
-    a.step_size = (float)((double)lr / bc1);
-    a.beta1_c = (float)(1.0 - b1); a.beta2 = (float)b2; a.beta2_c = (float)(1.0 - b2);
-    a.eps = 1e-8f; a.bc2_sqrt = (float)sqrt(bc2); a.inv_b = 1.f;
+    adam_hyper(a, lr, t);
+    a.inv_b = 1.f;
+}
+
+// the optimiser step of network r (0 actor, 1 and 2 the critics): no target network, no tensor-core images, no loss
+static AdamPtrs sac_adam_ptrs(const uavrl_sac *s, int r)
+{
+    AdamPtrs q;
+    memset(&q, 0, sizeof(q));
+    q.partials = s->part[r]; q.loss_partials = s->lossbuf; q.grad = s->grad[r]; q.local = s->p[r]; q.m = s->m[r]; q.v = s->v[r];
+    q.img_local = s->img[r]; q.img_map = r == 0 ? s->map_a : s->map_c;
+    return q;
 }
 
 // gradient partial / stat slots per trainer for a per-trainer batch B: the tile kernels' grid.  They grow (never shrink) when a
@@ -646,9 +629,7 @@ static int sac_update_impl(uavrl_sac *s, const BatchSrc &src, int B, const float
     AdamArgs aa;
     for (int c = 1; c <= 2; ++c) {
         adam_args(aa, s->sh.critic, grid, s->cfg.critic_lr, s->adam_t);
-        reduce_adam_kernel<<<dim3((aa.P + 63) / 64, s->G), 256, 0, st>>>(aa, s->part[c], s->lossbuf, s->grad[c], s->p[c], s->m[c], s->v[c], nullptr,
-                                                                        s->img[c], nullptr, s->map_c, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                                        nullptr, nullptr);
+        UAVRL_CUDA(launch_reduce_adam(dim3((aa.P + 63) / 64, s->G), st, false, aa, sac_adam_ptrs(s, c)));
         UAVRL_LAUNCHED();
     }
     sac_fill_args(s, a, src, B, eps_cur, 2 * (uint64_t)s->epoch + 1);
@@ -656,17 +637,15 @@ static int sac_update_impl(uavrl_sac *s, const BatchSrc &src, int B, const float
     else sac_actor_kernel<false><<<grid, kNetThreads, smem_actor(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
     adam_args(aa, s->sh.actor, grid, s->cfg.actor_lr, s->adam_t);
-    reduce_adam_kernel<<<dim3((aa.P + 63) / 64, s->G), 256, 0, st>>>(aa, s->part[0], s->lossbuf, s->grad[0], s->p[0], s->m[0], s->v[0], nullptr,
-                                                                    s->img[0], nullptr, s->map_a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                                    nullptr);
+    UAVRL_CUDA(launch_reduce_adam(dim3((aa.P + 63) / 64, s->G), st, false, aa, sac_adam_ptrs(s, 0)));
     UAVRL_LAUNCHED();
     SacFinishArgs f;
     memset(&f, 0, sizeof(f));
     f.Pc = s->sh.critic.P; f.nparts = grid; f.img_floats = s->sh.critic.smem_w_floats;
     f.tau = s->cfg.tau; f.alpha_lr = s->cfg.alpha_lr; f.target_entropy = s->cfg.target_entropy;
     f.inv_n = 1.f / ((float)B * (float)kSacA); f.do_alpha = 1;
-    const double bc1 = 1.0 - pow(0.9, (double)s->adam_t), bc2 = 1.0 - pow(0.999, (double)s->adam_t);
-    f.step_size_scale = (float)((double)s->cfg.alpha_lr / bc1); f.bc2_sqrt = (float)sqrt(bc2);
+    adam_hyper(aa, s->cfg.alpha_lr, s->adam_t);                    // the alpha step's bias corrections
+    f.step_size_scale = aa.step_size; f.bc2_sqrt = aa.bc2_sqrt;
     sac_finish_kernel<<<dim3((f.Pc + 255) / 256, s->G), 256, 0, st>>>(f, s->stat, s->scal, s->p[1], s->p[2], s->p[3], s->p[4], s->img[3],
                                                                      s->img[4], s->map_c, losses_dev ? losses_dev : s->out);
     UAVRL_LAUNCHED();
@@ -703,18 +682,7 @@ static int sac_alloc(uavrl_sac *s)
     std::vector<float> init(3 * G, 0.f);
     for (size_t g = 0; g < G; ++g) init[3 * g] = logf(0.01f);          // SAC_Trainer.py:53
     UAVRL_CUDA(cudaMemcpy(s->scal, init.data(), init.size() * 4, cudaMemcpyHostToDevice));
-    if (cfg->lockstep_envs > 0) {
-        // the ring holds, for every trainer, the frames a stand-alone learner with replay_capacity / G transitions over N / G
-        // envs would keep
-        const int64_t N = cfg->lockstep_envs, Ng = N / s->G, cap_g = cfg->replay_capacity / s->G;
-        int64_t cap_frames = (cap_g + Ng - 1) / Ng;
-        if (cap_frames < 2) cap_frames = 2;
-        s->ring_frames = cap_frames + 1;
-        const size_t slots = (size_t)s->ring_frames * N;
-        if ((rc = dev_alloc(&s->frames, slots * cfg->obs_dim)) || (rc = dev_alloc(&s->r_act2, slots * kSacA)) || (rc = dev_alloc(&s->r_rew, slots)) ||
-            (rc = dev_alloc(&s->r_done, slots)))
-            return rc;
-    }
+    if (cfg->lockstep_envs > 0 && (rc = s->replay.alloc(cfg->replay_capacity, cfg->lockstep_envs, s->G, cfg->obs_dim, true))) return rc;
     if ((rc = raise_dyn_smem(sac_target_kernel<false>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<false>, smem_critic(s->sh))) ||
         (rc = raise_dyn_smem(sac_actor_kernel<false>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<false>, smem_act(s->sh))) ||
         (rc = raise_dyn_smem(sac_target_kernel<true>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true>, smem_critic(s->sh))) ||
@@ -793,8 +761,9 @@ int uavrl_sac_destroy(uavrl_sac *s)
     cudaDeviceSynchronize();
     for (int r = 0; r < 5; ++r) { cudaFree(s->p[r]); cudaFree(s->img[r]); }
     for (int r = 0; r < 3; ++r) { cudaFree(s->m[r]); cudaFree(s->v[r]); cudaFree(s->grad[r]); cudaFree(s->part[r]); }
-    void *ptrs[] = { s->map_a, s->map_c, s->stat, s->scal, s->out, s->td, s->lossbuf, s->frames, s->r_act2, s->r_rew, s->r_done };
+    void *ptrs[] = { s->map_a, s->map_c, s->stat, s->scal, s->out, s->td, s->lossbuf };
     for (void *p : ptrs) cudaFree(p);
+    s->replay.release();
     delete s;
     return 0;
 }
@@ -910,64 +879,27 @@ int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const fl
     return sac_update_impl(s, src, B / s->G, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
 }
 
-// the lockstep ring as a batch source: idx_tape (device, [G][batch_size] trainer-local logical indices, 0 = oldest) or Philox
-// sampling keyed by the epoch.  Every trainer samples its own block of N / G envs (trainer_src), count = its transitions
-static BatchSrc sac_ring_source(const uavrl_sac *s, const int32_t *idx_tape)
-{
-    const int64_t N = s->cfg.lockstep_envs, R = s->ring_frames;
-    BatchSrc src;
-    memset(&src, 0, sizeof(src));
-    src.mode = kReplayLockstep; src.frames = s->frames; src.act2 = s->r_act2; src.rew = s->r_rew; src.done_u8 = s->r_done;
-    src.count = s->count / s->G; src.cap = R; src.n_envs = (int32_t)(N / s->G); src.row_stride = (int32_t)N;
-    src.oldest = ((s->head - s->count / N) % R + R) % R;
-    src.key = s->cfg.seed ^ kSampleSalt; src.epoch = (uint64_t)s->epoch;
-    src.idx_tape = idx_tape;
-    return src;
-}
-
-int64_t uavrl_sac_replay_size(const uavrl_sac *s) { return s ? s->count : 0; }
+int64_t uavrl_sac_replay_size(const uavrl_sac *s) { return s ? s->replay.count : 0; }
 
 int uavrl_sac_replay_gather(uavrl_sac *s, int32_t n, const int64_t *idx, float *s_host, float *a_host, float *r_host, float *s2_host,
                             uint8_t *d_host)
 {
     if (!s || n <= 0 || !idx) return fail(UAVRL_ERR_INVALID, "bad argument");
-    if (!s->frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
-    for (int i = 0; i < n; ++i)
-        if (idx[i] < 0 || idx[i] >= s->count) return fail(UAVRL_ERR_INVALID, "logical index out of range");
+    if (!s->replay.frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
-    UAVRL_CUDA(cudaDeviceSynchronize());
-    BatchSrc src = sac_ring_source(s, nullptr);
-    src.n_envs = src.row_stride;                                // whole-ring logical indices, whatever the trainer count
-    const size_t in = (size_t)s->cfg.obs_dim;
-    int64_t *d_idx = nullptr; float *d_s = nullptr, *d_s2 = nullptr, *d_a = nullptr, *d_r = nullptr; uint8_t *d_d = nullptr;
-    struct Free { void **p[6]; ~Free() { for (auto q : p) if (*q) cudaFree(*q); } } guard{ { (void **)&d_idx, (void **)&d_s, (void **)&d_s2,
-                                                                                             (void **)&d_a, (void **)&d_r, (void **)&d_d } };
-    UAVRL_CUDA(cudaMalloc((void **)&d_idx, (size_t)n * 8));
-    UAVRL_CUDA(cudaMemcpy(d_idx, idx, (size_t)n * 8, cudaMemcpyHostToDevice));
-    if (s_host) UAVRL_CUDA(cudaMalloc((void **)&d_s, (size_t)n * in * 4));
-    if (s2_host) UAVRL_CUDA(cudaMalloc((void **)&d_s2, (size_t)n * in * 4));
-    if (a_host) UAVRL_CUDA(cudaMalloc((void **)&d_a, (size_t)n * kSacA * 4));
-    if (r_host) UAVRL_CUDA(cudaMalloc((void **)&d_r, (size_t)n * 4));
-    if (d_host) UAVRL_CUDA(cudaMalloc((void **)&d_d, (size_t)n));
-    sac_gather_kernel<<<(n + 7) / 8, 256>>>(n, (int)in, src, d_idx, d_s, d_s2, d_a, d_r, d_d);
-    UAVRL_CUDA(cudaGetLastError());
-    if (s_host) UAVRL_CUDA(cudaMemcpy(s_host, d_s, (size_t)n * in * 4, cudaMemcpyDeviceToHost));
-    if (s2_host) UAVRL_CUDA(cudaMemcpy(s2_host, d_s2, (size_t)n * in * 4, cudaMemcpyDeviceToHost));
-    if (a_host) UAVRL_CUDA(cudaMemcpy(a_host, d_a, (size_t)n * kSacA * 4, cudaMemcpyDeviceToHost));
-    if (r_host) UAVRL_CUDA(cudaMemcpy(r_host, d_r, (size_t)n * 4, cudaMemcpyDeviceToHost));
-    if (d_host) UAVRL_CUDA(cudaMemcpy(d_host, d_d, (size_t)n, cudaMemcpyDeviceToHost));
-    return 0;
+    return s->replay.gather(n, idx, s_host, nullptr, a_host, r_host, s2_host, d_host);
 }
 
 int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const float *eps_next_dev, const float *eps_cur_dev, float *losses_dev,
                             void *stream)
 {
     if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
-    if (!s->frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
+    if (!s->replay.frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;                                             // SAC_Trainer.py:320
-    if (s->count / s->G <= s->cfg.batch_size) return 0;        // PathPlan_City.py:383: nothing sampled yet (per trainer)
-    return sac_update_impl(s, sac_ring_source(s, idx_tape_dev), s->cfg.batch_size, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
+    if (s->replay.count / s->G <= s->cfg.batch_size) return 0; // PathPlan_City.py:383: nothing sampled yet (per trainer)
+    return sac_update_impl(s, s->replay.source(s->cfg.seed, s->epoch, idx_tape_dev), s->cfg.batch_size, eps_next_dev, eps_cur_dev, losses_dev,
+                           (cudaStream_t)stream);
 }
 
 int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
@@ -985,47 +917,33 @@ int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
 int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t do_update, uavrl_train_stats *stats_host, void *stream)
 {
     if (!env || !s || n_iters < 0) return fail(UAVRL_ERR_INVALID, "bad argument");
-    if (s->cfg.lockstep_envs != env->d.n || !s->frames) return fail(UAVRL_ERR_INVALID, "sac.lockstep_envs must equal env.n_envs");
+    if (s->cfg.lockstep_envs != env->d.n || !s->replay.frames) return fail(UAVRL_ERR_INVALID, "sac.lockstep_envs must equal env.n_envs");
     if (!env->reset_done) return fail(UAVRL_ERR_STATE, "uavrl_sac_train_run before uavrl_env_reset");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
     cudaStream_t st = (cudaStream_t)stream;
-    const int64_t N = env->d.n, in = s->cfg.obs_dim, R = s->ring_frames;
-    unsigned long long c0[8] = { 0 }; double r0 = 0.0;
-    if (stats_host) {
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        UAVRL_CUDA(cudaMemcpy(c0, env->d.stat_counts, sizeof(c0), cudaMemcpyDeviceToHost));
-        UAVRL_CUDA(cudaMemcpy(&r0, env->d.stat_reward, sizeof(r0), cudaMemcpyDeviceToHost));
-    }
+    ReplayStore &rs = s->replay;
+    EnvStatsMark mark;
     int rc; int64_t updates = 0;
+    if ((rc = mark.begin(env->d, st, stats_host))) return rc;
     for (int it = 0; it < n_iters; ++it) {
-        const int64_t f = s->head, fn = (s->head + 1) % R;
-        float *obs_t = s->frames + f * N * in, *obs_next = s->frames + fn * N * in, *act = s->r_act2 + f * N * kSacA, *rew = s->r_rew + f * N;
-        uint8_t *done = s->r_done + f * N;
-        if (!s->frame0_valid) { if ((rc = launch_env_observe(env->d, obs_t, st))) return rc; s->frame0_valid = true; }
-        if ((rc = uavrl_sac_act(s, obs_t, (int32_t)N, nullptr, act, st))) return rc;
-        if ((rc = launch_env_step(env->d, UAVRL_ACT_CONT_F32X2, act, obs_next, rew, done, nullptr, nullptr, nullptr, st))) return rc;
-        s->head = fn;
-        const int64_t maxc = (R - 1) * N;
-        s->count = s->count + N > maxc ? maxc : s->count + N;
+        const ReplayStore::Iteration io = rs.begin();
+        if (!rs.frame0_valid) { if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc; rs.frame0_valid = true; }
+        if ((rc = uavrl_sac_act(s, io.obs_t, (int32_t)rs.N, nullptr, io.act2, st))) return rc;
+        if ((rc = launch_env_step(env->d, UAVRL_ACT_CONT_F32X2, io.act2, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st))) return rc;
+        rs.commit();
         if (do_update) {
             s->epoch += 1;
-            if (s->count / s->G <= s->cfg.batch_size) continue;     // per trainer
-            if ((rc = sac_update_impl(s, sac_ring_source(s, nullptr), s->cfg.batch_size, nullptr, nullptr, nullptr, st))) return rc;
+            if (rs.count / s->G <= s->cfg.batch_size) continue;     // per trainer
+            if ((rc = sac_update_impl(s, rs.source(s->cfg.seed, s->epoch, nullptr), s->cfg.batch_size, nullptr, nullptr, nullptr, st))) return rc;
             ++updates;
         }
     }
+    if ((rc = mark.end(env->d, st, updates, stats_host))) return rc;
     if (stats_host) {
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        unsigned long long c1[8]; double r1;
-        UAVRL_CUDA(cudaMemcpy(c1, env->d.stat_counts, sizeof(c1), cudaMemcpyDeviceToHost));
-        UAVRL_CUDA(cudaMemcpy(&r1, env->d.stat_reward, sizeof(r1), cudaMemcpyDeviceToHost));
         std::vector<float> o((size_t)s->G * 4);                 // [G][4]; last_loss = the mean actor loss over trainers
         UAVRL_CUDA(cudaMemcpy(o.data(), s->out, o.size() * sizeof(float), cudaMemcpyDeviceToHost));
         double lsum = 0.0;
         for (int g = 0; g < s->G; ++g) lsum += o[4 * (size_t)g];
-        stats_host->env_steps = (int64_t)(c1[0] - c0[0]); stats_host->episodes_ended = (int64_t)(c1[1] - c0[1]);
-        stats_host->collisions = (int64_t)(c1[2] - c0[2]); stats_host->n_success = (int64_t)(c1[3] - c0[3]);
-        stats_host->n_lose = (int64_t)(c1[4] - c0[4]); stats_host->sum_reward = r1 - r0; stats_host->updates = updates;
         stats_host->last_loss = (float)(lsum / (double)s->G);
     }
     return 0;

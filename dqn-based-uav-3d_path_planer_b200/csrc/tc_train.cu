@@ -857,11 +857,7 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
         if ((uint32_t)l->dw_bar_total == 0u) l->dw_bar_total += 1;     // tag 0 = "never written"
         d.fuse_adam = 1; d.part64 = l->dw_bar; d.ll_epoch = (uint32_t)l->dw_bar_total;
         d.adam = *adam; d.adam.nparts = d.n_slices; d.adam.n_loss_parts = grid;
-        AdamPtrs &q = d.ptrs;
-        q.partials = l->partials; q.loss_partials = l->loss_partials; q.grad = l->grad; q.local = l->local; q.m = l->m; q.v = l->v;
-        q.target = l->target; q.img_local = l->img_local; q.img_target = l->img_target; q.img_map = l->img_map;
-        q.tc_local = (float *)l->tc_img_local; q.tc_target = (float *)l->tc_img_target; q.tc_hi = l->tc_hi_map; q.tc_lo = l->tc_lo_map;
-        q.tc_hi2 = l->tc_hi2_map; q.tc_lo2 = l->tc_lo2_map; q.loss_out = loss_out;
+        d.ptrs = learner_adam_ptrs(l, loss_out);
     }
     if (trace_on) d.trace = tr;
     UAVRL_CUDA(launch_kernel(fuse ? tc_dw_kernel<true> : tc_dw_kernel<false>, dim3(dw_grid, l->G), dim3(kTcThreads), dw_smem_bytes(tc), st,

@@ -16,7 +16,7 @@ extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters
                                int32_t do_update, uavrl_train_stats *stats_host, void *stream)
 {
     if (!env || !l || n_iters < 0) return fail(UAVRL_ERR_INVALID, "bad argument");
-    if (l->mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n)
+    if (l->replay.mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n)
         return fail(UAVRL_ERR_INVALID, "learner.lockstep_envs must equal env.n_envs");
     if (l->net.in_dim != kObsDim) return fail(UAVRL_ERR_INVALID, "learner.in_dim must be 100 (the UAV observation)");
     if (!env->reset_done) return fail(UAVRL_ERR_STATE, "uavrl_train_run before uavrl_env_reset");
@@ -24,30 +24,24 @@ extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    unsigned long long c0[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    double r0 = 0.0;
-    if (stats_host) {
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        UAVRL_CUDA(cudaMemcpy(c0, env->d.stat_counts, sizeof(c0), cudaMemcpyDeviceToHost));
-        UAVRL_CUDA(cudaMemcpy(&r0, env->d.stat_reward, sizeof(r0), cudaMemcpyDeviceToHost));
-    }
+    EnvStatsMark mark;
+    if ((rc = mark.begin(env->d, st, stats_host))) return rc;
     int64_t updates = 0;
     l->pdl_chain = true; l->pdl_prev = kPdlNone;          // the first kernel of the loop is launched plainly
     struct ChainOff { uavrl_learner *l; ~ChainOff() { l->pdl_chain = false; l->pdl_prev = kPdlNone; } } chain_off{ l };
     for (int it = 0; it < n_iters; ++it) {
-        float *obs_t, *obs_next, *rew; int32_t *act; uint8_t *done;
-        lockstep_begin(l, &obs_t, &obs_next, &act, &rew, &done);
-        if (!l->frame0_valid) {                          // very first iteration: materialise obs_0
-            if ((rc = launch_env_observe(env->d, obs_t, st))) return rc;
-            l->frame0_valid = true;
+        const ReplayStore::Iteration io = l->replay.begin();
+        if (!l->replay.frame0_valid) {                   // very first iteration: materialise obs_0
+            if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc;
+            l->replay.frame0_valid = true;
         }
         // Choose_Action2 -> Trainer.get_action (PathPlan_City.py:338-346), then Move_Agent + replay add (:371-382):
         // reward/done land in the ring slots.  One fused kernel when the tensor-core path is on.
-        rc = launch_act_env(l, env->d, obs_t, eps, act, obs_next, rew, done, st);
+        rc = launch_act_env(l, env->d, io.obs_t, eps, io.act, io.obs_next, io.rew, io.done, st);
         if (rc < 0) return rc;
         if (rc == 1) {
-            if ((rc = launch_act(l, obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, act, nullptr, st))) return rc;
-            if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, act, obs_next, rew, done, nullptr, nullptr, nullptr, st,
+            if ((rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
+            if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
                                       l->pdl_prev == kPdlAct && g_pdl.load()))) return rc;
             l->pdl_prev = kPdlEnv;
         }
@@ -55,31 +49,20 @@ extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters
         if (do_update) {
             for (int u = 0; u < updates_per_iter; ++u) {  // PathPlan_City.update -> Trainer.update (:757-776)
                 l->epoch += 1;
-                if (l->count / l->G <= l->cfg.batch_size) continue;      // per trainer
-                BatchSrc src = replay_source(l, nullptr);
+                if (l->replay.count / l->G <= l->cfg.batch_size) continue;   // per trainer
+                BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, nullptr);
                 if ((rc = launch_update(l, src, l->cfg.batch_size, l->cfg.batch_size, l->loss_dev, true, st))) return rc;
                 ++updates;
             }
         }
     }
+    if ((rc = mark.end(env->d, st, updates, stats_host))) return rc;
     if (stats_host) {
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        unsigned long long c1[8]; double r1; float loss;
-        UAVRL_CUDA(cudaMemcpy(c1, env->d.stat_counts, sizeof(c1), cudaMemcpyDeviceToHost));
-        UAVRL_CUDA(cudaMemcpy(&r1, env->d.stat_reward, sizeof(r1), cudaMemcpyDeviceToHost));
         std::vector<float> losses((size_t)l->G);                // grouped learner: the mean over trainers
         UAVRL_CUDA(cudaMemcpy(losses.data(), l->loss_dev, losses.size() * sizeof(float), cudaMemcpyDeviceToHost));
         double lsum = 0.0;
         for (float x : losses) lsum += x;
-        loss = (float)(lsum / (double)l->G);
-        stats_host->env_steps = (int64_t)(c1[0] - c0[0]);
-        stats_host->episodes_ended = (int64_t)(c1[1] - c0[1]);
-        stats_host->collisions = (int64_t)(c1[2] - c0[2]);
-        stats_host->n_success = (int64_t)(c1[3] - c0[3]);
-        stats_host->n_lose = (int64_t)(c1[4] - c0[4]);
-        stats_host->sum_reward = r1 - r0;
-        stats_host->updates = updates;
-        stats_host->last_loss = loss;
+        stats_host->last_loss = (float)(lsum / (double)l->G);
     }
     return 0;
 }
@@ -88,7 +71,7 @@ extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_it
 {
     if (!env || !l || n_iters < 0 || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     if (l->G > 1) return fail(UAVRL_ERR_INVALID, "uavrl_train_run_dp is not available on a learner with several trainers");
-    if (l->mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n)
+    if (l->replay.mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n)
         return fail(UAVRL_ERR_INVALID, "learner.lockstep_envs must equal env.n_envs");
     if (!l->comm_ready) return fail(UAVRL_ERR_STATE, "uavrl_train_run_dp before uavrl_learner_comm_connect");
     if (!env->reset_done) return fail(UAVRL_ERR_STATE, "uavrl_train_run_dp before uavrl_env_reset");
@@ -98,25 +81,24 @@ extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_it
     l->pdl_chain = true; l->pdl_prev = kPdlNone;
     struct ChainOff { uavrl_learner *l; ~ChainOff() { l->pdl_chain = false; l->pdl_prev = kPdlNone; } } chain_off{ l };
     for (int it = 0; it < n_iters; ++it) {
-        float *obs_t, *obs_next, *rew; int32_t *act; uint8_t *done;
-        lockstep_begin(l, &obs_t, &obs_next, &act, &rew, &done);
-        if (!l->frame0_valid) {
-            if ((rc = launch_env_observe(env->d, obs_t, st))) return rc;
-            l->frame0_valid = true;
+        const ReplayStore::Iteration io = l->replay.begin();
+        if (!l->replay.frame0_valid) {
+            if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc;
+            l->replay.frame0_valid = true;
         }
-        rc = launch_act_env(l, env->d, obs_t, eps, act, obs_next, rew, done, st);
+        rc = launch_act_env(l, env->d, io.obs_t, eps, io.act, io.obs_next, io.rew, io.done, st);
         if (rc < 0) return rc;
         if (rc == 1) {
-            if ((rc = launch_act(l, obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, act, nullptr, st))) return rc;
-            if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, act, obs_next, rew, done, nullptr, nullptr, nullptr, st,
+            if ((rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
+            if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
                                       l->pdl_prev == kPdlAct && g_pdl.load()))) return rc;
             l->pdl_prev = kPdlEnv;
         }
         lockstep_commit(l, st);
         l->epoch += 1;
         // every rank must take part in every all-reduce: the caller warms the replay up first
-        if (l->count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions (warm up with uavrl_train_run first)");
-        BatchSrc src = replay_source(l, nullptr);
+        if (l->replay.count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions (warm up with uavrl_train_run first)");
+        BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, nullptr);
         if ((rc = launch_update_dp(l, src, l->cfg.batch_size, global_batch, l->loss_dev, st))) return rc;
     }
     return 0;
@@ -125,7 +107,7 @@ extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_it
 extern "C" int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, float *ms_out, void *stream)
 {
     if (!env || !l || n_iters <= 0 || !ms_out) return fail(UAVRL_ERR_INVALID, "bad argument");
-    if (l->mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n || !env->reset_done || !l->frame0_valid)
+    if (l->replay.mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n || !env->reset_done || !l->replay.frame0_valid)
         return fail(UAVRL_ERR_STATE, "uavrl_train_profile needs a warmed-up lockstep env/learner pair");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -134,21 +116,20 @@ extern "C" int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_i
     for (auto &e : ev) UAVRL_CUDA(cudaEventCreate(&e));
     int rc;
     for (int it = 0; it < n_iters; ++it) {
-        float *obs_t, *obs_next, *rew; int32_t *act; uint8_t *done;
-        lockstep_begin(l, &obs_t, &obs_next, &act, &rew, &done);
+        const ReplayStore::Iteration io = l->replay.begin();
         cudaEvent_t *e = &ev[(size_t)it * NE];
         UAVRL_CUDA(cudaEventRecord(e[0], st));
-        rc = launch_act_env(l, env->d, obs_t, eps, act, obs_next, rew, done, st);      // fused: slot 0 = act + step, slot 1 = 0
+        rc = launch_act_env(l, env->d, io.obs_t, eps, io.act, io.obs_next, io.rew, io.done, st);      // fused: slot 0 = act + step, slot 1 = 0
         if (rc < 0) return rc;
         const bool fused = (rc == 0);
-        if (!fused && (rc = launch_act(l, obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, act, nullptr, st))) return rc;
+        if (!fused && (rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
         UAVRL_CUDA(cudaEventRecord(e[1], st));
-        if (!fused && (rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, act, obs_next, rew, done, nullptr, nullptr, nullptr, st))) return rc;
+        if (!fused && (rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st))) return rc;
         UAVRL_CUDA(cudaEventRecord(e[2], st));
         lockstep_commit(l, st);
         l->epoch += 1;
-        if (l->count / l->G <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay not warmed up");
-        BatchSrc src = replay_source(l, nullptr);
+        if (l->replay.count / l->G <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay not warmed up");
+        BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, nullptr);
         if ((rc = launch_update_split(l, src, l->cfg.batch_size, st, &e[3]))) return rc;   // records e[3], e[4], e[5]
         UAVRL_CUDA(cudaEventRecord(e[6], st));
     }
