@@ -88,6 +88,7 @@ SIGNATURES = {
     "uavrl_env_get_path": (C.c_int, [VP, C.c_int32, C.c_int32, C.c_int32, VP, VP]),
     "uavrl_env_get_subgoals": (C.c_int, [VP, VP]),
     "uavrl_per_enable": (C.c_int, [VP, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double]),
+    "uavrl_per_enable_trainers": (C.c_int, [VP, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double]),
     "uavrl_per_sample": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP]),
     "uavrl_per_set_errors": (C.c_int, [VP, C.c_int32, VP, VP, C.c_int32, VP]),
     "uavrl_per_set_priorities": (C.c_int, [VP, C.c_int32, VP, VP, VP]),

@@ -728,7 +728,8 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
     BatchSrc src = src_in;
     const bool per_batch = l->per.enabled && src.mode != kBatchExplicit && !src.idx_tape;
     if (per_batch) {
-        // ReplayTree.sample2 -> slots + importance weights; |Q - y| comes back for batch_update (end of this function)
+        // ReplayTree.sample2 -> slots + importance weights; |Q - y| comes back for batch_update (end of this function).
+        // Grouped learner: [G][B] trainer-local slots, weights and errors; trainer_src hands trainer g its row of each
         int rc = per_sample(l, B, nullptr, nullptr, nullptr, st);
         if (rc) return rc;
         src.idx_tape = l->per.idx; src.idx_is_slot = 1; src.is_w = l->per.w; src.abs_err = l->per.abs_err;
@@ -898,9 +899,10 @@ void lockstep_commit(uavrl_learner *l, cudaStream_t st)
 {
     if (l->per.enabled) {
         // the frame just completed becomes sampleable with the priority of an error-less push; the frame that now
-        // receives the next observations (the ring's oldest) stops being a transition
-        const int64_t N = l->replay.N;
-        per_fill_range(l, l->replay.head * N, 2 * N, per_new_priority(l->per), st, N, 0.0);
+        // receives the next observations (the ring's oldest) stops being a transition.  Trainer-local slots: every trainer's
+        // tree gets the same Ng + Ng slots of its own env block
+        const int64_t Ng = l->replay.N / l->G;
+        per_fill_range(l, l->replay.head * Ng, 2 * Ng, per_new_priority(l->per), st, Ng, 0.0);
         l->pdl_prev = kPdlNone;
     }
     l->replay.commit();
@@ -1233,9 +1235,10 @@ int uavrl_learner_lockstep_restart(uavrl_learner *l)
     if (l->per.enabled) {
         UAVRL_CUDA(cudaSetDevice(l->cfg.device));
         UAVRL_CUDA(cudaDeviceSynchronize());
-        UAVRL_CUDA(cudaMemset(l->per.leaf, 0, (size_t)l->per.cap * 8));
-        UAVRL_CUDA(cudaMemset(l->per.l1, 0, (size_t)l->per.n1 * 8));
-        UAVRL_CUDA(cudaMemset(l->per.l2, 0, (size_t)l->per.n2 * 8));
+        const size_t G = (size_t)l->per.G;                     // every trainer's tree
+        UAVRL_CUDA(cudaMemset(l->per.leaf, 0, G * l->per.cap * 8));
+        UAVRL_CUDA(cudaMemset(l->per.l1, 0, G * l->per.n1 * 8));
+        UAVRL_CUDA(cudaMemset(l->per.l2, 0, G * l->per.n2 * 8));
     }
     return 0;
 }

@@ -29,20 +29,22 @@ __device__ __forceinline__ double warp_scan_incl(double x, int lane)
 // ---- leaves
 // mode 0: explicit priorities; 1: ReplayTree.push (:152-154)  p = (|e| + eps)^alpha ; 2: batch_update (:216-221) with the clip.
 // The reference computes both in float32 (the errors arrive as float32 tensors / arrays).
+// Trainer blockIdx.y: its tree, and row g of [G][n] slots / priorities / errors (a range fill covers the same slots of every tree).
 __global__ void per_leaf_kernel(PerDev p, int n, const int32_t *__restrict__ slots, int64_t first, const double *__restrict__ prio,
                                 const float *__restrict__ err, int mode, double fill, int n_first, double fill_rest)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int64_t s = slots ? (int64_t)slots[i] : (first + i) % p.cap;
+    const size_t r = (size_t)blockIdx.y * (size_t)n + (size_t)i;
+    const int64_t s = slots ? (int64_t)slots[r] : (first + i) % p.cap;
     double v;
-    if (mode == 0) v = prio ? prio[i] : (i < n_first ? fill : fill_rest);
+    if (mode == 0) v = prio ? prio[r] : (i < n_first ? fill : fill_rest);
     else {
-        float e = fabsf(err[i]) + (float)p.eps;
+        float e = fabsf(err[r]) + (float)p.eps;
         if (mode == 2) e = fminf(e, (float)p.err_upper);
         v = (double)powf(e, (float)p.alpha);
     }
-    p.leaf[s] = v;
+    p.leaf[(size_t)blockIdx.y * (size_t)p.cap + s] = v;
 }
 
 // one warp per touched slot: recompute the l1 entry (level 1) or the l2 entry (level 2) that covers it
@@ -50,22 +52,27 @@ __global__ void per_level_kernel(PerDev p, int n, const int32_t *__restrict__ sl
 {
     const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (w >= n) return;
-    const int64_t s = slots ? (int64_t)slots[w] : (first + w) % p.cap;
+    const size_t t = blockIdx.y;                                  // trainer: its tree and row t of [G][n] slots
+    const double *leaf = p.leaf + t * (size_t)p.cap;
+    double *l1 = p.l1 + t * (size_t)p.n1, *l2 = p.l2 + t * (size_t)p.n2;
+    const int64_t s = slots ? (int64_t)slots[t * (size_t)n + w] : (first + w) % p.cap;
     const int64_t pos = per_pos(p, s);
     if (level == 1) {
         const int64_t g = pos >> 5, j = (g << 5) + lane;
-        const double x = j < p.cap ? p.leaf[per_slot(p, j)] : 0.0;
+        const double x = j < p.cap ? leaf[per_slot(p, j)] : 0.0;
         const double sum = warp_sum(x);
-        if (lane == 0) p.l1[g] = sum;
+        if (lane == 0) l1[g] = sum;
     } else {
         const int64_t b = pos >> 10, j = (b << 5) + lane;
-        const double x = j < p.n1 ? p.l1[j] : 0.0;
+        const double x = j < p.n1 ? l1[j] : 0.0;
         const double sum = warp_sum(x);
-        if (lane == 0) p.l2[b] = sum;
+        if (lane == 0) l2[b] = sum;
     }
 }
 
 // ---- ReplayTree.sample2 (:186-213)
+// Trainer blockIdx.y samples B from its own tree with its own key (trainer_key: what a stand-alone learner seeded with seed + g
+// draws), into row g of the [G][B] outputs, and normalises by its own maximum weight (wmax_bits[g]).
 __global__ void __launch_bounds__(256) per_sample_kernel(PerDev p, int B, const double *__restrict__ u_tape, uint64_t key, uint64_t call,
                                                          double n_entries, double beta, int32_t *__restrict__ slot_out,
                                                          double *__restrict__ w_raw, unsigned long long *wmax_bits)
@@ -73,6 +80,11 @@ __global__ void __launch_bounds__(256) per_sample_kernel(PerDev p, int B, const 
     __shared__ double pre[kPerMaxL2];       // inclusive prefix of l2
     __shared__ double wsum[8];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const size_t t = blockIdx.y, r0 = t * (size_t)B;
+    p.leaf += t * (size_t)p.cap; p.l1 += t * (size_t)p.n1; p.l2 += t * (size_t)p.n2;
+    if (u_tape) u_tape += r0;
+    slot_out += r0; w_raw += r0; wmax_bits += t;
+    key = trainer_key(key, kPerSalt, (int)t);
     // inclusive scan of l2 (n2 <= 4096): 16 consecutive entries per thread, then a scan of the 256 thread totals
     constexpr int PER_T = kPerMaxL2 / 256;
     double loc[PER_T], run = 0.0;
@@ -134,13 +146,14 @@ __global__ void __launch_bounds__(256) per_sample_kernel(PerDev p, int B, const 
 __global__ void per_norm_kernel(int B, const double *__restrict__ w_raw, const unsigned long long *wmax_bits, float *__restrict__ w)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < B) w[i] = (float)(w_raw[i] / __longlong_as_double((long long)*wmax_bits));      // :210
+    const size_t r = (size_t)blockIdx.y * (size_t)B + (size_t)i;  // row blockIdx.y: that trainer's own maximum
+    if (i < B) w[r] = (float)(w_raw[r] / __longlong_as_double((long long)wmax_bits[blockIdx.y]));      // :210
 }
 
 static int per_refresh(uavrl_learner *l, int n, const int32_t *slots, int64_t first, cudaStream_t st)
 {
     const PerDev &p = l->per;
-    const int blocks = (int)(((int64_t)n * 32 + 255) / 256);
+    const dim3 blocks((unsigned)(((int64_t)n * 32 + 255) / 256), (unsigned)p.G);
     per_level_kernel<<<blocks, 256, 0, st>>>(p, n, slots, first, 1);
     UAVRL_LAUNCHED();
     per_level_kernel<<<blocks, 256, 0, st>>>(p, n, slots, first, 2);
@@ -152,15 +165,17 @@ static int per_refresh(uavrl_learner *l, int n, const int32_t *slots, int64_t fi
 int per_fill_range(uavrl_learner *l, int64_t first_slot, int64_t n, double value, cudaStream_t st, int64_t n_first, double value_rest)
 {
     if (n <= 0) return 0;
-    per_leaf_kernel<<<(int)((n + 255) / 256), 256, 0, st>>>(l->per, (int)n, nullptr, first_slot % l->per.cap, nullptr, nullptr, 0, value,
-                                                          (int)(n_first < 0 ? n : n_first), value_rest);
+    per_leaf_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)l->per.G), 256, 0, st>>>(l->per, (int)n, nullptr, first_slot % l->per.cap,
+                                                                                        nullptr, nullptr, 0, value,
+                                                                                        (int)(n_first < 0 ? n : n_first), value_rest);
     UAVRL_LAUNCHED();
     return per_refresh(l, (int)n, nullptr, first_slot % l->per.cap, st);
 }
 
 int per_set(uavrl_learner *l, int n, const int32_t *slots, const double *prio, const float *abs_err, int clip, cudaStream_t st)
 {
-    per_leaf_kernel<<<(n + 255) / 256, 256, 0, st>>>(l->per, n, slots, 0, prio, abs_err, prio ? 0 : (clip ? 2 : 1), 0.0, n, 0.0);
+    per_leaf_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)l->per.G), 256, 0, st>>>(l->per, n, slots, 0, prio, abs_err,
+                                                                                        prio ? 0 : (clip ? 2 : 1), 0.0, n, 0.0);
     UAVRL_LAUNCHED();
     return per_refresh(l, n, slots, 0, st);
 }
@@ -168,23 +183,25 @@ int per_set(uavrl_learner *l, int n, const int32_t *slots, const double *prio, c
 int per_sample(uavrl_learner *l, int B, const double *u_tape, int32_t *slot_out, float *w_out, cudaStream_t st)
 {
     PerDev &p = l->per;
+    const size_t G = (size_t)p.G;
     if (B > p.scratch_cap) {
         UAVRL_CUDA(cudaStreamSynchronize(st));
         cudaFree(p.idx); cudaFree(p.w); cudaFree(p.abs_err); cudaFree(p.w_raw);
-        UAVRL_CUDA(cudaMalloc((void **)&p.idx, (size_t)B * 4));
-        UAVRL_CUDA(cudaMalloc((void **)&p.w, (size_t)B * 4));
-        UAVRL_CUDA(cudaMalloc((void **)&p.abs_err, (size_t)B * 4));
-        UAVRL_CUDA(cudaMalloc((void **)&p.w_raw, (size_t)B * 8));
+        UAVRL_CUDA(cudaMalloc((void **)&p.idx, G * B * 4));
+        UAVRL_CUDA(cudaMalloc((void **)&p.w, G * B * 4));
+        UAVRL_CUDA(cudaMalloc((void **)&p.abs_err, G * B * 4));
+        UAVRL_CUDA(cudaMalloc((void **)&p.w_raw, G * B * 8));
         p.scratch_cap = B;
     }
     p.beta = fmin(1.0, p.beta + p.beta_inc);                  // :195
-    UAVRL_CUDA(cudaMemsetAsync(p.wmax_bits, 0, 8, st));
-    int grid = (B + 7) / 8;
+    UAVRL_CUDA(cudaMemsetAsync(p.wmax_bits, 0, G * 8, st));
+    int grid = (B + 7) / 8;                                   // per trainer, as a stand-alone learner picks it
     if (grid > num_sms() * 4) grid = num_sms() * 4;
-    per_sample_kernel<<<grid, 256, 0, st>>>(p, B, u_tape, l->cfg.seed ^ 0x9E12ull, l->per_calls++, (double)l->replay.count, p.beta,
-                                          slot_out ? slot_out : p.idx, p.w_raw, p.wmax_bits);
+    // n_entries: the trainer's own transition count (every trainer holds the same number)
+    per_sample_kernel<<<dim3(grid, p.G), 256, 0, st>>>(p, B, u_tape, l->cfg.seed ^ kPerSalt, l->per_calls++, (double)(l->replay.count / l->G),
+                                                       p.beta, slot_out ? slot_out : p.idx, p.w_raw, p.wmax_bits);
     UAVRL_LAUNCHED();
-    per_norm_kernel<<<(B + 255) / 256, 256, 0, st>>>(B, p.w_raw, p.wmax_bits, w_out ? w_out : p.w);
+    per_norm_kernel<<<dim3((B + 255) / 256, p.G), 256, 0, st>>>(B, p.w_raw, p.wmax_bits, w_out ? w_out : p.w);
     UAVRL_LAUNCHED();
     l->pdl_prev = kPdlNone;
     return 0;
@@ -205,16 +222,17 @@ using namespace uavrl;
 
 extern "C" {
 
-int uavrl_per_enable(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
+static int per_enable_impl(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
 {
-    if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
-    if (l->G > 1) return fail(UAVRL_ERR_INVALID, "prioritised replay is not available on a learner with several trainers");
     if (l->per.enabled) return fail(UAVRL_ERR_STATE, "prioritised replay is already enabled");
     if (l->replay.count != 0) return fail(UAVRL_ERR_STATE, "enable prioritised replay before the first transition is stored");
+    if (l->G > 1 && l->replay.mode != kReplayLockstep)
+        return fail(UAVRL_ERR_INVALID, "prioritised replay on a learner with several trainers needs the lockstep ring (lockstep_envs > 0)");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     PerDev &p = l->per;
     memset(&p, 0, sizeof(p));
-    p.cap = l->replay.slots;
+    p.G = l->G;
+    p.cap = l->replay.slots / l->G;                               // trainer-local slots: ring_frames x Ng
     int64_t pow2 = 1;
     while (pow2 < p.cap) pow2 <<= 1;
     p.rot = pow2 - p.cap;
@@ -223,11 +241,25 @@ int uavrl_per_enable(uavrl_learner *l, double alpha, double beta0, double beta_i
     p.alpha = alpha >= 0 ? alpha : 0.6; p.beta = beta0 >= 0 ? beta0 : 0.4; p.beta_inc = beta_inc >= 0 ? beta_inc : 0.001;   // :141-148
     p.eps = eps >= 0 ? eps : 0.01; p.err_upper = err_upper >= 0 ? err_upper : 1.0;
     int rc;
-    if ((rc = dev_alloc(&p.leaf, (size_t)p.cap)) || (rc = dev_alloc(&p.l1, (size_t)p.n1)) || (rc = dev_alloc(&p.l2, (size_t)p.n2)) ||
-        (rc = dev_alloc(&p.wmax_bits, 1)))
+    const size_t G = (size_t)p.G;
+    if ((rc = dev_alloc(&p.leaf, G * p.cap)) || (rc = dev_alloc(&p.l1, G * p.n1)) || (rc = dev_alloc(&p.l2, G * p.n2)) ||
+        (rc = dev_alloc(&p.wmax_bits, G)))
         return rc;
     p.enabled = 1;
     return 0;
+}
+
+int uavrl_per_enable(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
+{
+    if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
+    if (l->G > 1) return fail(UAVRL_ERR_INVALID, "prioritised replay is not available on a learner with several trainers");
+    return per_enable_impl(l, alpha, beta0, beta_inc, eps, err_upper);
+}
+
+int uavrl_per_enable_trainers(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
+{
+    if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
+    return per_enable_impl(l, alpha, beta0, beta_inc, eps, err_upper);
 }
 
 int uavrl_per_set_priorities(uavrl_learner *l, int32_t n, const int32_t *slots_dev, const double *prio_dev, void *stream)
@@ -258,13 +290,16 @@ int uavrl_per_get(uavrl_learner *l, double *leaves_host, double *total_out, doub
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     UAVRL_CUDA(cudaDeviceSynchronize());
     const PerDev &p = l->per;
-    if (leaves_host) UAVRL_CUDA(cudaMemcpy(leaves_host, p.leaf, (size_t)p.cap * 8, cudaMemcpyDeviceToHost));
-    if (total_out) {
-        std::vector<double> h((size_t)p.n2);
-        UAVRL_CUDA(cudaMemcpy(h.data(), p.l2, (size_t)p.n2 * 8, cudaMemcpyDeviceToHost));
-        double s = 0.0;
-        for (double x : h) s += x;
-        *total_out = s;
+    const size_t G = (size_t)p.G;
+    if (leaves_host) UAVRL_CUDA(cudaMemcpy(leaves_host, p.leaf, G * p.cap * 8, cudaMemcpyDeviceToHost));
+    if (total_out) {                                              // [G]: each tree's l2 entries summed in order
+        std::vector<double> h(G * p.n2);
+        UAVRL_CUDA(cudaMemcpy(h.data(), p.l2, G * p.n2 * 8, cudaMemcpyDeviceToHost));
+        for (size_t g = 0; g < G; ++g) {
+            double s = 0.0;
+            for (int64_t k = 0; k < p.n2; ++k) s += h[g * p.n2 + k];
+            total_out[g] = s;
+        }
     }
     if (beta_out) *beta_out = p.beta;
     return 0;

@@ -12,6 +12,12 @@
 // Updating B priorities: three small launches (leaves, touched l1 entries, touched l2 entries), each entry recomputed
 // from its 32 children in a fixed order -> deterministic, no atomics, duplicates idempotent.  The sums differ from the
 // reference's incrementally updated heap nodes only in fp64 rounding (~1e-16 relative).
+//
+// Grouped learner (uavrl_per_enable_trainers): one tree per trainer, as every reference Trainer owns its replay.  Trainer g's
+// tree covers its own transitions under trainer-local slots j = f Ng + (e - g Ng) (ring frame f, env e of block g), which is
+// how a stand-alone learner over Ng envs numbers its slots.  Every array is [G][...] (leaf [G][cap], l1 [G][n1], l2 [G][n2],
+// scratch [G][B], wmax_bits [G]) and every kernel takes the trainer from blockIdx.y; cap, rot, alpha, beta and the sampling
+// call counter are shared (the trainers sample in lockstep).  G = 1 is the single tree above.
 #pragma once
 #include <math.h>
 
@@ -19,14 +25,15 @@
 
 namespace uavrl {
 
-constexpr int kPerMaxL2 = 4096;          // l2 entries scanned in shared memory: capacity <= 4096 * 1024 slots
+constexpr int kPerMaxL2 = 4096;          // l2 entries scanned in shared memory: capacity <= 4096 * 1024 slots (per trainer)
 
 struct PerDev {
     int32_t enabled;
-    int64_t cap, rot, n1, n2;
+    int32_t G;                            // trees (one per trainer)
+    int64_t cap, rot, n1, n2;             // per tree
     double *leaf, *l1, *l2;
     double alpha, beta, beta_inc, eps, err_upper;
-    // scratch of the integrated update path
+    // scratch of the integrated update path, [G][scratch_cap] (wmax_bits [G])
     int32_t *idx; float *w, *abs_err; double *w_raw; unsigned long long *wmax_bits;
     int32_t scratch_cap;
 };
@@ -35,6 +42,8 @@ struct PerDev {
 
 struct uavrl_learner;
 namespace uavrl {
+// Every call below acts on each trainer's tree at once (grid y = G): per_fill_range fills the same trainer-local range in
+// every tree; per_set takes [G][n] slots / values; per_sample draws B per trainer into [G][B] outputs (u_tape [G][B]).
 // contiguous slots (mod cap): the first n_first get `value`, the rest `value_rest` (n_first < 0: all get `value`)
 int per_fill_range(uavrl_learner *l, int64_t first_slot, int64_t n, double value, cudaStream_t st, int64_t n_first = -1,
                    double value_rest = 0.0);

@@ -40,7 +40,8 @@ struct BatchSrc {
 // Philox key salts of a learner seeded with `seed`: the eps-greedy draws use seed ^ kActSalt, replay sampling seed ^ kSampleSalt.
 // Trainer g of a grouped learner draws exactly what a stand-alone learner seeded with seed + g draws.
 // Federation probe draws (federate.cu) use seed ^ kFedSalt.
-constexpr uint64_t kActSalt = 0xAC7ull, kSampleSalt = 0x5EEDull, kFedSalt = 0xFEDull;
+// Prioritised-replay draws (per.cu) use seed ^ kPerSalt.
+constexpr uint64_t kActSalt = 0xAC7ull, kSampleSalt = 0x5EEDull, kFedSalt = 0xFEDull, kPerSalt = 0x9E12ull;
 __host__ __device__ __forceinline__ uint64_t trainer_key(uint64_t key, uint64_t salt, int g) { return ((key ^ salt) + (uint64_t)g) ^ salt; }
 
 #if defined(__CUDACC__)
@@ -76,10 +77,13 @@ __device__ __forceinline__ uint64_t perm_index(uint64_t i, uint64_t M, const uin
 
 // Trainer g's view of a batch source (grouped learner: gridDim.y = G trainers, B rows each).  Explicit batches: block g of the
 // G x B rows.  Lockstep ring: env block [g n_envs, (g + 1) n_envs), trainer g's sampling key and row g of a [G][B] index tape.
+// Both: row g of [G][B] importance weights and |Q - y| outputs (prioritised replay).
 __device__ __forceinline__ BatchSrc trainer_src(BatchSrc s, int g, int B, int in_dim)
 {
     if (g == 0) return s;
     const size_t r0 = (size_t)g * (size_t)B;
+    if (s.is_w) s.is_w += r0;
+    if (s.abs_err) s.abs_err += r0;
     if (s.mode == kBatchExplicit) {
         s.frames += r0 * in_dim; s.s2_rows += r0 * in_dim; s.rew += r0; s.done_f32 += r0;
         if (s.act) s.act += r0;

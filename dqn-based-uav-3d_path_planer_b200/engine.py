@@ -395,25 +395,42 @@ class Learner:
         check(_lib.lib().uavrl_per_enable(self.h, alpha, beta0, beta_inc, eps, err_upper))
         self.per_slots = int(self.cfg.replay_capacity) if not self.cfg.lockstep_envs else None
 
+    def per_enable_trainers(self, alpha=-1.0, beta0=-1.0, beta_inc=-1.0, eps=-1.0, err_upper=-1.0):
+        """Prioritised replay with one tree per trainer (include/uavrl.h uavrl_per_enable_trainers); per_enable when G = 1.
+        With G > 1 the per_* methods then take and return (G, ...) arrays of trainer-local slots."""
+        check(_lib.lib().uavrl_per_enable_trainers(self.h, alpha, beta0, beta_inc, eps, err_upper))
+        self.per_slots = int(self.cfg.replay_capacity) if not self.cfg.lockstep_envs else None
+
+    def _per_shape(self, n):
+        return (n,) if self.G == 1 else (self.G, n)
+
     def per_sample(self, batch, u_tape=None):
-        """ReplayTree.sample2: (slots int32 [B], importance weights float32 [B]) on the device."""
-        slots = torch.empty(batch, dtype=torch.int32, device=self.device)
-        w = torch.empty(batch, dtype=torch.float32, device=self.device)
+        """ReplayTree.sample2: (slots int32 [B], importance weights float32 [B]) on the device; (G, B) each on a grouped
+        learner, u_tape (G, B)."""
+        slots = torch.empty(self._per_shape(batch), dtype=torch.int32, device=self.device)
+        w = torch.empty(self._per_shape(batch), dtype=torch.float32, device=self.device)
         check(_lib.lib().uavrl_per_sample(self.h, int(batch), _ptr(u_tape), _ptr(slots), _ptr(w), _stream(self.device)))
         return slots, w
 
+    def _per_n(self, slots):
+        """Slots per trainer of a (n,) or, grouped, (G, n) slot array."""
+        if self.G > 1 and (slots.dim() != 2 or slots.shape[0] != self.G):
+            raise ValueError("a learner with %d trainers takes (%d, n) slots, got %s" % (self.G, self.G, tuple(slots.shape)))
+        return int(slots.shape[-1])
+
     def per_set_errors(self, slots, abs_err, clip=True):
-        check(_lib.lib().uavrl_per_set_errors(self.h, slots.shape[0], _ptr(slots), _ptr(abs_err), int(bool(clip)),
+        check(_lib.lib().uavrl_per_set_errors(self.h, self._per_n(slots), _ptr(slots), _ptr(abs_err), int(bool(clip)),
                                               _stream(self.device)))
 
     def per_set_priorities(self, slots, priorities):
-        check(_lib.lib().uavrl_per_set_priorities(self.h, slots.shape[0], _ptr(slots), _ptr(priorities), _stream(self.device)))
+        check(_lib.lib().uavrl_per_set_priorities(self.h, self._per_n(slots), _ptr(slots), _ptr(priorities), _stream(self.device)))
 
     def per_state(self, n_slots):
-        leaves = np.zeros(int(n_slots), np.float64)
-        total, beta = C.c_double(), C.c_double()
-        check(_lib.lib().uavrl_per_get(self.h, _ptr(leaves), C.byref(total), C.byref(beta)))
-        return leaves, total.value, beta.value
+        """(leaves, total, beta); grouped: n_slots per trainer, leaves (G, n_slots) and totals (G,)."""
+        leaves = np.zeros(self._per_shape(int(n_slots)), np.float64)
+        totals, beta = np.zeros(self.G, np.float64), C.c_double()
+        check(_lib.lib().uavrl_per_get(self.h, _ptr(leaves), totals.ctypes.data_as(C.POINTER(C.c_double)), C.byref(beta)))
+        return leaves, (float(totals[0]) if self.G == 1 else totals), beta.value
 
     def compute_grads(self, global_batch, idx_tape=None, loss=None):
         check(_lib.lib().uavrl_learner_compute_grads(self.h, _ptr(idx_tape), int(global_batch), _ptr(loss),

@@ -112,7 +112,12 @@ class TrainerB200:
         if self.IsPriority_Replay:
             if self.lockstep_envs == 0 and self.replay_size > 4 * 1024 * 1024:
                 raise ValueError("prioritised replay supports at most 4194304 slots")
-            self._learner.per_enable()                   # ReplayTree constants (replay_buffer.py:141-148)
+            # ReplayTree constants (replay_buffer.py:141-148); several trainers: one tree per trainer, as each reference
+            # Trainer owns its ReplayTree (BaseTrainer.py:39).  The host-driven paths below stay single-trainer.
+            if G > 1:
+                self._learner.per_enable_trainers()
+            else:
+                self._learner.per_enable()
         self.replay_memory = _ReplayFacade(self)
         self.model_dir = None2Value(param.get('model_path'), None)
         self.Load_Mod(self.model_dir)

@@ -206,6 +206,9 @@ int64_t uavrl_learner_param_count(const uavrl_learner *l);
  *   - refused with UAVRL_ERR_INVALID: n_trainers outside [1, 65535] (one grid row per trainer), lockstep_envs % n_trainers != 0, uavrl_per_enable,
  *     uavrl_learner_update_batch_per, uavrl_replay_push, uavrl_learner_comm_init / comm_connect / update_dp / compute_grads /
  *     apply_grads, uavrl_train_run_dp, and act / update_batch sizes that are not multiples of G;
+ *   - prioritised replay is enabled with uavrl_per_enable_trainers (one tree per trainer, trainer-local slots and [G][...] arrays
+ *     in every uavrl_per_* call; see the prioritised-replay block).  uavrl_per_enable keeps refusing G > 1 because the grouped
+ *     form changes the slot numbering and array shapes of the other uavrl_per_* calls, so a caller opts in by name;
  *   - the process-wide fused act + step and fused weight-gradient + optimiser paths are not taken (the separate kernels run). */
 int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_trainers, uavrl_learner **out);
 int32_t uavrl_learner_trainer_count(const uavrl_learner *l);
@@ -433,8 +436,21 @@ int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float
  * uavrl_per_sample = ReplayTree.sample2 (:186-213): physical slot indices (tree index = slot + capacity - 1) and
  * weights; u_tape_dev (optional, [batch] doubles in [0,1)) replaces the uniform draws.  uavrl_per_set_errors:
  * clip = 0 is ReplayTree.push's rule (:152-154), clip = 1 batch_update's (:216-223).  uavrl_per_set_priorities is
- * SumTree.update with explicit values.  uavrl_per_get copies the leaves [slots] to the host. */
+ * SumTree.update with explicit values.  uavrl_per_get copies the leaves [slots] to the host.
+ *
+ * uavrl_per_enable_trainers: the same for a learner with G >= 1 trainers (identical to uavrl_per_enable when G = 1; G > 1 needs
+ * the lockstep ring).  Trainer g gets its own tree over its own transitions, as each reference Trainer owns its ReplayTree, and
+ * computes bit for bit what a stand-alone learner with prioritised replay, seed + g and Ng = lockstep_envs / G envs computes.
+ * Slots are trainer-local: transition (ring frame f, env e) of trainer g's block is slot j = f Ng + (e - g Ng), in
+ * [0, cap_g), cap_g = ring_frames Ng (the numbering of a stand-alone learner over Ng envs).  cap_g <= 4194304.  Refused after
+ * the first stored transition.  Afterwards, on a grouped learner:
+ *   - uavrl_per_sample: batch is per trainer; u_tape_dev [G][batch]; slots / weights out [G][batch], each row normalised by
+ *     that trainer's own maximum weight, n = that trainer's transition count; trainer g's draws are keyed by seed + g;
+ *   - uavrl_per_set_errors / uavrl_per_set_priorities: n is per trainer; slots and values [G][n];
+ *   - uavrl_per_get: leaves [G][cap_g], total_out [G], beta (shared: the trainers sample in lockstep);
+ *   - uavrl_learner_update / uavrl_train_run sample every trainer from its own tree and write |Q - y| back into it. */
 int uavrl_per_enable(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper);
+int uavrl_per_enable_trainers(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper);
 int uavrl_per_sample(uavrl_learner *l, int32_t batch, const double *u_tape_dev, int32_t *slots_out_dev,
                      float *weights_out_dev, void *stream);
 int uavrl_per_set_errors(uavrl_learner *l, int32_t n, const int32_t *slots_dev, const float *abs_err_dev, int32_t clip,

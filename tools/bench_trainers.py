@@ -3,8 +3,9 @@
 iterations, after warm-up), env steps/s, trainer updates/s, the weight-image bytes the kernels stage into shared memory per
 iteration (computed from the shapes) and that traffic over time as a share of the H100 SXM's 3.35 TB/s, the per-kernel split
 of one iteration, and the GPU's name and power limit read in the same run.  bench.py stays the headline measurement.
+--per gives every trainer its own prioritised replay (uavrl_per_enable_trainers); the line then carries "prioritised_replay".
 
-    python tools/bench_trainers.py [--envs 4096] [--trainers 1,16,256,4096] [--steps 2000] [--warmup 200]"""
+    python tools/bench_trainers.py [--envs 4096] [--trainers 1,16,256,4096] [--steps 2000] [--warmup 200] [--per]"""
 import argparse
 import json
 import os
@@ -70,6 +71,7 @@ def main():
     ap.add_argument("--steps", type=int, default=2000)
     ap.add_argument("--warmup", type=int, default=200)
     ap.add_argument("--frames", type=int, default=128, help="replay ring frames (every trainer holds frames x envs/G transitions)")
+    ap.add_argument("--per", action="store_true", help="prioritised replay, one SumTree per trainer")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_trainers needs a CUDA device")
@@ -92,6 +94,8 @@ def main():
         L = engine.Learner(100, hidden, 27, False, engine.ALGO_DQN, lr=5e-4, gamma=0.99, batch_size=B, update_loop=3,
                            replay_capacity=N * a.frames, lockstep_envs=N, seed=1234, device=0, trainers=G)
         L.init_params(0)
+        if a.per:
+            L.per_enable_trainers()
         engine.train_run(env, L, max(a.warmup, (B * G) // N + 2), 0.1, want_stats=False)   # every trainer holds > B transitions
         torch.cuda.synchronize()
         footprint = free0 - torch.cuda.mem_get_info(0)[0]
@@ -104,6 +108,7 @@ def main():
         assert st.updates == a.steps and torch.isfinite(torch.tensor(st.last_loss))
         prof = engine.train_profile(env, L, 200, 0.1) / 200           # event-separated kernels: a split, not a throughput
         sb = staged_bytes(L, N, G, B, True, fwd, train)
+        extra = {"prioritised_replay": True} if a.per else {}
         print(json.dumps({
             "trainers": G, "envs": N, "envs_per_trainer": N // G, "batch_per_trainer": B, "network": "DQN 100-64-64-27",
             "iteration_us": ms * 1e3, "env_steps_per_s": N / (ms * 1e-3), "trainer_updates_per_s": G / (ms * 1e-3),
@@ -111,7 +116,7 @@ def main():
             "staged_share_of_3.35TBps": sb / (ms * 1e-3) / HBM_BYTES_PER_S,
             "profile_us": dict(zip(("act", "env_step", "td_target", "train", "weight_grad", "optimiser"), (float(x) * 1e3 for x in prof))),
             "device_footprint_bytes": int(footprint), "timed_iterations": a.steps, "last_loss": float(st.last_loss),
-            "gpu": info, "launches": int(_lib.launch_count())}), flush=True)
+            "gpu": info, "launches": int(_lib.launch_count()), **extra}), flush=True)
         L.close(); env.close()
         del L, env
         torch.cuda.synchronize()
