@@ -1,5 +1,5 @@
-// env_block.cuh -- the per-CTA body of the env step / observation kernel, callable from env_kernel (env.cu) and from
-// the fused act+step kernel (tc_forward.cu): EPB envs starting at e0, NT threads, shared-memory scratch passed in.
+// env_block.cuh -- the per-CTA body of the env step / observation kernel (env_kernel, env.cu): EPB envs starting at e0,
+// NT threads, shared-memory scratch passed in.
 // Phases and references: see env.cu.
 #pragma once
 #include "env.cuh"

@@ -389,130 +389,13 @@ cudaError_t launch_reduce_adam(dim3 grid, cudaStream_t st, bool pdl, const AdamA
                          q.img_local, q.img_target, q.img_map, q.tc_local, q.tc_target, q.tc_hi, q.tc_lo, q.tc_hi2, q.tc_lo2, q.loss_out);
 }
 
-// ---- data-parallel pair (one-shot NVLink all-reduce fused with the optimiser).
-// Every rank owns a symmetric receive buffer recv[2][world][P+1] (double-buffered by update parity; slot q belongs to
-// rank q) and a flag word per peer.
-//   (1) reduce_publish_kernel: reduce this rank's gradient partials and PUSH the result -- fire-and-forget remote stores
-//       over NVLink -- into slot `rank` of every rank's receive buffer (its own included); once the whole grid is done
-//       (last-block detection), fence at system scope and raise this rank's flag on every peer.
-//   (2) allreduce_adam_kernel: wait for all `world` flags in LOCAL memory, read the `world` gradient vectors from the LOCAL
-//       receive buffer, sum them in rank order (bit-identical replicas) and apply Adam.  Nothing is pulled across NVLink on
-//       the critical path: the only remote traffic are the posted writes of (1).
-__global__ void __launch_bounds__(256)
-reduce_publish_kernel(int P, int nparts, int n_loss_parts, float inv_b, const float *__restrict__ partials,
-                      const float *__restrict__ loss_partials, float *const *peer_recv, size_t slot_off, unsigned *counter,
-                      unsigned *const *peer_flags, int rank, int world, unsigned epoch)
-{
-    __shared__ float red[4][64];
-    const int ix = threadIdx.x & 63, cg = threadIdx.x >> 6;
-    const int i = blockIdx.x * 64 + ix;
-    pdl_wait();                 // PDL (common.cuh): the gradient partials come from the predecessor
-    pdl_trigger();
-    float g = 0.f;
-    if (i < P) {
-        float acc[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) acc[u] = 0.f;
-        int c = cg;
-        for (; c + 28 < nparts; c += 32) {
-#pragma unroll
-            for (int u = 0; u < 8; ++u) acc[u] += partials[(size_t)(c + 4 * u) * P + i];
-        }
-        for (; c < nparts; c += 4) acc[0] += partials[(size_t)c * P + i];
-        g = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
-    }
-    red[cg][ix] = g;
-    __syncthreads();
-    // thread (cg, ix) pushes element i to peers cg, cg+4, ...: 64 consecutive floats = 256 contiguous bytes per peer
-    if (i < P) {
-        const float gs = (red[0][ix] + red[1][ix]) + (red[2][ix] + red[3][ix]);
-        for (int q = cg; q < world; q += 4) peer_recv[q][slot_off + i] = gs;
-    }
-    if (blockIdx.x == 0 && threadIdx.x >= 224) {                 // last warp of block 0: this rank's loss share
-        const int lane = threadIdx.x & 31;
-        float s = 0.f;
-        for (int c = lane; c < n_loss_parts; c += 32) s += loss_partials[c];
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (lane == 0)
-            for (int q = 0; q < world; ++q) peer_recv[q][slot_off + P] = s * inv_b;
-    }
-    __syncthreads();                                             // every thread's remote stores are ordered before thread 0's fence
-    if (threadIdx.x == 0) {
-        __threadfence_system();                                  // ONE cumulative system fence per block, not one in each of the
-                                                                 // 256 threads
-        const unsigned prev = atomicAdd(counter, 1u);
-        if (prev == gridDim.x - 1) {                             // every block's slice has been pushed to every peer
-            *counter = 0u;
-            __threadfence_system();
-            for (int q = 0; q < world; ++q) {
-                volatile unsigned *f = peer_flags[q] + rank;
-                *f = epoch;
-            }
-        }
-    }
-}
-
-__device__ __forceinline__ unsigned ld_acquire_sys(const unsigned *p)
-{
-    unsigned v;
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ float ld_relaxed_sys(const float *p)
-{
-    float v;
-    asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
-    return v;
-}
-
-__global__ void __launch_bounds__(256)
-allreduce_adam_kernel(AdamArgs a, const float *recv, size_t stride, const unsigned *my_flags, unsigned epoch,
-                      float *__restrict__ grad, float *__restrict__ local, float *__restrict__ m, float *__restrict__ v,
-                      float *__restrict__ target, float *__restrict__ img_local, float *__restrict__ img_target,
-                      const int32_t *__restrict__ img_map, float *__restrict__ tc_local, float *__restrict__ tc_target,
-                      const int32_t *__restrict__ tc_hi, const int32_t *__restrict__ tc_lo, const int32_t *__restrict__ tc_hi2,
-                      const int32_t *__restrict__ tc_lo2, float *__restrict__ loss_out)
-{
-    pdl_wait();                 // PDL: nothing may still read the weight images this kernel rewrites
-    pdl_trigger();
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (threadIdx.x < a.world) {                                  // one thread per peer spins on that peer's flag (local memory)
-        while (ld_acquire_sys(my_flags + threadIdx.x) < epoch) { }
-    }
-    __syncthreads();
-    if (i < a.P) {
-        // `world` vectors of the LOCAL receive buffer, summed in rank order; loads issued 8 at a time
-        float g = 0.f;
-        int q = 0;
-        for (; q + 8 <= a.world; q += 8) {
-            float t[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) t[u] = ld_relaxed_sys(recv + (size_t)(q + u) * stride + i);
-#pragma unroll
-            for (int u = 0; u < 8; ++u) g += t[u];
-        }
-        for (; q < a.world; ++q) g += ld_relaxed_sys(recv + (size_t)q * stride + i);
-        grad[i] = g;
-        AdamPtrs ap;
-        ap.partials = nullptr; ap.loss_partials = nullptr; ap.grad = grad; ap.local = local; ap.m = m; ap.v = v; ap.target = target;
-        ap.img_local = img_local; ap.img_target = img_target; ap.img_map = img_map; ap.tc_local = tc_local; ap.tc_target = tc_target;
-        ap.tc_hi = tc_hi; ap.tc_lo = tc_lo; ap.tc_hi2 = tc_hi2; ap.tc_lo2 = tc_lo2; ap.loss_out = loss_out;
-        adam_update_one(a, ap, i, g);
-    }
-    if (i == 0 && loss_out) {
-        float s = 0.f;
-        for (int q = 0; q < a.world; ++q) s += ld_relaxed_sys(recv + (size_t)q * stride + a.P);
-        *loss_out = s;
-    }
-}
-
-// ---- the same exchange in ONE kernel, block by block, with NO fence and NO flag words (default): block b owns parameters
+// ---- data-parallel optimiser step: one-shot NVLink all-reduce fused with Adam, in ONE kernel, block by block, with no fence
+// and no flag words.  Every rank owns a symmetric receive buffer (slot q belongs to rank q); block b owns parameters
 // [64 b, 64 b + 64).  It reduces its slice of this rank's partials and pushes each value into slot `rank` of every rank's
 // receive buffer as ONE 8-byte word {epoch : value} (a single-copy-atomic store: the value can never be seen without its
 // epoch -- the "LL" idea of NCCL's low-latency protocol).  Then the 64 threads of the block poll -- in local memory -- the
 // `world` words of their own parameter until every epoch matches, sum the values in rank order and apply Adam.  A
-// A __threadfence_system() between data and flag would cost a system-scope fence per launch even on one GPU; here nothing
+// __threadfence_system() between data and a flag would cost a system-scope fence per launch even on one GPU; here nothing
 // orders two stores, so nothing needs a fence.  recv[2][world][P + 1] alternates by epoch parity: a sender can
 // overwrite a slot only two exchanges later, and it cannot finish the exchange in between before the receiver has read.
 __device__ __forceinline__ void st_relaxed_sys_u64(unsigned long long *p, unsigned long long v)
@@ -683,26 +566,6 @@ int launch_fed_loss(uavrl_learner *l, const float *probes, const float *q_ref, f
     return 0;
 }
 
-// Trainer.get_action + BaseEnv.Move_Agent for the lockstep loops in ONE kernel (tc_forward.cu, FUSE_ENV): each CTA steps
-// the envs whose actions it has just computed.  Returns 1 when the fused path is not available (tensor-core path off /
-// switched off): the caller then launches the two kernels.
-// Off by default: the stand-alone env kernel spreads its fp64 chains over many small CTAs, while the fused kernel steps the
-// envs with the few CTAs of the act pass.
-std::atomic<int> g_fuse_act_env{0};
-int launch_act_env(uavrl_learner *l, const EnvDev &d, const float *obs, float eps, int32_t *actions, float *obs_next, float *rew,
-                   uint8_t *done, cudaStream_t st)
-{
-    if (!(l->tc_ok && l->use_tc && l->fuse_ok) || !g_fuse_act_env.load() || l->G > 1) return 1;
-    TcArgs a;
-    memset(&a, 0, sizeof(a));
-    a.img = l->tc_img_local; a.obs = obs; a.n = d.n; a.n_tiles = (d.n + kTcTile - 1) / kTcTile; a.mode = kTcAct;
-    a.eps = eps; a.is_train = l->is_train;
-    a.key = l->cfg.seed ^ kActSalt; a.call = l->act_calls++; a.actions = actions;
-    EnvFuse ef;
-    ef.d = d; ef.obs_next = obs_next; ef.reward = rew; ef.done = done;
-    return launch_tc_forward(l, a, st, &ef);
-}
-
 static int launch_update_impl(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, bool apply,
                               cudaStream_t st, cudaEvent_t *mid, bool partials_only = false);
 
@@ -777,7 +640,6 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
     }
     if (mid) UAVRL_CUDA(cudaEventRecord(mid[0], st));
     int nparts = grid, n_loss_parts = grid;
-    // optimiser step arguments (needed before the weight-gradient launch: small batches fuse the step behind it)
     AdamArgs a;
     memset(&a, 0, sizeof(a));
     a.P = l->net.P; a.apply = apply ? 1 : 0; a.world = l->world;
@@ -787,7 +649,6 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
         adam_hyper(a, l->cfg.lr, ++l->adam_t);
         a.hard = hard_update_due(l);
     }
-    bool adam_done = false;
     if (y_in && l->tc_train_ok) {
         // the whole update on the tensor cores: forward + dX chain, then split-K weight gradients (tc_train.cu)
         if (B > l->train_cap) {
@@ -797,9 +658,7 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
             UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, (size_t)l->G * B * (size_t)l->tc.dz_stride * 4));
             l->train_cap = B;
         }
-        const bool may_fuse = apply && !partials_only && !per_batch;
-        int rc = launch_tc_train(l, src, B, global_batch, y_in, &nparts, &n_loss_parts, st, mid ? mid[1] : nullptr,
-                                 may_fuse ? &a : nullptr, loss_out ? loss_out : l->loss_dev, &adam_done, fuse_td);
+        int rc = launch_tc_train(l, src, B, global_batch, y_in, &nparts, &n_loss_parts, st, mid ? mid[1] : nullptr, fuse_td);
         if (rc) return rc;
     } else {
     UpdateArgs ua;
@@ -821,7 +680,6 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
         if (per_batch) return per_set(l, B, l->per.idx, nullptr, l->per.abs_err, 1, st);
         return 0;
     }
-    if (adam_done) return 0;                                    // the weight-gradient kernel applied the optimiser step itself
     a.nparts = nparts; a.n_loss_parts = n_loss_parts;
     const bool chain = l->pdl_chain && g_pdl.load();
     UAVRL_CUDA(launch_reduce_adam(dim3((a.P + 63) / 64, l->G), st, chain && l->pdl_prev == kPdlDw && !mid, a,
@@ -852,16 +710,16 @@ static int repack_images(uavrl_learner *l, cudaStream_t st)
     return 0;
 }
 
-// local gradient partials (same kernels as the single-GPU update, no optimiser step), then the fused
-// publish / all-reduce+Adam pair
+// local gradient partials (same kernels as the single-GPU update, no optimiser step), then the exchange fused with Adam
+// (dp_allreduce_adam_kernel)
 int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, cudaStream_t st)
 {
     int rc = launch_update_impl(l, src, B, global_batch, nullptr, false, st, nullptr, true);
     if (rc) return rc;
-    l->flag_epoch += 1;
+    l->comm_epoch += 1;
     const int P = l->net.P;
     const size_t stride = (size_t)P + 1;                                        // one rank's slot: gradient vector + loss share
-    const size_t parity_off = (size_t)(l->flag_epoch & 1u) * (size_t)l->world * stride;
+    const size_t parity_off = (size_t)(l->comm_epoch & 1u) * (size_t)l->world * stride;
     const bool chain = l->pdl_chain && g_pdl.load();
     AdamArgs a;
     memset(&a, 0, sizeof(a));
@@ -869,27 +727,13 @@ int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_ba
     adam_hyper(a, l->cfg.lr, ++l->adam_t);
     a.hard = hard_update_due(l);
     a.inv_b = 1.0f / (float)global_batch;
-    static const bool two_kernels = getenv("UAVRL_DP_TWO_KERNELS") != nullptr;     // the grid-wide publish + all-reduce pair
     static const bool dp_trace = getenv("UAVRL_DP_TRACE") != nullptr;
     if (dp_trace && !l->dp_trace) { UAVRL_CUDA(cudaMalloc((void **)&l->dp_trace, 5 * 8)); UAVRL_CUDA(cudaMemsetAsync(l->dp_trace, 0, 40, st)); }
     const int nblk = (P + 63) / 64;
-    if (!two_kernels) {
-        UAVRL_CUDA(launch_kernel(dp_allreduce_adam_kernel, dim3(nblk), dim3(256), 0, st, chain && l->pdl_prev == kPdlDw, a, l->last_nparts,
-                                 l->last_n_loss_parts, (const float *)l->partials, (const float *)l->loss_partials,
-                                 (unsigned long long *const *)l->peer_grad_dev, (const unsigned long long *)l->comm_grad, stride, parity_off,
-                                 l->rank, l->flag_epoch, learner_adam_ptrs(l, loss_out ? loss_out : l->loss_dev), l->dp_trace));
-        UAVRL_LAUNCHED();
-        l->pdl_prev = chain ? kPdlAdam : kPdlNone;
-        return 0;
-    }
-    UAVRL_CUDA(launch_kernel(reduce_publish_kernel, dim3((P + 63) / 64), dim3(256), 0, st, chain && l->pdl_prev == kPdlDw, P, l->last_nparts,
-                             l->last_n_loss_parts, 1.0f / (float)global_batch, l->partials, l->loss_partials, l->peer_grad_dev,
-                             parity_off + (size_t)l->rank * stride, l->comm_counter, l->peer_flag_dev, l->rank, l->world, l->flag_epoch));
-    UAVRL_LAUNCHED();
-    UAVRL_CUDA(launch_kernel(allreduce_adam_kernel, dim3((P + 255) / 256), dim3(256), 0, st, chain && l->pdl_prev == kPdlDw, a,
-                             (const float *)(l->comm_grad + parity_off), stride, l->comm_flags, l->flag_epoch, l->grad, l->local, l->m, l->v,
-                             l->target, l->img_local, l->img_target, l->img_map, (float *)l->tc_img_local, (float *)l->tc_img_target,
-                             l->tc_hi_map, l->tc_lo_map, l->tc_hi2_map, l->tc_lo2_map, loss_out ? loss_out : l->loss_dev));
+    UAVRL_CUDA(launch_kernel(dp_allreduce_adam_kernel, dim3(nblk), dim3(256), 0, st, chain && l->pdl_prev == kPdlDw, a, l->last_nparts,
+                             l->last_n_loss_parts, (const float *)l->partials, (const float *)l->loss_partials,
+                             (unsigned long long *const *)l->peer_grad_dev, (const unsigned long long *)l->comm_grad, stride, parity_off,
+                             l->rank, l->comm_epoch, learner_adam_ptrs(l, loss_out ? loss_out : l->loss_dev), l->dp_trace));
     UAVRL_LAUNCHED();
     l->pdl_prev = chain ? kPdlAdam : kPdlNone;
     return 0;
@@ -1008,12 +852,11 @@ int uavrl_learner_destroy(uavrl_learner *l)
     for (int q = 0; q < l->world && l->comm_ready; ++q) {
         if (q == l->rank) continue;
         if (l->peer_grad_host[q]) cudaIpcCloseMemHandle(l->peer_grad_host[q]);
-        if (l->peer_flag_host[q]) cudaIpcCloseMemHandle(l->peer_flag_host[q]);
     }
     l->replay.release();
-    void *ptrs[] = { l->local, l->target, l->m, l->v, l->grad, l->partials, l->loss_partials, l->loss_dev, l->comm_grad, l->comm_flags, l->comm_counter, l->peer_grad_dev, l->peer_flag_dev, l->img_local, l->img_target,
+    void *ptrs[] = { l->local, l->target, l->m, l->v, l->grad, l->partials, l->loss_partials, l->loss_dev, l->comm_grad, l->peer_grad_dev, l->img_local, l->img_target,
                      l->img_map, l->tc_img_local, l->tc_img_target, l->tc_hi_map, l->tc_lo_map, l->y_buf, l->astar_buf, l->tc_hi2_map,
-                     l->tc_lo2_map, l->act_buf, l->dz_buf, l->dw_bar };
+                     l->tc_lo2_map, l->act_buf, l->dz_buf };
     for (void *p : ptrs) cudaFree(p);
     per_free(l);
     delete l;
@@ -1110,7 +953,11 @@ int uavrl_replay_push(uavrl_learner *l, int32_t n, const float *obs, const int32
 
 int64_t uavrl_replay_size(const uavrl_learner *l) { return l ? l->replay.count : 0; }
 
-int uavrl_set_fuse_act_env(int32_t on) { g_fuse_act_env.store(on ? 1 : 0); return 0; }
+// kept for ABI compatibility: the lockstep loops always launch get_action and the env step as two kernels
+int uavrl_set_fuse_act_env(int32_t on)
+{
+    return on ? fail(UAVRL_ERR_INVALID, "uavrl_set_fuse_act_env: the fused get_action + env step variant was removed") : 0;
+}
 
 int uavrl_replay_gather(uavrl_learner *l, int32_t n, const int64_t *idx, float *s, int32_t *a, float *r, float *s2,
                         uint8_t *d)
@@ -1244,57 +1091,48 @@ int uavrl_learner_lockstep_restart(uavrl_learner *l)
 }
 
 // ------------------------------------------------------------------ fused NVLink all-reduce + Adam
+// flag_handle_out / flag_handles: unused (kept for ABI compatibility), may be NULL
 int uavrl_learner_comm_init(uavrl_learner *l, int32_t rank, int32_t world, void *grad_handle_out, void *flag_handle_out)
 {
-    if (!l || world < 1 || world > 64 || rank < 0 || rank >= world || !grad_handle_out || !flag_handle_out)
+    (void)flag_handle_out;
+    if (!l || world < 1 || world > 64 || rank < 0 || rank >= world || !grad_handle_out)
         return fail(UAVRL_ERR_INVALID, "bad rank/world/handle pointer");
     if (int rc = refuse_grouped(l, "uavrl_learner_comm_init (data-parallel training)")) return rc;
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     l->rank = rank; l->world = world;
     if (l->comm_grad && l->comm_world != world) {                // re-initialised with another world size
         UAVRL_CUDA(cudaDeviceSynchronize());
-        cudaFree(l->comm_grad); cudaFree(l->comm_flags); cudaFree(l->comm_counter);
-        l->comm_grad = nullptr; l->comm_flags = nullptr; l->comm_counter = nullptr;
+        cudaFree(l->comm_grad);
+        l->comm_grad = nullptr;
     }
     l->comm_world = world;
     if (!l->comm_grad) {
-        // recv[2][world][P+1] words of 8 bytes {epoch : value} (the default one-kernel exchange; epoch 0 = never written).  The
-        // two-kernel pair (UAVRL_DP_TWO_KERNELS=1) uses the first half as plain floats plus the flag words below.
+        // recv[2][world][P+1] words of 8 bytes {epoch : value} (epoch 0 = never written)
         const size_t n = 2 * (size_t)world * ((size_t)l->net.P + 1);
         UAVRL_CUDA(cudaMalloc((void **)&l->comm_grad, n * sizeof(unsigned long long)));
         UAVRL_CUDA(cudaMemset(l->comm_grad, 0, n * sizeof(unsigned long long)));
-        l->comm_flag_words = 0;
-        UAVRL_CUDA(cudaMalloc((void **)&l->comm_flags, (size_t)64 * sizeof(unsigned)));        // one flag per rank (the two-kernel pair)
-        UAVRL_CUDA(cudaMemset(l->comm_flags, 0, (size_t)64 * sizeof(unsigned)));
-        UAVRL_CUDA(cudaMalloc((void **)&l->comm_counter, sizeof(unsigned)));
-        UAVRL_CUDA(cudaMemset(l->comm_counter, 0, sizeof(unsigned)));
     }
-    cudaIpcMemHandle_t hg, hf;
+    cudaIpcMemHandle_t hg;
     UAVRL_CUDA(cudaIpcGetMemHandle(&hg, l->comm_grad));
-    UAVRL_CUDA(cudaIpcGetMemHandle(&hf, l->comm_flags));
     memcpy(grad_handle_out, &hg, sizeof(hg));
-    memcpy(flag_handle_out, &hf, sizeof(hf));
     return 0;
 }
 
 int uavrl_learner_comm_connect(uavrl_learner *l, const void *grad_handles, const void *flag_handles)
 {
+    (void)flag_handles;
     if (int rc = refuse_grouped(l, "uavrl_learner_comm_connect (data-parallel training)")) return rc;
-    if (!l || !grad_handles || !flag_handles || !l->comm_grad) return fail(UAVRL_ERR_STATE, "uavrl_learner_comm_connect before comm_init");
+    if (!l || !grad_handles || !l->comm_grad) return fail(UAVRL_ERR_STATE, "uavrl_learner_comm_connect before comm_init");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     for (int q = 0; q < l->world; ++q) {
-        if (q == l->rank) { l->peer_grad_host[q] = l->comm_grad; l->peer_flag_host[q] = l->comm_flags; continue; }
-        cudaIpcMemHandle_t hg, hf;
+        if (q == l->rank) { l->peer_grad_host[q] = l->comm_grad; continue; }
+        cudaIpcMemHandle_t hg;
         memcpy(&hg, (const char *)grad_handles + (size_t)q * sizeof(hg), sizeof(hg));
-        memcpy(&hf, (const char *)flag_handles + (size_t)q * sizeof(hf), sizeof(hf));
         UAVRL_CUDA(cudaIpcOpenMemHandle(&l->peer_grad_host[q], hg, cudaIpcMemLazyEnablePeerAccess));
-        UAVRL_CUDA(cudaIpcOpenMemHandle(&l->peer_flag_host[q], hf, cudaIpcMemLazyEnablePeerAccess));
     }
-    cudaFree(l->peer_grad_dev); cudaFree(l->peer_flag_dev);
+    cudaFree(l->peer_grad_dev);
     UAVRL_CUDA(cudaMalloc((void **)&l->peer_grad_dev, sizeof(void *) * l->world));
-    UAVRL_CUDA(cudaMalloc((void **)&l->peer_flag_dev, sizeof(void *) * l->world));
     UAVRL_CUDA(cudaMemcpy(l->peer_grad_dev, l->peer_grad_host, sizeof(void *) * l->world, cudaMemcpyHostToDevice));
-    UAVRL_CUDA(cudaMemcpy(l->peer_flag_dev, l->peer_flag_host, sizeof(void *) * l->world, cudaMemcpyHostToDevice));
     l->comm_ready = true;
     return 0;
 }

@@ -98,7 +98,6 @@ struct uavrl_learner {
     int64_t epoch = 0, adam_t = 0;
     uavrl::ReplayStore replay;        // int32 actions
     // programmatic dependent launch chain of the lockstep loops (common.cuh)
-    bool fuse_ok = false;             // the fused get_action + step kernel fits (tc_forward.cu)
     bool pdl_chain = false;
     int pdl_prev = 0;
     // prioritised replay (per.cuh); off unless uavrl_per_enable was called
@@ -109,17 +108,12 @@ struct uavrl_learner {
     // data-parallel: one-shot NVLink all-reduce fused with Adam (symmetric buffers exchanged through CUDA IPC)
     int32_t rank = 0, world = 1;
     float *comm_grad = nullptr;       // own receive buffer recv[2][world][P+1]: slot q is written by rank q (remote stores)
-    int32_t comm_world = 0, comm_flag_words = 0;
+    int32_t comm_world = 0;
     unsigned long long *dp_trace = nullptr;    // UAVRL_DP_TRACE=1: phase times of the data-parallel optimiser kernel
-    unsigned *comm_flags = nullptr;   // own, [64]: slot q is raised by rank q
-    unsigned *comm_counter = nullptr; // last-block detection of the publish kernel
     float **peer_grad_dev = nullptr;  // device array [world]: every rank's receive buffer as mapped on THIS device
-    unsigned **peer_flag_dev = nullptr;
-    void *peer_grad_host[64] = { nullptr }, *peer_flag_host[64] = { nullptr };
+    void *peer_grad_host[64] = { nullptr };
     bool comm_ready = false;
-    unsigned flag_epoch = 0;
-    unsigned long long *dw_bar = nullptr;      // fused weight-gradient + optimiser kernel: {epoch : value} partials [slices][P]
-    unsigned long long dw_bar_total = 0;
+    unsigned comm_epoch = 0;          // tag of the latest exchange (launch_update_dp); 0 = never written
     int last_nparts = 0, last_n_loss_parts = 0;
     int last_global_batch = 0;
 };
@@ -182,8 +176,8 @@ __device__ __forceinline__ AdamPre adam_prefetch(const AdamPtrs &q, int i)
 }
 __device__ __forceinline__ void adam_update_pre(const AdamArgs &a, const AdamPtrs &q, int i, float g, const AdamPre &pre)
 {
-    // every operation individually rounded (no FMA contraction): the optimiser kernels that share this function (stand-alone,
-    // fused behind the weight-gradient kernel, all-reduce) then produce bit-identical parameters by construction
+    // every operation individually rounded (no FMA contraction): the optimiser kernels that share this function
+    // (reduce_adam_kernel, dp_allreduce_adam_kernel) then produce bit-identical parameters by construction
     float mi = pre.m, vi = pre.v, p = pre.p;
     mi = __fadd_rn(mi, __fmul_rn(__fsub_rn(g, mi), a.beta1_c));                                  // exp_avg.lerp_(grad, 1 - beta1)
     vi = __fadd_rn(__fmul_rn(vi, a.beta2), __fmul_rn(__fmul_rn(a.beta2_c, g), g));               // exp_avg_sq.mul_(beta2).addcmul_(g, g, 1 - beta2)
@@ -209,11 +203,6 @@ __device__ __forceinline__ void adam_update_pre(const AdamArgs &a, const AdamPtr
     }
 }
 
-__device__ __forceinline__ void adam_update_one(const AdamArgs &a, const AdamPtrs &q, int i, float g)
-{
-    adam_update_pre(a, q, i, g, adam_prefetch(q, i));
-}
-
 #endif
 // reduce_adam_kernel (learner.cu) on `grid` (y: trainer) with the pointers of q; pdl: programmatic dependent launch
 cudaError_t launch_reduce_adam(dim3 grid, cudaStream_t st, bool pdl, const AdamArgs &a, const AdamPtrs &q);
@@ -226,10 +215,6 @@ AdamPtrs learner_adam_ptrs(const uavrl_learner *l, float *loss_out);
 
 // generic MLP description: trunk widths + head = `head_main` rows (+ `head_extra` rows from a second parameter block)
 int build_mlp(int in_dim, int n_hidden, const int32_t *hidden, int head_main, int head_extra, NetDev &n);
-struct EnvDev;
-extern std::atomic<int> g_fuse_act_env;
-int launch_act_env(uavrl_learner *l, const EnvDev &d, const float *obs, float eps, int32_t *actions, float *obs_next, float *rew,
-                   uint8_t *done, cudaStream_t st);
 int launch_act(uavrl_learner *l, const float *obs, int n, float eps, int is_train, const float *u_tape,
                const int32_t *rand_tape, int32_t *actions, float *q_out, cudaStream_t st);
 // the loss variant of the act pass (federation): weight sets w0 .. w0 + n_weights - 1 on the probe rows [G][kFedProbes][in_dim]

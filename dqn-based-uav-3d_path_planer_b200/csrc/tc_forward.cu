@@ -12,7 +12,6 @@
 // the next layer's A operand straight back into SMEM -- activations never touch HBM.  The head's epilogue
 // forms Q (dueling combine), then eps-greedy / argmax / max / gather depending on the mode.
 #include "tc_forward.cuh"
-#include "env_block.cuh"
 
 #include <stdlib.h>
 #include <string.h>
@@ -115,15 +114,13 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
 
 #define TC_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
 
-// FUSE_ENV: after a tile's actions are written, the same CTA steps those R envs (env_block.cuh) -- the act -> step
-// dependency is per env, so no grid-wide boundary is needed between Trainer.get_action and BaseEnv.Move_Agent.
 // ACT (a.mode == kTcAct) and DUELING are compile-time: the kernel a pass runs carries no code of the other modes.
 // FIXED: every layer product is one unbroken compile-time wgmma chain (wgmma.cuh mma_fixed; tc_fixed_chains).
 // LOSS (with ACT, federation): grid row y evaluates weight set loss_w0 + y on a probe-row range (TcArgs::loss_*); a tile
 // takes whole groups of kFedProbes rows, and its head epilogue reduces each group to one loss entry.
 // The kernels below are thin entry points over this body: tc_forward_kernel_t (LOSS = false) and tc_loss_kernel_t.
-template <bool FUSE_ENV, bool ACT, bool DUELING, bool FIXED, bool LOSS>
-__device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a, const EnvFuse &ef)
+template <bool ACT, bool DUELING, bool FIXED, bool LOSS>
+__device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a)
 {
     TC_TRACE(0);
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -352,28 +349,20 @@ __device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a
                 }
             }
         }
-        if (FUSE_ENV) {
-            // the tile's actions are in global memory (written by this CTA before the barrier above)
-            __shared__ EnvSmem<32> env_sm;
-            for (int sb = 0; sb < R; sb += 32)
-                env_block<true, 32, kTcThreads, false, 8>(ef.d, env_sm, base + sb, tid, UAVRL_ACT_DISCRETE27, a.actions, ef.obs_next,
-                                                       ef.reward, ef.done, nullptr, nullptr, nullptr);
-            __syncthreads();
-        }
     }
     TC_TRACE(20);
 }
 
-template <bool FUSE_ENV, bool ACT, bool DUELING, bool FIXED>
-__global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, TcArgs a, EnvFuse ef)
+template <bool ACT, bool DUELING, bool FIXED>
+__global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel_t(TcNet tc, TcArgs a)
 {
-    tc_forward_body<FUSE_ENV, ACT, DUELING, FIXED, false>(tc, a, ef);
+    tc_forward_body<ACT, DUELING, FIXED, false>(tc, a);
 }
 
 template <bool DUELING, bool FIXED>
-__global__ void __launch_bounds__(kTcThreads, 1) tc_loss_kernel_t(TcNet tc, TcArgs a, EnvFuse ef)
+__global__ void __launch_bounds__(kTcThreads, 1) tc_loss_kernel_t(TcNet tc, TcArgs a)
 {
-    tc_forward_body<false, true, DUELING, FIXED, true>(tc, a, ef);
+    tc_forward_body<true, DUELING, FIXED, true>(tc, a);
 }
 
 bool tc_fixed_chains(const TcNet &tc, bool train)
@@ -386,16 +375,14 @@ bool tc_fixed_chains(const TcNet &tc, bool train)
     return true;
 }
 
-typedef void (*ForwardKernel)(TcNet, TcArgs, EnvFuse);
-template <bool F, bool A, bool D>
-static ForwardKernel pick_fwd_x(bool fixed) { return fixed ? tc_forward_kernel_t<F, A, D, true> : tc_forward_kernel_t<F, A, D, false>; }
-template <bool F, bool A>
-static ForwardKernel pick_fwd_d(bool dueling, bool fixed) { return dueling ? pick_fwd_x<F, A, true>(fixed) : pick_fwd_x<F, A, false>(fixed); }
-// the fused act + env step variant exists for the act mode only
-static ForwardKernel pick_forward_kernel(bool fuse_env, bool act, bool dueling, bool fixed)
+typedef void (*ForwardKernel)(TcNet, TcArgs);
+template <bool A, bool D>
+static ForwardKernel pick_fwd_x(bool fixed) { return fixed ? tc_forward_kernel_t<A, D, true> : tc_forward_kernel_t<A, D, false>; }
+template <bool A>
+static ForwardKernel pick_fwd_d(bool dueling, bool fixed) { return dueling ? pick_fwd_x<A, true>(fixed) : pick_fwd_x<A, false>(fixed); }
+static ForwardKernel pick_forward_kernel(bool act, bool dueling, bool fixed)
 {
-    if (fuse_env) return pick_fwd_d<true, true>(dueling, fixed);
-    return act ? pick_fwd_d<false, true>(dueling, fixed) : pick_fwd_d<false, false>(dueling, fixed);
+    return act ? pick_fwd_d<true>(dueling, fixed) : pick_fwd_d<false>(dueling, fixed);
 }
 
 template <bool D>
@@ -408,7 +395,7 @@ int tc_forward_rows_per_tile(const TcNet &tc, int n)
     return (n >= 128 * n_sm && tc.max_rows == 128) ? 128 : (n >= 64 * n_sm) ? 64 : 32;
 }
 
-int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st, const EnvFuse *fuse)
+int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st)
 {
     TcArgs a = a_in;
     a.img_stride = l->tc.train_img_bytes;
@@ -431,16 +418,8 @@ int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st, con
             a.pdl |= kPdlEarlyWeights;                             // neither the env step nor a TD pass writes weight images
         }
     }
-    EnvFuse ef;
-    memset(&ef, 0, sizeof(ef));
-    if (fuse) {
-        ef = *fuse;
-        UAVRL_CUDA(launch_kernel(pick_forward_kernel(true, a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
-        l->pdl_prev = l->pdl_chain ? kPdlEnv : kPdlNone;
-    } else {
-        UAVRL_CUDA(launch_kernel(pick_forward_kernel(false, a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid, l->G), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a, ef));
-        l->pdl_prev = l->pdl_chain ? (a.mode == kTcAct ? kPdlAct : kPdlTd) : kPdlNone;
-    }
+    UAVRL_CUDA(launch_kernel(pick_forward_kernel(a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid, l->G), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a));
+    l->pdl_prev = l->pdl_chain ? (a.mode == kTcAct ? kPdlAct : kPdlTd) : kPdlNone;
     UAVRL_LAUNCHED();
     if (trace_on) {
         long long h[32];
@@ -463,10 +442,8 @@ int launch_tc_loss(uavrl_learner *l, const TcArgs &a_in, int n_weights, int max_
     const int tiles = (max_rows + step - 1) / step, n_sm = num_sms();
     a.n_tiles = tiles;
     a.pdl = 0;
-    EnvFuse ef;
-    memset(&ef, 0, sizeof(ef));
     UAVRL_CUDA(launch_kernel(pick_loss_kernel(l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(tiles < n_sm ? tiles : n_sm, n_weights),
-                             dim3(kTcThreads), tc_smem_bytes(l->tc), st, false, l->tc, a, ef));
+                             dim3(kTcThreads), tc_smem_bytes(l->tc), st, false, l->tc, a));
     l->pdl_prev = kPdlNone;
     UAVRL_LAUNCHED();
     return 0;
@@ -482,7 +459,7 @@ int tc_init(uavrl_learner *l)
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du) {
             cudaFuncAttributes fa;
-            UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_forward_kernel(false, ac != 0, du != 0, fixed)));
+            UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_forward_kernel(ac != 0, du != 0, fixed)));
             if (fa.sharedSizeBytes > fwd_static) fwd_static = fa.sharedSizeBytes;
         }
     if (tc_smem_bytes(l->tc) + fwd_static > 227 * 1024) return 0;
@@ -503,20 +480,9 @@ int tc_init(uavrl_learner *l)
     UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->G * l->cfg.batch_size * 4));
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du)
-            if (int rc = raise_dyn_smem(pick_forward_kernel(false, ac != 0, du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
+            if (int rc = raise_dyn_smem(pick_forward_kernel(ac != 0, du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
     for (int du = 0; du < 2; ++du)                               // the loss variant: the act kernel's static shared memory
         if (int rc = raise_dyn_smem(pick_loss_kernel(du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
-    {   // the fused act+step variant carries the env scratch as static shared memory on top: it must still fit one CTA
-        l->fuse_ok = true;
-        for (int du = 0; du < 2; ++du) {
-            cudaFuncAttributes fa;
-            UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_forward_kernel(true, true, du != 0, fixed)));
-            if (fa.sharedSizeBytes + tc_smem_bytes(l->tc) > (size_t)227 * 1024) l->fuse_ok = false;
-        }
-        if (l->fuse_ok)
-            for (int du = 0; du < 2; ++du)
-                if (int rc = raise_dyn_smem(pick_forward_kernel(true, true, du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
-    }
     l->y_cap = l->cfg.batch_size;
     l->tc_ok = true;
     return tc_train_init(l);

@@ -2,7 +2,6 @@
 #pragma once
 #include <vector>
 
-#include "env.cuh"
 #include "learner.cuh"
 
 namespace uavrl {
@@ -38,10 +37,8 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
              std::vector<int32_t> &hi2_map, std::vector<int32_t> &lo2_map);
 // tensor-core training path (tc_train.cu): forward + dX chain, then split-K dW; gradients land in l->partials
 int tc_train_init(uavrl_learner *l);
-// adam != nullptr: the optimiser step may be fused behind the weight-gradient kernel (*adam_done tells whether it was)
 int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, const float *y, int *n_grad_parts,
-                    int *n_loss_parts, cudaStream_t st, cudaEvent_t after_chain = nullptr, const AdamArgs *adam = nullptr,
-                    float *loss_out = nullptr, bool *adam_done = nullptr, bool fused_td = false);
+                    int *n_loss_parts, cudaStream_t st, cudaEvent_t after_chain = nullptr, bool fused_td = false);
 // the TD-target pass(es) can run inside the training kernel (one tile per CTA): no separate launch_tc_forward TD calls
 bool tc_train_can_fuse_td(const uavrl_learner *l, int B);
 // rows per tile of an act / TD pass over n samples (launch_tc_forward) and of the training kernel for a batch of B
@@ -51,9 +48,7 @@ size_t tc_smem_bytes(const TcNet &tc);
 // every layer product (train: also those of the dX chain) has a compile-time wgmma chain (wgmma.cuh mma_fixed): the kernels'
 // FIXED variants apply
 bool tc_fixed_chains(const TcNet &tc, bool train);
-// the env step fused behind the act pass (tc_forward.cu): env batch + where the step writes
-struct EnvFuse { EnvDev d; float *obs_next; float *reward; uint8_t *done; };
-int launch_tc_forward(uavrl_learner *l, const TcArgs &a, cudaStream_t st, const EnvFuse *fuse = nullptr);
+int launch_tc_forward(uavrl_learner *l, const TcArgs &a, cudaStream_t st);
 // the loss variant over n_weights weight sets (grid rows), max_rows = the most probe rows one of them evaluates
 int launch_tc_loss(uavrl_learner *l, const TcArgs &a, int n_weights, int max_rows, cudaStream_t st);
 int tc_init(uavrl_learner *l);        // builds the TC images/maps; leaves l->tc_ok = false when the net does not fit

@@ -13,8 +13,7 @@
 //                    row yields the bias gradient for free -- and stores its slice of partial `chunk`.
 //                    The contraction runs over SAMPLES while both operands are stored [sample][feature]: the rows are
 //                    transposed into K-major operands on their way into SMEM (wgmma reads tf32 K-major only).
-//                    Small batches (grid <= SMs): the same kernel then meets at a grid barrier and performs the partial reduction + Adam + image refresh itself (one launch less);
-//                    otherwise reduce_adam_kernel sums the B/128 partials.
+//                    reduce_adam_kernel then sums the partials.
 // All products use the hi*hi + hi*lo + lo*hi TF32 split (fp32-grade, see tc_forward.cu).
 #include <string.h>
 #include <stdlib.h>
@@ -57,13 +56,6 @@ struct TcDwArgs {
     const float *act_buf, *dz_buf;
     float *partials;                   // [n_slices][P]
     long long *trace;                  // debug (UAVRL_TC_TRACE): CTA (0, 0) / thread 0 stage timestamps
-    // fused optimiser tail (fuse_adam = 1, only when every CTA of the grid is resident at once): the partials travel as 8-byte
-    // words {epoch : value} (part64 [n_slices][P]); a reader polls the word itself -- no grid barrier, no fence, no flag
-    int32_t fuse_adam;
-    unsigned long long *part64;
-    uint32_t ll_epoch;                 // this launch's tag (never 0: the buffer starts zeroed)
-    AdamArgs adam;
-    AdamPtrs ptrs;
 };
 #define DW_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
 
@@ -518,7 +510,6 @@ __device__ __forceinline__ void dw_store_rows(const float4 (&v)[U], const float 
     }
 }
 
-template <bool FUSE_ADAM>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs a)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -619,13 +610,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     }
     __syncthreads();
     DW_TRACE(6);
-    // epilogue: row f = input feature (or the ones column), column o = output unit.
-    // Partial slice `chunk`: plain floats for the separate optimiser kernel, or 8-byte words {epoch : value} for the fused tail.
+    // epilogue: row f = input feature (or the ones column), column o = output unit, into partial slice `chunk`.
     // Lanes hold consecutive f, so every store instruction writes 32 consecutive elements of one weight row; the 32 columns of a
     // thread walk the rows with a pointer increment and a predicate each (the address arithmetic used to dominate this epilogue).
     float *part = a.partials + ((size_t)grp * a.n_slices + chunk) * a.P;
-    unsigned long long *part64 = FUSE_ADAM ? a.part64 + (size_t)chunk * a.P : nullptr;
-    const unsigned long long tag = (unsigned long long)a.ll_epoch << 32;
     const int f = quad * 32 + lane;
     for (int c0 = half * 32; c0 < T.N_pad; c0 += 64) {
         if (quad * 32 >= rowsA) break;
@@ -637,91 +625,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
         const int stride = brow ? 1 : T.K_real;
         const int i_main = brow ? T.b_off + c0 : T.w_off + f + c0 * T.K_real;
         const int i_val = brow ? T.b2_off + (c0 - T.out_main) : (T.w2_off >= 0 ? T.w2_off : 0) + f + (c0 - T.out_main) * T.K_real;
-        if (FUSE_ADAM) {
-            unsigned long long *p = part64 + i_main;
+        float *p = part + i_main;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+            if (j < n_main) *p = v[j];
+            p += stride;
+        }
+        if (n_all > n_main) {
+            float *q = part + i_val;
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
-                if (j < n_main) asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" :: "l"(p), "l"(tag | __float_as_uint(v[j])) : "memory");
-                p += stride;
-            }
-            if (n_all > n_main) {
-                unsigned long long *q = part64 + i_val;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    if (j >= n_main && j < n_all) asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" :: "l"(q), "l"(tag | __float_as_uint(v[j])) : "memory");
-                    q += stride;
-                }
-            }
-        } else {
-            float *p = part + i_main;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                if (j < n_main) *p = v[j];
-                p += stride;
-            }
-            if (n_all > n_main) {
-                float *q = part + i_val;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    if (j >= n_main && j < n_all) *q = v[j];
-                    q += stride;
-                }
+                if (j >= n_main && j < n_all) *q = v[j];
+                q += stride;
             }
         }
     }
     DW_TRACE(7);
-    if (!FUSE_ADAM) return;
-    // ---- fused optimiser tail: this CTA reduces its slice of the parameter vector over all partials in reduce_adam_kernel's
-    // order and applies Adam.  Every word it needs is polled until it carries this launch's epoch (all CTAs are resident: grid
-    // <= SMs, one CTA per SM, and each writes its partial before it polls) -- nothing to fence, no barrier to wait at.
-    const int per = (a.P + (int)gridDim.x - 1) / (int)gridDim.x;
-    const int i_end = min(a.P, ((int)blockIdx.x + 1) * per);
-    for (int i = (int)blockIdx.x * per + tid; i < i_end; i += kTcThreads) {
-        const unsigned long long *pp = a.part64 + i;
-        const uint32_t ep = a.ll_epoch;
-        auto poll = [ep](const unsigned long long *q) {
-            unsigned long long w;
-            asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(w) : "l"(q) : "memory");
-            return w;
-        };
-        float g4[4];
-#pragma unroll
-        for (int cg = 0; cg < 4; ++cg) {
-            float acc[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) acc[u] = 0.f;
-            int c = cg;
-            for (; c + 28 < a.adam.nparts; c += 32) {
-                unsigned long long w[8];
-                bool ok;
-                do {
-                    ok = true;
-#pragma unroll
-                    for (int u = 0; u < 8; ++u) w[u] = poll(pp + (size_t)(c + 4 * u) * a.P);
-#pragma unroll
-                    for (int u = 0; u < 8; ++u) ok = ok && (uint32_t)(w[u] >> 32) == ep;
-                } while (!ok);
-#pragma unroll
-                for (int u = 0; u < 8; ++u) acc[u] += __uint_as_float((uint32_t)w[u]);
-            }
-            for (; c < a.adam.nparts; c += 4) {
-                unsigned long long w;
-                do { w = poll(pp + (size_t)c * a.P); } while ((uint32_t)(w >> 32) != ep);
-                acc[0] += __uint_as_float((uint32_t)w);
-            }
-            g4[cg] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
-        }
-        const float g = (g4[0] + g4[1]) + (g4[2] + g4[3]);
-        a.ptrs.grad[i] = g;
-        adam_update_one(a.adam, a.ptrs, i, g);
-    }
-    if (blockIdx.x == 0 && warp == 7 && a.ptrs.loss_out) {          // loss = sum of the training kernel's per-CTA partials / B
-        float sl = 0.f;
-        for (int c = lane; c < a.adam.n_loss_parts; c += 32) sl += __ldcg(a.ptrs.loss_partials + c);
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) sl += __shfl_xor_sync(0xffffffffu, sl, off);
-        if (lane == 0) *a.ptrs.loss_out = sl * a.adam.inv_b;
-    }
 }
 
 typedef void (*TrainKernel)(TcNet, TcTrainArgs);
@@ -761,10 +680,10 @@ int tc_train_init(uavrl_learner *l)
             UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_train_kernel(np, du != 0, fixed)));
             if (fa.sharedSizeBytes > train_static) train_static = fa.sharedSizeBytes;
         }
-    for (int fu = 0; fu < 2; ++fu) {
+    {
         cudaFuncAttributes fa;
-        UAVRL_CUDA(cudaFuncGetAttributes(&fa, fu ? tc_dw_kernel<true> : tc_dw_kernel<false>));
-        if (fa.sharedSizeBytes > dw_static) dw_static = fa.sharedSizeBytes;
+        UAVRL_CUDA(cudaFuncGetAttributes(&fa, tc_dw_kernel));
+        dw_static = fa.sharedSizeBytes;
     }
     const size_t train_budget = (size_t)227 * 1024 - train_static;
     // the m64 MMA reads 8 row groups from each A buffer: with fewer real rows it runs into the next buffers,
@@ -775,8 +694,7 @@ int tc_train_init(uavrl_learner *l)
     for (int np = 0; np < 3; ++np)
         for (int du = 0; du < 2; ++du)
             if (int rc = raise_dyn_smem(pick_train_kernel(np, du != 0, fixed), train_smem_bytes(tc, tc.train_max_rows))) return rc;
-    if (int rc = raise_dyn_smem(tc_dw_kernel<false>, dw_smem_bytes(tc))) return rc;
-    if (int rc = raise_dyn_smem(tc_dw_kernel<true>, dw_smem_bytes(tc))) return rc;
+    if (int rc = raise_dyn_smem(tc_dw_kernel, dw_smem_bytes(tc))) return rc;
     const size_t cap = (size_t)l->cfg.batch_size, G = (size_t)l->G;
     UAVRL_CUDA(cudaMalloc((void **)&l->act_buf, G * cap * (size_t)(tc.act_stride > 0 ? tc.act_stride : 4) * 4));
     UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, G * cap * (size_t)tc.dz_stride * 4));
@@ -800,11 +718,8 @@ bool tc_train_can_fuse_td(const uavrl_learner *l, int B)
     const int R = train_rows_per_tile(l->tc, B);
     return (B + R - 1) / R <= num_sms();
 }
-std::atomic<int> g_fuse_dw_adam{0};          // uavrl_set_fuse_dw_adam(); default off: the PDL-chained pair already hides the optimiser's launch
-
 int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, const float *y, int *n_grad_parts,
-                    int *n_loss_parts, cudaStream_t st, cudaEvent_t after_chain, const AdamArgs *adam, float *loss_out, bool *adam_done,
-                    bool fused_td)
+                    int *n_loss_parts, cudaStream_t st, cudaEvent_t after_chain, bool fused_td)
 {
     const TcNet &tc = l->tc;
     TcTrainArgs a;
@@ -824,12 +739,8 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     if (trace_on) { UAVRL_CUDA(cudaMalloc((void **)&tr, 48 * sizeof(long long))); UAVRL_CUDA(cudaMemset(tr, 0, 48 * sizeof(long long))); a.trace = tr + 16; }
     const bool use_pdl = chain && (fused_td ? (l->pdl_prev == kPdlEnv) : (l->pdl_prev == kPdlTd));
     const int npre = fused_td ? (l->cfg.algo != UAVRL_ALGO_DQN ? 2 : 1) : 0;
-    auto train_fn = pick_train_kernel(npre, tc.dueling != 0, tc_fixed_chains(tc, true));
-    UAVRL_CUDA(launch_kernel(train_fn, dim3(grid, l->G), dim3(kTcThreads), train_smem_bytes(tc, a.R), st, use_pdl, tc, a));
-    // experiment (with UAVRL_TC_TRACE): the same launch again, back to back -- the kernel is idempotent, the second run finds
-    // its code in the instruction caches, and the stage trace printed below is the second run's
-    static const bool twice = trace_on && getenv("UAVRL_TRAIN_TWICE") != nullptr;
-    if (twice) UAVRL_CUDA(launch_kernel(train_fn, dim3(grid, l->G), dim3(kTcThreads), train_smem_bytes(tc, a.R), st, false, tc, a));
+    UAVRL_CUDA(launch_kernel(pick_train_kernel(npre, tc.dueling != 0, tc_fixed_chains(tc, true)), dim3(grid, l->G), dim3(kTcThreads),
+                             train_smem_bytes(tc, a.R), st, use_pdl, tc, a));
     l->pdl_prev = chain ? kPdlTrain : kPdlNone;
     UAVRL_LAUNCHED();
     if (after_chain) UAVRL_CUDA(cudaEventRecord(after_chain, st));
@@ -842,27 +753,9 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     const int max_slices = n_sm / tc.n_layers > 0 ? n_sm / tc.n_layers : 1;
     d.n_slices = d.n_chunks < max_slices ? d.n_chunks : max_slices;
     const int dw_grid = d.n_slices * tc.n_layers;
-    // Fused optimiser tail: the kernel's grid barrier needs every CTA resident at once -- one CTA per SM (193 KB of shared
-    // memory each), so only when the grid fits the SMs; larger batches keep the separate reduce_adam_kernel.
-    const bool fuse = adam != nullptr && g_fuse_dw_adam.load() && dw_grid <= n_sm && l->G == 1;
-    if (adam_done) *adam_done = fuse;
-    if (fuse) {
-        if (!l->dw_bar) {                                        // the {epoch : value} partial buffer [max_slices][P], zeroed once
-            const size_t n = (size_t)max_slices * (size_t)l->net.P * sizeof(unsigned long long);
-            UAVRL_CUDA(cudaMalloc((void **)&l->dw_bar, n));
-            UAVRL_CUDA(cudaMemsetAsync(l->dw_bar, 0, n, st));
-            l->dw_bar_total = 0;
-        }
-        l->dw_bar_total += 1;
-        if ((uint32_t)l->dw_bar_total == 0u) l->dw_bar_total += 1;     // tag 0 = "never written"
-        d.fuse_adam = 1; d.part64 = l->dw_bar; d.ll_epoch = (uint32_t)l->dw_bar_total;
-        d.adam = *adam; d.adam.nparts = d.n_slices; d.adam.n_loss_parts = grid;
-        d.ptrs = learner_adam_ptrs(l, loss_out);
-    }
     if (trace_on) d.trace = tr;
-    UAVRL_CUDA(launch_kernel(fuse ? tc_dw_kernel<true> : tc_dw_kernel<false>, dim3(dw_grid, l->G), dim3(kTcThreads), dw_smem_bytes(tc), st,
-                             chain && !after_chain, tc, d));
-    l->pdl_prev = chain ? (fuse ? kPdlAdam : kPdlDw) : kPdlNone;
+    UAVRL_CUDA(launch_kernel(tc_dw_kernel, dim3(dw_grid, l->G), dim3(kTcThreads), dw_smem_bytes(tc), st, chain && !after_chain, tc, d));
+    l->pdl_prev = chain ? kPdlDw : kPdlNone;
     UAVRL_LAUNCHED();
     if (trace_on) {
         long long h[48];
@@ -883,7 +776,11 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
 
 }  // namespace uavrl
 
-extern "C" int uavrl_set_fuse_dw_adam(int32_t on) { uavrl::g_fuse_dw_adam.store(on ? 1 : 0); return 0; }
+// kept for ABI compatibility: the optimiser step always runs as its own kernel
+extern "C" int uavrl_set_fuse_dw_adam(int32_t on)
+{
+    return on ? uavrl::fail(UAVRL_ERR_INVALID, "uavrl_set_fuse_dw_adam: the fused weight-gradient + optimiser variant was removed") : 0;
+}
 extern "C" int uavrl_set_fuse_td(int32_t on) { uavrl::g_fuse_td.store(on ? 1 : 0); return 0; }
 extern "C" int uavrl_learner_td_fused(const uavrl_learner *l, int32_t batch) { return (l && l->tc_ok && l->use_tc && uavrl::tc_train_can_fuse_td(l, batch)) ? 1 : 0; }
 // the same decisions launch_act / launch_update_impl take (uavrl.h)

@@ -12,6 +12,25 @@
 
 using namespace uavrl;
 
+// the start of every lockstep iteration: begin the ring's iteration (the very first one also materialises obs_0), then
+// Choose_Action2 -> Trainer.get_action (PathPlan_City.py:338-346) and Move_Agent + replay add (:371-382) -- reward/done land
+// in the ring slots -- and commit the frame
+static int act_step_commit(uavrl_env *env, uavrl_learner *l, float eps, cudaStream_t st)
+{
+    int rc;
+    const ReplayStore::Iteration io = l->replay.begin();
+    if (!l->replay.frame0_valid) {
+        if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc;
+        l->replay.frame0_valid = true;
+    }
+    if ((rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
+    if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
+                              l->pdl_prev == kPdlAct && g_pdl.load()))) return rc;
+    l->pdl_prev = kPdlEnv;
+    lockstep_commit(l, st);
+    return 0;
+}
+
 extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, int32_t updates_per_iter,
                                int32_t do_update, uavrl_train_stats *stats_host, void *stream)
 {
@@ -30,22 +49,7 @@ extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters
     l->pdl_chain = true; l->pdl_prev = kPdlNone;          // the first kernel of the loop is launched plainly
     struct ChainOff { uavrl_learner *l; ~ChainOff() { l->pdl_chain = false; l->pdl_prev = kPdlNone; } } chain_off{ l };
     for (int it = 0; it < n_iters; ++it) {
-        const ReplayStore::Iteration io = l->replay.begin();
-        if (!l->replay.frame0_valid) {                   // very first iteration: materialise obs_0
-            if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc;
-            l->replay.frame0_valid = true;
-        }
-        // Choose_Action2 -> Trainer.get_action (PathPlan_City.py:338-346), then Move_Agent + replay add (:371-382):
-        // reward/done land in the ring slots.  One fused kernel when the tensor-core path is on.
-        rc = launch_act_env(l, env->d, io.obs_t, eps, io.act, io.obs_next, io.rew, io.done, st);
-        if (rc < 0) return rc;
-        if (rc == 1) {
-            if ((rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
-            if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
-                                      l->pdl_prev == kPdlAct && g_pdl.load()))) return rc;
-            l->pdl_prev = kPdlEnv;
-        }
-        lockstep_commit(l, st);
+        if ((rc = act_step_commit(env, l, eps, st))) return rc;
         if (do_update) {
             for (int u = 0; u < updates_per_iter; ++u) {  // PathPlan_City.update -> Trainer.update (:757-776)
                 l->epoch += 1;
@@ -81,20 +85,7 @@ extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_it
     l->pdl_chain = true; l->pdl_prev = kPdlNone;
     struct ChainOff { uavrl_learner *l; ~ChainOff() { l->pdl_chain = false; l->pdl_prev = kPdlNone; } } chain_off{ l };
     for (int it = 0; it < n_iters; ++it) {
-        const ReplayStore::Iteration io = l->replay.begin();
-        if (!l->replay.frame0_valid) {
-            if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc;
-            l->replay.frame0_valid = true;
-        }
-        rc = launch_act_env(l, env->d, io.obs_t, eps, io.act, io.obs_next, io.rew, io.done, st);
-        if (rc < 0) return rc;
-        if (rc == 1) {
-            if ((rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
-            if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
-                                      l->pdl_prev == kPdlAct && g_pdl.load()))) return rc;
-            l->pdl_prev = kPdlEnv;
-        }
-        lockstep_commit(l, st);
+        if ((rc = act_step_commit(env, l, eps, st))) return rc;
         l->epoch += 1;
         // every rank must take part in every all-reduce: the caller warms the replay up first
         if (l->replay.count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions (warm up with uavrl_train_run first)");
@@ -119,12 +110,9 @@ extern "C" int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_i
         const ReplayStore::Iteration io = l->replay.begin();
         cudaEvent_t *e = &ev[(size_t)it * NE];
         UAVRL_CUDA(cudaEventRecord(e[0], st));
-        rc = launch_act_env(l, env->d, io.obs_t, eps, io.act, io.obs_next, io.rew, io.done, st);      // fused: slot 0 = act + step, slot 1 = 0
-        if (rc < 0) return rc;
-        const bool fused = (rc == 0);
-        if (!fused && (rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
+        if ((rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
         UAVRL_CUDA(cudaEventRecord(e[1], st));
-        if (!fused && (rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st))) return rc;
+        if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st))) return rc;
         UAVRL_CUDA(cudaEventRecord(e[2], st));
         lockstep_commit(l, st);
         l->epoch += 1;

@@ -443,24 +443,23 @@ class Learner:
         return _DevView(ptr, self.P, self.device).tensor()
 
     def connect_peers(self, dist, rank, world):
-        """Exchange the CUDA IPC handles of the symmetric gradient / flag buffers over torch.distributed and map
-        every peer's buffers (NVLink P2P) -- enables update_dp(), the fused one-shot all-reduce + Adam."""
-        hg = (C.c_ubyte * 64)(); hf = (C.c_ubyte * 64)()
-        check(_lib.lib().uavrl_learner_comm_init(self.h, rank, world, hg, hf))
-        mine = torch.tensor(list(bytes(hg)) + list(bytes(hf)), dtype=torch.uint8, device=self.device)
+        """Exchange the CUDA IPC handles of the symmetric gradient receive buffers over torch.distributed and map
+        every peer's buffer (NVLink P2P) -- enables update_dp(), the fused one-shot all-reduce + Adam."""
+        hg = (C.c_ubyte * 64)()
+        check(_lib.lib().uavrl_learner_comm_init(self.h, rank, world, hg, None))
+        mine = torch.tensor(list(bytes(hg)), dtype=torch.uint8, device=self.device)
         allh = [torch.zeros_like(mine) for _ in range(world)]
         dist.all_gather(allh, mine)
-        allh = torch.stack(allh).cpu().numpy()
-        g = np.ascontiguousarray(allh[:, :64]); f = np.ascontiguousarray(allh[:, 64:])
-        check(_lib.lib().uavrl_learner_comm_connect(self.h, _ptr(g), _ptr(f)))
+        g = np.ascontiguousarray(torch.stack(allh).cpu().numpy())
+        check(_lib.lib().uavrl_learner_comm_connect(self.h, _ptr(g), None))
         dist.barrier(device_ids=[self.device.index])
 
     def connect_self(self):
-        """world = 1: the data-parallel kernel pair (push into the local receive buffer, flag, all-reduce + Adam) on one GPU --
-        the self-test of the fused path that needs no second device."""
-        hg = (C.c_ubyte * 64)(); hf = (C.c_ubyte * 64)()
-        check(_lib.lib().uavrl_learner_comm_init(self.h, 0, 1, hg, hf))
-        check(_lib.lib().uavrl_learner_comm_connect(self.h, hg, hf))
+        """world = 1: the data-parallel optimiser kernel (push into the local receive buffer, gather, all-reduce + Adam) on
+        one GPU -- the self-test of the fused path that needs no second device."""
+        hg = (C.c_ubyte * 64)()
+        check(_lib.lib().uavrl_learner_comm_init(self.h, 0, 1, hg, None))
+        check(_lib.lib().uavrl_learner_comm_connect(self.h, hg, None))
 
     def update_dp(self, global_batch, idx_tape=None, loss=None):
         check(_lib.lib().uavrl_learner_update_dp(self.h, _ptr(idx_tape), int(global_batch), _ptr(loss), _stream(self.device)))

@@ -208,8 +208,7 @@ int64_t uavrl_learner_param_count(const uavrl_learner *l);
  *     apply_grads, uavrl_train_run_dp, and act / update_batch sizes that are not multiples of G;
  *   - prioritised replay is enabled with uavrl_per_enable_trainers (one tree per trainer, trainer-local slots and [G][...] arrays
  *     in every uavrl_per_* call; see the prioritised-replay block).  uavrl_per_enable keeps refusing G > 1 because the grouped
- *     form changes the slot numbering and array shapes of the other uavrl_per_* calls, so a caller opts in by name;
- *   - the process-wide fused act + step and fused weight-gradient + optimiser paths are not taken (the separate kernels run). */
+ *     form changes the slot numbering and array shapes of the other uavrl_per_* calls, so a caller opts in by name. */
 int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_trainers, uavrl_learner **out);
 int32_t uavrl_learner_trainer_count(const uavrl_learner *l);
 
@@ -298,15 +297,17 @@ int uavrl_learner_set_is_train(uavrl_learner *l, int32_t is_train);
 int uavrl_learner_lockstep_restart(uavrl_learner *l);
 
 /* One-shot NVLink all-reduce fused with the optimiser (data-parallel training, one process per GPU):
- *   uavrl_learner_comm_init     allocate this rank's symmetric receive buffer recv[2][world][P+1] + flag words, return their
- *                               CUDA IPC handles (64 bytes each) for exchange (e.g. torch.distributed.all_gather)
- *   uavrl_learner_comm_connect  open every rank's handles (grad_handles / flag_handles: [world][64] bytes)
- *   uavrl_learner_update_dp     epoch += 1; local gradient (loss scaled by 1/global_batch) -> reduced and PUSHED with remote
- *                               stores over NVLink into slot `rank` of every rank's receive buffer -> flags raised on every
- *                               peer -> the optimiser kernel waits for all ranks' flags in local memory, sums the `world`
- *                               vectors of its local receive buffer in rank order (bit-identical replicas) and applies Adam.
- *                               No NCCL call, nothing pulled across NVLink on the critical path.  world = 1 runs the same two
- *                               kernels on the local buffer (self-test on one GPU).
+ *   uavrl_learner_comm_init     allocate this rank's symmetric receive buffer recv[2][world][P+1] of 8-byte words, return its
+ *                               CUDA IPC handle (64 bytes) for exchange (e.g. torch.distributed.all_gather)
+ *   uavrl_learner_comm_connect  open every rank's handle (grad_handles: [world][64] bytes)
+ *   uavrl_learner_update_dp     epoch += 1; local gradient (loss scaled by 1/global_batch), then ONE optimiser kernel: each
+ *                               block reduces its slice of the gradient and PUSHES it with remote stores over NVLink into
+ *                               slot `rank` of every rank's receive buffer, every value as one word {exchange tag : value};
+ *                               it then polls its own receive buffer (local memory) until all `world` words of each of its
+ *                               parameters carry the current tag, sums them in rank order (bit-identical replicas) and
+ *                               applies Adam.  No NCCL call, no flag, no fence, nothing pulled across NVLink on the
+ *                               critical path.  world = 1 runs the same kernel on the local buffer (self-test on one GPU).
+ * flag_handle_out / flag_handles are unused (kept for ABI compatibility) and may be NULL.
  * loss_dev (optional) receives the GLOBAL batch loss. */
 int uavrl_learner_comm_init(uavrl_learner *l, int32_t rank, int32_t world, void *grad_handle_out, void *flag_handle_out);
 int uavrl_learner_comm_connect(uavrl_learner *l, const void *grad_handles, const void *flag_handles);
@@ -471,15 +472,11 @@ int64_t uavrl_launch_count(void);
 /* Programmatic dependent launch inside the lockstep loops (each kernel's prologue overlaps its predecessor's
  * tail; results are unchanged).  Process-wide switch, default 1; 0 launches every kernel fully serialised. */
 int uavrl_set_pdl(int32_t on);
-/* Lockstep loops on the tensor-core path: get_action and Move_Agent as one kernel (each CTA steps the envs whose
- * actions it has just computed; results unchanged).  Process-wide switch, default 0: the fused kernel steps the envs
- * with the few CTAs of the act pass, while the stand-alone env kernel spreads them over many small CTAs. */
+/* Kept for ABI compatibility; 0 only.  The lockstep loops launch get_action and Move_Agent as two kernels.  on = 0 returns 0;
+ * any other value returns UAVRL_ERR_INVALID (the fused variant was removed). */
 int uavrl_set_fuse_act_env(int32_t on);
-/* Small batches (weight-gradient grid <= number of SMs, one CTA per SM): the weight-gradient kernel writes its partials as 8-byte
- * words {epoch : value}, polls the words of the parameter slice it owns until every slice has delivered (no grid barrier, no fence)
- * and applies the partial reduction + Adam + weight-image refresh itself instead of a separate optimiser launch (results unchanged:
- * the reduction order is the optimiser kernel's).  Process-wide switch, default 0 (the PDL-chained
- * pair already hides the optimiser's launch latency). */
+/* Kept for ABI compatibility; 0 only.  The optimiser step runs as its own kernel behind the weight-gradient kernel.  on = 0
+ * returns 0; any other value returns UAVRL_ERR_INVALID (the fused variant was removed). */
 int uavrl_set_fuse_dw_adam(int32_t on);
 /* Batches of at most 132 x 32 transitions (132 x 64 on 64-row tiles when the operands fit shared memory) on the tensor-core path: the TD-target forward pass(es) (target network on the next
  * states; double DQN: the local network first) run inside the training kernel, each CTA on the tile it then trains on

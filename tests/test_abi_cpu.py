@@ -56,6 +56,10 @@ def test_argument_validation_without_gpu():
     cfg.n_envs, cfg.max_subgoals, cfg.n_buildings = 4, 8, 100     # > 64 cylinders is rejected up front
     h = C.c_void_p()
     assert L.uavrl_env_create(C.byref(cfg), C.byref(h)) == -1
+    # the two removed scheduling variants keep their setters for ABI compatibility: 0 is accepted, anything else refused
+    for setter in (L.uavrl_set_fuse_act_env, L.uavrl_set_fuse_dw_adam):
+        assert setter(0) == 0
+        assert setter(1) == -1 and b"removed" in L.uavrl_last_error()
 
 
 def test_host_scenario_generator(env_golden):

@@ -89,9 +89,10 @@ def test_two_rank_nccl_data_parallel(tmp_path):
 
 
 def test_fused_allreduce_pair_world1_equals_plain_update(dqn_golden):
-    """The data-parallel kernel pair on ONE GPU (world = 1): reduce + push into the local receive buffer + flag, then
-    flag wait + rank-ordered sum + Adam -- must equal the single-GPU update (same partials, same Adam arithmetic), through
-    hard updates and both parities of the double-buffered receive buffer; the loss is the batch loss."""
+    """The data-parallel optimiser kernel on ONE GPU (world = 1): reduce + push {tag : value} words into the local receive
+    buffer, then poll for the current tag + rank-ordered sum + Adam -- must equal the single-GPU update (same partials, same
+    Adam arithmetic), through hard updates and both parities of the double-buffered receive buffer; the loss is the batch
+    loss."""
     import numpy as np
     from uavrl_b200 import engine
     g = dqn_golden

@@ -76,8 +76,7 @@ def test_training_loop_learns_and_counts(env_golden, env27_golden):
 @pytest.mark.parametrize("algo", ["dqn", "ddqn"])
 def test_dependent_launch_overlap_changes_nothing(env_golden, env27_golden, algo):
     """Programmatic dependent launch inside the loop (kernel k+1's prologue overlaps kernel k's tail,
-    uavrl_set_pdl), the fused get_action + Move_Agent kernel (uavrl_set_fuse_act_env) and the optimiser step fused behind
-    the weight-gradient kernel's grid barrier (uavrl_set_fuse_dw_adam) are scheduling changes only:
+    uavrl_set_pdl) and the TD-target pass folded into the training kernel (uavrl_set_fuse_td) are scheduling changes only:
     150 lockstep iterations with every on/off combination end in bit-identical parameters, replay contents, env state
     and counters."""
     from uavrl_b200 import _lib, engine
@@ -85,12 +84,8 @@ def test_dependent_launch_overlap_changes_nothing(env_golden, env27_golden, algo
     N = 1024
     out = []
     try:
-        # the fused act+step kernel and the optimiser step fused behind the weight-gradient kernel are the same kind of change
-        # ... and so is the TD-target pass folded into the training kernel (uavrl_set_fuse_td)
-        for pdl, fuse, fuse_dw, fuse_td in ((1, 1, 1, 1), (0, 0, 0, 0), (1, 0, 1, 0), (0, 1, 1, 1), (1, 0, 0, 1), (1, 0, 0, 0)):
+        for pdl, fuse_td in ((1, 1), (0, 0), (1, 0), (0, 1)):
             _lib.lib().uavrl_set_pdl(pdl)
-            _lib.lib().uavrl_set_fuse_act_env(fuse)
-            _lib.lib().uavrl_set_fuse_dw_adam(fuse_dw)
             _lib.lib().uavrl_set_fuse_td(fuse_td)
             env = engine.EnvBatch(city, params, N, max_subgoals=64, auto_reset=True)
             sc = env.make_scenarios(1024, seed=8)
@@ -109,9 +104,7 @@ def test_dependent_launch_overlap_changes_nothing(env_golden, env27_golden, algo
                                    st.sum_reward, st.last_loss)))
             env.close(); L.close()
     finally:
-        _lib.lib().uavrl_set_pdl(1)                 # library defaults: PDL on, fused act+step off, optimiser not fused behind dW
-        _lib.lib().uavrl_set_fuse_act_env(0)
-        _lib.lib().uavrl_set_fuse_dw_adam(0)
+        _lib.lib().uavrl_set_pdl(1)                 # library defaults: PDL on, fused TD on
         _lib.lib().uavrl_set_fuse_td(1)
     a = out[0]
     for b in out[1:]:

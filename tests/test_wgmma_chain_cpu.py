@@ -10,10 +10,10 @@ import pytest
 
 from uavrl_b200 import _lib
 
-# (FUSE_ENV, ACT, DUELING, FIXED) / (NPRE, DUELING, FIXED): the variants the shipped networks run
+# (ACT, DUELING, FIXED) / (NPRE, DUELING, FIXED): the variants the shipped networks run
 KERNELS = [
-    "_ZN5uavrl19tc_forward_kernel_tILb0ELb1ELb0ELb1EEEvNS_5TcNetENS_6TcArgsENS_7EnvFuseE",
-    "_ZN5uavrl19tc_forward_kernel_tILb0ELb1ELb1ELb1EEEvNS_5TcNetENS_6TcArgsENS_7EnvFuseE",
+    "_ZN5uavrl19tc_forward_kernel_tILb1ELb0ELb1EEEvNS_5TcNetENS_6TcArgsE",
+    "_ZN5uavrl19tc_forward_kernel_tILb1ELb1ELb1EEEvNS_5TcNetENS_6TcArgsE",
     "_ZN5uavrl15tc_train_kernelILi1ELb0ELb1EEEvNS_5TcNetENS_11TcTrainArgsE",
     "_ZN5uavrl15tc_train_kernelILi2ELb0ELb1EEEvNS_5TcNetENS_11TcTrainArgsE",
     "_ZN5uavrl15tc_train_kernelILi2ELb1ELb1EEEvNS_5TcNetENS_11TcTrainArgsE",
