@@ -140,25 +140,13 @@ act_kernel_t(NetDev net, const float *__restrict__ params, const float *__restri
                 sA[threadIdx.x] = d2;                     // sA: free scratch once the forward is done
             }
             __syncthreads();
-            if (threadIdx.x * kFedProbes < kStep && e0 + (int)threadIdx.x * kFedProbes < n_rows) {
-                float s2 = 0.f;
-                for (int r = 0; r < kFedProbes; ++r) s2 += sA[threadIdx.x * kFedProbes + r];
-                const size_t p = (row0 + e0 + threadIdx.x * kFedProbes) / kFedProbes;
-                fl.loss_out[p * (size_t)(n / kFedProbes) + w_set] = s2 / (float)(kFedProbes * net.n_actions);
-            }
+            if (threadIdx.x * kFedProbes < kStep && e0 + (int)threadIdx.x * kFedProbes < n_rows)
+                fed_group_loss(sA + threadIdx.x * kFedProbes, row0 + e0 + threadIdx.x * kFedProbes, n, w_set, net.n_actions, fl.loss_out);
         } else if (threadIdx.x < kTile && e0 + threadIdx.x < n) {
             const int e = e0 + threadIdx.x;
             const float *row = head + threadIdx.x * 32;
-            float u; int ra;
-            if (u_tape) { u = u_tape[e]; ra = rand_tape ? rand_tape[e] : 0; }
-            else {
-                uint32_t r[4];
-                Philox::gen(key, call, (uint64_t)e, r);
-                u = Philox::u01(r[0]);
-                ra = (int)(((uint64_t)r[1] * (uint64_t)net.n_actions) >> 32);
-            }
-            // DuelingDQN_Trainer.py:89-97: sample > eps or not training -> greedy, else random
-            const int a = (u > eps || !is_train) ? argmax_row(row, net.n_actions) : ra;
+            int ra;
+            const int a = eps_greedy(eps, is_train, u_tape, rand_tape, e, key, call, e, net.n_actions, ra) ? argmax_row(row, net.n_actions) : ra;
             actions[e] = a;
             if (actions2) actions2[e] = a;
             if (q_out) for (int k = 0; k < net.n_actions; ++k) q_out[(size_t)e * net.n_actions + k] = row[k];
@@ -276,21 +264,11 @@ update_kernel(NetDev net, BatchSrc src, UpdateArgs ua)
                     float nq;
                     if (ua.algo == UAVRL_ALGO_DQN) nq = qt[argmax_row(qt, nA)];       // DQN_Trainer.py:109
                     else nq = qt[argmax_row(Ql2 + b * 32, nA)];                      // DDQN_Trainer.py:94-95
-                    y = s_rew[b] + (ua.gamma * nq * (1.f - s_done[b]));              // :99 / :114 / :171
+                    y = td_target(s_rew[b], ua.gamma, nq, s_done[b]);
                 }
                 const int a = s_act[b];
-                const float diff = Q[b * 32 + a] - y;
-                const float wb = src.is_w ? src.is_w[t * kTile + b] : 1.f;
-                if (src.abs_err) src.abs_err[t * kTile + b] = fabsf(diff);
                 float gq;
-                if (ua.loss_kind == 0) {                          // MSELoss (BaseTrainer.py:40)
-                    lossb = wb * (diff * diff);
-                    gq = (2.f * diff * wb) * ua.inv_global_b;
-                } else {                                          // SmoothL1Loss(beta = 1)
-                    const float ad = fabsf(diff);
-                    lossb = wb * (ad < 1.f ? 0.5f * (diff * diff) : ad - 0.5f);
-                    gq = (fminf(fmaxf(diff, -1.f), 1.f) * wb) * ua.inv_global_b;
-                }
+                lossb = td_loss(src, t * kTile + b, Q[b * 32 + a] - y, ua.loss_kind, ua.inv_global_b, gq);
                 if (net.dueling) {
                     const float inv = 1.f / (float)nA;
                     for (int o = 0; o < nA; ++o) g[o] = gq * ((o == a ? 1.f : 0.f) - inv);

@@ -60,6 +60,55 @@ struct TcNet {
     TcLayer L[kMaxLayers];
 };
 
+#if defined(__CUDACC__)
+// ---- Q-head arithmetic shared by the fp32 kernels (learner.cu) and the tensor-core kernels (tc_chain.cuh).  Device code is
+// compiled with FMA contraction on: each expression keeps its operand order, so both paths produce the same bits.
+
+// TD target y = r + gamma * next_q * (1 - d)  (DQN_Trainer.py:99 / :114, DuelingDQN_Trainer.py:171)
+__device__ __forceinline__ float td_target(float r, float gamma, float next_q, float d) { return r + (gamma * next_q * (1.f - d)); }
+
+// Per-sample loss term of diff = Q(s, a) - y with the importance weight of sample b (prioritised replay; 1 without), and
+// dLoss/dQ(s, a) into gq; writes |diff| for the priority update.  kind 0: MSELoss (BaseTrainer.py:40), 1: SmoothL1Loss(beta = 1)
+__device__ __forceinline__ float td_loss(const BatchSrc &src, int b, float diff, int kind, float inv_global_b, float &gq)
+{
+    const float wb = src.is_w ? src.is_w[b] : 1.f;
+    if (src.abs_err) src.abs_err[b] = fabsf(diff);
+    if (kind == 0) {
+        gq = (2.f * diff * wb) * inv_global_b;
+        return wb * (diff * diff);
+    }
+    const float ad = fabsf(diff);
+    gq = (fminf(fmaxf(diff, -1.f), 1.f) * wb) * inv_global_b;
+    return wb * (ad < 1.f ? 0.5f * (diff * diff) : ad - 0.5f);
+}
+
+// eps-greedy draw of row `row` (DuelingDQN_Trainer.py:89-97): true = take the greedy action, else the random action ra.  The
+// uniform and the random action come from the tapes at tape_row when given, else from Philox(key, call, row).
+__device__ __forceinline__ bool eps_greedy(float eps, int is_train, const float *u_tape, const int32_t *rand_tape, size_t tape_row,
+                                           uint64_t key, uint64_t call, int row, int n_actions, int &ra)
+{
+    float u;
+    if (u_tape) { u = u_tape[tape_row]; ra = rand_tape ? rand_tape[tape_row] : 0; }
+    else {
+        uint32_t r[4];
+        Philox::gen(key, call, (uint64_t)row, r);
+        u = Philox::u01(r[0]);
+        ra = (int)(((uint64_t)r[1] * (uint64_t)n_actions) >> 32);
+    }
+    return u > eps || !is_train;
+}
+
+// Federation: the loss entry of one probe group, M[p][w_set] = (sum of its kFedProbes rows' squared Q differences d2, in row
+// order) / (S A); first_row = the group's first row in the [G][S] probe rows.
+__device__ __forceinline__ void fed_group_loss(const float *d2, size_t first_row, int n, int w_set, int n_actions, float *loss_out)
+{
+    float s2 = 0.f;
+    for (int r = 0; r < kFedProbes; ++r) s2 += d2[r];
+    const size_t p = first_row / kFedProbes;
+    loss_out[p * (size_t)(n / kFedProbes) + w_set] = s2 / (float)(kFedProbes * n_actions);
+}
+#endif
+
 }  // namespace uavrl
 
 struct uavrl_learner {

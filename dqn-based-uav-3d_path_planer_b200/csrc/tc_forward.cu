@@ -10,14 +10,13 @@
 // split, fp32 grade, so results stay inside the parity tolerance of the fp32 path).
 // The accumulator is staged in a shared-memory tile; the epilogue adds the bias, applies ReLU, re-splits and writes
 // the next layer's A operand straight back into SMEM -- activations never touch HBM.  The head's epilogue
-// forms Q (dueling combine), then eps-greedy / argmax / max / gather depending on the mode.
-#include "tc_forward.cuh"
-
+// forms Q (dueling combine), then eps-greedy / argmax / max / gather depending on the mode.  The chain itself (gather,
+// epilogues, layer loop, head, staging) is tc_chain.cuh, shared with the training kernel's fused TD pass (tc_train.cu).
+#include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
 
-#include "tma.cuh"
-#include "wgmma.cuh"
+#include "tc_chain.cuh"
 
 namespace uavrl {
 
@@ -112,8 +111,6 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
 }
 
 
-#define TC_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
-
 // ACT (a.mode == kTcAct) and DUELING are compile-time: the kernel a pass runs carries no code of the other modes.
 // FIXED: every layer product is one unbroken compile-time wgmma chain (wgmma.cuh mma_fixed; tc_fixed_chains).
 // LOSS (with ACT, federation): grid row y evaluates weight set loss_w0 + y on a probe-row range (TcArgs::loss_*); a tile
@@ -122,7 +119,7 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
 template <bool ACT, bool DUELING, bool FIXED, bool LOSS>
 __device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a)
 {
-    TC_TRACE(0);
+    stage_trace(a.trace, 0);
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *Ahi = smem, *Alo = smem + tc.a_bytes, *W = smem + 2 * tc.a_bytes;
     float *acc = reinterpret_cast<float *>(W + tc.img_bytes);        // accumulator tile [tc.max_rows][tc.acc_ld]
@@ -151,20 +148,11 @@ __device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a
     // already gather the first tile; the CTA-wide barrier in front of the first weight wait publishes the barriers.
     constexpr int kCtl = kTcThreads - 32;
     const bool early_w = (a.pdl & kPdlEarlyWeights) != 0;
-    // The image travels in two pieces: layer 0's hi|lo block first (all the first MMA needs), the other layers and the biases
-    // behind it on a second barrier that is first waited for in layer 0's epilogue -- when the image can only be requested
-    // after the dependent-launch wait (act after the optimiser step) half of its latency is covered by the first layer.
-    const uint32_t w_split = tc.n_layers > 1 ? (uint32_t)tc.L[1].hi_off : (uint32_t)tc.img_bytes;
-    auto stage_image = [&]() {
-        fence_proxy_async();
-        bulk_g2s_chunked(W, img, w_split, &wbar);
-        if (w_split < (uint32_t)tc.img_bytes) bulk_g2s_chunked(W + w_split, img + w_split, (uint32_t)tc.img_bytes - w_split, &wbar2);
-    };
     if (tid == kCtl) {
         mbar_init(&wbar, 1); mbar_init(&wbar2, 1); fence_barrier_init();
-        if (early_w) stage_image();
+        if (early_w) stage_forward_image(tc, W, img, &wbar, &wbar2);
     }
-    TC_TRACE(1);
+    stage_trace(a.trace, 1);
     // PDL prologue (common.cuh): the weight image may be fetched before the wait when the predecessor does not write
     // it (TD passes after the env step); the first tile's rows may be gathered before the wait when the predecessor
     // does not write them (act after the optimiser kernel: observations were written two kernels back).
@@ -172,9 +160,8 @@ __device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a
     if (waited) {
         pdl_wait();
         pdl_trigger();
-        if (tid == kCtl && !early_w) stage_image();
+        if (tid == kCtl && !early_w) stage_forward_image(tc, W, img, &wbar, &wbar2);
     }
-    const float *bias_all = reinterpret_cast<const float *>(W + tc.bias_base);
 
     // act mode: row b of the tile is simply obs[base + b] -- no replay sampling (Philox), no pointer table, no barrier
     constexpr bool direct = ACT;
@@ -186,7 +173,10 @@ __device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a
     // R = real rows per tile (32 / 64 / 128, at most tc.max_rows).  A warpgroup's m64 MMA runs when its rows hold real
     // samples; accumulator rows >= R are computed from whatever SMEM follows the R-row operand (still inside this CTA's allocation) and never stored.
     // Small batches use R = 32 so that 4096 samples spread over 128 CTAs instead of 32.
-    const int R = a.rows_per_tile, lgR = 31 - __clz(R);
+    const int R = a.rows_per_tile;
+    const EpiSlice e(R, kTcThreads);
+    const int row = quad * 32 + lane;                            // the head epilogue's sample row (warps 0-3)
+    const bool live = quad * 32 < R;                             // this warp's rows are real rows
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int base = tile * tile_step;
         if (!direct) {
@@ -202,155 +192,75 @@ __device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a
             }
             __syncthreads();
         }
-        TC_TRACE(27);
-        // ---- A operand of layer 0: gathered rows -> TF32 hi/lo, canonical K-major layout (4 loads in flight per thread).
-        //      Item i = (chunk j = i / R, row r = i % R): consecutive lanes take consecutive rows of the same 16-byte chunk, so
-        //      a quarter-warp's 16-byte stores cover one whole core-matrix column = 128 contiguous bytes, and no division.
-        {
-            const int K0 = tc.L[0].K_pad, chunks = K0 / 4, total = R * chunks;
-            const uint32_t sbo = mma_sbo(K0);
-            for (int i0 = tid; i0 < total; i0 += 4 * kTcThreads) {
-                float4 v[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int i = i0 + u * kTcThreads;
-                    v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (i < total) {
-                        const int r = i & (R - 1), j = i >> lgR;
-                        const float *rp = direct ? ((base + r < n_rows && r < tile_step) ? a.obs + (r0 + base + r) * tc.in_dim : nullptr) : rows[r];
-                        if (rp && 4 * j < tc.in_dim) v[u] = __ldg(reinterpret_cast<const float4 *>(rp) + j);
-                    }
-                }
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int i = i0 + u * kTcThreads;
-                    if (i < total) {
-                        const int r = i & (R - 1), j = i >> lgR;
-                        float4 h, l;
-                        tf32_split(v[u].x, h.x, l.x); tf32_split(v[u].y, h.y, l.y); tf32_split(v[u].z, h.z, l.z); tf32_split(v[u].w, h.w, l.w);
-                        const uint32_t off = mma_off(r, 4 * j, sbo);
-                        *reinterpret_cast<float4 *>(Ahi + off) = h;
-                        *reinterpret_cast<float4 *>(Alo + off) = l;
-                    }
-                }
-            }
-        }
-        TC_TRACE(2);
+        stage_trace(a.trace, 27);
+        a0_gather([&](int r) -> const float * {
+            if (direct) return (base + r < n_rows && r < tile_step) ? a.obs + (r0 + base + r) * tc.in_dim : nullptr;
+            return rows[r];
+        }, R, tc.in_dim, tc.L[0].K_pad, Ahi, Alo);
+        stage_trace(a.trace, 2);
         if (!waited) {
             pdl_wait();
             pdl_trigger();
             waited = true;
-            if (tid == kCtl && !early_w) stage_image();
+            if (tid == kCtl && !early_w) stage_forward_image(tc, W, img, &wbar, &wbar2);
         }
         if (!wready) {                                           // first tile: the control thread's barriers become visible
             __syncthreads();
             mbar_wait(&wbar, 0);
             wready = true;
         }
-        TC_TRACE(3);
+        stage_trace(a.trace, 3);
         fence_proxy_async();
         __syncthreads();
-        TC_TRACE(4);
+        stage_trace(a.trace, 4);
 
-        for (int l = 0; l < tc.n_layers; ++l) {
-            const TcLayer T = tc.L[l];
-            mma_3xtf32<kMmaFwd, FIXED>(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
-            TC_TRACE(5 + 3 * l);
-            if (!w2ready) { if (w_split < (uint32_t)tc.img_bytes) mbar_wait(&wbar2, 0); w2ready = true; }   // biases + the next layers' weights
-            TC_TRACE(6 + 3 * l);
-            const float *bias = bias_all + T.bias_off;
-            const int row = quad * 32 + lane;
-            const bool live = quad * 32 < R;                       // this warp's rows are real rows
-            if (l + 1 < tc.n_layers) {
-                // hidden layer epilogue on every thread (EpiSlice): bias + ReLU, re-split, write the next A operand (K_next = N_pad)
-                const uint32_t sbon = mma_sbo(T.N_pad);
-                const EpiSlice e(R, kTcThreads);
-                for (int c = e.c0; c < T.N_pad; c += e.step) {
-                    const float4 v = e.ld(acc, tc.acc_ld, c);
-                    float4 h, lo4;
-                    const float x0 = fmaxf(v.x + bias[c + 0], 0.f), x1 = fmaxf(v.y + bias[c + 1], 0.f);
-                    const float x2 = fmaxf(v.z + bias[c + 2], 0.f), x3 = fmaxf(v.w + bias[c + 3], 0.f);
-                    tf32_split(x0, h.x, lo4.x); tf32_split(x1, h.y, lo4.y); tf32_split(x2, h.z, lo4.z); tf32_split(x3, h.w, lo4.w);
-                    const uint32_t off = mma_off(e.row, c, sbon);
-                    *reinterpret_cast<float4 *>(Ahi + off) = h;
-                    *reinterpret_cast<float4 *>(Alo + off) = lo4;
-                }
-                fence_proxy_async();
-                __syncthreads();
-                TC_TRACE(7 + 3 * l);
-            } else {
-                // head epilogue: Q row of this sample, then the mode's output
-                if (half == 0 && live) {
-                    float q[32];
-                    acc_ld32(acc, tc.acc_ld, row, 0, q);
-                    const int nA = tc.n_actions;
+        const auto mid = [&](int l) {
+            stage_trace(a.trace, 5 + 3 * l);
+            if (!w2ready) { if (fwd_image_split(tc) < (uint32_t)tc.img_bytes) mbar_wait(&wbar2, 0); w2ready = true; }
+            stage_trace(a.trace, 6 + 3 * l);
+        };
+        // head epilogue: Q row of this sample, then the mode's output
+        const auto head = [&](int, const float *bias) {
+            if (half == 0 && live) {
+                const int nA = tc.n_actions;
+                float q[32], bv;
+                q_row<DUELING>(acc, tc.acc_ld, row, bias, nA, q);
+                const int best = q_argmax(q, nA, bv);
+                const int b = base + row;                               // trainer-local row
+                const size_t ob = r0 + b;                               // its row in the [G][n] inputs / outputs
+                if (LOSS) {
+                    float d2 = 0.f;
+                    if (b < n_rows && row < tile_step) {
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) q[j] += bias[j];
-                    if (DUELING) {                                 // Q = V + A - mean(A)  (BaseCNN.py:138)
-                        float s = 0.f;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) if (j < nA) s += q[j];
-                        const float mean = s / (float)nA;
-                        float V = 0.f;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) if (j == nA) V = q[j];
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) q[j] = V + q[j] - mean;
+                        for (int j = 0; j < 32; ++j)
+                            if (j < nA) { const float d = a.q_ref[ob * nA + j] - q[j]; d2 += d * d; }
                     }
-                    int best = 0; float bv = q[0];
+                    s_rew[row] = d2;
+                } else if (b < a.n) {
+                    if (a.q_out) {
 #pragma unroll
-                    for (int j = 1; j < 32; ++j) if (j < nA && q[j] > bv) { bv = q[j]; best = j; }
-                    const int b = base + row;                               // trainer-local row
-                    const size_t ob = r0 + b;                               // its row in the [G][n] inputs / outputs
-                    if (LOSS) {
-                        float d2 = 0.f;
-                        if (b < n_rows && row < tile_step) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j)
-                                if (j < nA) { const float d = a.q_ref[ob * nA + j] - q[j]; d2 += d * d; }
-                        }
-                        s_rew[row] = d2;
-                    } else if (b < a.n) {
-                        if (a.q_out) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) if (j < nA) a.q_out[ob * nA + j] = q[j];
-                        }
-                        if (ACT) {
-                            float u; int ra;
-                            if (a.u_tape) { u = a.u_tape[ob]; ra = a.rand_tape ? a.rand_tape[ob] : 0; }
-                            else {
-                                uint32_t rr[4];
-                                Philox::gen(trainer_key(a.key, kActSalt, grp), a.call, (uint64_t)b, rr);
-                                u = Philox::u01(rr[0]);
-                                ra = (int)(((uint64_t)rr[1] * (uint64_t)nA) >> 32);
-                            }
-                            a.actions[ob] = (u > a.eps || !a.is_train) ? best : ra;     // DuelingDQN_Trainer.py:89-97
-                        } else if (!ACT && a.mode == kTcArgmax) {
-                            a.actions[ob] = best;                                       // DDQN_Trainer.py:94
-                        } else {
-                            float nq = bv;                                              // DQN_Trainer.py:109
-                            if (a.mode == kTcTdGather) {                                // DDQN_Trainer.py:95
-                                const int as = a.actions[ob];
-                                nq = 0.f;
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) if (j == as) nq = q[j];
-                            }
-                            a.y_out[ob] = s_rew[row] + (a.gamma * nq * (1.f - s_done[row]));  // :99 / :114 / :171
-                        }
+                        for (int j = 0; j < 32; ++j) if (j < nA) a.q_out[ob * nA + j] = q[j];
                     }
-                }
-                __syncthreads();
-                if (LOSS && tid * kFedProbes < tile_step && base + tid * kFedProbes < n_rows) {
-                    // one probe group (trainer p's rows) per thread: its rows' squared differences in row order
-                    float s2 = 0.f;
-                    for (int r = 0; r < kFedProbes; ++r) s2 += s_rew[tid * kFedProbes + r];
-                    const size_t p = (r0 + base + tid * kFedProbes) / kFedProbes;
-                    a.loss_out[p * (size_t)(a.n / kFedProbes) + w_set] = s2 / (float)(kFedProbes * tc.n_actions);
+                    if (ACT) {
+                        int ra;
+                        const bool greedy = eps_greedy(a.eps, a.is_train, a.u_tape, a.rand_tape, ob, trainer_key(a.key, kActSalt, grp), a.call, b, nA, ra);
+                        a.actions[ob] = greedy ? best : ra;
+                    } else if (!ACT && a.mode == kTcArgmax) {
+                        a.actions[ob] = best;                                       // DDQN_Trainer.py:94
+                    } else {                                                        // DQN_Trainer.py:109; DDQN_Trainer.py:95
+                        const float nq = a.mode == kTcTdGather ? q_at(q, a.actions[ob]) : bv;
+                        a.y_out[ob] = td_target(s_rew[row], a.gamma, nq, s_done[row]);
+                    }
                 }
             }
-        }
+            __syncthreads();
+            if (LOSS && tid * kFedProbes < tile_step && base + tid * kFedProbes < n_rows)   // one probe group per thread
+                fed_group_loss(s_rew + tid * kFedProbes, r0 + base + tid * kFedProbes, a.n, w_set, tc.n_actions, a.loss_out);
+        };
+        forward_layers<FIXED, false>(tc, R, e, Ahi, Alo, W, acc, nullptr, false, mid, head,
+                                     [&](int l, uint32_t) { stage_trace(a.trace, 7 + 3 * l); });
     }
-    TC_TRACE(20);
+    stage_trace(a.trace, 20);
 }
 
 template <bool ACT, bool DUELING, bool FIXED>
@@ -389,6 +299,34 @@ template <bool D>
 static ForwardKernel pick_loss_d(bool fixed) { return fixed ? tc_loss_kernel_t<D, true> : tc_loss_kernel_t<D, false>; }
 static ForwardKernel pick_loss_kernel(bool dueling, bool fixed) { return dueling ? pick_loss_d<true>(fixed) : pick_loss_d<false>(fixed); }
 
+int stage_trace_alloc(long long **t)
+{
+    static const bool on = getenv("UAVRL_TC_TRACE") != nullptr;
+    *t = nullptr;
+    if (!on) return 0;
+    UAVRL_CUDA(cudaMalloc((void **)t, kTraceSlots * sizeof(long long)));
+    UAVRL_CUDA(cudaMemset(*t, 0, kTraceSlots * sizeof(long long)));
+    return 0;
+}
+
+int stage_trace_print(cudaStream_t st, long long *t, const char *fmt, ...)
+{
+    if (!t) return 0;
+    long long h[kTraceSlots];
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = cudaMemcpy(h, t, sizeof(h), cudaMemcpyDeviceToHost);
+    cudaFree(t);
+    UAVRL_CUDA(e);
+    va_list ap;
+    va_start(ap, fmt);
+    vfprintf(stderr, fmt, ap);
+    va_end(ap);
+    fprintf(stderr, " cycles since start:");
+    for (int i = 1; i < kTraceSlots; ++i) if (h[i]) fprintf(stderr, " [%d]=%lld", i, h[i] - h[0]);
+    fprintf(stderr, "\n");
+    return 0;
+}
+
 int tc_forward_rows_per_tile(const TcNet &tc, int n)
 {
     const int n_sm = num_sms();
@@ -403,9 +341,7 @@ int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st)
     a.rows_per_tile = tc_forward_rows_per_tile(l->tc, a.n);
     a.n_tiles = (a.n + a.rows_per_tile - 1) / a.rows_per_tile;
     const int grid = a.n_tiles < n_sm ? a.n_tiles : n_sm;
-    static const bool trace_on = getenv("UAVRL_TC_TRACE") != nullptr;
-    long long *tr = nullptr;
-    if (trace_on) { UAVRL_CUDA(cudaMalloc((void **)&tr, 32 * sizeof(long long))); UAVRL_CUDA(cudaMemset(tr, 0, 32 * sizeof(long long))); a.trace = tr; }
+    if (int rc = stage_trace_alloc(&a.trace)) return rc;
     // PDL chain state (see common.cuh): what this kernel may touch before its griddepcontrol.wait
     const int prev = (l->pdl_chain && g_pdl.load()) ? l->pdl_prev : kPdlNone;
     a.pdl = 0;
@@ -421,16 +357,7 @@ int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st)
     UAVRL_CUDA(launch_kernel(pick_forward_kernel(a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid, l->G), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a));
     l->pdl_prev = l->pdl_chain ? (a.mode == kTcAct ? kPdlAct : kPdlTd) : kPdlNone;
     UAVRL_LAUNCHED();
-    if (trace_on) {
-        long long h[32];
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        UAVRL_CUDA(cudaMemcpy(h, tr, sizeof(h), cudaMemcpyDeviceToHost));
-        cudaFree(tr);
-        fprintf(stderr, "[tc_trace] mode=%d n=%d R=%d grid=%d cycles since start:", a.mode, a.n, a.rows_per_tile, grid);
-        for (int i = 1; i < 32; ++i) if (h[i]) fprintf(stderr, " [%d]=%lld", i, h[i] - h[0]);
-        fprintf(stderr, "\n");
-    }
-    return 0;
+    return stage_trace_print(st, a.trace, "[tc_trace] mode=%d n=%d R=%d grid=%d", a.mode, a.n, a.rows_per_tile, grid);
 }
 
 int launch_tc_loss(uavrl_learner *l, const TcArgs &a_in, int n_weights, int max_rows, cudaStream_t st)

@@ -3,7 +3,7 @@
 // Replaces the arithmetic of Trainer.update (Trainer/DuelingDQN_Trainer.py:164-180, DDQN_Trainer.py:93-107,
 // DQN_Trainer.py:107-126): Q(s).gather(a), MSE against the TD target, loss.backward().
 //
-//   tc_train_kernel  one CTA = R (32/64) sampled transitions.  Forward chain exactly like tc_forward.cu, then the
+//   tc_train_kernel  one CTA = R (32/64) sampled transitions.  The forward chain (tc_chain.cuh), then the
 //                    loss / dLoss/dQ in the head epilogue, then the dX chain with the TRANSPOSED weight blocks of the
 //                    training image:  dH_l = dZ_{l+1} * W_{l+1}  (A = dZ rows, B = W^T K-major), ReLU mask applied
 //                    in the epilogue.  Hidden activations and every dZ are written once to a per-sample scratch
@@ -20,9 +20,7 @@
 
 #include <atomic>
 
-#include "tc_forward.cuh"
-#include "tma.cuh"
-#include "wgmma.cuh"
+#include "tc_chain.cuh"
 
 namespace uavrl {
 
@@ -47,7 +45,6 @@ struct TcTrainArgs {
                                        // and the batch are [G][B], the loss partials [G][gridDim.x]
     long long *trace;                  // debug (UAVRL_TC_TRACE): CTA (0, 0) / thread 0 stage timestamps
 };
-#define TR_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
 
 struct TcDwArgs {
     BatchSrc src;
@@ -57,91 +54,6 @@ struct TcDwArgs {
     float *partials;                   // [n_slices][P]
     long long *trace;                  // debug (UAVRL_TC_TRACE): CTA (0, 0) / thread 0 stage timestamps
 };
-#define DW_TRACE(slot) do { if (a.trace && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) a.trace[slot] = clock64(); } while (0)
-
-// Gather R rows (pointers in rows[]) into the layer-0 A operand.  All of a thread's loads are issued before any
-// is consumed (4 in flight), so the gather costs one L2 round trip instead of one per chunk.  Item i = (chunk j = i / R,
-// row r = i % R; R is a power of two): consecutive lanes take consecutive rows of the same 16-byte chunk, so a quarter-warp's
-// 16-byte stores cover one whole core matrix column = 128 contiguous bytes (lanes walking along a row would all hit the
-// same 4 banks) and the index needs no division.
-__device__ __forceinline__ void build_a0(const float *const *rows, int R, int in_dim, int K0, unsigned char *Ahi, unsigned char *Alo)
-{
-    const int chunks = K0 / 4, total = R * chunks, lgR = 31 - __clz(R);
-    const uint32_t sbo = mma_sbo(K0);
-    for (int i0 = threadIdx.x; i0 < total; i0 += 4 * kTcThreads) {
-        float4 v[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const int i = i0 + u * kTcThreads;
-            v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (i < total) {
-                const int r = i & (R - 1), j = i >> lgR;
-                if (rows[r] && 4 * j < in_dim) v[u] = __ldg(reinterpret_cast<const float4 *>(rows[r]) + j);
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const int i = i0 + u * kTcThreads;
-            if (i < total) {
-                const int r = i & (R - 1), j = i >> lgR;
-                float4 h, l;
-                tf32_split(v[u].x, h.x, l.x); tf32_split(v[u].y, h.y, l.y); tf32_split(v[u].z, h.z, l.z); tf32_split(v[u].w, h.w, l.w);
-                const uint32_t off = mma_off(r, 4 * j, sbo);
-                *reinterpret_cast<float4 *>(Ahi + off) = h;
-                *reinterpret_cast<float4 *>(Alo + off) = l;
-            }
-        }
-    }
-}
-
-// The same gather in two halves for a tile of at most 4 * kTcThreads items (R = 32: 832): the loads are issued long before the
-// operand buffer is free (the fused TD pre-pass runs in between), so the HBM latency of the sampled rows is off the chain.
-__device__ __forceinline__ void a0_load(const float *const *rows, int R, int in_dim, int K0, float4 (&v)[4])
-{
-    const int total = R * (K0 / 4), lgR = 31 - __clz(R);
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-        const int i = threadIdx.x + u * kTcThreads;
-        const int r = i & (R - 1), j = i >> lgR;
-        const float *rp = (i < total) ? rows[r] : nullptr;
-        v[u] = (rp && 4 * j < in_dim) ? __ldg(reinterpret_cast<const float4 *>(rp) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-}
-// want_fresh = false: every row NOT flagged in fresh[] (everything else zero) -- may run before the dependent-launch wait;
-// want_fresh = true: only the flagged rows, read from L2 (the env step of this iteration has just written them), into the
-// same registers.
-__device__ __forceinline__ void a0_load_sel(const float *const *rows, const uint8_t *fresh, bool want_fresh, int R, int in_dim, int K0, float4 (&v)[4])
-{
-    const int total = R * (K0 / 4), lgR = 31 - __clz(R);
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-        const int i = threadIdx.x + u * kTcThreads;
-        const int r = i & (R - 1), j = i >> lgR;
-        const float *rp = (i < total) ? rows[r] : nullptr;
-        const bool take = rp && 4 * j < in_dim && ((fresh[r] != 0) == want_fresh);
-        if (!want_fresh) v[u] = take ? __ldg(reinterpret_cast<const float4 *>(rp) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-        else if (take) v[u] = __ldcg(reinterpret_cast<const float4 *>(rp) + j);
-    }
-}
-__device__ __forceinline__ void a0_store(const float4 (&v)[4], int R, int K0, unsigned char *Ahi, unsigned char *Alo)
-{
-    const int total = R * (K0 / 4), lgR = 31 - __clz(R);
-    const uint32_t sbo = mma_sbo(K0);
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-        const int i = threadIdx.x + u * kTcThreads;
-        if (i < total) {
-            const int r = i & (R - 1), j = i >> lgR;
-            float4 h, l;
-            tf32_split(v[u].x, h.x, l.x); tf32_split(v[u].y, h.y, l.y); tf32_split(v[u].z, h.z, l.z); tf32_split(v[u].w, h.w, l.w);
-            const uint32_t off = mma_off(r, 4 * j, sbo);
-            *reinterpret_cast<float4 *>(Ahi + off) = h;
-            *reinterpret_cast<float4 *>(Alo + off) = l;
-        }
-    }
-}
-
-__device__ __forceinline__ uint32_t nl_split(const TcNet &tc) { return tc.n_layers > 1 ? (uint32_t)tc.L[1].hi_off : (uint32_t)tc.img_bytes; }
 
 // NPRE / DUELING are compile-time so that the kernel a configuration runs carries no code of the others: a third of the
 // live warps' stall samples of the generic kernel were instruction-fetch stalls (143 KB of code, executed once per CTA).
@@ -150,7 +62,7 @@ __device__ __forceinline__ uint32_t nl_split(const TcNet &tc) { return tc.n_laye
 template <int NPRE, bool DUELING, bool FIXED>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTrainArgs a)
 {
-    TR_TRACE(0);
+    stage_trace(a.trace, 0);
     extern __shared__ __align__(1024) unsigned char smem[];
     const int R = a.R;
     const uint32_t a_bytes = (uint32_t)(R / 8) * mma_sbo(tc.max_k);
@@ -174,7 +86,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
     float *act_buf = a.act_buf + r0 * tc.act_stride, *dz_buf = a.dz_buf + r0 * tc.dz_stride;
     const float *y_in = a.y ? a.y + r0 : nullptr;
     // control thread (first of the last warp): barrier init and weight copies -- concurrently with warp 0 resolving the tile's
-    // samples; the first CTA-wide barrier (behind the sample table) publishes the barriers (tc_forward.cu)
+    // samples; the first CTA-wide barrier (behind the sample table) publishes the barriers
     constexpr int kCtl = kTcThreads - 32;
     if (tid == 0) s_loss = 0.f;
     constexpr bool fused = NPRE > 0;
@@ -197,12 +109,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
                 bulk_g2s_chunked(W + tc.img_bytes, img + tc.img_bytes, (uint32_t)(tc.train_img_bytes - tc.img_bytes), &wbar3);
         }
     }
-    // fused: after the TD passes the forward part of the training image comes in two pieces -- layer 0's block on wbar (all the
-    // first MMA needs), the other layers + biases on wbar2 (first waited for in layer 0's epilogue)
-    const uint32_t w_split = nl_split(tc);
-    TR_TRACE(1);
+    stage_trace(a.trace, 1);
     bool waited = false;
-    const float *bias_all = reinterpret_cast<const float *>(W + tc.bias_base);
 
     uint32_t pkey[4];
     Philox::gen(src.key, src.epoch, 0x5A17ull, pkey);
@@ -215,6 +123,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
     // ReLU' for the dX chain: bit 4i + j of hmK = (H_K[e.row][e.c0 + i * e.step + j] > 0), kept from the forward epilogue of the
     // same thread (hidden layers are at most 64 wide and R <= 64 here: at most 16 elements per thread) -- no reload of H
     uint32_t hm1 = 0u, hm2 = 0u, hm3 = 0u, hm4 = 0u;
+    const auto table = [](const float *const *t) { return [t](int r) { return t[r]; }; };
 
     for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
         const int base = tile * R;
@@ -239,86 +148,47 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         float4 vmain[4], vnext[4];
         if (early_rows) {
             a0_load_sel(rows2, s_fresh, false, R, tc.in_dim, tc.L[0].K_pad, vnext);
-            a0_load(rows, R, tc.in_dim, tc.L[0].K_pad, vmain);
+            a0_load(table(rows), tid, R, tc.in_dim, tc.L[0].K_pad, vmain);
         }
         if (fused && !waited) { pdl_wait(); pdl_trigger(); waited = true; }
         int m_act = 0; float m_rew = 0.f, m_done = 0.f;
         if (my_slot >= 0) load_meta(src, my_slot, m_act, m_rew, m_done);
         if (early_rows) a0_load_sel(rows2, s_fresh, true, R, tc.in_dim, tc.L[0].K_pad, vnext);
         auto park_meta = [&]() { if (tid < R) { s_act[tid] = m_act; if (fused) { s_rew[tid] = m_rew; s_done[tid] = m_done; } } };
-        TR_TRACE(2);
-        // ---------------- fused TD target: forward-only pass(es) on the next states (tc_forward.cu's chain and head)
+        stage_trace(a.trace, 2);
+        // ---------------- fused TD target: forward-only pass(es) on the next states
         for (int pass = 0; pass < n_pre; ++pass) {
-            if (pass > 0 && tid == kTcThreads - 32) {                          // the target image replaces the local one (all its readers are done)
+            if (pass > 0 && tid == kCtl) {                                     // the target image replaces the local one (all its readers are done)
                 fence_proxy_async();
                 bulk_g2s_chunked(W, img_t, (uint32_t)tc.img_bytes, &wbar);
             }
-            if (pass == 0 && early_rows) a0_store(vnext, R, tc.L[0].K_pad, Ahi, Alo);
-            else build_a0(rows2, R, tc.in_dim, tc.L[0].K_pad, Ahi, Alo);
-            if (pass == 0) { park_meta(); TR_TRACE(3); }
+            if (pass == 0 && early_rows) a0_store(vnext, tid, R, tc.L[0].K_pad, Ahi, Alo);
+            else a0_gather(table(rows2), R, tc.in_dim, tc.L[0].K_pad, Ahi, Alo);
+            if (pass == 0) { park_meta(); stage_trace(a.trace, 3); }
             mbar_wait(&wbar, wphase); wphase ^= 1;
             fence_proxy_async();
             __syncthreads();
-            if (pass == 0) TR_TRACE(4);
+            if (pass == 0) stage_trace(a.trace, 4);
             const bool td_pass = (pass == n_pre - 1);
-            for (int l = 0; l < nl; ++l) {
-                const TcLayer T = tc.L[l];
-                mma_3xtf32<kMmaFwd, FIXED>(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
-                const float *bias = bias_all + T.bias_off;
-                if (l + 1 < nl) {
-                    const uint32_t sbon = mma_sbo(T.N_pad);
-                    for (int c = e.c0; c < T.N_pad; c += e.step) {
-                        const float4 v = e.ld(acc, tc.acc_ld, c);
-                        float4 x, h, lo4;
-                        x.x = fmaxf(v.x + bias[c + 0], 0.f); x.y = fmaxf(v.y + bias[c + 1], 0.f);
-                        x.z = fmaxf(v.z + bias[c + 2], 0.f); x.w = fmaxf(v.w + bias[c + 3], 0.f);
-                        tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
-                        const uint32_t off = mma_off(e.row, c, sbon);
-                        *reinterpret_cast<float4 *>(Ahi + off) = h;
-                        *reinterpret_cast<float4 *>(Alo + off) = lo4;
-                    }
-                } else if (half == 0 && live) {
-                    float q[32];
-                    acc_ld32(acc, tc.acc_ld, row, 0, q);
-                    const int nA = tc.n_actions;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) q[j] += bias[j];
-                    if (DUELING) {                                 // Q = V + A - mean(A)  (BaseCNN.py:138)
-                        float sA = 0.f, V = 0.f;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) { if (j < nA) sA += q[j]; if (j == nA) V = q[j]; }
-                        const float mean = sA / (float)nA;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) q[j] = V + q[j] - mean;
-                    }
-                    int best = 0; float bv = q[0];
-#pragma unroll
-                    for (int j = 1; j < 32; ++j) if (j < nA && q[j] > bv) { bv = q[j]; best = j; }
-                    if (!td_pass) s_astar[row] = best;                // DDQN_Trainer.py:94
-                    else {
-                        float nq = bv;                                // DQN_Trainer.py:109
-                        if (n_pre == 2) {                             // DDQN_Trainer.py:95: gather at a*
-                            const int as = s_astar[row];
-                            nq = 0.f;
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) if (j == as) nq = q[j];
-                        }
-                        s_y[row] = s_rew[row] + (a.gamma * nq * (1.f - s_done[row]));      // :99 / :114 / :171
-                    }
+            const auto head = [&](int l, const float *bias) {
+                if (half == 0 && live) {
+                    float q[32], bv;
+                    q_row<DUELING>(acc, tc.acc_ld, row, bias, tc.n_actions, q);
+                    const int best = q_argmax(q, tc.n_actions, bv);
+                    if (!td_pass) s_astar[row] = best;                                  // DDQN_Trainer.py:94
+                    else s_y[row] = td_target(s_rew[row], a.gamma, n_pre == 2 ? q_at(q, s_astar[row]) : bv, s_done[row]);  // DDQN_Trainer.py:95
                 }
                 fence_proxy_async();
                 __syncthreads();
-                if (pass == 0) TR_TRACE(5 + l);
-            }
+                if (pass == 0) stage_trace(a.trace, 5 + l);
+            };
+            forward_layers<FIXED, false>(tc, R, e, Ahi, Alo, W, acc, nullptr, false, [](int) {}, head,
+                                         [&](int l, uint32_t) { if (pass == 0) stage_trace(a.trace, 5 + l); });
         }
-        if (fused && tid == kTcThreads - 32) {                                  // the training image (every reader of the TD image is done)
-            fence_proxy_async();
-            bulk_g2s_chunked(W, img, w_split, &wbar);
-            if (w_split < (uint32_t)tc.img_bytes) bulk_g2s_chunked(W + w_split, img + w_split, (uint32_t)tc.img_bytes - w_split, &wbar2);
-        }
-        if (early_rows) a0_store(vmain, R, tc.L[0].K_pad, Ahi, Alo);
-        else build_a0(rows, R, tc.in_dim, tc.L[0].K_pad, Ahi, Alo);
-        TR_TRACE(9);
+        if (fused && tid == kCtl) stage_forward_image(tc, W, img, &wbar, &wbar2);     // the training image (every reader of the TD image is done)
+        if (early_rows) a0_store(vmain, tid, R, tc.L[0].K_pad, Ahi, Alo);
+        else a0_gather(table(rows), R, tc.in_dim, tc.L[0].K_pad, Ahi, Alo);
+        stage_trace(a.trace, 9);
         if (!waited) { pdl_wait(); pdl_trigger(); waited = true; }
         if (n_pre == 0) park_meta();
         if (!fused && tid < R) s_y[tid] = (base + tid < a.B) ? y_in[base + tid] : 0.f;      // visible after the barrier below
@@ -326,108 +196,70 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         else if (!wready) { mbar_wait(&wbar, 0); wready = true; }
         fence_proxy_async();
         __syncthreads();
-        TR_TRACE(10);
+        stage_trace(a.trace, 10);
         const int gb = base + row;                          // this thread's sample in the head epilogue (valid when live && gb < B)
         const bool mine = live && gb < a.B;
         const int egb = base + e.row;                       // ... and in the hidden-layer / dX epilogues
         const bool emine = egb < a.B;
 
-        // ---------------- forward chain
-        for (int l = 0; l < nl; ++l) {
-            const TcLayer T = tc.L[l];
-            mma_3xtf32<kMmaFwd, FIXED>(acc, tc.acc_ld, Ahi, Alo, W + T.hi_off, W + T.lo_off, mma_sbo(T.K_pad), T.N_pad, T.K_pad / 8, R);
-            if (fused && l == 0 && w_split < (uint32_t)tc.img_bytes) mbar_wait(&wbar2, 0);     // biases + the later layers' weights
-            if (l < 4) TR_TRACE(27 + l);
-            const float *bias = bias_all + T.bias_off;
-            if (l + 1 < nl) {
+        // ---------------- forward chain: activations kept for dW, ReLU masks for the dX chain
+        const auto mid = [&](int l) {
+            if (fused && l == 0 && fwd_image_split(tc) < (uint32_t)tc.img_bytes) mbar_wait(&wbar2, 0);     // biases + the later layers' weights
+            if (l < 4) stage_trace(a.trace, 27 + l);
+        };
+        // head: Q(s, .), loss, dLoss/dHead -> next A operand (K = 32) and the dz scratch
+        const auto head = [&](int l, const float *bias) {
+            const TcLayer &T = tc.L[l];
+            if (half == 0 && live) {
+                const int nA = tc.n_actions;
+                float q[32];
+                acc_ld32(acc, tc.acc_ld, row, 0, q);
+                stage_trace(a.trace, 21);
+                q_combine<DUELING>(bias, nA, q);
+                const int act = s_act[row];
+                const float qa = q_at(q, act);
+                stage_trace(a.trace, 22);
+                float gq = 0.f, lterm = 0.f;
+                if (mine) lterm = td_loss(src, gb, qa - s_y[row], a.loss_kind, a.inv_global_b, gq);
+                // the warp's 32 loss terms: butterfly sum, ONE shared-memory add per warp (an atomicAdd per lane on the same
+                // word is a 32-deep compare-and-swap chain) -- and a fixed order
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) lterm += __shfl_xor_sync(0xffffffffu, lterm, off);
+                stage_trace(a.trace, 23);
+                if (lane == 0) atomicAdd(&s_loss, lterm);
+                stage_trace(a.trace, 24);
+                float g[32];
+                const float inv = 1.f / (float)nA;
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    float gj;
+                    if (DUELING) gj = (j < nA) ? gq * ((j == act ? 1.f : 0.f) - inv) : (j == nA ? gq : 0.f);
+                    else gj = (j == act) ? gq : 0.f;
+                    g[j] = gj;
+                }
+                stage_trace(a.trace, 25);
                 const uint32_t sbon = mma_sbo(T.N_pad);
-                float *act_row = act_buf + (size_t)egb * tc.act_stride + tc.L[l + 1].act_off;
-                uint32_t mk = 0u;
-                for (int c = e.c0, sh = 0; c < T.N_pad; c += e.step, sh += 4) {
-                    const float4 v = e.ld(acc, tc.acc_ld, c);
-                    float4 x, h, lo4;
-                    x.x = fmaxf(v.x + bias[c + 0], 0.f); x.y = fmaxf(v.y + bias[c + 1], 0.f);
-                    x.z = fmaxf(v.z + bias[c + 2], 0.f); x.w = fmaxf(v.w + bias[c + 3], 0.f);
+                float *dz_row = dz_buf + (size_t)gb * tc.dz_stride + T.dz_off;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    float4 x = make_float4(g[4 * j], g[4 * j + 1], g[4 * j + 2], g[4 * j + 3]), h, lo4;
                     tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
-                    const uint32_t off = mma_off(e.row, c, sbon);
+                    const uint32_t off = mma_off(row, 4 * j, sbon);
                     *reinterpret_cast<float4 *>(Ahi + off) = h;
                     *reinterpret_cast<float4 *>(Alo + off) = lo4;
-                    if (emine) *reinterpret_cast<float4 *>(act_row + c) = x;      // kept for dW
-                    mk |= ((x.x > 0.f ? 1u : 0u) | (x.y > 0.f ? 2u : 0u) | (x.z > 0.f ? 4u : 0u) | (x.w > 0.f ? 8u : 0u)) << sh;
+                    if (mine) *reinterpret_cast<float4 *>(dz_row + 4 * j) = x;
                 }
-                if (!emine) mk = 0u;
-                if (l == 0) hm1 = mk; else if (l == 1) hm2 = mk; else if (l == 2) hm3 = mk; else hm4 = mk;
-            } else {
-                // head: Q(s, .), loss, dLoss/dHead -> next A operand (K = 32) and the dz scratch
-                const uint32_t sbon = mma_sbo(T.N_pad);
-                if (half == 0 && live) {
-                    float q[32];
-                    acc_ld32(acc, tc.acc_ld, row, 0, q);
-                    TR_TRACE(21);
-                    const int nA = tc.n_actions;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) q[j] += bias[j];
-                    if (DUELING) {
-                        float s = 0.f, V = 0.f;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) { if (j < nA) s += q[j]; if (j == nA) V = q[j]; }
-                        const float mean = s / (float)nA;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) q[j] = V + q[j] - mean;
-                    }
-                    const int act = s_act[row];
-                    float qa = 0.f;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) if (j == act) qa = q[j];
-                    TR_TRACE(22);
-                    float gq = 0.f, lterm = 0.f;
-                    if (mine) {
-                        const float diff = qa - s_y[row];
-                        const float wb = src.is_w ? src.is_w[gb] : 1.f;
-                        if (src.abs_err) src.abs_err[gb] = fabsf(diff);
-                        if (a.loss_kind == 0) {                       // MSELoss (BaseTrainer.py:40)
-                            lterm = wb * (diff * diff);
-                            gq = (2.f * diff * wb) * a.inv_global_b;
-                        } else {                                      // SmoothL1Loss(beta = 1)
-                            const float ad = fabsf(diff);
-                            lterm = wb * (ad < 1.f ? 0.5f * (diff * diff) : ad - 0.5f);
-                            gq = (fminf(fmaxf(diff, -1.f), 1.f) * wb) * a.inv_global_b;
-                        }
-                    }
-                    // the warp's 32 loss terms: butterfly sum, ONE shared-memory add per warp (an atomicAdd per lane on the same
-                    // word is a 32-deep compare-and-swap chain) -- and a fixed order
-#pragma unroll
-                    for (int off = 16; off > 0; off >>= 1) lterm += __shfl_xor_sync(0xffffffffu, lterm, off);
-                    TR_TRACE(23);
-                    if (lane == 0) atomicAdd(&s_loss, lterm);
-                    TR_TRACE(24);
-                    float g[32];
-                    const float inv = 1.f / (float)nA;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        float gj;
-                        if (DUELING) gj = (j < nA) ? gq * ((j == act ? 1.f : 0.f) - inv) : (j == nA ? gq : 0.f);
-                        else gj = (j == act) ? gq : 0.f;
-                        g[j] = gj;
-                    }
-                    TR_TRACE(25);
-                    float *dz_row = dz_buf + (size_t)gb * tc.dz_stride + T.dz_off;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float4 x = make_float4(g[4 * j], g[4 * j + 1], g[4 * j + 2], g[4 * j + 3]), h, lo4;
-                        tf32_split(x.x, h.x, lo4.x); tf32_split(x.y, h.y, lo4.y); tf32_split(x.z, h.z, lo4.z); tf32_split(x.w, h.w, lo4.w);
-                        const uint32_t off = mma_off(row, 4 * j, sbon);
-                        *reinterpret_cast<float4 *>(Ahi + off) = h;
-                        *reinterpret_cast<float4 *>(Alo + off) = lo4;
-                        if (mine) *reinterpret_cast<float4 *>(dz_row + 4 * j) = x;
-                    }
-                    TR_TRACE(26);
-                }
+                stage_trace(a.trace, 26);
             }
             fence_proxy_async();
             __syncthreads();
-            TR_TRACE(11 + l);
-        }
+            stage_trace(a.trace, 11 + l);
+        };
+        forward_layers<FIXED, true>(tc, R, e, Ahi, Alo, W, acc, act_buf + (size_t)egb * tc.act_stride, emine, mid, head,
+                                    [&](int l, uint32_t mk) {
+                                        if (l == 0) hm1 = mk; else if (l == 1) hm2 = mk; else if (l == 2) hm3 = mk; else hm4 = mk;
+                                        stage_trace(a.trace, 11 + l);
+                                    });
 
         if (fused && tc.train_img_bytes > tc.img_bytes) mbar_wait(&wbar3, 0);                     // transposed blocks (requested at kernel start)
         // ---------------- dX chain: dZ_{l-1} = (dZ_l * W_l) .* (H_l > 0), l = nl-1 .. 1
@@ -454,10 +286,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
             }
             fence_proxy_async();
             __syncthreads();
-            TR_TRACE(16 + l);
+            stage_trace(a.trace, 16 + l);
         }
     }
-    TR_TRACE(20);
+    stage_trace(a.trace, 20);
     if (tid == 0) a.loss_partials[(size_t)grp * gridDim.x + blockIdx.x] = s_loss;
 }
 
@@ -528,7 +360,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     __shared__ const float *drows[2][kDwChunk];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = warp & 3, half = warp >> 2;
-    DW_TRACE(0);
+    stage_trace(a.trace, 0);
     uint32_t pkey[4];
     Philox::gen(src.key, src.epoch, 0x5A17ull, pkey);
     auto resolve_chunk = [&](int c, int buf) {                // row pointers of chunk c (128 samples)
@@ -547,7 +379,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     // PDL: hidden activations and dZ come from the training chain (the predecessor); the layer-0 CTAs' A operand is
     // built from replay rows (written >= 2 kernels back) and is gathered before the wait
     if (l != 0) { pdl_wait(); pdl_trigger(); }
-    DW_TRACE(1);
+    stage_trace(a.trace, 1);
     // A: 128 samples x 128 columns (features, the ones column, zero padding) = 16 float4 per thread; B: 128 x N_pad.
     // Persistent over this slice's chunks: the loads of chunk c + 1 are issued before the MMAs of chunk c and land while they
     // run; the products accumulate in the same registers -> one partial per slice however large the batch.
@@ -575,7 +407,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     } else {
         load_chunk(0);
     }
-    DW_TRACE(2);
+    stage_trace(a.trace, 2);
     // warpgroup g owns features [64g, 64g + 64); its MMAs run when that range holds real rows
     const int row0 = (tid >> 7) * 64;
     const bool wg_live = row0 < rowsA;
@@ -590,7 +422,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
         resolve_chunk(cn, (it + 1) & 1);
         fence_proxy_async();
         __syncthreads();
-        DW_TRACE(4);
+        stage_trace(a.trace, 4);
         if (cn < a.n_chunks) load_chunk((it + 1) & 1);         // next chunk's rows -> registers while the MMAs run
         if (wg_live) {
             const uint64_t ah = mma_desc(Ahi + (row0 / 8) * kDwSbo, kDwSbo), al = mma_desc(Alo + (row0 / 8) * kDwSbo, kDwSbo);
@@ -599,7 +431,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
             else wgmma_3xtf32<64>(d, ah, al, bh, bl, kDwChunk / 8, it > 0 ? 1u : 0u);
         }
     }
-    DW_TRACE(5);
+    stage_trace(a.trace, 5);
     // the accumulator -> a [feature][out] tile in the A operand's space (every MMA has read it), one feature row per thread
     __syncthreads();
     float *acc = reinterpret_cast<float *>(smem);
@@ -609,7 +441,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
         else store_frag<64>(d, acc, acc_ld, row0, 0, kDwARows);
     }
     __syncthreads();
-    DW_TRACE(6);
+    stage_trace(a.trace, 6);
     // epilogue: row f = input feature (or the ones column), column o = output unit, into partial slice `chunk`.
     // Lanes hold consecutive f, so every store instruction writes 32 consecutive elements of one weight row; the 32 columns of a
     // thread walk the rows with a pointer increment and a predicate each (the address arithmetic used to dominate this epilogue).
@@ -640,7 +472,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
             }
         }
     }
-    DW_TRACE(7);
+    stage_trace(a.trace, 7);
 }
 
 typedef void (*TrainKernel)(TcNet, TcTrainArgs);
@@ -734,9 +566,10 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     const int grid = a.n_tiles < num_sms() ? a.n_tiles : num_sms();
     const bool chain = l->pdl_chain && g_pdl.load();
     if (fused_td && a.n_tiles > grid) return fail(UAVRL_ERR_INVALID, "fused TD needs one tile per CTA");
-    static const bool trace_on = getenv("UAVRL_TC_TRACE") != nullptr;
-    long long *tr = nullptr;
-    if (trace_on) { UAVRL_CUDA(cudaMalloc((void **)&tr, 48 * sizeof(long long))); UAVRL_CUDA(cudaMemset(tr, 0, 48 * sizeof(long long))); a.trace = tr + 16; }
+    TcDwArgs d;
+    memset(&d, 0, sizeof(d));
+    if (int rc = stage_trace_alloc(&a.trace)) return rc;
+    if (int rc = stage_trace_alloc(&d.trace)) { cudaFree(a.trace); return rc; }
     const bool use_pdl = chain && (fused_td ? (l->pdl_prev == kPdlEnv) : (l->pdl_prev == kPdlTd));
     const int npre = fused_td ? (l->cfg.algo != UAVRL_ALGO_DQN ? 2 : 1) : 0;
     UAVRL_CUDA(launch_kernel(pick_train_kernel(npre, tc.dueling != 0, tc_fixed_chains(tc, true)), dim3(grid, l->G), dim3(kTcThreads),
@@ -744,8 +577,6 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     l->pdl_prev = chain ? kPdlTrain : kPdlNone;
     UAVRL_LAUNCHED();
     if (after_chain) UAVRL_CUDA(cudaEventRecord(after_chain, st));
-    TcDwArgs d;
-    memset(&d, 0, sizeof(d));
     d.src = src; d.B = B; d.n_chunks = (B + kDwChunk - 1) / kDwChunk; d.P = l->net.P;
     d.act_buf = l->act_buf; d.dz_buf = l->dz_buf; d.partials = l->partials;
     const int n_sm = num_sms();
@@ -753,22 +584,12 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     const int max_slices = n_sm / tc.n_layers > 0 ? n_sm / tc.n_layers : 1;
     d.n_slices = d.n_chunks < max_slices ? d.n_chunks : max_slices;
     const int dw_grid = d.n_slices * tc.n_layers;
-    if (trace_on) d.trace = tr;
     UAVRL_CUDA(launch_kernel(tc_dw_kernel, dim3(dw_grid, l->G), dim3(kTcThreads), dw_smem_bytes(tc), st, chain && !after_chain, tc, d));
     l->pdl_prev = chain ? kPdlDw : kPdlNone;
     UAVRL_LAUNCHED();
-    if (trace_on) {
-        long long h[48];
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        UAVRL_CUDA(cudaMemcpy(h, tr, sizeof(h), cudaMemcpyDeviceToHost));
-        cudaFree(tr);
-        fprintf(stderr, "[train_trace] B=%d R=%d fused_td=%d cycles since start:", B, a.R, a.fused_td);
-        for (int i = 1; i < 32; ++i) if (h[16 + i]) fprintf(stderr, " [%d]=%lld", i, h[16 + i] - h[16]);
-        fprintf(stderr, "\n");
-        fprintf(stderr, "[dw_trace] B=%d chunks=%d (CTA 0 = layer 0) cycles since start:", B, d.n_chunks);
-        for (int i = 1; i < 9; ++i) fprintf(stderr, " [%d]=%lld", i, h[i] - h[0]);
-        fprintf(stderr, "\n");
-    }
+    const int rc_train = stage_trace_print(st, a.trace, "[train_trace] B=%d R=%d fused_td=%d", B, a.R, a.fused_td);
+    const int rc_dw = stage_trace_print(st, d.trace, "[dw_trace] B=%d chunks=%d (CTA 0 = layer 0)", B, d.n_chunks);     // frees d.trace either way
+    if (rc_train || rc_dw) return rc_train ? rc_train : rc_dw;
     *n_grad_parts = d.n_slices;
     *n_loss_parts = grid;
     return 0;

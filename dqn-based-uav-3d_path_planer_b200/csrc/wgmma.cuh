@@ -173,6 +173,14 @@ __device__ __forceinline__ void mma_chunk(float *acc, int ld, int row0, int n0, 
                                           const unsigned char *b_lo, uint32_t sbo, int ksteps, int R)
 {
     float d[N / 2];
+    // The runtime-K chain's first product overwrites d only through a runtime scale-d predicate, so to ptxas d is read
+    // before it is written.  Left undefined, its registers may get a definition placed inside the wgmma pipeline stage,
+    // depending on the surrounding code, and ptxas then serialises every wgmma of the kernel (C7515).  Zeroing d ahead of
+    // the fence rules that out; the products are unchanged.
+    if (!FIXED) {
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+    }
     const uint32_t boff = (uint32_t)(n0 >> 3) * sbo;
     const uint64_t bh = mma_desc(b_hi + boff, sbo), bl = mma_desc(b_lo + boff, sbo);
     if (FIXED) wgmma_3xtf32_fixed<N, KIND>(d, a_hi, a_lo, bh, bl, ksteps);
