@@ -185,6 +185,9 @@ int uavrl_env_create(const uavrl_env_config *cfg, uavrl_env **out)
         return fail(UAVRL_ERR_INVALID, "n_buildings must be in [0,64] (candidate sets are 64-bit masks)");
     if (cfg->n_buildings > 0 && !cfg->buildings_host) return fail(UAVRL_ERR_INVALID, "buildings_host is null");
     if (cfg->max_step <= 0 || !(cfg->max_v > 0)) return fail(UAVRL_ERR_INVALID, "max_step and max_v must be > 0");
+    // A negative speed level turns V_vector against the heading the step carries (UAV.py:414-416 recomputes it from
+    // V_vector every step, the cached heading does not), so the discrete-27 speeds Min_V, (Min_V + Max_V) / 2 must be >= 0.
+    if (!(cfg->min_v >= 0)) return fail(UAVRL_ERR_INVALID, "min_v must be >= 0: a negative speed reverses V_vector against the heading");
     // RRT.py:69-71 makes sub_goals[0] the UAV's own position object: a collision on the very first step moves that entry with
     // the UAV.  The kernel does not write the moved entry back to the queue -- immaterial while one step is shorter than the 7 m
     // sub-goal radius (the entry is popped on that same step; reference Max_V = 1), a divergence from the reference beyond it.

@@ -90,8 +90,10 @@ UAVRL_HD double angle_xy(double dx, double dy)
 // cos|calculate_angle(a) - calculate_angle(b)| for two planar vectors WITHOUT the angles: the reference forms both angles with
 // atan2 -> degrees -> (+360) % 360 -> radians and takes the cosine of their difference (UAV.py:422-423,435,488-490), which
 // is the cosine of the angle between the vectors = their normalised dot product (the % 360 wrap and |.| do not change a
-// cosine).  calculate_angle of the zero vector is atan2(0, 0) = 0, i.e. the direction (1, 0).  Agrees with the literal
-// evaluation to a few 1e-16 (both are ~1 ulp evaluations of the same real number); nothing but the reward depends on it.
+// cosine).  calculate_angle of a zero vector is atan2 of its signed zeros: atan2(+-0, -0) = +-pi, the direction (-1, 0),
+// and atan2(+-0, +0) = +-0, the direction (1, 0).  A zero V_vector carries the signs of speed 0 times (cos, sin), so both
+// occur.  Agrees with the literal evaluation to a few 1e-16 (both are ~1 ulp evaluations of the same real number); nothing
+// but the reward depends on it.
 // UAVRL_LITERAL_ANGLES=1 compiles the literal atan2 / cos chain instead (about 400 more dependent fp64 instructions per step).
 #ifndef UAVRL_LITERAL_ANGLES
 #define UAVRL_LITERAL_ANGLES 0
@@ -100,18 +102,28 @@ UAVRL_HD double cos_between(double ax, double ay, double bx, double by)
 {
     double na = dsqrt(dadd(dmul(ax, ax), dmul(ay, ay)));
     double nb = dsqrt(dadd(dmul(bx, bx), dmul(by, by)));
-    if (na == 0.0) { ax = 1.0; ay = 0.0; na = 1.0; }
-    if (nb == 0.0) { bx = 1.0; by = 0.0; nb = 1.0; }
+    if (na == 0.0) { ax = copysign(1.0, ax); ay = 0.0; na = 1.0; }
+    if (nb == 0.0) { bx = copysign(1.0, bx); by = 0.0; nb = 1.0; }
     return ddiv(dadd(dmul(ax, bx), dmul(ay, by)), dmul(na, nb));
 }
 
-// calculate_angle(0, V_vector) of V_vector = speed * (cos t, sin t), speed > 0: t wrapped into [0, 2 pi) -- what the
-// reference's atan2 -> degrees -> % 360 -> radians round trip returns up to its own rounding (~1e-15).
+// calculate_angle(0, V_vector) of V_vector = V * (cos t, sin t), V > 0: t wrapped into [0, 2 pi) -- what the reference's
+// atan2 -> degrees -> % 360 -> radians round trip returns up to its own rounding (~1e-15).  One wrap covers |t| < 4 pi minus
+// the old heading, i.e. |a0 * steering| < 2 pi; beyond that the step takes the angle of V_vector itself (heading_of).
 UAVRL_HD double wrap_2pi(double t)
 {
     if (t < 0.0) t = dadd(t, 2.0 * kPi);
     if (t >= 2.0 * kPi) t = dsub(t, 2.0 * kPi);
     return t;
+}
+
+// The cached heading after a step that set V_vector = speed * (cos t, sin t) (speed >= 0, uavrl_env_create refuses a
+// negative Min_V): t wrapped once when that lands in [0, 2 pi), else calculate_angle(0, V_vector) itself -- a zero
+// V_vector (speed 0) or a turn of 2 pi or more, which one wrap cannot bring back.
+UAVRL_HD double heading_of(double t, double V, double vx, double vy)
+{
+    const double w = wrap_2pi(t);
+    return (V > 0.0 && w >= 0.0 && w < 2.0 * kPi) ? w : angle_xy(vx, vy);
 }
 
 // The reference evaluates calculate_angle(0, V_vector) three times per step on the SAME vector
@@ -253,7 +265,7 @@ UAVRL_HD void step_core_apf(const EnvConst &k, EnvRegs &s, int act_mode, double 
     double tri_V = s.theta;                                          // :423
 #else
     const double tgx = dsub(sg.x, s.px), tgy = dsub(sg.y, s.py);     // :422 tri_goal = the direction of this vector
-    s.theta = (s.V > 0.0) ? wrap_2pi(seta_new) : angle_xy(s.vx, s.vy);
+    s.theta = heading_of(seta_new, s.V, s.vx, s.vy);
     double tvx = s.vx, tvy = s.vy;                                   // :423 tri_V = the direction of V_vector
 #endif
     if (threat(s.px, s.py, s.pz)) {                                  // :425
