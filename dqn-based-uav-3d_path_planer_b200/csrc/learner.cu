@@ -997,8 +997,9 @@ int uavrl_learner_compute_grads(uavrl_learner *l, const int32_t *idx_tape_dev, i
 {
     if (!l || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     if (int rc = refuse_grouped(l, "uavrl_learner_compute_grads (data-parallel training)")) return rc;
-    l->epoch += 1;
+    // refused before the epoch counts: a rank that retries must stay on the other ranks' sample keys and target schedule
     if (l->replay.count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
+    l->epoch += 1;
     BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, idx_tape_dev);
     return do_update(l, src, l->cfg.batch_size, global_batch, loss_dev, false, stream);
 }
@@ -1120,9 +1121,9 @@ int uavrl_learner_update_dp(uavrl_learner *l, const int32_t *idx_tape_dev, int32
     if (!l || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     if (int rc = refuse_grouped(l, "uavrl_learner_update_dp (data-parallel training)")) return rc;
     if (!l->comm_ready) return fail(UAVRL_ERR_STATE, "uavrl_learner_update_dp before uavrl_learner_comm_connect");
+    if (l->replay.count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     l->epoch += 1;
-    if (l->replay.count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
     BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, idx_tape_dev);
     return launch_update_dp(l, src, l->cfg.batch_size, global_batch, loss_dev, (cudaStream_t)stream);
 }

@@ -88,8 +88,13 @@ ReplayStore::Iteration ReplayStore::begin() const
 void ReplayStore::commit()
 {
     head = (head + 1) % ring_frames;
+    count = count_after_commit();
+}
+
+int64_t ReplayStore::count_after_commit() const
+{
     const int64_t max_count = (ring_frames - 1) * N;
-    count = (count + N > max_count) ? max_count : count + N;
+    return (count + N > max_count) ? max_count : count + N;
 }
 
 void ReplayStore::restart()

@@ -194,6 +194,7 @@ struct ReplayStore {
     struct Iteration { float *obs_t, *obs_next; int32_t *act; float *act2, *rew; uint8_t *done; };
     Iteration begin() const;
     void commit();
+    int64_t count_after_commit() const;   // lockstep: `count` once the next commit has run
     // forget every transition; the next iteration re-observes into frame `head`
     void restart();
     // n whole-store logical indices (0 = oldest) to host arrays; any output may be null

@@ -75,7 +75,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
     __shared__ int s_act[kTcTile], s_astar[kTcTile];
     __shared__ uint8_t s_fresh[kTcTile];                     // fused TD: the next-state row is being written by this iteration's env step
     __shared__ float s_y[kTcTile], s_rew[kTcTile], s_done[kTcTile];
-    __shared__ float s_loss;
+    __shared__ float s_loss[4];                              // per head warp, summed in warp order at the end: run-to-run exact
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = warp & 3, half = warp >> 2;
     // trainer blockIdx.y of a grouped learner: its images, batch, TD targets and scratch rows
@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
     // control thread (first of the last warp): barrier init and weight copies -- concurrently with warp 0 resolving the tile's
     // samples; the first CTA-wide barrier (behind the sample table) publishes the barriers
     constexpr int kCtl = kTcThreads - 32;
-    if (tid == 0) s_loss = 0.f;
+    if (tid == 0) s_loss[0] = s_loss[1] = s_loss[2] = s_loss[3] = 0.f;
     constexpr bool fused = NPRE > 0;
     constexpr int n_pre = NPRE;                                      // forward-only passes ahead of the training chain
     // PDL.  Unfused: the training image was written by the previous optimiser kernel (>= 2 kernels back: a TD pass always
@@ -221,12 +221,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
                 stage_trace(a.trace, 22);
                 float gq = 0.f, lterm = 0.f;
                 if (mine) lterm = td_loss(src, gb, qa - s_y[row], a.loss_kind, a.inv_global_b, gq);
-                // the warp's 32 loss terms: butterfly sum, ONE shared-memory add per warp (an atomicAdd per lane on the same
-                // word is a 32-deep compare-and-swap chain) -- and a fixed order
+                // the warp's 32 loss terms: butterfly sum, then one add into the warp's own shared word.  A shared atomicAdd of
+                // every head warp into one word summed the warps in arrival order, so a CTA with two 64-row tiles reported a
+                // loss that could differ by an ulp from run to run
 #pragma unroll
                 for (int off = 16; off > 0; off >>= 1) lterm += __shfl_xor_sync(0xffffffffu, lterm, off);
                 stage_trace(a.trace, 23);
-                if (lane == 0) atomicAdd(&s_loss, lterm);
+                if (lane == 0) s_loss[quad] += lterm;
                 stage_trace(a.trace, 24);
                 float g[32];
                 const float inv = 1.f / (float)nA;
@@ -290,7 +291,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
         }
     }
     stage_trace(a.trace, 20);
-    if (tid == 0) a.loss_partials[(size_t)grp * gridDim.x + blockIdx.x] = s_loss;
+    // the head epilogue ends with a CTA barrier: every warp's last add is visible here
+    if (tid == 0) a.loss_partials[(size_t)grp * gridDim.x + blockIdx.x] = ((s_loss[0] + s_loss[1]) + s_loss[2]) + s_loss[3];
 }
 
 // ------------------------------------------------------------------ split-K weight gradients

@@ -77,8 +77,14 @@ extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_it
     if (l->G > 1) return fail(UAVRL_ERR_INVALID, "uavrl_train_run_dp is not available on a learner with several trainers");
     if (l->replay.mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n)
         return fail(UAVRL_ERR_INVALID, "learner.lockstep_envs must equal env.n_envs");
+    if (l->net.in_dim != kObsDim) return fail(UAVRL_ERR_INVALID, "learner.in_dim must be 100 (the UAV observation)");
     if (!l->comm_ready) return fail(UAVRL_ERR_STATE, "uavrl_train_run_dp before uavrl_learner_comm_connect");
     if (!env->reset_done) return fail(UAVRL_ERR_STATE, "uavrl_train_run_dp before uavrl_env_reset");
+    if (env->cfg.device != l->cfg.device) return fail(UAVRL_ERR_INVALID, "env and learner live on different devices");
+    // every rank must take part in every all-reduce, so every iteration must update: the caller warms the replay up first.
+    // The count never shrinks, so the first iteration's sample decides, and a refusal leaves env, ring and epoch untouched
+    if (n_iters > 0 && l->replay.count_after_commit() <= l->cfg.batch_size)
+        return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions (warm up with uavrl_train_run first)");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
@@ -87,8 +93,6 @@ extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_it
     for (int it = 0; it < n_iters; ++it) {
         if ((rc = act_step_commit(env, l, eps, st))) return rc;
         l->epoch += 1;
-        // every rank must take part in every all-reduce: the caller warms the replay up first
-        if (l->replay.count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions (warm up with uavrl_train_run first)");
         BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, nullptr);
         if ((rc = launch_update_dp(l, src, l->cfg.batch_size, global_batch, l->loss_dev, st))) return rc;
     }
@@ -98,6 +102,8 @@ extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_it
 extern "C" int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, float *ms_out, void *stream)
 {
     if (!env || !l || n_iters <= 0 || !ms_out) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (l->net.in_dim != kObsDim) return fail(UAVRL_ERR_INVALID, "learner.in_dim must be 100 (the UAV observation)");
+    if (env->cfg.device != l->cfg.device) return fail(UAVRL_ERR_INVALID, "env and learner live on different devices");
     if (l->replay.mode != kReplayLockstep || l->cfg.lockstep_envs != env->d.n || !env->reset_done || !l->replay.frame0_valid)
         return fail(UAVRL_ERR_STATE, "uavrl_train_profile needs a warmed-up lockstep env/learner pair");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));

@@ -279,7 +279,9 @@ int uavrl_learner_update_batch(uavrl_learner *l, int32_t B, const float *s_dev, 
 
 /* Split form for data-parallel training: grads only (sum over the local batch of d(loss)/d(theta),
  * loss normalised by global_batch), then -- after the caller all-reduced uavrl_learner_grad_ptr()
- * across ranks -- the optimiser step.  */
+ * across ranks -- the optimiser step.  Unlike uavrl_learner_update, compute_grads refuses a replay holding
+ * <= batch_size transitions with UAVRL_ERR_STATE, before the epoch counts: every rank must take part in every
+ * exchange, and a rank that retries keeps the other ranks' sample keys and target-update schedule. */
 int uavrl_learner_compute_grads(uavrl_learner *l, const int32_t *idx_tape_dev, int32_t global_batch,
                                 float *loss_dev, void *stream);
 float *uavrl_learner_grad_ptr(uavrl_learner *l);          /* device, [param_count] fp32 */
@@ -308,7 +310,8 @@ int uavrl_learner_lockstep_restart(uavrl_learner *l);
  *                               applies Adam.  No NCCL call, no flag, no fence, nothing pulled across NVLink on the
  *                               critical path.  world = 1 runs the same kernel on the local buffer (self-test on one GPU).
  * flag_handle_out / flag_handles are unused (kept for ABI compatibility) and may be NULL.
- * loss_dev (optional) receives the GLOBAL batch loss. */
+ * loss_dev (optional) receives the GLOBAL batch loss.  update_dp refuses, before the epoch counts: a learner not connected
+ * (UAVRL_ERR_STATE) and a replay holding <= batch_size transitions (UAVRL_ERR_STATE), as compute_grads does. */
 int uavrl_learner_comm_init(uavrl_learner *l, int32_t rank, int32_t world, void *grad_handle_out, void *flag_handle_out);
 int uavrl_learner_comm_connect(uavrl_learner *l, const void *grad_handles, const void *flag_handles);
 int uavrl_learner_update_dp(uavrl_learner *l, const int32_t *idx_tape_dev, int32_t global_batch, float *loss_dev, void *stream);
@@ -415,13 +418,19 @@ int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const flo
 int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t do_update, uavrl_train_stats *stats_host, void *stream);
 
 /* Data-parallel form of uavrl_train_run (after uavrl_learner_comm_connect): every iteration ends with
- * uavrl_learner_update_dp on this rank's replay shard; global_batch = batch_size x world. */
+ * uavrl_learner_update_dp on this rank's replay shard; global_batch = batch_size x world.  Refused before anything is
+ * enqueued, leaving env, ring, parameters and counters untouched: global_batch <= 0, a grouped learner, lockstep_envs !=
+ * env.n_envs, in_dim != 100 or env and learner on different devices (UAVRL_ERR_INVALID, as uavrl_train_run); no
+ * uavrl_learner_comm_connect, no uavrl_env_reset, or a ring that would hold <= batch_size transitions at the first
+ * update (UAVRL_ERR_STATE: warm it up with uavrl_train_run first; the count never shrinks, so every later update runs). */
 int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, int32_t global_batch, void *stream);
 
 /* The same loop with a CUDA event recorded on `stream` before/after every kernel: ms_out[6] receives the
  * summed device time of {act, env_step, td_target, fwd_bwd, weight_grad, reduce_adam} over the n_iters
  * iterations (bench.py's roofline pass; on the CUDA-core path td_target and weight_grad are 0 because
- * fwd_bwd does everything; event gaps make the loop slower, never use it for throughput). */
+ * fwd_bwd does everything; event gaps make the loop slower, never use it for throughput).  Refused before anything is
+ * enqueued: in_dim != 100 or env and learner on different devices (UAVRL_ERR_INVALID, as uavrl_train_run), a pair that
+ * has never run uavrl_train_run (UAVRL_ERR_STATE). */
 int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, float *ms_out, void *stream);
 
 /* ---- prioritised experience replay (SURVEY.md 8f-3) ------------------------------------------------------------
