@@ -77,6 +77,7 @@ SIGNATURES = {
     "uavrl_env_reset": (C.c_int, [VP, C.c_int32, VP]),
     "uavrl_make_scenarios": (C.c_int, [C.POINTER(EnvConfig), C.c_uint64, C.c_int32, C.c_int32, VP, VP, VP, VP, VP]),
     "uavrl_set_pdl": (C.c_int, [C.c_int32]),
+    "uavrl_test_fail_alloc": (C.c_int, [C.c_int32]),
     "uavrl_set_fuse_act_env": (C.c_int, [C.c_int32]),
     "uavrl_set_fuse_dw_adam": (C.c_int, [C.c_int32]),
     "uavrl_set_fuse_td": (C.c_int, [C.c_int32]),

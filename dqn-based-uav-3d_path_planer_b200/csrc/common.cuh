@@ -7,6 +7,7 @@
 #include <atomic>
 #include <mutex>
 #include <string>
+#include <vector>
 
 #include "../../include/uavrl.h"
 
@@ -101,11 +102,60 @@ inline int raise_dyn_smem(K *kernel, size_t bytes)
     return 0;
 }
 
-template <class T>
-inline int dev_alloc(T **p, size_t n)
+extern std::atomic<int> g_fail_alloc;    // uavrl_test_fail_alloc(); -1 = off
+
+// Owner of a group of device buffers that live and die together: every pointer alloc() hands out is freed by release() or the
+// destructor.  Host handles hold one DevMem per group; the kernel-argument structs keep plain pointers into them.  A failed
+// alloc() leaves p untouched, clears the runtime's error state and returns UAVRL_ERR_CUDA ("out of memory").
+class DevMem {
+public:
+    DevMem() = default;
+    DevMem(DevMem &&o) noexcept : ptrs_(std::move(o.ptrs_)) {}
+    DevMem &operator=(DevMem &&o) noexcept { if (this != &o) { release(); ptrs_.swap(o.ptrs_); } return *this; }
+    ~DevMem() { release(); }
+    void release() { for (void *p : ptrs_) cudaFree(p); ptrs_.clear(); }
+    // n elements of T, zeroed unless zero = false
+    template <class T>
+    int alloc(T *&p, size_t n, bool zero = true)
+    {
+        int k = g_fail_alloc.load(std::memory_order_relaxed);
+        while (k >= 0 && !g_fail_alloc.compare_exchange_weak(k, k - 1, std::memory_order_relaxed)) {}
+        void *q = nullptr;
+        const cudaError_t e = k == 0 ? cudaErrorMemoryAllocation : cudaMalloc(&q, n * sizeof(T));
+        if (e != cudaSuccess) {
+            cudaGetLastError();                                  // a failed cudaMalloc must not surface at the next launch check
+            return fail(UAVRL_ERR_CUDA, "cudaMalloc of " + std::to_string(n * sizeof(T)) + " bytes failed: " + cudaGetErrorString(e));
+        }
+        ptrs_.push_back(q);
+        if (zero) UAVRL_CUDA(cudaMemset(q, 0, n * sizeof(T)));
+        p = static_cast<T *>(q);
+        return 0;
+    }
+
+private:
+    std::vector<void *> ptrs_;
+};
+
+// Scratch that grows with the batch: when need exceeds cap, wait for st, free the group, then allocate every buffer of bufs
+// (pointer, element count) afresh and set cap = need.  On failure the group is empty, every pointer null and cap 0, so the
+// next call grows again.
+template <class T> struct Buf { T *&p; size_t n; };
+template <class T> Buf<T> buf(T *&p, size_t n) { return Buf<T>{ p, n }; }
+template <class Cap, class... T>
+int grow(DevMem &m, Cap &cap, Cap need, cudaStream_t st, bool zero, Buf<T>... bufs)
 {
-    UAVRL_CUDA(cudaMalloc((void **)p, n * sizeof(T)));
-    UAVRL_CUDA(cudaMemset(*p, 0, n * sizeof(T)));
+    if (need <= cap) return 0;
+    UAVRL_CUDA(cudaStreamSynchronize(st));
+    m.release();
+    cap = 0;
+    int rc = 0;
+    ((rc = rc ? rc : m.alloc(bufs.p, bufs.n, zero)), ...);
+    if (rc) {
+        m.release();
+        ((bufs.p = nullptr), ...);
+        return rc;
+    }
+    cap = need;
     return 0;
 }
 

@@ -33,6 +33,7 @@ namespace uavrl {
 thread_local std::string g_last_error;
 std::atomic<long long> g_launches{0};
 std::atomic<int> g_pdl{1};
+std::atomic<int> g_fail_alloc{-1};
 
 template <bool DO_STEP, int EPB, bool EXTRAS = false>
 __global__ void __launch_bounds__(kEnvThreads)
@@ -89,10 +90,11 @@ int launch_env_step(const EnvDev &d_in, int action_kind, const void *actions, fl
 {
     EnvDev d = d_in;
     static const bool trace_on = getenv("UAVRL_ENV_TRACE") != nullptr;
+    static DevMem tr_mem;
     static long long *tr = nullptr;
     static int n_traced = 0;
     if (trace_on) {
-        if (!tr) { UAVRL_CUDA(cudaMalloc((void **)&tr, 16 * sizeof(long long))); UAVRL_CUDA(cudaMemset(tr, 0, 16 * sizeof(long long))); }
+        if (!tr) { if (int rc = tr_mem.alloc(tr, 16)) return rc; }
         else if (++n_traced % 64 == 0) {                         // print the PREVIOUS launch's stamps every 64 launches
             long long h[16];
             UAVRL_CUDA(cudaStreamSynchronize(st));
@@ -158,12 +160,66 @@ int EnvStatsMark::end(const EnvDev &d, cudaStream_t st, int64_t updates, uavrl_t
 }  // namespace uavrl
 
 namespace uavrl {
-void free_pool(EnvDev &d)
+int pool_alloc(PoolBuild &b, size_t P, size_t K)
 {
-    cudaFree((void *)d.pool_start); cudaFree((void *)d.pool_goal); cudaFree((void *)d.pool_v0);
-    cudaFree((void *)d.pool_sub); cudaFree((void *)d.pool_nsub); cudaFree((void *)d.pool_alias);
-    d.pool_start = d.pool_goal = d.pool_v0 = d.pool_sub = nullptr;
-    d.pool_nsub = nullptr; d.pool_alias = nullptr;
+    int rc;
+    if ((rc = b.mem.alloc(b.start, P * 3, false)) || (rc = b.mem.alloc(b.goal, P * 3, false)) || (rc = b.mem.alloc(b.v0, P * 3, false)) ||
+        (rc = b.mem.alloc(b.sub, P * K * 3, false)) || (rc = b.mem.alloc(b.nsub, P, false)) || (rc = b.mem.alloc(b.alias, P, false)))
+        return rc;
+    return 0;
+}
+
+int pool_install(uavrl_env *env, PoolBuild &b, int32_t P)
+{
+    UAVRL_CUDA(cudaDeviceSynchronize());            // nothing may still read the pool being replaced
+    EnvDev &d = env->d;
+    env->pool_mem = std::move(b.mem);
+    d.pool_start = b.start; d.pool_goal = b.goal; d.pool_v0 = b.v0; d.pool_sub = b.sub; d.pool_nsub = b.nsub; d.pool_alias = b.alias;
+    d.P = P; env->pool_set = true; env->reset_done = false;
+    return 0;
+}
+
+// everything uavrl_env_create builds; on failure the caller destroys the half-built handle
+static int env_init(uavrl_env *env, const uavrl_env_config *cfg)
+{
+    env->cfg = *cfg;
+    env->cfg.buildings_host = nullptr;
+    EnvDev &d = env->d;
+    memset(&d, 0, sizeof(d));
+    d.k.width = cfg->width; d.k.h = cfg->h;
+    d.k.max_v = cfg->max_v; d.k.min_v = cfg->min_v; d.k.steering = cfg->steering_angle;
+    d.k.climb = cfg->climb_rate; d.k.max_step = cfg->max_step; d.k.n_cyl = cfg->n_buildings;
+    d.n = cfg->n_envs; d.K = cfg->max_subgoals; d.P = 0; d.auto_reset = cfg->auto_reset;
+    d.cull_w = 20.0 + cfg->max_v + 0.5;
+
+    std::vector<Cyl> cyl((size_t)(cfg->n_buildings > 0 ? cfg->n_buildings : 1));
+    for (int i = 0; i < cfg->n_buildings; ++i) {
+        const double *b = cfg->buildings_host + 5 * i;
+        Cyl c;
+        c.cx = b[0]; c.cy = b[1]; c.R = b[3]; c.H = b[4];      // b[2] = base z: only ever subtracted from itself
+        env->base_z.push_back(b[2]);                           // (the APF distance is 3-D: it does see it)
+        const double r2 = c.R * c.R;
+        c.r2lo = r2 * (1.0 - 1e-12); c.r2hi = r2 * (1.0 + 1e-12);
+        cyl[i] = c;
+    }
+    DevMem &m = env->mem;
+    int rc;
+    Cyl *dcyl = nullptr;
+    if ((rc = m.alloc(dcyl, cyl.size(), false))) return rc;
+    UAVRL_CUDA(cudaMemcpy(dcyl, cyl.data(), cyl.size() * sizeof(Cyl), cudaMemcpyHostToDevice));
+    d.cyl = dcyl;
+
+    const size_t n = (size_t)d.n;
+    double **f64[] = { &d.px, &d.py, &d.pz, &d.vx, &d.vy, &d.V, &d.score, &d.total, &d.path_len,
+                       &d.gx, &d.gy, &d.gz, &d.rew64, &d.theta };
+    for (auto p : f64) if ((rc = m.alloc(*p, n))) return rc;
+    int32_t **i32[] = { &d.step, &d.cursor, &d.n_sub, &d.scen };
+    for (auto p : i32) if ((rc = m.alloc(*p, n))) return rc;
+    if ((rc = m.alloc(d.done, n)) || (rc = m.alloc(d.alias, n)) || (rc = m.alloc(d.stat_counts, 8)) ||
+        (rc = m.alloc(d.stat_reward, 2)))                      // [0] sum of rewards, [1] total flight energy (extras)
+        return rc;
+    UAVRL_CUDA(cudaStreamCreateWithFlags(&env->own_stream, cudaStreamNonBlocking));
+    return 0;
 }
 }  // namespace uavrl
 
@@ -174,6 +230,7 @@ extern "C" {
 
 const char *uavrl_last_error(void) { return g_last_error.c_str(); }
 int uavrl_set_pdl(int32_t on) { g_pdl.store(on ? 1 : 0); return 0; }
+int uavrl_test_fail_alloc(int32_t n) { g_fail_alloc.store(n >= 0 ? n : -1); return 0; }
 const char *uavrl_version(void) { return "uavrl-b200 0.1 (sm_90a)"; }
 int64_t uavrl_launch_count(void) { return (int64_t)g_launches.load(); }
 
@@ -198,58 +255,15 @@ int uavrl_env_create(const uavrl_env_config *cfg, uavrl_env **out)
     UAVRL_CUDA(cudaSetDevice(cfg->device));
 
     uavrl_env *env = new uavrl_env();
-    env->cfg = *cfg;
-    env->cfg.buildings_host = nullptr;
-    EnvDev &d = env->d;
-    memset(&d, 0, sizeof(d));
-    d.k.width = cfg->width; d.k.h = cfg->h;
-    d.k.max_v = cfg->max_v; d.k.min_v = cfg->min_v; d.k.steering = cfg->steering_angle;
-    d.k.climb = cfg->climb_rate; d.k.max_step = cfg->max_step; d.k.n_cyl = cfg->n_buildings;
-    d.n = cfg->n_envs; d.K = cfg->max_subgoals; d.P = 0; d.auto_reset = cfg->auto_reset;
-    d.cull_w = 20.0 + cfg->max_v + 0.5;
-
-    std::vector<Cyl> cyl((size_t)(cfg->n_buildings > 0 ? cfg->n_buildings : 1));
-    for (int i = 0; i < cfg->n_buildings; ++i) {
-        const double *b = cfg->buildings_host + 5 * i;
-        Cyl c;
-        c.cx = b[0]; c.cy = b[1]; c.R = b[3]; c.H = b[4];      // b[2] = base z: only ever subtracted from itself
-        env->base_z.push_back(b[2]);                           // (the APF distance is 3-D: it does see it)
-        const double r2 = c.R * c.R;
-        c.r2lo = r2 * (1.0 - 1e-12); c.r2hi = r2 * (1.0 + 1e-12);
-        cyl[i] = c;
-    }
-    Cyl *dcyl = nullptr;
-    UAVRL_CUDA(cudaMalloc((void **)&dcyl, cyl.size() * sizeof(Cyl)));
-    UAVRL_CUDA(cudaMemcpy(dcyl, cyl.data(), cyl.size() * sizeof(Cyl), cudaMemcpyHostToDevice));
-    d.cyl = dcyl;
-
-    const size_t n = (size_t)d.n;
-    double **f64[] = { &d.px, &d.py, &d.pz, &d.vx, &d.vy, &d.V, &d.score, &d.total, &d.path_len,
-                       &d.gx, &d.gy, &d.gz, &d.rew64, &d.theta };
-    for (auto p : f64) { int rc = dev_alloc(p, n); if (rc) return rc; }
-    int32_t **i32[] = { &d.step, &d.cursor, &d.n_sub, &d.scen };
-    for (auto p : i32) { int rc = dev_alloc(p, n); if (rc) return rc; }
-    { int rc = dev_alloc(&d.done, n); if (rc) return rc; }
-    { int rc = dev_alloc(&d.alias, n); if (rc) return rc; }
-    { int rc = dev_alloc(&d.stat_counts, 8); if (rc) return rc; }
-    { int rc = dev_alloc(&d.stat_reward, 2); if (rc) return rc; }      // [0] sum of rewards, [1] total flight energy (extras)
-    UAVRL_CUDA(cudaStreamCreateWithFlags(&env->own_stream, cudaStreamNonBlocking));
+    if (int rc = env_init(env, cfg)) { uavrl_env_destroy(env); return rc; }
     *out = env;
     return 0;
 }
 
-
 int uavrl_env_destroy(uavrl_env *env)
 {
     if (!env) return 0;
-    EnvDev &d = env->d;
     cudaSetDevice(env->cfg.device);
-    void *ptrs[] = { (void *)d.cyl, d.px, d.py, d.pz, d.vx, d.vy, d.V, d.score, d.total, d.path_len, d.gx, d.gy,
-                     d.gz, d.rew64, d.theta, d.step, d.cursor, d.n_sub, d.scen, d.done, d.alias, d.stat_counts,
-                     d.stat_reward, env->h_act_dev, env->h_obs_dev, env->h_rew_dev, env->h_flags_dev };
-    for (void *p : ptrs) cudaFree(p);
-    cudaFree(d.energy); cudaFree((void *)d.apf_obs); cudaFree(d.sub_env); cudaFree(d.path_buf); cudaFree(d.path_n); cudaFree(d.path_cur);
-    free_pool(d);
     if (env->own_stream) cudaStreamDestroy(env->own_stream);
     delete env;
     return 0;
@@ -275,27 +289,16 @@ int uavrl_env_set_pool(uavrl_env *env, int32_t P, const double *start, const dou
         v0[3 * i] = vx; v0[3 * i + 1] = vy; v0[3 * i + 2] = V;
         if (alias0) al[i] = alias0[i];
     }
-    UAVRL_CUDA(cudaDeviceSynchronize());
-    free_pool(d);
-    double *ps, *pg, *pv, *pq; int32_t *pn; uint8_t *pa;
+    PoolBuild b;
     const size_t sub_n = (size_t)P * d.K * 3;
-    UAVRL_CUDA(cudaMalloc((void **)&ps, (size_t)P * 3 * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&pg, (size_t)P * 3 * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&pv, (size_t)P * 3 * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&pq, sub_n * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&pn, (size_t)P * sizeof(int32_t)));
-    UAVRL_CUDA(cudaMalloc((void **)&pa, (size_t)P));
-    UAVRL_CUDA(cudaMemcpy(ps, start, (size_t)P * 3 * sizeof(double), cudaMemcpyHostToDevice));
-    UAVRL_CUDA(cudaMemcpy(pg, goal, (size_t)P * 3 * sizeof(double), cudaMemcpyHostToDevice));
-    UAVRL_CUDA(cudaMemcpy(pv, v0.data(), (size_t)P * 3 * sizeof(double), cudaMemcpyHostToDevice));
-    UAVRL_CUDA(cudaMemcpy(pq, sub, sub_n * sizeof(double), cudaMemcpyHostToDevice));
-    UAVRL_CUDA(cudaMemcpy(pn, n_sub, (size_t)P * sizeof(int32_t), cudaMemcpyHostToDevice));
-    UAVRL_CUDA(cudaMemcpy(pa, al.data(), (size_t)P, cudaMemcpyHostToDevice));
-    d.pool_start = ps; d.pool_goal = pg; d.pool_v0 = pv; d.pool_sub = pq; d.pool_nsub = pn; d.pool_alias = pa;
-    d.P = P;
-    env->pool_set = true;
-    env->reset_done = false;
-    return 0;
+    if (int rc = pool_alloc(b, (size_t)P, (size_t)d.K)) return rc;
+    UAVRL_CUDA(cudaMemcpy(b.start, start, (size_t)P * 3 * sizeof(double), cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(b.goal, goal, (size_t)P * 3 * sizeof(double), cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(b.v0, v0.data(), (size_t)P * 3 * sizeof(double), cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(b.sub, sub, sub_n * sizeof(double), cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(b.nsub, n_sub, (size_t)P * sizeof(int32_t), cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(b.alias, al.data(), (size_t)P, cudaMemcpyHostToDevice));
+    return pool_install(env, b, P);
 }
 
 int uavrl_env_reset(uavrl_env *env, int32_t first, void *stream)
@@ -339,13 +342,10 @@ int uavrl_env_step_host(uavrl_env *env, int32_t action_kind, const void *actions
     if (!env->reset_done) return fail(UAVRL_ERR_STATE, "uavrl_env_step_host before uavrl_env_reset");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
     const size_t n = (size_t)env->d.n;
-    if (!env->h_act_dev) {
-        UAVRL_CUDA(cudaMalloc(&env->h_act_dev, n * sizeof(double)));
-        UAVRL_CUDA(cudaMalloc((void **)&env->h_obs_dev, n * kObsDim * sizeof(float)));
-        UAVRL_CUDA(cudaMalloc((void **)&env->h_rew_dev, n * sizeof(float)));
-        UAVRL_CUDA(cudaMalloc((void **)&env->h_flags_dev, n * 4));
-    }
     cudaStream_t st = env->own_stream;
+    if (int rc = grow(env->staging_mem, env->staging_n, env->d.n, st, false, buf(env->h_act_dev, n), buf(env->h_obs_dev, n * kObsDim),
+                      buf(env->h_rew_dev, n), buf(env->h_flags_dev, n * 4)))
+        return rc;
     const size_t asz = (action_kind == UAVRL_ACT_CONT_F64 || action_kind == UAVRL_ACT_CONT_F32X2) ? 8 : 4;
     UAVRL_CUDA(cudaMemcpyAsync(env->h_act_dev, actions_host, n * asz, cudaMemcpyHostToDevice, st));
     uint8_t *f = env->h_flags_dev;
@@ -407,18 +407,19 @@ int uavrl_env_set_extras(uavrl_env *env, const uavrl_env_extras *x)
     if (x->apf_enabled && !x->obstacle_v_host && env->cfg.n_buildings > 0) return fail(UAVRL_ERR_INVALID, "apf_enabled needs obstacle_v_host");
     if (x->track_envs < 0 || x->track_envs > env->d.n || (x->track_envs > 0 && x->track_capacity <= 0))
         return fail(UAVRL_ERR_INVALID, "track_envs must be in [0, n_envs] with a positive track_capacity");
+    if (x->energy_enabled && (!(x->v_0 > 0) || !(x->F_b > 0))) return fail(UAVRL_ERR_INVALID, "energy model: v_0 and F_b must be > 0");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
-    UAVRL_CUDA(cudaDeviceSynchronize());
-    EnvDev &d = env->d;
-    cudaFree(d.energy); cudaFree((void *)d.apf_obs); cudaFree(d.sub_env); cudaFree(d.path_buf); cudaFree(d.path_n); cudaFree(d.path_cur);
+    // the new extras are built beside the old ones and replace them only once complete
+    EnvDev d = env->d;
+    DevMem m;
     d.energy = nullptr; d.apf_obs = nullptr; d.sub_env = nullptr; d.path_buf = nullptr; d.path_n = nullptr; d.path_cur = nullptr;
     d.extras = 0; d.track_n = 0; d.track_cap = 0;
     const size_t n = (size_t)d.n;
+    int rc;
     if (x->energy_enabled) {
-        if (!(x->v_0 > 0) || !(x->F_b > 0)) return fail(UAVRL_ERR_INVALID, "energy model: v_0 and F_b must be > 0");
         d.pw.P_i = x->P_i; d.pw.v_0 = x->v_0; d.pw.d_0 = x->d_0; d.pw.rho = x->rho; d.pw.s = x->s; d.pw.A = x->A;
         d.pw.P_b = x->P_b; d.pw.F_b = x->F_b; d.pw.xi = x->xi;
-        int rc = dev_alloc(&d.energy, n); if (rc) return rc;
+        if ((rc = m.alloc(d.energy, n))) return rc;
         d.extras |= kExtraEnergy;
     }
     if (x->apf_enabled) {
@@ -437,19 +438,22 @@ int uavrl_env_set_extras(uavrl_env *env, const uavrl_env_extras *x)
             ob[(size_t)i] = o;
         }
         ApfObs *dob = nullptr;
-        UAVRL_CUDA(cudaMalloc((void **)&dob, ob.size() * sizeof(ApfObs)));
+        if ((rc = m.alloc(dob, ob.size(), false))) return rc;
         UAVRL_CUDA(cudaMemcpy(dob, ob.data(), ob.size() * sizeof(ApfObs), cudaMemcpyHostToDevice));
         d.apf_obs = dob;
-        int rc = dev_alloc(&d.sub_env, n * (size_t)d.K * 3); if (rc) return rc;
+        if ((rc = m.alloc(d.sub_env, n * (size_t)d.K * 3))) return rc;
         d.extras |= kExtraApf;
     }
     if (x->track_envs > 0) {
         d.track_n = x->track_envs; d.track_cap = x->track_capacity;
-        int rc = dev_alloc(&d.path_buf, (size_t)2 * d.track_n * d.track_cap * 3); if (rc) return rc;
-        if ((rc = dev_alloc(&d.path_n, (size_t)2 * d.track_n))) return rc;
-        if ((rc = dev_alloc(&d.path_cur, (size_t)d.track_n))) return rc;
+        if ((rc = m.alloc(d.path_buf, (size_t)2 * d.track_n * d.track_cap * 3)) || (rc = m.alloc(d.path_n, (size_t)2 * d.track_n)) ||
+            (rc = m.alloc(d.path_cur, (size_t)d.track_n)))
+            return rc;
         d.extras |= kExtraTrack;
     }
+    UAVRL_CUDA(cudaDeviceSynchronize());                         // nothing may still read the extras being replaced
+    env->extras_mem = std::move(m);
+    env->d = d;
     env->extras_set = true;
     env->reset_done = false;                                     // the new columns are initialised by uavrl_env_reset
     return 0;
@@ -515,14 +519,14 @@ int uavrl_env_threaten_rate(uavrl_env *env, int32_t n, const double *pts_host, u
 {
     if (!env || n <= 0 || !pts_host || !out_host) return fail(UAVRL_ERR_INVALID, "null/empty argument");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
+    DevMem m;
     double *dp = nullptr; uint8_t *dout = nullptr;
-    UAVRL_CUDA(cudaMalloc((void **)&dp, (size_t)n * 3 * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&dout, (size_t)n));
+    int rc;
+    if ((rc = m.alloc(dp, (size_t)n * 3, false)) || (rc = m.alloc(dout, (size_t)n, false))) return rc;
     UAVRL_CUDA(cudaMemcpy(dp, pts_host, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice));
     threat_kernel<<<(n + 127) / 128, 128>>>(env->d, n, dp, dout);
     UAVRL_LAUNCHED();
     UAVRL_CUDA(cudaMemcpy(out_host, dout, (size_t)n, cudaMemcpyDeviceToHost));
-    cudaFree(dp); cudaFree(dout);
     return 0;
 }
 

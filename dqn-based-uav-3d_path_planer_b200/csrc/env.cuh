@@ -51,9 +51,12 @@ constexpr int kExtraEnergy = 1, kExtraApf = 2, kExtraTrack = 4;
 struct uavrl_env {
     uavrl_env_config cfg;
     uavrl::EnvDev d;
+    // owners of the device arrays: cylinders, state columns and counters; the scenario pool; the extras; the host-step staging
+    uavrl::DevMem mem, pool_mem, extras_mem, staging_mem;
     bool pool_set = false, reset_done = false;
-    // staging for the host-buffer entry point
-    void *h_act_dev = nullptr;
+    // staging for the host-buffer entry point, allocated (grow) by its first call: staging_n envs, 0 until then
+    int32_t staging_n = 0;
+    double *h_act_dev = nullptr;
     float *h_obs_dev = nullptr, *h_rew_dev = nullptr;
     uint8_t *h_flags_dev = nullptr;      // done | info | collision | ended, each [n]
     cudaStream_t own_stream = nullptr;
@@ -75,5 +78,9 @@ struct EnvStatsMark {
     int begin(const EnvDev &d, cudaStream_t st, const uavrl_train_stats *out);
     int end(const EnvDev &d, cudaStream_t st, int64_t updates, uavrl_train_stats *out) const;
 };
-void free_pool(EnvDev &d);            // scenario.cu replaces the pool with a device-generated one
+// A scenario pool under construction (uavrl_env_set_pool fills it from the host, uavrl_env_generate_pool on the device):
+// pool_alloc gives it P scenarios of K sub-goals, pool_install waits for the device and swaps it in for the env's pool.
+struct PoolBuild { DevMem mem; double *start, *goal, *v0, *sub; int32_t *nsub; uint8_t *alias; };
+int pool_alloc(PoolBuild &b, size_t P, size_t K);
+int pool_install(uavrl_env *env, PoolBuild &b, int32_t P);
 }  // namespace uavrl

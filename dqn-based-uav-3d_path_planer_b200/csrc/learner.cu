@@ -577,34 +577,25 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
     }
     const int n_tiles = (B + kTile - 1) / kTile;
     const int grid = n_tiles < l->max_ctas ? n_tiles : l->max_ctas;
-    if (grid > l->parts_cap) {                           // grouped learner, batch larger than batch_size: more partial slots
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        cudaFree(l->partials); cudaFree(l->loss_partials);
-        l->partials = nullptr; l->loss_partials = nullptr;
-        int rc;
-        if ((rc = dev_alloc(&l->partials, (size_t)l->G * grid * l->net.P)) || (rc = dev_alloc(&l->loss_partials, (size_t)l->G * grid)))
-            return rc;
-        l->parts_cap = grid;
-    }
+    if (int rc = grow(l->parts_mem, l->parts_cap, grid, st, true,      // grouped learner, batch larger than batch_size: more slots
+                      buf(l->partials, (size_t)l->G * grid * l->net.P), buf(l->loss_partials, (size_t)l->G * grid)))
+        return rc;
     const float *y_in = nullptr;
-    const bool fuse_td = l->tc_ok && l->use_tc && tc_train_can_fuse_td(l, B);
-    if (l->tc_ok && l->use_tc && fuse_td) {
+    // the route follows the learner's flags, never the scratch: y_buf is null after a failed grow until the next one succeeds
+    const bool tc_route = l->tc_ok && l->use_tc;
+    const bool fuse_td = tc_route && tc_train_can_fuse_td(l, B);
+    if (fuse_td) {
         y_in = l->y_buf;                                  // not read: the training kernel forms the TD targets itself
-    } else if (l->tc_ok && l->use_tc) {
+    } else if (tc_route) {
         // TD targets on the tensor cores: y = r + gamma * next_q * (1 - d) for the whole batch, then the
         // update kernel only evaluates the local network (forward on s, backward)
-        if (B > l->y_cap) {
-            UAVRL_CUDA(cudaStreamSynchronize(st));
-            cudaFree(l->y_buf); cudaFree(l->astar_buf);
-            UAVRL_CUDA(cudaMalloc((void **)&l->y_buf, (size_t)l->G * B * 4));
-            UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->G * B * 4));
-            l->y_cap = B;
-        }
+        int rc;
+        if ((rc = grow(l->td_mem, l->y_cap, B, st, false, buf(l->y_buf, (size_t)l->G * B), buf(l->astar_buf, (size_t)l->G * B))))
+            return rc;
         TcArgs a;
         memset(&a, 0, sizeof(a));
         a.src = src; a.n = B; a.n_tiles = (B + kTcTile - 1) / kTcTile; a.use_next = 1; a.gamma = l->cfg.gamma;
         a.actions = l->astar_buf; a.y_out = l->y_buf;
-        int rc;
         if (l->cfg.algo != UAVRL_ALGO_DQN) {             // double DQN: a* = argmax_a q_local(s')
             a.img = l->tc_img_local; a.mode = kTcArgmax;
             if ((rc = launch_tc_forward(l, a, st))) return rc;
@@ -627,16 +618,14 @@ static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, i
         adam_hyper(a, l->cfg.lr, ++l->adam_t);
         a.hard = hard_update_due(l);
     }
-    if (y_in && l->tc_train_ok) {
+    if (tc_route && l->tc_train_ok) {
         // the whole update on the tensor cores: forward + dX chain, then split-K weight gradients (tc_train.cu)
-        if (B > l->train_cap) {
-            UAVRL_CUDA(cudaStreamSynchronize(st));
-            cudaFree(l->act_buf); cudaFree(l->dz_buf);
-            UAVRL_CUDA(cudaMalloc((void **)&l->act_buf, (size_t)l->G * B * (size_t)(l->tc.act_stride > 0 ? l->tc.act_stride : 4) * 4));
-            UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, (size_t)l->G * B * (size_t)l->tc.dz_stride * 4));
-            l->train_cap = B;
-        }
-        int rc = launch_tc_train(l, src, B, global_batch, y_in, &nparts, &n_loss_parts, st, mid ? mid[1] : nullptr, fuse_td);
+        int rc;
+        if ((rc = grow(l->rows_mem, l->train_cap, B, st, false,
+                       buf(l->act_buf, (size_t)l->G * B * (size_t)(l->tc.act_stride > 0 ? l->tc.act_stride : 4)),
+                       buf(l->dz_buf, (size_t)l->G * B * (size_t)l->tc.dz_stride))))
+            return rc;
+        rc = launch_tc_train(l, src, B, global_batch, y_in, &nparts, &n_loss_parts, st, mid ? mid[1] : nullptr, fuse_td);
         if (rc) return rc;
     } else {
     UpdateArgs ua;
@@ -706,7 +695,10 @@ int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_ba
     a.hard = hard_update_due(l);
     a.inv_b = 1.0f / (float)global_batch;
     static const bool dp_trace = getenv("UAVRL_DP_TRACE") != nullptr;
-    if (dp_trace && !l->dp_trace) { UAVRL_CUDA(cudaMalloc((void **)&l->dp_trace, 5 * 8)); UAVRL_CUDA(cudaMemsetAsync(l->dp_trace, 0, 40, st)); }
+    if (dp_trace && !l->dp_trace) {
+        if ((rc = l->mem.alloc(l->dp_trace, 5, false))) return rc;
+        UAVRL_CUDA(cudaMemsetAsync(l->dp_trace, 0, 40, st));
+    }
     const int nblk = (P + 63) / 64;
     UAVRL_CUDA(launch_kernel(dp_allreduce_adam_kernel, dim3(nblk), dim3(256), 0, st, chain && l->pdl_prev == kPdlDw, a, l->last_nparts,
                              l->last_n_loss_parts, (const float *)l->partials, (const float *)l->loss_partials,
@@ -749,6 +741,43 @@ AdamPtrs learner_adam_ptrs(const uavrl_learner *l, float *loss_out)
     return q;
 }
 
+// everything uavrl_learner_create_trainers builds; on failure the caller destroys the half-built handle
+static int learner_init(uavrl_learner *l, const uavrl_learner_config *cfg, int32_t n_trainers)
+{
+    l->cfg = *cfg;
+    l->G = n_trainers;
+    int rc = build_net(*cfg, l->net);
+    if (rc) return rc;
+    // the fp32 kernels hold the whole network in shared memory: refuse a network that does not fit before allocating anything
+    l->dual_weights = upd_smem_bytes(l->net, 1) <= kMaxDynSmem ? 1 : 0;
+    if (upd_smem_bytes(l->net, l->dual_weights) > kMaxDynSmem || act_smem_bytes(l->net) > kMaxDynSmem)
+        return fail(UAVRL_ERR_INVALID, "network too large for the shared-memory resident kernels");
+    const size_t G = (size_t)n_trainers, P = (size_t)l->net.P;
+    l->max_ctas = 4 * num_sms();
+    // gradient / loss partial slots per trainer: one learner keeps max_ctas (any batch); a grouped learner sizes them from the
+    // per-trainer batch (the fp32 update kernel's grid, the largest of the update routes) and grows them for larger batches
+    const int tiles = (cfg->batch_size + kTile - 1) / kTile;
+    l->parts_cap = (G == 1 || tiles > l->max_ctas) ? l->max_ctas : tiles;
+    DevMem &m = l->mem, &pm = l->parts_mem;
+    if ((rc = m.alloc(l->local, G * P)) || (rc = m.alloc(l->target, G * P)) || (rc = m.alloc(l->m, G * P)) ||
+        (rc = m.alloc(l->v, G * P)) || (rc = m.alloc(l->grad, G * P)) ||
+        (rc = pm.alloc(l->partials, G * P * (size_t)l->parts_cap)) || (rc = pm.alloc(l->loss_partials, G * (size_t)l->parts_cap)) ||
+        (rc = m.alloc(l->loss_dev, G)))
+        return rc;
+    {
+        const size_t wf = (size_t)l->net.smem_w_floats;
+        if ((rc = m.alloc(l->img_local, G * wf)) || (rc = m.alloc(l->img_target, G * wf)) || (rc = m.alloc(l->img_map, P))) return rc;
+        std::vector<int32_t> map;
+        build_image_map(l->net, map);
+        UAVRL_CUDA(cudaMemcpy(l->img_map, map.data(), P * sizeof(int32_t), cudaMemcpyHostToDevice));
+    }
+    if ((rc = tc_init(l))) return rc;
+    if ((rc = l->replay.alloc(cfg->replay_capacity, cfg->lockstep_envs, n_trainers, cfg->in_dim, false))) return rc;
+    if ((rc = raise_dyn_smem(act_kernel_t<false>, act_smem_bytes(l->net))) || (rc = raise_dyn_smem(act_kernel_t<true>, act_smem_bytes(l->net))) || (rc = raise_dyn_smem(update_kernel, upd_smem_bytes(l->net, l->dual_weights))))
+        return rc;
+    return 0;
+}
+
 }  // namespace uavrl
 
 using namespace uavrl;
@@ -777,40 +806,7 @@ int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_tra
         return fail(UAVRL_ERR_CUDA, "no CUDA device: the learner has no CPU fallback");
     UAVRL_CUDA(cudaSetDevice(cfg->device));
     uavrl_learner *l = new uavrl_learner();
-    l->cfg = *cfg;
-    l->G = n_trainers;
-    int rc = build_net(*cfg, l->net);
-    if (rc) { delete l; return rc; }
-    // the fp32 kernels hold the whole network in shared memory: refuse a network that does not fit before allocating anything
-    l->dual_weights = upd_smem_bytes(l->net, 1) <= kMaxDynSmem ? 1 : 0;
-    if (upd_smem_bytes(l->net, l->dual_weights) > kMaxDynSmem || act_smem_bytes(l->net) > kMaxDynSmem) {
-        delete l;
-        return fail(UAVRL_ERR_INVALID, "network too large for the shared-memory resident kernels");
-    }
-    const size_t G = (size_t)n_trainers, P = (size_t)l->net.P;
-    l->max_ctas = 4 * num_sms();
-    // gradient / loss partial slots per trainer: one learner keeps max_ctas (any batch); a grouped learner sizes them from the
-    // per-trainer batch (the fp32 update kernel's grid, the largest of the update routes) and grows them for larger batches
-    {
-        const int tiles = (cfg->batch_size + kTile - 1) / kTile;
-        l->parts_cap = (G == 1 || tiles > l->max_ctas) ? l->max_ctas : tiles;
-    }
-    if ((rc = dev_alloc(&l->local, G * P)) || (rc = dev_alloc(&l->target, G * P)) || (rc = dev_alloc(&l->m, G * P)) ||
-        (rc = dev_alloc(&l->v, G * P)) || (rc = dev_alloc(&l->grad, G * P)) ||
-        (rc = dev_alloc(&l->partials, G * P * (size_t)l->parts_cap)) || (rc = dev_alloc(&l->loss_partials, G * (size_t)l->parts_cap)) ||
-        (rc = dev_alloc(&l->loss_dev, G)))
-        return rc;
-    {
-        const size_t wf = (size_t)l->net.smem_w_floats;
-        if ((rc = dev_alloc(&l->img_local, G * wf)) || (rc = dev_alloc(&l->img_target, G * wf)) || (rc = dev_alloc(&l->img_map, P))) return rc;
-        std::vector<int32_t> map;
-        build_image_map(l->net, map);
-        UAVRL_CUDA(cudaMemcpy(l->img_map, map.data(), P * sizeof(int32_t), cudaMemcpyHostToDevice));
-    }
-    if ((rc = tc_init(l))) return rc;
-    if ((rc = l->replay.alloc(cfg->replay_capacity, cfg->lockstep_envs, n_trainers, cfg->in_dim, false))) return rc;
-    if ((rc = raise_dyn_smem(act_kernel_t<false>, act_smem_bytes(l->net))) || (rc = raise_dyn_smem(act_kernel_t<true>, act_smem_bytes(l->net))) || (rc = raise_dyn_smem(update_kernel, upd_smem_bytes(l->net, l->dual_weights))))
-        return rc;
+    if (int rc = learner_init(l, cfg, n_trainers)) { uavrl_learner_destroy(l); return rc; }
     *out = l;
     return 0;
 }
@@ -825,18 +821,11 @@ int uavrl_learner_destroy(uavrl_learner *l)
         cudaMemcpy(h, l->dp_trace, sizeof(h), cudaMemcpyDeviceToHost);
         if (h[4]) fprintf(stderr, "[dp_trace] rank %d/%d: %llu launches, block 0 mean ns: reduce %.0f  push %.0f  wait for peers' words %.0f  adam %.0f\n",
                           l->rank, l->world, h[4], (double)h[0] / h[4], (double)h[1] / h[4], (double)h[2] / h[4], (double)h[3] / h[4]);
-        cudaFree(l->dp_trace);
     }
     for (int q = 0; q < l->world && l->comm_ready; ++q) {
         if (q == l->rank) continue;
         if (l->peer_grad_host[q]) cudaIpcCloseMemHandle(l->peer_grad_host[q]);
     }
-    l->replay.release();
-    void *ptrs[] = { l->local, l->target, l->m, l->v, l->grad, l->partials, l->loss_partials, l->loss_dev, l->comm_grad, l->peer_grad_dev, l->img_local, l->img_target,
-                     l->img_map, l->tc_img_local, l->tc_img_target, l->tc_hi_map, l->tc_lo_map, l->y_buf, l->astar_buf, l->tc_hi2_map,
-                     l->tc_lo2_map, l->act_buf, l->dz_buf };
-    for (void *p : ptrs) cudaFree(p);
-    per_free(l);
     delete l;
     return 0;
 }
@@ -1078,19 +1067,17 @@ int uavrl_learner_comm_init(uavrl_learner *l, int32_t rank, int32_t world, void 
         return fail(UAVRL_ERR_INVALID, "bad rank/world/handle pointer");
     if (int rc = refuse_grouped(l, "uavrl_learner_comm_init (data-parallel training)")) return rc;
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    l->rank = rank; l->world = world;
-    if (l->comm_grad && l->comm_world != world) {                // re-initialised with another world size
-        UAVRL_CUDA(cudaDeviceSynchronize());
-        cudaFree(l->comm_grad);
-        l->comm_grad = nullptr;
-    }
-    l->comm_world = world;
-    if (!l->comm_grad) {
+    if (!l->comm_grad || l->comm_world != world) {               // first call, or re-initialised with another world size
         // recv[2][world][P+1] words of 8 bytes {epoch : value} (epoch 0 = never written)
         const size_t n = 2 * (size_t)world * ((size_t)l->net.P + 1);
-        UAVRL_CUDA(cudaMalloc((void **)&l->comm_grad, n * sizeof(unsigned long long)));
-        UAVRL_CUDA(cudaMemset(l->comm_grad, 0, n * sizeof(unsigned long long)));
+        DevMem m;
+        unsigned long long *recv = nullptr;
+        if (int rc = m.alloc(recv, n)) return rc;
+        UAVRL_CUDA(cudaDeviceSynchronize());                     // nothing may still use the buffer being replaced
+        l->comm_mem = std::move(m);
+        l->comm_grad = (float *)recv; l->comm_world = world;
     }
+    l->rank = rank; l->world = world;
     cudaIpcMemHandle_t hg;
     UAVRL_CUDA(cudaIpcGetMemHandle(&hg, l->comm_grad));
     memcpy(grad_handle_out, &hg, sizeof(hg));
@@ -1109,9 +1096,12 @@ int uavrl_learner_comm_connect(uavrl_learner *l, const void *grad_handles, const
         memcpy(&hg, (const char *)grad_handles + (size_t)q * sizeof(hg), sizeof(hg));
         UAVRL_CUDA(cudaIpcOpenMemHandle(&l->peer_grad_host[q], hg, cudaIpcMemLazyEnablePeerAccess));
     }
-    cudaFree(l->peer_grad_dev);
-    UAVRL_CUDA(cudaMalloc((void **)&l->peer_grad_dev, sizeof(void *) * l->world));
-    UAVRL_CUDA(cudaMemcpy(l->peer_grad_dev, l->peer_grad_host, sizeof(void *) * l->world, cudaMemcpyHostToDevice));
+    DevMem m;
+    float **table = nullptr;
+    if (int rc = m.alloc(table, (size_t)l->world, false)) return rc;
+    UAVRL_CUDA(cudaMemcpy(table, l->peer_grad_host, sizeof(void *) * l->world, cudaMemcpyHostToDevice));
+    l->peer_mem = std::move(m);                                  // cudaFree of the old table waits for the device
+    l->peer_grad_dev = table;
     l->comm_ready = true;
     return 0;
 }

@@ -165,6 +165,9 @@ struct uavrl_learner {
     unsigned comm_epoch = 0;          // tag of the latest exchange (launch_update_dp); 0 = never written
     int last_nparts = 0, last_n_loss_parts = 0;
     int last_global_batch = 0;
+    // owners of the buffers above, one per group allocated and replaced together: parameters, images, maps and dp_trace; the
+    // grown scratch (partials, y / astar, act / dz rows); the receive buffer; the peer table; the PER trees; their scratch
+    uavrl::DevMem mem, parts_mem, td_mem, rows_mem, comm_mem, peer_mem, per_mem, per_scratch_mem;
 };
 
 namespace uavrl {

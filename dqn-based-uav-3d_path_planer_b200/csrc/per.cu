@@ -184,15 +184,9 @@ int per_sample(uavrl_learner *l, int B, const double *u_tape, int32_t *slot_out,
 {
     PerDev &p = l->per;
     const size_t G = (size_t)p.G;
-    if (B > p.scratch_cap) {
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        cudaFree(p.idx); cudaFree(p.w); cudaFree(p.abs_err); cudaFree(p.w_raw);
-        UAVRL_CUDA(cudaMalloc((void **)&p.idx, G * B * 4));
-        UAVRL_CUDA(cudaMalloc((void **)&p.w, G * B * 4));
-        UAVRL_CUDA(cudaMalloc((void **)&p.abs_err, G * B * 4));
-        UAVRL_CUDA(cudaMalloc((void **)&p.w_raw, G * B * 8));
-        p.scratch_cap = B;
-    }
+    if (int rc = grow(l->per_scratch_mem, p.scratch_cap, B, st, false, buf(p.idx, G * B), buf(p.w, G * B), buf(p.abs_err, G * B),
+                      buf(p.w_raw, G * B)))
+        return rc;
     p.beta = fmin(1.0, p.beta + p.beta_inc);                  // :195
     UAVRL_CUDA(cudaMemsetAsync(p.wmax_bits, 0, G * 8, st));
     int grid = (B + 7) / 8;                                   // per trainer, as a stand-alone learner picks it
@@ -205,15 +199,6 @@ int per_sample(uavrl_learner *l, int B, const double *u_tape, int32_t *slot_out,
     UAVRL_LAUNCHED();
     l->pdl_prev = kPdlNone;
     return 0;
-}
-
-void per_free(uavrl_learner *l)
-{
-    PerDev &p = l->per;
-    if (!p.enabled) return;
-    cudaFree(p.leaf); cudaFree(p.l1); cudaFree(p.l2); cudaFree(p.idx); cudaFree(p.w); cudaFree(p.abs_err); cudaFree(p.w_raw);
-    cudaFree(p.wmax_bits);
-    memset(&p, 0, sizeof(p));
 }
 
 }  // namespace uavrl
@@ -229,7 +214,7 @@ static int per_enable_impl(uavrl_learner *l, double alpha, double beta0, double 
     if (l->G > 1 && l->replay.mode != kReplayLockstep)
         return fail(UAVRL_ERR_INVALID, "prioritised replay on a learner with several trainers needs the lockstep ring (lockstep_envs > 0)");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    PerDev &p = l->per;
+    PerDev p;                                                     // swapped in once complete
     memset(&p, 0, sizeof(p));
     p.G = l->G;
     p.cap = l->replay.slots / l->G;                               // trainer-local slots: ring_frames x Ng
@@ -242,10 +227,13 @@ static int per_enable_impl(uavrl_learner *l, double alpha, double beta0, double 
     p.eps = eps >= 0 ? eps : 0.01; p.err_upper = err_upper >= 0 ? err_upper : 1.0;
     int rc;
     const size_t G = (size_t)p.G;
-    if ((rc = dev_alloc(&p.leaf, G * p.cap)) || (rc = dev_alloc(&p.l1, G * p.n1)) || (rc = dev_alloc(&p.l2, G * p.n2)) ||
-        (rc = dev_alloc(&p.wmax_bits, G)))
+    DevMem m;
+    if ((rc = m.alloc(p.leaf, G * p.cap)) || (rc = m.alloc(p.l1, G * p.n1)) || (rc = m.alloc(p.l2, G * p.n2)) ||
+        (rc = m.alloc(p.wmax_bits, G)))
         return rc;
     p.enabled = 1;
+    l->per = p;
+    l->per_mem = std::move(m);
     return 0;
 }
 

@@ -51,5 +51,4 @@ int per_fill_range(uavrl_learner *l, int64_t first_slot, int64_t n, double value
 inline double per_new_priority(const PerDev &p) { return (double)powf((float)p.eps, (float)p.alpha); }
 int per_sample(uavrl_learner *l, int B, const double *u_tape, int32_t *slot_out, float *w_out, cudaStream_t st);
 int per_set(uavrl_learner *l, int n, const int32_t *slots, const double *prio, const float *abs_err, int clip, cudaStream_t st);
-void per_free(uavrl_learner *l);
 }  // namespace uavrl

@@ -42,16 +42,10 @@ int ReplayStore::alloc(int64_t capacity, int32_t n_envs, int32_t n_trainers, int
         rows = 2 * (size_t)slots;
     }
     int rc;
-    if ((rc = dev_alloc(&frames, rows * in)) || (rc = pair_actions ? dev_alloc(&act2, 2 * (size_t)slots) : dev_alloc(&act, (size_t)slots)) ||
-        (rc = dev_alloc(&rew, (size_t)slots)) || (rc = dev_alloc(&done, (size_t)slots)))
+    if ((rc = mem.alloc(frames, rows * in)) || (rc = pair_actions ? mem.alloc(act2, 2 * (size_t)slots) : mem.alloc(act, (size_t)slots)) ||
+        (rc = mem.alloc(rew, (size_t)slots)) || (rc = mem.alloc(done, (size_t)slots)))
         return rc;
     return 0;
-}
-
-void ReplayStore::release()
-{
-    cudaFree(frames); cudaFree(act); cudaFree(act2); cudaFree(rew); cudaFree(done);
-    frames = nullptr; act = nullptr; act2 = nullptr; rew = nullptr; done = nullptr;
 }
 
 BatchSrc ReplayStore::source(uint64_t seed, int64_t epoch, const int32_t *idx_tape) const
@@ -113,16 +107,14 @@ int ReplayStore::gather(int32_t n, const int64_t *idx, float *s, int32_t *a, flo
     const size_t in = (size_t)in_dim;
     // one gather kernel into a packed staging block, then one device->host copy per output array
     int64_t *d_idx = nullptr; float *d_s = nullptr, *d_s2 = nullptr, *d_a2 = nullptr, *d_r = nullptr; int32_t *d_a = nullptr; uint8_t *d_d = nullptr;
-    struct Free { void **p[7]; ~Free() { for (auto q : p) if (*q) cudaFree(*q); } } guard{ { (void **)&d_idx, (void **)&d_s, (void **)&d_s2,
-                                                                                             (void **)&d_a, (void **)&d_a2, (void **)&d_r, (void **)&d_d } };
-    UAVRL_CUDA(cudaMalloc((void **)&d_idx, (size_t)n * 8));
+    DevMem m;
+    int rc;
+    if ((rc = m.alloc(d_idx, (size_t)n, false))) return rc;
     UAVRL_CUDA(cudaMemcpy(d_idx, idx, (size_t)n * 8, cudaMemcpyHostToDevice));
-    if (s) UAVRL_CUDA(cudaMalloc((void **)&d_s, (size_t)n * in * 4));
-    if (s2) UAVRL_CUDA(cudaMalloc((void **)&d_s2, (size_t)n * in * 4));
-    if (a) UAVRL_CUDA(cudaMalloc((void **)&d_a, (size_t)n * 4));
-    if (a2) UAVRL_CUDA(cudaMalloc((void **)&d_a2, (size_t)n * 2 * 4));
-    if (r) UAVRL_CUDA(cudaMalloc((void **)&d_r, (size_t)n * 4));
-    if (d) UAVRL_CUDA(cudaMalloc((void **)&d_d, (size_t)n));
+    if ((s && (rc = m.alloc(d_s, (size_t)n * in, false))) || (s2 && (rc = m.alloc(d_s2, (size_t)n * in, false))) ||
+        (a && (rc = m.alloc(d_a, (size_t)n, false))) || (a2 && (rc = m.alloc(d_a2, (size_t)n * 2, false))) ||
+        (r && (rc = m.alloc(d_r, (size_t)n, false))) || (d && (rc = m.alloc(d_d, (size_t)n, false))))
+        return rc;
     replay_gather_kernel<<<(n + 7) / 8, 256>>>(n, (int)in, src, d_idx, d_s, d_s2, d_a, d_a2, d_r, d_d);
     UAVRL_CUDA(cudaGetLastError());
     if (s) UAVRL_CUDA(cudaMemcpy(s, d_s, (size_t)n * in * 4, cudaMemcpyDeviceToHost));

@@ -182,11 +182,11 @@ struct ReplayStore {
     int64_t head = 0;                 // paired: next slot to write ; lockstep: frame holding obs_t
     int64_t count = 0;                // valid transitions
     bool frame0_valid = false;        // lockstep: frame `head` holds the current observations
+    DevMem mem;                       // owns frames, act / act2, rew and done
 
     // capacity transitions over all trainers; N > 0: lockstep ring, where every trainer keeps the frames a stand-alone store
     // with capacity / G transitions over N / G envs would keep (at least 2); N == 0: paired rows
     int alloc(int64_t capacity, int32_t n_envs, int32_t n_trainers, int32_t in, bool pair_actions);
-    void release();
     // trainer-local sampling: Philox keyed by seed ^ kSampleSalt and the epoch, or a device tape of logical indices
     BatchSrc source(uint64_t seed, int64_t epoch, const int32_t *idx_tape) const;
     // lockstep iteration: where this iteration's observations, actions, rewards and done flags go; commit makes them a

@@ -544,6 +544,7 @@ struct uavrl_sac {
     int64_t epoch = 0, adam_t = 0;
     uint64_t calls = 0;
     ReplayStore replay;                                    // lockstep ring (float[2] actions); none when lockstep_envs == 0
+    DevMem mem, parts_mem, td_mem;                         // owners: networks, moments, maps, scalars; partials / stat; td
 };
 
 static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
@@ -587,26 +588,11 @@ static AdamPtrs sac_adam_ptrs(const uavrl_sac *s, int r)
 // larger explicit batch arrives; TD targets likewise
 static int sac_scratch(uavrl_sac *s, int B, int grid, cudaStream_t st)
 {
-    const size_t G = (size_t)s->G;
-    int rc;
-    if (grid > s->parts_cap) {
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        for (int r = 0; r < 3; ++r) { cudaFree(s->part[r]); s->part[r] = nullptr; }
-        cudaFree(s->stat); s->stat = nullptr;
-        s->parts_cap = 0;
-        for (int r = 0; r < 3; ++r)
-            if ((rc = dev_alloc(&s->part[r], G * grid * (size_t)(r == 0 ? s->sh.actor.P : s->sh.critic.P)))) return rc;
-        if ((rc = dev_alloc(&s->stat, G * grid * 4))) return rc;
-        s->parts_cap = grid;
-    }
-    if (B > s->td_cap) {
-        UAVRL_CUDA(cudaStreamSynchronize(st));
-        cudaFree(s->td); s->td = nullptr;
-        s->td_cap = 0;
-        if ((rc = dev_alloc(&s->td, G * B * kSacA))) return rc;
-        s->td_cap = B;
-    }
-    return 0;
+    const size_t G = (size_t)s->G, Pa = (size_t)s->sh.actor.P, Pc = (size_t)s->sh.critic.P;
+    if (int rc = grow(s->parts_mem, s->parts_cap, grid, st, true, buf(s->part[0], G * grid * Pa), buf(s->part[1], G * grid * Pc),
+                      buf(s->part[2], G * grid * Pc), buf(s->stat, G * grid * 4)))
+        return rc;
+    return grow(s->td_mem, s->td_cap, B, st, true, buf(s->td, G * B * kSacA));
 }
 
 // one SAC_Trainer.update of every trainer on the batch described by src (B rows per trainer)
@@ -658,18 +644,19 @@ static int sac_alloc(uavrl_sac *s)
 {
     const uavrl_sac_config *cfg = &s->cfg;
     const size_t G = (size_t)s->G;
+    DevMem &mem = s->mem;
     int rc;
     for (int r = 0; r < 5; ++r) {
         const NetDev &n = r == 0 ? s->sh.actor : s->sh.critic;
-        if ((rc = dev_alloc(&s->p[r], G * n.P)) || (rc = dev_alloc(&s->img[r], G * n.smem_w_floats))) return rc;
+        if ((rc = mem.alloc(s->p[r], G * n.P)) || (rc = mem.alloc(s->img[r], G * n.smem_w_floats))) return rc;
     }
     for (int r = 0; r < 3; ++r) {
         const NetDev &n = r == 0 ? s->sh.actor : s->sh.critic;
-        if ((rc = dev_alloc(&s->m[r], G * n.P)) || (rc = dev_alloc(&s->v[r], G * n.P)) || (rc = dev_alloc(&s->grad[r], G * n.P))) return rc;
+        if ((rc = mem.alloc(s->m[r], G * n.P)) || (rc = mem.alloc(s->v[r], G * n.P)) || (rc = mem.alloc(s->grad[r], G * n.P))) return rc;
     }
     std::vector<int32_t> ma, mc;
     build_image_map(s->sh.actor, ma); build_image_map(s->sh.critic, mc);
-    if ((rc = dev_alloc(&s->map_a, ma.size())) || (rc = dev_alloc(&s->map_c, mc.size()))) return rc;
+    if ((rc = mem.alloc(s->map_a, ma.size())) || (rc = mem.alloc(s->map_c, mc.size()))) return rc;
     UAVRL_CUDA(cudaMemcpy(s->map_a, ma.data(), ma.size() * 4, cudaMemcpyHostToDevice));
     UAVRL_CUDA(cudaMemcpy(s->map_c, mc.data(), mc.size() * 4, cudaMemcpyHostToDevice));
     {   // gradient partial / stat slots per trainer: one learner keeps max_ctas (any batch); a grouped learner sizes them from the
@@ -678,7 +665,7 @@ static int sac_alloc(uavrl_sac *s)
         const int cap = (G == 1 || tiles > s->max_ctas) ? s->max_ctas : tiles;
         if ((rc = sac_scratch(s, cfg->batch_size, cap, 0))) return rc;
     }
-    if ((rc = dev_alloc(&s->scal, 3 * G)) || (rc = dev_alloc(&s->out, 4 * G)) || (rc = dev_alloc(&s->lossbuf, 1))) return rc;
+    if ((rc = mem.alloc(s->scal, 3 * G)) || (rc = mem.alloc(s->out, 4 * G)) || (rc = mem.alloc(s->lossbuf, 1))) return rc;
     std::vector<float> init(3 * G, 0.f);
     for (size_t g = 0; g < G; ++g) init[3 * g] = logf(0.01f);          // SAC_Trainer.py:53
     UAVRL_CUDA(cudaMemcpy(s->scal, init.data(), init.size() * 4, cudaMemcpyHostToDevice));
@@ -747,7 +734,6 @@ int uavrl_sac_create_trainers(const uavrl_sac_config *cfg, int32_t n_trainers, u
     }
     if ((rc = sac_alloc(s))) {
         uavrl_sac_destroy(s);
-        cudaGetLastError();                                  // a failed cudaMalloc must not surface at the next launch check
         return rc;
     }
     *out = s;
@@ -759,11 +745,6 @@ int uavrl_sac_destroy(uavrl_sac *s)
     if (!s) return 0;
     cudaSetDevice(s->cfg.device);
     cudaDeviceSynchronize();
-    for (int r = 0; r < 5; ++r) { cudaFree(s->p[r]); cudaFree(s->img[r]); }
-    for (int r = 0; r < 3; ++r) { cudaFree(s->m[r]); cudaFree(s->v[r]); cudaFree(s->grad[r]); cudaFree(s->part[r]); }
-    void *ptrs[] = { s->map_a, s->map_c, s->stat, s->scal, s->out, s->td, s->lossbuf };
-    for (void *p : ptrs) cudaFree(p);
-    s->replay.release();
     delete s;
     return 0;
 }

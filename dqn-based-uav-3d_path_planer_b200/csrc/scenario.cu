@@ -217,36 +217,23 @@ extern "C" int uavrl_env_generate_pool(uavrl_env *env, int32_t P, uint64_t seed,
     RrtCity c;
     c.k = d.k; c.len = env->cfg.len; c.cyl = d.cyl;
     const double step = rrt_step > 0 ? (double)rrt_step : 30.0;
-    double *ps, *pg, *pv, *pq; int32_t *pn; uint8_t *pa; int *failed;
-    const size_t sub_n = (size_t)P * d.K * 3;
-    UAVRL_CUDA(cudaMalloc((void **)&ps, (size_t)P * 3 * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&pg, (size_t)P * 3 * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&pv, (size_t)P * 3 * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&pq, sub_n * sizeof(double)));
-    UAVRL_CUDA(cudaMalloc((void **)&pn, (size_t)P * sizeof(int32_t)));
-    UAVRL_CUDA(cudaMalloc((void **)&pa, (size_t)P));
-    UAVRL_CUDA(cudaMalloc((void **)&failed, sizeof(int)));
+    PoolBuild b;
+    DevMem tmp;
+    int *failed = nullptr;
+    int rc;
+    if ((rc = pool_alloc(b, (size_t)P, (size_t)d.K)) || (rc = tmp.alloc(failed, 1, false))) return rc;
     UAVRL_CUDA(cudaMemsetAsync(failed, 0, sizeof(int), st));
     const size_t smem = sizeof(WarpTree) * kRrtWarpsPerCta;          // 2 x 18 KB
     UAVRL_CUDA(cudaFuncSetAttribute(rrt_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   // per device: set on every call
     const int blocks = (P + kRrtWarpsPerCta - 1) / kRrtWarpsPerCta;
-    rrt_pool_kernel<<<blocks, 32 * kRrtWarpsPerCta, smem, st>>>(c, seed, P, step, d.K, ps, pg, pv, pq, pn, pa, failed);
+    rrt_pool_kernel<<<blocks, 32 * kRrtWarpsPerCta, smem, st>>>(c, seed, P, step, d.K, b.start, b.goal, b.v0, b.sub, b.nsub, b.alias,
+                                                                 failed);
     UAVRL_LAUNCHED();
     int h_failed = 0;
     UAVRL_CUDA(cudaMemcpyAsync(&h_failed, failed, sizeof(int), cudaMemcpyDeviceToHost, st));
     UAVRL_CUDA(cudaStreamSynchronize(st));
-    cudaFree(failed);
-    if (h_failed) {
-        cudaFree(ps); cudaFree(pg); cudaFree(pv); cudaFree(pq); cudaFree(pn); cudaFree(pa);
-        return fail(UAVRL_ERR_INVALID, "device RRT found no path within max_subgoals for a scenario");
-    }
-    UAVRL_CUDA(cudaDeviceSynchronize());            // nothing may still read the pool being replaced
-    free_pool(d);
-    d.pool_start = ps; d.pool_goal = pg; d.pool_v0 = pv; d.pool_sub = pq; d.pool_nsub = pn; d.pool_alias = pa;
-    d.P = P;
-    env->pool_set = true;
-    env->reset_done = false;
-    return 0;
+    if (h_failed) return fail(UAVRL_ERR_INVALID, "device RRT found no path within max_subgoals for a scenario");
+    return pool_install(env, b, P);
 }
 
 extern "C" int uavrl_env_get_pool(uavrl_env *env, double *start, double *goal, double *v0, double *sub, int32_t *n_sub)

@@ -299,24 +299,20 @@ template <bool D>
 static ForwardKernel pick_loss_d(bool fixed) { return fixed ? tc_loss_kernel_t<D, true> : tc_loss_kernel_t<D, false>; }
 static ForwardKernel pick_loss_kernel(bool dueling, bool fixed) { return dueling ? pick_loss_d<true>(fixed) : pick_loss_d<false>(fixed); }
 
-int stage_trace_alloc(long long **t)
+int stage_trace_alloc(DevMem &m, long long *&t)
 {
     static const bool on = getenv("UAVRL_TC_TRACE") != nullptr;
-    *t = nullptr;
+    t = nullptr;
     if (!on) return 0;
-    UAVRL_CUDA(cudaMalloc((void **)t, kTraceSlots * sizeof(long long)));
-    UAVRL_CUDA(cudaMemset(*t, 0, kTraceSlots * sizeof(long long)));
-    return 0;
+    return m.alloc(t, kTraceSlots);
 }
 
-int stage_trace_print(cudaStream_t st, long long *t, const char *fmt, ...)
+int stage_trace_print(cudaStream_t st, const long long *t, const char *fmt, ...)
 {
     if (!t) return 0;
     long long h[kTraceSlots];
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess) e = cudaMemcpy(h, t, sizeof(h), cudaMemcpyDeviceToHost);
-    cudaFree(t);
-    UAVRL_CUDA(e);
+    UAVRL_CUDA(cudaStreamSynchronize(st));
+    UAVRL_CUDA(cudaMemcpy(h, t, sizeof(h), cudaMemcpyDeviceToHost));
     va_list ap;
     va_start(ap, fmt);
     vfprintf(stderr, fmt, ap);
@@ -341,7 +337,8 @@ int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st)
     a.rows_per_tile = tc_forward_rows_per_tile(l->tc, a.n);
     a.n_tiles = (a.n + a.rows_per_tile - 1) / a.rows_per_tile;
     const int grid = a.n_tiles < n_sm ? a.n_tiles : n_sm;
-    if (int rc = stage_trace_alloc(&a.trace)) return rc;
+    DevMem trace_mem;
+    if (int rc = stage_trace_alloc(trace_mem, a.trace)) return rc;
     // PDL chain state (see common.cuh): what this kernel may touch before its griddepcontrol.wait
     const int prev = (l->pdl_chain && g_pdl.load()) ? l->pdl_prev : kPdlNone;
     a.pdl = 0;
@@ -393,23 +390,21 @@ int tc_init(uavrl_learner *l)
     const size_t P = (size_t)l->net.P;
     const size_t img = (size_t)l->tc.train_img_bytes;
     const size_t img_all = (size_t)l->G * img;                  // [G] images of a grouped learner
-    UAVRL_CUDA(cudaMalloc((void **)&l->tc_img_local, img_all));
-    UAVRL_CUDA(cudaMalloc((void **)&l->tc_img_target, img_all));
-    UAVRL_CUDA(cudaMemset(l->tc_img_local, 0, img_all));
-    UAVRL_CUDA(cudaMemset(l->tc_img_target, 0, img_all));
+    int rc;
+    if ((rc = l->mem.alloc(l->tc_img_local, img_all)) || (rc = l->mem.alloc(l->tc_img_target, img_all))) return rc;
     int32_t **maps[] = { &l->tc_hi_map, &l->tc_lo_map, &l->tc_hi2_map, &l->tc_lo2_map };
     std::vector<int32_t> *src[] = { &hi, &lo, &hi2, &lo2 };
     for (int i = 0; i < 4; ++i) {
-        UAVRL_CUDA(cudaMalloc((void **)maps[i], P * 4));
+        if ((rc = l->mem.alloc(*maps[i], P, false))) return rc;
         UAVRL_CUDA(cudaMemcpy(*maps[i], src[i]->data(), P * 4, cudaMemcpyHostToDevice));
     }
-    UAVRL_CUDA(cudaMalloc((void **)&l->y_buf, (size_t)l->G * l->cfg.batch_size * 4));
-    UAVRL_CUDA(cudaMalloc((void **)&l->astar_buf, (size_t)l->G * l->cfg.batch_size * 4));
+    const size_t B = (size_t)l->G * l->cfg.batch_size;
+    if ((rc = l->td_mem.alloc(l->y_buf, B, false)) || (rc = l->td_mem.alloc(l->astar_buf, B, false))) return rc;
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du)
-            if (int rc = raise_dyn_smem(pick_forward_kernel(ac != 0, du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
+            if ((rc = raise_dyn_smem(pick_forward_kernel(ac != 0, du != 0, fixed), tc_smem_bytes(l->tc)))) return rc;
     for (int du = 0; du < 2; ++du)                               // the loss variant: the act kernel's static shared memory
-        if (int rc = raise_dyn_smem(pick_loss_kernel(du != 0, fixed), tc_smem_bytes(l->tc))) return rc;
+        if ((rc = raise_dyn_smem(pick_loss_kernel(du != 0, fixed), tc_smem_bytes(l->tc)))) return rc;
     l->y_cap = l->cfg.batch_size;
     l->tc_ok = true;
     return tc_train_init(l);

@@ -54,11 +54,11 @@ int launch_tc_loss(uavrl_learner *l, const TcArgs &a, int n_weights, int max_row
 int tc_init(uavrl_learner *l);        // builds the TC images/maps; leaves l->tc_ok = false when the net does not fit
 
 // Stage timestamps of the tensor-core kernels (UAVRL_TC_TRACE=1, DESIGN §7): stage_trace_alloc gives a zeroed device buffer of
-// kTraceSlots clock64() slots, or nullptr when tracing is off; stage_trace_print (nothing for nullptr) waits for the stream,
-// frees the buffer and prints one stderr line, the printf-formatted label then "cycles since start:" and [i]=t_i - t_0 for
-// every written slot i >= 1.
+// kTraceSlots clock64() slots owned by m, or nullptr when tracing is off; stage_trace_print (nothing for nullptr) waits for the
+// stream and prints one stderr line, the printf-formatted label then "cycles since start:" and [i]=t_i - t_0 for every written
+// slot i >= 1.
 constexpr int kTraceSlots = 32;
-int stage_trace_alloc(long long **t);
-int stage_trace_print(cudaStream_t st, long long *t, const char *fmt, ...);
+int stage_trace_alloc(DevMem &m, long long *&t);
+int stage_trace_print(cudaStream_t st, const long long *t, const char *fmt, ...);
 
 }  // namespace uavrl

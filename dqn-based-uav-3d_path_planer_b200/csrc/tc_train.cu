@@ -530,8 +530,8 @@ int tc_train_init(uavrl_learner *l)
             if (int rc = raise_dyn_smem(pick_train_kernel(np, du != 0, fixed), train_smem_bytes(tc, tc.train_max_rows))) return rc;
     if (int rc = raise_dyn_smem(tc_dw_kernel, dw_smem_bytes(tc))) return rc;
     const size_t cap = (size_t)l->cfg.batch_size, G = (size_t)l->G;
-    UAVRL_CUDA(cudaMalloc((void **)&l->act_buf, G * cap * (size_t)(tc.act_stride > 0 ? tc.act_stride : 4) * 4));
-    UAVRL_CUDA(cudaMalloc((void **)&l->dz_buf, G * cap * (size_t)tc.dz_stride * 4));
+    if (int rc = l->rows_mem.alloc(l->act_buf, G * cap * (size_t)(tc.act_stride > 0 ? tc.act_stride : 4), false)) return rc;
+    if (int rc = l->rows_mem.alloc(l->dz_buf, G * cap * (size_t)tc.dz_stride, false)) return rc;
     l->train_cap = (int32_t)cap;
     l->tc_train_ok = true;
     return 0;
@@ -570,8 +570,9 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     if (fused_td && a.n_tiles > grid) return fail(UAVRL_ERR_INVALID, "fused TD needs one tile per CTA");
     TcDwArgs d;
     memset(&d, 0, sizeof(d));
-    if (int rc = stage_trace_alloc(&a.trace)) return rc;
-    if (int rc = stage_trace_alloc(&d.trace)) { cudaFree(a.trace); return rc; }
+    DevMem trace_mem;
+    if (int rc = stage_trace_alloc(trace_mem, a.trace)) return rc;
+    if (int rc = stage_trace_alloc(trace_mem, d.trace)) return rc;
     const bool use_pdl = chain && (fused_td ? (l->pdl_prev == kPdlEnv) : (l->pdl_prev == kPdlTd));
     const int npre = fused_td ? (l->cfg.algo != UAVRL_ALGO_DQN ? 2 : 1) : 0;
     UAVRL_CUDA(launch_kernel(pick_train_kernel(npre, tc.dueling != 0, tc_fixed_chains(tc, true)), dim3(grid, l->G), dim3(kTcThreads),
@@ -590,7 +591,7 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     l->pdl_prev = chain ? kPdlDw : kPdlNone;
     UAVRL_LAUNCHED();
     const int rc_train = stage_trace_print(st, a.trace, "[train_trace] B=%d R=%d fused_td=%d", B, a.R, a.fused_td);
-    const int rc_dw = stage_trace_print(st, d.trace, "[dw_trace] B=%d chunks=%d (CTA 0 = layer 0)", B, d.n_chunks);     // frees d.trace either way
+    const int rc_dw = stage_trace_print(st, d.trace, "[dw_trace] B=%d chunks=%d (CTA 0 = layer 0)", B, d.n_chunks);
     if (rc_train || rc_dw) return rc_train ? rc_train : rc_dw;
     *n_grad_parts = d.n_slices;
     *n_loss_parts = grid;

@@ -14,6 +14,10 @@
  *   - `stream` is a cudaStream_t passed as void* (NULL = the legacy default stream).  All work is
  *     enqueued on it; there are no hidden synchronisations except where a _host output is written.
  *   - one host thread per handle.
+ *   - a call that runs out of device memory returns UAVRL_ERR_CUDA ("out of memory") and leaves the handle usable: a create
+ *     frees everything it took, a call that replaces state (uavrl_env_set_pool, uavrl_env_generate_pool,
+ *     uavrl_env_set_extras, uavrl_learner_comm_init, ...) leaves the old state in place, and scratch that failed to grow is
+ *     grown again by the next call.
  */
 #ifndef UAVRL_H
 #define UAVRL_H
@@ -481,6 +485,10 @@ int64_t uavrl_launch_count(void);
 /* Programmatic dependent launch inside the lockstep loops (each kernel's prologue overlaps its predecessor's
  * tail; results are unchanged).  Process-wide switch, default 1; 0 launches every kernel fully serialised. */
 int uavrl_set_pdl(int32_t on);
+/* Test hook for the out-of-memory paths.  n >= 0: of the library's device allocations from now on, the first n succeed and
+ * the next one fails as an exhausted cudaMalloc does (UAVRL_ERR_CUDA, "out of memory"); the hook then turns itself off.
+ * n = -1 (the default) turns it off.  Process-wide. */
+int uavrl_test_fail_alloc(int32_t n);
 /* Kept for ABI compatibility; 0 only.  The lockstep loops launch get_action and Move_Agent as two kernels.  on = 0 returns 0;
  * any other value returns UAVRL_ERR_INVALID (the fused variant was removed). */
 int uavrl_set_fuse_act_env(int32_t on);
