@@ -35,7 +35,7 @@ ROUTES = [
     _pick(100, [64, 64, 64], 27, 0),      # FIXED TD feeding the fp32 update in single-weights mode
     _pick(100, [128, 64, 64], 27, 1),     # fp32 only, single weights, dueling
     _pick(99, [64], 27, 0),               # fp32 only, in_dim % 4 != 0
-    (100, [64, 64], 27, 0, FIXED_SHIPPED),
+    (100, [64, 64], 27, 0, ("fixed", "fixed", False, True, True)),   # shipped; its 128-row forward image does not fit
     (100, [64], 27, 1, FIXED_SHIPPED),
 ]
 # B, algorithms: 32-row tiles with fused TD at NPRE = 1 and 2; bench.py's PER batch (32-row tiles, fused TD, 128 CTAs); 64-row
@@ -59,7 +59,7 @@ def _cases():
             else:
                 algo = engine.ALGO_DUELING if shape[3] else engine.ALGO_DDQN
             marks = []
-            if leg.startswith("B4096") and shape[4] != FIXED_SHIPPED:
+            if leg.startswith("B4096") and shape[4] != FIXED_SHIPPED and shape[:4] != (100, [64, 64], 27, 0):
                 marks = [pytest.mark.skip(reason="B = 4096 takes B64-ddqn's route (32-row tiles, fused TD, NPRE = 2) on 128 CTAs; "
                                                  "it runs on the shipped shapes, which bench.py --per 1 trains at that batch")]
             for v in VARIANTS:
