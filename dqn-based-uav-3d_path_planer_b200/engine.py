@@ -229,6 +229,26 @@ NET_KINDS = {                       # BaseClass/BaseCNN.py class name -> (hidden
 }
 
 
+def _linears(*layers):
+    """Layout of torch.nn.Linear layers given as (name, out, in): a list of (state_dict key, shape)."""
+    return [(k, s) for nm, o, i in layers for k, s in ((nm + ".weight", (o, i)), (nm + ".bias", (o,)))]
+
+
+def _size(layout):
+    return sum(int(np.prod(s)) for _, s in layout)
+
+
+def init_draw(layout, gen):
+    """torch.nn.Linear default init (kaiming_uniform(a=sqrt(5)) == U(+-1/sqrt(fan_in)) for W and b) of every tensor of a
+    layout, in order, from torch generator `gen`: the flat float32 parameters."""
+    parts = []
+    for _, shape in layout:
+        if len(shape) == 2:                 # a weight; its bias follows and shares the fan-in
+            bound = 1.0 / np.sqrt(shape[1])
+        parts.append((torch.rand(int(np.prod(shape)), generator=gen) * 2 - 1) * bound)
+    return torch.cat(parts).numpy()
+
+
 class Learner:
     """Q-network + Adam + replay on one GPU (DQN / DDQN / DuelingDQN trainers of the reference).
 
@@ -255,6 +275,16 @@ class Learner:
         check(_lib.lib().uavrl_learner_create_trainers(C.byref(c), int(trainers), C.byref(self.h)))
         self.P = int(_lib.lib().uavrl_learner_param_count(self.h))
         self.G = int(_lib.lib().uavrl_learner_trainer_count(self.h))
+        assert _size(self.layout()) == self.P, (self.layout(), self.P)
+
+    def layout(self):
+        """(state_dict key, shape) of every tensor in flat-parameter order, named as the reference's networks
+        (BaseClass/BaseCNN.py) name them: fc1 .. fcN, then fc_A and fc_V for a dueling head."""
+        ins = [self.in_dim] + self.hidden
+        trunk = [("fc%d" % (i + 1), w, ins[i]) for i, w in enumerate(self.hidden)]
+        if self.dueling:
+            return _linears(*trunk, ("fc_A", self.n_actions, ins[-1]), ("fc_V", 1, ins[-1]))
+        return _linears(*trunk, ("fc%d" % len(ins), self.n_actions, ins[-1]))
 
     def close(self):
         if self.h:
@@ -272,27 +302,10 @@ class Learner:
         """torch.nn.Linear default init (kaiming_uniform(a=sqrt(5)) == U(+-1/sqrt(fan_in)) for W and b),
         independent draws for q_local and q_target like the reference's two Create_Network calls.
         Trainer g of a grouped learner draws with seed + g."""
-        draws = [self._init_draw(seed + g) for g in range(self.G)]
+        gens = [torch.Generator().manual_seed(seed + g) for g in range(self.G)]
+        draws = [[init_draw(self.layout(), gen) for _ in (0, 1)] for gen in gens]
         for which in (0, 1):
-            flat = draws[0][which] if self.G == 1 else np.stack([d[which] for d in draws])
-            self.set_params(flat, which)
-
-    def _init_draw(self, seed):
-        g = torch.Generator().manual_seed(seed)
-        outs = []
-        for _ in range(2):
-            parts, fan_in = [], self.in_dim
-            widths = self.hidden + [self.n_actions] + ([1] if self.dueling else [])
-            for li, out in enumerate(widths):
-                fi = fan_in if li < len(self.hidden) + 1 else self.hidden[-1]
-                bound = 1.0 / np.sqrt(fi)
-                parts.append((torch.rand(out * fi, generator=g) * 2 - 1) * bound)
-                parts.append((torch.rand(out, generator=g) * 2 - 1) * bound)
-                if li < len(self.hidden):
-                    fan_in = out
-            outs.append(torch.cat(parts).numpy().astype(np.float32))
-        assert outs[0].size == self.P
-        return outs
+            self.set_params(np.stack([d[which] for d in draws]), which)
 
     def _param_shape(self):
         return (self.P,) if self.G == 1 else (self.G, self.P)
@@ -553,6 +566,15 @@ class SacLearner:
         check(_lib.lib().uavrl_sac_create_trainers(C.byref(c), int(trainers), C.byref(self.h)))
         self.P = [int(_lib.lib().uavrl_sac_param_count(self.h, r)) for r in range(5)]
         self.G = int(_lib.lib().uavrl_sac_trainer_count(self.h))
+        assert [_size(self.layout(r)) for r in range(5)] == self.P, self.P
+
+    def layout(self, role):
+        """(state_dict key, shape) of every tensor of network `role` in flat-parameter order, named as the reference's
+        PolicyNetContinuous_SAC (role 0) and QValueNetContinuous_SAC (roles 1-4: the critics and their targets) name them."""
+        o, h, a = self.cfg.obs_dim, self.cfg.hidden, self.cfg.act_dim
+        if role == 0:
+            return _linears(("fc1", h, o), ("fc_mu", a, h), ("fc_std", a, h))
+        return _linears(("fc1", h, o + a), ("fc2", h, h), ("fc_out", a, h))
 
     def close(self):
         if self.h:
@@ -587,16 +609,8 @@ class SacLearner:
     def init_params(self, seed=0):
         """nn.Linear default init for actor and the two critics; targets copy the critics (SAC_Trainer.py:33-34).
         Trainer g of a grouped learner draws with seed + g."""
-        o, h, a = self.cfg.obs_dim, self.cfg.hidden, self.cfg.act_dim
-        draws = []
-        for t in range(self.G):
-            g = torch.Generator().manual_seed(seed + t)
-
-            def lin(out, fi):
-                b = 1.0 / np.sqrt(fi)
-                return [(torch.rand(out * fi, generator=g) * 2 - 1) * b, (torch.rand(out, generator=g) * 2 - 1) * b]
-            draws.append([torch.cat(lin(h, o) + lin(a, h) + lin(a, h)).numpy()] +
-                         [torch.cat(lin(h, o + a) + lin(h, h) + lin(a, h)).numpy() for _ in (1, 2)])
+        gens = [torch.Generator().manual_seed(seed + g) for g in range(self.G)]
+        draws = [[init_draw(self.layout(r), gen) for r in range(3)] for gen in gens]
         for r in range(3):
             flat = np.stack([d[r] for d in draws])
             self.set_params(r, flat)

@@ -1,6 +1,5 @@
 """Trainer plug-in: SAC with continuous actions (Trainer/SAC_Trainer.py, the trainer config/Trainer.xml ships) on the
 H100 library.  Constructor takes the reference's parsed Trainer.xml dict (actor / critic / SAC_param sub-dicts)."""
-import collections
 import os
 
 import numpy as np
@@ -8,6 +7,7 @@ import torch
 
 import uavrl_b200  # noqa: F401  (repository root must be on sys.path)
 from uavrl_b200 import engine
+from uavrl_b200.plugins import checkpoint
 from uavrl_b200.plugins.xmlconfig import None2Value
 
 
@@ -90,30 +90,6 @@ class SAC_Trainer_B200:
         """Role `role` of every trainer, (G, P), in ONE device read."""
         return self._learner.get_params(role).reshape(self.n_trainers, -1)
 
-    def _state_dict(self, role, flat):
-        o, h, a = self.w, self.hidden, self.act_dim
-        if role == 0:
-            shapes = [("fc1.weight", (h, o)), ("fc1.bias", (h,)), ("fc_mu.weight", (a, h)), ("fc_mu.bias", (a,)),
-                      ("fc_std.weight", (a, h)), ("fc_std.bias", (a,))]
-        else:
-            shapes = [("fc1.weight", (h, o + a)), ("fc1.bias", (h,)), ("fc2.weight", (h, h)), ("fc2.bias", (h,)),
-                      ("fc_out.weight", (a, h)), ("fc_out.bias", (a,))]
-        sd, off = collections.OrderedDict(), 0
-        for nm, shp in shapes:
-            n = int(np.prod(shp))
-            sd[nm] = torch.from_numpy(flat[off:off + n].reshape(shp).copy()); off += n
-        return sd
-
-    def _optim_dict(self, sd, m, v, t, lr):
-        state, off = {}, 0
-        for i, p in enumerate(sd.values()):
-            k = p.numel()
-            state[i] = {'step': torch.tensor(float(t)), 'exp_avg': torch.from_numpy(m[off:off + k].reshape(p.shape).copy()),
-                        'exp_avg_sq': torch.from_numpy(v[off:off + k].reshape(p.shape).copy())}
-            off += k
-        return {'state': state, 'param_groups': [{'lr': lr, 'betas': (0.9, 0.999), 'eps': 1e-08, 'weight_decay': 0,
-                                                  'amsgrad': False, 'params': list(range(len(sd)))}]}
-
     def _paths(self, directory, g):
         return [os.path.join(directory, '%s_SAC_%s.pth' % (nm, self.names[g])) for nm in self.ROLE_FILES]
 
@@ -128,8 +104,9 @@ class SAC_Trainer_B200:
         epoch, t = sc["epoch"], sc["adam_step"]
         for g in range(self.n_trainers):
             for role, path in enumerate(self._paths(directory, g)):
-                sd = self._state_dict(role, p[role][g])
-                torch.save({'model': sd, 'optimizer': self._optim_dict(sd, m[role][g], v[role][g], t, lrs[role]), 'epoch': epoch}, path)
+                lay = self._learner.layout(role)
+                torch.save({'model': checkpoint.model_dict(lay, p[role][g]),
+                            'optimizer': checkpoint.adam_dict(lay, m[role][g], v[role][g], t, lrs[role]), 'epoch': epoch}, path)
 
     def Load_Mod(self, Mod=None):
         """SAC_Trainer.Load_Mod (:70-106): resume actor / critics (+ their Adam moments) of every trainer whose three files
@@ -142,32 +119,18 @@ class SAC_Trainer_B200:
             if not all(os.path.exists(p) for p in paths):
                 continue
             try:
-                mine, ep = [], 0
-                for role, p in enumerate(paths):
-                    ck = torch.load(p, weights_only=False, map_location='cpu')
-                    flat = np.concatenate([v.detach().cpu().numpy().ravel() for v in ck['model'].values()]).astype(np.float32)
-                    if flat.size != self._learner.P[role]:
-                        raise ValueError("%s holds %d parameters, the network has %d" % (p, flat.size, self._learner.P[role]))
-                    m = v = None
-                    st = ck['optimizer'].get('state', {})
-                    if st:
-                        keys = sorted(st.keys())
-                        m = np.concatenate([st[k]['exp_avg'].detach().cpu().numpy().ravel() for k in keys]).astype(np.float32)
-                        v = np.concatenate([st[k]['exp_avg_sq'].detach().cpu().numpy().ravel() for k in keys]).astype(np.float32)
-                        if m.size != flat.size or v.size != flat.size:
-                            raise ValueError("%s: optimizer state does not match the model" % p)
-                        step = int(float(st[keys[0]]['step']))
-                    ep = int(ck['epoch'])
-                    mine.append((flat, m, v))
+                mine = [checkpoint.read(p, self._learner.layout(role)) for role, p in enumerate(paths)]
             except Exception as e:          # the reference prints and carries on (SAC_Trainer.py:105-106); nothing was applied
                 print(e.args)
                 continue
-            staged[g], epoch = mine, ep
+            staged[g], epoch = mine, mine[-1][4]
+            for _, m, _, st, _ in mine:     # the last network with optimizer state sets the Adam step
+                step = st if m is not None else step
         if not staged:
             return
         rows = {r: self._rows(r) for r in (0, 1, 2, 5, 6, 7, 8, 9, 10)}
         for g, mine in staged.items():
-            for role, (flat, m, v) in enumerate(mine):
+            for role, (flat, m, v, _, _) in enumerate(mine):
                 rows[role][g] = flat
                 if m is not None:
                     rows[5 + role][g], rows[8 + role][g] = m, v

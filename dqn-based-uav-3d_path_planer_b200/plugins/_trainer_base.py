@@ -1,6 +1,5 @@
 """Shared implementation of the DQN-family trainer plug-ins (the reference's BaseTrainer + the three
 concrete trainers): same constructor dict, attributes and methods; the math runs in libuavrl_b200."""
-import collections
 import os
 
 import numpy as np
@@ -8,6 +7,7 @@ import torch
 
 import uavrl_b200  # noqa: F401  (repository root must be on sys.path)
 from uavrl_b200 import engine
+from uavrl_b200.plugins import checkpoint
 from uavrl_b200.plugins.xmlconfig import None2Value
 
 # BaseClass/BaseCNN.py class name -> (hidden widths as a function of hiden_dim, dueling flag)
@@ -253,44 +253,17 @@ class TrainerB200:
         self._learner.set_params(_flat_from(target), 1)
 
     # ---- checkpoints: the reference's {'model', 'optimizer', 'epoch'} .pth files (DuelingDQN_Trainer.py:41-84)
-    def _names(self):
-        names = ["fc%d" % (i + 1) for i in range(len(self._learner.hidden))]
-        names += ["fc_A", "fc_V"] if self._learner.dueling else ["fc%d" % (len(self._learner.hidden) + 1)]
-        return names
-
-    def _param_shapes(self):
-        """(state_dict key, shape) of every tensor, in state_dict order -- from the network description, no device read."""
-        out, fan_in = [], self.w
-        widths = self._learner.hidden + [self.output] + ([1] if self._learner.dueling else [])
-        for i, (nm, o) in enumerate(zip(self._names(), widths)):
-            fi = fan_in if i <= len(self._learner.hidden) else self._learner.hidden[-1]
-            out += [(nm + ".weight", (o, fi)), (nm + ".bias", (o,))]
-            if i < len(self._learner.hidden):
-                fan_in = o
-        return out
-
     def _rows(self, which):
         """Vector `which` of every trainer, (G, P), in ONE device read: checkpoints of many trainers slice these rows
         instead of reading the whole [G][P] vector once per trainer."""
         return self._learner.get_params(which).reshape(self.n_trainers, -1)
 
-    @staticmethod
-    def _flat_of(tensors):
-        return np.concatenate([np.asarray(v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v, np.float32).ravel()
-                               for v in tensors])
-
     def state_dict(self, which=0, g=0, flat=None):
         """Trainer g's network `which` (0 q_local, 1 q_target) as a state_dict; `flat` = its row when already on the host."""
-        flat = self._rows(which)[g] if flat is None else flat
-        sd, off = collections.OrderedDict(), 0
-        for nm, shape in self._param_shapes():
-            k = int(np.prod(shape))
-            sd[nm] = torch.from_numpy(flat[off:off + k].reshape(shape).copy())
-            off += k
-        return sd
+        return checkpoint.model_dict(self._learner.layout(), self._rows(which)[g] if flat is None else flat)
 
     def load_state_dict(self, sd, which=0, g=0):
-        flat = self._flat_of(sd.values())
+        flat = checkpoint.flat(sd.values())
         if self.n_trainers > 1:                 # trainer g's row of the [G][P] parameters
             rows = self._rows(which)
             rows[g] = flat
@@ -299,32 +272,12 @@ class TrainerB200:
 
     def optimizer_state_dict(self, g=0, m=None, v=None):
         """torch.optim.Adam state_dict of trainer g; m / v = its exp_avg / exp_avg_sq rows when already on the host."""
-        shapes = self._param_shapes()
-        t = self._learner.counters()[1]
         m = self._rows(2)[g] if m is None else m
         v = self._rows(3)[g] if v is None else v
-        state, off = {}, 0
-        for i, (_, shape) in enumerate(shapes):
-            k = int(np.prod(shape))
-            state[i] = {'step': torch.tensor(float(t)), 'exp_avg': torch.from_numpy(m[off:off + k].reshape(shape).copy()),
-                        'exp_avg_sq': torch.from_numpy(v[off:off + k].reshape(shape).copy())}
-            off += k
-        group = {'lr': self.LEARNING_RATE, 'betas': (0.9, 0.999), 'eps': 1e-08, 'weight_decay': 0, 'amsgrad': False,
-                 'params': list(range(len(shapes)))}
-        return {'state': state, 'param_groups': [group]}
-
-    @classmethod
-    def _adam_rows(cls, osd):
-        """(exp_avg, exp_avg_sq, step) of an optimizer state_dict, or None when it holds no state."""
-        st = osd.get('state', {})
-        if not st:
-            return None
-        keys = sorted(st.keys())
-        return (cls._flat_of(st[k]['exp_avg'] for k in keys), cls._flat_of(st[k]['exp_avg_sq'] for k in keys),
-                int(float(st[keys[0]]['step'])))
+        return checkpoint.adam_dict(self._learner.layout(), m, v, self._learner.counters()[1], self.LEARNING_RATE)
 
     def load_optimizer_state_dict(self, osd, g=0):
-        mvs = self._adam_rows(osd)
+        mvs = checkpoint.adam_moments(self._learner.layout(), osd)
         if mvs is None:
             return
         for which, x in ((2, mvs[0]), (3, mvs[1])):
@@ -352,8 +305,9 @@ class TrainerB200:
 
     def Load_Mod(self, Mod_path=None):
         """DuelingDQN_Trainer.Load_Mod (:40-69): <root>/Mod by default; a given Mod_path is tried as written and, like the
-        reference's `root + Mod_path`, relative to the working directory.  Every trainer whose file pair exists is restored
-        into host copies of the four vectors, which go to the device once each."""
+        reference's `root + Mod_path`, relative to the working directory.  Every trainer whose file pair exists and parses
+        as this network is restored into host copies of the four vectors, which go to the device once each; a trainer
+        whose files do not parse is left as it is."""
         directory = Mod_path or os.path.join(os.getcwd(), 'Mod')
         if Mod_path and not os.path.isdir(directory) and os.path.isdir(os.path.join(os.getcwd(), Mod_path.lstrip('/'))):
             directory = os.path.join(os.getcwd(), Mod_path.lstrip('/'))
@@ -363,19 +317,16 @@ class TrainerB200:
             if not (os.path.exists(pt) and os.path.exists(pl)):
                 continue
             try:
-                mt = torch.load(pt, weights_only=False, map_location='cpu')
-                ml = torch.load(pl, weights_only=False, map_location='cpu')
-                tgt, loc = self._flat_of(mt['model'].values()), self._flat_of(ml['model'].values())
-                mvs = self._adam_rows(ml['optimizer'])
-                ep = int(ml['epoch'])
-            except Exception as e:          # the reference prints and carries on (:56-57)
+                tgt = checkpoint.read(pt, self._learner.layout())[0]
+                loc, m, v, st, ep = checkpoint.read(pl, self._learner.layout())
+            except Exception as e:          # the reference prints and carries on (:56-57); nothing was applied
                 print(e.args)
                 continue
             if rows is None:
                 rows = [self._rows(w) for w in range(4)]
             rows[0][g], rows[1][g] = loc, tgt
-            if mvs is not None:
-                rows[2][g], rows[3][g], step = mvs
+            if m is not None:
+                rows[2][g], rows[3][g], step = m, v, st
             epoch = ep
         if rows is None:
             return

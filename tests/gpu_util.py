@@ -1,4 +1,8 @@
 """Shared helpers for the -m gpu parity tests (CUDA path vs the CPU oracle / golden vectors)."""
+import contextlib
+import importlib
+import os
+
 import numpy as np
 import torch
 
@@ -33,3 +37,28 @@ def assert_obs(got, want64, what=""):
     got = np.asarray(got); want64 = np.asarray(want64, np.float64)
     assert np.array_equal(got[..., BIN], want64[..., BIN].astype(np.float32)), what
     np.testing.assert_allclose(got[..., REAL], want64[..., REAL], rtol=1e-5, atol=1e-5, err_msg=what)
+
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+@contextlib.contextmanager
+def env_plugin(model_path):
+    """The env plug-in module, run from the repository root, whose trainers read a small batch and replay, no periodic
+    save and checkpoints under model_path."""
+    cwd = os.getcwd()
+    os.chdir(ROOT)
+    mod = importlib.import_module("uavrl_b200.plugins.PathPlan_City_B200")
+    orig = mod.XML2Dict
+
+    def patched(path):
+        d = orig(path)
+        if "Trainer" in d and isinstance(d["Trainer"], dict):
+            d["Trainer"].update(Batch_Size="16", replay_size="512", save_loop="0", model_path=str(model_path))
+        return d
+    mod.XML2Dict = patched
+    try:
+        yield mod
+    finally:
+        mod.XML2Dict = orig
+        os.chdir(cwd)

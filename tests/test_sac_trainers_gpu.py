@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_util import city_and_params
+from gpu_util import city_and_params, env_plugin
 from test_fl_ac_cpu import GOLDEN as FL_AC_GOLDEN, federate_actors
 from uavrl_b200 import _lib, engine
 
@@ -343,65 +343,51 @@ class CountTransfers:
         L.get_params, L.set_params = g, s
 
 
+def env_dict(**kw):
+    """The shipped env configuration with num_UAV = num_trainers = 8, the continuous step and the SAC trainer."""
+    from uavrl_b200.plugins import xmlconfig
+    ed = xmlconfig.XML2Dict(os.path.join(ROOT, "configs", "PathPlan_City_B200.xml"))["simulator"]["env"]
+    ed["num_UAV"], ed["scenario_pool"], ed["num_trainers"] = "8", "64", "8"
+    ed["Obstacles"]["buildings"] = os.path.join(ROOT, "configs", "buildings.xml")
+    ed["Agent"]["xml_path_agent"] = os.path.join(ROOT, "configs", "UAV_continuous_B200.xml")
+    ed["Agent"]["Trainer"]["Trainer_path"] = os.path.join(ROOT, "configs", "Trainer_SAC_B200.xml")
+    ed.update(kw)
+    return ed
+
+
 def test_env_plugin_one_sac_trainer_per_uav(tmp_path):
     """num_UAV = num_trainers = 8 with the shipped SAC trainer and the continuous step: run_eposide runs, save() writes the
     reference's three files per UAV, Load_Mod in a fresh env restores every trainer bit for bit, each moving every role's
     vector between host and device once whatever G is; Is_FL = Is_AC = FL_Loop = 1 leaves every actor equal to the sum."""
-    import importlib
-    from uavrl_b200.plugins import xmlconfig
-    cwd = os.getcwd()
-    os.chdir(ROOT)
-    try:
-        def env_dict(**kw):
-            ed = xmlconfig.XML2Dict(os.path.join(ROOT, "configs", "PathPlan_City_B200.xml"))["simulator"]["env"]
-            ed["num_UAV"], ed["scenario_pool"], ed["num_trainers"] = "8", "64", "8"
-            ed["Obstacles"]["buildings"] = os.path.join(ROOT, "configs", "buildings.xml")
-            ed["Agent"]["xml_path_agent"] = os.path.join(ROOT, "configs", "UAV_continuous_B200.xml")
-            ed["Agent"]["Trainer"]["Trainer_path"] = os.path.join(ROOT, "configs", "Trainer_SAC_B200.xml")
-            ed.update(kw)
-            return ed
-        mod = importlib.import_module("uavrl_b200.plugins.PathPlan_City_B200")
-        orig = mod.XML2Dict
+    with env_plugin(tmp_path) as mod:
+        env = mod.PathPlan_City_B200(env_dict())
+        tr = env.Trainer
+        assert tr._learner.trainer_count() == 8 and tr.names == ["UAV_%d" % i for i in range(8)]
+        with pytest.raises(ValueError, match="batch"):
+            tr.get_action(np.zeros(100, np.float32))
+        assert tr.get_action(np.zeros((8, 100), np.float32)).shape == (8, 2)
+        info = env.run_eposide(0.3)
+        assert info["updates"] > 0 and np.isfinite(info["loss"])
+        n = CountTransfers(tr._learner)
+        tr.save()
+        assert (n.get, n.set) == (9, 0)
+        env2 = mod.PathPlan_City_B200(env_dict())                   # Load_Mod in the constructor
+        n = CountTransfers(env2.Trainer._learner)
+        env2.Trainer.Load_Mod()
+        assert (n.get, n.set) == (9, 11)
+        # federated aggregation of the actors after every episode
+        env3 = mod.PathPlan_City_B200(env_dict(Is_FL="1", Is_AC="1", FL_Loop="1"))
+        L3 = env3.Trainer._learner
+        seen = []
+        fed = L3.federate_actors
 
-        def patched(path):
-            d = orig(path)
-            if "Trainer" in d and isinstance(d["Trainer"], dict):
-                d["Trainer"].update(Batch_Size="16", replay_size="512", save_loop="0", model_path=str(tmp_path))
-            return d
-        mod.XML2Dict = patched
-        try:
-            env = mod.PathPlan_City_B200(env_dict())
-            tr = env.Trainer
-            assert tr._learner.trainer_count() == 8 and tr.names == ["UAV_%d" % i for i in range(8)]
-            with pytest.raises(ValueError, match="batch"):
-                tr.get_action(np.zeros(100, np.float32))
-            assert tr.get_action(np.zeros((8, 100), np.float32)).shape == (8, 2)
-            info = env.run_eposide(0.3)
-            assert info["updates"] > 0 and np.isfinite(info["loss"])
-            n = CountTransfers(tr._learner)
-            tr.save()
-            assert (n.get, n.set) == (9, 0)
-            env2 = mod.PathPlan_City_B200(env_dict())                   # Load_Mod in the constructor
-            n = CountTransfers(env2.Trainer._learner)
-            env2.Trainer.Load_Mod()
-            assert (n.get, n.set) == (9, 11)
-            # federated aggregation of the actors after every episode
-            env3 = mod.PathPlan_City_B200(env_dict(Is_FL="1", Is_AC="1", FL_Loop="1"))
-            L3 = env3.Trainer._learner
-            seen = []
-            fed = L3.federate_actors
-
-            def spy():
-                seen.append(L3.get_params(0))
-                fed()
-            L3.federate_actors = spy
-            env3.run_eposide(0.3)
-            assert len(seen) == 1
-            assert_same(L3.get_params(0), federate_actors(seen[0]), "actors after the episode")
-        finally:
-            mod.XML2Dict = orig
-    finally:
-        os.chdir(cwd)
+        def spy():
+            seen.append(L3.get_params(0))
+            fed()
+        L3.federate_actors = spy
+        env3.run_eposide(0.3)
+        assert len(seen) == 1
+        assert_same(L3.get_params(0), federate_actors(seen[0]), "actors after the episode")
     files = sorted(os.listdir(tmp_path))
     assert files == sorted(["%s_SAC_UAV_%d.pth" % (k, i) for k in ("actor", "critic_1", "critic_2") for i in range(8)]), files
     ck = torch.load(os.path.join(tmp_path, "critic_2_SAC_UAV_5.pth"), weights_only=False)
@@ -413,3 +399,32 @@ def test_env_plugin_one_sac_trainer_per_uav(tmp_path):
     for role in (1, 2):
         assert_same(L2.get_params(role + 2), L.get_params(role), "target %d copies the critic" % role)
     assert (L2.scalars()["epoch"], L2.scalars()["adam_step"]) == (L.scalars()["epoch"], L.scalars()["adam_step"])
+
+
+def test_env_plugin_skips_malformed_checkpoint(tmp_path, capsys):
+    """Trainer 3's critic_1 file holds a renamed key.  As in the reference (SAC_Trainer.py:105-106), the constructor prints
+    the error and carries on: trainer 3 keeps its fresh networks, targets and moments, every other trainer is restored bit
+    for bit with its targets copying its critics."""
+    with env_plugin(tmp_path) as mod:
+        tr = mod.PathPlan_City_B200(env_dict()).Trainer                  # no files yet: fresh parameters
+        L = tr._learner
+        fresh = {r: L.get_params(r) for r in range(11)}
+        rng = np.random.default_rng(5)
+        saved = {r: rng.normal(0, 1, fresh[r].shape).astype(np.float32) for r in (0, 1, 2, 5, 6, 7, 8, 9, 10)}
+        for r, x in saved.items():
+            L.set_params(r, x)
+        tr._set_counters(123, 45)
+        tr.save()
+        p = os.path.join(tmp_path, "critic_1_SAC_UAV_3.pth")
+        ck = torch.load(p, weights_only=False)
+        ck["model"] = {("fc3.weight" if k == "fc_out.weight" else k): t for k, t in ck["model"].items()}
+        torch.save(ck, p)
+        capsys.readouterr()
+        L2 = mod.PathPlan_City_B200(env_dict()).Trainer._learner         # Load_Mod in the constructor
+        out = capsys.readouterr().out
+    assert "critic_1_SAC_UAV_3.pth holds" in out and "fc3.weight" in out, out
+    for r in range(11):
+        want = saved.get(r, saved.get(r - 2))                            # targets 3, 4 copy critics 1, 2
+        for g in range(8):
+            assert_same(L2.get_params(r)[g], fresh[r][g] if g == 3 else want[g], "role %d of trainer %d" % (r, g))
+    assert (L2.scalars()["epoch"], L2.scalars()["adam_step"]) == (123, 45)

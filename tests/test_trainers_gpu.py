@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_util import city_and_params
+from gpu_util import city_and_params, env_plugin
 from test_qnet_shapes_gpu import SHAPES, SHIPPED
 from test_tc_gpu import big_inputs
 from uavrl_b200 import _lib, engine
@@ -268,52 +268,38 @@ class CountTransfers:
         L.get_params, L.set_params = g, s
 
 
+def env_dict(**kw):
+    """The shipped env configuration with num_UAV = num_trainers = 8 and the DDQN trainer."""
+    from uavrl_b200.plugins import xmlconfig
+    ed = xmlconfig.XML2Dict(os.path.join(ROOT, "configs", "PathPlan_City_B200.xml"))["simulator"]["env"]
+    ed["num_UAV"], ed["scenario_pool"], ed["num_trainers"] = "8", "64", "8"
+    ed["Obstacles"]["buildings"] = os.path.join(ROOT, "configs", "buildings.xml")
+    ed["Agent"]["Trainer"]["Trainer_path"] = os.path.join(ROOT, "configs", "Trainer_DDQN_B200.xml")
+    ed.update(kw)
+    return ed
+
+
 def test_env_plugin_one_trainer_per_uav(tmp_path):
     """num_UAV = num_trainers = 8: the reference's one trainer per UAV.  run_eposide runs, save() writes one q_local / q_target
     pair per trainer in the reference's per-UAV naming, and Load_Mod in a fresh env restores every trainer bit for bit.  Both
     move each of the four vectors between host and device once, whatever the trainer count."""
-    import importlib
-    from uavrl_b200.plugins import xmlconfig
-    cwd = os.getcwd()
-    os.chdir(ROOT)
-    try:
-        def env_dict(**kw):
-            ed = xmlconfig.XML2Dict(os.path.join(ROOT, "configs", "PathPlan_City_B200.xml"))["simulator"]["env"]
-            ed["num_UAV"], ed["scenario_pool"], ed["num_trainers"] = "8", "64", "8"
-            ed["Obstacles"]["buildings"] = os.path.join(ROOT, "configs", "buildings.xml")
-            ed["Agent"]["Trainer"]["Trainer_path"] = os.path.join(ROOT, "configs", "Trainer_DDQN_B200.xml")
-            ed.update(kw)
-            return ed
-        mod = importlib.import_module("uavrl_b200.plugins.PathPlan_City_B200")
-        orig = mod.XML2Dict
-
-        def patched(path):
-            d = orig(path)
-            if "Trainer" in d and isinstance(d["Trainer"], dict):
-                d["Trainer"].update(Batch_Size="16", replay_size="512", save_loop="0", model_path=str(tmp_path))
-            return d
-        mod.XML2Dict = patched
-        try:
-            env = mod.PathPlan_City_B200(env_dict())
-            with pytest.raises(ValueError, match="multiple of num_trainers"):
-                mod.PathPlan_City_B200(env_dict(num_trainers="3"))
-            with pytest.raises(ValueError, match="num_trainers = 1"):
-                mod.PathPlan_City_B200(env_dict(host_driven="1"))
-            tr = env.Trainer
-            assert tr._learner.trainer_count() == 8 and tr.names == ["UAV_%d" % i for i in range(8)]
-            info = env.run_eposide(0.3)
-            assert info["updates"] > 0 and np.isfinite(info["loss"])
-            n = CountTransfers(tr._learner)
-            tr.save()
-            assert (n.get, n.set) == (4, 0)
-            env2 = mod.PathPlan_City_B200(env_dict())                   # Load_Mod in the constructor
-            n = CountTransfers(env2.Trainer._learner)
-            env2.Trainer.Load_Mod(str(tmp_path))
-            assert (n.get, n.set) == (4, 4)
-        finally:
-            mod.XML2Dict = orig
-    finally:
-        os.chdir(cwd)
+    with env_plugin(tmp_path) as mod:
+        env = mod.PathPlan_City_B200(env_dict())
+        with pytest.raises(ValueError, match="multiple of num_trainers"):
+            mod.PathPlan_City_B200(env_dict(num_trainers="3"))
+        with pytest.raises(ValueError, match="num_trainers = 1"):
+            mod.PathPlan_City_B200(env_dict(host_driven="1"))
+        tr = env.Trainer
+        assert tr._learner.trainer_count() == 8 and tr.names == ["UAV_%d" % i for i in range(8)]
+        info = env.run_eposide(0.3)
+        assert info["updates"] > 0 and np.isfinite(info["loss"])
+        n = CountTransfers(tr._learner)
+        tr.save()
+        assert (n.get, n.set) == (4, 0)
+        env2 = mod.PathPlan_City_B200(env_dict())                   # Load_Mod in the constructor
+        n = CountTransfers(env2.Trainer._learner)
+        env2.Trainer.Load_Mod(str(tmp_path))
+        assert (n.get, n.set) == (4, 4)
     files = sorted(os.listdir(tmp_path))
     assert files == sorted(["q_%s_DDQN_UAV_%d.pth" % (k, i) for k in ("local", "target") for i in range(8)]), files
     ck = torch.load(os.path.join(tmp_path, "q_local_DDQN_UAV_5.pth"), weights_only=False)
@@ -322,3 +308,35 @@ def test_env_plugin_one_trainer_per_uav(tmp_path):
     for which in range(4):
         assert_same(env2.Trainer._learner.get_params(which), tr._learner.get_params(which), "restored vector %d" % which)
     assert env2.Trainer._learner.counters() == tr._learner.counters()
+
+
+def test_env_plugin_skips_malformed_checkpoints(tmp_path, capsys):
+    """Of 8 trainers' checkpoint pairs, trainer 2's q_local holds a network of the wrong size and trainer 6's q_target a
+    renamed key.  As in the reference (DuelingDQN_Trainer.py:56-57), the constructor prints each error and carries on: those
+    two trainers keep their fresh parameters and moments, every other trainer is restored bit for bit."""
+    with env_plugin(tmp_path) as mod:
+        tr = mod.PathPlan_City_B200(env_dict()).Trainer                  # no files yet: fresh parameters
+        fresh = [tr._rows(which) for which in range(4)]
+        rng = np.random.default_rng(5)
+        saved = [rng.normal(0, 1, f.shape).astype(np.float32) for f in fresh]
+        for which in range(4):
+            tr._learner.set_params(saved[which], which)
+        tr._learner.set_counters(123, 45)
+        tr.save()
+        pl, pt = (os.path.join(tmp_path, "q_%s_DDQN_UAV_%d.pth" % kg) for kg in (("local", 2), ("target", 6)))
+        ck = torch.load(pl, weights_only=False)
+        ck["model"]["fc1.weight"] = ck["model"]["fc1.weight"][:, :99].clone()   # a network of 99 inputs
+        torch.save(ck, pl)
+        ck = torch.load(pt, weights_only=False)
+        ck["model"] = {("fc0.bias" if k == "fc1.bias" else k): t for k, t in ck["model"].items()}
+        torch.save(ck, pt)
+        capsys.readouterr()
+        tr2 = mod.PathPlan_City_B200(env_dict()).Trainer                 # Load_Mod in the constructor
+        out = capsys.readouterr().out
+    assert "q_local_DDQN_UAV_2.pth: fc1.weight is (64, 99)" in out and "q_target_DDQN_UAV_6.pth holds" in out, out
+    for which in range(4):
+        got = tr2._rows(which)
+        for g in range(8):
+            want = fresh[which][g] if g in (2, 6) else saved[which][g]
+            assert_same(got[g], want, "vector %d of trainer %d" % (which, g))
+    assert tr2._learner.counters() == (123, 45)
