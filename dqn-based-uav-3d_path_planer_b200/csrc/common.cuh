@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/uavrl.h"
+#include "launch_chain.cuh"
 
 namespace uavrl {
 
@@ -60,8 +61,8 @@ inline int fail(int code, const std::string &msg)
 // kernel k+1 may start while kernel k is still running, does what does not depend on k (mbarrier init, TMA of weights / loads of state last written >= 2 kernels back) and then blocks in griddepcontrol.wait
 // until k has completed and its writes are visible.  Every loop kernel triggers its dependents right after its own
 // wait, so kernel k+1 only ever overlaps kernel k (everything <= k-1 is complete when k+1's prologue runs).
-// Launched without the attribute, both instructions are no-ops.
-extern std::atomic<int> g_pdl;            // uavrl_set_pdl(); default on
+// Launched without the attribute, both instructions are no-ops.  Which kernel launches so, and what it may fetch before its
+// wait, is decided in launch_chain.cuh.
 
 #if defined(__CUDACC__)
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -81,11 +82,6 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 #endif
-
-// which loop kernel was launched last on the learner's stream (decides what a prologue may touch before its wait)
-enum PdlPrev { kPdlNone = 0, kPdlAct, kPdlEnv, kPdlTd, kPdlTrain, kPdlDw, kPdlAdam };
-// TcArgs.pdl / kernel flags
-constexpr int kPdlOn = 1, kPdlEarlyWeights = 2, kPdlEarlyRows = 4;
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize belongs to the kernel (process-wide, per device), not to the learner that sets
 // it: raise it to what this instance launches with, never lower it.  Setting it to a smaller instance's size would make every

@@ -190,7 +190,7 @@ int uavrl_learner_federate(uavrl_learner *l, const float *probe_states_dev, cons
         // the new theta_p on the probes of every later round: column p of M
         if (p + 1 < G && (rc = launch_fed_loss(l, pr, q_ref, M, p, 1, false, st))) return done(rc);
     }
-    l->pdl_prev = kPdlNone;
+    l->chain.launched(kChainNone);
     return done(0);
 }
 

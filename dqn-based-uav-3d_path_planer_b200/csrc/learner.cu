@@ -497,17 +497,41 @@ static size_t upd_smem_bytes(const NetDev &n, int dual)
 }
 static const size_t kMaxDynSmem = 227 * 1024;
 
+std::atomic<int> g_fuse_td{1};               // uavrl_set_fuse_td(); default on
+
+Route learner_route(const uavrl_learner *l, int n)
+{
+    Route r;
+    memset(&r, 0, sizeof(r));
+    r.fp32_dual = l->dual_weights != 0;
+    if (!l->tc_ok || !l->use_tc) return r;
+    const int n_sm = num_sms();
+    r.fwd = l->tc_fixed_fwd ? 2 : 1;
+    // act / TD pass: the largest tile of which the rows fill a wave (128 rows only when that image fits shared memory)
+    r.fwd_rows = (n >= 128 * n_sm && l->tc.max_rows == 128) ? 128 : (n >= 64 * n_sm) ? 64 : 32;
+    if (!l->tc_train_ok) return r;
+    r.train = l->tc_fixed_train ? 2 : 1;
+    // training kernel: 32 rows while the batch fits one wave of 32-row tiles, else 64 (when the 64-row operands fit)
+    r.train_rows = (n > 32 * n_sm && l->tc.train_max_rows == 64) ? 64 : 32;
+    // TD passes inside the training kernel at one tile per CTA (32-row tiles up to 4 736 samples, 64-row tiles up to 9 472): the
+    // weight images are restaged inside the kernel, which only pays when a CTA does it once; larger batches keep the separate
+    // TD-target kernel(s), whose CTAs reuse one image over several tiles
+    r.td_fused = g_fuse_td.load() && (n + r.train_rows - 1) / r.train_rows <= n_sm;
+    return r;
+}
+
 int launch_act(uavrl_learner *l, const float *obs, int n_all, float eps, int is_train, const float *u_tape,
                const int32_t *rand_tape, int32_t *actions, float *q_out, cudaStream_t st)
 {
     const int n = n_all / l->G;                          // rows per trainer (grouped learner: G equal blocks)
-    if (l->tc_ok && l->use_tc) {                         // tensor-core forward chain (tc_forward.cu)
+    const Route r = learner_route(l, n);
+    if (r.fwd) {                                         // tensor-core forward chain (tc_forward.cu)
         TcArgs a;
         memset(&a, 0, sizeof(a));
-        a.img = l->tc_img_local; a.obs = obs; a.n = n; a.n_tiles = (n + kTcTile - 1) / kTcTile; a.mode = kTcAct;
+        a.img = l->tc_img_local; a.obs = obs; a.n = n; a.mode = kTcAct;
         a.eps = eps; a.is_train = is_train; a.u_tape = u_tape; a.rand_tape = rand_tape;
         a.key = l->cfg.seed ^ kActSalt; a.call = l->act_calls++; a.actions = actions; a.q_out = q_out;
-        return launch_tc_forward(l, a, st);
+        return launch_tc_forward(l, r, a, st);
     }
     const int n_tiles = (n + kTile - 1) / kTile;
     const int grid = n_tiles < 4 * num_sms() ? n_tiles : 4 * num_sms();
@@ -515,7 +539,7 @@ int launch_act(uavrl_learner *l, const float *obs, int n_all, float eps, int is_
                                                                                       rand_tape, l->cfg.seed ^ kActSalt, l->act_calls++,
                                                                                       actions, nullptr, q_out, n_tiles, l->net.smem_w_floats,
                                                                                       FedLossArgs{});
-    l->pdl_prev = kPdlNone;
+    l->chain.launched(kChainNone);
     UAVRL_LAUNCHED();
     return 0;
 }
@@ -526,12 +550,13 @@ int launch_fed_loss(uavrl_learner *l, const float *probes, const float *q_ref, f
     const int n = l->G * kFedProbes;                     // every probe row; a weight set evaluates at most n - S of them
     const int max_rows = n - kFedProbes;
     if (max_rows <= 0 || n_weights <= 0) return 0;
-    if (l->tc_ok && l->use_tc) {
+    const Route r = learner_route(l, max_rows);
+    if (r.fwd) {
         TcArgs a;
         memset(&a, 0, sizeof(a));
         a.img = l->tc_img_local; a.obs = probes; a.n = n; a.mode = kTcAct;
         a.q_ref = q_ref; a.loss_out = loss_out; a.loss_w0 = w0; a.loss_tri = tri ? 1 : 0;
-        return launch_tc_loss(l, a, n_weights, max_rows, st);
+        return launch_tc_loss(l, r, a, n_weights, max_rows, st);
     }
     constexpr int step = (kTile / kFedProbes) * kFedProbes;
     const int n_tiles = (max_rows + step - 1) / step;
@@ -539,122 +564,176 @@ int launch_fed_loss(uavrl_learner *l, const float *probes, const float *q_ref, f
     act_kernel_t<true><<<dim3(grid, n_weights), kNetThreads, act_smem_bytes(l->net), st>>>(l->net, l->img_local, probes, n, 0.f, 0, nullptr,
                                                                                           nullptr, 0, 0, nullptr, nullptr, nullptr, n_tiles,
                                                                                           l->net.smem_w_floats, FedLossArgs{ q_ref, loss_out, w0, tri ? 1 : 0 });
-    l->pdl_prev = kPdlNone;
+    l->chain.launched(kChainNone);
     UAVRL_LAUNCHED();
     return 0;
 }
 
-static int launch_update_impl(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, bool apply,
-                              cudaStream_t st, cudaEvent_t *mid, bool partials_only = false);
+// ---- one Trainer.update: the gradient step (launch_grads), the optimiser step (adam_args and a launcher per kind), and the
+// prioritised-replay write-back (per_write_back), always in that order
 
-// hard_update (DuelingDQN_Trainer.py:199-202): the optimiser step of every update_loop-th epoch also copies local -> target
-static int hard_update_due(const uavrl_learner *l) { return (l->cfg.update_loop > 0 && (l->epoch % l->cfg.update_loop) == 0) ? 1 : 0; }
+// what the gradient step leaves for the optimiser step
+struct Grads {
+    int rc;                       // != 0: the gradient step failed
+    int nparts, n_loss_parts;     // gradient / loss partial slots written per trainer; 0: l->grad already holds the gradient
+    float inv_b;                  // 1 / the batch the loss averages over
+    bool per;                     // sampled from the SumTree: the |Q - y| of the batch go back to it
+};
 
-int launch_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, bool apply,
-                  cudaStream_t st)
+// the fp32 CUDA-core update kernel on `grid` CTAs per trainer: TD targets (unless y_in holds them), forward, backward and the
+// weight-gradient partials in one launch
+static int launch_fp32_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, int grid, const float *y_in,
+                              cudaStream_t st)
 {
-    return launch_update_impl(l, src, B, global_batch, loss_out, apply, st, nullptr);
+    UpdateArgs ua;
+    ua.img_local = l->img_local; ua.img_target = l->img_target; ua.partials = l->partials; ua.loss_partials = l->loss_partials;
+    ua.B = B; ua.n_tiles = (B + kTile - 1) / kTile; ua.algo = l->cfg.algo; ua.gamma = l->cfg.gamma; ua.dual = l->dual_weights;
+    ua.loss_kind = l->cfg.loss_kind; ua.img_floats = l->net.smem_w_floats;
+    ua.inv_global_b = 1.0f / (float)global_batch;
+    ua.y_in = y_in;
+    update_kernel<<<dim3(grid, l->G), kNetThreads, upd_smem_bytes(l->net, l->dual_weights), st>>>(l->net, src, ua);
+    l->chain.launched(kChainNone);
+    UAVRL_LAUNCHED();
+    return 0;
 }
 
-// profiling form: mid[0] after the TD-target pass, mid[1] after the forward/backward kernel, mid[2] after the
-// weight-gradient kernel (== mid[1] on the CUDA-core path); the optimiser kernel follows
-int launch_update_split(uavrl_learner *l, const BatchSrc &src, int B, cudaStream_t st, cudaEvent_t *mid)
+static int mark(cudaEvent_t *marks, int k, cudaStream_t st)
 {
-    return launch_update_impl(l, src, B, B, l->loss_dev, true, st, mid);
+    if (marks) UAVRL_CUDA(cudaEventRecord(marks[k], st));
+    return 0;
 }
 
-static int launch_update_impl(uavrl_learner *l, const BatchSrc &src_in, int B, int global_batch, float *loss_out, bool apply,
-                              cudaStream_t st, cudaEvent_t *mid, bool partials_only)
+// Sample (prioritised replay), TD-target pass(es) and training kernel(s): the gradient partials of B transitions per trainer.
+// marks (profiling, may be null): events after the TD-target pass, the training kernel and the weight-gradient kernel (the
+// training kernel on the fp32 path, which computes the weight gradients itself)
+static Grads launch_grads(uavrl_learner *l, const BatchSrc &src_in, int B, int global_batch, cudaStream_t st, cudaEvent_t *marks)
 {
+    Grads g = { 0, 0, 0, 1.0f / (float)global_batch, l->per.enabled && src_in.mode != kBatchExplicit && !src_in.idx_tape };
     BatchSrc src = src_in;
-    const bool per_batch = l->per.enabled && src.mode != kBatchExplicit && !src.idx_tape;
-    if (per_batch) {
-        // ReplayTree.sample2 -> slots + importance weights; |Q - y| comes back for batch_update (end of this function).
+    if (g.per) {
+        // ReplayTree.sample2 -> slots + importance weights; |Q - y| comes back for batch_update (per_write_back).
         // Grouped learner: [G][B] trainer-local slots, weights and errors; trainer_src hands trainer g its row of each
-        int rc = per_sample(l, B, nullptr, nullptr, nullptr, st);
-        if (rc) return rc;
+        if ((g.rc = per_sample(l, B, nullptr, nullptr, nullptr, st))) return g;
         src.idx_tape = l->per.idx; src.idx_is_slot = 1; src.is_w = l->per.w; src.abs_err = l->per.abs_err;
     }
+    const Route r = learner_route(l, B);
     const int n_tiles = (B + kTile - 1) / kTile;
     const int grid = n_tiles < l->max_ctas ? n_tiles : l->max_ctas;
-    if (int rc = grow(l->parts_mem, l->parts_cap, grid, st, true,      // grouped learner, batch larger than batch_size: more slots
-                      buf(l->partials, (size_t)l->G * grid * l->net.P), buf(l->loss_partials, (size_t)l->G * grid)))
-        return rc;
+    if ((g.rc = grow(l->parts_mem, l->parts_cap, grid, st, true,      // grouped learner, batch larger than batch_size: more slots
+                     buf(l->partials, (size_t)l->G * grid * l->net.P), buf(l->loss_partials, (size_t)l->G * grid))))
+        return g;
     const float *y_in = nullptr;
-    // the route follows the learner's flags, never the scratch: y_buf is null after a failed grow until the next one succeeds
-    const bool tc_route = l->tc_ok && l->use_tc;
-    const bool fuse_td = tc_route && tc_train_can_fuse_td(l, B);
-    if (fuse_td) {
+    if (r.td_fused) {
         y_in = l->y_buf;                                  // not read: the training kernel forms the TD targets itself
-    } else if (tc_route) {
-        // TD targets on the tensor cores: y = r + gamma * next_q * (1 - d) for the whole batch, then the
-        // update kernel only evaluates the local network (forward on s, backward)
-        int rc;
-        if ((rc = grow(l->td_mem, l->y_cap, B, st, false, buf(l->y_buf, (size_t)l->G * B), buf(l->astar_buf, (size_t)l->G * B))))
-            return rc;
+    } else if (r.fwd) {
+        // TD targets on the tensor cores: y = r + gamma * next_q * (1 - d) for the whole batch, then the training kernel
+        // only evaluates the local network (forward on s, backward)
+        if ((g.rc = grow(l->td_mem, l->y_cap, B, st, false, buf(l->y_buf, (size_t)l->G * B), buf(l->astar_buf, (size_t)l->G * B))))
+            return g;
         TcArgs a;
         memset(&a, 0, sizeof(a));
-        a.src = src; a.n = B; a.n_tiles = (B + kTcTile - 1) / kTcTile; a.use_next = 1; a.gamma = l->cfg.gamma;
+        a.src = src; a.n = B; a.use_next = 1; a.gamma = l->cfg.gamma;
         a.actions = l->astar_buf; a.y_out = l->y_buf;
         if (l->cfg.algo != UAVRL_ALGO_DQN) {             // double DQN: a* = argmax_a q_local(s')
             a.img = l->tc_img_local; a.mode = kTcArgmax;
-            if ((rc = launch_tc_forward(l, a, st))) return rc;
+            if ((g.rc = launch_tc_forward(l, r, a, st))) return g;
             a.mode = kTcTdGather;
         } else {
             a.mode = kTcTdMax;
         }
         a.img = l->tc_img_target;
-        if ((rc = launch_tc_forward(l, a, st))) return rc;
+        if ((g.rc = launch_tc_forward(l, r, a, st))) return g;
         y_in = l->y_buf;
     }
-    if (mid) UAVRL_CUDA(cudaEventRecord(mid[0], st));
-    int nparts = grid, n_loss_parts = grid;
+    if ((g.rc = mark(marks, 0, st))) return g;
+    if (r.train) {
+        // the whole update on the tensor cores: forward + dX chain, then split-K weight gradients (tc_train.cu)
+        if ((g.rc = grow(l->rows_mem, l->train_cap, B, st, false,
+                         buf(l->act_buf, (size_t)l->G * B * (size_t)(l->tc.act_stride > 0 ? l->tc.act_stride : 4)),
+                         buf(l->dz_buf, (size_t)l->G * B * (size_t)l->tc.dz_stride))))
+            return g;
+        if ((g.rc = launch_tc_train(l, r, src, B, global_batch, y_in, &g.nparts, &g.n_loss_parts, st, marks ? marks[1] : nullptr)))
+            return g;
+    } else {
+        if ((g.rc = launch_fp32_update(l, src, B, global_batch, grid, y_in, st)) || (g.rc = mark(marks, 1, st))) return g;
+        g.nparts = g.n_loss_parts = grid;
+    }
+    g.rc = mark(marks, 2, st);
+    return g;
+}
+
+// hard_update (DuelingDQN_Trainer.py:199-202): the optimiser step of every update_loop-th epoch also copies local -> target
+static int hard_update_due(const uavrl_learner *l) { return (l->cfg.update_loop > 0 && (l->epoch % l->cfg.update_loop) == 0) ? 1 : 0; }
+
+// The optimiser step's arguments for the partials g.  apply: the Adam step follows the reduction; it counts one step and
+// copies local -> target when a hard update is due.
+static AdamArgs adam_args(uavrl_learner *l, const Grads &g, bool apply)
+{
     AdamArgs a;
     memset(&a, 0, sizeof(a));
-    a.P = l->net.P; a.apply = apply ? 1 : 0; a.world = l->world;
+    a.P = l->net.P; a.nparts = g.nparts; a.n_loss_parts = g.n_loss_parts; a.apply = apply ? 1 : 0; a.world = l->world;
     a.img_floats = l->net.smem_w_floats; a.tc_floats = l->tc.train_img_bytes / 4;
-    a.inv_b = 1.0f / (float)global_batch;
-    if (apply && !partials_only) {
+    a.inv_b = g.inv_b;
+    if (apply) {
         adam_hyper(a, l->cfg.lr, ++l->adam_t);
         a.hard = hard_update_due(l);
     }
-    if (tc_route && l->tc_train_ok) {
-        // the whole update on the tensor cores: forward + dX chain, then split-K weight gradients (tc_train.cu)
-        int rc;
-        if ((rc = grow(l->rows_mem, l->train_cap, B, st, false,
-                       buf(l->act_buf, (size_t)l->G * B * (size_t)(l->tc.act_stride > 0 ? l->tc.act_stride : 4)),
-                       buf(l->dz_buf, (size_t)l->G * B * (size_t)l->tc.dz_stride))))
-            return rc;
-        rc = launch_tc_train(l, src, B, global_batch, y_in, &nparts, &n_loss_parts, st, mid ? mid[1] : nullptr, fuse_td);
-        if (rc) return rc;
-    } else {
-    UpdateArgs ua;
-    ua.img_local = l->img_local; ua.img_target = l->img_target; ua.partials = l->partials; ua.loss_partials = l->loss_partials;
-    ua.B = B; ua.n_tiles = n_tiles; ua.algo = l->cfg.algo; ua.gamma = l->cfg.gamma; ua.dual = l->dual_weights;
-    ua.loss_kind = l->cfg.loss_kind; ua.img_floats = l->net.smem_w_floats;
-    ua.inv_global_b = 1.0f / (float)global_batch;
-    ua.y_in = y_in;
-    update_kernel<<<dim3(grid, l->G), kNetThreads, upd_smem_bytes(l->net, l->dual_weights), st>>>(l->net, src, ua);
-    l->pdl_prev = kPdlNone;
+    return a;
+}
+
+// reduce_adam_kernel, one grid row per trainer: reduce + Adam, reduce only (a.apply = 0), or Adam on the gradient already in
+// l->grad (a.nparts = 0)
+static int launch_reduce_adam_step(uavrl_learner *l, const AdamArgs &a, ChainKernel kind, float *loss_out, cudaStream_t st)
+{
+    UAVRL_CUDA(launch_reduce_adam(dim3((a.P + 63) / 64, l->G), st, l->chain.next(kind).pdl, a, learner_adam_ptrs(l, loss_out)));
+    l->chain.launched(kind);
     UAVRL_LAUNCHED();
-    if (mid) UAVRL_CUDA(cudaEventRecord(mid[1], st));
-    }
-    if (mid) UAVRL_CUDA(cudaEventRecord(mid[2], st));
-    l->last_nparts = nparts;
-    l->last_n_loss_parts = n_loss_parts;
-    l->last_global_batch = global_batch;
-    if (partials_only) {                                        // the data-parallel pair follows (launch_update_dp)
-        if (per_batch) return per_set(l, B, l->per.idx, nullptr, l->per.abs_err, 1, st);
-        return 0;
-    }
-    a.nparts = nparts; a.n_loss_parts = n_loss_parts;
-    const bool chain = l->pdl_chain && g_pdl.load();
-    UAVRL_CUDA(launch_reduce_adam(dim3((a.P + 63) / 64, l->G), st, chain && l->pdl_prev == kPdlDw && !mid, a,
-                                  learner_adam_ptrs(l, loss_out ? loss_out : l->loss_dev)));
-    l->pdl_prev = chain ? kPdlAdam : kPdlNone;
-    UAVRL_LAUNCHED();
-    if (per_batch) return per_set(l, B, l->per.idx, nullptr, l->per.abs_err, 1, st);      // ReplayTree.batch_update
     return 0;
+}
+
+// dp_allreduce_adam_kernel: this rank's partials g summed with every other rank's, then Adam
+static int launch_allreduce_adam(uavrl_learner *l, const Grads &g, float *loss_out, cudaStream_t st)
+{
+    l->comm_epoch += 1;
+    const int P = l->net.P;
+    const size_t stride = (size_t)P + 1;                                        // one rank's slot: gradient vector + loss share
+    const size_t parity_off = (size_t)(l->comm_epoch & 1u) * (size_t)l->world * stride;
+    const AdamArgs a = adam_args(l, g, true);
+    static const bool dp_trace = getenv("UAVRL_DP_TRACE") != nullptr;
+    if (dp_trace && !l->dp_trace) {
+        if (int rc = l->mem.alloc(l->dp_trace, 5, false)) return rc;
+        UAVRL_CUDA(cudaMemsetAsync(l->dp_trace, 0, 40, st));
+    }
+    UAVRL_CUDA(launch_kernel(dp_allreduce_adam_kernel, dim3((P + 63) / 64), dim3(256), 0, st, l->chain.next(kChainAdam).pdl, a,
+                             g.nparts, g.n_loss_parts, (const float *)l->partials, (const float *)l->loss_partials,
+                             (unsigned long long *const *)l->peer_grad_dev, (const unsigned long long *)l->comm_grad, stride, parity_off,
+                             l->rank, l->comm_epoch, learner_adam_ptrs(l, loss_out), l->dp_trace));
+    l->chain.launched(kChainAdam);
+    UAVRL_LAUNCHED();
+    return 0;
+}
+
+// ReplayTree.batch_update: the |Q - y| of a SumTree-sampled batch become its priorities
+static int per_write_back(uavrl_learner *l, const Grads &g, int B, cudaStream_t st)
+{
+    return g.per ? per_set(l, B, l->per.idx, nullptr, l->per.abs_err, 1, st) : 0;
+}
+
+int launch_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, bool apply, cudaStream_t st,
+                  cudaEvent_t *marks)
+{
+    const Grads g = launch_grads(l, src, B, global_batch, st, marks);
+    if (g.rc) return g.rc;
+    if (int rc = launch_reduce_adam_step(l, adam_args(l, g, apply), kChainAdam, loss_out ? loss_out : l->loss_dev, st)) return rc;
+    return per_write_back(l, g, B, st);
+}
+
+int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, cudaStream_t st)
+{
+    const Grads g = launch_grads(l, src, B, global_batch, st, nullptr);
+    if (g.rc) return g.rc;
+    if (int rc = launch_allreduce_adam(l, g, loss_out ? loss_out : l->loss_dev, st)) return rc;
+    return per_write_back(l, g, B, st);
 }
 
 static int repack_images(uavrl_learner *l, cudaStream_t st)
@@ -677,38 +756,6 @@ static int repack_images(uavrl_learner *l, cudaStream_t st)
     return 0;
 }
 
-// local gradient partials (same kernels as the single-GPU update, no optimiser step), then the exchange fused with Adam
-// (dp_allreduce_adam_kernel)
-int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, cudaStream_t st)
-{
-    int rc = launch_update_impl(l, src, B, global_batch, nullptr, false, st, nullptr, true);
-    if (rc) return rc;
-    l->comm_epoch += 1;
-    const int P = l->net.P;
-    const size_t stride = (size_t)P + 1;                                        // one rank's slot: gradient vector + loss share
-    const size_t parity_off = (size_t)(l->comm_epoch & 1u) * (size_t)l->world * stride;
-    const bool chain = l->pdl_chain && g_pdl.load();
-    AdamArgs a;
-    memset(&a, 0, sizeof(a));
-    a.P = P; a.apply = 1; a.world = l->world;
-    adam_hyper(a, l->cfg.lr, ++l->adam_t);
-    a.hard = hard_update_due(l);
-    a.inv_b = 1.0f / (float)global_batch;
-    static const bool dp_trace = getenv("UAVRL_DP_TRACE") != nullptr;
-    if (dp_trace && !l->dp_trace) {
-        if ((rc = l->mem.alloc(l->dp_trace, 5, false))) return rc;
-        UAVRL_CUDA(cudaMemsetAsync(l->dp_trace, 0, 40, st));
-    }
-    const int nblk = (P + 63) / 64;
-    UAVRL_CUDA(launch_kernel(dp_allreduce_adam_kernel, dim3(nblk), dim3(256), 0, st, chain && l->pdl_prev == kPdlDw, a, l->last_nparts,
-                             l->last_n_loss_parts, (const float *)l->partials, (const float *)l->loss_partials,
-                             (unsigned long long *const *)l->peer_grad_dev, (const unsigned long long *)l->comm_grad, stride, parity_off,
-                             l->rank, l->comm_epoch, learner_adam_ptrs(l, loss_out ? loss_out : l->loss_dev), l->dp_trace));
-    UAVRL_LAUNCHED();
-    l->pdl_prev = chain ? kPdlAdam : kPdlNone;
-    return 0;
-}
-
 void lockstep_commit(uavrl_learner *l, cudaStream_t st)
 {
     if (l->per.enabled) {
@@ -717,7 +764,6 @@ void lockstep_commit(uavrl_learner *l, cudaStream_t st)
         // tree gets the same Ng + Ng slots of its own env block
         const int64_t Ng = l->replay.N / l->G;
         per_fill_range(l, l->replay.head * Ng, 2 * Ng, per_new_priority(l->per), st, Ng, 0.0);
-        l->pdl_prev = kPdlNone;
     }
     l->replay.commit();
 }
@@ -938,12 +984,8 @@ static int do_update(uavrl_learner *l, const BatchSrc &src, int B, int global_ba
 {
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     // one Trainer.update call = TD pass(es) -> training chain -> weight gradients -> optimiser: chain them with PDL
-    // (the first kernel is launched plainly: whatever precedes it on the stream is not ours)
-    const bool outer = l->pdl_chain;
-    if (!outer) { l->pdl_chain = true; l->pdl_prev = kPdlNone; }
-    const int rc = launch_update(l, src, B, global_batch, loss_dev, apply, (cudaStream_t)stream);
-    if (!outer) { l->pdl_chain = false; l->pdl_prev = kPdlNone; }
-    return rc;
+    ChainScope chain(l->chain);
+    return launch_update(l, src, B, global_batch, loss_dev, apply, (cudaStream_t)stream);
 }
 
 int uavrl_learner_update(uavrl_learner *l, const int32_t *idx_tape_dev, float *loss_dev, void *stream)
@@ -1000,14 +1042,7 @@ int uavrl_learner_apply_grads(uavrl_learner *l, void *stream)
     if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
     if (int rc = refuse_grouped(l, "uavrl_learner_apply_grads (data-parallel training)")) return rc;
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    AdamArgs a;
-    memset(&a, 0, sizeof(a));
-    a.P = l->net.P; a.nparts = 0; a.apply = 1;
-    adam_hyper(a, l->cfg.lr, ++l->adam_t);
-    a.hard = hard_update_due(l);
-    UAVRL_CUDA(launch_reduce_adam(dim3((a.P + 63) / 64), (cudaStream_t)stream, false, a, learner_adam_ptrs(l, nullptr)));
-    UAVRL_LAUNCHED();
-    return 0;
+    return launch_reduce_adam_step(l, adam_args(l, Grads{}, true), kChainNone, nullptr, (cudaStream_t)stream);
 }
 
 int uavrl_learner_hard_update(uavrl_learner *l, void *stream)
@@ -1025,6 +1060,17 @@ int uavrl_learner_hard_update(uavrl_learner *l, void *stream)
         launch_copy(G * (size_t)(l->tc.train_img_bytes / 4), (const float *)l->tc_img_local, (float *)l->tc_img_target, st);
         UAVRL_LAUNCHED();
     }
+    return 0;
+}
+
+int uavrl_set_fuse_td(int32_t on) { g_fuse_td.store(on ? 1 : 0); return 0; }
+int uavrl_learner_td_fused(const uavrl_learner *l, int32_t batch) { return (l && learner_route(l, batch).td_fused) ? 1 : 0; }
+
+int uavrl_learner_tc_route(const uavrl_learner *l, int32_t n, int32_t *out)
+{
+    if (!l || !out || n <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    const Route r = learner_route(l, n);
+    out[0] = r.fwd; out[1] = r.train; out[2] = r.fwd_rows; out[3] = r.train_rows; out[4] = r.td_fused; out[5] = r.fp32_dual;
     return 0;
 }
 

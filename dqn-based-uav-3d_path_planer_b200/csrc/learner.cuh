@@ -124,6 +124,7 @@ struct uavrl_learner {
     // tensor-core forward path (act + TD target); tc_ok = the network fits the SMEM-resident wgmma kernel
     uavrl::TcNet tc;
     bool tc_ok = false;
+    bool tc_fixed_fwd = false, tc_fixed_train = false;   // tc_fixed_chains(tc, false / true), set by tc_init
     bool use_tc = true;               // runtime switch (uavrl_learner_set_tensor_cores): false = fp32 CUDA-core path
     int32_t is_train = 1;             // Trainer.Is_Train for the lockstep loops (uavrl_learner_set_is_train): 0 = always greedy
     unsigned char *tc_img_local = nullptr, *tc_img_target = nullptr;
@@ -146,9 +147,7 @@ struct uavrl_learner {
     int32_t G = 1;
     int64_t epoch = 0, adam_t = 0;
     uavrl::ReplayStore replay;        // int32 actions
-    // programmatic dependent launch chain of the lockstep loops (common.cuh)
-    bool pdl_chain = false;
-    int pdl_prev = 0;
+    uavrl::LaunchChain chain;         // programmatic dependent launch state of the learner's stream (launch_chain.cuh)
     // prioritised replay (per.cuh); off unless uavrl_per_enable was called
     uavrl::PerDev per = {};
     uint64_t per_calls = 0;
@@ -163,8 +162,6 @@ struct uavrl_learner {
     void *peer_grad_host[64] = { nullptr };
     bool comm_ready = false;
     unsigned comm_epoch = 0;          // tag of the latest exchange (launch_update_dp); 0 = never written
-    int last_nparts = 0, last_n_loss_parts = 0;
-    int last_global_batch = 0;
     // owners of the buffers above, one per group allocated and replaced together: parameters, images, maps and dp_trace; the
     // grown scratch (partials, y / astar, act / dz rows); the receive buffer; the peer table; the PER trees; their scratch
     uavrl::DevMem mem, parts_mem, td_mem, rows_mem, comm_mem, peer_mem, per_mem, per_scratch_mem;
@@ -265,6 +262,16 @@ void adam_hyper(AdamArgs &a, float lr, int64_t t);
 // every vector and image of a learner's optimiser step (trainer 0; the kernels offset by trainer)
 AdamPtrs learner_adam_ptrs(const uavrl_learner *l, float *loss_out);
 
+// Which kernels a pass over n rows per trainer takes on this learner, with its current switches (uavrl_learner_tc_route reports
+// it): the act / TD pass and the update's training kernel each run on the tensor cores (generic or FIXED variant) or not.
+struct Route {
+    int fwd, train;               // tensor-core act / TD pass, training kernel: 0 = not used (fp32 kernel), 1 = generic, 2 = FIXED
+    int fwd_rows, train_rows;     // their rows per tile (0 when not used)
+    bool td_fused;                // the TD-target pass(es) run inside the training kernel
+    bool fp32_dual;               // the fp32 update kernel keeps both networks' weights in shared memory at once
+};
+Route learner_route(const uavrl_learner *l, int n);
+
 // generic MLP description: trunk widths + head = `head_main` rows (+ `head_extra` rows from a second parameter block)
 int build_mlp(int in_dim, int n_hidden, const int32_t *hidden, int head_main, int head_extra, NetDev &n);
 int launch_act(uavrl_learner *l, const float *obs, int n, float eps, int is_train, const float *u_tape,
@@ -273,10 +280,13 @@ int launch_act(uavrl_learner *l, const float *obs, int n, float eps, int is_trai
 // (tc_forward.cuh TcArgs::loss_* for the row ranges), losses into loss_out[G][G]
 int launch_fed_loss(uavrl_learner *l, const float *probes, const float *q_ref, float *loss_out, int w0, int n_weights, bool tri,
                     cudaStream_t st);
-int launch_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out,
-                  bool apply, cudaStream_t st);
+// One Trainer.update of B transitions per trainer (global_batch: the batch the loss averages over): gradient step, reduce (+ Adam
+// when apply) into loss_out ([G]), prioritised-replay write-back.  marks (profiling, may be null): events recorded after the
+// TD-target pass, the training kernel and the weight-gradient kernel; they change no launch.
+int launch_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, bool apply, cudaStream_t st,
+                  cudaEvent_t *marks = nullptr);
+// the data-parallel form: the gradient step, then the NVLink all-reduce fused with Adam
 int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, cudaStream_t st);
-int launch_update_split(uavrl_learner *l, const BatchSrc &src, int B, cudaStream_t st, cudaEvent_t *mid);
 // the lockstep ring's commit plus, with prioritised replay, the priorities of the frames it makes and drops sampleable
 void lockstep_commit(uavrl_learner *l, cudaStream_t st = nullptr);
 }  // namespace uavrl

@@ -158,7 +158,7 @@ static int per_refresh(uavrl_learner *l, int n, const int32_t *slots, int64_t fi
     UAVRL_LAUNCHED();
     per_level_kernel<<<blocks, 256, 0, st>>>(p, n, slots, first, 2);
     UAVRL_LAUNCHED();
-    l->pdl_prev = kPdlNone;
+    l->chain.launched(kChainNone);
     return 0;
 }
 
@@ -197,7 +197,7 @@ int per_sample(uavrl_learner *l, int B, const double *u_tape, int32_t *slot_out,
     UAVRL_LAUNCHED();
     per_norm_kernel<<<dim3((B + 255) / 256, p.G), 256, 0, st>>>(B, p.w_raw, p.wmax_bits, w_out ? w_out : p.w);
     UAVRL_LAUNCHED();
-    l->pdl_prev = kPdlNone;
+    l->chain.launched(kChainNone);
     return 0;
 }
 

@@ -323,52 +323,37 @@ int stage_trace_print(cudaStream_t st, const long long *t, const char *fmt, ...)
     return 0;
 }
 
-int tc_forward_rows_per_tile(const TcNet &tc, int n)
-{
-    const int n_sm = num_sms();
-    return (n >= 128 * n_sm && tc.max_rows == 128) ? 128 : (n >= 64 * n_sm) ? 64 : 32;
-}
-
-int launch_tc_forward(uavrl_learner *l, const TcArgs &a_in, cudaStream_t st)
+int launch_tc_forward(uavrl_learner *l, const Route &r, const TcArgs &a_in, cudaStream_t st)
 {
     TcArgs a = a_in;
     a.img_stride = l->tc.train_img_bytes;
     const int n_sm = num_sms();
-    a.rows_per_tile = tc_forward_rows_per_tile(l->tc, a.n);
+    a.rows_per_tile = r.fwd_rows;
     a.n_tiles = (a.n + a.rows_per_tile - 1) / a.rows_per_tile;
     const int grid = a.n_tiles < n_sm ? a.n_tiles : n_sm;
     DevMem trace_mem;
     if (int rc = stage_trace_alloc(trace_mem, a.trace)) return rc;
-    // PDL chain state (see common.cuh): what this kernel may touch before its griddepcontrol.wait
-    const int prev = (l->pdl_chain && g_pdl.load()) ? l->pdl_prev : kPdlNone;
-    a.pdl = 0;
-    if (prev != kPdlNone) {
-        a.pdl = kPdlOn;
-        if (a.mode == kTcAct) {
-            if (prev == kPdlAdam) a.pdl |= kPdlEarlyRows;          // obs frame written by the env step, weights by Adam
-            else if (prev == kPdlEnv) a.pdl |= kPdlEarlyWeights;   // collection-only loop: weights untouched, obs just written
-        } else if (prev == kPdlEnv || prev == kPdlTd) {
-            a.pdl |= kPdlEarlyWeights;                             // neither the env step nor a TD pass writes weight images
-        }
-    }
-    UAVRL_CUDA(launch_kernel(pick_forward_kernel(a.mode == kTcAct, l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(grid, l->G), dim3(kTcThreads), tc_smem_bytes(l->tc), st, a.pdl != 0, l->tc, a));
-    l->pdl_prev = l->pdl_chain ? (a.mode == kTcAct ? kPdlAct : kPdlTd) : kPdlNone;
+    const ChainKernel kind = a.mode == kTcAct ? kChainAct : kChainTd;
+    const ChainLaunch c = l->chain.next(kind);
+    a.pdl = c.flags();
+    UAVRL_CUDA(launch_kernel(pick_forward_kernel(a.mode == kTcAct, l->tc.dueling != 0, r.fwd == 2), dim3(grid, l->G), dim3(kTcThreads), tc_smem_bytes(l->tc), st, c.pdl, l->tc, a));
+    l->chain.launched(kind);
     UAVRL_LAUNCHED();
     return stage_trace_print(st, a.trace, "[tc_trace] mode=%d n=%d R=%d grid=%d", a.mode, a.n, a.rows_per_tile, grid);
 }
 
-int launch_tc_loss(uavrl_learner *l, const TcArgs &a_in, int n_weights, int max_rows, cudaStream_t st)
+int launch_tc_loss(uavrl_learner *l, const Route &r, const TcArgs &a_in, int n_weights, int max_rows, cudaStream_t st)
 {
     TcArgs a = a_in;
     a.img_stride = l->tc.train_img_bytes;
-    a.rows_per_tile = tc_forward_rows_per_tile(l->tc, max_rows);
+    a.rows_per_tile = r.fwd_rows;
     const int step = (a.rows_per_tile / kFedProbes) * kFedProbes;
     const int tiles = (max_rows + step - 1) / step, n_sm = num_sms();
     a.n_tiles = tiles;
     a.pdl = 0;
-    UAVRL_CUDA(launch_kernel(pick_loss_kernel(l->tc.dueling != 0, tc_fixed_chains(l->tc, false)), dim3(tiles < n_sm ? tiles : n_sm, n_weights),
+    UAVRL_CUDA(launch_kernel(pick_loss_kernel(l->tc.dueling != 0, r.fwd == 2), dim3(tiles < n_sm ? tiles : n_sm, n_weights),
                              dim3(kTcThreads), tc_smem_bytes(l->tc), st, false, l->tc, a));
-    l->pdl_prev = kPdlNone;
+    l->chain.launched(kChainNone);
     UAVRL_LAUNCHED();
     return 0;
 }
@@ -378,7 +363,9 @@ int tc_init(uavrl_learner *l)
     std::vector<int32_t> hi, lo, hi2, lo2;
     l->tc_ok = false; l->tc_train_ok = false;
     if (tc_build(l->cfg, l->net, l->tc, hi, lo, hi2, lo2) != 0) return 0;
-    const bool fixed = tc_fixed_chains(l->tc, false);
+    l->tc_fixed_fwd = tc_fixed_chains(l->tc, false);
+    l->tc_fixed_train = tc_fixed_chains(l->tc, true);
+    const bool fixed = l->tc_fixed_fwd;
     size_t fwd_static = 0;                                       // the kernels' static shared memory (row table, barriers)
     for (int ac = 0; ac < 2; ++ac)
         for (int du = 0; du < 2; ++du) {

@@ -37,20 +37,18 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
              std::vector<int32_t> &hi2_map, std::vector<int32_t> &lo2_map);
 // tensor-core training path (tc_train.cu): forward + dX chain, then split-K dW; gradients land in l->partials
 int tc_train_init(uavrl_learner *l);
-int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, const float *y, int *n_grad_parts,
-                    int *n_loss_parts, cudaStream_t st, cudaEvent_t after_chain = nullptr, bool fused_td = false);
-// the TD-target pass(es) can run inside the training kernel (one tile per CTA): no separate launch_tc_forward TD calls
-bool tc_train_can_fuse_td(const uavrl_learner *l, int B);
-// rows per tile of an act / TD pass over n samples (launch_tc_forward) and of the training kernel for a batch of B
-int tc_forward_rows_per_tile(const TcNet &tc, int n);
-int train_rows_per_tile(const TcNet &tc, int B);
+// on route r = learner_route(l, B); after_chain (may be null): an event recorded after the training kernel
+int launch_tc_train(uavrl_learner *l, const Route &r, const BatchSrc &src, int B, int global_batch, const float *y, int *n_grad_parts,
+                    int *n_loss_parts, cudaStream_t st, cudaEvent_t after_chain);
 size_t tc_smem_bytes(const TcNet &tc);
 // every layer product (train: also those of the dX chain) has a compile-time wgmma chain (wgmma.cuh mma_fixed): the kernels'
 // FIXED variants apply
 bool tc_fixed_chains(const TcNet &tc, bool train);
-int launch_tc_forward(uavrl_learner *l, const TcArgs &a, cudaStream_t st);
-// the loss variant over n_weights weight sets (grid rows), max_rows = the most probe rows one of them evaluates
-int launch_tc_loss(uavrl_learner *l, const TcArgs &a, int n_weights, int max_rows, cudaStream_t st);
+// an act / TD pass over a.n rows per trainer on route r = learner_route(l, a.n)
+int launch_tc_forward(uavrl_learner *l, const Route &r, const TcArgs &a, cudaStream_t st);
+// the loss variant over n_weights weight sets (grid rows) on route r = learner_route(l, max_rows), max_rows = the most probe
+// rows one of them evaluates
+int launch_tc_loss(uavrl_learner *l, const Route &r, const TcArgs &a, int n_weights, int max_rows, cudaStream_t st);
 int tc_init(uavrl_learner *l);        // builds the TC images/maps; leaves l->tc_ok = false when the net does not fit
 
 // Stage timestamps of the tensor-core kernels (UAVRL_TC_TRACE=1, DESIGN §7): stage_trace_alloc gives a zeroed device buffer of

@@ -506,7 +506,7 @@ int tc_train_init(uavrl_learner *l)
     for (int i = 0; i < tc.n_layers; ++i)
         if (tc.L[i].K_real + 1 > 128 || tc.L[i].K_real % 4 != 0 || (tc.L[i].N_pad != 32 && tc.L[i].N_pad != 64)) return 0;   // ones column / float4 chunks / 1-2 blocks
     // a block's 227 KB hold the kernels' static shared memory (sample tables, barriers) as well as the dynamic allocation
-    const bool fixed = tc_fixed_chains(tc, true);
+    const bool fixed = l->tc_fixed_train;
     size_t train_static = 0, dw_static = 0;
     for (int np = 0; np < 3; ++np)
         for (int du = 0; du < 2; ++du) {
@@ -537,23 +537,8 @@ int tc_train_init(uavrl_learner *l)
     return 0;
 }
 
-std::atomic<int> g_fuse_td{1};               // uavrl_set_fuse_td(); default on
-// rows per tile of the training kernel: 32 while the batch fits one wave of 32-row tiles, else 64 (when the 64-row operands fit)
-int train_rows_per_tile(const TcNet &tc, int B)
-{
-    return (B > 32 * num_sms() && tc.train_max_rows == 64) ? 64 : 32;
-}
-bool tc_train_can_fuse_td(const uavrl_learner *l, int B)
-{
-    // one tile per CTA (32-row tiles up to 4 736 samples, 64-row tiles up to 9 472): the weight images are restaged inside the
-    // kernel, which only pays when a CTA does it once; larger batches keep the separate TD-target kernel(s) whose CTAs reuse
-    // one image over several tiles
-    if (!g_fuse_td.load() || !l->tc_train_ok) return false;
-    const int R = train_rows_per_tile(l->tc, B);
-    return (B + R - 1) / R <= num_sms();
-}
-int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, const float *y, int *n_grad_parts,
-                    int *n_loss_parts, cudaStream_t st, cudaEvent_t after_chain, bool fused_td)
+int launch_tc_train(uavrl_learner *l, const Route &r, const BatchSrc &src, int B, int global_batch, const float *y, int *n_grad_parts,
+                    int *n_loss_parts, cudaStream_t st, cudaEvent_t after_chain)
 {
     const TcNet &tc = l->tc;
     TcTrainArgs a;
@@ -561,23 +546,21 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     a.img = l->tc_img_local; a.src = src; a.B = B; a.y = y; a.inv_global_b = 1.0f / (float)global_batch;
     a.act_buf = l->act_buf; a.dz_buf = l->dz_buf; a.loss_partials = l->loss_partials;
     a.loss_kind = l->cfg.loss_kind;
-    a.fused_td = fused_td ? 1 : 0; a.algo = l->cfg.algo; a.gamma = l->cfg.gamma; a.img_target = l->tc_img_target;
+    a.fused_td = r.td_fused ? 1 : 0; a.algo = l->cfg.algo; a.gamma = l->cfg.gamma; a.img_target = l->tc_img_target;
     a.img_stride = tc.train_img_bytes;
-    a.R = train_rows_per_tile(tc, B);
+    a.R = r.train_rows;
     a.n_tiles = (B + a.R - 1) / a.R;
     const int grid = a.n_tiles < num_sms() ? a.n_tiles : num_sms();
-    const bool chain = l->pdl_chain && g_pdl.load();
-    if (fused_td && a.n_tiles > grid) return fail(UAVRL_ERR_INVALID, "fused TD needs one tile per CTA");
     TcDwArgs d;
     memset(&d, 0, sizeof(d));
     DevMem trace_mem;
     if (int rc = stage_trace_alloc(trace_mem, a.trace)) return rc;
     if (int rc = stage_trace_alloc(trace_mem, d.trace)) return rc;
-    const bool use_pdl = chain && (fused_td ? (l->pdl_prev == kPdlEnv) : (l->pdl_prev == kPdlTd));
-    const int npre = fused_td ? (l->cfg.algo != UAVRL_ALGO_DQN ? 2 : 1) : 0;
-    UAVRL_CUDA(launch_kernel(pick_train_kernel(npre, tc.dueling != 0, tc_fixed_chains(tc, true)), dim3(grid, l->G), dim3(kTcThreads),
-                             train_smem_bytes(tc, a.R), st, use_pdl, tc, a));
-    l->pdl_prev = chain ? kPdlTrain : kPdlNone;
+    const ChainKernel train = r.td_fused ? kChainTrainFusedTd : kChainTrain;
+    const int npre = r.td_fused ? (l->cfg.algo != UAVRL_ALGO_DQN ? 2 : 1) : 0;
+    UAVRL_CUDA(launch_kernel(pick_train_kernel(npre, tc.dueling != 0, r.train == 2), dim3(grid, l->G), dim3(kTcThreads),
+                             train_smem_bytes(tc, a.R), st, l->chain.next(train).pdl, tc, a));
+    l->chain.launched(train);
     UAVRL_LAUNCHED();
     if (after_chain) UAVRL_CUDA(cudaEventRecord(after_chain, st));
     d.src = src; d.B = B; d.n_chunks = (B + kDwChunk - 1) / kDwChunk; d.P = l->net.P;
@@ -587,8 +570,8 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
     const int max_slices = n_sm / tc.n_layers > 0 ? n_sm / tc.n_layers : 1;
     d.n_slices = d.n_chunks < max_slices ? d.n_chunks : max_slices;
     const int dw_grid = d.n_slices * tc.n_layers;
-    UAVRL_CUDA(launch_kernel(tc_dw_kernel, dim3(dw_grid, l->G), dim3(kTcThreads), dw_smem_bytes(tc), st, chain && !after_chain, tc, d));
-    l->pdl_prev = chain ? kPdlDw : kPdlNone;
+    UAVRL_CUDA(launch_kernel(tc_dw_kernel, dim3(dw_grid, l->G), dim3(kTcThreads), dw_smem_bytes(tc), st, l->chain.next(kChainDw).pdl, tc, d));
+    l->chain.launched(kChainDw);
     UAVRL_LAUNCHED();
     const int rc_train = stage_trace_print(st, a.trace, "[train_trace] B=%d R=%d fused_td=%d", B, a.R, a.fused_td);
     const int rc_dw = stage_trace_print(st, d.trace, "[dw_trace] B=%d chunks=%d (CTA 0 = layer 0)", B, d.n_chunks);
@@ -604,19 +587,4 @@ int launch_tc_train(uavrl_learner *l, const BatchSrc &src, int B, int global_bat
 extern "C" int uavrl_set_fuse_dw_adam(int32_t on)
 {
     return on ? uavrl::fail(UAVRL_ERR_INVALID, "uavrl_set_fuse_dw_adam: the fused weight-gradient + optimiser variant was removed") : 0;
-}
-extern "C" int uavrl_set_fuse_td(int32_t on) { uavrl::g_fuse_td.store(on ? 1 : 0); return 0; }
-extern "C" int uavrl_learner_td_fused(const uavrl_learner *l, int32_t batch) { return (l && l->tc_ok && l->use_tc && uavrl::tc_train_can_fuse_td(l, batch)) ? 1 : 0; }
-// the same decisions launch_act / launch_update_impl take (uavrl.h)
-extern "C" int uavrl_learner_tc_route(const uavrl_learner *l, int32_t n, int32_t *out)
-{
-    if (!l || !out || n <= 0) return uavrl::fail(UAVRL_ERR_INVALID, "bad argument");
-    const bool fwd = l->tc_ok && l->use_tc, train = fwd && l->tc_train_ok;
-    out[0] = fwd ? (uavrl::tc_fixed_chains(l->tc, false) ? 2 : 1) : 0;
-    out[1] = train ? (uavrl::tc_fixed_chains(l->tc, true) ? 2 : 1) : 0;
-    out[2] = fwd ? uavrl::tc_forward_rows_per_tile(l->tc, n) : 0;
-    out[3] = train ? uavrl::train_rows_per_tile(l->tc, n) : 0;
-    out[4] = (train && uavrl::tc_train_can_fuse_td(l, n)) ? 1 : 0;
-    out[5] = l->dual_weights;
-    return 0;
 }

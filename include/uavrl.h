@@ -434,7 +434,8 @@ int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float 
  * iterations (bench.py's roofline pass; on the CUDA-core path td_target and weight_grad are 0 because
  * fwd_bwd does everything; event gaps make the loop slower, never use it for throughput).  Refused before anything is
  * enqueued: in_dim != 100 or env and learner on different devices (UAVRL_ERR_INVALID, as uavrl_train_run), a pair that
- * has never run uavrl_train_run (UAVRL_ERR_STATE). */
+ * has never run uavrl_train_run or a ring that would hold <= batch_size transitions per trainer at the first update
+ * (UAVRL_ERR_STATE, as uavrl_train_run_dp). */
 int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, float *ms_out, void *stream);
 
 /* ---- prioritised experience replay (SURVEY.md 8f-3) ------------------------------------------------------------

@@ -499,11 +499,11 @@ R_N = 64
 
 
 def refusal_case(scenarios, case):
-    """(env, learner, call, code, message) of one refused train_run_dp call."""
+    """(env, learner, call, code, message) of one refused train_run_dp call, or train_profile call (case "profile-...")."""
     B, warm, kw, connect = 64, 3, {}, True
     if case == "grouped":
         kw, connect = dict(trainers=2), False
-    elif case == "cold-ring":
+    elif case in ("cold-ring", "profile-cold-ring"):
         B, warm = 256, 2                           # 128 transitions, 192 after the first iteration's commit: <= 256
     elif case == "lockstep-mismatch":
         kw, warm = dict(lockstep_envs=R_N // 2), 0
@@ -534,17 +534,21 @@ def refusal_case(scenarios, case):
         "in_dim-64": (ERR_INVALID, "in_dim must be 100"),
         "in_dim-128": (ERR_INVALID, "in_dim must be 100"),
         "cold-ring": (ERR_STATE, "replay holds <= batch_size transitions"),
+        "profile-cold-ring": (ERR_STATE, "replay holds <= batch_size transitions"),
     }[case]
+    if case.startswith("profile-"):
+        return env, L, (lambda: engine.train_profile(env, L, 2, 0.2)), expect
     return env, L, (lambda: engine.train_run_dp(env, L, 5, 0.2, gb)), expect
 
 
 @pytest.mark.parametrize("case", ["not-connected", "grouped", "gb0", "gb-neg", "lockstep-mismatch", "in_dim-64", "in_dim-128",
-                                  "cold-ring"])
+                                  "cold-ring", "profile-cold-ring"])
 def test_train_run_dp_refusals(scenarios, case):
     """train_run_dp refuses, before it launches anything and leaving env, ring, parameters and counters as they were: a learner
     not connected, a grouped learner, global_batch <= 0, lockstep_envs != env.n, a learner whose in_dim is not the 100-float
     observation (the env step writes 100-float rows into the ring), and a ring that would hold <= batch_size transitions at
-    the first update (every rank must take part in every exchange)."""
+    the first update (every rank must take part in every exchange).  train_profile refuses that ring the same way (every
+    iteration's update is timed)."""
     env, L, call, (code, match) = refusal_case(scenarios, case)
     assert_refused(call, code, match, [(env, L)])
     env.close(); L.close()
