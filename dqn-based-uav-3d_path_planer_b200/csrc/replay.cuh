@@ -44,8 +44,8 @@ struct BatchSrc {
 constexpr uint64_t kActSalt = 0xAC7ull, kSampleSalt = 0x5EEDull, kFedSalt = 0xFEDull, kPerSalt = 0x9E12ull;
 __host__ __device__ __forceinline__ uint64_t trainer_key(uint64_t key, uint64_t salt, int g) { return ((key ^ salt) + (uint64_t)g) ^ salt; }
 
-#if defined(__CUDACC__)
-__device__ __forceinline__ uint32_t mix32(uint32_t x)
+// Host and device: the host compile lets the sampler be checked without a GPU.
+__host__ __device__ __forceinline__ uint32_t mix32(uint32_t x)
 {
     x ^= x >> 16; x *= 0x7feb352dU; x ^= x >> 15; x *= 0x846ca68bU; x ^= x >> 16;
     return x;
@@ -54,7 +54,7 @@ __device__ __forceinline__ uint32_t mix32(uint32_t x)
 // i-th element of a keyed pseudo-random permutation of [0, M): 4-round Feistel on 2*h bits with
 // cycle walking.  perm(0..B-1) = B distinct uniform indices = random.sample(range(M), B)
 // (BaseClass/replay_buffer.py:49).
-__device__ __forceinline__ uint64_t perm_index(uint64_t i, uint64_t M, const uint32_t key[4])
+__host__ __device__ __forceinline__ uint64_t perm_index(uint64_t i, uint64_t M, const uint32_t key[4])
 {
     int bits = 1;
     while ((1ull << bits) < M) ++bits;
@@ -75,6 +75,7 @@ __device__ __forceinline__ uint64_t perm_index(uint64_t i, uint64_t M, const uin
     return x;
 }
 
+#if defined(__CUDACC__)
 // Trainer g's view of a batch source (grouped learner: gridDim.y = G trainers, B rows each).  Explicit batches: block g of the
 // G x B rows.  Lockstep ring: env block [g n_envs, (g + 1) n_envs), trainer g's sampling key and row g of a [G][B] index tape.
 // Both: row g of [G][B] importance weights and |Q - y| outputs (prioritised replay).
