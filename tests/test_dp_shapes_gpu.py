@@ -16,31 +16,19 @@ import pytest
 import torch
 
 import oracle as O
-from gpu_util import city_and_params
-from test_qnet_shapes_gpu import expected_route, shape_id
-from test_tc_gpu import big_inputs, dev, net_layers
-from test_weighted_f64_cpu import draw_batch, f64_update_w
-from test_weighted_update_shapes_gpu import FIXED_SHIPPED, LEGS, ROUTES
+from gpu_util import city_and_params, dev, n_sm  # noqa: F401  (module fixture)
+from qnet_restatement import big_inputs, draw_batch, f64_update, net_layers
+from qnet_restatement import loss_kind_reset  # noqa: F401  (fixture)
+from shapes import FIXED_SHIPPED, LEGS, ROUTES, SHIPPED, expected_route, shape_id
 from uavrl_b200 import _lib, engine
 
 pytestmark = pytest.mark.gpu
 
-SHIPPED = next(s for s in ROUTES if s[:4] == (100, [64, 64], 27, 0))
+SHIPPED_ROUTE = next(s for s in ROUTES if s[:4] == SHIPPED[0])
 GENERIC = next(s for s in ROUTES if s[4][0] == "generic" and s[4][1] == "generic")
 FP32 = next(s for s in ROUTES if s[4][0] is None)
 KINDS = ("mse", "huber")
 LR = 5e-4
-
-
-@pytest.fixture(scope="module")
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-@pytest.fixture
-def loss_kind_reset():
-    yield
-    O.set_loss_kind("mse")            # the oracle's loss kind is process-wide state
 
 
 def algo_of(leg, dueling):
@@ -182,7 +170,7 @@ def test_global_batch_scaling_vs_float64(dqn_golden, shape, kind, n_sm):
             s, a, r, s2, d, _, redrawn = draw_batch(dqn_golden, rng, layers, dueling, algo, [local], target, B, in_dim,
                                                     n_actions, kind, False)
             assert max(redrawn.values()) <= 0.05 * B + 4, (step, redrawn)
-            l64, g64, _, _, mag64 = f64_update_w(layers, algo, dueling, local, target, s, a, r, s2, d, None, kind, abs_terms=True)
+            l64, g64, _, _, mag64 = f64_update(layers, algo, dueling, local, target, s, a, r, s2, d, None, kind, abs_terms=True)
             for L in pair:                      # B transitions, then one dummy: capacity B + 1, logical index i = slot i
                 push(L, s, a, r, s2, d)
                 push(L, s[:1], a[:1], r[:1], s2[:1], d[:1])
@@ -213,7 +201,7 @@ def _c_cases():
         for B in C_ALGO:
             for kind in KINDS:
                 out.append(pytest.param(shape, 2, B, kind, id="%s-W2-B%d-%s" % (shape_id(shape), B, kind)))
-    for shape in (SHIPPED, GENERIC, FP32):
+    for shape in (SHIPPED_ROUTE, GENERIC, FP32):
         for W in (3, 8):
             for B in (37, 64):
                 for kind in KINDS:
@@ -257,7 +245,7 @@ def test_simulated_allreduce_vs_float64_and_oracle(dqn_golden, shape, W, B, kind
         s, a, r, s2, d, _, redrawn = draw_batch(dqn_golden, rng, layers, dueling, algo, [local], target, n, in_dim, n_actions,
                                                 kind, False)
         assert max(redrawn.values()) <= 0.05 * n + 4, (step, redrawn)
-        l64, g64, _, _, mag64 = f64_update_w(layers, algo, dueling, local, target, s, a, r, s2, d, None, kind, abs_terms=True)
+        l64, g64, _, _, mag64 = f64_update(layers, algo, dueling, local, target, s, a, r, s2, d, None, kind, abs_terms=True)
         _, g_or, _ = OL.update(s, a, r, s2, d, is_w=np.ones(n, np.float32))
         for q, L in enumerate(ranks):
             sh = slice(q * B, (q + 1) * B)
@@ -298,7 +286,7 @@ def test_simulated_allreduce_vs_float64_and_oracle(dqn_golden, shape, W, B, kind
 # ---------------------------------------------------------------------------------------------------------------------
 # d. prioritised replay: the SumTree draws the batch, and every form refreshes it the same way
 @pytest.mark.parametrize("B", [64, 4096])
-@pytest.mark.parametrize("shape", [SHIPPED, GENERIC, FP32], ids=shape_id)
+@pytest.mark.parametrize("shape", [SHIPPED_ROUTE, GENERIC, FP32], ids=shape_id)
 def test_per_forms_are_bit_identical(dqn_golden, shape, B, n_sm):
     """A (update), B (compute_grads + apply_grads) and C (connect_self + update_dp) with prioritised replay on, the same seed
     and no index tape, over a wrapped flat replay with random priorities: after each of 5 steps the parameters, Adam moments,
@@ -590,7 +578,7 @@ def test_compute_grads_and_update_dp_refuse_cold_replay(dqn_golden):
     transition and both run, at epoch 1."""
     B = 64
     rng = np.random.default_rng(3)
-    shape = SHIPPED
+    shape = SHIPPED_ROUTE
     pair = [make(shape, engine.ALGO_DDQN, B, 4 * B) for _ in range(2)]
     Bl, C = pair
     C.connect_self()

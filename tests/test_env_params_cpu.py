@@ -11,7 +11,7 @@ import pytest
 
 import oracle as O
 from conftest import GOLDEN, episode
-from test_env_core_host import shim, shim_step  # noqa: F401  (module fixture: the host compile of env_core.cuh)
+from env_core_shim import shim, shim_step  # noqa: F401  (module fixture: the host compile of env_core.cuh)
 
 F64 = ("px", "py", "pz", "vx", "vy", "V", "score", "total_score", "path_len")
 

@@ -2,29 +2,24 @@
 PathPlan_City.Federated_Learning_choice :644-684) on the device.
 
 The judge is the numpy restatement tests/fl_restatement.py, pinned to the reference's own run in test_federate_cpu.py.
-Each trainer changes only in its own round, so round p is fully determined by the final parameters of the trainers
-q < p, the initial parameters of the trainers q > p and its probes: every round is checked on its own --
-float64 losses within a magnitude bound, a selection that is the (loss, index)-sorted prefix up to float64 near-ties,
-and theta_p bit for bit the float32 in-order average of the selection the device made."""
+Each trainer changes only in its own round, so every round is checked on its own (fl_restatement.check_rounds)."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
-import fl_restatement as flr
-from gpu_util import city_and_params
-from test_qnet_shapes_gpu import SHAPES
+from fl_restatement import check_rounds
+from gpu_util import DEV, ROOT, city_and_params, env_dict
+from shapes import SHAPES, pick
 from uavrl_b200 import _lib, engine
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
 S = 10
-# one shape per route (test_qnet_shapes_gpu.SHAPES): tensor-core FIXED, tensor-core generic, fp32 only (in_dim % 4 != 0)
-ROUTES = {"fixed": (100, [60], 27, 1), "generic": (100, [64, 32], 27, 1), "fp32": (99, [64], 27, 0)}
-for _s in ROUTES.values():
+# one network per route of shapes.SHAPES: tensor-core FIXED, tensor-core generic, fp32 only (in_dim % 4 != 0)
+ROUTE_NETS = {"fixed": pick(100, [60], 27, 1)[:4], "generic": pick(100, [64, 32], 27, 1)[:4], "fp32": pick(99, [64], 27, 0)[:4]}
+for _s in ROUTE_NETS.values():
     assert any(tuple(x[:4]) == (_s[0], _s[1], _s[2], _s[3]) for x in SHAPES), _s
 
 
@@ -44,74 +39,6 @@ def make(shape, G, seed=3, tc=True, **kw):
 
 def snapshot(L):
     return [L.get_params(w).reshape(L.G, L.P).copy() for w in range(4)], L.counters()
-
-
-def net_of(shape):
-    in_dim, hidden, nA, dueling = shape
-    return (in_dim, list(hidden), nA, bool(dueling))
-
-
-def magnitude(theta, x, net):
-    """|Q| bound per row and action: the forward with |W|, |b| and |x| (ReLU never increases a magnitude)."""
-    in_dim, hidden, nA, dueling = net
-    off, h, blocks = 0, np.abs(np.asarray(x, np.float64)), []
-    for r, c in flr.layers(in_dim, hidden, nA, dueling):
-        W = np.abs(theta[off:off + r * c].astype(np.float64)).reshape(r, c); off += r * c
-        b = np.abs(theta[off:off + r].astype(np.float64)); off += r
-        blocks.append((W, b))
-    for W, b in blocks[:len(hidden)]:
-        h = h @ W.T + b
-    A = h @ blocks[len(hidden)][0].T + blocks[len(hidden)][1]
-    if dueling:
-        V = h @ blocks[len(hidden) + 1][0].T + blocks[len(hidden) + 1][1]
-        A = V + 2 * A.max(axis=1, keepdims=True) + A
-    return A
-
-
-def check_rounds(before, after, probes, losses, chosen, shape, rounds):
-    """Item-by-item check of the rounds `rounds` (see the module docstring)."""
-    net = net_of(shape)
-    G = before.shape[0]
-    k = (G - 1) // 2
-    gamma = 8e-6 * (len(net[1]) + 1)                      # fp32-grade forward: relative error per layer of the magnitude chain
-    for p in rounds:
-        cur = np.concatenate([after[:p], before[p:]])
-        x = probes[p]
-        own = flr.forward64(cur[p], x, *net)
-        mag_p = magnitude(cur[p], x, net)
-        m64, tol = np.zeros(G), np.zeros(G)
-        for q in range(G):
-            if q == p:
-                continue
-            Qq = flr.forward64(cur[q], x, *net)
-            d = own - Qq
-            m64[q] = np.mean(d * d)
-            delta = gamma * (mag_p + magnitude(cur[q], x, net))
-            tol[q] = np.mean(2 * np.abs(d) * delta + delta * delta) + 1e-6 * m64[q] + 1e-30
-        got = losses[p].astype(np.float64)
-        assert got[p] == 0.0
-        bad = np.abs(got - m64) > tol
-        assert not bad.any(), (p, np.nonzero(bad)[0][:5], got[bad][:5], m64[bad][:5], tol[bad][:5])
-        if k == 0:
-            assert (chosen[p] == -1).all()
-            assert np.array_equal(after[p], before[p])
-            continue
-        c = [int(v) for v in chosen[p][:k]]
-        assert len(set(c)) == k and p not in c and all(0 <= v < G for v in c), (p, c)
-        # the device's own ranking: (loss, index) order along the chosen list
-        for a, b in zip(c, c[1:]):
-            assert (got[a], a) < (got[b], b), (p, c)
-        # against float64: a chosen trainer may only beat an unchosen one it lies within the bounds of
-        rest = [q for q in range(G) if q != p and q not in c]
-        if rest:
-            worst = max(c, key=lambda q: m64[q] - tol[q])
-            best = min(rest, key=lambda q: m64[q] + tol[q])
-            assert m64[worst] - tol[worst] <= m64[best] + tol[best], (p, worst, best)
-            ref = flr.rank(m64, p)
-            for q in set(c) ^ set(ref):
-                others = [r for r in (set(c) | set(ref)) if r != q]
-                assert any(abs(m64[q] - m64[r]) <= tol[q] + tol[r] for r in others), (p, q)
-        assert np.array_equal(after[p], flr.average(cur, p, c)), "round %d: theta_p is not the in-order float32 average" % p
 
 
 def run_explicit(L, probes):
@@ -147,12 +74,12 @@ def test_golden_bit_for_bit(fl_golden, name, tc):
 
 
 # ---------------------------------------------------------------- 2. every round at every route
-LEGS = [(r, tc, G) for r in ROUTES for tc in ((True, False) if r != "fp32" else (False,)) for G in (2, 3, 8, 33, 256)]
+LEGS = [(r, tc, G) for r in ROUTE_NETS for tc in ((True, False) if r != "fp32" else (False,)) for G in (2, 3, 8, 33, 256)]
 
 
 @pytest.mark.parametrize("route,tc,G", LEGS, ids=["%s-%s-G%d" % (r, "tc" if t else "fp32", g) for r, t, g in LEGS])
 def test_rounds_vs_float64(route, tc, G):
-    shape = ROUTES[route]
+    shape = ROUTE_NETS[route]
     L = make(shape, G, seed=5 + G, tc=tc)
     rng = np.random.default_rng(G)
     probes = rng.uniform(-1, 1, size=(G, S, shape[0])).astype(np.float32)
@@ -169,7 +96,7 @@ def test_rounds_vs_float64(route, tc, G):
 # ---------------------------------------------------------------- 3. weight images refreshed
 @pytest.mark.parametrize("route,tc", [("fixed", True), ("generic", True), ("fixed", False)])
 def test_images_refreshed(route, tc):
-    shape, G = ROUTES[route], 8
+    shape, G = ROUTE_NETS[route], 8
     L = make(shape, G, seed=9, tc=tc)
     rng = np.random.default_rng(1)
     run_explicit(L, rng.uniform(-1, 1, size=(G, S, shape[0])).astype(np.float32))
@@ -290,19 +217,10 @@ def test_refusals(env_golden, env27_golden):
 # ---------------------------------------------------------------- 7. the env plug-in
 def test_env_plugin_is_fl(tmp_path):
     import importlib
-    from uavrl_b200.plugins import xmlconfig
     cwd = os.getcwd()
     os.chdir(ROOT)
     mod = importlib.import_module("uavrl_b200.plugins.PathPlan_City_B200")
     orig = mod.XML2Dict
-
-    def env_dict(**kw):
-        ed = xmlconfig.XML2Dict(os.path.join(ROOT, "configs", "PathPlan_City_B200.xml"))["simulator"]["env"]
-        ed["num_UAV"], ed["scenario_pool"], ed["num_trainers"] = "8", "64", "8"
-        ed["Obstacles"]["buildings"] = os.path.join(ROOT, "configs", "buildings.xml")
-        ed["Agent"]["Trainer"]["Trainer_path"] = os.path.join(ROOT, "configs", "Trainer_DDQN_B200.xml")
-        ed.update(kw)
-        return ed
 
     def patched(path):
         d = orig(path)
@@ -311,7 +229,7 @@ def test_env_plugin_is_fl(tmp_path):
         return d
     mod.XML2Dict = patched
     try:
-        env = mod.PathPlan_City_B200(env_dict(Is_FL="1", FL_Loop="2"))
+        env = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml", Is_FL="1", FL_Loop="2"))
         L = env.Trainer._learner
         calls, fed = [], L.federate
         L.federate = lambda *a, **k: (calls.append(env.epoch), fed(*a, **k))[1]
@@ -321,7 +239,7 @@ def test_env_plugin_is_fl(tmp_path):
             changed = not np.array_equal(before, L.get_params(0))
             assert changed                                # training (and, on even episodes, aggregation) moved q_local
         assert calls == [2, 4]
-        off = mod.PathPlan_City_B200(env_dict())
+        off = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml"))
         assert off.Is_FL == 0 and off.FL_Loop == 3
 
         def boom(*a, **k):
@@ -329,8 +247,8 @@ def test_env_plugin_is_fl(tmp_path):
         off.Trainer._learner.federate = boom
         off.run_eposide(0.3)
         with pytest.raises(ValueError, match="Is_AC"):
-            mod.PathPlan_City_B200(env_dict(Is_FL="1", Is_AC="1"))
-        single = mod.PathPlan_City_B200(env_dict(Is_FL="1", FL_Loop="1", num_trainers="1"))
+            mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml", Is_FL="1", Is_AC="1"))
+        single = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml", Is_FL="1", FL_Loop="1", num_trainers="1"))
         single.Trainer._learner.federate = boom
         single.run_eposide(0.3)                          # one trainer: accepted, nothing to aggregate
     finally:

@@ -1,21 +1,14 @@
-"""Federated_Learning_AC (Envs/PathPlan_City.py:590-601) restated in numpy and pinned, bit for bit, to the reference's own run
-(tests/golden/fl_ac_golden.npz, made by make_fl_ac_golden.py on real reference SAC trainers).  No GPU: this fixes what the
+"""Federated_Learning_AC (Envs/PathPlan_City.py:590-601) restated in numpy (fl_restatement.federate_actors) and pinned, bit
+for bit, to the reference's own run (tests/golden/fl_ac_golden.npz, made by make_fl_ac_golden.py on real reference SAC
+trainers).  No GPU: this fixes what the
 device kernel (uavrl_sac_federate_actors) must compute before any GPU test compares against it."""
 import os
 
 import numpy as np
 
+from fl_restatement import federate_actors
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "fl_ac_golden.npz")
-
-
-def federate_actors(actors):
-    """Every actor <- the float32 sum theta_0 + theta_1 + ... + theta_{G-1}, added left to right in trainer order.  The
-    reference's division by G assigns into a temporary state_dict and is lost, so nothing is divided."""
-    actors = np.asarray(actors, np.float32)
-    s = actors[0].copy()
-    for g in range(1, actors.shape[0]):
-        s = np.add(s, actors[g], dtype=np.float32)
-    return np.broadcast_to(s, actors.shape).copy()
 
 
 def test_restatement_matches_reference_golden():

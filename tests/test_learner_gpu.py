@@ -7,16 +7,12 @@ import pytest
 import torch
 
 import oracle as O
+from gpu_util import dev
 
 pytestmark = pytest.mark.gpu
 
 CASES = {"dueling_vanet2": ([64], 1, 2), "dueling_vanet3": ([128, 64], 1, 2),
          "ddqn_qvalue3": ([64, 64], 0, 1), "dqn_qvalue3": ([64, 64], 0, 0), "dqn_qnet2": ([64], 0, 0)}
-
-
-def dev(x, dt=None):
-    t = torch.as_tensor(np.ascontiguousarray(x)).cuda()
-    return t if dt is None else t.to(dt)
 
 
 @pytest.mark.parametrize("name", list(CASES))

@@ -94,14 +94,11 @@ def test_fused_allreduce_pair_world1_equals_plain_update(dqn_golden):
     Adam arithmetic), through hard updates and both parities of the double-buffered receive buffer; the loss is the batch
     loss."""
     import numpy as np
+    from gpu_util import dev
     from uavrl_b200 import engine
     g = dqn_golden
     s = g["batch_s"].reshape(-1, 100)[:300]; s2 = g["batch_s2"].reshape(-1, 100)[:300]
     a = g["batch_a"].reshape(-1)[:300]; r = g["batch_r"].reshape(-1)[:300]; d = g["batch_d"].reshape(-1)[:300]
-
-    def dev(x, dt=None):
-        t = torch.as_tensor(np.ascontiguousarray(x)).cuda()
-        return t if dt is None else t.to(dt)
     Ls = []
     for _ in range(2):
         L = engine.Learner(100, [64, 64], 27, False, engine.ALGO_DDQN, batch_size=256, replay_capacity=300, update_loop=2)

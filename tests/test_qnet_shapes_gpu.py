@@ -1,61 +1,21 @@
 """Q-network shapes beyond the shipped ones (input 100, hidden [64, 64] / [64] / [128, 64], 27 actions) against a float64
-reference: the learner accepts in_dim 1-128, 1-4 hidden layers of up to 128 units and 1-31 actions, and the host routes each
-shape to one of several kernel variants.  The tensor-core act / TD kernel and training kernel come as a FIXED variant
-(compile-time wgmma chains, wgmma.cuh mma_fixed) and a generic one (runtime k-step chains, 16-column tail chunks); shapes
-that do not fit the training kernel get tensor-core TD targets feeding the fp32 update kernel, and shapes that do not fit
-the tensor-core kernels at all run fp32 only.  SHAPES names the route each shape must take (pinned through
-Learner.route), so every variant is compared by value here and a shape that silently moves to another route fails."""
+reference: every row of shapes.SHAPES, with the route it must take pinned through Learner.route, so every kernel variant is
+compared by value here and a shape that silently moves to another route fails."""
 import numpy as np
 import pytest
 import torch
 
 import oracle as O
-from test_tc_gpu import big_inputs, dev, f64_forward, f64_unpack, f64_update, net_layers
+from gpu_util import dev, n_sm  # noqa: F401  (module fixture)
+from qnet_restatement import big_inputs, f64_forward, f64_unpack, f64_update, near_relu_kink, net_layers
+from shapes import SHAPES, SHIPPED, act_sizes, expected_route, shape_id
 from uavrl_b200 import engine
 
 pytestmark = pytest.mark.gpu
 
-SHIPPED = [(100, [64, 64], 27, 0), (100, [64], 27, 0), (100, [64], 27, 1), (100, [128, 64], 27, 1)]
-
-# (in_dim, hidden, n_actions, dueling, expected route): the route is (tensor-core act / TD kernel, tensor-core training
-# kernel, forward tiles can reach 128 rows, training tiles can reach 64 rows, fp32 update kernel keeps both networks in
-# shared memory).  The kernels' static shared memory counts against the 227 KB too: the last shape's tensor-core image fits
-# only without it, and (32, [64, 64, 64]) trains in 32-row tiles for that reason.
-SHAPES = [
-    # generic forward + generic training kernel
-    (100, [32], 27, 0, ("generic", "generic", True, True, True)),           # head over K = 32: 4 k-steps
-    (100, [64, 32], 27, 1, ("generic", "generic", True, True, True)),       # 32-wide hidden layer into a dueling head
-    (96, [64, 64], 27, 0, ("generic", "generic", False, True, True)),       # layer 0 over 12 k-steps
-    (36, [64], 27, 0, ("generic", "generic", True, True, True)),            # layer 0 over 5 k-steps, in_dim padded to 40
-    (12, [32, 32, 32, 32], 7, 1, ("generic", "generic", True, True, True)),  # 4 hidden layers: hm3 / hm4, dX over 5 layers
-    (32, [64, 64, 64], 8, 0, ("generic", "generic", True, False, True)),    # 3 hidden layers of 64; 64-row training tiles do not fit
-    (100, [20], 5, 0, ("generic", "generic", True, True, True)),            # 20 units padded to 32, 5 actions
-    # FIXED forward + FIXED training kernel at shapes that are not shipped
-    (100, [60], 27, 1, ("fixed", "fixed", True, True, True)),               # 4 zero units per 64
-    (100, [64], 31, 1, ("fixed", "fixed", True, True, True)),               # V at head column 31
-    (100, [64], 31, 0, ("fixed", "fixed", True, True, True)),               # every head column an action
-    (124, [64], 27, 0, ("fixed", "fixed", False, True, True)),              # dW: 16 k-steps, ones column at row 124
-    # tensor-core TD targets feeding the fp32 update kernel
-    (100, [48], 27, 0, ("generic", None, True, False, True)),                # 32 + 16-column tail chunk
-    (100, [112], 27, 0, ("generic", None, False, False, True)),              # 64 + 32 + 16-column tail chunk
-    (128, [64], 27, 0, ("fixed", None, False, False, True)),                 # in_dim 128: no room for the dW ones column
-    (100, [64, 64, 64], 27, 0, ("fixed", None, False, False, False)),        # training image too large; fp32 single-weights mode
-    (64, [64, 64, 64, 64], 27, 1, ("fixed", None, False, False, False)),     # 4 hidden layers in the act / TD kernel
-    # fp32 only
-    (100, [128, 64, 64], 27, 1, (None, None, False, False, False)),          # VAnet4 at hiden_dim 64
-    (99, [64], 27, 0, (None, None, False, False, True)),                     # in_dim % 4 != 0
-    (12, [128, 64, 64], 27, 0, (None, None, False, False, True)),            # 64-row image fits only without the static smem
-]
-
 
 def rup(x, m):
     return -(-x // m) * m
-
-
-def shape_id(s):
-    in_dim, hidden, n_actions, dueling, (fwd, train, _, _, _) = s
-    return "%d-%s-%d%s-fwd_%s-train_%s" % (in_dim, "x".join(map(str, hidden)), n_actions, "-duel" if dueling else "",
-                                          fwd or "fp32", train or "fp32")
 
 
 def test_table_covers_every_route():
@@ -73,42 +33,12 @@ def test_table_covers_every_route():
             assert r[0] == "generic", "a 16-column chunk has no FIXED chain"
 
 
-@pytest.fixture(scope="module")
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def act_sizes(route, n_sm):
-    """1000 (32-row tiles), 64 n_sm + 37 (64-row tiles) and, where forward tiles reach 128 rows, 128 n_sm + 101."""
-    return [1000, 64 * n_sm + 37] + ([128 * n_sm + 101] if route[2] else [])
-
-
 UPDATE_LEGS = {                        # B, algo: fused TD with NPRE = 1 / 2, fused TD with 64-row tiles, separate TD passes
     "B64-dqn": (64, engine.ALGO_DQN),
     "B64-ddqn": (64, engine.ALGO_DDQN),
     "B6000-ddqn": (6000, engine.ALGO_DDQN),
     "B12000-dqn": (12000, engine.ALGO_DQN),
 }
-
-
-def expected_route(route, n, n_sm, tc=True):
-    fwd, train, fwd128, train64, dual = route if tc else (None, None, False, False, route[4])
-    fwd_rows = None if fwd is None else 128 if (n >= 128 * n_sm and fwd128) else 64 if n >= 64 * n_sm else 32
-    train_rows = None if train is None else 64 if (n > 32 * n_sm and train64) else 32
-    return dict(tc_fwd=fwd, tc_train=train, fwd_rows=fwd_rows, train_rows=train_rows,
-                td_fused=train is not None and -(-n // train_rows) <= n_sm, fp32_dual=dual)
-
-
-def near_relu_kink(P, dueling, x, rel=2e-5):
-    """Rows of x for which a hidden pre-activation of the float64 network P lies within rel x (the sum of its terms'
-    magnitudes) of 0: 3xTF32 products (2^-21) and fp32 sums over <= 128 terms stay well inside that."""
-    h = np.asarray(x, np.float64)
-    near = np.zeros(h.shape[0], bool)
-    for W, b in P[:len(P) - (2 if dueling else 1)]:
-        z = h @ W.T + b
-        near |= (np.abs(z) <= rel * (np.abs(h) @ np.abs(W).T + np.abs(b))).any(1)
-        h = np.maximum(z, 0.0)
-    return near
 
 
 def make_learner(shape, algo=engine.ALGO_DQN):
@@ -209,7 +139,7 @@ def test_update_vs_float64_and_oracle(dqn_golden, shape, leg, n_sm):
             # pick different a*: such samples are marked terminal (as test_tc_update_large_batch_vs_oracle does)
             ql = np.sort(O.net_forward(net, L.get_params(0), s2).astype(np.float64), 1)
             d[(ql[:, -1] - ql[:, -2]) < 1e-3] = 1.0
-        l64, g64 = f64_update(layers, algo, dueling, L.get_params(0), L.get_params(1), s, a, r, s2, d)
+        l64, g64 = f64_update(layers, algo, dueling, L.get_params(0), L.get_params(1), s, a, r, s2, d)[:2]
         L.update_batch(dev(s), dev(a), dev(r), dev(s2), dev(d), loss)
         lo, _ = OL.update(s, a, r, s2, d)
         torch.cuda.synchronize()

@@ -16,10 +16,10 @@ import torch
 
 import oracle as O
 import replay_restatement as R
-from gpu_util import city_and_params
-from test_qnet_shapes_gpu import SHAPES, expected_route
-from test_sac_shapes_gpu import HP, check_step, near_decision, read_state, sac_update64
-from test_tc_gpu import dev, f64_forward, f64_unpack, f64_update, net_layers
+from gpu_util import city_and_params, dev, n_sm  # noqa: F401  (module fixture)
+from qnet_restatement import f64_forward, f64_unpack, f64_update, net_layers
+from sac_restatement import HP, check_step, near_decision, read_state, sac_update64
+from shapes import SHAPES, SHIPPED, expected_route
 from uavrl_b200 import _lib, engine
 
 pytestmark = pytest.mark.gpu
@@ -30,11 +30,6 @@ LR, GAMMA = 5e-4, 0.99
 @pytest.fixture(scope="module")
 def world(env_golden, env27_golden):
     return city_and_params(env_golden, env27_golden)[:2]
-
-
-@pytest.fixture(scope="module")
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def make_env(world, N, seed=8):
@@ -285,7 +280,7 @@ def run_qnet_loop(world, shape, algo, tc, B, N, U, n_iters, cap_frames, G=1, eps
                 s, a, r, s2, d = batch
                 d = d.astype(np.float32)
                 P64 = f64_unpack(layers, OL.local)
-                l64, g64 = f64_update(layers, algo, dueling, OL.local, OL.target, s, a, r, s2, d, GAMMA)
+                l64, g64 = f64_update(layers, algo, dueling, OL.local, OL.target, s, a, r, s2, d, gamma=GAMMA)[:2]
                 kmask, krows = trunk_exempt(layers, n_trunk, P64, dueling, s)
                 lal, gal, trows = tie_allowance(layers, algo, dueling, OL.local, OL.target, (s, a, r, s2, d), L.P)
                 tally.rows += B; tally.kink_rows += krows; tally.tie_rows += trows
@@ -318,9 +313,7 @@ def run_qnet_loop(world, shape, algo, tc, B, N, U, n_iters, cap_frames, G=1, eps
     return dict(skipped=skipped, hard=hard_seen, wrapped=wrapped)
 
 
-SHIPPED = {"dqn": ((100, [64, 64], 27, False), engine.ALGO_DQN),
-           "ddqn": ((100, [64, 64], 27, False), engine.ALGO_DDQN),
-           "dueling": ((100, [64], 27, True), engine.ALGO_DUELING)}
+NETS = {"dqn": (SHIPPED[0], engine.ALGO_DQN), "ddqn": (SHIPPED[0], engine.ALGO_DDQN), "dueling": (SHIPPED[2], engine.ALGO_DUELING)}
 
 # (net, tensor cores, B, N, updates per iteration, fused TD): 32-row training tiles (B = 64) with the TD pass fused, 64-row
 # tiles (B = 4 500 > 32 x 132) fused, and separate TD passes
@@ -342,7 +335,7 @@ def test_qnet_loop_updates_vs_float64(world, leg, n_sm):
     """The shipped networks in the loop: warm-up iterations (count <= B) advance only the epoch, every update equals float64 /
     the oracle on the restated rows, hard target updates land on every third epoch, and the ring wraps."""
     name, tc, B, N, U, fuse = LOOP_LEGS[leg]
-    shape, algo = SHIPPED[name]
+    shape, algo = NETS[name]
     try:
         _lib.lib().uavrl_set_fuse_td(fuse)
         n_iters = 9 if B <= 64 else 7
@@ -352,7 +345,7 @@ def test_qnet_loop_updates_vs_float64(world, leg, n_sm):
     assert out["skipped"] >= 1 and out["hard"] >= 1 and out["wrapped"]
 
 
-ROUTE_SHAPES = {                       # one shape of each route of test_qnet_shapes_gpu.SHAPES with in_dim 100 (the UAV observation)
+ROUTE_SHAPES = {                       # one shape of each route of shapes.SHAPES with in_dim 100 (the UAV observation)
     "generic": next(s for s in SHAPES if s[0] == 100 and s[4][:2] == ("generic", "generic")),
     "tc_td_fp32_update": next(s for s in SHAPES if s[0] == 100 and s[4][0] is not None and s[4][1] is None),
     "fp32": next(s for s in SHAPES if s[0] == 100 and s[4][0] is None),
@@ -383,7 +376,7 @@ def test_loop_call_matches_twin_replay(world, pdl, fuse_td):
     twin's chain stays within the oracle's bounds at every step.  The ring (24 frames) does not wrap, so every transition the
     loop sampled is still readable afterwards."""
     N, B, seed, n_iters, eps = 256, 384, 5, 20, 0.2
-    shape, algo = SHIPPED["ddqn"]
+    shape, algo = NETS["ddqn"]
     try:
         _lib.lib().uavrl_set_pdl(pdl)
         _lib.lib().uavrl_set_fuse_td(fuse_td)
@@ -422,7 +415,7 @@ def test_loop_call_matches_twin_replay(world, pdl, fuse_td):
             OL = O.OracleLearner(net, algo, X.get_params(0), gamma=GAMMA, lr=LR, update_loop=3)
             OL.target[:] = X.get_params(1); OL.m[:] = X.get_params(2); OL.v[:] = X.get_params(3); OL.t.value = X.counters()[1]
             OL.epoch = epoch - 1
-            l64, g64 = f64_update(layers, algo, False, X.get_params(0), X.get_params(1), s, a, r, s2, d.astype(np.float32), GAMMA)
+            l64, g64 = f64_update(layers, algo, False, X.get_params(0), X.get_params(1), s, a, r, s2, d.astype(np.float32), gamma=GAMMA)[:2]
             lal, gal, _ = tie_allowance(layers, algo, False, X.get_params(0), X.get_params(1), (s, a, r, s2, d.astype(np.float32)), X.P)
             kmask, _ = trunk_exempt(layers, 2, f64_unpack(layers, X.get_params(0)), False, s)
             xl = explicit_update(X, batch, 1)
@@ -507,7 +500,7 @@ def test_benchmark_scale_updates(world):
     bit for bit to update_batch on the restated rows and within 2e-5 of the float64 loss."""
     N = B = 8192
     seed = 1
-    shape, algo = SHIPPED["ddqn"]
+    shape, algo = NETS["ddqn"]
     env = make_env(world, N)
     L = engine.Learner(*shape, algo, lr=LR, gamma=GAMMA, batch_size=B, update_loop=3, replay_capacity=1 << 20, lockstep_envs=N, seed=seed)
     L.init_params(0)
@@ -527,7 +520,7 @@ def test_benchmark_scale_updates(world):
         epoch, idx, _ = u
         assert L.counters()[0] == epoch
         batch = L.gather(ring.logical(idx[0]))
-        l64, _ = f64_update(layers, algo, False, X.get_params(0), X.get_params(1), *batch[:4], batch[4].astype(np.float32), GAMMA)
+        l64 = f64_update(layers, algo, False, X.get_params(0), X.get_params(1), *batch[:4], batch[4].astype(np.float32), gamma=GAMMA)[0]
         lal, _, _ = tie_allowance(layers, algo, False, X.get_params(0), X.get_params(1), batch[:4] + (batch[4].astype(np.float32),), X.P)
         xl = explicit_update(X, batch, 1)
         torch.cuda.synchronize()

@@ -9,14 +9,9 @@ import torch
 
 import oracle as O
 from conftest import GOLDEN
-from gpu_util import city_and_params
+from gpu_util import city_and_params, dev
 
 pytestmark = pytest.mark.gpu
-
-
-def dev(x, dt=None):
-    t = torch.as_tensor(np.ascontiguousarray(x)).cuda()
-    return t if dt is None else t.to(dt)
 
 
 def load(S, g):

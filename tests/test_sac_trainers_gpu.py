@@ -8,65 +8,17 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_util import city_and_params, env_plugin
-from test_fl_ac_cpu import GOLDEN as FL_AC_GOLDEN, federate_actors
+from conftest import GOLDEN
+from fl_restatement import federate_actors
+from gpu_util import (DEV, CountTransfers, assert_sac_trainers_equal, assert_same, city_and_params, dev, distinct_alphas, env_dict,
+                      env_plugin, make_env, sac, sac_standalone_like)
 from uavrl_b200 import _lib, engine
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
 G = 4
 OBS, A = 100, 2
-HP = dict(actor_lr=1e-4, critic_lr=1e-3, alpha_lr=1e-4, target_entropy=1.0, gamma=0.99, tau=0.05)
-ROLES = 14                       # 0-4 networks, 5-10 Adam moments, 11-13 last gradients
-
-
-def sac(trainers=1, seed=7, **kw):
-    kw.setdefault("batch_size", 64)
-    return engine.SacLearner(seed=seed, trainers=trainers, **HP, **kw)
-
-
-def dev(x):
-    return torch.as_tensor(np.ascontiguousarray(x)).to(DEV)
-
-
-def assert_same(a, b, what):
-    a, b = np.asarray(a), np.asarray(b)
-    assert a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8)), what
-
-
-def distinct_alphas(S, rng):
-    """Every trainer gets its own (log_alpha, exp_avg, exp_avg_sq): a trainer reading another's alpha shows."""
-    al = np.stack([[np.log(0.01) + 0.3 * g, 1e-3 * (g + 1), 1e-6 * (g + 2)] for g in range(S.G)]).astype(np.float32)
-    al += rng.normal(0, 1e-4, al.shape).astype(np.float32) * np.array([1, 0, 0], np.float32)
-    S.set_alpha(al)
-    return al
-
-
-def standalone_like(grouped, g, seed=7, **kw):
-    """Trainer g of `grouped` as a stand-alone learner: its parameters, Adam moments, alpha triple and counters, seed + g."""
-    s = sac(1, seed + g, **kw)
-    for role in range(11):
-        s.set_params(role, grouped.get_params(role)[g])
-    sc = grouped.scalars()
-    s.set_scalars(*grouped.alpha()[g], sc["epoch"], sc["adam_step"])
-    return s
-
-
-def assert_trainers_equal(S, solo, losses=None, solo_losses=None):
-    for role in range(ROLES):
-        allp = S.get_params(role).reshape(S.G, -1)
-        for g, X in enumerate(solo):
-            assert_same(allp[g], X.get_params(role), "role %d of trainer %d" % (role, g))
-    al = S.alpha()
-    for g, X in enumerate(solo):
-        assert_same(al[g], X.alpha()[0], "alpha triple of trainer %d" % g)
-        sg, sx = S.scalars(), X.scalars()
-        assert (sg["epoch"], sg["adam_step"]) == (sx["epoch"], sx["adam_step"])
-    if losses is not None:
-        for g in range(len(solo)):
-            assert_same(losses[4 * g:4 * g + 4], solo_losses[g], "losses of trainer %d" % g)
+SAC_XML = ("Trainer_SAC_B200.xml", "UAV_continuous_B200.xml")     # the plug-in tests' trainer and agent: continuous step
 
 
 def states(rng, n):
@@ -85,7 +37,7 @@ def test_act_blocks_equal_standalone():
     S = sac(G)
     S.init_params(3)
     assert S.get_params(0).shape == (G, S.P[0]) and S.trainer_count() == G
-    solo = [standalone_like(S, g) for g in range(G)]
+    solo = [sac_standalone_like(S, g) for g in range(G)]
     obs = dev(states(rng, G * Ng))
     eps = dev(rng.normal(size=(G * Ng, A)).astype(np.float32))
     a_inj = S.act(obs, eps).cpu().numpy()                  # call 0 of every learner
@@ -108,7 +60,7 @@ def test_explicit_update_equals_standalone(B, ctas, monkeypatch):
     S = sac(G)
     S.init_params(5)
     distinct_alphas(S, rng)
-    solo = [standalone_like(S, g) for g in range(G)]
+    solo = [sac_standalone_like(S, g) for g in range(G)]
     for step in range(4):
         s, a, r, s2, d = (dev(x) for x in batch(rng, G * B))
         injected = step % 2 == 1                              # Philox noise on steps 0 and 2, injected noise on 1 and 3
@@ -123,18 +75,11 @@ def test_explicit_update_equals_standalone(B, ctas, monkeypatch):
             l1 = torch.zeros(4, device=DEV)
             X.update_batch(part(s), part(a), part(r), part(s2), part(d), part(e1), part(e2), l1)
             solo_losses.append(l1.cpu().numpy())
-        assert_trainers_equal(S, solo, losses.cpu().numpy(), solo_losses)
+        assert_sac_trainers_equal(S, solo, losses.cpu().numpy(), solo_losses)
     assert S.scalars()["epoch"] == 4 and S.scalars()["adam_step"] == 4
 
 
 # ------------------------------------------------------------------ the lockstep ring
-def make_env(env_golden, env27_golden, n, pool):
-    city, params, _, _ = city_and_params(env_golden, env27_golden)
-    env = engine.EnvBatch(city, params, n, max_subgoals=64, auto_reset=False)
-    env.set_pool(pool["start"], pool["goal"], pool["heading"], pool["sub"], pool["n_sub"])
-    return env
-
-
 def grouped_and_pairs(env_golden, env27_golden, Ng, cap_g, seed, pool_seed):
     """A grouped learner on N = G Ng envs and, for every trainer, a stand-alone learner (seed + g, cap_g, Ng envs) on an env
     that starts from the same scenarios as the trainer's block."""
@@ -150,7 +95,7 @@ def grouped_and_pairs(env_golden, env27_golden, Ng, cap_g, seed, pool_seed):
     for g in range(G):
         e1 = make_env(env_golden, env27_golden, Ng, pool)
         e1.reset(g * Ng)
-        pairs.append((e1, standalone_like(S, g, seed=seed, replay_capacity=cap_g, lockstep_envs=Ng)))
+        pairs.append((e1, sac_standalone_like(S, g, seed=seed, replay_capacity=cap_g, lockstep_envs=Ng)))
     return env, S, pairs
 
 
@@ -172,7 +117,7 @@ def test_ring_sampled_updates_equal_standalone(env_golden, env27_golden):
             l1 = torch.zeros(4, device=DEV)
             X.update_replay(dev(tape[g]) if mode == "tape" else None, losses=l1)
             solo_losses.append(l1.cpu().numpy())
-        assert_trainers_equal(S, [X for _, X in pairs], losses.cpu().numpy(), solo_losses)
+        assert_sac_trainers_equal(S, [X for _, X in pairs], losses.cpu().numpy(), solo_losses)
     # the tape rows are the trainer's transitions: whole-ring index (k / Ng) N + g Ng + k % Ng
     k = tape[1].astype(np.int64)
     for x, y in zip(S.gather((k // Ng) * G * Ng + Ng + k % Ng), pairs[1][1].gather(k)):
@@ -190,7 +135,7 @@ def test_lockstep_loop_equals_standalone_pairs(env_golden, env27_golden):
         s1 = engine.sac_train_run(e1, X, iters)
         assert s1.updates == st.updates
         losses.append(np.float32(s1.last_loss))
-    assert_trainers_equal(S, [X for _, X in pairs])
+    assert_sac_trainers_equal(S, [X for _, X in pairs])
     assert np.float32(st.last_loss) == np.float32(sum(float(x) for x in losses) / G)
     sg = env.get_state()
     n_g = S.replay_size() // G
@@ -212,7 +157,7 @@ def test_lockstep_loop_equals_standalone_pairs(env_golden, env27_golden):
         l1 = torch.zeros(4, device=DEV)
         X.update_replay(losses=l1)
         solo_losses.append(l1.cpu().numpy())
-    assert_trainers_equal(S, [X for _, X in pairs], out.cpu().numpy(), solo_losses)
+    assert_sac_trainers_equal(S, [X for _, X in pairs], out.cpu().numpy(), solo_losses)
 
 
 # ------------------------------------------------------------------ entry points, refusals, round trips
@@ -265,13 +210,13 @@ def test_refusals_round_trips_and_one_trainer():
     s, a, r, s2, d = (dev(v) for v in batch(rng, 256))
     for L in (L0, L1):
         L.update_batch(s, a, r, s2, d)
-    assert_trainers_equal(L1, [L0])
+    assert_sac_trainers_equal(L1, [L0])
     assert_same(L0.act(s).cpu().numpy(), L1.act(s).cpu().numpy(), "actions")
 
 
 # ------------------------------------------------------------------ Federated_Learning_AC
 def test_federate_matches_reference_golden():
-    g = np.load(FL_AC_GOLDEN)
+    g = np.load(os.path.join(GOLDEN, "fl_ac_golden.npz"))
     n = int(g["G"])
     S = sac(n)
     assert S.P[0] == g["actor0"].shape[1]
@@ -326,41 +271,12 @@ def test_federate_one_trainer_keeps_actor():
 
 
 # ------------------------------------------------------------------ plug-ins
-class CountTransfers:
-    """Counts a learner's get_params / set_params calls: each moves one role's whole [G][P] vector between host and device."""
-
-    def __init__(self, L):
-        self.get = self.set = 0
-        get, set_ = L.get_params, L.set_params
-
-        def g(*a, **k):
-            self.get += 1
-            return get(*a, **k)
-
-        def s(*a, **k):
-            self.set += 1
-            return set_(*a, **k)
-        L.get_params, L.set_params = g, s
-
-
-def env_dict(**kw):
-    """The shipped env configuration with num_UAV = num_trainers = 8, the continuous step and the SAC trainer."""
-    from uavrl_b200.plugins import xmlconfig
-    ed = xmlconfig.XML2Dict(os.path.join(ROOT, "configs", "PathPlan_City_B200.xml"))["simulator"]["env"]
-    ed["num_UAV"], ed["scenario_pool"], ed["num_trainers"] = "8", "64", "8"
-    ed["Obstacles"]["buildings"] = os.path.join(ROOT, "configs", "buildings.xml")
-    ed["Agent"]["xml_path_agent"] = os.path.join(ROOT, "configs", "UAV_continuous_B200.xml")
-    ed["Agent"]["Trainer"]["Trainer_path"] = os.path.join(ROOT, "configs", "Trainer_SAC_B200.xml")
-    ed.update(kw)
-    return ed
-
-
 def test_env_plugin_one_sac_trainer_per_uav(tmp_path):
     """num_UAV = num_trainers = 8 with the shipped SAC trainer and the continuous step: run_eposide runs, save() writes the
     reference's three files per UAV, Load_Mod in a fresh env restores every trainer bit for bit, each moving every role's
     vector between host and device once whatever G is; Is_FL = Is_AC = FL_Loop = 1 leaves every actor equal to the sum."""
     with env_plugin(tmp_path) as mod:
-        env = mod.PathPlan_City_B200(env_dict())
+        env = mod.PathPlan_City_B200(env_dict(*SAC_XML))
         tr = env.Trainer
         assert tr._learner.trainer_count() == 8 and tr.names == ["UAV_%d" % i for i in range(8)]
         with pytest.raises(ValueError, match="batch"):
@@ -371,12 +287,12 @@ def test_env_plugin_one_sac_trainer_per_uav(tmp_path):
         n = CountTransfers(tr._learner)
         tr.save()
         assert (n.get, n.set) == (9, 0)
-        env2 = mod.PathPlan_City_B200(env_dict())                   # Load_Mod in the constructor
+        env2 = mod.PathPlan_City_B200(env_dict(*SAC_XML))                     # Load_Mod in the constructor
         n = CountTransfers(env2.Trainer._learner)
         env2.Trainer.Load_Mod()
         assert (n.get, n.set) == (9, 11)
         # federated aggregation of the actors after every episode
-        env3 = mod.PathPlan_City_B200(env_dict(Is_FL="1", Is_AC="1", FL_Loop="1"))
+        env3 = mod.PathPlan_City_B200(env_dict(*SAC_XML, Is_FL="1", Is_AC="1", FL_Loop="1"))
         L3 = env3.Trainer._learner
         seen = []
         fed = L3.federate_actors
@@ -406,7 +322,7 @@ def test_env_plugin_skips_malformed_checkpoint(tmp_path, capsys):
     the error and carries on: trainer 3 keeps its fresh networks, targets and moments, every other trainer is restored bit
     for bit with its targets copying its critics."""
     with env_plugin(tmp_path) as mod:
-        tr = mod.PathPlan_City_B200(env_dict()).Trainer                  # no files yet: fresh parameters
+        tr = mod.PathPlan_City_B200(env_dict(*SAC_XML)).Trainer                  # no files yet: fresh parameters
         L = tr._learner
         fresh = {r: L.get_params(r) for r in range(11)}
         rng = np.random.default_rng(5)
@@ -420,7 +336,7 @@ def test_env_plugin_skips_malformed_checkpoint(tmp_path, capsys):
         ck["model"] = {("fc3.weight" if k == "fc_out.weight" else k): t for k, t in ck["model"].items()}
         torch.save(ck, p)
         capsys.readouterr()
-        L2 = mod.PathPlan_City_B200(env_dict()).Trainer._learner         # Load_Mod in the constructor
+        L2 = mod.PathPlan_City_B200(env_dict(*SAC_XML)).Trainer._learner         # Load_Mod in the constructor
         out = capsys.readouterr().out
     assert "critic_1_SAC_UAV_3.pth holds" in out and "fc3.weight" in out, out
     for r in range(11):

@@ -1,30 +1,23 @@
 """Grouped SAC trainers (uavrl_sac_create_trainers) at every shape of the SAC shape sweep, away from the shipped G = 4.  The
 four SAC tile kernels launch a separate instance for one trainer, with the trainer offset compiled out, so the shape sweep
-never runs the grouped instances; here G = 3 runs them at every row of test_sac_shapes_gpu.SHAPES.  Trainer g must equal,
+never runs the grouped instances; here G = 3 runs them at every row of shapes.SAC_SHAPES.  Trainer g must equal,
 bit for bit, a stand-alone SacLearner with its parameters, moments and alpha triple, seed + g, replay_capacity / G and
 Ng = lockstep_envs / G envs, and the last trainer (the largest offsets) is held to the float64 update of
-test_sac_shapes_gpu with that sweep's bounds.  The ring loop runs at one env per trainer and at G = 4096, and the actor
+sac_restatement with the SAC sweep's bounds.  The ring loop runs at one env per trainer and at G = 4096, and the actor
 aggregation at every shape."""
 import numpy as np
 import pytest
 import torch
 
-from test_fl_ac_cpu import federate_actors
-from test_sac_shapes_gpu import SHAPES, A, actor_fwd, check_step, clean_batch, draw_batch, init_state, read_state, sac_update64
-from test_sac_shapes_gpu import shape_id, unpack
-from test_sac_trainers_gpu import assert_same, distinct_alphas, sac, standalone_like
-from test_trainers_shapes_gpu import ring_env, short_episode_env
+from fl_restatement import federate_actors
+from gpu_util import DEV, SAC_ROLES, assert_same, dev, distinct_alphas, ring_env, sac, sac_standalone_like, short_episode_env
+from sac_restatement import A, actor_fwd, check_step, clean_batch, draw_batch, init_state, read_state, sac_update64, unpack
+from shapes import SAC_SHAPES, sac_shape_id
 from uavrl_b200 import engine
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 G = 3
 KEYS = ("actor", "c1", "c2", "t1", "t2", "actor_m", "c1_m", "c2_m", "actor_v", "c1_v", "c2_v")
-ROLES = 14                       # 0-4 networks, 5-10 Adam moments, 11-13 last gradients
-
-
-def dev(x):
-    return torch.as_tensor(np.ascontiguousarray(x)).to(DEV)
 
 
 class Trainer:
@@ -54,12 +47,12 @@ def grouped(shape, rng, **kw):
     for role, k in enumerate(KEYS):
         S.set_params(role, np.stack([st[k] for st in states]))
     distinct_alphas(S, rng)
-    return S, [standalone_like(S, g, **net, **kw) for g in range(G)], states
+    return S, [sac_standalone_like(S, g, **net, **kw) for g in range(G)], states
 
 
 def assert_trainer_equal(S, g, X, roles=None):
-    roles = roles if roles is not None else [S.get_params(r) for r in range(ROLES)]
-    for role in range(ROLES):
+    roles = roles if roles is not None else [S.get_params(r) for r in range(SAC_ROLES)]
+    for role in range(SAC_ROLES):
         assert_same(roles[role][g], X.get_params(role), "role %d of trainer %d" % (role, g))
     assert_same(S.alpha()[g], X.alpha()[0], "alpha triple of trainer %d" % g)
     sg, sx = S.scalars(), X.scalars()
@@ -67,7 +60,7 @@ def assert_trainer_equal(S, g, X, roles=None):
 
 
 # ------------------------------------------------------------------ act
-@pytest.mark.parametrize("shape", SHAPES, ids=shape_id)
+@pytest.mark.parametrize("shape", SAC_SHAPES, ids=sac_shape_id)
 def test_act_equals_standalone_and_float64(shape):
     """n = 1, 33 and 1000 rows per trainer, injected noise and Philox draws: every trainer bit for bit as its stand-alone
     learner; the last trainer's actions (injected noise) within test_sac_shapes_gpu.test_act_vs_float64's bound of float64,
@@ -108,10 +101,10 @@ LEGS = {"B1": (1, 0), "B64": (64, 0), "B200": (200, 0), "B200-3ctas": (200, 3)} 
 
 
 @pytest.mark.parametrize("leg", list(LEGS))
-@pytest.mark.parametrize("shape", SHAPES, ids=shape_id)
+@pytest.mark.parametrize("shape", SAC_SHAPES, ids=sac_shape_id)
 def test_update_equals_standalone_and_float64(shape, leg, monkeypatch):
     """4 updates: every trainer bit for bit as its stand-alone learner after each (the fourth draws its noise with Philox);
-    the last trainer's first three against the float64 update (test_sac_shapes_gpu.check_step), its batch drawn clear of
+    the last trainer's first three against the float64 update (sac_restatement.check_step), its batch drawn clear of
     the float64 update's decision points."""
     obs, hid, bound, _ = shape
     B, ctas = LEGS[leg]
@@ -136,7 +129,7 @@ def test_update_equals_standalone_and_float64(shape, leg, monkeypatch):
             l1 = torch.zeros(4, device=DEV)
             X.update_batch(part(s), part(a), part(r), part(s2), part(d), part(e1), part(e2), l1)
             assert_same(got[4 * g:4 * g + 4], l1.cpu().numpy(), "losses of trainer %d, step %d" % (g, step))
-        roles = [S.get_params(r) for r in range(ROLES)]
+        roles = [S.get_params(r) for r in range(SAC_ROLES)]
         for g, X in enumerate(solo):
             assert_trainer_equal(S, g, X, roles)
         if not philox:
@@ -166,14 +159,14 @@ def sac_loop_pairs(env_golden, env27_golden, shape, G_, Ng, iters, frames, batch
     S.init_params(1)
     distinct_alphas(S, np.random.default_rng(seed))
     pairs = {g: (ring_env(city, params, Ng, pool, g * Ng),
-                 standalone_like(S, g, seed=seed, replay_capacity=frames * Ng, lockstep_envs=Ng, **net)) for g in trainers}
+                 sac_standalone_like(S, g, seed=seed, replay_capacity=frames * Ng, lockstep_envs=Ng, **net)) for g in trainers}
     st = engine.sac_train_run(env, S, iters)
     assert st.updates > 0 and st.env_steps == iters * N
     stats = {g: engine.sac_train_run(e1, X, iters) for g, (e1, X) in pairs.items()}
     assert all(s1.updates == st.updates for s1 in stats.values())
     if len(pairs) == G_:
         assert np.float32(st.last_loss) == np.float32(sum(float(np.float32(s1.last_loss)) for s1 in stats.values()) / G_)
-    roles = [S.get_params(r) for r in range(ROLES)]
+    roles = [S.get_params(r) for r in range(SAC_ROLES)]
     sg = env.get_state()
     n_g = S.replay_size() // G_
     for g, (e1, X) in pairs.items():
@@ -202,10 +195,10 @@ def sac_loop_pairs(env_golden, env27_golden, shape, G_, Ng, iters, frames, batch
     return st, n_g
 
 
-RING_LEGS = [(sh, Ng) for sh in SHAPES if sh[0] == 100 for Ng in (1, 37)]
+RING_LEGS = [(sh, Ng) for sh in SAC_SHAPES if sh[0] == 100 for Ng in (1, 37)]
 
 
-@pytest.mark.parametrize("shape,Ng", RING_LEGS, ids=["%s-Ng%d" % (shape_id(sh), Ng) for sh, Ng in RING_LEGS])
+@pytest.mark.parametrize("shape,Ng", RING_LEGS, ids=["%s-Ng%d" % (sac_shape_id(sh), Ng) for sh, Ng in RING_LEGS])
 def test_lockstep_loop_equals_standalone_pairs(env_golden, env27_golden, shape, Ng):
     """G = 3 at the obs-100 shapes, 40 iterations through a 24-frame ring (it wraps) with episodes ending."""
     st, n_g = sac_loop_pairs(env_golden, env27_golden, shape, G, Ng, 40, 24, 16, range(G))
@@ -217,12 +210,12 @@ def test_lockstep_loop_g4096_one_env_per_trainer(env_golden, env27_golden):
     2047, 4094, 4095 and three drawn at random against stand-alone pairs."""
     Gb = 4096
     pick = sorted({0, 1, 2047, 4094, 4095} | set(np.random.default_rng(3).choice(Gb, 3, replace=False).tolist()))
-    st, n_g = sac_loop_pairs(env_golden, env27_golden, SHAPES[0], Gb, 1, 72, 80, 64, pick, pool_n=Gb - 1)
+    st, n_g = sac_loop_pairs(env_golden, env27_golden, SAC_SHAPES[0], Gb, 1, 72, 80, 64, pick, pool_n=Gb - 1)
     assert st.updates == 72 - 64 and n_g == 72
 
 
 # ------------------------------------------------------------------ Federated_Learning_AC
-@pytest.mark.parametrize("shape", SHAPES, ids=shape_id)
+@pytest.mark.parametrize("shape", SAC_SHAPES, ids=sac_shape_id)
 def test_federate_actors_every_shape(shape):
     """Every actor becomes the float32 left-to-right sum of the G actors (full mantissas, so the order shows), nothing else
     changes, and the next act pass (Philox noise) equals stand-alone learners loaded with the summed actor: the actor

@@ -6,13 +6,10 @@ import pytest
 import torch
 
 import oracle as O
+from gpu_util import dev
+from qnet_restatement import big_inputs, f64_update, net_layers
 
 pytestmark = pytest.mark.gpu
-
-
-def dev(x, dt=None):
-    t = torch.as_tensor(np.ascontiguousarray(x)).cuda()
-    return t if dt is None else t.to(dt)
 
 
 @pytest.mark.parametrize("hidden,dueling", [([64, 64], 0), ([64], 1), ([64], 0), ([128, 64], 1)])
@@ -83,15 +80,6 @@ def test_tc_td_targets_keep_update_parity(dqn_golden, name):
 # ---------------------------------------------------------------------------------------------------------------------
 # The tile variants the large BASELINE configs select (launch_tc_forward: R = 64 rows per tile from n >= 64 x 132,
 # R = 128 from n >= 128 x 132 when 128-row tiles fit shared memory; tc_train: R = 64 from B >= 32 x 132) compared with the oracle by VALUE, ragged last tiles.
-def big_inputs(g, n, rng, in_dim=100):
-    """n rows of the golden observations (columns cropped or tiled to in_dim) plus noise: occupancy bits and real-valued
-    entries at the scales the learner sees."""
-    base = np.concatenate([g["batch_s"].reshape(-1, 100), g["batch_s2"].reshape(-1, 100)])
-    base = np.tile(base, (1, -(-in_dim // 100)))[:, :in_dim]
-    x = np.tile(base, (n // base.shape[0] + 1, 1))[:n]
-    return (x + rng.normal(0, 0.02, x.shape)).astype(np.float32)
-
-
 @pytest.mark.parametrize("n", [12000, 20011])
 @pytest.mark.parametrize("hidden,dueling", [([64, 64], 0), ([64], 1)])
 def test_tc_act_large_tiles_vs_oracle(dqn_golden, n, hidden, dueling):
@@ -112,74 +100,6 @@ def test_tc_act_large_tiles_vs_oracle(dqn_golden, n, hidden, dueling):
     assert clear.mean() > 0.99
     assert np.array_equal(a_tc.cpu().numpy()[clear], a_or[clear])
     L.close()
-
-
-def net_layers(in_dim, hidden, n_actions, dueling):
-    """(out, in) of every Linear in state_dict order: the trunk, then fc_A (or the Q head) and fc_V."""
-    dims = [in_dim] + list(hidden)
-    head = [(n_actions, hidden[-1]), (1, hidden[-1])] if dueling else [(n_actions, hidden[-1])]
-    return [(dims[i + 1], dims[i]) for i in range(len(hidden))] + head
-
-
-def f64_unpack(layers, flat):
-    out, off = [], 0
-    for (o, i) in layers:
-        W = flat[off:off + o * i].reshape(o, i).astype(np.float64); off += o * i
-        b = flat[off:off + o].astype(np.float64); off += o
-        out.append((W, b))
-    assert off == flat.size
-    return out
-
-
-def f64_forward(P, dueling, x):
-    """Q(x) of the unpacked float64 network P, and the activations [x, H1, ..] kept for the backward pass."""
-    x = np.asarray(x, np.float64)
-    acts, h = [x], x
-    nt = len(P) - (2 if dueling else 1)
-    for W, b in P[:nt]:
-        h = np.maximum(h @ W.T + b, 0.0); acts.append(h)
-    if dueling:
-        (WA, bA), (WV, bV) = P[nt], P[nt + 1]
-        A = h @ WA.T + bA; V = h @ WV.T + bV
-        return V + A - A.mean(1, keepdims=True), acts
-    W, b = P[nt]
-    return h @ W.T + b, acts
-
-
-def f64_update(layers, algo, dueling, local, target, s, a, r, s2, d, gamma=0.99):
-    """The TD update's loss and gradient in float64 numpy (the arbiter between two fp32 implementations whose summation
-    orders differ): DQN_Trainer.py:107-124 / DDQN_Trainer.py:93-107 / DuelingDQN_Trainer.py:164-180."""
-    def fwd(P, x):
-        return f64_forward(P, dueling, x)
-    PL, PT = f64_unpack(layers, local), f64_unpack(layers, target)
-    s, s2 = s.astype(np.float64), s2.astype(np.float64)
-    B = s.shape[0]
-    qt, _ = fwd(PT, s2)
-    if algo == 0:
-        nq = qt.max(1)
-    else:
-        nq = qt[np.arange(B), fwd(PL, s2)[0].argmax(1)]
-    y = r.astype(np.float64) + gamma * nq * (1.0 - d.astype(np.float64))
-    q, acts = fwd(PL, s)
-    diff = q[np.arange(B), a] - y
-    loss = float((diff ** 2).mean())
-    gq = np.zeros_like(q); gq[np.arange(B), a] = 2.0 * diff / B
-    grads = []
-    nt = len(PL) - (2 if dueling else 1)
-    h = acts[-1]
-    if dueling:
-        gA = gq - gq.sum(1, keepdims=True) / q.shape[1]; gV = gq.sum(1, keepdims=True)
-        gh = gA @ PL[nt][0] + gV @ PL[nt + 1][0]
-        head = [gA.T @ h, gA.sum(0), gV.T @ h, gV.sum(0)]
-    else:
-        gh = gq @ PL[nt][0]
-        head = [gq.T @ h, gq.sum(0)]
-    trunk = []
-    for l in range(nt - 1, -1, -1):
-        gz = gh * (acts[l + 1] > 0)
-        trunk = [gz.T @ acts[l], gz.sum(0)] + trunk
-        gh = gz @ PL[l][0]
-    return loss, np.concatenate([g.ravel() for g in trunk + head])
 
 
 @pytest.mark.parametrize("B", [12000, 20011])
@@ -216,7 +136,7 @@ def test_tc_update_large_batch_vs_oracle(dqn_golden, name, B):
             # q_target gap on that sample.  Such samples are marked terminal (the next-state value is multiplied by 0).
             ql = np.sort(O.net_forward(net, L.get_params(0), s2).astype(np.float64), 1)
             d[(ql[:, -1] - ql[:, -2]) < 1e-3] = 1.0
-        l64, g64 = f64_update(layers, algo, dueling, L.get_params(0), L.get_params(1), s, a, r, s2, d)
+        l64, g64 = f64_update(layers, algo, dueling, L.get_params(0), L.get_params(1), s, a, r, s2, d)[:2]
         L.update_batch(dev(s), dev(a), dev(r), dev(s2), dev(d), loss)
         lo, grads = OL.update(s, a, r, s2, d)
         torch.cuda.synchronize()

@@ -7,46 +7,19 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_util import city_and_params, env_plugin
-from test_qnet_shapes_gpu import SHAPES, SHIPPED
-from test_tc_gpu import big_inputs
+from gpu_util import (DEV, CountTransfers, assert_same, assert_trainers_equal, city_and_params, env_dict, env_plugin, learner,
+                      make_env, standalone_like)
+from qnet_restatement import big_inputs
+from shapes import SHAPES, SHIPPED, net_id
 from uavrl_b200 import _lib, engine
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
 G = 4
-
-
-def learner(shape, trainers=1, seed=7, **kw):
-    in_dim, hidden, n_actions, dueling = shape[:4]
-    kw.setdefault("algo", engine.ALGO_DQN)
-    kw.setdefault("batch_size", 64)
-    return engine.Learner(in_dim, hidden, n_actions, dueling, seed=seed, trainers=trainers, **kw)
-
-
-def standalone_like(grouped, shape, g, seed=7, **kw):
-    """Trainer g of `grouped` as a stand-alone learner: its parameters and optimiser state, seed + g."""
-    s = learner(shape, 1, seed + g, **kw)
-    for which in range(4):
-        s.set_params(grouped.get_params(which)[g], which)
-    return s
-
-
-def assert_same(a, b, what):
-    a, b = np.asarray(a), np.asarray(b)
-    assert a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8)), what
-
-
-def shape_id(s):
-    return "%d-%s-%d-%s" % (s[0], "x".join(map(str, s[1])), s[2], "duel" if s[3] else "q")
-
-
 ACT_SHAPES = SHIPPED + [SHAPES[0][:4]]         # the four shipped networks and one generic-route shape
 
 
-@pytest.mark.parametrize("shape", ACT_SHAPES, ids=shape_id)
+@pytest.mark.parametrize("shape", ACT_SHAPES, ids=net_id)
 def test_act_blocks_equal_standalone(dqn_golden, shape):
     Ng = 1000                                          # ragged last tile of every tile size
     rng = np.random.default_rng(1)
@@ -80,18 +53,6 @@ def batch(dqn_golden, rng, n, shape):
     return s, a, r, s2, d
 
 
-def assert_trainers_equal(Lg, solo, losses=None, solo_losses=None):
-    for which, what in enumerate(("local", "target", "exp_avg", "exp_avg_sq", "grad")):
-        allp = Lg.get_params(which).reshape(-1, Lg.P)
-        for g, S in enumerate(solo):
-            assert_same(allp[g], S.get_params(which), "%s of trainer %d" % (what, g))
-    if losses is not None:
-        for g in range(len(solo)):
-            assert_same(losses[g:g + 1], solo_losses[g], "loss of trainer %d" % g)
-    for S in solo:
-        assert S.counters() == Lg.counters()
-
-
 @pytest.mark.parametrize("tc", [True, False], ids=["tc", "fp32"])
 @pytest.mark.parametrize("B", [64, 6000, 9000])     # 32- / 64-row tiles, TD fused / separate (132 SMs)
 @pytest.mark.parametrize("algo,shape", [(engine.ALGO_DQN, SHIPPED[0]), (engine.ALGO_DDQN, SHIPPED[0]),
@@ -116,13 +77,6 @@ def test_explicit_update_equals_standalone(dqn_golden, algo, shape, B, tc):
             S.update_batch(s[blk].contiguous(), a[blk].contiguous(), r[blk].contiguous(), s2[blk].contiguous(), d[blk].contiguous(), l1)
             solo_loss.append(l1.cpu().numpy())
         assert_trainers_equal(Lg, solo, loss.cpu().numpy(), solo_loss)
-
-
-def make_env(env_golden, env27_golden, n, pool):
-    city, params, _, _ = city_and_params(env_golden, env27_golden)
-    env = engine.EnvBatch(city, params, n, max_subgoals=64, auto_reset=False)
-    env.set_pool(pool["start"], pool["goal"], pool["heading"], pool["sub"], pool["n_sub"])
-    return env
 
 
 def test_index_tape_maps_to_ring_rows(env_golden, env27_golden):
@@ -251,44 +205,16 @@ def test_refusals_and_round_trips(dqn_golden):
     assert_same(L0.act(s, 0.5).cpu().numpy(), L1.act(s, 0.5).cpu().numpy(), "actions")
 
 
-class CountTransfers:
-    """Counts a learner's get_params / set_params calls: each moves the whole [G][P] vector between host and device."""
-
-    def __init__(self, L):
-        self.get = self.set = 0
-        get, set_ = L.get_params, L.set_params
-
-        def g(*a, **k):
-            self.get += 1
-            return get(*a, **k)
-
-        def s(*a, **k):
-            self.set += 1
-            return set_(*a, **k)
-        L.get_params, L.set_params = g, s
-
-
-def env_dict(**kw):
-    """The shipped env configuration with num_UAV = num_trainers = 8 and the DDQN trainer."""
-    from uavrl_b200.plugins import xmlconfig
-    ed = xmlconfig.XML2Dict(os.path.join(ROOT, "configs", "PathPlan_City_B200.xml"))["simulator"]["env"]
-    ed["num_UAV"], ed["scenario_pool"], ed["num_trainers"] = "8", "64", "8"
-    ed["Obstacles"]["buildings"] = os.path.join(ROOT, "configs", "buildings.xml")
-    ed["Agent"]["Trainer"]["Trainer_path"] = os.path.join(ROOT, "configs", "Trainer_DDQN_B200.xml")
-    ed.update(kw)
-    return ed
-
-
 def test_env_plugin_one_trainer_per_uav(tmp_path):
     """num_UAV = num_trainers = 8: the reference's one trainer per UAV.  run_eposide runs, save() writes one q_local / q_target
     pair per trainer in the reference's per-UAV naming, and Load_Mod in a fresh env restores every trainer bit for bit.  Both
     move each of the four vectors between host and device once, whatever the trainer count."""
     with env_plugin(tmp_path) as mod:
-        env = mod.PathPlan_City_B200(env_dict())
+        env = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml"))
         with pytest.raises(ValueError, match="multiple of num_trainers"):
-            mod.PathPlan_City_B200(env_dict(num_trainers="3"))
+            mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml", num_trainers="3"))
         with pytest.raises(ValueError, match="num_trainers = 1"):
-            mod.PathPlan_City_B200(env_dict(host_driven="1"))
+            mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml", host_driven="1"))
         tr = env.Trainer
         assert tr._learner.trainer_count() == 8 and tr.names == ["UAV_%d" % i for i in range(8)]
         info = env.run_eposide(0.3)
@@ -296,7 +222,7 @@ def test_env_plugin_one_trainer_per_uav(tmp_path):
         n = CountTransfers(tr._learner)
         tr.save()
         assert (n.get, n.set) == (4, 0)
-        env2 = mod.PathPlan_City_B200(env_dict())                   # Load_Mod in the constructor
+        env2 = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml"))                   # Load_Mod in the constructor
         n = CountTransfers(env2.Trainer._learner)
         env2.Trainer.Load_Mod(str(tmp_path))
         assert (n.get, n.set) == (4, 4)
@@ -315,7 +241,7 @@ def test_env_plugin_skips_malformed_checkpoints(tmp_path, capsys):
     renamed key.  As in the reference (DuelingDQN_Trainer.py:56-57), the constructor prints each error and carries on: those
     two trainers keep their fresh parameters and moments, every other trainer is restored bit for bit."""
     with env_plugin(tmp_path) as mod:
-        tr = mod.PathPlan_City_B200(env_dict()).Trainer                  # no files yet: fresh parameters
+        tr = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml")).Trainer                  # no files yet: fresh parameters
         fresh = [tr._rows(which) for which in range(4)]
         rng = np.random.default_rng(5)
         saved = [rng.normal(0, 1, f.shape).astype(np.float32) for f in fresh]
@@ -331,7 +257,7 @@ def test_env_plugin_skips_malformed_checkpoints(tmp_path, capsys):
         ck["model"] = {("fc0.bias" if k == "fc1.bias" else k): t for k, t in ck["model"].items()}
         torch.save(ck, pt)
         capsys.readouterr()
-        tr2 = mod.PathPlan_City_B200(env_dict()).Trainer                 # Load_Mod in the constructor
+        tr2 = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml")).Trainer                 # Load_Mod in the constructor
         out = capsys.readouterr().out
     assert "q_local_DDQN_UAV_2.pth: fc1.weight is (64, 99)" in out and "q_target_DDQN_UAV_6.pth holds" in out, out
     for which in range(4):

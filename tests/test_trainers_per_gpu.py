@@ -10,37 +10,21 @@ import pytest
 import torch
 
 import oracle as O
-from gpu_util import city_and_params
-from test_qnet_shapes_gpu import SHIPPED
-from test_trainers_gpu import ROOT, assert_same, assert_trainers_equal, learner, make_env
+from gpu_util import (DEV, PER_MAX, ROOT, assert_same, assert_trainers_equal, assert_trees_equal, city_and_params, env_dict,
+                      learner, make_env, n_sm)  # noqa: F401  (module fixture)
+from shapes import SHIPPED
 from uavrl_b200 import engine
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
-
-
-@pytest.fixture(scope="module")
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 P0 = float(np.float32(0.01) ** np.float32(0.6))        # priority of a transition stored without an error
 
 
-def ring_env(env_golden, env27_golden, n, pool=256):
+def generated_env(env_golden, env27_golden, n, pool=256):
     city, params, _, _ = city_and_params(env_golden, env27_golden)
     env = engine.EnvBatch(city, params, n, max_subgoals=64, auto_reset=True)
     env.generate_pool(pool, seed=2)
     env.reset(0)
     return env
-
-
-def assert_trees_equal(Lg, solo, n_slots):
-    leaves, totals, beta = Lg.per_state(n_slots)
-    assert leaves.shape == (len(solo), n_slots) and totals.shape == (len(solo),)
-    for g, S in enumerate(solo):
-        l1, t1, b1 = S.per_state(n_slots)
-        assert_same(leaves[g], l1, "leaves of trainer %d" % g)
-        assert_same(totals[g:g + 1], np.array([t1]), "total of trainer %d" % g)
-        assert beta == b1
 
 
 CASES = [  # algo, shape, tensor cores, per-trainer batch, loss
@@ -114,7 +98,7 @@ def test_lockstep_loop_with_per_equals_standalone_pairs(env_golden, env27_golden
 
 def filled_learner(env_golden, env27_golden, G, Ng, frames, iters, **kw):
     """A grouped learner with prioritised replay whose ring holds `iters` transition groups (no updates)."""
-    env = ring_env(env_golden, env27_golden, G * Ng)
+    env = generated_env(env_golden, env27_golden, G * Ng)
     L = learner(SHIPPED[0], G, replay_capacity=G * Ng * frames, lockstep_envs=G * Ng, **kw)
     L.init_params(0)
     L.per_enable_trainers()
@@ -192,7 +176,7 @@ def test_lockstep_commit_layout(env_golden, env27_golden):
     every trainer), stored transitions carry priorities in [eps^alpha, 1], sampled ones were re-prioritised, and each total is
     the sum of that trainer's leaves."""
     G, Ng, F = 16, 64, 12
-    env = ring_env(env_golden, env27_golden, G * Ng, pool=512)
+    env = generated_env(env_golden, env27_golden, G * Ng, pool=512)
     L = learner(SHIPPED[0], G, seed=1, algo=engine.ALGO_DDQN, batch_size=Ng, replay_capacity=G * Ng * F, lockstep_envs=G * Ng,
                 update_loop=3)
     L.init_params(0)
@@ -215,14 +199,11 @@ def test_lockstep_commit_layout(env_golden, env27_golden):
     env.close(); L.close()
 
 
-PER_MAX = 4194304
-
-
 def test_one_trainer_and_refusals(env_golden, env27_golden):
     # G = 1: per_enable_trainers is per_enable
     runs = []
     for enable in ("per_enable", "per_enable_trainers"):
-        env = ring_env(env_golden, env27_golden, 256)
+        env = generated_env(env_golden, env27_golden, 256)
         L = learner(SHIPPED[0], 1, seed=3, algo=engine.ALGO_DDQN, batch_size=64, replay_capacity=256 * 12, lockstep_envs=256)
         L.init_params(0)
         getattr(L, enable)()
@@ -238,7 +219,7 @@ def test_one_trainer_and_refusals(env_golden, env27_golden):
     for e, L in runs:
         e.close(); L.close()
     # refused once a transition is stored
-    env = ring_env(env_golden, env27_golden, 64)
+    env = generated_env(env_golden, env27_golden, 64)
     Lg = learner(SHIPPED[0], 4, replay_capacity=64 * 8, lockstep_envs=64)
     engine.train_run(env, Lg, 1, eps=0.5, do_update=False)
     with pytest.raises(engine.UavrlError, match="before the first transition"):
@@ -273,17 +254,9 @@ def test_env_plugin_prioritised_replay_per_trainer(tmp_path):
     run_eposide trains, every tree holds re-prioritised leaves; with Is_FL = 1, FL_Loop = 1 the aggregation runs and leaves
     every tree as it was; save() / Load_Mod round-trip the trainers."""
     import importlib
-    from uavrl_b200.plugins import xmlconfig
     cwd = os.getcwd()
     os.chdir(ROOT)
     try:
-        def env_dict(**kw):
-            ed = xmlconfig.XML2Dict(os.path.join(ROOT, "configs", "PathPlan_City_B200.xml"))["simulator"]["env"]
-            ed["num_UAV"], ed["scenario_pool"], ed["num_trainers"] = "8", "64", "8"
-            ed["Obstacles"]["buildings"] = os.path.join(ROOT, "configs", "buildings.xml")
-            ed["Agent"]["Trainer"]["Trainer_path"] = os.path.join(ROOT, "configs", "Trainer_DDQN_B200.xml")
-            ed.update(kw)
-            return ed
         mod = importlib.import_module("uavrl_b200.plugins.PathPlan_City_B200")
         orig = mod.XML2Dict
 
@@ -295,7 +268,7 @@ def test_env_plugin_prioritised_replay_per_trainer(tmp_path):
             return d
         mod.XML2Dict = patched
         try:
-            env = mod.PathPlan_City_B200(env_dict(Is_FL="1", FL_Loop="1"))
+            env = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml", Is_FL="1", FL_Loop="1"))
             tr = env.Trainer
             assert tr._learner.trainer_count() == 8 and tr.IsPriority_Replay
             calls = []
@@ -322,7 +295,7 @@ def test_env_plugin_prioritised_replay_per_trainer(tmp_path):
                 assert stored.size > 0 and (np.abs(stored - P0) > 1e-9).any(), g
                 assert abs(totals[g] - leaves[g].sum()) <= 1e-9 * totals[g]
             tr.save()
-            env2 = mod.PathPlan_City_B200(env_dict())                       # Load_Mod in the constructor
+            env2 = mod.PathPlan_City_B200(env_dict("Trainer_DDQN_B200.xml"))                       # Load_Mod in the constructor
             assert env2.Trainer._learner.per_state(n_slots)[0].shape == (8, n_slots)
         finally:
             mod.XML2Dict = orig

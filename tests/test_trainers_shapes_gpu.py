@@ -15,26 +15,20 @@ import pytest
 import torch
 
 import oracle as O
-from gpu_util import city_and_params
-from test_federate_gpu import check_rounds
-from test_qnet_shapes_gpu import SHAPES, act_sizes, expected_route
-from test_qnet_shapes_gpu import shape_id as route_id
-from test_tc_gpu import big_inputs, f64_forward, f64_unpack, net_layers
-from test_trainers_gpu import assert_same, assert_trainers_equal, learner, standalone_like
-from test_trainers_per_gpu import assert_trees_equal
-from test_weighted_f64_cpu import abs_err_bound, draw_batch, f64_update_w
-from test_weighted_update_shapes_gpu import ROUTES
+from fl_restatement import check_rounds
+from gpu_util import (DEV, assert_same, assert_trainers_equal, assert_trees_equal, dev, learner, n_sm,  # noqa: F401  (fixture)
+                      ring_env, short_episode_env, standalone_like)
+from qnet_restatement import abs_err_bound, big_inputs, draw_batch, f64_forward, f64_unpack, f64_update, net_layers
+from shapes import ROUTES, SHAPES, SHIPPED, act_sizes, expected_route
+from shapes import shape_id as route_id
 from uavrl_b200 import _lib, engine
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 
 # the lockstep loop steps the 27-action UAV env on the 100-d observation: the routes of ROUTES it can drive
 LOOP_ROUTES = [s for s in ROUTES if s[0] == 100 and s[2] == 27]
 GENERIC = (100, [64, 32], 27, 1)          # generic forward + generic training kernel
 FP32_ONLY = (100, [128, 64, 64], 27, 1)   # no tensor-core kernel at all
-SHIPPED = (100, [64, 64], 27, 0)
-MAX_STEP = 12                             # episodes end within the loops below, so done transitions enter the rings
 
 
 def test_tables_cover_every_route():
@@ -47,12 +41,7 @@ def test_tables_cover_every_route():
     assert any(r[0] is not None and r[1] is None and r[4] for r in loop)
     assert any(r[0] is not None and r[1] is None and not r[4] for r in loop)
     assert any(r[0] is None for r in loop)
-    assert all(any(s[:4] == want for s in LOOP_ROUTES) for want in (GENERIC, FP32_ONLY, SHIPPED))
-
-
-@pytest.fixture(scope="module")
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
+    assert all(any(s[:4] == want for s in LOOP_ROUTES) for want in (GENERIC, FP32_ONLY, SHIPPED[0]))
 
 
 @pytest.fixture(autouse=True)
@@ -73,10 +62,6 @@ def distinct_moments(L, rng):
     """Adam moments of every trainer drawn apart: a trainer reading another's moments shows in its next step."""
     L.set_params(rng.normal(0, 1e-3, (L.G, L.P)).astype(np.float32), 2)
     L.set_params(np.abs(rng.normal(0, 1e-6, (L.G, L.P))).astype(np.float32), 3)
-
-
-def dev(x):
-    return torch.as_tensor(np.ascontiguousarray(x)).to(DEV)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -150,7 +135,7 @@ def check_last_vs_float64(Lg, layers, algo, dueling, local, target, batch, kind,
     delta = abs_err_bound (the act tests' bound on Q carried through y), 2 |diff| delta + delta^2 per sample (MSE) or
     min(|diff|, 1) delta (Huber).  At B = 1 the loss is one sample's: no average hides that error, and q_a - y cancels."""
     G = Lg.G
-    l64, g64, ae64, y64, mag64 = f64_update_w(layers, algo, dueling, local, target, *batch, None, kind, abs_terms=True)
+    l64, g64, ae64, y64, mag64 = f64_update(layers, algo, dueling, local, target, *batch, None, kind, abs_terms=True)
     delta = abs_err_bound(y64, batch[2], ae64)
     moved = np.mean(2.0 * ae64 * delta + delta ** 2 if kind == "mse" else np.minimum(ae64, 1.0) * delta)
     tol = 2e-5 * abs(l64) + (moved if len(ae64) < 64 else 0.0)
@@ -217,20 +202,6 @@ def test_update_b12000_two_trainers(dqn_golden, shape):
 
 # ---------------------------------------------------------------------------------------------------------------------
 # 3 - 5. the lockstep loop
-def short_episode_env(env_golden, env27_golden):
-    """The golden city and UAV parameters with episodes capped at MAX_STEP steps."""
-    city, _, _, _ = city_and_params(env_golden, env27_golden)
-    p = env_golden["uav_params"]
-    return city, engine.UavParams(p[0], p[1], p[2], float(env27_golden["climb_rate"]), MAX_STEP)
-
-
-def ring_env(city, params, n, pool, first):
-    env = engine.EnvBatch(city, params, n, max_subgoals=64, auto_reset=True)
-    env.set_pool(pool["start"], pool["goal"], pool["heading"], pool["sub"], pool["n_sub"])
-    env.reset(first)
-    return env
-
-
 class LoopRun:
     """A grouped learner on N = G Ng auto-resetting envs run through `iters` lockstep iterations.  The scenario pool holds
     pool_n scenarios with pool_n dividing (G - 1) Ng: grouped env g Ng + j restarts at (g Ng + j + k N) mod pool_n, which is
@@ -395,7 +366,7 @@ def test_lockstep_loop_with_per_equals_standalone_pairs(env_golden, env27_golden
 
 
 @pytest.mark.parametrize("per", [False, True], ids=["uniform", "per"])
-@pytest.mark.parametrize("shape", [SHIPPED, GENERIC], ids=["100-64x64-27", "generic"])
+@pytest.mark.parametrize("shape", [SHIPPED[0], GENERIC], ids=["100-64x64-27", "generic"])
 def test_reference_scale_g4096_one_env_per_trainer(env_golden, env27_golden, shape, per):
     """README's benchmark layout: 4096 trainers of one env each, batch 64, run until every trainer holds more than 64
     transitions and updates have run (72 iterations, 80 ring frames).  Trainers 0, 1, 2047, 4094, 4095 and three drawn at
@@ -538,9 +509,9 @@ def test_launch_count_does_not_depend_on_g(env_golden, env27_golden, shape, per)
 def test_federate_ring_probes_one_env_per_trainer(env_golden, env27_golden):
     """G = 64 trainers of one env each: federate() draws 10 probes per trainer from the ring (Philox).  They are distinct,
     trainer-local indices in range, and every round, evaluated on the rows those indices name in the trainer's own ring
-    column, passes test_federate_gpu.check_rounds against float64."""
+    column, passes fl_restatement.check_rounds against float64."""
     G, Ng, iters = 64, 1, 30
-    shape = SHIPPED
+    shape = SHIPPED[0]
     city, params = short_episode_env(env_golden, env27_golden)
     pool = engine.EnvBatch(city, params, G - 1, max_subgoals=64).make_scenarios(G - 1, seed=3)
     env = ring_env(city, params, G, pool, 0)

@@ -1,4 +1,4 @@
-"""Prioritised-replay and Huber updates at every Q-network route against float64 (test_weighted_f64_cpu.f64_update_w): the
+"""Prioritised-replay and Huber updates at every Q-network route against float64 (qnet_restatement.f64_update): the
 importance weight is_w, the |Q - y| write-back abs_err and the loss_kind branch pass through the fp32 update kernel
 (learner.cu update_kernel) and the head epilogue of the tensor-core training kernel (tc_train.cu) on every route the shape
 sweep pins; the integrated PER update (update() drawing from the SumTree) is pinned to its composition from the public
@@ -8,39 +8,15 @@ import pytest
 import torch
 
 import oracle as O
-from gpu_util import city_and_params
-from test_qnet_shapes_gpu import SHAPES, expected_route, shape_id
-from test_tc_gpu import dev, f64_forward, f64_unpack, net_layers
-from test_weighted_f64_cpu import abs_err_bound, draw_batch, f64_update_w
+from gpu_util import PER_MAX, city_and_params, dev, n_sm  # noqa: F401  (module fixture)
+from qnet_restatement import abs_err_bound, draw_batch, f64_forward, f64_unpack, f64_update, net_layers
+from qnet_restatement import loss_kind_reset  # noqa: F401  (fixture)
+from shapes import FIXED_SHIPPED, LEGS, ROUTES, SHAPES, expected_route, shape_id
 from uavrl_b200 import engine
 
 pytestmark = pytest.mark.gpu
 
 
-# one shape of every route in the shape sweep's table (test_qnet_shapes_gpu.SHAPES), then the shipped 100-64-64-27 and VAnet2
-def _pick(in_dim, hidden, n_actions, dueling):
-    return next(s for s in SHAPES if s[:4] == (in_dim, hidden, n_actions, dueling))
-
-
-FIXED_SHIPPED = ("fixed", "fixed", True, True, True)
-ROUTES = [
-    _pick(100, [64, 32], 27, 1),          # generic forward + generic training, dueling head
-    _pick(96, [64, 64], 27, 0),           # generic, forward tiles stop at 64 rows
-    _pick(32, [64, 64, 64], 8, 0),        # generic, training tiles stop at 32 rows
-    _pick(100, [64], 31, 1),              # FIXED + FIXED, V at head column 31
-    _pick(124, [64], 27, 0),              # FIXED + FIXED, forward tiles stop at 64 rows
-    _pick(100, [48], 27, 0),              # tensor-core TD (16-column tail chunk) feeding the fp32 update
-    _pick(100, [112], 27, 0),             # the same, forward tiles stop at 64 rows
-    _pick(128, [64], 27, 0),              # FIXED TD feeding the fp32 update
-    _pick(100, [64, 64, 64], 27, 0),      # FIXED TD feeding the fp32 update in single-weights mode
-    _pick(100, [128, 64, 64], 27, 1),     # fp32 only, single weights, dueling
-    _pick(99, [64], 27, 0),               # fp32 only, in_dim % 4 != 0
-    (100, [64, 64], 27, 0, ("fixed", "fixed", False, True, True)),   # shipped; its 128-row forward image does not fit
-    (100, [64], 27, 1, FIXED_SHIPPED),
-]
-# B, algorithms: 32-row tiles with fused TD at NPRE = 1 and 2; bench.py's PER batch (32-row tiles, fused TD, 128 CTAs); 64-row
-# tiles with fused TD; separate TD passes with 64 / 128-row forward tiles.  "ddqn" is the dueling trainer on a dueling head.
-LEGS = {"B64-dqn": 64, "B64-ddqn": 64, "B4096-ddqn": 4096, "B6000-ddqn": 6000, "B12000-dqn": 12000}
 VARIANTS = {                          # weighted, abs_err requested, loss kind
     "w-mse": (True, True, "mse"),
     "huber": (False, True, "huber"),
@@ -70,17 +46,6 @@ def _cases():
 def test_route_table_covers_every_route():
     """ROUTES keeps one shape of every distinct route of the shape sweep's table."""
     assert {s[4] for s in SHAPES} <= {s[4] for s in ROUTES}
-
-
-@pytest.fixture(scope="module")
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-@pytest.fixture
-def loss_kind_reset():
-    yield
-    O.set_loss_kind("mse")            # the oracle's loss kind is process-wide state
 
 
 @pytest.mark.parametrize("shape,leg,algo,variant", _cases())
@@ -136,7 +101,7 @@ def test_weighted_update_vs_float64_and_oracle(dqn_golden, shape, leg, algo, var
         s_d, a_d, r_d, s2_d, d_d = dev(s), dev(a), dev(r), dev(s2), dev(d)
         w_d = dev(w) if weighted else None
         for (tc, L), loc, tgt in zip(learners, locals_, targets):
-            l64, g64, ae64, y64, mag64 = f64_update_w(layers, algo, dueling, loc, tgt, s, a, r, s2, d, w, kind, abs_terms=True)
+            l64, g64, ae64, y64, mag64 = f64_update(layers, algo, dueling, loc, tgt, s, a, r, s2, d, w, kind, abs_terms=True)
             if kind == "huber":
                 assert (ae64 < 1).mean() >= 0.1 and (ae64 > 1).mean() >= 0.1, (step, tc, float((ae64 < 1).mean()))
             ae = torch.full((B,), float("nan"), device="cuda") if want_err else None
@@ -233,7 +198,7 @@ def judge_composed(layers, algo, sl, ae, batch, leaves):
     s, a, r, s2, d = [x[first] for x in batch[:5]]
     local, target = batch[6:]
     sl, ae = sl[first], ae[first]
-    _, _, ae64, y64 = f64_update_w(layers, algo, 0, local, target, s, a, r, s2, d)
+    _, _, ae64, y64 = f64_update(layers, algo, 0, local, target, s, a, r, s2, d)
     tie = ddqn_ties(layers, local, s2) & (d == 0) if algo != engine.ALGO_DQN else np.zeros(len(sl), bool)
     assert tie.mean() <= 0.05
     err = np.abs(ae - ae64) - abs_err_bound(y64, r, ae64)
@@ -328,7 +293,6 @@ def test_per_update_is_its_composition_lockstep(env_golden, env27_golden, B):
 
 # ---------------------------------------------------------------------------------------------------------------------
 # The SumTree at its edges
-PER_MAX = 4194304                      # n1 = 131 072 group sums, n2 = 4096 = kPerMaxL2: the sampler's whole prefix scan
 
 
 def test_per_max_capacity_vs_oracle(n_sm):
