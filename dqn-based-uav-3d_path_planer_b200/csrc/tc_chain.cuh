@@ -8,10 +8,10 @@
 
 namespace uavrl {
 
-// UAVRL_TC_TRACE=1: CTA (0, 0) / thread 0 writes clock64() to slot `slot` at a stage boundary (stage_trace_print reads them)
-__device__ __forceinline__ void stage_trace(long long *t, int slot)
+// UAVRL_TC_TRACE=1: CTA (cta, 0) / thread 0 writes clock64() to slot `slot` at a stage boundary (stage_trace_print reads them)
+__device__ __forceinline__ void stage_trace(long long *t, int slot, int cta = 0)
 {
-    if (t && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) t[slot] = clock64();
+    if (t && blockIdx.x == cta && blockIdx.y == 0 && threadIdx.x == 0) t[slot] = clock64();
 }
 
 // ---- A operand of layer 0: R gathered rows -> TF32 hi/lo, canonical K-major layout.  Item i = (chunk j = i / R, row r = i % R;

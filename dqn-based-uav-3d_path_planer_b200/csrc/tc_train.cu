@@ -52,7 +52,7 @@ struct TcDwArgs {
     int32_t n_slices;                  // CTAs per layer; slice i accumulates chunks i, i + n_slices, ... into partial i
     const float *act_buf, *dz_buf;
     float *partials;                   // [n_slices][P]
-    long long *trace;                  // debug (UAVRL_TC_TRACE): CTA (0, 0) / thread 0 stage timestamps
+    long long *trace, *trace1;         // debug (UAVRL_TC_TRACE): CTA (0, 0) (layer 0) / CTA (1, 0) (layer 1) thread 0 stage timestamps
 };
 
 // NPRE / DUELING are compile-time so that the kernel a configuration runs carries no code of the others: a third of the
@@ -298,48 +298,72 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_train_kernel(TcNet tc, TcTra
 // ------------------------------------------------------------------ split-K weight gradients
 // Both products contract over the chunk's 128 samples, and wgmma reads tf32 operands K-major only: the rows ([sample][feature]
 // in global memory) are transposed on their way into shared memory, element (feature f, sample b) of a [features][128 samples]
-// K-major operand.  The SBO carries 16 bytes of padding so that a warp's scalar stores (one sample, 128 consecutive features)
-// spread over 8 banks instead of 2.
+// K-major operand.  A 16-byte core-matrix row of that operand is one feature of 4 consecutive samples, so a thread loads the
+// same float4 feature group of 4 consecutive samples -- a 4 x 4 block, transposed by register naming alone -- and writes its 4
+// features as 4 whole core-matrix rows, one 16-byte store each per hi / lo half.  The 8 lanes of a quarter-warp store the same
+// feature offset e of 8 consecutive groups, i.e. rows e and 4 + e of 4 consecutive 8-feature groups: the 16 bytes of SBO
+// padding put those 8 rows on 8 different 4-bank slots (no bank conflict).
 constexpr uint32_t kDwSbo = (kDwChunk / 4) * 128u + 16u;   // bytes per 8-feature group: 128 samples x 4 B x 8 (+ 16)
-constexpr int kDwARows = 128;                               // A operand: input features + the ones column, zero padded
+constexpr int kDwARows = 128;                               // A operand rows the two warpgroups' m64 MMAs read
 
-// rows [128 samples][width floats] in global memory -> hi/lo K-major operands.  8 consecutive lanes load one 128-byte
-// row segment (coalesced).
-// LOG2F4 = log2(float4 per row) (5 for the 128-wide A operand, 3 / 4 for a 32- / 64-wide B operand); U float4 per thread,
-// ALL loaded before the first is converted (the loads are the latency that matters: one round trip per operand).
-// ones_col >= 0: that feature column is set to 1 for valid samples (bias gradient).
-template <int LOG2F4, int U>
-__device__ __forceinline__ void dw_load_rows(const float *const *rows, int width, float4 (&v)[U])
+// Staging step s covers float4 feature groups [8s, 8s + 8) of all 128 samples: lane 8i + q of warp w takes samples
+// 16w + 4i .. 16w + 4i + 3 and group 8s + q, so the 8 lanes of a sample quad read one 128-byte row segment per sample
+// (coalesced).  Steps s < dw_steps(groups) cover groups [0, groups).
+static_assert(kTcThreads == 256 && kDwChunk == 128, "dW staging: 8 warps x 4 sample quads cover the 32 sample quads of a chunk");
+struct DwItem { int b0, jc; };                             // samples b0 .. b0 + 3, float4 group jc
+__device__ __forceinline__ DwItem dw_item(int s)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    return {16 * warp + 4 * (lane >> 3), 8 * s + (lane & 7)};
+}
+__device__ __forceinline__ int dw_steps(int groups) { return (groups + 7) >> 3; }
+
+// rows [128 samples][width floats] in global memory -> registers: the float4 groups [0, groups) of every sample (zero past
+// width and for samples without a row), 4 float4 per step, U >= 4 dw_steps(groups) float4 per thread, ALL loaded before the first
+// is converted (the loads are the latency that matters: one round trip per operand).
+template <int U>
+__device__ __forceinline__ void dw_load_rows(const float *const *rows, int width, int groups, float4 (&v)[U])
 {
     // nothing but loads here: a register that a load is still going to write must not be touched again before the data
     // is consumed, or the warp stalls on that load before issuing the next one (the ones column is applied at store time)
+    const int n = dw_steps(groups);
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-        const int i = threadIdx.x + u * kTcThreads;
-        const int b = i >> LOG2F4, jc = i & ((1 << LOG2F4) - 1);
-        const float *r = (b < kDwChunk) ? rows[b] : nullptr;
-        v[u] = (r && 4 * jc < width) ? __ldg(reinterpret_cast<const float4 *>(r) + jc) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-}
-// ones_col >= 0: that feature column (a multiple of 4: K_real % 4 == 0, tc_train_init) becomes 1 for valid samples
-template <int LOG2F4, int U>
-__device__ __forceinline__ void dw_store_rows(const float4 (&v)[U], const float *const *rows, int ones_col, unsigned char *hi, unsigned char *lo)
-{
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-        const int i = threadIdx.x + u * kTcThreads;
-        const int b = i >> LOG2F4, jc = i & ((1 << LOG2F4) - 1);
-        if (b >= kDwChunk) continue;
-        float4 x = v[u];
-        if (ones_col >= 0 && (ones_col >> 2) == jc && rows[b]) x.x = 1.f;
-        const float xs[4] = {x.x, x.y, x.z, x.w};
+    for (int s = 0; s < U / 4; ++s) {
+        if (s >= n) break;
+        const DwItem it = dw_item(s);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            float h, l;
-            tf32_split(xs[e], h, l);
-            const uint32_t off = mma_off(4 * jc + e, b, kDwSbo);
-            *reinterpret_cast<float *>(hi + off) = h;
-            *reinterpret_cast<float *>(lo + off) = l;
+            const float *r = rows[it.b0 + e];
+            v[4 * s + e] = (r && 4 * it.jc < width) ? __ldg(reinterpret_cast<const float4 *>(r) + it.jc) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    }
+}
+// registers (dw_load_rows) -> hi/lo K-major operands, feature rows [0, 4 groups).  ones_col >= 0: that feature column (a
+// multiple of 4: K_real % 4 == 0, tc_train_init) becomes 1 for valid samples (bias gradient).
+template <int U>
+__device__ __forceinline__ void dw_store_rows(const float4 (&v)[U], int groups, const float *const *rows, int ones_col, unsigned char *hi,
+                                              unsigned char *lo)
+{
+    const int n = dw_steps(groups);
+#pragma unroll
+    for (int s = 0; s < U / 4; ++s) {
+        if (s >= n) break;
+        const DwItem it = dw_item(s);
+        if (it.jc >= groups) continue;
+        float x[4][4];                                       // x[e][i]: feature 4 jc + e of sample b0 + i
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float4 t = v[4 * s + i];
+            x[0][i] = (ones_col >= 0 && (ones_col >> 2) == it.jc && rows[it.b0 + i]) ? 1.f : t.x;
+            x[1][i] = t.y; x[2][i] = t.z; x[3][i] = t.w;
+        }
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            float4 h, lo4;
+            tf32_split(x[e][0], h.x, lo4.x); tf32_split(x[e][1], h.y, lo4.y); tf32_split(x[e][2], h.z, lo4.z); tf32_split(x[e][3], h.w, lo4.w);
+            const uint32_t off = mma_off(4 * it.jc + e, it.b0, kDwSbo);
+            *reinterpret_cast<float4 *>(hi + off) = h;
+            *reinterpret_cast<float4 *>(lo + off) = lo4;
         }
     }
 }
@@ -355,14 +379,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     const float *act_buf = a.act_buf + (size_t)grp * a.B * tc.act_stride, *dz_buf = a.dz_buf + (size_t)grp * a.B * tc.dz_stride;
     const TcLayer T = tc.L[l];
     const int rowsA = T.K_real + 1;                           // input features + the all-ones column (bias gradient)
-    // A = [act ; 1]^T as [feature][sample] (rows past rowsA are zero), B = dZ^T as [out][sample]; hi and lo images of each
+    // A = [act ; 1]^T as [feature][sample], B = dZ^T as [out][sample]; hi and lo images of each.  A holds rows [0, 4 gA):
+    // rowsA rounded up to whole core matrices, zero past rowsA.  The m64 MMAs also read the rows behind those, which are never
+    // written: they only feed accumulator rows >= rowsA, which the epilogue does not store.
+    const int gA = (rowsA + 7) / 8 * 2;                       // float4 feature groups of A
     unsigned char *Ahi = smem, *Alo = Ahi + (kDwARows / 8) * kDwSbo, *Bhi = Alo + (kDwARows / 8) * kDwSbo;
     unsigned char *Blo = Bhi + (T.N_pad / 8) * kDwSbo;
     __shared__ const float *rows[2][kDwChunk];               // double buffered: chunk c + 1 is resolved while chunk c is loaded
     __shared__ const float *drows[2][kDwChunk];
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, quad = warp & 3, half = warp >> 2;
-    stage_trace(a.trace, 0);
+    const int tid = threadIdx.x;
+    const auto dw_trace = [&](int slot) { stage_trace(a.trace, slot); stage_trace(a.trace1, slot, 1); };
+    dw_trace(0);
     uint32_t pkey[4];
     Philox::gen(src.key, src.epoch, 0x5A17ull, pkey);
     auto resolve_chunk = [&](int c, int buf) {                // row pointers of chunk c (128 samples)
@@ -381,35 +409,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     // PDL: hidden activations and dZ come from the training chain (the predecessor); the layer-0 CTAs' A operand is
     // built from replay rows (written >= 2 kernels back) and is gathered before the wait
     if (l != 0) { pdl_wait(); pdl_trigger(); }
-    stage_trace(a.trace, 1);
-    // A: 128 samples x 128 columns (features, the ones column, zero padding) = 16 float4 per thread; B: 128 x N_pad.
+    dw_trace(1);
+    // A: 128 samples x 4 gA features, 4 float4 per thread and staging step (at most 16); B: 128 x N_pad (at most 8).
     // Persistent over this slice's chunks: the loads of chunk c + 1 are issued before the MMAs of chunk c and land while they
     // run; the products accumulate in the same registers -> one partial per slice however large the batch.
     float4 va[16], vb[8];
-    auto load_chunk = [&](int buf) {
-        dw_load_rows<5, 16>(rows[buf], T.K_real, va);
-        if (T.N_pad == 32) {
-#pragma unroll
-            for (int u = 4; u < 8; ++u) vb[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-            dw_load_rows<3, 4>(drows[buf], 32, reinterpret_cast<float4 (&)[4]>(vb));
-        } else {
-            dw_load_rows<4, 8>(drows[buf], 64, vb);         // N_pad = 64
-        }
-    };
-    if (l == 0) {                                              // replay rows first, dZ after the predecessor has finished
-        dw_load_rows<5, 16>(rows[0], T.K_real, va);
-        pdl_wait(); pdl_trigger();
-        if (T.N_pad == 32) {
-#pragma unroll
-            for (int u = 4; u < 8; ++u) vb[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-            dw_load_rows<3, 4>(drows[0], 32, reinterpret_cast<float4 (&)[4]>(vb));
-        } else {
-            dw_load_rows<4, 8>(drows[0], 64, vb);
-        }
-    } else {
-        load_chunk(0);
-    }
-    stage_trace(a.trace, 2);
+    auto load_a = [&](int buf) { dw_load_rows(rows[buf], T.K_real, gA, va); };
+    auto load_b = [&](int buf) { dw_load_rows(drows[buf], T.N_pad, T.N_pad / 4, vb); };
+    load_a(0);
+    if (l == 0) { pdl_wait(); pdl_trigger(); }                 // replay rows first, dZ after the predecessor has finished
+    load_b(0);
+    dw_trace(2);
     // warpgroup g owns features [64g, 64g + 64); its MMAs run when that range holds real rows
     const int row0 = (tid >> 7) * 64;
     const bool wg_live = row0 < rowsA;
@@ -417,15 +427,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
     int it = 0;
     for (int c = slice; c < a.n_chunks; c += a.n_slices, ++it) {
         if (it > 0) __syncthreads();                           // both warpgroups' MMAs of the previous chunk have read SMEM
-        dw_store_rows<5, 16>(va, rows[it & 1], T.K_real, Ahi, Alo);
-        if (T.N_pad == 32) dw_store_rows<3, 4>(reinterpret_cast<float4 (&)[4]>(vb), drows[it & 1], -1, Bhi, Blo);
-        else dw_store_rows<4, 8>(vb, drows[it & 1], -1, Bhi, Blo);
+        dw_store_rows(va, gA, rows[it & 1], T.K_real, Ahi, Alo);
+        dw_store_rows(vb, T.N_pad / 4, drows[it & 1], -1, Bhi, Blo);
         const int cn = c + a.n_slices;
         resolve_chunk(cn, (it + 1) & 1);
         fence_proxy_async();
         __syncthreads();
-        stage_trace(a.trace, 4);
-        if (cn < a.n_chunks) load_chunk((it + 1) & 1);         // next chunk's rows -> registers while the MMAs run
+        dw_trace(4);
+        if (cn < a.n_chunks) { load_a((it + 1) & 1); load_b((it + 1) & 1); }   // next chunk's rows -> registers while the MMAs run
         if (wg_live) {
             const uint64_t ah = mma_desc(Ahi + (row0 / 8) * kDwSbo, kDwSbo), al = mma_desc(Alo + (row0 / 8) * kDwSbo, kDwSbo);
             const uint64_t bh = mma_desc(Bhi, kDwSbo), bl = mma_desc(Blo, kDwSbo);
@@ -433,48 +442,47 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcNet tc, TcDwArgs
             else wgmma_3xtf32<64>(d, ah, al, bh, bl, kDwChunk / 8, it > 0 ? 1u : 0u);
         }
     }
-    stage_trace(a.trace, 5);
-    // the accumulator -> a [feature][out] tile in the A operand's space (every MMA has read it), one feature row per thread
-    __syncthreads();
-    float *acc = reinterpret_cast<float *>(smem);
-    const int acc_ld = T.N_pad + 4;
+    dw_trace(5);
+    // epilogue: row f = input feature (or the ones column), column o = output unit, into partial slice `chunk`.  Each warpgroup
+    // stages its own fragment row-major over its own rows of the A operand -- its MMAs are done and the other warpgroup's read
+    // other rows and B -- so a 128-thread barrier suffices and it does not wait for the other warpgroup's MMAs.  Thread t then
+    // takes row row0 + t % 64 and 32 columns: lanes hold consecutive f, so every store instruction writes 32 consecutive
+    // elements of one weight row; the 32 columns of a thread walk the rows with a pointer increment and a predicate each (the
+    // address arithmetic used to dominate this epilogue).
     if (wg_live) {
-        if (T.N_pad == 32) store_frag<32>(d, acc, acc_ld, row0, 0, kDwARows);
-        else store_frag<64>(d, acc, acc_ld, row0, 0, kDwARows);
-    }
-    __syncthreads();
-    stage_trace(a.trace, 6);
-    // epilogue: row f = input feature (or the ones column), column o = output unit, into partial slice `chunk`.
-    // Lanes hold consecutive f, so every store instruction writes 32 consecutive elements of one weight row; the 32 columns of a
-    // thread walk the rows with a pointer increment and a predicate each (the address arithmetic used to dominate this epilogue).
-    float *part = a.partials + ((size_t)grp * a.n_slices + chunk) * a.P;
-    const int f = quad * 32 + lane;
-    for (int c0 = half * 32; c0 < T.N_pad; c0 += 64) {
-        if (quad * 32 >= rowsA) break;
-        float v[32];
-        acc_ld32(acc, acc_ld, f, c0, v);
-        const int n_main = min(max(T.out_main - c0, 0), 32), n_all = min(max(T.N_real - c0, 0), 32);   // columns [0, n_main): main block, [n_main, n_all): value head
-        if (f > T.K_real) continue;
-        const bool brow = (f == T.K_real);                       // the ones column: bias gradients (stride 1), else weight row f (stride K_real)
-        const int stride = brow ? 1 : T.K_real;
-        const int i_main = brow ? T.b_off + c0 : T.w_off + f + c0 * T.K_real;
-        const int i_val = brow ? T.b2_off + (c0 - T.out_main) : (T.w2_off >= 0 ? T.w2_off : 0) + f + (c0 - T.out_main) * T.K_real;
-        float *p = part + i_main;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            if (j < n_main) *p = v[j];
-            p += stride;
-        }
-        if (n_all > n_main) {
-            float *q = part + i_val;
+        float *acc = reinterpret_cast<float *>(Ahi + (row0 / 8) * kDwSbo);
+        const int acc_ld = T.N_pad + 4, t = tid & 127, c0 = 32 * (t >> 6), f = row0 + (t & 63);
+        if (T.N_pad == 32) store_frag<32>(d, acc, acc_ld, 0, 0, 64);
+        else store_frag<64>(d, acc, acc_ld, 0, 0, 64);
+        if (row0 == 0) asm volatile("bar.sync 1, 128;" ::: "memory");             // this warpgroup's 128 threads
+        else asm volatile("bar.sync 2, 128;" ::: "memory");
+        dw_trace(6);
+        float *part = a.partials + ((size_t)grp * a.n_slices + chunk) * a.P;
+        if (c0 < T.N_pad && f <= T.K_real) {
+            float v[32];
+            acc_ld32(acc, acc_ld, t & 63, c0, v);
+            const int n_main = min(max(T.out_main - c0, 0), 32), n_all = min(max(T.N_real - c0, 0), 32);   // columns [0, n_main): main block, [n_main, n_all): value head
+            const bool brow = (f == T.K_real);                   // the ones column: bias gradients (stride 1), else weight row f (stride K_real)
+            const int stride = brow ? 1 : T.K_real;
+            const int i_main = brow ? T.b_off + c0 : T.w_off + f + c0 * T.K_real;
+            const int i_val = brow ? T.b2_off + (c0 - T.out_main) : (T.w2_off >= 0 ? T.w2_off : 0) + f + (c0 - T.out_main) * T.K_real;
+            float *p = part + i_main;
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
-                if (j >= n_main && j < n_all) *q = v[j];
-                q += stride;
+                if (j < n_main) *p = v[j];
+                p += stride;
+            }
+            if (n_all > n_main) {
+                float *q = part + i_val;
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    if (j >= n_main && j < n_all) *q = v[j];
+                    q += stride;
+                }
             }
         }
     }
-    stage_trace(a.trace, 7);
+    dw_trace(7);
 }
 
 typedef void (*TrainKernel)(TcNet, TcTrainArgs);
@@ -556,6 +564,7 @@ int launch_tc_train(uavrl_learner *l, const Route &r, const BatchSrc &src, int B
     DevMem trace_mem;
     if (int rc = stage_trace_alloc(trace_mem, a.trace)) return rc;
     if (int rc = stage_trace_alloc(trace_mem, d.trace)) return rc;
+    if (int rc = stage_trace_alloc(trace_mem, d.trace1)) return rc;
     const ChainKernel train = r.td_fused ? kChainTrainFusedTd : kChainTrain;
     const int npre = r.td_fused ? (l->cfg.algo != UAVRL_ALGO_DQN ? 2 : 1) : 0;
     UAVRL_CUDA(launch_kernel(pick_train_kernel(npre, tc.dueling != 0, r.train == 2), dim3(grid, l->G), dim3(kTcThreads),
@@ -575,7 +584,8 @@ int launch_tc_train(uavrl_learner *l, const Route &r, const BatchSrc &src, int B
     UAVRL_LAUNCHED();
     const int rc_train = stage_trace_print(st, a.trace, "[train_trace] B=%d R=%d fused_td=%d", B, a.R, a.fused_td);
     const int rc_dw = stage_trace_print(st, d.trace, "[dw_trace] B=%d chunks=%d (CTA 0 = layer 0)", B, d.n_chunks);
-    if (rc_train || rc_dw) return rc_train ? rc_train : rc_dw;
+    const int rc_dw1 = stage_trace_print(st, d.trace1, "[dw_trace] B=%d chunks=%d (CTA 1 = layer 1)", B, d.n_chunks);
+    if (rc_train || rc_dw || rc_dw1) return rc_train ? rc_train : rc_dw ? rc_dw : rc_dw1;
     *n_grad_parts = d.n_slices;
     *n_loss_parts = grid;
     return 0;

@@ -10,7 +10,7 @@ x = torch.randn(4096, 100, device="cuda")
 for _ in range(5):
     L.act(x, 0.1)
 torch.cuda.synchronize()
-# training kernels: [tc_trace] lines for the TD pass and [dw_trace] for the weight-gradient kernel (layer-0 CTA)
+# training kernels: [tc_trace] lines for the TD pass and [dw_trace] for the weight-gradient kernel (a layer-0 and a layer-1 CTA)
 B = 4096
 s = torch.randn(B, 100, device="cuda"); s2 = torch.randn(B, 100, device="cuda")
 a = torch.randint(0, 27, (B,), device="cuda", dtype=torch.int32); r = torch.randn(B, device="cuda"); d = torch.zeros(B, device="cuda")
