@@ -800,10 +800,7 @@ static int learner_init(uavrl_learner *l, const uavrl_learner_config *cfg, int32
         return fail(UAVRL_ERR_INVALID, "network too large for the shared-memory resident kernels");
     const size_t G = (size_t)n_trainers, P = (size_t)l->net.P;
     l->max_ctas = 4 * num_sms();
-    // gradient / loss partial slots per trainer: one learner keeps max_ctas (any batch); a grouped learner sizes them from the
-    // per-trainer batch (the fp32 update kernel's grid, the largest of the update routes) and grows them for larger batches
-    const int tiles = (cfg->batch_size + kTile - 1) / kTile;
-    l->parts_cap = (G == 1 || tiles > l->max_ctas) ? l->max_ctas : tiles;
+    l->parts_cap = trainer_parts_cap(n_trainers, cfg->batch_size, l->max_ctas);   // the fp32 update kernel's grid is the widest
     DevMem &m = l->mem, &pm = l->parts_mem;
     if ((rc = m.alloc(l->local, G * P)) || (rc = m.alloc(l->target, G * P)) || (rc = m.alloc(l->m, G * P)) ||
         (rc = m.alloc(l->v, G * P)) || (rc = m.alloc(l->grad, G * P)) ||
@@ -838,19 +835,9 @@ int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out)
 int uavrl_learner_create_trainers(const uavrl_learner_config *cfg, int32_t n_trainers, uavrl_learner **out)
 {
     if (!cfg || !out) return fail(UAVRL_ERR_INVALID, "uavrl_learner_create: null argument");
-    if (n_trainers < 1 || n_trainers > 65535)        // every grouped kernel runs one grid row per trainer: gridDim.y <= 65535
-        return fail(UAVRL_ERR_INVALID, "n_trainers must be in [1, 65535]");
-    if (n_trainers > 1 && (cfg->lockstep_envs < 0 || cfg->lockstep_envs % n_trainers != 0))
-        return fail(UAVRL_ERR_INVALID, "lockstep_envs must be a multiple of n_trainers (every trainer owns lockstep_envs / n_trainers envs)");
-    if (n_trainers > 1 && cfg->replay_capacity / n_trainers <= 0)
-        return fail(UAVRL_ERR_INVALID, "replay_capacity / n_trainers must be > 0");
-    if (cfg->batch_size <= 0 || cfg->replay_capacity <= 0) return fail(UAVRL_ERR_INVALID, "batch_size and replay_capacity must be > 0");
     if (cfg->algo < 0 || cfg->algo > 2) return fail(UAVRL_ERR_INVALID, "unknown algo");
     if (cfg->loss_kind < 0 || cfg->loss_kind > 1) return fail(UAVRL_ERR_INVALID, "loss_kind must be 0 (MSE) or 1 (Huber)");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-        return fail(UAVRL_ERR_CUDA, "no CUDA device: the learner has no CPU fallback");
-    UAVRL_CUDA(cudaSetDevice(cfg->device));
+    if (int rc = check_trainer_group(*cfg, n_trainers, "learner")) return rc;
     uavrl_learner *l = new uavrl_learner();
     if (int rc = learner_init(l, cfg, n_trainers)) { uavrl_learner_destroy(l); return rc; }
     *out = l;
@@ -992,7 +979,7 @@ int uavrl_learner_update(uavrl_learner *l, const int32_t *idx_tape_dev, float *l
 {
     if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
     l->epoch += 1;                                              // DuelingDQN_Trainer.py:152
-    if (l->replay.count / l->G <= l->cfg.batch_size) return 0;  // PathPlan_City.py:383: nothing sampled yet (per trainer)
+    if (!l->replay.ready(l->cfg.batch_size)) return 0;          // nothing sampled yet
     BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, idx_tape_dev);
     return do_update(l, src, l->cfg.batch_size, l->cfg.batch_size, loss_dev, true, stream);
 }
@@ -1029,7 +1016,7 @@ int uavrl_learner_compute_grads(uavrl_learner *l, const int32_t *idx_tape_dev, i
     if (!l || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     if (int rc = refuse_grouped(l, "uavrl_learner_compute_grads (data-parallel training)")) return rc;
     // refused before the epoch counts: a rank that retries must stay on the other ranks' sample keys and target schedule
-    if (l->replay.count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
+    if (!l->replay.ready(l->cfg.batch_size)) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
     l->epoch += 1;
     BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, idx_tape_dev);
     return do_update(l, src, l->cfg.batch_size, global_batch, loss_dev, false, stream);
@@ -1157,7 +1144,7 @@ int uavrl_learner_update_dp(uavrl_learner *l, const int32_t *idx_tape_dev, int32
     if (!l || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     if (int rc = refuse_grouped(l, "uavrl_learner_update_dp (data-parallel training)")) return rc;
     if (!l->comm_ready) return fail(UAVRL_ERR_STATE, "uavrl_learner_update_dp before uavrl_learner_comm_connect");
-    if (l->replay.count <= l->cfg.batch_size) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
+    if (!l->replay.ready(l->cfg.batch_size)) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     l->epoch += 1;
     BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, idx_tape_dev);

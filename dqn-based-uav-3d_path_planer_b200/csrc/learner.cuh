@@ -272,6 +272,34 @@ struct Route {
 };
 Route learner_route(const uavrl_learner *l, int n);
 
+// The refusals both trainer-group create entry points make (uavrl_learner_create_trainers, uavrl_sac_create_trainers) after the
+// learner's own configuration checks and before anything is allocated; on success cfg.device is current.  `learner` names the
+// handle in the no-device message.
+template <class Config>
+int check_trainer_group(const Config &cfg, int32_t n_trainers, const char *learner)
+{
+    if (n_trainers < 1 || n_trainers > 65535)        // every grouped kernel runs one grid row per trainer: gridDim.y <= 65535
+        return fail(UAVRL_ERR_INVALID, "n_trainers must be in [1, 65535]");
+    if (n_trainers > 1 && (cfg.lockstep_envs < 0 || cfg.lockstep_envs % n_trainers != 0))
+        return fail(UAVRL_ERR_INVALID, "lockstep_envs must be a multiple of n_trainers (every trainer owns lockstep_envs / n_trainers envs)");
+    if (n_trainers > 1 && cfg.replay_capacity / n_trainers <= 0)
+        return fail(UAVRL_ERR_INVALID, "replay_capacity / n_trainers must be > 0");
+    if (cfg.batch_size <= 0 || cfg.replay_capacity <= 0) return fail(UAVRL_ERR_INVALID, "batch_size and replay_capacity must be > 0");
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+        return fail(UAVRL_ERR_CUDA, std::string("no CUDA device: the ") + learner + " has no CPU fallback");
+    UAVRL_CUDA(cudaSetDevice(cfg.device));
+    return 0;
+}
+
+// Gradient / loss partial slots per trainer: a single trainer keeps max_ctas (any batch); a grouped learner sizes them from its
+// per-trainer batch (the grid of its widest update kernel) and grows them when a larger explicit batch arrives.
+inline int32_t trainer_parts_cap(int32_t G, int32_t batch_size, int32_t max_ctas)
+{
+    const int32_t tiles = (batch_size + kTile - 1) / kTile;
+    return (G == 1 || tiles > max_ctas) ? max_ctas : tiles;
+}
+
 // generic MLP description: trunk widths + head = `head_main` rows (+ `head_extra` rows from a second parameter block)
 int build_mlp(int in_dim, int n_hidden, const int32_t *hidden, int head_main, int head_extra, NetDev &n);
 int launch_act(uavrl_learner *l, const float *obs, int n, float eps, int is_train, const float *u_tape,

@@ -196,6 +196,10 @@ struct ReplayStore {
     Iteration begin() const;
     void commit();
     int64_t count_after_commit() const;   // lockstep: `count` once the next commit has run
+    // an update of `batch` transitions per trainer may sample (PathPlan_City.py:383): every trainer holds more than batch, now or
+    // (lockstep) once the next commit has run
+    bool ready(int64_t batch) const { return count / G > batch; }
+    bool ready_after_commit(int64_t batch) const { return count_after_commit() / G > batch; }
     // forget every transition; the next iteration re-observes into frame `head`
     void restart();
     // n whole-store logical indices (0 = oldest) to host arrays; any output may be null

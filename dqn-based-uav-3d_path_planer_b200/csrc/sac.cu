@@ -24,8 +24,8 @@
 
 #include <vector>
 
-#include "env.cuh"
 #include "mlp_tile.cuh"
+#include "sac.cuh"
 
 namespace uavrl {
 
@@ -488,10 +488,7 @@ __global__ void sac_federate_kernel(int P, int G, float *__restrict__ actor)
 
 using namespace uavrl;
 
-// ------------------------------------------------------------------ host handle
-// the two networks of a SAC learner and the stride of its gradient planes: everything the kernels' shared memory follows from
-struct SacShape { NetDev actor, critic; int32_t gld; };
-
+// ------------------------------------------------------------------ host handle (sac.cuh)
 constexpr size_t kSacMaxSmem = 227 * 1024;     // shared memory one block may use on sm_90
 
 // refuses a configuration before anything is allocated
@@ -527,25 +524,6 @@ static int sac_smem_total(const SacShape &s, size_t out[4])
     }
     return 0;
 }
-
-// A grouped learner (uavrl_sac_create_trainers) holds G trainers: every per-network vector, weight image and scratch array
-// below is [G][...]; trainer g acts for envs [g Ng, (g + 1) Ng) of the shared ring frames and samples only their transitions.
-struct uavrl_sac {
-    uavrl_sac_config cfg;
-    SacShape sh;
-    int32_t G = 1;
-    float *p[5] = { nullptr }, *img[5] = { nullptr };      // actor, c1, c2, t1, t2
-    float *m[3] = { nullptr }, *v[3] = { nullptr }, *grad[3] = { nullptr };
-    int32_t *map_a = nullptr, *map_c = nullptr;
-    float *part[3] = { nullptr };                          // gradient partials [G][parts_cap][P]
-    float *stat = nullptr, *out = nullptr, *td = nullptr, *lossbuf = nullptr;   // [G][parts_cap][4], [G][4], [G][td_cap][2]
-    float *scal = nullptr;                                 // [G][3]: log_alpha, its Adam exp_avg, exp_avg_sq
-    int32_t td_cap = 0, parts_cap = 0, max_ctas = 4 * num_sms();
-    int64_t epoch = 0, adam_t = 0;
-    uint64_t calls = 0;
-    ReplayStore replay;                                    // lockstep ring (float[2] actions); none when lockstep_envs == 0
-    DevMem mem, parts_mem, td_mem;                         // owners: networks, moments, maps, scalars; partials / stat; td
-};
 
 static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
 {
@@ -595,8 +573,22 @@ static int sac_scratch(uavrl_sac *s, int B, int grid, cudaStream_t st)
     return grow(s->td_mem, s->td_cap, B, st, true, buf(s->td, G * B * kSacA));
 }
 
-// one SAC_Trainer.update of every trainer on the batch described by src (B rows per trainer)
-static int sac_update_impl(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev, cudaStream_t st)
+int uavrl::launch_sac_act(uavrl_sac *s, const float *obs, int n, const float *eps, float *actions, cudaStream_t st)
+{
+    SacArgs a;
+    BatchSrc none;
+    memset(&none, 0, sizeof(none));
+    const int ng = n / s->G;                                   // rows per trainer: block g belongs to trainer g
+    sac_fill_args(s, a, none, ng, eps, 0x8000000000000000ull | s->calls++);
+    const int grid = a.n_tiles < s->max_ctas ? a.n_tiles : s->max_ctas;
+    if (s->G > 1) sac_act_kernel<true><<<dim3(grid, s->G), kNetThreads, smem_act(s->sh), st>>>(a, obs, ng, actions);
+    else sac_act_kernel<false><<<grid, kNetThreads, smem_act(s->sh), st>>>(a, obs, ng, actions);
+    UAVRL_LAUNCHED();
+    return 0;
+}
+
+int uavrl::launch_sac_update(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev,
+                             cudaStream_t st)
 {
     const int n_tiles = (B + kTile - 1) / kTile;
     const int grid = n_tiles < s->max_ctas ? n_tiles : s->max_ctas;
@@ -659,12 +651,7 @@ static int sac_alloc(uavrl_sac *s)
     if ((rc = mem.alloc(s->map_a, ma.size())) || (rc = mem.alloc(s->map_c, mc.size()))) return rc;
     UAVRL_CUDA(cudaMemcpy(s->map_a, ma.data(), ma.size() * 4, cudaMemcpyHostToDevice));
     UAVRL_CUDA(cudaMemcpy(s->map_c, mc.data(), mc.size() * 4, cudaMemcpyHostToDevice));
-    {   // gradient partial / stat slots per trainer: one learner keeps max_ctas (any batch); a grouped learner sizes them from the
-        // per-trainer batch and grows them for larger explicit batches (sac_scratch)
-        const int tiles = (cfg->batch_size + kTile - 1) / kTile;
-        const int cap = (G == 1 || tiles > s->max_ctas) ? s->max_ctas : tiles;
-        if ((rc = sac_scratch(s, cfg->batch_size, cap, 0))) return rc;
-    }
+    if ((rc = sac_scratch(s, cfg->batch_size, trainer_parts_cap(s->G, cfg->batch_size, s->max_ctas), 0))) return rc;
     if ((rc = mem.alloc(s->scal, 3 * G)) || (rc = mem.alloc(s->out, 4 * G)) || (rc = mem.alloc(s->lossbuf, 1))) return rc;
     std::vector<float> init(3 * G, 0.f);
     for (size_t g = 0; g < G; ++g) init[3 * g] = logf(0.01f);          // SAC_Trainer.py:53
@@ -703,19 +690,9 @@ int uavrl_sac_create(const uavrl_sac_config *cfg, uavrl_sac **out)
 int uavrl_sac_create_trainers(const uavrl_sac_config *cfg, int32_t n_trainers, uavrl_sac **out)
 {
     if (!cfg || !out) return fail(UAVRL_ERR_INVALID, "uavrl_sac_create: null argument");
-    if (n_trainers < 1 || n_trainers > 65535)        // every grouped kernel runs one grid row per trainer: gridDim.y <= 65535
-        return fail(UAVRL_ERR_INVALID, "n_trainers must be in [1, 65535]");
-    if (n_trainers > 1 && (cfg->lockstep_envs < 0 || cfg->lockstep_envs % n_trainers != 0))
-        return fail(UAVRL_ERR_INVALID, "lockstep_envs must be a multiple of n_trainers (every trainer owns lockstep_envs / n_trainers envs)");
-    if (n_trainers > 1 && cfg->replay_capacity / n_trainers <= 0)
-        return fail(UAVRL_ERR_INVALID, "replay_capacity / n_trainers must be > 0");
-    if (cfg->batch_size <= 0 || cfg->replay_capacity <= 0) return fail(UAVRL_ERR_INVALID, "batch_size and replay_capacity must be > 0");
     SacShape sh;
     int rc = sac_shape(*cfg, sh);
-    if (rc) return rc;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(UAVRL_ERR_CUDA, "no CUDA device: the SAC learner has no CPU fallback");
-    UAVRL_CUDA(cudaSetDevice(cfg->device));
+    if (rc || (rc = check_trainer_group(*cfg, n_trainers, "SAC learner"))) return rc;
     size_t smem[4];
     if ((rc = sac_smem_total(sh, smem))) return rc;
     for (int i = 0; i < 4; ++i)
@@ -835,16 +812,7 @@ int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *ep
     if (!s || !obs_dev || !actions_dev || n <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     if (n % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_act: n must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
-    SacArgs a;
-    BatchSrc none;
-    memset(&none, 0, sizeof(none));
-    const int ng = n / s->G;                                   // rows per trainer: block g belongs to trainer g
-    sac_fill_args(s, a, none, ng, eps_dev, 0x8000000000000000ull | s->calls++);
-    const int grid = a.n_tiles < s->max_ctas ? a.n_tiles : s->max_ctas;
-    if (s->G > 1) sac_act_kernel<true><<<dim3(grid, s->G), kNetThreads, smem_act(s->sh), (cudaStream_t)stream>>>(a, obs_dev, ng, actions_dev);
-    else sac_act_kernel<false><<<grid, kNetThreads, smem_act(s->sh), (cudaStream_t)stream>>>(a, obs_dev, ng, actions_dev);
-    UAVRL_LAUNCHED();
-    return 0;
+    return launch_sac_act(s, obs_dev, n, eps_dev, actions_dev, (cudaStream_t)stream);
 }
 
 int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev,
@@ -857,7 +825,7 @@ int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const fl
     BatchSrc src;
     memset(&src, 0, sizeof(src));
     src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.act2 = a_dev; src.rew = r_dev; src.done_f32 = d_dev;
-    return sac_update_impl(s, src, B / s->G, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
+    return launch_sac_update(s, src, B / s->G, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
 }
 
 int64_t uavrl_sac_replay_size(const uavrl_sac *s) { return s ? s->replay.count : 0; }
@@ -878,9 +846,9 @@ int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const flo
     if (!s->replay.frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;                                             // SAC_Trainer.py:320
-    if (s->replay.count / s->G <= s->cfg.batch_size) return 0; // PathPlan_City.py:383: nothing sampled yet (per trainer)
-    return sac_update_impl(s, s->replay.source(s->cfg.seed, s->epoch, idx_tape_dev), s->cfg.batch_size, eps_next_dev, eps_cur_dev, losses_dev,
-                           (cudaStream_t)stream);
+    if (!s->replay.ready(s->cfg.batch_size)) return 0;         // nothing sampled yet
+    return launch_sac_update(s, s->replay.source(s->cfg.seed, s->epoch, idx_tape_dev), s->cfg.batch_size, eps_next_dev, eps_cur_dev,
+                             losses_dev, (cudaStream_t)stream);
 }
 
 int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
@@ -892,42 +860,6 @@ int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
     sac_federate_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, s->G, s->p[0]);
     UAVRL_LAUNCHED();
     return sac_pack(s, 0, st);                                 // the G actor images
-}
-
-// lockstep loop with the continuous env step: state -> actor sample -> Move_Agent -> replay add -> update
-int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t do_update, uavrl_train_stats *stats_host, void *stream)
-{
-    if (!env || !s || n_iters < 0) return fail(UAVRL_ERR_INVALID, "bad argument");
-    if (s->cfg.lockstep_envs != env->d.n || !s->replay.frames) return fail(UAVRL_ERR_INVALID, "sac.lockstep_envs must equal env.n_envs");
-    if (!env->reset_done) return fail(UAVRL_ERR_STATE, "uavrl_sac_train_run before uavrl_env_reset");
-    UAVRL_CUDA(cudaSetDevice(env->cfg.device));
-    cudaStream_t st = (cudaStream_t)stream;
-    ReplayStore &rs = s->replay;
-    EnvStatsMark mark;
-    int rc; int64_t updates = 0;
-    if ((rc = mark.begin(env->d, st, stats_host))) return rc;
-    for (int it = 0; it < n_iters; ++it) {
-        const ReplayStore::Iteration io = rs.begin();
-        if (!rs.frame0_valid) { if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc; rs.frame0_valid = true; }
-        if ((rc = uavrl_sac_act(s, io.obs_t, (int32_t)rs.N, nullptr, io.act2, st))) return rc;
-        if ((rc = launch_env_step(env->d, UAVRL_ACT_CONT_F32X2, io.act2, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st))) return rc;
-        rs.commit();
-        if (do_update) {
-            s->epoch += 1;
-            if (rs.count / s->G <= s->cfg.batch_size) continue;     // per trainer
-            if ((rc = sac_update_impl(s, rs.source(s->cfg.seed, s->epoch, nullptr), s->cfg.batch_size, nullptr, nullptr, nullptr, st))) return rc;
-            ++updates;
-        }
-    }
-    if ((rc = mark.end(env->d, st, updates, stats_host))) return rc;
-    if (stats_host) {
-        std::vector<float> o((size_t)s->G * 4);                 // [G][4]; last_loss = the mean actor loss over trainers
-        UAVRL_CUDA(cudaMemcpy(o.data(), s->out, o.size() * sizeof(float), cudaMemcpyDeviceToHost));
-        double lsum = 0.0;
-        for (int g = 0; g < s->G; ++g) lsum += o[4 * (size_t)g];
-        stats_host->last_loss = (float)(lsum / (double)s->G);
-    }
-    return 0;
 }
 
 }  // extern "C"

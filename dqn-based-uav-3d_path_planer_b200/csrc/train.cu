@@ -1,4 +1,5 @@
-// train.cu -- the fused lockstep training loop over the env batch and the learner.
+// train.cu -- the fused lockstep training loops over the env batch and a learner: the Q-network learner's (uavrl_train_run,
+// uavrl_train_run_dp, uavrl_train_profile) and the SAC learner's (uavrl_sac_train_run) run the same iteration.
 //
 // Replaces PathPlan_City.run_thread_OffPolicy + PathPlan_City.update (Envs/PathPlan_City.py:364-385,
 // 757-776) for N envs: state -> get_action -> Move_Agent -> replay add -> sample -> Trainer.update.
@@ -7,6 +8,7 @@
 // separate push kernel; 412 B per stored transition instead of 812 B).
 #include "env.cuh"
 #include "learner.cuh"
+#include "sac.cuh"
 
 #include <vector>
 
@@ -14,60 +16,135 @@ using namespace uavrl;
 
 enum Loop { kLoopRun, kLoopDp, kLoopProfile };
 
-// The refusals the three loops share, each loop's in the order it reports them; nothing is enqueued before they pass.
-static int check_loop(const uavrl_env *env, const uavrl_learner *l, Loop loop, int32_t n_iters)
+// ------------------------------------------------------------------ what the loop does differently per learner
+// uavrl_learner_comm_connect has run: the data-parallel loop's precondition (there is no data-parallel SAC loop)
+static bool connected(const uavrl_learner *l) { return l->comm_ready; }
+static bool connected(const uavrl_sac *) { return false; }
+
+// get_action on the ring's current frame: Choose_Action2 -> Trainer.get_action (PathPlan_City.py:338-346)
+static int act(uavrl_learner *l, const ReplayStore::Iteration &io, int n, float eps, cudaStream_t st)
 {
-    const bool paired = l->replay.mode == kReplayLockstep && l->cfg.lockstep_envs == env->d.n;
+    return launch_act(l, io.obs_t, n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st);
+}
+static int act(uavrl_sac *s, const ReplayStore::Iteration &io, int n, float, cudaStream_t st)
+{
+    return launch_sac_act(s, io.obs_t, n, nullptr, io.act2, st);
+}
+
+// Move_Agent + replay add (:371-382) on those actions: reward / done land in the ring slots, the observations in the next frame.
+// The Q-network's step joins the learner's dependent-launch chain.
+static int env_step(uavrl_env *env, uavrl_learner *l, const ReplayStore::Iteration &io, cudaStream_t st)
+{
+    if (int rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
+                                 l->chain.next(kChainEnv).pdl))
+        return rc;
+    l->chain.launched(kChainEnv);
+    return 0;
+}
+static int env_step(uavrl_env *env, uavrl_sac *, const ReplayStore::Iteration &io, cudaStream_t st)
+{
+    return launch_env_step(env->d, UAVRL_ACT_CONT_F32X2, io.act2, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st);
+}
+
+static void commit(uavrl_learner *l, cudaStream_t st) { lockstep_commit(l, st); }    // + prioritised-replay priorities
+static void commit(uavrl_sac *s, cudaStream_t) { s->replay.commit(); }
+
+// PathPlan_City.update -> Trainer.update (:757-776) on batch_size transitions per trainer sampled through src.  dp_batch > 0:
+// data-parallel over that global batch; marks (profiling, may be null): launch_update's three events
+static int update(uavrl_learner *l, const BatchSrc &src, int dp_batch, cudaStream_t st, cudaEvent_t *marks)
+{
+    const int B = l->cfg.batch_size;
+    return dp_batch > 0 ? launch_update_dp(l, src, B, dp_batch, l->loss_dev, st) : launch_update(l, src, B, B, l->loss_dev, true, st, marks);
+}
+static int update(uavrl_sac *s, const BatchSrc &src, int, cudaStream_t st, cudaEvent_t *)
+{
+    return launch_sac_update(s, src, s->cfg.batch_size, nullptr, nullptr, nullptr, st);
+}
+
+// where each trainer's loss of its last update lives: element 0 of [G][stride] device floats
+struct Losses { const float *dev; int stride; };
+static Losses losses(const uavrl_learner *l) { return { l->loss_dev, 1 }; }
+static Losses losses(const uavrl_sac *s) { return { s->out, 4 }; }       // actor, critic 1, critic 2, alpha loss
+
+// ------------------------------------------------------------------ the loop
+// The refusals the loops share, each loop's in the order it reports them; nothing is enqueued before they pass.  fn: the entry
+// point, named in the reset refusal.
+template <class Learner>
+static int check_loop(const uavrl_env *env, const Learner *l, Loop loop, int32_t n_iters, const char *fn)
+{
+    const ReplayStore &rs = l->replay;
+    const bool paired = rs.mode == kReplayLockstep && l->cfg.lockstep_envs == env->d.n;
     if (loop == kLoopDp && l->G > 1) return fail(UAVRL_ERR_INVALID, "uavrl_train_run_dp is not available on a learner with several trainers");
     if (loop != kLoopProfile && !paired) return fail(UAVRL_ERR_INVALID, "learner.lockstep_envs must equal env.n_envs");
-    if (l->net.in_dim != kObsDim) return fail(UAVRL_ERR_INVALID, "learner.in_dim must be 100 (the UAV observation)");
-    if (loop == kLoopDp && !l->comm_ready) return fail(UAVRL_ERR_STATE, "uavrl_train_run_dp before uavrl_learner_comm_connect");
-    if (loop != kLoopProfile && !env->reset_done)
-        return fail(UAVRL_ERR_STATE, loop == kLoopDp ? "uavrl_train_run_dp before uavrl_env_reset" : "uavrl_train_run before uavrl_env_reset");
+    // the env step writes kObsDim floats per env into the ring's frames
+    if (rs.in_dim != kObsDim) return fail(UAVRL_ERR_INVALID, "learner.in_dim must be 100 (the UAV observation)");
+    if (loop == kLoopDp && !connected(l)) return fail(UAVRL_ERR_STATE, "uavrl_train_run_dp before uavrl_learner_comm_connect");
+    if (loop != kLoopProfile && !env->reset_done) return fail(UAVRL_ERR_STATE, std::string(fn) + " before uavrl_env_reset");
     if (env->cfg.device != l->cfg.device) return fail(UAVRL_ERR_INVALID, "env and learner live on different devices");
-    if (loop == kLoopProfile && (!paired || !env->reset_done || !l->replay.frame0_valid))
+    if (loop == kLoopProfile && (!paired || !env->reset_done || !rs.frame0_valid))
         return fail(UAVRL_ERR_STATE, "uavrl_train_profile needs a warmed-up lockstep env/learner pair");
     // the data-parallel loop: every rank must take part in every all-reduce; the profile: every iteration's update is timed.
     // So every iteration must update: the caller warms the replay up first.  The count never shrinks, so the first
     // iteration's sample decides, and a refusal leaves env, ring and epoch untouched
-    if (loop != kLoopRun && n_iters > 0 && l->replay.count_after_commit() / l->G <= l->cfg.batch_size)
+    if (loop != kLoopRun && n_iters > 0 && !rs.ready_after_commit(l->cfg.batch_size))
         return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions (warm up with uavrl_train_run first)");
     return 0;
 }
 
-// One lockstep iteration: begin the ring's iteration (the very first one also materialises obs_0), Choose_Action2 ->
-// Trainer.get_action (PathPlan_City.py:338-346) and Move_Agent + replay add (:371-382) -- reward/done land in the ring slots --
-// commit the frame, then n_updates x PathPlan_City.update -> Trainer.update (:757-776), each counting an epoch and skipped
-// while a trainer's ring holds <= batch_size transitions.  dp_batch > 0: data-parallel updates over that global batch.
+// One lockstep iteration: begin the ring's iteration (the very first one also materialises obs_0), act, env step, commit the
+// frame, then n_updates updates, each counting an epoch and skipped while a trainer's ring holds <= batch_size transitions.
 // ev (profiling, may be null): 7 events, before act, after act, after the env step, the update's three marks
 // (launch_update), after the optimiser step.
-static int iteration(uavrl_env *env, uavrl_learner *l, float eps, int n_updates, int dp_batch, cudaStream_t st, cudaEvent_t *ev,
+template <class Learner>
+static int iteration(uavrl_env *env, Learner *l, float eps, int n_updates, int dp_batch, cudaStream_t st, cudaEvent_t *ev,
                      int64_t &updates)
 {
     int rc;
-    const ReplayStore::Iteration io = l->replay.begin();
-    if (!l->replay.frame0_valid) {
+    ReplayStore &rs = l->replay;
+    const ReplayStore::Iteration io = rs.begin();
+    if (!rs.frame0_valid) {
         if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc;
-        l->replay.frame0_valid = true;
+        rs.frame0_valid = true;
     }
     if (ev) UAVRL_CUDA(cudaEventRecord(ev[0], st));
-    if ((rc = launch_act(l, io.obs_t, env->d.n, eps, l->is_train, nullptr, nullptr, io.act, nullptr, st))) return rc;
+    if ((rc = act(l, io, env->d.n, eps, st))) return rc;
     if (ev) UAVRL_CUDA(cudaEventRecord(ev[1], st));
-    if ((rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
-                              l->chain.next(kChainEnv).pdl))) return rc;
-    l->chain.launched(kChainEnv);
+    if ((rc = env_step(env, l, io, st))) return rc;
     if (ev) UAVRL_CUDA(cudaEventRecord(ev[2], st));
-    lockstep_commit(l, st);
-    const int B = l->cfg.batch_size;
+    commit(l, st);
     for (int u = 0; u < n_updates; ++u) {
         l->epoch += 1;
-        if (l->replay.count / l->G <= B) continue;      // per trainer
-        const BatchSrc src = l->replay.source(l->cfg.seed, l->epoch, nullptr);
-        if ((rc = dp_batch > 0 ? launch_update_dp(l, src, B, dp_batch, l->loss_dev, st)
-                               : launch_update(l, src, B, B, l->loss_dev, true, st, ev ? ev + 3 : nullptr))) return rc;
+        if (!rs.ready(l->cfg.batch_size)) continue;
+        if ((rc = update(l, rs.source(l->cfg.seed, l->epoch, nullptr), dp_batch, st, ev ? ev + 3 : nullptr))) return rc;
         ++updates;
     }
     if (ev) UAVRL_CUDA(cudaEventRecord(ev[6], st));
+    return 0;
+}
+
+// n_iters iterations of n_updates updates each; stats_host (may be null) receives what they added
+template <class Learner>
+static int run(uavrl_env *env, Learner *l, const char *fn, int32_t n_iters, float eps, int n_updates, uavrl_train_stats *stats_host,
+               void *stream)
+{
+    int rc;
+    if ((rc = check_loop(env, l, kLoopRun, n_iters, fn))) return rc;
+    UAVRL_CUDA(cudaSetDevice(env->cfg.device));
+    cudaStream_t st = (cudaStream_t)stream;
+    EnvStatsMark mark;
+    if ((rc = mark.begin(env->d, st, stats_host))) return rc;
+    int64_t updates = 0;
+    for (int it = 0; it < n_iters; ++it)
+        if ((rc = iteration(env, l, eps, n_updates, 0, st, nullptr, updates))) return rc;
+    if ((rc = mark.end(env->d, st, updates, stats_host))) return rc;
+    if (stats_host) {
+        const Losses ls = losses(l);                            // grouped learner: the mean over trainers
+        std::vector<float> v((size_t)l->G * ls.stride);
+        UAVRL_CUDA(cudaMemcpy(v.data(), ls.dev, v.size() * sizeof(float), cudaMemcpyDeviceToHost));
+        double lsum = 0.0;
+        for (size_t g = 0; g < (size_t)l->G; ++g) lsum += v[g * ls.stride];
+        stats_host->last_loss = (float)(lsum / (double)l->G);
+    }
     return 0;
 }
 
@@ -75,34 +152,22 @@ extern "C" int uavrl_train_run(uavrl_env *env, uavrl_learner *l, int32_t n_iters
                                int32_t do_update, uavrl_train_stats *stats_host, void *stream)
 {
     if (!env || !l || n_iters < 0) return fail(UAVRL_ERR_INVALID, "bad argument");
-    int rc;
-    if ((rc = check_loop(env, l, kLoopRun, n_iters))) return rc;
-    UAVRL_CUDA(cudaSetDevice(env->cfg.device));
-    cudaStream_t st = (cudaStream_t)stream;
-    EnvStatsMark mark;
-    if ((rc = mark.begin(env->d, st, stats_host))) return rc;
-    int64_t updates = 0;
-    {
-        ChainScope chain(l->chain);
-        for (int it = 0; it < n_iters; ++it)
-            if ((rc = iteration(env, l, eps, do_update ? updates_per_iter : 0, 0, st, nullptr, updates))) return rc;
-    }
-    if ((rc = mark.end(env->d, st, updates, stats_host))) return rc;
-    if (stats_host) {
-        std::vector<float> losses((size_t)l->G);                // grouped learner: the mean over trainers
-        UAVRL_CUDA(cudaMemcpy(losses.data(), l->loss_dev, losses.size() * sizeof(float), cudaMemcpyDeviceToHost));
-        double lsum = 0.0;
-        for (float x : losses) lsum += x;
-        stats_host->last_loss = (float)(lsum / (double)l->G);
-    }
-    return 0;
+    ChainScope chain(l->chain);
+    return run(env, l, "uavrl_train_run", n_iters, eps, do_update ? updates_per_iter : 0, stats_host, stream);
+}
+
+extern "C" int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t do_update, uavrl_train_stats *stats_host,
+                                   void *stream)
+{
+    if (!env || !s || n_iters < 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    return run(env, s, "uavrl_sac_train_run", n_iters, 0.f, do_update ? 1 : 0, stats_host, stream);
 }
 
 extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, int32_t global_batch, void *stream)
 {
     if (!env || !l || n_iters < 0 || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     int rc;
-    if ((rc = check_loop(env, l, kLoopDp, n_iters))) return rc;
+    if ((rc = check_loop(env, l, kLoopDp, n_iters, "uavrl_train_run_dp"))) return rc;
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
     ChainScope chain(l->chain);
     int64_t updates = 0;
@@ -116,7 +181,7 @@ extern "C" int uavrl_train_profile(uavrl_env *env, uavrl_learner *l, int32_t n_i
 {
     if (!env || !l || n_iters <= 0 || !ms_out) return fail(UAVRL_ERR_INVALID, "bad argument");
     int rc;
-    if ((rc = check_loop(env, l, kLoopProfile, n_iters))) return rc;
+    if ((rc = check_loop(env, l, kLoopProfile, n_iters, "uavrl_train_profile"))) return rc;
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
     cudaStream_t st = (cudaStream_t)stream;
     constexpr int NE = 7;                      // events per iteration -> 6 intervals

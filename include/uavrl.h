@@ -418,7 +418,11 @@ int uavrl_sac_replay_gather(uavrl_sac *s, int32_t n, const int64_t *logical_idx_
  * and losses_dev as in uavrl_sac_update_batch. */
 int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const float *eps_next_dev, const float *eps_cur_dev, float *losses_dev,
                             void *stream);
-/* PathPlan_City.run_thread_OffPolicy + update with the SAC trainer and the reference's continuous step, N envs in lockstep */
+/* PathPlan_City.run_thread_OffPolicy + update with the SAC trainer and the reference's continuous step, N envs in lockstep:
+ * the iteration of uavrl_train_run with one SAC update per iteration when do_update (stats_host->last_loss: the mean actor
+ * loss over trainers).  Refused before anything is enqueued, leaving env, ring, parameters and counters untouched:
+ * lockstep_envs != env.n_envs or no ring, obs_dim != 100 (the env step writes 100-float observations into the ring) or env and
+ * learner on different devices (UAVRL_ERR_INVALID, as uavrl_train_run); no uavrl_env_reset (UAVRL_ERR_STATE). */
 int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t do_update, uavrl_train_stats *stats_host, void *stream);
 
 /* Data-parallel form of uavrl_train_run (after uavrl_learner_comm_connect): every iteration ends with
