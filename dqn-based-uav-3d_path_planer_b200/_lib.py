@@ -17,6 +17,7 @@ MAX_HIDDEN = 4
 ACT_CONT_F32, ACT_CONT_F64, ACT_DISCRETE27, ACT_CONT_F32X2 = 0, 1, 2, 3
 ALGO_DQN, ALGO_DDQN, ALGO_DUELING = 0, 1, 2
 INFO_NAMES = ("normal", "success", "lose")
+SAC_COMM_HANDLE_BYTES = 128         # UAVRL_SAC_COMM_HANDLE_BYTES: CUDA IPC handle + PCI bus id
 
 
 class UavrlError(RuntimeError):
@@ -149,6 +150,16 @@ SIGNATURES = {
     "uavrl_sac_replay_size": (C.c_int64, [VP]),
     "uavrl_sac_replay_gather": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP, VP, VP]),
     "uavrl_sac_update_replay": (C.c_int, [VP, VP, VP, VP, VP, VP]),
+    "uavrl_sac_comm_init": (C.c_int, [VP, C.c_int32, C.c_int32, VP]),
+    "uavrl_sac_comm_connect": (C.c_int, [VP, VP]),
+    "uavrl_sac_update_replay_dp": (C.c_int, [VP, VP, VP, VP, C.c_int32, VP, VP]),
+    "uavrl_sac_critic_grads_replay": (C.c_int, [VP, VP, VP, C.c_int32, VP]),
+    "uavrl_sac_critic_grads_batch": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP, VP, VP, C.c_int32, VP]),
+    "uavrl_sac_apply_critic_grads": (C.c_int, [VP, VP]),
+    "uavrl_sac_actor_grads": (C.c_int, [VP, VP, VP]),
+    "uavrl_sac_apply_actor_grads": (C.c_int, [VP, VP, VP]),
+    "uavrl_sac_exchange_ptr": (VP, [VP, C.c_int32, C.POINTER(C.c_int64)]),
+    "uavrl_sac_train_run_dp": (C.c_int, [VP, VP, C.c_int32, C.c_int32, VP]),
     "uavrl_train_run_dp": (C.c_int, [VP, VP, C.c_int32, C.c_float, C.c_int32, VP]),
     "uavrl_train_profile": (C.c_int, [VP, VP, C.c_int32, C.c_float, VP, VP]),
     "uavrl_last_error": (C.c_char_p, []),

@@ -368,14 +368,19 @@ cudaError_t launch_reduce_adam(dim3 grid, cudaStream_t st, bool pdl, const AdamA
 }
 
 // ---- data-parallel optimiser step: one-shot NVLink all-reduce fused with Adam, in ONE kernel, block by block, with no fence
-// and no flag words.  Every rank owns a symmetric receive buffer (slot q belongs to rank q); block b owns parameters
-// [64 b, 64 b + 64).  It reduces its slice of this rank's partials and pushes each value into slot `rank` of every rank's
-// receive buffer as ONE 8-byte word {epoch : value} (a single-copy-atomic store: the value can never be seen without its
-// epoch -- the "LL" idea of NCCL's low-latency protocol).  Then the 64 threads of the block poll -- in local memory -- the
-// `world` words of their own parameter until every epoch matches, sum the values in rank order and apply Adam.  A
-// __threadfence_system() between data and a flag would cost a system-scope fence per launch even on one GPU; here nothing
-// orders two stores, so nothing needs a fence.  recv[2][world][P + 1] alternates by epoch parity: a sender can
-// overwrite a slot only two exchanges later, and it cannot finish the exchange in between before the receiver has read.
+// and no flag words.  Every rank owns a symmetric receive buffer (slot q belongs to rank q); block b owns 64 parameters of
+// one network of the exchange (DpExchange: up to two networks, by block range).  It reduces its slice of this rank's
+// partials and pushes each value into slot `rank` of every rank's receive buffer as ONE 8-byte word {tag : value} (a
+// single-copy-atomic store: the value can never be seen without its tag -- the "LL" idea of NCCL's low-latency protocol).
+// Then the 64 threads of the block poll -- in local memory -- the `world` words of their own parameter until every tag
+// matches, sum the values in rank order and apply Adam.  The exchange's scalar words (a loss share, an update's stat sums)
+// travel the same way from block 0.  A __threadfence_system() between data and a flag would cost a system-scope fence per
+// launch even on one GPU; here nothing orders two stores, so nothing needs a fence.
+// The buffer alternates halves by the parity of the tag, which advances once per exchange (an update may make several: a SAC
+// update exchanges its critics, then its actor).  A rank writes exchange e + 2 into exchange e's half only after its own
+// exchange e + 1 kernel has completed; completing e + 1 needs every rank's e + 1 words, and each rank pushes those only after
+// its own exchange-e kernel -- the last reader of e's half on that rank -- has finished.  So no word is overwritten before
+// its reader has summed it, whatever the exchanges carry.
 __device__ __forceinline__ void st_relaxed_sys_u64(unsigned long long *p, unsigned long long v)
 {
     asm volatile("st.relaxed.sys.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
@@ -386,7 +391,7 @@ __device__ __forceinline__ unsigned long long ld_relaxed_sys_u64(const unsigned 
     asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
     return v;
 }
-// sum over ranks (fixed order: every rank computes the same bits) of the words {epoch : value} at recv[w * stride]
+// sum over ranks (fixed order: every rank computes the same bits) of the words {tag : value} at recv[w * stride]
 __device__ __forceinline__ float ll_gather_sum(const unsigned long long *recv, size_t stride, int world, unsigned epoch)
 {
     float gsum = 0.f;
@@ -406,52 +411,63 @@ __device__ __forceinline__ float ll_gather_sum(const unsigned long long *recv, s
     return gsum;
 }
 
+// partials0 / partials1 / extra_parts: the segments' and the scalar words' partials of x, as __restrict__ kernel parameters
+// (reduce_adam_kernel says why)
 __global__ void __launch_bounds__(256)
-dp_allreduce_adam_kernel(AdamArgs a, int nparts, int n_loss_parts, const float *__restrict__ partials,
-                         const float *__restrict__ loss_partials, unsigned long long *const *peer_recv,
+dp_allreduce_adam_kernel(AdamArgs a, DpExchange x, const float *__restrict__ partials0, const float *__restrict__ partials1,
+                         const float *__restrict__ extra_parts, unsigned long long *const *peer_recv,
                          const unsigned long long *recv_local, size_t stride, size_t parity_off, int rank, unsigned epoch,
-                         AdamPtrs q, unsigned long long *trace)
+                         unsigned long long *trace)
 {
     // trace (UAVRL_DP_TRACE=1): block 0 accumulates nanoseconds spent in {reduce, push, wait for the peers' words, Adam} and a launch count
     unsigned long long t0 = 0, t1 = 0, t2 = 0, t3 = 0;
     auto now = [] { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; };
     __shared__ float red[4][64];
+    const int sg = (x.n_seg > 1 && (int)blockIdx.x >= x.seg[0].blocks) ? 1 : 0;
+    const int P = sg ? x.seg[1].P : x.seg[0].P, nparts = sg ? x.seg[1].nparts : x.seg[0].nparts;
+    const float *partials = sg ? partials1 : partials0;
+    const size_t woff = sg ? (size_t)x.seg[0].P : 0;                 // the segment's first word in a rank's slot
     const int ix = threadIdx.x & 63, cg = threadIdx.x >> 6;
-    const int i = blockIdx.x * 64 + ix;
+    const int i = ((int)blockIdx.x - (sg ? x.seg[0].blocks : 0)) * 64 + ix;
     AdamPre pre;
-    if (cg == 0 && i < a.P) pre = adam_prefetch(q, i);   // before the wait: nothing here is the predecessor's output
+    if (cg == 0 && i < P) pre = adam_prefetch(sg ? x.seg[1].q : x.seg[0].q, i);     // before the wait: nothing here is the predecessor's output
     pdl_wait();                 // PDL (common.cuh): the gradient partials come from the predecessor
     pdl_trigger();
     if (trace && blockIdx.x == 0 && threadIdx.x == 0) t0 = now();
     float g = 0.f;
-    if (i < a.P) g = reduce_group(partials, a.P, nparts, i, cg);
+    if (i < P) g = reduce_group(partials, P, nparts, i, cg);
     red[cg][ix] = g;
     __syncthreads();
     if (trace && blockIdx.x == 0 && threadIdx.x == 0) t1 = now();
     const size_t slot = parity_off + (size_t)rank * stride;
     const unsigned long long tag = (unsigned long long)epoch << 32;
-    if (i < a.P) {
+    if (i < P) {
         const float gs = (red[0][ix] + red[1][ix]) + (red[2][ix] + red[3][ix]);
-        for (int w = cg; w < a.world; w += 4) st_relaxed_sys_u64(peer_recv[w] + slot + i, tag | __float_as_uint(gs));   // 512 contiguous bytes per peer
+        for (int w = cg; w < a.world; w += 4) st_relaxed_sys_u64(peer_recv[w] + slot + woff + i, tag | __float_as_uint(gs));   // 512 contiguous bytes per peer
     }
-    if (blockIdx.x == 0 && threadIdx.x >= 224) {                 // last warp of block 0: this rank's loss share
-        const int lane = threadIdx.x & 31;
-        float s = 0.f;
-        for (int c = lane; c < n_loss_parts; c += 32) s += loss_partials[c];
+    const size_t xoff = (size_t)x.seg[0].P + (x.n_seg > 1 ? (size_t)x.seg[1].P : 0);   // the scalar words follow the segments
+    if (blockIdx.x == 0 && threadIdx.x >= 224) {                 // last warp of block 0: this rank's scalar words
 #pragma unroll
-        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (lane == 0)
-            for (int w = 0; w < a.world; ++w) st_relaxed_sys_u64(peer_recv[w] + slot + a.P, tag | __float_as_uint(s * a.inv_b));
+        for (int j = 0; j < kDpMaxExtra; ++j) {
+            if (j >= x.n_extra) break;
+            const float s = warp_column_sum(extra_parts, x.n_extra_parts, x.extra_stride, j);
+            if ((threadIdx.x & 31) == 0)
+                for (int w = 0; w < a.world; ++w) st_relaxed_sys_u64(peer_recv[w] + slot + xoff + j, tag | __float_as_uint(s * x.extra_scale));
+        }
     }
     if (trace && blockIdx.x == 0 && threadIdx.x == 0) t2 = now();
     const unsigned long long *recv = recv_local + parity_off;
-    if (cg == 0 && i < a.P) {
-        const float gsum = ll_gather_sum(recv + i, stride, a.world, epoch);
+    if (cg == 0 && i < P) {
+        const float gsum = ll_gather_sum(recv + woff + i, stride, a.world, epoch);
         if (trace && blockIdx.x == 0 && threadIdx.x == 0) t3 = now();
+        const AdamPtrs &q = sg ? x.seg[1].q : x.seg[0].q;
         q.grad[i] = gsum;
         adam_update_pre(a, q, i, gsum, pre);
     }
-    if (blockIdx.x == 0 && threadIdx.x == 255 && q.loss_out) *q.loss_out = ll_gather_sum(recv + a.P, stride, a.world, epoch);
+    if (blockIdx.x == 0 && threadIdx.x >= 256 - x.n_extra && x.extra_out) {
+        const int j = 255 - threadIdx.x;
+        x.extra_out[j] = ll_gather_sum(recv + xoff + j, stride, a.world, epoch);
+    }
     if (trace && blockIdx.x == 0) {
         __syncthreads();
         if (threadIdx.x == 0) {
@@ -459,6 +475,17 @@ dp_allreduce_adam_kernel(AdamArgs a, int nparts, int n_loss_parts, const float *
             trace[0] += t1 - t0; trace[1] += t2 - t1; trace[2] += t3 - t2; trace[3] += t4 - t3; trace[4] += 1;
         }
     }
+}
+
+cudaError_t launch_dp_exchange(PeerComm &c, const AdamArgs &a, const DpExchange &x, cudaStream_t st, bool pdl, unsigned long long *trace)
+{
+    c.tag += 1;
+    const size_t stride = (size_t)x.seg[0].P + (x.n_seg > 1 ? (size_t)x.seg[1].P : 0) + (size_t)x.n_extra;   // this exchange's slot
+    const size_t parity_off = (size_t)(c.tag & 1u) * (size_t)c.world * c.words;
+    const int blocks = x.seg[0].blocks + (x.n_seg > 1 ? x.seg[1].blocks : 0);
+    return launch_kernel(dp_allreduce_adam_kernel, dim3(blocks), dim3(256), 0, st, pdl, a, x, x.seg[0].partials,
+                         x.n_seg > 1 ? x.seg[1].partials : nullptr, x.extra_parts, (unsigned long long *const *)c.peer_dev,
+                         (const unsigned long long *)c.recv, stride, parity_off, (int)c.rank, c.tag, trace);
 }
 
 __global__ void copy_kernel(size_t n, const float *__restrict__ src, float *__restrict__ dst)
@@ -671,7 +698,7 @@ static AdamArgs adam_args(uavrl_learner *l, const Grads &g, bool apply)
 {
     AdamArgs a;
     memset(&a, 0, sizeof(a));
-    a.P = l->net.P; a.nparts = g.nparts; a.n_loss_parts = g.n_loss_parts; a.apply = apply ? 1 : 0; a.world = l->world;
+    a.P = l->net.P; a.nparts = g.nparts; a.n_loss_parts = g.n_loss_parts; a.apply = apply ? 1 : 0; a.world = l->comm.world;
     a.img_floats = l->net.smem_w_floats; a.tc_floats = l->tc.train_img_bytes / 4;
     a.inv_b = g.inv_b;
     if (apply) {
@@ -694,20 +721,21 @@ static int launch_reduce_adam_step(uavrl_learner *l, const AdamArgs &a, ChainKer
 // dp_allreduce_adam_kernel: this rank's partials g summed with every other rank's, then Adam
 static int launch_allreduce_adam(uavrl_learner *l, const Grads &g, float *loss_out, cudaStream_t st)
 {
-    l->comm_epoch += 1;
     const int P = l->net.P;
-    const size_t stride = (size_t)P + 1;                                        // one rank's slot: gradient vector + loss share
-    const size_t parity_off = (size_t)(l->comm_epoch & 1u) * (size_t)l->world * stride;
     const AdamArgs a = adam_args(l, g, true);
     static const bool dp_trace = getenv("UAVRL_DP_TRACE") != nullptr;
     if (dp_trace && !l->dp_trace) {
         if (int rc = l->mem.alloc(l->dp_trace, 5, false)) return rc;
         UAVRL_CUDA(cudaMemsetAsync(l->dp_trace, 0, 40, st));
     }
-    UAVRL_CUDA(launch_kernel(dp_allreduce_adam_kernel, dim3((P + 63) / 64), dim3(256), 0, st, l->chain.next(kChainAdam).pdl, a,
-                             g.nparts, g.n_loss_parts, (const float *)l->partials, (const float *)l->loss_partials,
-                             (unsigned long long *const *)l->peer_grad_dev, (const unsigned long long *)l->comm_grad, stride, parity_off,
-                             l->rank, l->comm_epoch, learner_adam_ptrs(l, loss_out), l->dp_trace));
+    DpExchange x;                                                               // one rank's slot: gradient vector + loss share
+    memset(&x, 0, sizeof(x));
+    x.n_seg = 1;
+    x.seg[0].partials = l->partials; x.seg[0].nparts = g.nparts; x.seg[0].P = P; x.seg[0].blocks = (P + 63) / 64;
+    x.seg[0].q = learner_adam_ptrs(l, loss_out);
+    x.extra_parts = l->loss_partials; x.n_extra_parts = g.n_loss_parts; x.extra_stride = 1; x.n_extra = 1;
+    x.extra_scale = a.inv_b; x.extra_out = x.seg[0].q.loss_out;
+    UAVRL_CUDA(launch_dp_exchange(l->comm, a, x, st, l->chain.next(kChainAdam).pdl, l->dp_trace));
     l->chain.launched(kChainAdam);
     UAVRL_LAUNCHED();
     return 0;
@@ -825,6 +853,67 @@ static int learner_init(uavrl_learner *l, const uavrl_learner_config *cfg, int32
 
 using namespace uavrl;
 
+// ------------------------------------------------------------------ the data-parallel exchange's buffers (PeerComm)
+uavrl::PeerComm::~PeerComm()
+{
+    for (int q = 0; q < world && ready; ++q)
+        if (q != rank && peer_host[q]) cudaIpcCloseMemHandle(peer_host[q]);
+}
+
+constexpr size_t kBusIdBytes = 64;
+
+int uavrl::comm_init(PeerComm &c, int device, int32_t rank, int32_t world, size_t words, void *handle_out, bool bus_id)
+{
+    UAVRL_CUDA(cudaSetDevice(device));
+    if (!c.recv || c.recv_world != world || c.words != words) {   // first call, or re-initialised with another size
+        // recv[2][world][words] words of 8 bytes {tag : value} (tag 0 = never written)
+        DevMem m;
+        unsigned long long *recv = nullptr;
+        if (int rc = m.alloc(recv, 2 * (size_t)world * words)) return rc;
+        UAVRL_CUDA(cudaDeviceSynchronize());                     // nothing may still use the buffer being replaced
+        c.recv_mem = std::move(m);
+        c.recv = recv; c.recv_world = world; c.words = words;
+    }
+    c.rank = rank; c.world = world;
+    cudaIpcMemHandle_t hg;
+    UAVRL_CUDA(cudaIpcGetMemHandle(&hg, c.recv));
+    memcpy(handle_out, &hg, sizeof(hg));
+    if (bus_id) {
+        char id[kBusIdBytes] = { 0 };
+        UAVRL_CUDA(cudaDeviceGetPCIBusId(id, (int)kBusIdBytes - 1, device));
+        memcpy((char *)handle_out + sizeof(hg), id, kBusIdBytes);
+    }
+    return 0;
+}
+
+int uavrl::comm_connect(PeerComm &c, int device, const void *handles, bool bus_id)
+{
+    UAVRL_CUDA(cudaSetDevice(device));
+    const size_t rec = sizeof(cudaIpcMemHandle_t) + (bus_id ? kBusIdBytes : 0);
+    if (bus_id) {                               // every rank's device must differ from every other's: checked before any handle opens
+        for (int q = 0; q < c.world; ++q)
+            for (int p = 0; p < q; ++p)
+                if (!memcmp((const char *)handles + p * rec + sizeof(cudaIpcMemHandle_t),
+                            (const char *)handles + q * rec + sizeof(cudaIpcMemHandle_t), kBusIdBytes))
+                    return fail(UAVRL_ERR_INVALID, "ranks " + std::to_string(p) + " and " + std::to_string(q) +
+                                                       " share one device: each rank of the exchange needs its own GPU");
+    }
+    for (int q = 0; q < c.world; ++q) {
+        if (q == c.rank) { c.peer_host[q] = c.recv; continue; }
+        cudaIpcMemHandle_t hg;
+        memcpy(&hg, (const char *)handles + (size_t)q * rec, sizeof(hg));
+        UAVRL_CUDA(cudaIpcOpenMemHandle(&c.peer_host[q], hg, cudaIpcMemLazyEnablePeerAccess));
+    }
+    DevMem m;
+    unsigned long long **table = nullptr;
+    if (int rc = m.alloc(table, (size_t)c.world, false)) return rc;
+    UAVRL_CUDA(cudaMemcpy(table, c.peer_host, sizeof(void *) * c.world, cudaMemcpyHostToDevice));
+    c.peer_mem = std::move(m);                                   // cudaFree of the old table waits for the device
+    c.peer_dev = table;
+    c.ready = true;
+    return 0;
+}
+
 extern "C" {
 
 int uavrl_learner_create(const uavrl_learner_config *cfg, uavrl_learner **out)
@@ -853,11 +942,7 @@ int uavrl_learner_destroy(uavrl_learner *l)
         unsigned long long h[5] = { 0, 0, 0, 0, 0 };
         cudaMemcpy(h, l->dp_trace, sizeof(h), cudaMemcpyDeviceToHost);
         if (h[4]) fprintf(stderr, "[dp_trace] rank %d/%d: %llu launches, block 0 mean ns: reduce %.0f  push %.0f  wait for peers' words %.0f  adam %.0f\n",
-                          l->rank, l->world, h[4], (double)h[0] / h[4], (double)h[1] / h[4], (double)h[2] / h[4], (double)h[3] / h[4]);
-    }
-    for (int q = 0; q < l->world && l->comm_ready; ++q) {
-        if (q == l->rank) continue;
-        if (l->peer_grad_host[q]) cudaIpcCloseMemHandle(l->peer_grad_host[q]);
+                          l->comm.rank, l->comm.world, h[4], (double)h[0] / h[4], (double)h[1] / h[4], (double)h[2] / h[4], (double)h[3] / h[4]);
     }
     delete l;
     return 0;
@@ -1099,51 +1184,22 @@ int uavrl_learner_comm_init(uavrl_learner *l, int32_t rank, int32_t world, void 
     if (!l || world < 1 || world > 64 || rank < 0 || rank >= world || !grad_handle_out)
         return fail(UAVRL_ERR_INVALID, "bad rank/world/handle pointer");
     if (int rc = refuse_grouped(l, "uavrl_learner_comm_init (data-parallel training)")) return rc;
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    if (!l->comm_grad || l->comm_world != world) {               // first call, or re-initialised with another world size
-        // recv[2][world][P+1] words of 8 bytes {epoch : value} (epoch 0 = never written)
-        const size_t n = 2 * (size_t)world * ((size_t)l->net.P + 1);
-        DevMem m;
-        unsigned long long *recv = nullptr;
-        if (int rc = m.alloc(recv, n)) return rc;
-        UAVRL_CUDA(cudaDeviceSynchronize());                     // nothing may still use the buffer being replaced
-        l->comm_mem = std::move(m);
-        l->comm_grad = (float *)recv; l->comm_world = world;
-    }
-    l->rank = rank; l->world = world;
-    cudaIpcMemHandle_t hg;
-    UAVRL_CUDA(cudaIpcGetMemHandle(&hg, l->comm_grad));
-    memcpy(grad_handle_out, &hg, sizeof(hg));
-    return 0;
+    return comm_init(l->comm, l->cfg.device, rank, world, (size_t)l->net.P + 1, grad_handle_out, false);
 }
 
 int uavrl_learner_comm_connect(uavrl_learner *l, const void *grad_handles, const void *flag_handles)
 {
     (void)flag_handles;
     if (int rc = refuse_grouped(l, "uavrl_learner_comm_connect (data-parallel training)")) return rc;
-    if (!l || !grad_handles || !l->comm_grad) return fail(UAVRL_ERR_STATE, "uavrl_learner_comm_connect before comm_init");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    for (int q = 0; q < l->world; ++q) {
-        if (q == l->rank) { l->peer_grad_host[q] = l->comm_grad; continue; }
-        cudaIpcMemHandle_t hg;
-        memcpy(&hg, (const char *)grad_handles + (size_t)q * sizeof(hg), sizeof(hg));
-        UAVRL_CUDA(cudaIpcOpenMemHandle(&l->peer_grad_host[q], hg, cudaIpcMemLazyEnablePeerAccess));
-    }
-    DevMem m;
-    float **table = nullptr;
-    if (int rc = m.alloc(table, (size_t)l->world, false)) return rc;
-    UAVRL_CUDA(cudaMemcpy(table, l->peer_grad_host, sizeof(void *) * l->world, cudaMemcpyHostToDevice));
-    l->peer_mem = std::move(m);                                  // cudaFree of the old table waits for the device
-    l->peer_grad_dev = table;
-    l->comm_ready = true;
-    return 0;
+    if (!l || !grad_handles || !l->comm.recv) return fail(UAVRL_ERR_STATE, "uavrl_learner_comm_connect before comm_init");
+    return comm_connect(l->comm, l->cfg.device, grad_handles, false);
 }
 
 int uavrl_learner_update_dp(uavrl_learner *l, const int32_t *idx_tape_dev, int32_t global_batch, float *loss_dev, void *stream)
 {
     if (!l || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     if (int rc = refuse_grouped(l, "uavrl_learner_update_dp (data-parallel training)")) return rc;
-    if (!l->comm_ready) return fail(UAVRL_ERR_STATE, "uavrl_learner_update_dp before uavrl_learner_comm_connect");
+    if (!l->comm.ready) return fail(UAVRL_ERR_STATE, "uavrl_learner_update_dp before uavrl_learner_comm_connect");
     if (!l->replay.ready(l->cfg.batch_size)) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     l->epoch += 1;

@@ -109,6 +109,27 @@ __device__ __forceinline__ void fed_group_loss(const float *d2, size_t first_row
 }
 #endif
 
+// One rank's side of the data-parallel exchange (dp_allreduce_adam_kernel, learner.cu): its symmetric receive buffer
+// recv[2][world][words] of 8-byte words {exchange tag : value}, where slot q is written by rank q with remote stores, and every
+// rank's buffer as mapped on this device.  Both learners own one (uavrl_learner_comm_*, uavrl_sac_comm_*).
+struct PeerComm {
+    int32_t rank = 0, world = 1;
+    unsigned long long *recv = nullptr;
+    int32_t recv_world = 0;           // world the buffer was sized for
+    size_t words = 0;                 // words of one rank's slot: the largest exchange the owner makes
+    unsigned long long **peer_dev = nullptr;    // device array [world]
+    void *peer_host[64] = { nullptr };
+    bool ready = false;               // comm_connect has run
+    unsigned tag = 0;                 // tag of the latest exchange; 0 = never written
+    DevMem recv_mem, peer_mem;        // owners of recv and peer_dev
+    ~PeerComm();                      // closes the peers' mapped buffers
+};
+// comm_init: (re)size the receive buffer for `world` ranks of `words` words each and write its CUDA IPC handle into
+// handle_out; with bus_id, the handle is followed by this device's PCI bus id (64 bytes), which comm_connect checks: two
+// ranks on one device would spin forever in the exchange.  comm_connect: open every rank's handle (handles: [world] records).
+int comm_init(PeerComm &c, int device, int32_t rank, int32_t world, size_t words, void *handle_out, bool bus_id);
+int comm_connect(PeerComm &c, int device, const void *handles, bool bus_id);
+
 }  // namespace uavrl
 
 struct uavrl_learner {
@@ -153,18 +174,13 @@ struct uavrl_learner {
     uint64_t per_calls = 0;
     uint64_t act_calls = 0;
     uint64_t fed_calls = 0;           // ring-sampled federation calls: the Philox counter of their probe draws (federate.cu)
-    // data-parallel: one-shot NVLink all-reduce fused with Adam (symmetric buffers exchanged through CUDA IPC)
-    int32_t rank = 0, world = 1;
-    float *comm_grad = nullptr;       // own receive buffer recv[2][world][P+1]: slot q is written by rank q (remote stores)
-    int32_t comm_world = 0;
+    // data-parallel: one-shot NVLink all-reduce fused with Adam (symmetric buffers exchanged through CUDA IPC), slots of P + 1
+    // words (gradient, loss share)
+    uavrl::PeerComm comm;
     unsigned long long *dp_trace = nullptr;    // UAVRL_DP_TRACE=1: phase times of the data-parallel optimiser kernel
-    float **peer_grad_dev = nullptr;  // device array [world]: every rank's receive buffer as mapped on THIS device
-    void *peer_grad_host[64] = { nullptr };
-    bool comm_ready = false;
-    unsigned comm_epoch = 0;          // tag of the latest exchange (launch_update_dp); 0 = never written
     // owners of the buffers above, one per group allocated and replaced together: parameters, images, maps and dp_trace; the
-    // grown scratch (partials, y / astar, act / dz rows); the receive buffer; the peer table; the PER trees; their scratch
-    uavrl::DevMem mem, parts_mem, td_mem, rows_mem, comm_mem, peer_mem, per_mem, per_scratch_mem;
+    // grown scratch (partials, y / astar, act / dz rows); the PER trees; their scratch
+    uavrl::DevMem mem, parts_mem, td_mem, rows_mem, per_mem, per_scratch_mem;
 };
 
 namespace uavrl {
@@ -252,7 +268,36 @@ __device__ __forceinline__ void adam_update_pre(const AdamArgs &a, const AdamPtr
     }
 }
 
+// Sum of column j of n rows of `stride` floats, the order every scalar partial sum of an update takes: lane l adds rows l,
+// l + 32, ... in turn, then a butterfly over the warp.  Every lane of the (full) warp calls it and receives the sum.
+__device__ __forceinline__ float warp_column_sum(const float *p, int n, int stride, int j)
+{
+    float s = 0.f;
+    for (int c = threadIdx.x & 31; c < n; c += 32) s += p[(size_t)c * stride + j];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+    return s;
+}
 #endif
+
+// One exchange of dp_allreduce_adam_kernel (learner.cu): the optimiser steps of n_seg networks, segment k taking `blocks`
+// blocks of 64 parameters after segment k - 1's and words [sum of the earlier P, + P) of a rank's slot, then n_extra scalar
+// words: column j of the [n_extra_parts][extra_stride] partials, reduced by warp_column_sum and scaled, summed over ranks into
+// extra_out[j].  Every rank's slot holds the words in that order.
+struct DpSeg { const float *partials; int nparts, P, blocks; AdamPtrs q; };
+struct DpExchange {
+    DpSeg seg[2];
+    int n_seg;
+    const float *extra_parts;
+    int n_extra_parts, extra_stride, n_extra;
+    float extra_scale;
+    float *extra_out;
+};
+constexpr int kDpMaxExtra = 2;
+// the exchange x on comm (its tag advances by one) with the Adam hyper-parameters of a; trace (may be null): UAVRL_DP_TRACE
+cudaError_t launch_dp_exchange(PeerComm &comm, const AdamArgs &a, const DpExchange &x, cudaStream_t st, bool pdl,
+                               unsigned long long *trace);
+
 // reduce_adam_kernel (learner.cu) on `grid` (y: trainer) with the pointers of q; pdl: programmatic dependent launch
 cudaError_t launch_reduce_adam(dim3 grid, cudaStream_t st, bool pdl, const AdamArgs &a, const AdamPtrs &q);
 

@@ -41,6 +41,7 @@ struct SacArgs {
     NetDev actor, critic;
     BatchSrc src;
     int32_t B, n_tiles;                  // per trainer
+    int32_t Bg;                          // rows the losses average over: B, or the global batch of a data-parallel update
     int32_t gld;                         // row stride of the gradient planes (sac_gld)
     const float *img_actor, *img_c1, *img_c2, *img_t1, *img_t2;   // [G][smem_w_floats] weight images
     const float *eps;                    // [B][A] injected noise (nullptr -> Philox Box-Muller)
@@ -231,7 +232,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
     if (threadIdx.x == 0) { stage_weights(cn, sac_img<GR>(a.img_c1, cn), RC, &bar[0]); stage_weights(cn, sac_img<GR>(a.img_c2, cn), WC2, &bar[1]); }
     uint32_t pkey[4];
     Philox::gen(sac_sample_key<GR>(a), a.src.epoch, 0x5A17ull, pkey);
-    const float inv = 1.f / ((float)a.B * (float)kSacA);
+    const float inv = 1.f / ((float)a.Bg * (float)kSacA);
     float sq[2] = { 0.f, 0.f };
     bool ready = false;
     int iter = 0;
@@ -295,7 +296,7 @@ __global__ void __launch_bounds__(kNetThreads) sac_actor_kernel(SacArgs a)
     uint32_t pkey[4];
     Philox::gen(sac_sample_key<GR>(a), a.src.epoch, 0x5A17ull, pkey);
     const float alpha = expf(a.log_alpha[3 * sac_g<GR>()]);
-    const float inv = 1.f / ((float)a.B * (float)kSacA);
+    const float inv = 1.f / ((float)a.Bg * (float)kSacA);
     float loss_acc = 0.f, ent_acc = 0.f;
     bool ready = false;
     int iter = 0;
@@ -391,8 +392,11 @@ struct SacFinishArgs {
     int do_alpha;
 };
 
-// blockIdx.y = trainer g: its stat [nparts][4], scal [3], critics and targets [Pc], target images and out [4]
-__global__ void sac_finish_kernel(SacFinishArgs f, const float *__restrict__ stat, float *__restrict__ scal, const float *__restrict__ c1,
+// blockIdx.y = trainer g: its stat [nparts][4], scal [3], critics and targets [Pc], target images and out [4].  sums_c / sums_a
+// (data-parallel, one trainer): the squared-error sums / the actor-loss and entropy sums over every rank, which then replace
+// the stat partials
+__global__ void sac_finish_kernel(SacFinishArgs f, const float *__restrict__ stat, const float *__restrict__ sums_c,
+                                  const float *__restrict__ sums_a, float *__restrict__ scal, const float *__restrict__ c1,
                                   const float *__restrict__ c2, float *__restrict__ t1, float *__restrict__ t2, float *__restrict__ img_t1,
                                   float *__restrict__ img_t2, const int32_t *__restrict__ cmap, float *__restrict__ out)
 {
@@ -410,16 +414,14 @@ __global__ void sac_finish_kernel(SacFinishArgs f, const float *__restrict__ sta
     }
     if (blockIdx.x == 0 && threadIdx.x < 32) {
         // the per-CTA loss / entropy partials: lane-strided sums, then a butterfly (one thread walking all of them serially is a
-        // chain of dependent global loads)
-        float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-        for (int c = threadIdx.x; c < f.nparts; c += 32) {
-            const float4 t = *reinterpret_cast<const float4 *>(stat + 4 * c);
-            s0 += t.x; s1 += t.y; s2 += t.z; s3 += t.w;
-        }
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) {
-            s0 += __shfl_xor_sync(0xffffffffu, s0, off); s1 += __shfl_xor_sync(0xffffffffu, s1, off);
-            s2 += __shfl_xor_sync(0xffffffffu, s2, off); s3 += __shfl_xor_sync(0xffffffffu, s3, off);
+        // chain of dependent global loads).  A data-parallel exchange sums each rank's partials in this order, so one rank
+        // reads 0 + its own sums
+        float s0, s1, s2, s3;
+        if (sums_c) {
+            s0 = sums_c[0]; s1 = sums_c[1]; s2 = sums_a[0]; s3 = sums_a[1];
+        } else {
+            s0 = warp_column_sum(stat, f.nparts, 4, 0); s1 = warp_column_sum(stat, f.nparts, 4, 1);
+            s2 = warp_column_sum(stat, f.nparts, 4, 2); s3 = warp_column_sum(stat, f.nparts, 4, 3);
         }
         if (threadIdx.x != 0) return;
         // alpha_loss = mean((entropy - target_entropy).detach() * exp(log_alpha))  (:372-376), Adam on log_alpha
@@ -434,6 +436,14 @@ __global__ void sac_finish_kernel(SacFinishArgs f, const float *__restrict__ sta
         }
         if (out) { out[0] = s2 * f.inv_n; out[1] = s0 * f.inv_n; out[2] = s1 * f.inv_n; out[3] = g; }   // actor, critic1, critic2, alpha loss
     }
+}
+
+// the split data-parallel form's scalar words: columns j0 and j0 + 1 of the [nparts][4] stat partials, summed as the fused
+// exchange and sac_finish_kernel sum them
+__global__ void sac_stat_sums_kernel(const float *__restrict__ stat, int nparts, int j0, float *__restrict__ out)
+{
+    const float a = warp_column_sum(stat, nparts, 4, j0), b = warp_column_sum(stat, nparts, 4, j0 + 1);
+    if (threadIdx.x == 0) { out[0] = a; out[1] = b; }
 }
 
 // get_action (:444-448): action = actor(state)[0] with fresh noise.  Trainer blockIdx.y acts for rows [g n, (g + 1) n).
@@ -534,10 +544,10 @@ static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
     return 0;
 }
 
-static void sac_fill_args(uavrl_sac *s, SacArgs &a, const BatchSrc &src, int B, const float *eps, uint64_t ctr)
+static void sac_fill_args(uavrl_sac *s, SacArgs &a, const BatchSrc &src, int B, int Bg, const float *eps, uint64_t ctr)
 {
     memset(&a, 0, sizeof(a));
-    a.actor = s->sh.actor; a.critic = s->sh.critic; a.src = src; a.B = B; a.n_tiles = (B + kTile - 1) / kTile; a.gld = s->sh.gld;
+    a.actor = s->sh.actor; a.critic = s->sh.critic; a.src = src; a.B = B; a.Bg = Bg; a.n_tiles = (B + kTile - 1) / kTile; a.gld = s->sh.gld;
     a.img_actor = s->img[0]; a.img_c1 = s->img[1]; a.img_c2 = s->img[2]; a.img_t1 = s->img[3]; a.img_t2 = s->img[4];
     a.eps = eps; a.key = s->cfg.seed ^ kNoiseSalt; a.ctr = ctr; a.log_alpha = s->scal; a.td = s->td;
     a.part_a = s->part[0]; a.part_c1 = s->part[1]; a.part_c2 = s->part[2]; a.stat = s->stat;
@@ -579,7 +589,7 @@ int uavrl::launch_sac_act(uavrl_sac *s, const float *obs, int n, const float *ep
     BatchSrc none;
     memset(&none, 0, sizeof(none));
     const int ng = n / s->G;                                   // rows per trainer: block g belongs to trainer g
-    sac_fill_args(s, a, none, ng, eps, 0x8000000000000000ull | s->calls++);
+    sac_fill_args(s, a, none, ng, ng, eps, 0x8000000000000000ull | s->calls++);
     const int grid = a.n_tiles < s->max_ctas ? a.n_tiles : s->max_ctas;
     if (s->G > 1) sac_act_kernel<true><<<dim3(grid, s->G), kNetThreads, smem_act(s->sh), st>>>(a, obs, ng, actions);
     else sac_act_kernel<false><<<grid, kNetThreads, smem_act(s->sh), st>>>(a, obs, ng, actions);
@@ -587,49 +597,119 @@ int uavrl::launch_sac_act(uavrl_sac *s, const float *obs, int n, const float *ep
     return 0;
 }
 
-int uavrl::launch_sac_update(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev,
-                             cudaStream_t st)
+static int sac_grid(const uavrl_sac *s, int B)
 {
     const int n_tiles = (B + kTile - 1) / kTile;
-    const int grid = n_tiles < s->max_ctas ? n_tiles : s->max_ctas;
+    return n_tiles < s->max_ctas ? n_tiles : s->max_ctas;
+}
+
+// The update's first half on B rows per trainer (losses averaged over Bg rows): one Adam step counted, the TD targets, both
+// critics' gradient partials and squared-error sums
+static int sac_critic_phase(uavrl_sac *s, const BatchSrc &src, int B, int Bg, const float *eps_next, cudaStream_t st)
+{
+    const int grid = sac_grid(s, B);
     int rc = sac_scratch(s, B, grid, st);
     if (rc) return rc;
     const dim3 tiles(grid, s->G);                        // y: trainer
     SacArgs a;
     s->adam_t += 1;
-    sac_fill_args(s, a, src, B, eps_next, 2 * (uint64_t)s->epoch);
+    sac_fill_args(s, a, src, B, Bg, eps_next, 2 * (uint64_t)s->epoch);
     if (s->G > 1) sac_target_kernel<true><<<tiles, kNetThreads, smem_target(s->sh), st>>>(a);
     else sac_target_kernel<false><<<grid, kNetThreads, smem_target(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
     if (s->G > 1) sac_critic_kernel<true><<<tiles, kNetThreads, smem_critic(s->sh), st>>>(a);
     else sac_critic_kernel<false><<<grid, kNetThreads, smem_critic(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
-    AdamArgs aa;
-    for (int c = 1; c <= 2; ++c) {
-        adam_args(aa, s->sh.critic, grid, s->cfg.critic_lr, s->adam_t);
-        UAVRL_CUDA(launch_reduce_adam(dim3((aa.P + 63) / 64, s->G), st, false, aa, sac_adam_ptrs(s, c)));
-        UAVRL_LAUNCHED();
-    }
-    sac_fill_args(s, a, src, B, eps_cur, 2 * (uint64_t)s->epoch + 1);
-    if (s->G > 1) sac_actor_kernel<true><<<tiles, kNetThreads, smem_actor(s->sh), st>>>(a);
+    return 0;
+}
+
+// the second half, after the critics' step: the actor's gradient partials, loss and entropy sums on the same rows
+static int sac_actor_phase(uavrl_sac *s, const BatchSrc &src, int B, int Bg, const float *eps_cur, cudaStream_t st)
+{
+    const int grid = sac_grid(s, B);
+    SacArgs a;
+    sac_fill_args(s, a, src, B, Bg, eps_cur, 2 * (uint64_t)s->epoch + 1);
+    if (s->G > 1) sac_actor_kernel<true><<<dim3(grid, s->G), kNetThreads, smem_actor(s->sh), st>>>(a);
     else sac_actor_kernel<false><<<grid, kNetThreads, smem_actor(s->sh), st>>>(a);
-    UAVRL_LAUNCHED();
-    adam_args(aa, s->sh.actor, grid, s->cfg.actor_lr, s->adam_t);
-    UAVRL_CUDA(launch_reduce_adam(dim3((aa.P + 63) / 64, s->G), st, false, aa, sac_adam_ptrs(s, 0)));
-    UAVRL_LAUNCHED();
-    SacFinishArgs f;
-    memset(&f, 0, sizeof(f));
-    f.Pc = s->sh.critic.P; f.nparts = grid; f.img_floats = s->sh.critic.smem_w_floats;
-    f.tau = s->cfg.tau; f.alpha_lr = s->cfg.alpha_lr; f.target_entropy = s->cfg.target_entropy;
-    f.inv_n = 1.f / ((float)B * (float)kSacA); f.do_alpha = 1;
-    adam_hyper(aa, s->cfg.alpha_lr, s->adam_t);                    // the alpha step's bias corrections
-    f.step_size_scale = aa.step_size; f.bc2_sqrt = aa.bc2_sqrt;
-    sac_finish_kernel<<<dim3((f.Pc + 255) / 256, s->G), 256, 0, st>>>(f, s->stat, s->scal, s->p[1], s->p[2], s->p[3], s->p[4], s->img[3],
-                                                                     s->img[4], s->map_c, losses_dev ? losses_dev : s->out);
     UAVRL_LAUNCHED();
     return 0;
 }
 
+// reduce_adam_kernel on network r (0 actor, 1 and 2 the critics): reduce the grid's partials and step (nparts > 0, apply),
+// reduce only (apply false), or step on the gradient the caller all-reduced (nparts = 0)
+static int sac_reduce_adam(uavrl_sac *s, int r, int nparts, bool apply, cudaStream_t st)
+{
+    AdamArgs aa;
+    adam_args(aa, r == 0 ? s->sh.actor : s->sh.critic, nparts, r == 0 ? s->cfg.actor_lr : s->cfg.critic_lr, s->adam_t);
+    aa.apply = apply ? 1 : 0;
+    UAVRL_CUDA(launch_reduce_adam(dim3((aa.P + 63) / 64, s->G), st, false, aa, sac_adam_ptrs(s, r)));
+    UAVRL_LAUNCHED();
+    return 0;
+}
+
+// alpha step, soft target update and losses over Bg rows; exchanged: the stat sums are the exchange vectors' scalar words
+static int sac_finish(uavrl_sac *s, int grid, int Bg, bool exchanged, float *losses_dev, cudaStream_t st)
+{
+    SacFinishArgs f;
+    memset(&f, 0, sizeof(f));
+    f.Pc = s->sh.critic.P; f.nparts = grid; f.img_floats = s->sh.critic.smem_w_floats;
+    f.tau = s->cfg.tau; f.alpha_lr = s->cfg.alpha_lr; f.target_entropy = s->cfg.target_entropy;
+    f.inv_n = 1.f / ((float)Bg * (float)kSacA); f.do_alpha = 1;
+    AdamArgs aa;
+    adam_hyper(aa, s->cfg.alpha_lr, s->adam_t);                    // the alpha step's bias corrections
+    f.step_size_scale = aa.step_size; f.bc2_sqrt = aa.bc2_sqrt;
+    const float *sums_c = exchanged ? s->xc + 2 * (size_t)s->sh.critic.P : nullptr, *sums_a = exchanged ? s->xa + s->sh.actor.P : nullptr;
+    sac_finish_kernel<<<dim3((f.Pc + 255) / 256, s->G), 256, 0, st>>>(f, s->stat, sums_c, sums_a, s->scal, s->p[1], s->p[2], s->p[3], s->p[4],
+                                                                     s->img[3], s->img[4], s->map_c, losses_dev ? losses_dev : s->out);
+    UAVRL_LAUNCHED();
+    return 0;
+}
+
+int uavrl::launch_sac_update(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev,
+                             cudaStream_t st)
+{
+    const int grid = sac_grid(s, B);
+    int rc;
+    if ((rc = sac_critic_phase(s, src, B, B, eps_next, st)) || (rc = sac_reduce_adam(s, 1, grid, true, st)) ||
+        (rc = sac_reduce_adam(s, 2, grid, true, st)) || (rc = sac_actor_phase(s, src, B, B, eps_cur, st)) ||
+        (rc = sac_reduce_adam(s, 0, grid, true, st)))
+        return rc;
+    return sac_finish(s, grid, B, false, losses_dev, st);
+}
+
+// One fused exchange (dp_allreduce_adam_kernel) of this rank's gradients and stat sums: critics = both critics' gradients and
+// squared-error sums into xc, else the actor's gradient and its loss / entropy sums into xa; then Adam on those networks
+static int sac_exchange(uavrl_sac *s, bool critics, int grid, cudaStream_t st)
+{
+    const NetDev &n = critics ? s->sh.critic : s->sh.actor;
+    AdamArgs aa;
+    adam_args(aa, n, grid, critics ? s->cfg.critic_lr : s->cfg.actor_lr, s->adam_t);
+    aa.world = s->comm.world;
+    DpExchange x;
+    memset(&x, 0, sizeof(x));
+    x.n_seg = critics ? 2 : 1;
+    for (int k = 0; k < x.n_seg; ++k) {
+        const int r = critics ? 1 + k : 0;
+        x.seg[k].partials = s->part[r]; x.seg[k].nparts = grid; x.seg[k].P = n.P; x.seg[k].blocks = (n.P + 63) / 64;
+        x.seg[k].q = sac_adam_ptrs(s, r);
+    }
+    x.extra_parts = s->stat + (critics ? 0 : 2); x.n_extra_parts = grid; x.extra_stride = 4; x.n_extra = 2; x.extra_scale = 1.f;
+    x.extra_out = critics ? s->xc + 2 * (size_t)n.P : s->xa + n.P;
+    UAVRL_CUDA(launch_dp_exchange(s->comm, aa, x, st, false, nullptr));
+    UAVRL_LAUNCHED();
+    return 0;
+}
+
+int uavrl::launch_sac_update_dp(uavrl_sac *s, const BatchSrc &src, int B, int global_batch, const float *eps_next, const float *eps_cur,
+                                float *losses_dev, cudaStream_t st)
+{
+    const int grid = sac_grid(s, B);
+    int rc;
+    if ((rc = sac_critic_phase(s, src, B, global_batch, eps_next, st)) || (rc = sac_exchange(s, true, grid, st)) ||
+        (rc = sac_actor_phase(s, src, B, global_batch, eps_cur, st)) || (rc = sac_exchange(s, false, grid, st)))
+        return rc;
+    return sac_finish(s, grid, global_batch, true, losses_dev, st);
+}
 
 // everything a learner allocates; on failure the caller destroys the half-built handle
 static int sac_alloc(uavrl_sac *s)
@@ -644,8 +724,11 @@ static int sac_alloc(uavrl_sac *s)
     }
     for (int r = 0; r < 3; ++r) {
         const NetDev &n = r == 0 ? s->sh.actor : s->sh.critic;
-        if ((rc = mem.alloc(s->m[r], G * n.P)) || (rc = mem.alloc(s->v[r], G * n.P)) || (rc = mem.alloc(s->grad[r], G * n.P))) return rc;
+        if ((rc = mem.alloc(s->m[r], G * n.P)) || (rc = mem.alloc(s->v[r], G * n.P))) return rc;
     }
+    const size_t Pa = (size_t)s->sh.actor.P, Pc = (size_t)s->sh.critic.P;
+    if ((rc = mem.alloc(s->xa, G * Pa + 2)) || (rc = mem.alloc(s->xc, 2 * G * Pc + 2))) return rc;
+    s->grad[0] = s->xa; s->grad[1] = s->xc; s->grad[2] = s->xc + G * Pc;
     std::vector<int32_t> ma, mc;
     build_image_map(s->sh.actor, ma); build_image_map(s->sh.critic, mc);
     if ((rc = mem.alloc(s->map_a, ma.size())) || (rc = mem.alloc(s->map_c, mc.size()))) return rc;
@@ -860,6 +943,147 @@ int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
     sac_federate_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, s->G, s->p[0]);
     UAVRL_LAUNCHED();
     return sac_pack(s, 0, st);                                 // the G actor images
+}
+
+
+// ------------------------------------------------------------------ data-parallel training
+// entry points a grouped learner does not offer, and the refusals every data-parallel update makes before its epoch counts
+static int sac_refuse_grouped(const uavrl_sac *s, const char *fn)
+{
+    if (s->G > 1) return fail(UAVRL_ERR_INVALID, std::string(fn) + " is not available on a learner with " + std::to_string(s->G) + " trainers");
+    return 0;
+}
+
+static int sac_dp_checks(const uavrl_sac *s, int32_t global_batch, bool ring, const char *fn)
+{
+    if (int rc = sac_refuse_grouped(s, fn)) return rc;
+    if (global_batch <= 0) return fail(UAVRL_ERR_INVALID, std::string(fn) + ": global_batch must be > 0");
+    if (s->dp_phase != 0) return fail(UAVRL_ERR_STATE, std::string(fn) + " while a split update waits for its next phase");
+    if (ring && !s->replay.frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
+    // every rank must take part in every exchange, and a rank that retries stays on the other ranks' sample keys
+    if (ring && !s->replay.ready(s->cfg.batch_size)) return fail(UAVRL_ERR_STATE, "replay holds <= batch_size transitions");
+    return 0;
+}
+
+int uavrl_sac_comm_init(uavrl_sac *s, int32_t rank, int32_t world, void *handle_out)
+{
+    if (!s || world < 1 || world > 64 || rank < 0 || rank >= world || !handle_out) return fail(UAVRL_ERR_INVALID, "bad rank/world/handle pointer");
+    if (int rc = sac_refuse_grouped(s, "uavrl_sac_comm_init")) return rc;
+    const size_t Pa = (size_t)s->sh.actor.P, Pc = (size_t)s->sh.critic.P;
+    return comm_init(s->comm, s->cfg.device, rank, world, 2 * Pc + 2 > Pa + 2 ? 2 * Pc + 2 : Pa + 2, handle_out, true);
+}
+
+int uavrl_sac_comm_connect(uavrl_sac *s, const void *handles)
+{
+    if (!s || !handles) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = sac_refuse_grouped(s, "uavrl_sac_comm_connect")) return rc;
+    if (!s->comm.recv) return fail(UAVRL_ERR_STATE, "uavrl_sac_comm_connect before uavrl_sac_comm_init");
+    return comm_connect(s->comm, s->cfg.device, handles, true);
+}
+
+int uavrl_sac_update_replay_dp(uavrl_sac *s, const int32_t *idx_tape_dev, const float *eps_next_dev, const float *eps_cur_dev,
+                               int32_t global_batch, float *losses_dev, void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (int rc = sac_dp_checks(s, global_batch, true, "uavrl_sac_update_replay_dp")) return rc;
+    if (!s->comm.ready) return fail(UAVRL_ERR_STATE, "uavrl_sac_update_replay_dp before uavrl_sac_comm_connect");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    s->epoch += 1;                                             // SAC_Trainer.py:320
+    return launch_sac_update_dp(s, s->replay.source(s->cfg.seed, s->epoch, idx_tape_dev), s->cfg.batch_size, global_batch, eps_next_dev,
+                                eps_cur_dev, losses_dev, (cudaStream_t)stream);
+}
+
+// the split form's critic phase on src: the critics' gradients and squared-error sums into the critic exchange vector
+static int sac_split_critic(uavrl_sac *s, const BatchSrc &src, int B, int global_batch, const float *eps_next, cudaStream_t st)
+{
+    s->dp_src = src; s->dp_B = B; s->dp_global = global_batch;
+    const int grid = sac_grid(s, B);
+    int rc;
+    if ((rc = sac_critic_phase(s, src, B, global_batch, eps_next, st)) || (rc = sac_reduce_adam(s, 1, grid, false, st)) ||
+        (rc = sac_reduce_adam(s, 2, grid, false, st)))
+        return rc;
+    sac_stat_sums_kernel<<<1, 32, 0, st>>>(s->stat, grid, 0, s->xc + 2 * (size_t)s->sh.critic.P);
+    UAVRL_LAUNCHED();
+    s->dp_phase = 1;
+    return 0;
+}
+
+int uavrl_sac_critic_grads_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const float *eps_next_dev, int32_t global_batch, void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (int rc = sac_dp_checks(s, global_batch, true, "uavrl_sac_critic_grads_replay")) return rc;
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    s->epoch += 1;
+    return sac_split_critic(s, s->replay.source(s->cfg.seed, s->epoch, idx_tape_dev), s->cfg.batch_size, global_batch, eps_next_dev,
+                            (cudaStream_t)stream);
+}
+
+int uavrl_sac_critic_grads_batch(uavrl_sac *s, int32_t B, const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev,
+                                 const float *d_dev, const float *eps_next_dev, int32_t global_batch, void *stream)
+{
+    if (!s || B <= 0 || !s_dev || !a_dev || !r_dev || !s2_dev || !d_dev) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = sac_dp_checks(s, global_batch, false, "uavrl_sac_critic_grads_batch")) return rc;
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    s->epoch += 1;
+    BatchSrc src;
+    memset(&src, 0, sizeof(src));
+    src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.act2 = a_dev; src.rew = r_dev; src.done_f32 = d_dev;
+    return sac_split_critic(s, src, B, global_batch, eps_next_dev, (cudaStream_t)stream);
+}
+
+static int sac_phase_is(const uavrl_sac *s, int phase, const char *fn)
+{
+    if (int rc = sac_refuse_grouped(s, fn)) return rc;
+    static const char *want[4] = { "", "after uavrl_sac_critic_grads_*", "after uavrl_sac_apply_critic_grads", "after uavrl_sac_actor_grads" };
+    if (s->dp_phase != phase) return fail(UAVRL_ERR_STATE, std::string(fn) + " called out of order: it runs " + want[phase]);
+    return 0;
+}
+
+int uavrl_sac_apply_critic_grads(uavrl_sac *s, void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (int rc = sac_phase_is(s, 1, "uavrl_sac_apply_critic_grads")) return rc;
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if ((rc = sac_reduce_adam(s, 1, 0, true, st)) || (rc = sac_reduce_adam(s, 2, 0, true, st))) return rc;
+    s->dp_phase = 2;
+    return 0;
+}
+
+int uavrl_sac_actor_grads(uavrl_sac *s, const float *eps_cur_dev, void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (int rc = sac_phase_is(s, 2, "uavrl_sac_actor_grads")) return rc;
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int grid = sac_grid(s, s->dp_B);
+    int rc;
+    if ((rc = sac_actor_phase(s, s->dp_src, s->dp_B, s->dp_global, eps_cur_dev, st)) || (rc = sac_reduce_adam(s, 0, grid, false, st)))
+        return rc;
+    sac_stat_sums_kernel<<<1, 32, 0, st>>>(s->stat, grid, 2, s->xa + s->sh.actor.P);
+    UAVRL_LAUNCHED();
+    s->dp_phase = 3;
+    return 0;
+}
+
+int uavrl_sac_apply_actor_grads(uavrl_sac *s, float *losses_dev, void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (int rc = sac_phase_is(s, 3, "uavrl_sac_apply_actor_grads")) return rc;
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if ((rc = sac_reduce_adam(s, 0, 0, true, st)) || (rc = sac_finish(s, sac_grid(s, s->dp_B), s->dp_global, true, losses_dev, st))) return rc;
+    s->dp_phase = 0;
+    return 0;
+}
+
+float *uavrl_sac_exchange_ptr(uavrl_sac *s, int32_t phase, int64_t *len_out)
+{
+    if (!s || (phase != 0 && phase != 1)) return nullptr;
+    if (len_out) *len_out = phase == 0 ? 2 * (int64_t)s->sh.critic.P + 2 : (int64_t)s->sh.actor.P + 2;
+    return phase == 0 ? s->xc : s->xa;
 }
 
 }  // extern "C"

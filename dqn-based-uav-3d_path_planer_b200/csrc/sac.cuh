@@ -15,6 +15,10 @@ struct uavrl_sac {
     int32_t G = 1;
     float *p[5] = { nullptr }, *img[5] = { nullptr };      // actor, c1, c2, t1, t2
     float *m[3] = { nullptr }, *v[3] = { nullptr }, *grad[3] = { nullptr };
+    // the data-parallel exchange vectors, one per phase of an update: xc = [grad c1 | grad c2 | critic-1, critic-2 squared-error
+    // sums], xa = [grad actor | actor-loss sum, entropy sum] (grad[r] point into them; with G > 1 the gradients are [G][P] and
+    // only a one-trainer learner exchanges)
+    float *xc = nullptr, *xa = nullptr;
     int32_t *map_a = nullptr, *map_c = nullptr;
     float *part[3] = { nullptr };                          // gradient partials [G][parts_cap][P]
     float *stat = nullptr, *out = nullptr, *td = nullptr, *lossbuf = nullptr;   // [G][parts_cap][4], [G][4], [G][td_cap][2]
@@ -23,6 +27,11 @@ struct uavrl_sac {
     int64_t epoch = 0, adam_t = 0;
     uint64_t calls = 0;
     uavrl::ReplayStore replay;                             // lockstep ring (float[2] actions); none when lockstep_envs == 0
+    // data-parallel training: the fused exchange's buffers (slots of max(2 Pc + 2, Pa + 2) words), and the split form's
+    // phase (0 none, 1 critic gradients written, 2 critics stepped, 3 actor gradients written) with the batch it runs on
+    uavrl::PeerComm comm;
+    int32_t dp_phase = 0, dp_B = 0, dp_global = 0;
+    uavrl::BatchSrc dp_src;
     uavrl::DevMem mem, parts_mem, td_mem;                  // owners: networks, moments, maps, scalars; partials / stat; td
 };
 
@@ -34,4 +43,8 @@ int launch_sac_act(uavrl_sac *s, const float *obs, int n, const float *eps, floa
 // learner's own out) receives [G][4]
 int launch_sac_update(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev,
                       cudaStream_t st);
+// the data-parallel form over global_batch rows (B on this rank): the critics' gradients and squared-error sums go through one
+// fused exchange + Adam, then the actor's gradient, loss and entropy sums through a second; every rank ends bit-identical
+int launch_sac_update_dp(uavrl_sac *s, const BatchSrc &src, int B, int global_batch, const float *eps_next, const float *eps_cur,
+                         float *losses_dev, cudaStream_t st);
 }  // namespace uavrl

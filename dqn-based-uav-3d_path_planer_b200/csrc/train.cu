@@ -1,5 +1,6 @@
 // train.cu -- the fused lockstep training loops over the env batch and a learner: the Q-network learner's (uavrl_train_run,
-// uavrl_train_run_dp, uavrl_train_profile) and the SAC learner's (uavrl_sac_train_run) run the same iteration.
+// uavrl_train_run_dp, uavrl_train_profile) and the SAC learner's (uavrl_sac_train_run, uavrl_sac_train_run_dp) run the same
+// iteration.
 //
 // Replaces PathPlan_City.run_thread_OffPolicy + PathPlan_City.update (Envs/PathPlan_City.py:364-385,
 // 757-776) for N envs: state -> get_action -> Move_Agent -> replay add -> sample -> Trainer.update.
@@ -17,9 +18,11 @@ using namespace uavrl;
 enum Loop { kLoopRun, kLoopDp, kLoopProfile };
 
 // ------------------------------------------------------------------ what the loop does differently per learner
-// uavrl_learner_comm_connect has run: the data-parallel loop's precondition (there is no data-parallel SAC loop)
-static bool connected(const uavrl_learner *l) { return l->comm_ready; }
-static bool connected(const uavrl_sac *) { return false; }
+// uavrl_learner_comm_connect / uavrl_sac_comm_connect has run: the data-parallel loop's precondition
+static bool connected(const uavrl_learner *l) { return l->comm.ready; }
+static bool connected(const uavrl_sac *s) { return s->comm.ready; }
+static const char *connect_fn(const uavrl_learner *) { return "uavrl_learner_comm_connect"; }
+static const char *connect_fn(const uavrl_sac *) { return "uavrl_sac_comm_connect"; }
 
 // get_action on the ring's current frame: Choose_Action2 -> Trainer.get_action (PathPlan_City.py:338-346)
 static int act(uavrl_learner *l, const ReplayStore::Iteration &io, int n, float eps, cudaStream_t st)
@@ -56,9 +59,11 @@ static int update(uavrl_learner *l, const BatchSrc &src, int dp_batch, cudaStrea
     const int B = l->cfg.batch_size;
     return dp_batch > 0 ? launch_update_dp(l, src, B, dp_batch, l->loss_dev, st) : launch_update(l, src, B, B, l->loss_dev, true, st, marks);
 }
-static int update(uavrl_sac *s, const BatchSrc &src, int, cudaStream_t st, cudaEvent_t *)
+static int update(uavrl_sac *s, const BatchSrc &src, int dp_batch, cudaStream_t st, cudaEvent_t *)
 {
-    return launch_sac_update(s, src, s->cfg.batch_size, nullptr, nullptr, nullptr, st);
+    const int B = s->cfg.batch_size;
+    return dp_batch > 0 ? launch_sac_update_dp(s, src, B, dp_batch, nullptr, nullptr, nullptr, st)
+                        : launch_sac_update(s, src, B, nullptr, nullptr, nullptr, st);
 }
 
 // where each trainer's loss of its last update lives: element 0 of [G][stride] device floats
@@ -74,11 +79,11 @@ static int check_loop(const uavrl_env *env, const Learner *l, Loop loop, int32_t
 {
     const ReplayStore &rs = l->replay;
     const bool paired = rs.mode == kReplayLockstep && l->cfg.lockstep_envs == env->d.n;
-    if (loop == kLoopDp && l->G > 1) return fail(UAVRL_ERR_INVALID, "uavrl_train_run_dp is not available on a learner with several trainers");
+    if (loop == kLoopDp && l->G > 1) return fail(UAVRL_ERR_INVALID, std::string(fn) + " is not available on a learner with several trainers");
     if (loop != kLoopProfile && !paired) return fail(UAVRL_ERR_INVALID, "learner.lockstep_envs must equal env.n_envs");
     // the env step writes kObsDim floats per env into the ring's frames
     if (rs.in_dim != kObsDim) return fail(UAVRL_ERR_INVALID, "learner.in_dim must be 100 (the UAV observation)");
-    if (loop == kLoopDp && !connected(l)) return fail(UAVRL_ERR_STATE, "uavrl_train_run_dp before uavrl_learner_comm_connect");
+    if (loop == kLoopDp && !connected(l)) return fail(UAVRL_ERR_STATE, std::string(fn) + " before " + connect_fn(l));
     if (loop != kLoopProfile && !env->reset_done) return fail(UAVRL_ERR_STATE, std::string(fn) + " before uavrl_env_reset");
     if (env->cfg.device != l->cfg.device) return fail(UAVRL_ERR_INVALID, "env and learner live on different devices");
     if (loop == kLoopProfile && (!paired || !env->reset_done || !rs.frame0_valid))
@@ -163,17 +168,30 @@ extern "C" int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters
     return run(env, s, "uavrl_sac_train_run", n_iters, 0.f, do_update ? 1 : 0, stats_host, stream);
 }
 
-extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, int32_t global_batch, void *stream)
+// n_iters iterations whose update is the data-parallel one over global_batch
+template <class Learner>
+static int run_dp(uavrl_env *env, Learner *l, const char *fn, int32_t n_iters, float eps, int32_t global_batch, void *stream)
 {
-    if (!env || !l || n_iters < 0 || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
     int rc;
-    if ((rc = check_loop(env, l, kLoopDp, n_iters, "uavrl_train_run_dp"))) return rc;
+    if ((rc = check_loop(env, l, kLoopDp, n_iters, fn))) return rc;
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
-    ChainScope chain(l->chain);
     int64_t updates = 0;
     for (int it = 0; it < n_iters; ++it)
         if ((rc = iteration(env, l, eps, 1, global_batch, (cudaStream_t)stream, nullptr, updates))) return rc;
     return 0;
+}
+
+extern "C" int uavrl_train_run_dp(uavrl_env *env, uavrl_learner *l, int32_t n_iters, float eps, int32_t global_batch, void *stream)
+{
+    if (!env || !l || n_iters < 0 || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    ChainScope chain(l->chain);
+    return run_dp(env, l, "uavrl_train_run_dp", n_iters, eps, global_batch, stream);
+}
+
+extern "C" int uavrl_sac_train_run_dp(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t global_batch, void *stream)
+{
+    if (!env || !s || n_iters < 0 || global_batch <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    return run_dp(env, s, "uavrl_sac_train_run_dp", n_iters, 0.f, global_batch, stream);
 }
 
 // the loop of uavrl_train_run with the chain off and an event between every two kernels

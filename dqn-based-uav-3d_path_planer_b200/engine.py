@@ -455,24 +455,20 @@ class Learner:
         arr = (C.c_float * self.P).from_address(ptr) if False else None  # noqa: F841 (device memory: no host view)
         return _DevView(ptr, self.P, self.device).tensor()
 
+    def _comm(self):
+        lib = _lib.lib()
+        return (64, lambda rank, world, h: lib.uavrl_learner_comm_init(self.h, rank, world, h, None),
+                lambda handles: lib.uavrl_learner_comm_connect(self.h, handles, None))
+
     def connect_peers(self, dist, rank, world):
         """Exchange the CUDA IPC handles of the symmetric gradient receive buffers over torch.distributed and map
         every peer's buffer (NVLink P2P) -- enables update_dp(), the fused one-shot all-reduce + Adam."""
-        hg = (C.c_ubyte * 64)()
-        check(_lib.lib().uavrl_learner_comm_init(self.h, rank, world, hg, None))
-        mine = torch.tensor(list(bytes(hg)), dtype=torch.uint8, device=self.device)
-        allh = [torch.zeros_like(mine) for _ in range(world)]
-        dist.all_gather(allh, mine)
-        g = np.ascontiguousarray(torch.stack(allh).cpu().numpy())
-        check(_lib.lib().uavrl_learner_comm_connect(self.h, _ptr(g), None))
-        dist.barrier(device_ids=[self.device.index])
+        _connect_peers(dist, rank, world, self.device, *self._comm())
 
     def connect_self(self):
         """world = 1: the data-parallel optimiser kernel (push into the local receive buffer, gather, all-reduce + Adam) on
         one GPU -- the self-test of the fused path that needs no second device."""
-        hg = (C.c_ubyte * 64)()
-        check(_lib.lib().uavrl_learner_comm_init(self.h, 0, 1, hg, None))
-        check(_lib.lib().uavrl_learner_comm_connect(self.h, hg, None))
+        _connect_peers(None, 0, 1, self.device, *self._comm())
 
     def update_dp(self, global_batch, idx_tape=None, loss=None):
         check(_lib.lib().uavrl_learner_update_dp(self.h, _ptr(idx_tape), int(global_batch), _ptr(loss), _stream(self.device)))
@@ -509,6 +505,23 @@ class Learner:
     def set_is_train(self, is_train):
         """Trainer.Is_Train for the lockstep loops: False = get_action is always greedy (DuelingDQN_Trainer.py:90)."""
         check(_lib.lib().uavrl_learner_set_is_train(self.h, int(bool(is_train))))
+
+
+def _connect_peers(dist, rank, world, device, nbytes, init, connect):
+    """The handle exchange of the fused data-parallel optimiser, shared by Learner and SacLearner: init(rank, world, buf)
+    writes this rank's nbytes-byte record (the CUDA IPC handle of its receive buffer, ...), every rank's record is gathered
+    over torch.distributed in rank order, connect(records) maps every peer's buffer.  dist = None: world 1, no peers."""
+    mine = (C.c_ubyte * nbytes)()
+    check(init(rank, world, mine))
+    if dist is None:
+        check(connect(mine))
+        return
+    t = torch.tensor(list(bytes(mine)), dtype=torch.uint8, device=device)
+    allh = [torch.zeros_like(t) for _ in range(world)]
+    dist.all_gather(allh, t)
+    g = np.ascontiguousarray(torch.stack(allh).cpu().numpy())
+    check(connect(_ptr(g)))
+    dist.barrier(device_ids=[device.index])
 
 
 class _DevView:
@@ -685,6 +698,60 @@ class SacLearner:
         check(_lib.lib().uavrl_sac_update_replay(self.h, _ptr(idx_tape), _ptr(eps_next), _ptr(eps_cur), self._losses(losses),
                                                  _stream(self.device)))
 
+    # -- data-parallel training (include/uavrl.h, uavrl_sac_comm_init .. uavrl_sac_train_run_dp): one learner per GPU
+    def _comm(self):
+        lib = _lib.lib()
+        return (_lib.SAC_COMM_HANDLE_BYTES, lambda rank, world, h: lib.uavrl_sac_comm_init(self.h, rank, world, h),
+                lambda handles: lib.uavrl_sac_comm_connect(self.h, handles))
+
+    def connect_peers(self, dist, rank, world):
+        """Exchange every rank's receive-buffer handle and device over torch.distributed and map the peers' buffers: enables
+        update_replay_dp() and sac_train_run_dp(), two fused all-reduce + Adam exchanges per update.  Every rank needs its own
+        GPU (refused otherwise)."""
+        _connect_peers(dist, rank, world, self.device, *self._comm())
+
+    def connect_self(self):
+        """world = 1: the fused data-parallel update on one GPU (each exchange pushes into and gathers from the local buffer)."""
+        _connect_peers(None, 0, 1, self.device, *self._comm())
+
+    def update_replay_dp(self, global_batch, idx_tape=None, eps_next=None, eps_cur=None, losses=None):
+        """One data-parallel update from this rank's ring: losses averaged over global_batch rows, gradients and loss sums
+        summed over the ranks by the fused exchanges."""
+        check(_lib.lib().uavrl_sac_update_replay_dp(self.h, _ptr(idx_tape), _ptr(eps_next), _ptr(eps_cur), int(global_batch),
+                                                    self._losses(losses), _stream(self.device)))
+
+    def critic_grads(self, global_batch, batch=None, idx_tape=None, eps_next=None):
+        """Split form, phase 1: epoch += 1, then the critics' gradients and squared-error sums on batch = (s, a, r, s2, d)
+        device tensors (kept alive until actor_grads) or, with batch None, on rows sampled from the ring; they land in
+        exchange_tensor(0), which the caller sums over the ranks before apply_critic_grads()."""
+        st = _stream(self.device)
+        if batch is None:
+            check(_lib.lib().uavrl_sac_critic_grads_replay(self.h, _ptr(idx_tape), _ptr(eps_next), int(global_batch), st))
+        else:
+            s, a, r, s2, d = batch
+            check(_lib.lib().uavrl_sac_critic_grads_batch(self.h, s.shape[0], _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d),
+                                                          _ptr(eps_next), int(global_batch), st))
+
+    def apply_critic_grads(self):
+        check(_lib.lib().uavrl_sac_apply_critic_grads(self.h, _stream(self.device)))
+
+    def actor_grads(self, eps_cur=None):
+        """Split form, phase 3: the actor leg on the same rows with the stepped critics, into exchange_tensor(1)."""
+        check(_lib.lib().uavrl_sac_actor_grads(self.h, _ptr(eps_cur), _stream(self.device)))
+
+    def apply_actor_grads(self, losses=None):
+        """Split form, phase 4: the actor's Adam step, the alpha step, the soft target update and the global losses."""
+        check(_lib.lib().uavrl_sac_apply_actor_grads(self.h, self._losses(losses), _stream(self.device)))
+
+    def exchange_tensor(self, phase):
+        """The device vector a phase exchanges, as a torch view: 0 = [grad critic_1 | grad critic_2 | their squared-error
+        sums] (2 Pc + 2 floats), 1 = [grad actor | actor-loss sum, entropy sum] (Pa + 2)."""
+        n = C.c_int64()
+        ptr = _lib.lib().uavrl_sac_exchange_ptr(self.h, int(phase), C.byref(n))
+        if not ptr:
+            raise ValueError("phase must be 0 (critics) or 1 (actor)")
+        return _DevView(ptr, n.value, self.device).tensor()
+
 
 def sac_smem_bytes(obs_dim, hidden, device=0):
     """Shared memory (dynamic + static bytes) one block of each SAC kernel takes for these networks: [target, critic update,
@@ -701,3 +768,9 @@ def sac_train_run(env, sac, n_iters, do_update=True, want_stats=True):
     check(_lib.lib().uavrl_sac_train_run(env.h, sac.h, int(n_iters), int(bool(do_update)), C.byref(st) if want_stats else None,
                                          _stream(env.device)))
     return st
+
+
+def sac_train_run_dp(env, sac, n_iters, global_batch):
+    """uavrl_sac_train_run_dp: lockstep iterations whose update is the fused data-parallel SAC update (after connect_peers
+    or connect_self; warm the ring up with sac_train_run first)."""
+    check(_lib.lib().uavrl_sac_train_run_dp(env.h, sac.h, int(n_iters), int(global_batch), _stream(env.device)))

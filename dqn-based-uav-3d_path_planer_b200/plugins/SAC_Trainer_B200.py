@@ -46,6 +46,7 @@ class SAC_Trainer_B200:
         self._dev = self._learner.device
         self._losses = torch.zeros(4 * G, device=self._dev)
         self.loss = 0
+        self._dist, self._rank, self._world = None, 0, 1
         self.model_dir = None2Value(param.get('model_path'), None)
         self.Load_Mod()
 
@@ -67,6 +68,15 @@ class SAC_Trainer_B200:
         a = self._learner.act(torch.from_numpy(s.reshape(-1, self.w)).to(self._dev)).cpu().numpy()
         return a[0].tolist() if single else a
 
+    def attach_dist(self, dist, rank, world):
+        """Data-parallel training, one process per GPU, each with its own batches: with world > 1, update() sums both critics'
+        gradients and squared-error sums over the ranks (dist.all_reduce), steps the critics, then does the same for the
+        actor's gradient, loss and entropy sums; every rank's networks, moments and alpha stay bit-identical.  The losses
+        average over the global batch (this rank's rows x world)."""
+        self._dist, self._rank, self._world = dist, int(rank), int(world)
+        if self._world > 1:
+            self._xvec = (self._learner.exchange_tensor(0), self._learner.exchange_tensor(1))
+
     def update(self, transition_dict):
         """SAC_Trainer.update (:317-441), continuous branch, on the batch in transition_dict."""
         states = transition_dict['states']
@@ -79,7 +89,16 @@ class SAC_Trainer_B200:
         s = f(states, (-1, self.w)); s2 = f(transition_dict['next_states'], (-1, self.w))
         a = f(transition_dict['actions'], (-1, self.act_dim))
         r = f(transition_dict['rewards'], (-1,)); d = f(transition_dict['dones'], (-1,))
-        self._learner.update_batch(s, a, r, s2, d, None, None, self._losses)
+        if self._world > 1:
+            L, dist = self._learner, self._dist
+            L.critic_grads(s.shape[0] * self._world, batch=(s, a, r, s2, d))
+            dist.all_reduce(self._xvec[0], op=dist.ReduceOp.SUM)
+            L.apply_critic_grads()
+            L.actor_grads()
+            dist.all_reduce(self._xvec[1], op=dist.ReduceOp.SUM)
+            L.apply_actor_grads(self._losses)
+        else:
+            self._learner.update_batch(s, a, r, s2, d, None, None, self._losses)
         self.loss = self._losses[0::4]                           # every trainer's actor loss (one trainer: a 1-element tensor)
         if self.save_loop > 0 and self.epoch % self.save_loop == 0:
             self.save()

@@ -425,6 +425,57 @@ int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const flo
  * learner on different devices (UAVRL_ERR_INVALID, as uavrl_train_run); no uavrl_env_reset (UAVRL_ERR_STATE). */
 int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t do_update, uavrl_train_stats *stats_host, void *stream);
 
+/* Data-parallel SAC (one learner per GPU, each rank sampling batch_size rows from its own ring shard; global_batch =
+ * batch_size x world).  The actor loss is taken on the UPDATED critics, so an update makes two exchanges: both critics'
+ * gradients with the two critic squared-error sums, then -- after the critics' Adam step on every rank -- the actor's
+ * gradient with the actor-loss and entropy sums.  All losses, the alpha step and the soft target update then use the
+ * global sums over global_batch x 2 entries, and every rank holds bit-identical networks, Adam moments, alpha triple, epoch
+ * and adam_step.  Each rank keeps its own seed, so its sampling keys and reparameterisation noise are its own.  With world =
+ * 1 and global_batch = batch_size an update equals uavrl_sac_update_replay bit for bit (roles 11-13 hold 0 + g: a -0
+ * gradient entry reads +0).
+ *
+ * Fused form (no NCCL): uavrl_sac_comm_init allocates this rank's receive buffer recv[2][world][max(2 Pc + 2, Pa + 2)] of
+ * 8-byte words and writes UAVRL_SAC_COMM_HANDLE_BYTES bytes: its CUDA IPC handle followed by this device's PCI bus id;
+ * uavrl_sac_comm_connect takes every rank's record ([world][UAVRL_SAC_COMM_HANDLE_BYTES] bytes) and refuses
+ * (UAVRL_ERR_INVALID) two ranks on one device, whose exchange could never complete.  uavrl_sac_update_replay_dp is one
+ * update from the ring through the two exchanges of uavrl_learner_update_dp's kernel (one word {tag : value} per value,
+ * pushed to every rank, summed in rank order); a rank's exchange waits until every other rank's words arrive.
+ *
+ * Split form (e.g. NCCL, or a caller holding explicit batches), four calls in this order:
+ *   uavrl_sac_critic_grads_replay / _batch  epoch += 1; sample from the ring (idx_tape_dev as in uavrl_sac_update_replay) or
+ *                                           take B explicit rows (which must stay valid until the actor phase); write the
+ *                                           critic exchange vector uavrl_sac_exchange_ptr(s, 0, &n): [grad critic_1 | grad
+ *                                           critic_2 | critic-1, critic-2 squared-error sums], n = 2 Pc + 2;
+ *   uavrl_sac_apply_critic_grads            after the caller summed that vector over the ranks: Adam on both critics;
+ *   uavrl_sac_actor_grads                   the actor leg on the same rows (and the same ring contents) with eps_cur_dev;
+ *                                           writes uavrl_sac_exchange_ptr(s, 1, &n): [grad actor | actor-loss sum,
+ *                                           entropy sum], n = Pa + 2;
+ *   uavrl_sac_apply_actor_grads             after the sum: the actor's Adam step, the alpha step, the soft target update and
+ *                                           losses_dev [4] (global means).
+ * Refused before the epoch counts, leaving parameters, moments, alpha, counters and ring untouched: a learner with several
+ * trainers and global_batch <= 0 (UAVRL_ERR_INVALID); a call out of the order above, no ring or a ring holding <=
+ * batch_size transitions for the ring forms, uavrl_sac_update_replay_dp before uavrl_sac_comm_connect (UAVRL_ERR_STATE). */
+#define UAVRL_SAC_COMM_HANDLE_BYTES 128
+int uavrl_sac_comm_init(uavrl_sac *s, int32_t rank, int32_t world, void *handle_out);
+int uavrl_sac_comm_connect(uavrl_sac *s, const void *handles);
+int uavrl_sac_update_replay_dp(uavrl_sac *s, const int32_t *idx_tape_dev, const float *eps_next_dev, const float *eps_cur_dev,
+                               int32_t global_batch, float *losses_dev, void *stream);
+int uavrl_sac_critic_grads_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const float *eps_next_dev, int32_t global_batch, void *stream);
+int uavrl_sac_critic_grads_batch(uavrl_sac *s, int32_t B, const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev,
+                                 const float *d_dev, const float *eps_next_dev, int32_t global_batch, void *stream);
+int uavrl_sac_apply_critic_grads(uavrl_sac *s, void *stream);
+int uavrl_sac_actor_grads(uavrl_sac *s, const float *eps_cur_dev, void *stream);
+int uavrl_sac_apply_actor_grads(uavrl_sac *s, float *losses_dev, void *stream);
+/* phase 0: the critic exchange vector, 1: the actor's; *len_out (may be NULL) receives its length in floats.  Device memory
+ * owned by the learner; NULL for another phase. */
+float *uavrl_sac_exchange_ptr(uavrl_sac *s, int32_t phase, int64_t *len_out);
+/* Data-parallel form of uavrl_sac_train_run (after uavrl_sac_comm_connect): every iteration ends with one
+ * uavrl_sac_update_replay_dp on this rank's ring.  Refused before anything is enqueued, leaving env, ring, parameters and
+ * counters untouched: global_batch <= 0, a learner with several trainers, and what uavrl_sac_train_run refuses
+ * (UAVRL_ERR_INVALID); no uavrl_sac_comm_connect, no uavrl_env_reset, or a ring that would hold <= batch_size transitions
+ * at the first update (UAVRL_ERR_STATE: warm it up with uavrl_sac_train_run first). */
+int uavrl_sac_train_run_dp(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t global_batch, void *stream);
+
 /* Data-parallel form of uavrl_train_run (after uavrl_learner_comm_connect): every iteration ends with
  * uavrl_learner_update_dp on this rank's replay shard; global_batch = batch_size x world.  Refused before anything is
  * enqueued, leaving env, ring, parameters and counters untouched: global_batch <= 0, a grouped learner, lockstep_envs !=
