@@ -18,6 +18,7 @@ import torch
 
 import uavrl_b200  # noqa: F401  (repository root must be on sys.path)
 from uavrl_b200 import engine
+from uavrl_b200.plugins._trainer_base import TrainerB200
 from uavrl_b200.plugins.xmlconfig import None2Value, XML2Dict
 
 
@@ -166,7 +167,12 @@ class PathPlan_City_B200:
             mod = importlib.import_module("uavrl_b200.plugins." + ttype)
         except ImportError:
             mod = importlib.import_module(ttype)
-        self.Trainer = getattr(mod, ttype)(tdict)
+        tcls = getattr(mod, ttype)
+        if self.host_driven and not issubclass(tcls, TrainerB200):
+            # run_step_OffPolicy needs the trainer's host replay facade and learn_off_policy, which only the DQN family has
+            raise ValueError("host_driven = 1 drives the DQN-family trainers (DQN_Trainer_B200, DDQN_Trainer_B200, "
+                             "DuelingDQN_Trainer_B200); %s has no host replay or learn_off_policy: set host_driven = 0" % ttype)
+        self.Trainer = tcls(tdict)
         self.Agents = [UAVBatchView(self)]
         if self.record_csv:
             self.Agents[0].Init_Record_Mod()

@@ -65,9 +65,9 @@ def assert_obs(got, want64, what=""):
 
 
 @contextlib.contextmanager
-def env_plugin(model_path):
+def env_plugin(model_path, **trainer):
     """The env plug-in module, run from the repository root, whose trainers read a small batch and replay, no periodic
-    save and checkpoints under model_path."""
+    save and checkpoints under model_path; `trainer` overrides further Trainer XML entries (strings)."""
     cwd = os.getcwd()
     os.chdir(ROOT)
     mod = importlib.import_module("uavrl_b200.plugins.PathPlan_City_B200")
@@ -76,7 +76,7 @@ def env_plugin(model_path):
     def patched(path):
         d = orig(path)
         if "Trainer" in d and isinstance(d["Trainer"], dict):
-            d["Trainer"].update(Batch_Size="16", replay_size="512", save_loop="0", model_path=str(model_path))
+            d["Trainer"].update({**dict(Batch_Size="16", replay_size="512", save_loop="0", model_path=str(model_path)), **trainer})
         return d
     mod.XML2Dict = patched
     try:

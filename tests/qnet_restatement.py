@@ -1,10 +1,13 @@
 """The float64 restatement of the Q-network forward pass and of one TD update, with the batch draws the sweeps feed the
 kernels.  It is the one arbiter between fp32 implementations whose summation orders differ, and it is pinned to torch
-autograd and to the CPU oracle in test_weighted_f64_cpu.py before any GPU test compares against it."""
+autograd and to the CPU oracle in test_weighted_f64_cpu.py before any GPU test compares against it.  Also the judges of sampled
+updates and actions the loops' tests share: the entries a row near a ReLU kink may move, the double-DQN tie allowance, the
+tally that keeps both rare, and the eps-greedy / argmax check of an act call."""
 import numpy as np
 import pytest
 
 import oracle as O
+import replay_restatement as R
 
 GAMMA = 0.99
 
@@ -183,6 +186,96 @@ def huber_rewards(rng, layers, dueling, algo, Ps, local, target, s, a, s2, d, re
         t[near] = rng.normal(0.0, 1.5, int(near.sum()))
     assert not near.any()
     return r
+
+
+# ------------------------------------------------------------------ judging sampled updates and actions
+def trunk_exempt(layers, n_trunk, P64, dueling, s, rel=2e-5):
+    """Gradient entries the rows of s near a ReLU kink can move: for a unit of trunk layer l near its kink on some row, that
+    unit's weight row and bias and every entry of the layers below l.  Returns (mask, number of kink rows)."""
+    offs, o = [], 0
+    for (n_out, n_in) in layers:
+        offs.append((o, o + n_out * n_in, n_out, n_in)); o += n_out * n_in + n_out
+    mask = np.zeros(o, bool)
+    h = np.asarray(s, np.float64)
+    rows = np.zeros(h.shape[0], bool)
+    for l, (W, b) in enumerate(P64[:n_trunk]):
+        z = h @ W.T + b
+        near = np.abs(z) <= rel * (np.abs(h) @ np.abs(W).T + np.abs(b))
+        units = np.flatnonzero(near.any(0))
+        rows |= near.any(1)
+        w0, b0, n_out, n_in = offs[l]
+        for j in units:
+            mask[w0 + j * n_in:w0 + (j + 1) * n_in] = True
+            mask[b0 + j] = True
+        if units.size:
+            mask[:offs[l][0]] = True
+        h = np.maximum(z, 0.0)
+    return mask, int(rows.sum())
+
+
+def tie_allowance(layers, algo, dueling, local, target, batch, P, gamma=GAMMA):
+    """Double-DQN rows whose next-state top-2 local values tie within 1e-4: the loss and gradient change that choosing the
+    other action would make (row b moves y by delta_b = gamma |q_T(s2, a1) - q_T(s2, a2)| (1 - d); the gradient by
+    (2 / B) delta_b |dQ(s_b, a_b) / dtheta|).  Returns (loss allowance, gradient allowance [P], tied rows)."""
+    s, a, r, s2, d = batch
+    B = s.shape[0]
+    gal = np.zeros(P)
+    if algo == O.ALGO_DQN:
+        return 0.0, gal, 0
+    PL, PT = f64_unpack(layers, local), f64_unpack(layers, target)
+    ql = f64_forward(PL, dueling, s2)[0]
+    order = np.argsort(ql, 1)
+    top, second = order[:, -1], order[:, -2]
+    tie = (ql[np.arange(B), top] - ql[np.arange(B), second] < 1e-4) & (d == 0)
+    rows = np.flatnonzero(tie)
+    if not rows.size:
+        return 0.0, gal, 0
+    qt = f64_forward(PT, dueling, s2[rows])[0]
+    delta = gamma * np.abs(qt[np.arange(rows.size), top[rows]] - qt[np.arange(rows.size), second[rows]])
+    q = f64_forward(PL, dueling, s[rows])[0][np.arange(rows.size), a[rows]]
+    y = r[rows] + gamma * qt[np.arange(rows.size), top[rows]]
+    lal = float(np.sum(delta * (2 * np.abs(q - y) + delta)) / B)
+    for k, b in enumerate(rows):
+        one = lambda rr: f64_update(layers, algo, dueling, local, target, s[b:b + 1], a[b:b + 1], np.array([rr], np.float32),  # noqa: E731
+                                    s2[b:b + 1], np.zeros(1, np.float32), gamma=gamma)[1]
+        J = (one(0.0) - one(1.0)) / 2.0                        # dQ(s_b, a_b) / dtheta
+        gal += (2.0 / B) * delta[k] * np.abs(J)
+    return lal, gal * 1.01, int(rows.size)
+
+
+class Tally:
+    """Counts of the sampled rows near a kink or a tie over a leg: they must stay rare.  (One such row in a deep layer moves
+    every entry of the layers below it, so the exempted entries are counted but not bounded.)"""
+
+    def __init__(self):
+        self.rows = self.kink_rows = self.tie_rows = self.entries = self.exempt = 0
+
+    def check(self):
+        assert self.rows > 0
+        assert self.kink_rows <= 0.05 * self.rows + 2, (self.kink_rows, self.rows)
+        assert self.tie_rows <= 0.02 * self.rows + 2, (self.tie_rows, self.rows)
+
+
+def check_actions(s, a, seed, call, p_before, eps, shape, G=1):
+    """Actions a of the rows s that act call `call` of a learner seeded with `seed` chose (G equal trainer blocks): the restated
+    eps-greedy draw on random rows, the float64 argmax of the parameters before the call (p_before[g]) on greedy rows where the
+    top-2 gap exceeds 1e-4."""
+    in_dim, hidden, n_actions, dueling = shape
+    layers = net_layers(in_dim, hidden, n_actions, dueling)
+    N = s.shape[0]
+    Ng = N // G
+    n_clear = 0
+    for g in range(G):
+        rows = slice(g * Ng, (g + 1) * Ng)
+        greedy, ra = R.eps_greedy(seed, call, Ng, eps, n_actions, g)
+        ag = a[rows]
+        assert np.array_equal(ag[~greedy], ra[~greedy]), (g, call)
+        q = f64_forward(f64_unpack(layers, p_before[g]), dueling, s[rows])[0]
+        top2 = np.sort(q, 1)[:, -2:]
+        clear = greedy & ((top2[:, 1] - top2[:, 0]) > 1e-4)
+        assert np.array_equal(ag[clear], q[clear].argmax(1)), (g, call, int((ag[clear] != q[clear].argmax(1)).sum()))
+        n_clear += int(clear.sum()) + int((~greedy).sum())
+    assert n_clear >= 0.98 * N
 
 
 @pytest.fixture

@@ -4,8 +4,9 @@ learner.cuh, sac.cu), which the sampler tests judge the device against.
 Philox4x32-10 keyed by (seed, salt, trainer); the keyed permutation perm_index (4-round Feistel with cycle walking) that turns
 batch position b into the b-th of B distinct trainer-local replay indices; the lockstep ring (frames of N envs, trainer g owning
 envs [g Ng, (g + 1) Ng)) that maps such an index to a whole-ring logical index; the loop's schedule (an epoch per update,
-nothing sampled while a trainer holds <= batch_size transitions, a hard target update every update_loop-th epoch); the
-eps-greedy draw of the act pass and SAC's Box-Muller reparameterisation noise."""
+nothing sampled while a trainer holds <= batch_size transitions, a hard target update every update_loop-th epoch); the paired
+store of the host-driven path (lockstep_envs = 0) and the same schedule on it; the eps-greedy draw of the act pass, the
+prioritised sampler's uniforms and SAC's Box-Muller reparameterisation noise."""
 import numpy as np
 
 M64 = (1 << 64) - 1
@@ -162,6 +163,58 @@ class Loop:
         return out
 
 
+# ------------------------------------------------------------------ the paired store
+class Paired:
+    """ReplayStore in its paired layout (lockstep_envs = 0): a FIFO of `capacity` slots that uavrl_replay_push fills; head = the
+    next slot written, count = the valid transitions, logical index j (0 = oldest) in slot (oldest + j) mod capacity."""
+
+    def __init__(self, capacity):
+        self.slots = capacity
+        self.head = 0
+        self.count = 0
+
+    def push(self, n):
+        """n new transitions (1 <= n <= capacity; the push may wrap): the slots they land in, in push order."""
+        assert 1 <= n <= self.slots
+        out = (self.head + np.arange(n)) % self.slots
+        self.head = (self.head + n) % self.slots
+        self.count = min(self.count + n, self.slots)
+        return out
+
+    def oldest(self):
+        return (self.head - self.count) % self.slots
+
+    def slot(self, j):
+        """Logical index j -> slot (gather's mapping)."""
+        return (self.oldest() + np.asarray(j, np.int64)) % self.slots
+
+    def logical(self, slot):
+        return (np.asarray(slot, np.int64) - self.oldest()) % self.slots
+
+    def newest(self, n):
+        """Logical indices of the last n transitions pushed, in push order."""
+        return np.arange(self.count - n, self.count)
+
+
+class PairedLoop:
+    """The counters of a learner on a paired store as update() / learn_off_policy advance them: the epoch counts every call,
+    nothing is sampled while count <= batch_size, adam_t counts real updates only, and an update whose epoch is a multiple of
+    update_loop ends with the hard target update.  update() returns (epoch, logical indices, hard) or None for a skipped
+    call."""
+
+    def __init__(self, store, seed, batch_size, update_loop=0, epoch=0, adam_t=0):
+        self.store, self.seed, self.B, self.update_loop = store, seed, batch_size, update_loop
+        self.epoch, self.adam_t = epoch, adam_t
+
+    def update(self):
+        self.epoch += 1
+        if self.store.count <= self.B:
+            return None
+        self.adam_t += 1
+        hard = self.update_loop > 0 and self.epoch % self.update_loop == 0
+        return self.epoch, sample(self.seed, self.epoch, self.store.count, self.B), hard
+
+
 # ------------------------------------------------------------------ the act pass and SAC's noise
 def eps_greedy(seed, call, n_rows, eps, n_actions, g=0):
     """learner.cuh eps_greedy without tapes for rows 0..n_rows-1 of trainer g at act call `call`: (greedy mask, random action)."""
@@ -170,6 +223,14 @@ def eps_greedy(seed, call, n_rows, eps, n_actions, g=0):
     u = u01(r[:, 0])
     ra = ((r[:, 1].astype(np.uint64) * np.uint64(n_actions)) >> np.uint64(32)).astype(np.int32)
     return u > np.float32(eps), ra
+
+
+def per_uniforms(seed, call, B):
+    """per.cu per_sample_kernel without a u-tape: the B uniforms in [0, 1) (53 random bits) of sampling call `call` of a
+    stand-alone learner."""
+    r = philox((seed ^ K_PER_SALT) & M64, call, np.arange(B, dtype=np.uint64)).astype(np.uint64)
+    bits = ((r[:, 0] >> np.uint64(5)) << np.uint64(26)) | (r[:, 1] >> np.uint64(6))
+    return bits.astype(np.float64) * (1.0 / 9007199254740992.0)
 
 
 def sac_noise(seed, ctr, n_rows, g=0):

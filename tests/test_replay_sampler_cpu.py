@@ -1,7 +1,8 @@
 """The replay sampler of the lockstep loops without a GPU: Philox4x32-10 against Random123's published vectors, the numpy
 restatement (tests/replay_restatement.py) against csrc/replay.cuh and common.cuh compiled for the host, perm_index as a
 bijection, and perm_index as a fair sampler: every stored transition, whatever its age, equally likely to be drawn, with no
-excess or deficit of neighbouring pairs drawn together and consecutive epochs independent.
+excess or deficit of neighbouring pairs drawn together and consecutive epochs independent.  Also the paired store of the
+host-driven path (Paired) against a plain FIFO list, and the update schedule on it (PairedLoop).
 
 The statistics use fixed seeds and bounds chosen before the data: a chi-square p-value inside [1e-5, 1 - 1e-5] (too regular
 is as wrong as biased) and |z| <= 4.5 for the pair and overlap counts."""
@@ -247,3 +248,56 @@ def test_loop_schedule():
     assert loop.adam_t == 4 and loop.act_calls == 6 and loop.epoch == 6
     e, idx, _ = its[2][0]
     assert np.array_equal(idx[1], R.sample(5 + 1, e, 72, 64)) and not np.array_equal(idx[0], idx[1])
+
+
+# ------------------------------------------------------------------ the paired store of the host-driven path
+def paired_pushes(rng, cap, total):
+    """Ragged push sizes summing to at least `total`: single transitions, pushes larger than what is left before the wrap, and
+    pushes of exactly the capacity."""
+    out, done = [], 0
+    while done < total:
+        k = int(rng.integers(0, 4))
+        left = cap - (done % cap)
+        n = [1, int(rng.integers(1, cap + 1)), cap, min(cap, left + int(rng.integers(1, cap + 1)))][k]
+        out.append(n)
+        done += n
+    return out
+
+
+@pytest.mark.parametrize("cap", [1, 2, 7, 64, 1000])
+def test_paired_store_is_a_fifo(cap):
+    """Paired against a plain FIFO list: after every ragged push, logical index j (0 = oldest) names the slot that holds the
+    FIFO's j-th transition, oldest / count / head agree, and the newest indices are the last push in order."""
+    rng = np.random.default_rng(cap)
+    P = R.Paired(cap)
+    fifo, held = [], {}                   # transition ids oldest first; slot -> id it holds
+    nxt = 0
+    for n in paired_pushes(rng, cap, 6 * cap + 5):
+        ids = list(range(nxt, nxt + n))
+        nxt += n
+        slots = P.push(n)
+        assert slots.shape == (n,) and ((0 <= slots) & (slots < cap)).all()
+        for i, s in zip(ids, slots):
+            held[int(s)] = i
+        fifo = (fifo + ids)[-cap:]
+        assert P.count == len(fifo) and P.head == nxt % cap
+        j = np.arange(P.count)
+        assert [held[int(s)] for s in P.slot(j)] == fifo
+        assert np.array_equal(P.logical(P.slot(j)), j)
+        assert [held[int(s)] for s in P.slot(P.newest(min(n, cap)))] == ids[-cap:]
+        assert P.oldest() == (0 if nxt <= cap else nxt % cap)
+
+
+def test_paired_schedule():
+    """B = 5 on a 9-slot store: the epoch counts every call; count <= B samples nothing; adam_t counts real updates; the hard
+    update lands on epochs divisible by update_loop; the draw is sample(seed, epoch, count, B)."""
+    P = R.Paired(9)
+    loop = R.PairedLoop(P, seed=3, batch_size=5, update_loop=3)
+    got = []
+    for n in (2, 3, 1, 9, 4):             # count 2, 5 (= B), 6 (= B + 1), 9 (full), 9 (wrapped)
+        P.push(n)
+        got.append(loop.update())
+    assert [u is None for u in got] == [True, True, False, False, False]
+    assert [u[0] for u in got[2:]] == [3, 4, 5] and [u[2] for u in got[2:]] == [True, False, False]
+    assert loop.epoch == 5 and loop.adam_t == 3
+    assert np.array_equal(got[2][1], R.sample(3, 3, 6, 5)) and np.array_equal(got[4][1], R.sample(3, 5, 9, 5))

@@ -17,7 +17,7 @@ import torch
 import oracle as O
 import replay_restatement as R
 from gpu_util import city_and_params, dev, n_sm  # noqa: F401  (module fixture)
-from qnet_restatement import f64_forward, f64_unpack, f64_update, net_layers
+from qnet_restatement import Tally, check_actions, f64_forward, f64_unpack, f64_update, net_layers, tie_allowance, trunk_exempt
 from sac_restatement import HP, check_step, near_decision, read_state, sac_update64
 from shapes import SHAPES, SHIPPED, expected_route
 from uavrl_b200 import _lib, engine
@@ -139,94 +139,6 @@ def test_sac_ring_update_samples_restated_indices(world, G):
 
 
 # ------------------------------------------------------------------ (b) the Q-network loop, update by update, against float64
-def trunk_exempt(layers, n_trunk, P64, dueling, s, rel=2e-5):
-    """Gradient entries the rows of s near a ReLU kink can move: for a unit of trunk layer l near its kink on some row, that
-    unit's weight row and bias and every entry of the layers below l.  Returns (mask, number of kink rows)."""
-    offs, o = [], 0
-    for (n_out, n_in) in layers:
-        offs.append((o, o + n_out * n_in, n_out, n_in)); o += n_out * n_in + n_out
-    mask = np.zeros(o, bool)
-    h = np.asarray(s, np.float64)
-    rows = np.zeros(h.shape[0], bool)
-    for l, (W, b) in enumerate(P64[:n_trunk]):
-        z = h @ W.T + b
-        near = np.abs(z) <= rel * (np.abs(h) @ np.abs(W).T + np.abs(b))
-        units = np.flatnonzero(near.any(0))
-        rows |= near.any(1)
-        w0, b0, n_out, n_in = offs[l]
-        for j in units:
-            mask[w0 + j * n_in:w0 + (j + 1) * n_in] = True
-            mask[b0 + j] = True
-        if units.size:
-            mask[:offs[l][0]] = True
-        h = np.maximum(z, 0.0)
-    return mask, int(rows.sum())
-
-
-def tie_allowance(layers, algo, dueling, local, target, batch, P):
-    """Double-DQN rows whose next-state top-2 local values tie within 1e-4: the loss and gradient change that choosing the
-    other action would make (row b moves y by delta_b = gamma |q_T(s2, a1) - q_T(s2, a2)| (1 - d); the gradient by
-    (2 / B) delta_b |dQ(s_b, a_b) / dtheta|).  Returns (loss allowance, gradient allowance [P], tied rows)."""
-    s, a, r, s2, d = batch
-    B = s.shape[0]
-    gal = np.zeros(P)
-    if algo == engine.ALGO_DQN:
-        return 0.0, gal, 0
-    PL, PT = f64_unpack(layers, local), f64_unpack(layers, target)
-    ql = f64_forward(PL, dueling, s2)[0]
-    order = np.argsort(ql, 1)
-    top, second = order[:, -1], order[:, -2]
-    tie = (ql[np.arange(B), top] - ql[np.arange(B), second] < 1e-4) & (d == 0)
-    rows = np.flatnonzero(tie)
-    if not rows.size:
-        return 0.0, gal, 0
-    qt = f64_forward(PT, dueling, s2[rows])[0]
-    delta = GAMMA * np.abs(qt[np.arange(rows.size), top[rows]] - qt[np.arange(rows.size), second[rows]])
-    q = f64_forward(PL, dueling, s[rows])[0][np.arange(rows.size), a[rows]]
-    y = r[rows] + GAMMA * qt[np.arange(rows.size), top[rows]]
-    lal = float(np.sum(delta * (2 * np.abs(q - y) + delta)) / B)
-    for k, b in enumerate(rows):
-        one = lambda rr: f64_update(layers, algo, dueling, local, target, s[b:b + 1], a[b:b + 1], np.array([rr], np.float32),  # noqa: E731
-                                    s2[b:b + 1], np.zeros(1, np.float32))[1]
-        J = (one(0.0) - one(1.0)) / 2.0                        # dQ(s_b, a_b) / dtheta
-        gal += (2.0 / B) * delta[k] * np.abs(J)
-    return lal, gal * 1.01, int(rows.size)
-
-
-class Tally:
-    """Counts of the sampled rows near a kink or a tie over a leg: they must stay rare.  (One such row in a deep layer moves
-    every entry of the layers below it, so the exempted entries are counted but not bounded.)"""
-
-    def __init__(self):
-        self.rows = self.kink_rows = self.tie_rows = self.entries = self.exempt = 0
-
-    def check(self):
-        assert self.rows > 0
-        assert self.kink_rows <= 0.05 * self.rows + 2, (self.kink_rows, self.rows)
-        assert self.tie_rows <= 0.02 * self.rows + 2, (self.tie_rows, self.rows)
-
-
-def check_actions(L, ring, loop, p_before, eps, shape, G, tally):
-    """The newest transition group's actions: the restated eps-greedy draw on random rows, the float64 argmax of the
-    parameters before the iteration on greedy rows (where the top-2 gap exceeds 1e-4)."""
-    in_dim, hidden, n_actions, dueling = shape
-    layers = net_layers(in_dim, hidden, n_actions, dueling)
-    s, a, _, _, _ = L.gather(ring.newest())
-    Ng = ring.Ng
-    n_clear = 0
-    for g in range(G):
-        rows = slice(g * Ng, (g + 1) * Ng)
-        greedy, ra = R.eps_greedy(L.cfg.seed, loop.act_calls - 1, Ng, eps, n_actions, g)
-        ag = a[rows]
-        assert np.array_equal(ag[~greedy], ra[~greedy]), (g, loop.act_calls)
-        q = f64_forward(f64_unpack(layers, p_before[g]), dueling, s[rows])[0]
-        top2 = np.sort(q, 1)[:, -2:]
-        clear = greedy & ((top2[:, 1] - top2[:, 0]) > 1e-4)
-        assert np.array_equal(ag[clear], q[clear].argmax(1)), (g, loop.act_calls, int((ag[clear] != q[clear].argmax(1)).sum()))
-        n_clear += int(clear.sum()) + int((~greedy).sum())
-    assert n_clear >= 0.98 * ring.N
-
-
 def run_qnet_loop(world, shape, algo, tc, B, N, U, n_iters, cap_frames, G=1, eps=0.3, seed=3, route=None, n_sm=None, fused=None):
     """n_iters calls of train_run(1 iteration, updates_per_iter = U), each checked against the restated schedule, the float64
     update and the oracle's chain from the learner's state before the iteration."""
@@ -258,7 +170,8 @@ def run_qnet_loop(world, shape, algo, tc, B, N, U, n_iters, cap_frames, G=1, eps
         wrapped |= ring.head == 0
         assert L.counters() == (loop.epoch, ctr[1] + sum(u is not None for u in ups)), (it, L.counters())
         assert st.updates == sum(u is not None for u in ups)
-        check_actions(L, ring, loop, before[0], eps, shape, G, tally)
+        s_new, a_new, _, _, _ = L.gather(ring.newest())
+        check_actions(s_new, a_new, L.cfg.seed, loop.act_calls - 1, before[0], eps, shape, G)
         after = [L.get_params(w).reshape(G, -1) for w in range(4)]
         if all(u is None for u in ups):
             skipped += 1
