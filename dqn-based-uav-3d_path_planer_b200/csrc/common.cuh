@@ -32,6 +32,9 @@ inline int num_sms()
 }
 extern std::atomic<long long> g_launches;
 
+// shared memory one block may use on sm_90 (dynamic + static): every kernel that keeps a network resident is sized against it
+constexpr size_t kMaxBlockSmem = 227 * 1024;
+
 inline int fail(int code, const std::string &msg)
 {
     g_last_error = msg;

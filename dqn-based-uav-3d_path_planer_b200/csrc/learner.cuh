@@ -1,36 +1,13 @@
 // learner.cuh -- Q-network / replay / optimiser state of one learner (device-resident) + host handle.
 #pragma once
-#include "common.cuh"
+#include "net.cuh"
+#include "optim.cuh"
 #include "per.cuh"
 #include "replay.cuh"
 
 namespace uavrl {
 
-constexpr int kTile = 32;             // samples per CTA tile
-constexpr int kNetThreads = 256;      // 8 warps: lane -> output unit, warp -> 4 samples
-constexpr int kMaxDim = 128;          // every layer width (and in_dim) <= 128
-constexpr int kMaxLayers = UAVRL_MAX_HIDDEN + 1;   // trunk layers + (combined) head
 constexpr int kFedProbes = 10;        // probe states per trainer of a federation round (PathPlan_City.py:658)
-
-// One dense layer as the kernels see it.  Weights live in smem transposed: Wt[k][o], ld = out+1
-// (odd when out is even -> conflict-free whether lanes walk o or k).
-struct LayerDev {
-    int32_t in, out;                  // out of the head = n_actions (+1 value row when dueling)
-    int32_t w_off, b_off;             // offsets in the flat state_dict-ordered parameter vector
-    int32_t w2_off, b2_off;           // second head block (rows out_main..out-1): dueling fc_V, SAC actor fc_std; -1 if none
-    int32_t out_main;                 // rows served by (w_off, b_off)
-    int32_t smem_w, smem_b;           // offsets (floats) inside the smem weight area
-};
-
-struct NetDev {
-    int32_t in_dim, n_layers, n_actions, dueling;
-    int32_t P;                        // parameter count
-    int32_t smem_w_floats;            // total smem floats for Wt + biases
-    int32_t act_off[kMaxLayers + 1];  // smem offsets of the activation planes X0, H1.. (floats)
-    int32_t act_ld[kMaxLayers + 1];
-    int32_t smem_total_floats;        // whole dynamic smem carve-up for the update kernel
-    LayerDev L[kMaxLayers];
-};
 
 // ---- tensor-core (wgmma) forward path: one dense layer as a B operand [N_pad][K_pad], K-major canonical
 // layout (wgmma.cuh), hi and lo images of the 3xTF32 split
@@ -109,27 +86,6 @@ __device__ __forceinline__ void fed_group_loss(const float *d2, size_t first_row
 }
 #endif
 
-// One rank's side of the data-parallel exchange (dp_allreduce_adam_kernel, learner.cu): its symmetric receive buffer
-// recv[2][world][words] of 8-byte words {exchange tag : value}, where slot q is written by rank q with remote stores, and every
-// rank's buffer as mapped on this device.  Both learners own one (uavrl_learner_comm_*, uavrl_sac_comm_*).
-struct PeerComm {
-    int32_t rank = 0, world = 1;
-    unsigned long long *recv = nullptr;
-    int32_t recv_world = 0;           // world the buffer was sized for
-    size_t words = 0;                 // words of one rank's slot: the largest exchange the owner makes
-    unsigned long long **peer_dev = nullptr;    // device array [world]
-    void *peer_host[64] = { nullptr };
-    bool ready = false;               // comm_connect has run
-    unsigned tag = 0;                 // tag of the latest exchange; 0 = never written
-    DevMem recv_mem, peer_mem;        // owners of recv and peer_dev
-    ~PeerComm();                      // closes the peers' mapped buffers
-};
-// comm_init: (re)size the receive buffer for `world` ranks of `words` words each and write its CUDA IPC handle into
-// handle_out; with bus_id, the handle is followed by this device's PCI bus id (64 bytes), which comm_connect checks: two
-// ranks on one device would spin forever in the exchange.  comm_connect: open every rank's handle (handles: [world] records).
-int comm_init(PeerComm &c, int device, int32_t rank, int32_t world, size_t words, void *handle_out, bool bus_id);
-int comm_connect(PeerComm &c, int device, const void *handles, bool bus_id);
-
 }  // namespace uavrl
 
 struct uavrl_learner {
@@ -177,133 +133,12 @@ struct uavrl_learner {
     // data-parallel: one-shot NVLink all-reduce fused with Adam (symmetric buffers exchanged through CUDA IPC), slots of P + 1
     // words (gradient, loss share)
     uavrl::PeerComm comm;
-    unsigned long long *dp_trace = nullptr;    // UAVRL_DP_TRACE=1: phase times of the data-parallel optimiser kernel
-    // owners of the buffers above, one per group allocated and replaced together: parameters, images, maps and dp_trace; the
+    // owners of the buffers above, one per group allocated and replaced together: parameters, images, maps; the
     // grown scratch (partials, y / astar, act / dz rows); the PER trees; their scratch
     uavrl::DevMem mem, parts_mem, td_mem, rows_mem, per_mem, per_scratch_mem;
 };
 
 namespace uavrl {
-
-// optimiser kernel arguments (reduce_adam_kernel, learner.cu; also launched by sac.cu)
-struct AdamArgs {
-    int P, nparts, apply, hard, world, n_loss_parts;
-    int img_floats, tc_floats;        // grouped learner (gridDim.y = G): per-trainer strides of the fp32 / tensor-core weight images
-    float step_size, beta1_c, beta2, beta2_c, eps, bc2_sqrt, inv_b;
-};
-
-// everything the optimiser step reads / writes (flat state_dict-ordered vectors + the kernel-layout weight images)
-struct AdamPtrs {
-    const float *partials, *loss_partials;
-    float *grad, *local, *m, *v, *target, *img_local, *img_target;
-    const int32_t *img_map;
-    float *tc_local, *tc_target;
-    const int32_t *tc_hi, *tc_lo, *tc_hi2, *tc_lo2;
-    float *loss_out;
-};
-
-#if defined(__CUDACC__)
-// Partial-gradient reduction in a FIXED order (run-to-run deterministic, and the same whichever kernel performs it):
-// partial c belongs to group c % 4; a group keeps 8 accumulators (8 independent loads in flight per pass over 32 partials);
-// the total is (g0 + g1) + (g2 + g3).
-__device__ __forceinline__ float reduce_group(const float *__restrict__ partials, int P, int nparts, int i, int cg)
-{
-    float acc[8];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) acc[u] = 0.f;
-    int c = cg;
-    for (; c + 28 < nparts; c += 32) {
-#pragma unroll
-        for (int u = 0; u < 8; ++u) acc[u] += partials[(size_t)(c + 4 * u) * P + i];
-    }
-    for (; c < nparts; c += 4) acc[0] += partials[(size_t)c * P + i];
-    return ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
-}
-
-__device__ __forceinline__ void tf32_split_f(float x, float &hi, float &lo)
-{
-    hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);     // = cvt.rna.tf32.f32 for finite x (wgmma.cuh: tf32_split)
-    lo = x - hi;
-}
-
-// torch.optim.Adam single-tensor step for parameter i with gradient g (lerp, mul/addcmul, sqrt/div/add, addcdiv), the hard
-// target update (DuelingDQN_Trainer.py:199-202) and the refresh of the fp32 and tensor-core weight images
-// what the step reads besides the gradient: nothing a gradient-producing predecessor writes, so an optimiser kernel launched
-// programmatically behind one fetches it BEFORE griddepcontrol.wait (one memory round trip off the post-wait chain)
-struct AdamPre { float m, v, p; int im, ih, il, ih2, il2; };
-__device__ __forceinline__ AdamPre adam_prefetch(const AdamPtrs &q, int i)
-{
-    AdamPre r;
-    r.m = q.m[i]; r.v = q.v[i]; r.p = q.local[i]; r.im = q.img_map[i];
-    r.ih = r.il = r.ih2 = r.il2 = -1;
-    if (q.tc_local) { r.ih = q.tc_hi[i]; r.il = q.tc_lo[i]; r.ih2 = q.tc_hi2[i]; r.il2 = q.tc_lo2[i]; }
-    return r;
-}
-__device__ __forceinline__ void adam_update_pre(const AdamArgs &a, const AdamPtrs &q, int i, float g, const AdamPre &pre)
-{
-    // every operation individually rounded (no FMA contraction): the optimiser kernels that share this function
-    // (reduce_adam_kernel, dp_allreduce_adam_kernel) then produce bit-identical parameters by construction
-    float mi = pre.m, vi = pre.v, p = pre.p;
-    mi = __fadd_rn(mi, __fmul_rn(__fsub_rn(g, mi), a.beta1_c));                                  // exp_avg.lerp_(grad, 1 - beta1)
-    vi = __fadd_rn(__fmul_rn(vi, a.beta2), __fmul_rn(__fmul_rn(a.beta2_c, g), g));               // exp_avg_sq.mul_(beta2).addcmul_(g, g, 1 - beta2)
-    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vi), a.bc2_sqrt), a.eps);                 // (sqrt(v) / sqrt(bc2)).add_(eps)
-    p = __fsub_rn(p, __fmul_rn(a.step_size, __fdiv_rn(mi, denom)));                              // param.addcdiv_(m, denom, -step_size)
-    q.m[i] = mi; q.v[i] = vi; q.local[i] = p;
-    const int im = pre.im;
-    q.img_local[im] = p;
-    if (a.hard) { q.target[i] = p; q.img_target[im] = p; }
-    if (q.tc_local) {                                        // tensor-core images: TF32 hi/lo split of the new value
-        const int ih = pre.ih, il = pre.il;
-        float hi = p, lo = 0.f;
-        if (il >= 0) tf32_split_f(p, hi, lo);
-        q.tc_local[ih] = hi;
-        if (il >= 0) q.tc_local[il] = lo;
-        const int ih2 = pre.ih2, il2 = pre.il2;
-        if (ih2 >= 0) { q.tc_local[ih2] = hi; q.tc_local[il2] = lo; }
-        if (a.hard) {
-            q.tc_target[ih] = hi;
-            if (il >= 0) q.tc_target[il] = lo;
-            if (ih2 >= 0) { q.tc_target[ih2] = hi; q.tc_target[il2] = lo; }
-        }
-    }
-}
-
-// Sum of column j of n rows of `stride` floats, the order every scalar partial sum of an update takes: lane l adds rows l,
-// l + 32, ... in turn, then a butterfly over the warp.  Every lane of the (full) warp calls it and receives the sum.
-__device__ __forceinline__ float warp_column_sum(const float *p, int n, int stride, int j)
-{
-    float s = 0.f;
-    for (int c = threadIdx.x & 31; c < n; c += 32) s += p[(size_t)c * stride + j];
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-    return s;
-}
-#endif
-
-// One exchange of dp_allreduce_adam_kernel (learner.cu): the optimiser steps of n_seg networks, segment k taking `blocks`
-// blocks of 64 parameters after segment k - 1's and words [sum of the earlier P, + P) of a rank's slot, then n_extra scalar
-// words: column j of the [n_extra_parts][extra_stride] partials, reduced by warp_column_sum and scaled, summed over ranks into
-// extra_out[j].  Every rank's slot holds the words in that order.
-struct DpSeg { const float *partials; int nparts, P, blocks; AdamPtrs q; };
-struct DpExchange {
-    DpSeg seg[2];
-    int n_seg;
-    const float *extra_parts;
-    int n_extra_parts, extra_stride, n_extra;
-    float extra_scale;
-    float *extra_out;
-};
-constexpr int kDpMaxExtra = 2;
-// the exchange x on comm (its tag advances by one) with the Adam hyper-parameters of a; trace (may be null): UAVRL_DP_TRACE
-cudaError_t launch_dp_exchange(PeerComm &comm, const AdamArgs &a, const DpExchange &x, cudaStream_t st, bool pdl,
-                               unsigned long long *trace);
-
-// reduce_adam_kernel (learner.cu) on `grid` (y: trainer) with the pointers of q; pdl: programmatic dependent launch
-cudaError_t launch_reduce_adam(dim3 grid, cudaStream_t st, bool pdl, const AdamArgs &a, const AdamPtrs &q);
-
-// torch.optim.Adam (betas 0.9 / 0.999, eps 1e-8) at step t with learning rate lr: the fields of AdamArgs the step computes in
-// double precision on the host (bias corrections, step size)
-void adam_hyper(AdamArgs &a, float lr, int64_t t);
 // every vector and image of a learner's optimiser step (trainer 0; the kernels offset by trainer)
 AdamPtrs learner_adam_ptrs(const uavrl_learner *l, float *loss_out);
 
@@ -317,36 +152,6 @@ struct Route {
 };
 Route learner_route(const uavrl_learner *l, int n);
 
-// The refusals both trainer-group create entry points make (uavrl_learner_create_trainers, uavrl_sac_create_trainers) after the
-// learner's own configuration checks and before anything is allocated; on success cfg.device is current.  `learner` names the
-// handle in the no-device message.
-template <class Config>
-int check_trainer_group(const Config &cfg, int32_t n_trainers, const char *learner)
-{
-    if (n_trainers < 1 || n_trainers > 65535)        // every grouped kernel runs one grid row per trainer: gridDim.y <= 65535
-        return fail(UAVRL_ERR_INVALID, "n_trainers must be in [1, 65535]");
-    if (n_trainers > 1 && (cfg.lockstep_envs < 0 || cfg.lockstep_envs % n_trainers != 0))
-        return fail(UAVRL_ERR_INVALID, "lockstep_envs must be a multiple of n_trainers (every trainer owns lockstep_envs / n_trainers envs)");
-    if (n_trainers > 1 && cfg.replay_capacity / n_trainers <= 0)
-        return fail(UAVRL_ERR_INVALID, "replay_capacity / n_trainers must be > 0");
-    if (cfg.batch_size <= 0 || cfg.replay_capacity <= 0) return fail(UAVRL_ERR_INVALID, "batch_size and replay_capacity must be > 0");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-        return fail(UAVRL_ERR_CUDA, std::string("no CUDA device: the ") + learner + " has no CPU fallback");
-    UAVRL_CUDA(cudaSetDevice(cfg.device));
-    return 0;
-}
-
-// Gradient / loss partial slots per trainer: a single trainer keeps max_ctas (any batch); a grouped learner sizes them from its
-// per-trainer batch (the grid of its widest update kernel) and grows them when a larger explicit batch arrives.
-inline int32_t trainer_parts_cap(int32_t G, int32_t batch_size, int32_t max_ctas)
-{
-    const int32_t tiles = (batch_size + kTile - 1) / kTile;
-    return (G == 1 || tiles > max_ctas) ? max_ctas : tiles;
-}
-
-// generic MLP description: trunk widths + head = `head_main` rows (+ `head_extra` rows from a second parameter block)
-int build_mlp(int in_dim, int n_hidden, const int32_t *hidden, int head_main, int head_extra, NetDev &n);
 int launch_act(uavrl_learner *l, const float *obs, int n, float eps, int is_train, const float *u_tape,
                const int32_t *rand_tape, int32_t *actions, float *q_out, cudaStream_t st);
 // the loss variant of the act pass (federation): weight sets w0 .. w0 + n_weights - 1 on the probe rows [G][kFedProbes][in_dim]

@@ -4,13 +4,11 @@
 #pragma once
 #include <vector>
 
-#include "learner.cuh"
+#include "net.cuh"
 #include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace uavrl {
-
-__host__ __device__ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
 __device__ __forceinline__ int ldw_of(int out) { return (out & 1) ? out : out + 1; }
 

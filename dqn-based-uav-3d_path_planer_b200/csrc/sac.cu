@@ -24,8 +24,8 @@
 
 #include <vector>
 
-#include "mlp_tile.cuh"
 #include "sac.cuh"
+#include "mlp_tile.cuh"
 
 namespace uavrl {
 
@@ -499,8 +499,6 @@ __global__ void sac_federate_kernel(int P, int G, float *__restrict__ actor)
 using namespace uavrl;
 
 // ------------------------------------------------------------------ host handle (sac.cuh)
-constexpr size_t kSacMaxSmem = 227 * 1024;     // shared memory one block may use on sm_90
-
 // refuses a configuration before anything is allocated
 static int sac_shape(const uavrl_sac_config &c, SacShape &sh)
 {
@@ -642,7 +640,7 @@ static int sac_reduce_adam(uavrl_sac *s, int r, int nparts, bool apply, cudaStre
     AdamArgs aa;
     adam_args(aa, r == 0 ? s->sh.actor : s->sh.critic, nparts, r == 0 ? s->cfg.actor_lr : s->cfg.critic_lr, s->adam_t);
     aa.apply = apply ? 1 : 0;
-    UAVRL_CUDA(launch_reduce_adam(dim3((aa.P + 63) / 64, s->G), st, false, aa, sac_adam_ptrs(s, r)));
+    UAVRL_CUDA(launch_reduce_adam(s->G, st, false, aa, sac_adam_ptrs(s, r)));
     UAVRL_LAUNCHED();
     return 0;
 }
@@ -690,12 +688,12 @@ static int sac_exchange(uavrl_sac *s, bool critics, int grid, cudaStream_t st)
     x.n_seg = critics ? 2 : 1;
     for (int k = 0; k < x.n_seg; ++k) {
         const int r = critics ? 1 + k : 0;
-        x.seg[k].partials = s->part[r]; x.seg[k].nparts = grid; x.seg[k].P = n.P; x.seg[k].blocks = (n.P + 63) / 64;
+        x.seg[k].partials = s->part[r]; x.seg[k].nparts = grid; x.seg[k].P = n.P;
         x.seg[k].q = sac_adam_ptrs(s, r);
     }
     x.extra_parts = s->stat + (critics ? 0 : 2); x.n_extra_parts = grid; x.extra_stride = 4; x.n_extra = 2; x.extra_scale = 1.f;
     x.extra_out = critics ? s->xc + 2 * (size_t)n.P : s->xa + n.P;
-    UAVRL_CUDA(launch_dp_exchange(s->comm, aa, x, st, false, nullptr));
+    UAVRL_CUDA(launch_dp_exchange(s->comm, aa, x, st, false));
     UAVRL_LAUNCHED();
     return 0;
 }
@@ -779,9 +777,9 @@ int uavrl_sac_create_trainers(const uavrl_sac_config *cfg, int32_t n_trainers, u
     size_t smem[4];
     if ((rc = sac_smem_total(sh, smem))) return rc;
     for (int i = 0; i < 4; ++i)
-        if (smem[i] > kSacMaxSmem)
+        if (smem[i] > kMaxBlockSmem)
             return fail(UAVRL_ERR_INVALID, "networks too large for the SMEM-resident SAC kernels: " + std::to_string(smem[i]) +
-                                               " B of shared memory per block, at most " + std::to_string(kSacMaxSmem));
+                                               " B of shared memory per block, at most " + std::to_string(kMaxBlockSmem));
     uavrl_sac *s = new uavrl_sac();
     s->cfg = *cfg;
     s->sh = sh;
@@ -947,16 +945,10 @@ int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
 
 
 // ------------------------------------------------------------------ data-parallel training
-// entry points a grouped learner does not offer, and the refusals every data-parallel update makes before its epoch counts
-static int sac_refuse_grouped(const uavrl_sac *s, const char *fn)
-{
-    if (s->G > 1) return fail(UAVRL_ERR_INVALID, std::string(fn) + " is not available on a learner with " + std::to_string(s->G) + " trainers");
-    return 0;
-}
-
+// the refusals every data-parallel update makes before its epoch counts
 static int sac_dp_checks(const uavrl_sac *s, int32_t global_batch, bool ring, const char *fn)
 {
-    if (int rc = sac_refuse_grouped(s, fn)) return rc;
+    if (int rc = refuse_grouped(s->G, fn)) return rc;
     if (global_batch <= 0) return fail(UAVRL_ERR_INVALID, std::string(fn) + ": global_batch must be > 0");
     if (s->dp_phase != 0) return fail(UAVRL_ERR_STATE, std::string(fn) + " while a split update waits for its next phase");
     if (ring && !s->replay.frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
@@ -967,8 +959,8 @@ static int sac_dp_checks(const uavrl_sac *s, int32_t global_batch, bool ring, co
 
 int uavrl_sac_comm_init(uavrl_sac *s, int32_t rank, int32_t world, void *handle_out)
 {
-    if (!s || world < 1 || world > 64 || rank < 0 || rank >= world || !handle_out) return fail(UAVRL_ERR_INVALID, "bad rank/world/handle pointer");
-    if (int rc = sac_refuse_grouped(s, "uavrl_sac_comm_init")) return rc;
+    if (!s) return fail(UAVRL_ERR_INVALID, "bad rank/world/handle pointer");
+    if (int rc = refuse_grouped(s->G, "uavrl_sac_comm_init")) return rc;
     const size_t Pa = (size_t)s->sh.actor.P, Pc = (size_t)s->sh.critic.P;
     return comm_init(s->comm, s->cfg.device, rank, world, 2 * Pc + 2 > Pa + 2 ? 2 * Pc + 2 : Pa + 2, handle_out, true);
 }
@@ -976,7 +968,7 @@ int uavrl_sac_comm_init(uavrl_sac *s, int32_t rank, int32_t world, void *handle_
 int uavrl_sac_comm_connect(uavrl_sac *s, const void *handles)
 {
     if (!s || !handles) return fail(UAVRL_ERR_INVALID, "bad argument");
-    if (int rc = sac_refuse_grouped(s, "uavrl_sac_comm_connect")) return rc;
+    if (int rc = refuse_grouped(s->G, "uavrl_sac_comm_connect")) return rc;
     if (!s->comm.recv) return fail(UAVRL_ERR_STATE, "uavrl_sac_comm_connect before uavrl_sac_comm_init");
     return comm_connect(s->comm, s->cfg.device, handles, true);
 }
@@ -1033,7 +1025,7 @@ int uavrl_sac_critic_grads_batch(uavrl_sac *s, int32_t B, const float *s_dev, co
 
 static int sac_phase_is(const uavrl_sac *s, int phase, const char *fn)
 {
-    if (int rc = sac_refuse_grouped(s, fn)) return rc;
+    if (int rc = refuse_grouped(s->G, fn)) return rc;
     static const char *want[4] = { "", "after uavrl_sac_critic_grads_*", "after uavrl_sac_apply_critic_grads", "after uavrl_sac_actor_grads" };
     if (s->dp_phase != phase) return fail(UAVRL_ERR_STATE, std::string(fn) + " called out of order: it runs " + want[phase]);
     return 0;

@@ -1,6 +1,8 @@
 // sac.cuh -- host handle of the SAC learner (sac.cu) and the launches the lockstep loop (train.cu) makes on it.
 #pragma once
-#include "learner.cuh"
+#include "replay.cuh"
+#include "net.cuh"
+#include "optim.cuh"
 
 namespace uavrl {
 // the two networks of a SAC learner and the stride of its gradient planes: everything the kernels' shared memory follows from

@@ -69,7 +69,7 @@ int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::v
     }
     tc.max_rows = kTcTile;
     tc.a_bytes = (int)mma_tile_bytes(tc.max_rows, maxK);
-    if (tc_smem_bytes(tc) + 4096 > 227 * 1024) {                 // 128 rows of operands + accumulator, weights, static smem
+    if (tc_smem_bytes(tc) + 4096 > kMaxBlockSmem) {              // 128 rows of operands + accumulator, weights, static smem
         tc.max_rows = 64;
         tc.a_bytes = (int)mma_tile_bytes(tc.max_rows, maxK);
     }
@@ -373,7 +373,7 @@ int tc_init(uavrl_learner *l)
             UAVRL_CUDA(cudaFuncGetAttributes(&fa, pick_forward_kernel(ac != 0, du != 0, fixed)));
             if (fa.sharedSizeBytes > fwd_static) fwd_static = fa.sharedSizeBytes;
         }
-    if (tc_smem_bytes(l->tc) + fwd_static > 227 * 1024) return 0;
+    if (tc_smem_bytes(l->tc) + fwd_static > kMaxBlockSmem) return 0;
     const size_t P = (size_t)l->net.P;
     const size_t img = (size_t)l->tc.train_img_bytes;
     const size_t img_all = (size_t)l->G * img;                  // [G] images of a grouped learner

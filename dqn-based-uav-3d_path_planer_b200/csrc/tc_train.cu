@@ -527,10 +527,10 @@ int tc_train_init(uavrl_learner *l)
         UAVRL_CUDA(cudaFuncGetAttributes(&fa, tc_dw_kernel));
         dw_static = fa.sharedSizeBytes;
     }
-    const size_t train_budget = (size_t)227 * 1024 - train_static;
+    const size_t train_budget = kMaxBlockSmem - train_static;
     // the m64 MMA reads 8 row groups from each A buffer: with fewer real rows it runs into the next buffers,
     // which must still be inside the CTA's allocation
-    if (train_smem_bytes(tc, 32) > train_budget || dw_smem_bytes(tc) + dw_static > (size_t)227 * 1024) return 0;
+    if (train_smem_bytes(tc, 32) > train_budget || dw_smem_bytes(tc) + dw_static > kMaxBlockSmem) return 0;
     if (train_smem_bytes(tc, 32) < (size_t)(32 / 8) * mma_sbo(tc.max_k) + (size_t)8 * mma_sbo(tc.max_k)) return 0;
     tc.train_max_rows = train_smem_bytes(tc, 64) <= train_budget ? 64 : 32;
     for (int np = 0; np < 3; ++np)

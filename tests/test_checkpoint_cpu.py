@@ -33,7 +33,7 @@ def expand(weights):
 
 
 def build_mlp_count(in_dim, hidden, head_main, head_extra):
-    """Parameter count of csrc/learner.cu build_mlp: every trunk layer, then the head with its extra rows."""
+    """Parameter count of csrc/net.cuh build_mlp: every trunk layer, then the head with its extra rows."""
     P, fan_in = 0, in_dim
     for h in hidden:
         P, fan_in = P + h * fan_in + h, h
