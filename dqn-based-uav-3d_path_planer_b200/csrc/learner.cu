@@ -273,23 +273,6 @@ static void launch_copy(size_t n, const float *src, float *dst, cudaStream_t st)
     copy_kernel<<<(unsigned)(blocks < 65536 ? blocks : 65536), 256, 0, st>>>(n, src, dst);
 }
 
-// generic replay push (paired rows)
-__global__ void push_kernel(int n, int in, int64_t head, int64_t cap, const float *__restrict__ obs,
-                            const int32_t *__restrict__ act, const float *__restrict__ rew,
-                            const float *__restrict__ next_obs, const uint8_t *__restrict__ done,
-                            float *__restrict__ frames, int32_t *__restrict__ r_act, float *__restrict__ r_rew,
-                            uint8_t *__restrict__ r_done)
-{
-    const int64_t total = (int64_t)n * in;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t t = i / in, k = i - t * in;
-        const int64_t slot = (head + t) % cap;
-        frames[(2 * slot) * in + k] = obs[i];
-        frames[(2 * slot + 1) * in + k] = next_obs[i];
-        if (k == 0) { r_act[slot] = act[t]; r_rew[slot] = rew[t]; r_done[slot] = done[t]; }
-    }
-}
-
 // ------------------------------------------------------------------ host launchers
 static size_t act_smem_bytes(const NetDev &n) { return (size_t)(n.smem_total_floats + 2 * kTile * kMaxDim + kTile * 32) * 4; }
 static size_t upd_smem_bytes(const NetDev &n, int dual)
@@ -409,13 +392,15 @@ static int mark(cudaEvent_t *marks, int k, cudaStream_t st)
 // training kernel on the fp32 path, which computes the weight gradients itself)
 static Grads launch_grads(uavrl_learner *l, const BatchSrc &src_in, int B, int global_batch, cudaStream_t st, cudaEvent_t *marks)
 {
-    Grads g = { 0, 0, 0, 1.0f / (float)global_batch, l->per.enabled && src_in.mode != kBatchExplicit && !src_in.idx_tape };
+    Grads g = { 0, 0, 0, 1.0f / (float)global_batch, l->replay.per_enabled() && src_in.mode != kBatchExplicit && !src_in.idx_tape };
     BatchSrc src = src_in;
     if (g.per) {
         // ReplayTree.sample2 -> slots + importance weights; |Q - y| comes back for batch_update (per_write_back).
         // Grouped learner: [G][B] trainer-local slots, weights and errors; trainer_src hands trainer g its row of each
-        if ((g.rc = per_sample(l, B, nullptr, nullptr, nullptr, st))) return g;
-        src.idx_tape = l->per.idx; src.idx_is_slot = 1; src.is_w = l->per.w; src.abs_err = l->per.abs_err;
+        if ((g.rc = l->replay.per_sample(l->cfg.seed, B, nullptr, nullptr, nullptr, st))) return g;
+        l->chain.launched(kChainNone);                    // prioritised-replay kernels launch outside the chain
+        const PerDev &p = l->replay.per.dev;
+        src.idx_tape = p.idx; src.idx_is_slot = 1; src.is_w = p.w; src.abs_err = p.abs_err;
     }
     const Route r = learner_route(l, B);
     const int n_tiles = (B + kTile - 1) / kTile;
@@ -513,7 +498,11 @@ static int launch_allreduce_adam(uavrl_learner *l, const Grads &g, float *loss_o
 // ReplayTree.batch_update: the |Q - y| of a SumTree-sampled batch become its priorities
 static int per_write_back(uavrl_learner *l, const Grads &g, int B, cudaStream_t st)
 {
-    return g.per ? per_set(l, B, l->per.idx, nullptr, l->per.abs_err, 1, st) : 0;
+    if (!g.per) return 0;
+    const PerDev &p = l->replay.per.dev;
+    if (int rc = l->replay.per_set(B, p.idx, nullptr, p.abs_err, 1, st)) return rc;
+    l->chain.launched(kChainNone);
+    return 0;
 }
 
 int launch_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, bool apply, cudaStream_t st,
@@ -551,18 +540,6 @@ static int repack_images(uavrl_learner *l, cudaStream_t st)
         UAVRL_LAUNCHED();
     }
     return 0;
-}
-
-void lockstep_commit(uavrl_learner *l, cudaStream_t st)
-{
-    if (l->per.enabled) {
-        // the frame just completed becomes sampleable with the priority of an error-less push; the frame that now
-        // receives the next observations (the ring's oldest) stops being a transition.  Trainer-local slots: every trainer's
-        // tree gets the same Ng + Ng slots of its own env block
-        const int64_t Ng = l->replay.N / l->G;
-        per_fill_range(l, l->replay.head * Ng, 2 * Ng, per_new_priority(l->per), st, Ng, 0.0);
-    }
-    l->replay.commit();
 }
 
 AdamPtrs learner_adam_ptrs(const uavrl_learner *l, float *loss_out)
@@ -705,19 +682,8 @@ int uavrl_replay_push(uavrl_learner *l, int32_t n, const float *obs, const int32
     if (rs.mode != kReplayPaired) return fail(UAVRL_ERR_STATE, "uavrl_replay_push needs lockstep_envs == 0 (the lockstep ring is fed by uavrl_train_run)");
     if (n > rs.slots) return fail(UAVRL_ERR_INVALID, "push larger than the replay capacity");
     UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    const int64_t total = (int64_t)n * l->net.in_dim;
-    const int threads = 256;
-    int blocks = (int)((total + threads - 1) / threads);
-    if (blocks > num_sms() * 8) blocks = num_sms() * 8;
-    push_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(n, l->net.in_dim, rs.head, rs.slots, obs, act, rew, next_obs,
-                                                             done, rs.frames, rs.act, rs.rew, rs.done);
-    UAVRL_LAUNCHED();
-    if (l->per.enabled) {                                       // ReplayTree.push with error 0; uavrl_per_set_errors refines it
-        int rc = per_fill_range(l, rs.head, n, per_new_priority(l->per), (cudaStream_t)stream);
-        if (rc) return rc;
-    }
-    rs.head = (rs.head + n) % rs.slots;
-    rs.count = (rs.count + n > rs.slots) ? rs.slots : rs.count + n;
+    if (int rc = rs.push(n, obs, act, rew, next_obs, done, (cudaStream_t)stream)) return rc;
+    if (rs.per_enabled()) l->chain.launched(kChainNone);
     return 0;
 }
 
@@ -849,16 +815,60 @@ int uavrl_learner_lockstep_restart(uavrl_learner *l)
 {
     if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
     if (l->replay.mode != kReplayLockstep) return 0;
-    l->replay.restart();
-    if (l->per.enabled) {
-        UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-        UAVRL_CUDA(cudaDeviceSynchronize());
-        const size_t G = (size_t)l->per.G;                     // every trainer's tree
-        UAVRL_CUDA(cudaMemset(l->per.leaf, 0, G * l->per.cap * 8));
-        UAVRL_CUDA(cudaMemset(l->per.l1, 0, G * l->per.n1 * 8));
-        UAVRL_CUDA(cudaMemset(l->per.l2, 0, G * l->per.n2 * 8));
-    }
+    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
+    return l->replay.restart();
+}
+
+// ------------------------------------------------------------------ prioritised replay: the SumTrees of the learner's replay
+// store (per.cu).  Their kernels launch outside the dependent-launch chain.
+int uavrl_per_enable(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
+{
+    if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
+    if (l->G > 1) return fail(UAVRL_ERR_INVALID, "prioritised replay is not available on a learner with several trainers");
+    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
+    return l->replay.per_enable(alpha, beta0, beta_inc, eps, err_upper);
+}
+
+int uavrl_per_enable_trainers(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
+{
+    if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
+    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
+    return l->replay.per_enable(alpha, beta0, beta_inc, eps, err_upper);
+}
+
+int uavrl_per_set_priorities(uavrl_learner *l, int32_t n, const int32_t *slots_dev, const double *prio_dev, void *stream)
+{
+    if (!l || !l->replay.per_enabled() || n <= 0 || !slots_dev || !prio_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
+    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
+    if (int rc = l->replay.per_set(n, slots_dev, prio_dev, nullptr, 0, (cudaStream_t)stream)) return rc;
+    l->chain.launched(kChainNone);
     return 0;
+}
+
+int uavrl_per_set_errors(uavrl_learner *l, int32_t n, const int32_t *slots_dev, const float *abs_err_dev, int32_t clip, void *stream)
+{
+    if (!l || !l->replay.per_enabled() || n <= 0 || !slots_dev || !abs_err_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
+    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
+    if (int rc = l->replay.per_set(n, slots_dev, nullptr, abs_err_dev, clip, (cudaStream_t)stream)) return rc;
+    l->chain.launched(kChainNone);
+    return 0;
+}
+
+int uavrl_per_sample(uavrl_learner *l, int32_t B, const double *u_tape_dev, int32_t *slots_out_dev, float *weights_out_dev, void *stream)
+{
+    if (!l || !l->replay.per_enabled() || B <= 0 || !slots_out_dev || !weights_out_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
+    if (l->replay.count <= 0) return fail(UAVRL_ERR_STATE, "the replay is empty");
+    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
+    if (int rc = l->replay.per_sample(l->cfg.seed, B, u_tape_dev, slots_out_dev, weights_out_dev, (cudaStream_t)stream)) return rc;
+    l->chain.launched(kChainNone);
+    return 0;
+}
+
+int uavrl_per_get(uavrl_learner *l, double *leaves_host, double *total_out, double *beta_out)
+{
+    if (!l || !l->replay.per_enabled()) return fail(UAVRL_ERR_INVALID, "prioritised replay not enabled");
+    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
+    return l->replay.per_get(leaves_host, total_out, beta_out);
 }
 
 // ------------------------------------------------------------------ fused NVLink all-reduce + Adam

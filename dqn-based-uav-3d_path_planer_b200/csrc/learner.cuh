@@ -2,7 +2,6 @@
 #pragma once
 #include "net.cuh"
 #include "optim.cuh"
-#include "per.cuh"
 #include "replay.cuh"
 
 namespace uavrl {
@@ -123,19 +122,16 @@ struct uavrl_learner {
     // and weight image is [G][...], trainer g acts for envs [g Ng, (g + 1) Ng) and samples only their transitions
     int32_t G = 1;
     int64_t epoch = 0, adam_t = 0;
-    uavrl::ReplayStore replay;        // int32 actions
+    uavrl::ReplayStore replay;        // int32 actions; with prioritised replay, its SumTrees
     uavrl::LaunchChain chain;         // programmatic dependent launch state of the learner's stream (launch_chain.cuh)
-    // prioritised replay (per.cuh); off unless uavrl_per_enable was called
-    uavrl::PerDev per = {};
-    uint64_t per_calls = 0;
     uint64_t act_calls = 0;
     uint64_t fed_calls = 0;           // ring-sampled federation calls: the Philox counter of their probe draws (federate.cu)
     // data-parallel: one-shot NVLink all-reduce fused with Adam (symmetric buffers exchanged through CUDA IPC), slots of P + 1
     // words (gradient, loss share)
     uavrl::PeerComm comm;
     // owners of the buffers above, one per group allocated and replaced together: parameters, images, maps; the
-    // grown scratch (partials, y / astar, act / dz rows); the PER trees; their scratch
-    uavrl::DevMem mem, parts_mem, td_mem, rows_mem, per_mem, per_scratch_mem;
+    // grown scratch (partials, y / astar, act / dz rows)
+    uavrl::DevMem mem, parts_mem, td_mem, rows_mem;
 };
 
 namespace uavrl {
@@ -165,6 +161,4 @@ int launch_update(uavrl_learner *l, const BatchSrc &src, int B, int global_batch
                   cudaEvent_t *marks = nullptr);
 // the data-parallel form: the gradient step, then the NVLink all-reduce fused with Adam
 int launch_update_dp(uavrl_learner *l, const BatchSrc &src, int B, int global_batch, float *loss_out, cudaStream_t st);
-// the lockstep ring's commit plus, with prioritised replay, the priorities of the frames it makes and drops sampleable
-void lockstep_commit(uavrl_learner *l, cudaStream_t st = nullptr);
 }  // namespace uavrl

@@ -1,11 +1,11 @@
-// per.cu -- prioritised replay kernels + C ABI (design in per.cuh).
+// per.cu -- prioritised replay kernels and the tree operations of the replay store (design in per.cuh).
 #include "per.cuh"
 
 #include <math.h>
 
 #include <vector>
 
-#include "learner.cuh"
+#include "replay.cuh"
 
 namespace uavrl {
 
@@ -150,74 +150,26 @@ __global__ void per_norm_kernel(int B, const double *__restrict__ w_raw, const u
     if (i < B) w[r] = (float)(w_raw[r] / __longlong_as_double((long long)wmax_bits[blockIdx.y]));      // :210
 }
 
-static int per_refresh(uavrl_learner *l, int n, const int32_t *slots, int64_t first, cudaStream_t st)
+static int per_refresh(const PerDev &p, int n, const int32_t *slots, int64_t first, cudaStream_t st)
 {
-    const PerDev &p = l->per;
     const dim3 blocks((unsigned)(((int64_t)n * 32 + 255) / 256), (unsigned)p.G);
     per_level_kernel<<<blocks, 256, 0, st>>>(p, n, slots, first, 1);
     UAVRL_LAUNCHED();
     per_level_kernel<<<blocks, 256, 0, st>>>(p, n, slots, first, 2);
     UAVRL_LAUNCHED();
-    l->chain.launched(kChainNone);
     return 0;
 }
 
-int per_fill_range(uavrl_learner *l, int64_t first_slot, int64_t n, double value, cudaStream_t st, int64_t n_first, double value_rest)
+int ReplayStore::per_enable(double alpha, double beta0, double beta_inc, double eps, double err_upper)
 {
-    if (n <= 0) return 0;
-    per_leaf_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)l->per.G), 256, 0, st>>>(l->per, (int)n, nullptr, first_slot % l->per.cap,
-                                                                                        nullptr, nullptr, 0, value,
-                                                                                        (int)(n_first < 0 ? n : n_first), value_rest);
-    UAVRL_LAUNCHED();
-    return per_refresh(l, (int)n, nullptr, first_slot % l->per.cap, st);
-}
-
-int per_set(uavrl_learner *l, int n, const int32_t *slots, const double *prio, const float *abs_err, int clip, cudaStream_t st)
-{
-    per_leaf_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)l->per.G), 256, 0, st>>>(l->per, n, slots, 0, prio, abs_err,
-                                                                                        prio ? 0 : (clip ? 2 : 1), 0.0, n, 0.0);
-    UAVRL_LAUNCHED();
-    return per_refresh(l, n, slots, 0, st);
-}
-
-int per_sample(uavrl_learner *l, int B, const double *u_tape, int32_t *slot_out, float *w_out, cudaStream_t st)
-{
-    PerDev &p = l->per;
-    const size_t G = (size_t)p.G;
-    if (int rc = grow(l->per_scratch_mem, p.scratch_cap, B, st, false, buf(p.idx, G * B), buf(p.w, G * B), buf(p.abs_err, G * B),
-                      buf(p.w_raw, G * B)))
-        return rc;
-    p.beta = fmin(1.0, p.beta + p.beta_inc);                  // :195
-    UAVRL_CUDA(cudaMemsetAsync(p.wmax_bits, 0, G * 8, st));
-    int grid = (B + 7) / 8;                                   // per trainer, as a stand-alone learner picks it
-    if (grid > num_sms() * 4) grid = num_sms() * 4;
-    // n_entries: the trainer's own transition count (every trainer holds the same number)
-    per_sample_kernel<<<dim3(grid, p.G), 256, 0, st>>>(p, B, u_tape, l->cfg.seed ^ kPerSalt, l->per_calls++, (double)(l->replay.count / l->G),
-                                                       p.beta, slot_out ? slot_out : p.idx, p.w_raw, p.wmax_bits);
-    UAVRL_LAUNCHED();
-    per_norm_kernel<<<dim3((B + 255) / 256, p.G), 256, 0, st>>>(B, p.w_raw, p.wmax_bits, w_out ? w_out : p.w);
-    UAVRL_LAUNCHED();
-    l->chain.launched(kChainNone);
-    return 0;
-}
-
-}  // namespace uavrl
-
-using namespace uavrl;
-
-extern "C" {
-
-static int per_enable_impl(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
-{
-    if (l->per.enabled) return fail(UAVRL_ERR_STATE, "prioritised replay is already enabled");
-    if (l->replay.count != 0) return fail(UAVRL_ERR_STATE, "enable prioritised replay before the first transition is stored");
-    if (l->G > 1 && l->replay.mode != kReplayLockstep)
+    if (per.dev.enabled) return fail(UAVRL_ERR_STATE, "prioritised replay is already enabled");
+    if (count != 0) return fail(UAVRL_ERR_STATE, "enable prioritised replay before the first transition is stored");
+    if (G > 1 && mode != kReplayLockstep)
         return fail(UAVRL_ERR_INVALID, "prioritised replay on a learner with several trainers needs the lockstep ring (lockstep_envs > 0)");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     PerDev p;                                                     // swapped in once complete
     memset(&p, 0, sizeof(p));
-    p.G = l->G;
-    p.cap = l->replay.slots / l->G;                               // trainer-local slots: ring_frames x Ng
+    p.G = G;
+    p.cap = slots / G;                                            // trainer-local slots: ring_frames x Ng
     int64_t pow2 = 1;
     while (pow2 < p.cap) pow2 <<= 1;
     p.rot = pow2 - p.cap;
@@ -226,64 +178,67 @@ static int per_enable_impl(uavrl_learner *l, double alpha, double beta0, double 
     p.alpha = alpha >= 0 ? alpha : 0.6; p.beta = beta0 >= 0 ? beta0 : 0.4; p.beta_inc = beta_inc >= 0 ? beta_inc : 0.001;   // :141-148
     p.eps = eps >= 0 ? eps : 0.01; p.err_upper = err_upper >= 0 ? err_upper : 1.0;
     int rc;
-    const size_t G = (size_t)p.G;
+    const size_t Gs = (size_t)p.G;
     DevMem m;
-    if ((rc = m.alloc(p.leaf, G * p.cap)) || (rc = m.alloc(p.l1, G * p.n1)) || (rc = m.alloc(p.l2, G * p.n2)) ||
-        (rc = m.alloc(p.wmax_bits, G)))
+    if ((rc = m.alloc(p.leaf, Gs * p.cap)) || (rc = m.alloc(p.l1, Gs * p.n1)) || (rc = m.alloc(p.l2, Gs * p.n2)) ||
+        (rc = m.alloc(p.wmax_bits, Gs)))
         return rc;
     p.enabled = 1;
-    l->per = p;
-    l->per_mem = std::move(m);
+    per.dev = p;
+    per.mem = std::move(m);
     return 0;
 }
 
-int uavrl_per_enable(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
+int ReplayStore::per_fill_range(int64_t first_slot, int64_t n, double value, cudaStream_t st, int64_t n_first, double value_rest)
 {
-    if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
-    if (l->G > 1) return fail(UAVRL_ERR_INVALID, "prioritised replay is not available on a learner with several trainers");
-    return per_enable_impl(l, alpha, beta0, beta_inc, eps, err_upper);
+    if (n <= 0) return 0;
+    const PerDev &p = per.dev;
+    per_leaf_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)p.G), 256, 0, st>>>(p, (int)n, nullptr, first_slot % p.cap, nullptr,
+                                                                                   nullptr, 0, value, (int)(n_first < 0 ? n : n_first),
+                                                                                   value_rest);
+    UAVRL_LAUNCHED();
+    return per_refresh(p, (int)n, nullptr, first_slot % p.cap, st);
 }
 
-int uavrl_per_enable_trainers(uavrl_learner *l, double alpha, double beta0, double beta_inc, double eps, double err_upper)
+int ReplayStore::per_set(int n, const int32_t *slot_in, const double *prio, const float *abs_err, int clip, cudaStream_t st)
 {
-    if (!l) return fail(UAVRL_ERR_INVALID, "null learner");
-    return per_enable_impl(l, alpha, beta0, beta_inc, eps, err_upper);
+    const PerDev &p = per.dev;
+    per_leaf_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)p.G), 256, 0, st>>>(p, n, slot_in, 0, prio, abs_err,
+                                                                                   prio ? 0 : (clip ? 2 : 1), 0.0, n, 0.0);
+    UAVRL_LAUNCHED();
+    return per_refresh(p, n, slot_in, 0, st);
 }
 
-int uavrl_per_set_priorities(uavrl_learner *l, int32_t n, const int32_t *slots_dev, const double *prio_dev, void *stream)
+int ReplayStore::per_sample(uint64_t seed, int B, const double *u_tape, int32_t *slot_out, float *w_out, cudaStream_t st)
 {
-    if (!l || !l->per.enabled || n <= 0 || !slots_dev || !prio_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    return per_set(l, n, slots_dev, prio_dev, nullptr, 0, (cudaStream_t)stream);
+    PerDev &p = per.dev;
+    const size_t Gs = (size_t)p.G;
+    if (int rc = grow(per.scratch_mem, p.scratch_cap, B, st, false, buf(p.idx, Gs * B), buf(p.w, Gs * B), buf(p.abs_err, Gs * B),
+                      buf(p.w_raw, Gs * B)))
+        return rc;
+    p.beta = fmin(1.0, p.beta + p.beta_inc);                  // :195
+    UAVRL_CUDA(cudaMemsetAsync(p.wmax_bits, 0, Gs * 8, st));
+    int grid = (B + 7) / 8;                                   // per trainer, as a stand-alone learner picks it
+    if (grid > num_sms() * 4) grid = num_sms() * 4;
+    // n_entries: the trainer's own transition count (every trainer holds the same number)
+    per_sample_kernel<<<dim3(grid, p.G), 256, 0, st>>>(p, B, u_tape, seed ^ kPerSalt, per.calls++, (double)(count / G), p.beta,
+                                                       slot_out ? slot_out : p.idx, p.w_raw, p.wmax_bits);
+    UAVRL_LAUNCHED();
+    per_norm_kernel<<<dim3((B + 255) / 256, p.G), 256, 0, st>>>(B, p.w_raw, p.wmax_bits, w_out ? w_out : p.w);
+    UAVRL_LAUNCHED();
+    return 0;
 }
 
-int uavrl_per_set_errors(uavrl_learner *l, int32_t n, const int32_t *slots_dev, const float *abs_err_dev, int32_t clip, void *stream)
+int ReplayStore::per_get(double *leaves_host, double *total_out, double *beta_out) const
 {
-    if (!l || !l->per.enabled || n <= 0 || !slots_dev || !abs_err_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    return per_set(l, n, slots_dev, nullptr, abs_err_dev, clip, (cudaStream_t)stream);
-}
-
-int uavrl_per_sample(uavrl_learner *l, int32_t B, const double *u_tape_dev, int32_t *slots_out_dev, float *weights_out_dev, void *stream)
-{
-    if (!l || !l->per.enabled || B <= 0 || !slots_out_dev || !weights_out_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
-    if (l->replay.count <= 0) return fail(UAVRL_ERR_STATE, "the replay is empty");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    return per_sample(l, B, u_tape_dev, slots_out_dev, weights_out_dev, (cudaStream_t)stream);
-}
-
-int uavrl_per_get(uavrl_learner *l, double *leaves_host, double *total_out, double *beta_out)
-{
-    if (!l || !l->per.enabled) return fail(UAVRL_ERR_INVALID, "prioritised replay not enabled");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
     UAVRL_CUDA(cudaDeviceSynchronize());
-    const PerDev &p = l->per;
-    const size_t G = (size_t)p.G;
-    if (leaves_host) UAVRL_CUDA(cudaMemcpy(leaves_host, p.leaf, G * p.cap * 8, cudaMemcpyDeviceToHost));
+    const PerDev &p = per.dev;
+    const size_t Gs = (size_t)p.G;
+    if (leaves_host) UAVRL_CUDA(cudaMemcpy(leaves_host, p.leaf, Gs * p.cap * 8, cudaMemcpyDeviceToHost));
     if (total_out) {                                              // [G]: each tree's l2 entries summed in order
-        std::vector<double> h(G * p.n2);
-        UAVRL_CUDA(cudaMemcpy(h.data(), p.l2, G * p.n2 * 8, cudaMemcpyDeviceToHost));
-        for (size_t g = 0; g < G; ++g) {
+        std::vector<double> h(Gs * p.n2);
+        UAVRL_CUDA(cudaMemcpy(h.data(), p.l2, Gs * p.n2 * 8, cudaMemcpyDeviceToHost));
+        for (size_t g = 0; g < Gs; ++g) {
             double s = 0.0;
             for (int64_t k = 0; k < p.n2; ++k) s += h[g * p.n2 + k];
             total_out[g] = s;
@@ -293,4 +248,16 @@ int uavrl_per_get(uavrl_learner *l, double *leaves_host, double *total_out, doub
     return 0;
 }
 
-}  // extern "C"
+int ReplayStore::per_clear()
+{
+    if (!per.dev.enabled) return 0;
+    UAVRL_CUDA(cudaDeviceSynchronize());
+    const PerDev &p = per.dev;
+    const size_t Gs = (size_t)p.G;                                // every trainer's tree
+    UAVRL_CUDA(cudaMemset(p.leaf, 0, Gs * p.cap * 8));
+    UAVRL_CUDA(cudaMemset(p.l1, 0, Gs * p.n1 * 8));
+    UAVRL_CUDA(cudaMemset(p.l2, 0, Gs * p.n2 * 8));
+    return 0;
+}
+
+}  // namespace uavrl

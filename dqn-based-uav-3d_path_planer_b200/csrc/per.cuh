@@ -18,6 +18,9 @@
 // how a stand-alone learner over Ng envs numbers its slots.  Every array is [G][...] (leaf [G][cap], l1 [G][n1], l2 [G][n2],
 // scratch [G][B], wmax_bits [G]) and every kernel takes the trainer from blockIdx.y; cap, rot, alpha, beta and the sampling
 // call counter are shared (the trainers sample in lockstep).  G = 1 is the single tree above.
+//
+// The trees belong to the replay store whose slots they index (ReplayStore::per, replay.cuh); the tree operations are
+// ReplayStore members defined in per.cu.
 #pragma once
 #include <math.h>
 
@@ -38,17 +41,13 @@ struct PerDev {
     int32_t scratch_cap;
 };
 
-}  // namespace uavrl
+// Host state of a store's trees: off unless enabled (uavrl_per_enable / uavrl_per_enable_trainers)
+struct PerTree {
+    PerDev dev = {};                      // the kernels' by-value argument
+    uint64_t calls = 0;                   // sampling calls: the Philox counter of the draws
+    DevMem mem, scratch_mem;              // owners of the trees (and wmax_bits); of the sampling scratch
+    // priority of a transition stored without an error: ReplayTree.push with error 0 -> (0 + eps)^alpha, float32
+    double new_priority() const { return (double)powf((float)dev.eps, (float)dev.alpha); }
+};
 
-struct uavrl_learner;
-namespace uavrl {
-// Every call below acts on each trainer's tree at once (grid y = G): per_fill_range fills the same trainer-local range in
-// every tree; per_set takes [G][n] slots / values; per_sample draws B per trainer into [G][B] outputs (u_tape [G][B]).
-// contiguous slots (mod cap): the first n_first get `value`, the rest `value_rest` (n_first < 0: all get `value`)
-int per_fill_range(uavrl_learner *l, int64_t first_slot, int64_t n, double value, cudaStream_t st, int64_t n_first = -1,
-                   double value_rest = 0.0);
-// priority of a transition stored without an error: ReplayTree.push with error 0 -> (0 + eps)^alpha, float32
-inline double per_new_priority(const PerDev &p) { return (double)powf((float)p.eps, (float)p.alpha); }
-int per_sample(uavrl_learner *l, int B, const double *u_tape, int32_t *slot_out, float *w_out, cudaStream_t st);
-int per_set(uavrl_learner *l, int n, const int32_t *slots, const double *prio, const float *abs_err, int clip, cudaStream_t st);
 }  // namespace uavrl

@@ -1,5 +1,6 @@
-// replay.cu -- the replay store shared by the Q-network and SAC learners (replay.cuh): allocation, batch sources, the lockstep
-// iteration and the host read-back.
+// replay.cu -- the replay store shared by the Q-network and SAC learners (replay.cuh): allocation, batch sources, the paired
+// push, the lockstep iteration and the host read-back.  The prioritised-replay trees follow every change of the store here;
+// their operations are in per.cu.
 #include "replay.cuh"
 
 namespace uavrl {
@@ -21,6 +22,23 @@ __global__ void replay_gather_kernel(int n, int in, BatchSrc src, const int64_t 
         if (a2) { a2[2 * i] = src.act2[2 * t.slot]; a2[2 * i + 1] = src.act2[2 * t.slot + 1]; }
         if (r) r[i] = src.rew[t.slot];
         if (d) d[i] = src.done_u8[t.slot];
+    }
+}
+
+// ReplayStore::push (paired rows)
+__global__ void push_kernel(int n, int in, int64_t head, int64_t cap, const float *__restrict__ obs,
+                            const int32_t *__restrict__ act, const float *__restrict__ rew,
+                            const float *__restrict__ next_obs, const uint8_t *__restrict__ done,
+                            float *__restrict__ frames, int32_t *__restrict__ r_act, float *__restrict__ r_rew,
+                            uint8_t *__restrict__ r_done)
+{
+    const int64_t total = (int64_t)n * in;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t t = i / in, k = i - t * in;
+        const int64_t slot = (head + t) % cap;
+        frames[(2 * slot) * in + k] = obs[i];
+        frames[(2 * slot + 1) * in + k] = next_obs[i];
+        if (k == 0) { r_act[slot] = act[t]; r_rew[slot] = rew[t]; r_done[slot] = done[t]; }
     }
 }
 
@@ -67,6 +85,24 @@ BatchSrc ReplayStore::source(uint64_t seed, int64_t epoch, const int32_t *idx_ta
     return s;
 }
 
+int ReplayStore::push(int32_t n, const float *obs, const int32_t *a, const float *r, const float *next_obs, const uint8_t *d,
+                      cudaStream_t st)
+{
+    const int64_t total = (int64_t)n * in_dim;
+    const int threads = 256;
+    int blocks = (int)((total + threads - 1) / threads);
+    if (blocks > num_sms() * 8) blocks = num_sms() * 8;
+    push_kernel<<<blocks, threads, 0, st>>>(n, in_dim, head, slots, obs, a, r, next_obs, d, frames, act, rew, done);
+    UAVRL_LAUNCHED();
+    if (per_enabled()) {                                          // ReplayTree.push with error 0; uavrl_per_set_errors refines it
+        int rc = per_fill_range(head, n, per.new_priority(), st);
+        if (rc) return rc;
+    }
+    head = (head + n) % slots;
+    count = (count + n > slots) ? slots : count + n;
+    return 0;
+}
+
 ReplayStore::Iteration ReplayStore::begin() const
 {
     const int64_t f = head, fn = (head + 1) % ring_frames;
@@ -79,10 +115,18 @@ ReplayStore::Iteration ReplayStore::begin() const
     return it;
 }
 
-void ReplayStore::commit()
+int ReplayStore::commit(cudaStream_t st)
 {
+    if (per_enabled()) {
+        // the frame just completed becomes sampleable with the priority of an error-less push; the frame that now
+        // receives the next observations (the ring's oldest) stops being a transition.  Trainer-local slots: every trainer's
+        // tree gets the same Ng + Ng slots of its own env block
+        const int64_t Ng = N / G;
+        if (int rc = per_fill_range(head * Ng, 2 * Ng, per.new_priority(), st, Ng, 0.0)) return rc;
+    }
     head = (head + 1) % ring_frames;
     count = count_after_commit();
+    return 0;
 }
 
 int64_t ReplayStore::count_after_commit() const
@@ -91,10 +135,11 @@ int64_t ReplayStore::count_after_commit() const
     return (count + N > max_count) ? max_count : count + N;
 }
 
-void ReplayStore::restart()
+int ReplayStore::restart()
 {
     count = 0;
     frame0_valid = false;
+    return per_clear();
 }
 
 int ReplayStore::gather(int32_t n, const int64_t *idx, float *s, int32_t *a, float *a2, float *r, float *s2, uint8_t *d) const

@@ -10,6 +10,7 @@
 //             index (k / Ng) N + g Ng + k mod Ng.
 #pragma once
 #include "common.cuh"
+#include "per.cuh"
 
 namespace uavrl {
 
@@ -184,26 +185,48 @@ struct ReplayStore {
     int64_t count = 0;                // valid transitions
     bool frame0_valid = false;        // lockstep: frame `head` holds the current observations
     DevMem mem;                       // owns frames, act / act2, rew and done
+    PerTree per;                      // prioritised replay: one SumTree per trainer over its own slots (per.cuh)
 
     // capacity transitions over all trainers; N > 0: lockstep ring, where every trainer keeps the frames a stand-alone store
     // with capacity / G transitions over N / G envs would keep (at least 2); N == 0: paired rows
     int alloc(int64_t capacity, int32_t n_envs, int32_t n_trainers, int32_t in, bool pair_actions);
     // trainer-local sampling: Philox keyed by seed ^ kSampleSalt and the epoch, or a device tape of logical indices
     BatchSrc source(uint64_t seed, int64_t epoch, const int32_t *idx_tape) const;
+    // paired rows: n transitions at head (the oldest are overwritten once full), with prioritised replay at the priority of an
+    // error-less push
+    int push(int32_t n, const float *obs, const int32_t *a, const float *r, const float *next_obs, const uint8_t *d, cudaStream_t st);
     // lockstep iteration: where this iteration's observations, actions, rewards and done flags go; commit makes them a
-    // transition group (the oldest is dropped once the ring is full)
+    // transition group (the oldest is dropped once the ring is full), with prioritised replay first giving that group the
+    // priority of an error-less push and the dropped one 0
     struct Iteration { float *obs_t, *obs_next; int32_t *act; float *act2, *rew; uint8_t *done; };
     Iteration begin() const;
-    void commit();
+    int commit(cudaStream_t st);
     int64_t count_after_commit() const;   // lockstep: `count` once the next commit has run
     // an update of `batch` transitions per trainer may sample (PathPlan_City.py:383): every trainer holds more than batch, now or
     // (lockstep) once the next commit has run
     bool ready(int64_t batch) const { return count / G > batch; }
     bool ready_after_commit(int64_t batch) const { return count_after_commit() / G > batch; }
-    // forget every transition; the next iteration re-observes into frame `head`
-    void restart();
+    // forget every transition and clear the trees; the next iteration re-observes into frame `head`
+    int restart();
     // n whole-store logical indices (0 = oldest) to host arrays; any output may be null
     int gather(int32_t n, const int64_t *idx, float *s, int32_t *a, float *a2, float *r, float *s2, uint8_t *d) const;
+
+    // ---- prioritised replay (per.cu).  Every call acts on each trainer's tree at once (grid y = G) under trainer-local slots.
+    bool per_enabled() const { return per.dev.enabled != 0; }
+    // G trees of slots / G leaves; a negative hyper-parameter takes the reference's default.  Refused once a transition is
+    // stored, and on a grouped paired store
+    int per_enable(double alpha, double beta0, double beta_inc, double eps, double err_upper);
+    // contiguous slots (mod cap) of every tree: the first n_first get `value`, the rest `value_rest` (n_first < 0: all get `value`)
+    int per_fill_range(int64_t first_slot, int64_t n, double value, cudaStream_t st, int64_t n_first = -1, double value_rest = 0.0);
+    // [G][n] slots: explicit priorities (prio), or the push (clip = 0) / batch_update (clip = 1) rule on |errors|
+    int per_set(int n, const int32_t *slot_in, const double *prio, const float *abs_err, int clip, cudaStream_t st);
+    // ReplayTree.sample2 of B per trainer, keyed by seed ^ kPerSalt: [G][B] slots and weights (null: the scratch per.dev.idx /
+    // per.dev.w), uniforms from u_tape [G][B] when given
+    int per_sample(uint64_t seed, int B, const double *u_tape, int32_t *slot_out, float *w_out, cudaStream_t st);
+    // host read-back after a device synchronise: leaves [G][cap], totals [G], beta; any output may be null
+    int per_get(double *leaves, double *total, double *beta) const;
+    // every tree's leaves and sums to 0 (beta and the sampling counter are kept)
+    int per_clear();
 };
 
 }  // namespace uavrl

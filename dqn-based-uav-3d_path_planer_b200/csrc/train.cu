@@ -49,8 +49,9 @@ static int env_step(uavrl_env *env, uavrl_sac *, const ReplayStore::Iteration &i
     return launch_env_step(env->d, UAVRL_ACT_CONT_F32X2, io.act2, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st);
 }
 
-static void commit(uavrl_learner *l, cudaStream_t st) { lockstep_commit(l, st); }    // + prioritised-replay priorities
-static void commit(uavrl_sac *s, cudaStream_t) { s->replay.commit(); }
+// the commit's prioritised-replay priority fill launches outside the Q-network's dependent-launch chain
+static void committed(uavrl_learner *l) { if (l->replay.per_enabled()) l->chain.launched(kChainNone); }
+static void committed(uavrl_sac *) {}
 
 // PathPlan_City.update -> Trainer.update (:757-776) on batch_size transitions per trainer sampled through src.  dp_batch > 0:
 // data-parallel over that global batch; marks (profiling, may be null): launch_update's three events
@@ -116,7 +117,8 @@ static int iteration(uavrl_env *env, Learner *l, float eps, int n_updates, int d
     if (ev) UAVRL_CUDA(cudaEventRecord(ev[1], st));
     if ((rc = env_step(env, l, io, st))) return rc;
     if (ev) UAVRL_CUDA(cudaEventRecord(ev[2], st));
-    commit(l, st);
+    if ((rc = rs.commit(st))) return rc;
+    committed(l);
     for (int u = 0; u < n_updates; ++u) {
         l->epoch += 1;
         if (!rs.ready(l->cfg.batch_size)) continue;

@@ -406,13 +406,11 @@ class Learner:
     # -- prioritised replay (SumTree + ReplayTree of the reference, BaseClass/replay_buffer.py:57-223)
     def per_enable(self, alpha=-1.0, beta0=-1.0, beta_inc=-1.0, eps=-1.0, err_upper=-1.0):
         check(_lib.lib().uavrl_per_enable(self.h, alpha, beta0, beta_inc, eps, err_upper))
-        self.per_slots = int(self.cfg.replay_capacity) if not self.cfg.lockstep_envs else None
 
     def per_enable_trainers(self, alpha=-1.0, beta0=-1.0, beta_inc=-1.0, eps=-1.0, err_upper=-1.0):
         """Prioritised replay with one tree per trainer (include/uavrl.h uavrl_per_enable_trainers); per_enable when G = 1.
         With G > 1 the per_* methods then take and return (G, ...) arrays of trainer-local slots."""
         check(_lib.lib().uavrl_per_enable_trainers(self.h, alpha, beta0, beta_inc, eps, err_upper))
-        self.per_slots = int(self.cfg.replay_capacity) if not self.cfg.lockstep_envs else None
 
     def _per_shape(self, n):
         return (n,) if self.G == 1 else (self.G, n)

@@ -1,6 +1,7 @@
-"""The CUDA sources' include graph keeps the SAC learner and the shared optimiser apart from the Q-network learner: neither
-sac.cu nor what it includes reaches learner.cuh (the Q-network's handle, tensor-core net and Q-head arithmetic), so a change
-there cannot recompile or break SAC; and the optimiser / exchange header does not reach the SAC learner either."""
+"""The CUDA sources' include graph keeps the SAC learner, the shared optimiser and the replay store with its prioritised-replay
+trees apart from the Q-network learner: none of them reaches learner.cuh (the Q-network's handle, tensor-core net and Q-head
+arithmetic), so a change there cannot recompile or break them; and neither the optimiser / exchange header nor the replay and
+tree headers reach the SAC learner."""
 import os
 import re
 
@@ -24,7 +25,8 @@ def closure(name):
     return {os.path.basename(p) for p in seen}
 
 
-@pytest.mark.parametrize("name", ["sac.cu", "sac.cuh", "mlp_tile.cuh", "net.cuh", "optim.cuh", "optim.cu"])
+@pytest.mark.parametrize("name", ["sac.cu", "sac.cuh", "mlp_tile.cuh", "net.cuh", "optim.cuh", "optim.cu",
+                                  "per.cu", "per.cuh", "replay.cu", "replay.cuh"])
 def test_shared_and_sac_sources_do_not_reach_the_q_learner(name):
     assert os.path.exists(os.path.join(CSRC, name)), name
     assert "learner.cuh" not in closure(name)
@@ -32,6 +34,12 @@ def test_shared_and_sac_sources_do_not_reach_the_q_learner(name):
 
 def test_optimiser_header_does_not_reach_sac():
     assert "sac.cuh" not in closure("optim.cuh")
+
+
+@pytest.mark.parametrize("name", ["per.cuh", "replay.cuh"])
+def test_replay_headers_do_not_reach_sac(name):
+    assert os.path.exists(os.path.join(CSRC, name)), name
+    assert "sac.cuh" not in closure(name)
 
 
 def test_closure_follows_includes_transitively():

@@ -199,6 +199,40 @@ def test_lockstep_commit_layout(env_golden, env27_golden):
     env.close(); L.close()
 
 
+@pytest.mark.parametrize("G", [1, 4])
+def test_lockstep_restart_clears_trees(env_golden, env27_golden, G):
+    """lockstep_restart after updates have re-prioritised leaves empties the ring and every tree (leaves and totals 0, beta
+    kept); the first iteration after it gives exactly one frame of Ng slots per tree the push priority eps^alpha."""
+    Ng, F = 64, 12
+    cap = (F + 1) * Ng
+    env = generated_env(env_golden, env27_golden, G * Ng, pool=512)
+    L = learner(SHIPPED[0], G, seed=1, algo=engine.ALGO_DDQN, batch_size=Ng, replay_capacity=G * Ng * F, lockstep_envs=G * Ng,
+                update_loop=3)
+    L.init_params(0)
+    L.per_enable_trainers()
+    st = engine.train_run(env, L, 20, eps=0.3)
+    assert st.updates == 19
+    leaves, _, beta = L.per_state(cap)
+    leaves = leaves.reshape(G, cap)
+    for g in range(G):
+        assert (np.abs(leaves[g][leaves[g] != 0] - P0) > 1e-9).sum() > Ng, g     # sampled transitions were re-prioritised
+    L.lockstep_restart()
+    env.reset(0)
+    assert L.replay_size() == 0
+    leaves, totals, beta1 = L.per_state(cap)
+    assert not leaves.any() and not np.any(totals)
+    assert beta1 == beta
+    st = engine.train_run(env, L, 1, eps=0.3)
+    assert st.updates == 0 and L.replay_size() == G * Ng
+    leaves = L.per_state(cap)[0].reshape(G, F + 1, Ng)
+    for g in range(G):
+        full = np.where(leaves[g].any(1))[0]
+        assert len(full) == 1, g
+        assert (leaves[g, full[0]] != 0).all()
+        np.testing.assert_allclose(leaves[g, full[0]], P0, rtol=1e-6, atol=0)
+    env.close(); L.close()
+
+
 def test_one_trainer_and_refusals(env_golden, env27_golden):
     # G = 1: per_enable_trainers is per_enable
     runs = []

@@ -132,7 +132,7 @@ def test_weighted_update_vs_float64_and_oracle(dqn_golden, shape, leg, algo, var
 
 # ---------------------------------------------------------------------------------------------------------------------
 # The integrated PER update: uavrl_learner_update draws its slots with the sampler's Philox stream (key seed ^ 0x9E12, counter
-# per_calls), which per_sample without a tape reproduces on a twin learner.
+# the count of sampling calls), which per_sample without a tape reproduces on a twin learner.
 PER_BATCHES = [64, 4096, 6000, 12000]
 ALPHA, EPS_PER = 0.6, 0.01
 
