@@ -150,6 +150,12 @@ SIGNATURES = {
     "uavrl_sac_replay_size": (C.c_int64, [VP]),
     "uavrl_sac_replay_gather": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP, VP, VP]),
     "uavrl_sac_update_replay": (C.c_int, [VP, VP, VP, VP, VP, VP]),
+    "uavrl_sac_per_enable": (C.c_int, [VP, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double]),
+    "uavrl_sac_per_sample": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP]),
+    "uavrl_sac_per_set_errors": (C.c_int, [VP, C.c_int32, VP, VP, C.c_int32, VP]),
+    "uavrl_sac_per_set_priorities": (C.c_int, [VP, C.c_int32, VP, VP, VP]),
+    "uavrl_sac_per_get": (C.c_int, [VP, VP, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "uavrl_sac_update_batch_per": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP]),
     "uavrl_sac_comm_init": (C.c_int, [VP, C.c_int32, C.c_int32, VP]),
     "uavrl_sac_comm_connect": (C.c_int, [VP, VP]),
     "uavrl_sac_update_replay_dp": (C.c_int, [VP, VP, VP, VP, C.c_int32, VP, VP]),

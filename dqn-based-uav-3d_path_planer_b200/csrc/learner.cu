@@ -392,15 +392,13 @@ static int mark(cudaEvent_t *marks, int k, cudaStream_t st)
 // training kernel on the fp32 path, which computes the weight gradients itself)
 static Grads launch_grads(uavrl_learner *l, const BatchSrc &src_in, int B, int global_batch, cudaStream_t st, cudaEvent_t *marks)
 {
-    Grads g = { 0, 0, 0, 1.0f / (float)global_batch, l->replay.per_enabled() && src_in.mode != kBatchExplicit && !src_in.idx_tape };
+    Grads g = { 0, 0, 0, 1.0f / (float)global_batch, l->replay.per_samples(src_in) };
     BatchSrc src = src_in;
     if (g.per) {
-        // ReplayTree.sample2 -> slots + importance weights; |Q - y| comes back for batch_update (per_write_back).
-        // Grouped learner: [G][B] trainer-local slots, weights and errors; trainer_src hands trainer g its row of each
-        if ((g.rc = l->replay.per_sample(l->cfg.seed, B, nullptr, nullptr, nullptr, st))) return g;
+        // ReplayTree.sample2 -> slots + importance weights; |Q - y| comes back for batch_update (per_write_back)
+        src = l->replay.per_source(l->cfg.seed, B, src_in, st, &g.rc);
+        if (g.rc) return g;
         l->chain.launched(kChainNone);                    // prioritised-replay kernels launch outside the chain
-        const PerDev &p = l->replay.per.dev;
-        src.idx_tape = p.idx; src.idx_is_slot = 1; src.is_w = p.w; src.abs_err = p.abs_err;
     }
     const Route r = learner_route(l, B);
     const int n_tiles = (B + kTile - 1) / kTile;
@@ -499,8 +497,7 @@ static int launch_allreduce_adam(uavrl_learner *l, const Grads &g, float *loss_o
 static int per_write_back(uavrl_learner *l, const Grads &g, int B, cudaStream_t st)
 {
     if (!g.per) return 0;
-    const PerDev &p = l->replay.per.dev;
-    if (int rc = l->replay.per_set(B, p.idx, nullptr, p.abs_err, 1, st)) return rc;
+    if (int rc = l->replay.per_write_back(B, st)) return rc;
     l->chain.launched(kChainNone);
     return 0;
 }
@@ -838,37 +835,33 @@ int uavrl_per_enable_trainers(uavrl_learner *l, double alpha, double beta0, doub
 
 int uavrl_per_set_priorities(uavrl_learner *l, int32_t n, const int32_t *slots_dev, const double *prio_dev, void *stream)
 {
-    if (!l || !l->replay.per_enabled() || n <= 0 || !slots_dev || !prio_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    if (int rc = l->replay.per_set(n, slots_dev, prio_dev, nullptr, 0, (cudaStream_t)stream)) return rc;
+    if (int rc = per_entry_set(l ? &l->replay : nullptr, l ? l->cfg.device : 0, n, slots_dev, prio_dev, nullptr, 0,
+                               (cudaStream_t)stream))
+        return rc;
     l->chain.launched(kChainNone);
     return 0;
 }
 
 int uavrl_per_set_errors(uavrl_learner *l, int32_t n, const int32_t *slots_dev, const float *abs_err_dev, int32_t clip, void *stream)
 {
-    if (!l || !l->replay.per_enabled() || n <= 0 || !slots_dev || !abs_err_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    if (int rc = l->replay.per_set(n, slots_dev, nullptr, abs_err_dev, clip, (cudaStream_t)stream)) return rc;
+    if (int rc = per_entry_set(l ? &l->replay : nullptr, l ? l->cfg.device : 0, n, slots_dev, nullptr, abs_err_dev, clip, (cudaStream_t)stream))
+        return rc;
     l->chain.launched(kChainNone);
     return 0;
 }
 
 int uavrl_per_sample(uavrl_learner *l, int32_t B, const double *u_tape_dev, int32_t *slots_out_dev, float *weights_out_dev, void *stream)
 {
-    if (!l || !l->replay.per_enabled() || B <= 0 || !slots_out_dev || !weights_out_dev) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
-    if (l->replay.count <= 0) return fail(UAVRL_ERR_STATE, "the replay is empty");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    if (int rc = l->replay.per_sample(l->cfg.seed, B, u_tape_dev, slots_out_dev, weights_out_dev, (cudaStream_t)stream)) return rc;
+    if (int rc = per_entry_sample(l ? &l->replay : nullptr, l ? l->cfg.device : 0, l ? l->cfg.seed : 0, B, u_tape_dev, slots_out_dev,
+                                  weights_out_dev, (cudaStream_t)stream))
+        return rc;
     l->chain.launched(kChainNone);
     return 0;
 }
 
 int uavrl_per_get(uavrl_learner *l, double *leaves_host, double *total_out, double *beta_out)
 {
-    if (!l || !l->replay.per_enabled()) return fail(UAVRL_ERR_INVALID, "prioritised replay not enabled");
-    UAVRL_CUDA(cudaSetDevice(l->cfg.device));
-    return l->replay.per_get(leaves_host, total_out, beta_out);
+    return per_entry_get(l ? &l->replay : nullptr, l ? l->cfg.device : 0, leaves_host, total_out, beta_out);
 }
 
 // ------------------------------------------------------------------ fused NVLink all-reduce + Adam

@@ -229,6 +229,40 @@ int ReplayStore::per_sample(uint64_t seed, int B, const double *u_tape, int32_t 
     return 0;
 }
 
+BatchSrc ReplayStore::per_source(uint64_t seed, int B, const BatchSrc &src_in, cudaStream_t st, int *rc)
+{
+    BatchSrc src = src_in;
+    if ((*rc = per_sample(seed, B, nullptr, nullptr, nullptr, st))) return src;
+    // grouped learner: [G][B] trainer-local slots, weights and errors; trainer_src hands trainer g its row of each
+    const PerDev &p = per.dev;
+    src.idx_tape = p.idx; src.idx_is_slot = 1; src.is_w = p.w; src.abs_err = p.abs_err;
+    return src;
+}
+
+int per_entry_set(ReplayStore *rs, int device, int32_t n, const int32_t *slots, const double *prio, const float *abs_err, int32_t clip,
+                  cudaStream_t st)
+{
+    if (!rs || !rs->per_enabled() || n <= 0 || !slots || (!prio && !abs_err))
+        return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
+    UAVRL_CUDA(cudaSetDevice(device));
+    return rs->per_set(n, slots, prio, abs_err, clip, st);
+}
+
+int per_entry_sample(ReplayStore *rs, int device, uint64_t seed, int32_t B, const double *u_tape, int32_t *slots, float *w, cudaStream_t st)
+{
+    if (!rs || !rs->per_enabled() || B <= 0 || !slots || !w) return fail(UAVRL_ERR_INVALID, "bad argument / prioritised replay not enabled");
+    if (rs->count <= 0) return fail(UAVRL_ERR_STATE, "the replay is empty");
+    UAVRL_CUDA(cudaSetDevice(device));
+    return rs->per_sample(seed, B, u_tape, slots, w, st);
+}
+
+int per_entry_get(ReplayStore *rs, int device, double *leaves, double *total, double *beta)
+{
+    if (!rs || !rs->per_enabled()) return fail(UAVRL_ERR_INVALID, "prioritised replay not enabled");
+    UAVRL_CUDA(cudaSetDevice(device));
+    return rs->per_get(leaves, total, beta);
+}
+
 int ReplayStore::per_get(double *leaves_host, double *total_out, double *beta_out) const
 {
     UAVRL_CUDA(cudaDeviceSynchronize());

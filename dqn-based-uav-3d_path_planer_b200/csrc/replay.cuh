@@ -227,6 +227,20 @@ struct ReplayStore {
     int per_get(double *leaves, double *total, double *beta) const;
     // every tree's leaves and sums to 0 (beta and the sampling counter are kept)
     int per_clear();
+    // an update samples through the trees when they are enabled, the batch comes from the store and no index tape is injected
+    bool per_samples(const BatchSrc &src) const { return per_enabled() && src.mode != kBatchExplicit && !src.idx_tape; }
+    // such an update's batch: ReplayTree.sample2 of B per trainer into the scratch, and src reading its rows, importance
+    // weights and |errors| through it (*rc != 0: the sample failed)
+    BatchSrc per_source(uint64_t seed, int B, const BatchSrc &src, cudaStream_t st, int *rc);
+    // ReplayTree.batch_update of that batch, once the update has written the |errors| to the scratch
+    int per_write_back(int B, cudaStream_t st) { return per_set(B, per.dev.idx, nullptr, per.dev.abs_err, 1, st); }
 };
+
+// The checks and calls of the prioritised-replay entry points (uavrl_per_*, uavrl_sac_per_*) on a handle's store; rs is null
+// when the handle is.  Each refuses a store without trees
+int per_entry_set(ReplayStore *rs, int device, int32_t n, const int32_t *slots, const double *prio, const float *abs_err, int32_t clip,
+                  cudaStream_t st);
+int per_entry_sample(ReplayStore *rs, int device, uint64_t seed, int32_t B, const double *u_tape, int32_t *slots, float *w, cudaStream_t st);
+int per_entry_get(ReplayStore *rs, int device, double *leaves, double *total, double *beta);
 
 }  // namespace uavrl

@@ -216,7 +216,10 @@ __global__ void __launch_bounds__(kNetThreads) sac_target_kernel(SacArgs a)
 }
 
 // ------------------------------------------------------------------ critic update (:343-360)
-template <bool GR>
+// PW (prioritised replay): row b's squared errors and head gradient are scaled by its importance weight w_b (src.is_w), so
+// L_k = mean over B x A of w_b (Q_k - y)^2, and after critic 2 the row's priority error
+// e_b = 0.5 (|min(Q1, Q2)_0 - y_0| + |min(Q1, Q2)_1 - y_1|) goes to src.abs_err (when given), from the critics before this step
+template <bool GR, bool PW>
 __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
 {
     extern __shared__ __align__(16) float smem[];
@@ -227,27 +230,32 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
     __shared__ uint64_t bar[2];
     __shared__ const float *rows[kTile];
     __shared__ float s_act[kTile][kSacA], s_sq[kTile];
+    // PW: row weights; critic 1's outputs through critic 2; thread 0's squared-error sums and 1 / (Bg A) (kept out of registers)
+    __shared__ float s_w[PW ? kTile : 1], s_q1[PW ? kTile : 1][kSacA], s_acc[3];
     if (threadIdx.x == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); fence_barrier_init(); }
     __syncthreads();
     if (threadIdx.x == 0) { stage_weights(cn, sac_img<GR>(a.img_c1, cn), RC, &bar[0]); stage_weights(cn, sac_img<GR>(a.img_c2, cn), WC2, &bar[1]); }
-    uint32_t pkey[4];
-    Philox::gen(sac_sample_key<GR>(a), a.src.epoch, 0x5A17ull, pkey);
+    uint32_t pkey[4];                                                       // PW: derived per tile (kept out of registers)
+    if constexpr (!PW) Philox::gen(sac_sample_key<GR>(a), a.src.epoch, 0x5A17ull, pkey);
     const float inv = 1.f / ((float)a.Bg * (float)kSacA);
     float sq[2] = { 0.f, 0.f };
+    if constexpr (PW) { if (threadIdx.x == 0) { s_acc[0] = s_acc[1] = 0.f; s_acc[2] = inv; } }
     bool ready = false;
     int iter = 0;
     for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x, ++iter) {
         if (threadIdx.x < kTile) {
             const int gb = t * kTile + threadIdx.x;
             Transition tr; tr.s = nullptr; tr.ax = tr.ay = 0.f;
+            if constexpr (PW) Philox::gen(sac_sample_key<GR>(a), a.src.epoch, 0x5A17ull, pkey);
             if (gb < a.B) tr = resolve_transition(sac_src<GR>(a), gb, cn.in_dim - kSacA, pkey);
+            if constexpr (PW) s_w[threadIdx.x] = (gb < a.B) ? sac_src<GR>(a).is_w[gb] : 0.f;
             rows[threadIdx.x] = (gb < a.B) ? tr.s : nullptr; s_act[threadIdx.x][0] = tr.ax; s_act[threadIdx.x][1] = tr.ay;
         }
         __syncthreads();
         load_rows(rows, dYa, gld * 2, cn.in_dim - kSacA);                   // stage s in the (still unused) gradient planes: 32 x 2 gld
         __syncthreads();
         build_critic_input(dYa, gld * 2, cn.in_dim - kSacA, RC + cn.act_off[0], cn.act_ld[0], s_act);
-        if (!ready) { mbar_wait(&bar[0], 0); mbar_wait(&bar[1], 0); ready = true; }
+        if (PW ? iter == 0 : !ready) { mbar_wait(&bar[0], 0); mbar_wait(&bar[1], 0); ready = true; }
         __syncthreads();
         for (int which = 0; which < 2; ++which) {
             const float *sw = which ? WC2 : RC;
@@ -261,15 +269,31 @@ __global__ void __launch_bounds__(kNetThreads) sac_critic_kernel(SacArgs a)
                     for (int j = 0; j < kSacA; ++j) {
                         const float diff = Q[b * 32 + j] - sac_td<GR>(a)[(size_t)gb * kSacA + j];
                         e2 += diff * diff;
-                        g[j] = 2.f * diff * inv;
+                        if constexpr (PW) g[j] = 2.f * s_w[b] * diff * s_acc[2];
+                        else g[j] = 2.f * diff * inv;
                     }
-                s_sq[b] = e2;
+                if constexpr (PW) {
+                    s_sq[b] = s_w[b] * e2;
+                    if (which == 0) { s_q1[b][0] = Q[b * 32]; s_q1[b][1] = Q[b * 32 + 1]; }
+                } else {
+                    s_sq[b] = e2;
+                }
             }
             __syncthreads();
-            if (threadIdx.x == 0) { float s = 0.f; for (int b = 0; b < kTile; ++b) s += s_sq[b]; sq[which] += s; }
+            if (threadIdx.x == 0) { float s = 0.f; for (int b = 0; b < kTile; ++b) s += s_sq[b]; if constexpr (PW) s_acc[which] += s; else sq[which] += s; }
             critic_backward_tile(cn, sw, RC, dYa, dYb, gld, (which ? a.part_c2 : a.part_c1) + sac_part<GR>() * cn.P, iter > 0, nullptr, 0);
         }
+        if constexpr (PW) {                                                 // Q still holds critic 2's outputs
+            const int b = threadIdx.x, gb = t * kTile + b;
+            float *abs_err = sac_src<GR>(a).abs_err;
+            if (b < kTile && gb < a.B && abs_err) {
+                const float *y = sac_td<GR>(a) + (size_t)gb * kSacA;
+                const float m0 = fminf(s_q1[b][0], Q[b * 32]), m1 = fminf(s_q1[b][1], Q[b * 32 + 1]);
+                abs_err[gb] = 0.5f * (fabsf(m0 - y[0]) + fabsf(m1 - y[1]));
+            }
+        }
     }
+    if constexpr (PW) { if (threadIdx.x == 0) { sq[0] = s_acc[0]; sq[1] = s_acc[1]; } }
     if (threadIdx.x == 0) { a.stat[sac_part<GR>() * 4 + 0] = sq[0]; a.stat[sac_part<GR>() * 4 + 1] = sq[1]; }
 }
 
@@ -519,13 +543,15 @@ static size_t smem_critic(const SacShape &s) { return (size_t)(s.critic.smem_tot
 static size_t smem_actor(const SacShape &s) { return (size_t)(s.actor.smem_total_floats + s.critic.smem_total_floats + s.critic.smem_w_floats + 2 * kTile * s.gld + 3 * kTile * 32) * 4; }
 static size_t smem_act(const SacShape &s) { return (size_t)(s.actor.smem_total_floats + kTile * 32) * 4; }
 
-// dynamic and static shared memory of one CTA of each kernel: target, critic, actor, act
-static int sac_smem_total(const SacShape &s, size_t out[4])
+// dynamic and static shared memory of one CTA of each kernel: target, critic, actor, act, and the weighted (prioritised-replay)
+// critic, which adds its row weights, critic-1 outputs and loss sums to the critic's static shared memory
+static int sac_smem_total(const SacShape &s, size_t out[5])
 {
-    const void *k[4] = { (const void *)sac_target_kernel<true>, (const void *)sac_critic_kernel<true>, (const void *)sac_actor_kernel<true>,
-                         (const void *)sac_act_kernel<true> };     // the one-trainer instances declare the same static shared memory
-    const size_t dyn[4] = { smem_target(s), smem_critic(s), smem_actor(s), smem_act(s) };
-    for (int i = 0; i < 4; ++i) {
+    const void *k[5] = { (const void *)sac_target_kernel<true>, (const void *)sac_critic_kernel<true, false>, (const void *)sac_actor_kernel<true>,
+                         (const void *)sac_act_kernel<true>,      // the one-trainer instances declare the same static shared memory
+                         (const void *)sac_critic_kernel<true, true> };
+    const size_t dyn[5] = { smem_target(s), smem_critic(s), smem_actor(s), smem_act(s), smem_critic(s) };
+    for (int i = 0; i < 5; ++i) {
         cudaFuncAttributes fa;
         UAVRL_CUDA(cudaFuncGetAttributes(&fa, k[i]));
         out[i] = dyn[i] + fa.sharedSizeBytes;
@@ -602,12 +628,21 @@ static int sac_grid(const uavrl_sac *s, int B)
 }
 
 // The update's first half on B rows per trainer (losses averaged over Bg rows): one Adam step counted, the TD targets, both
-// critics' gradient partials and squared-error sums
-static int sac_critic_phase(uavrl_sac *s, const BatchSrc &src, int B, int Bg, const float *eps_next, cudaStream_t st)
+// critics' gradient partials and squared-error sums.  Prioritised replay (ReplayStore::per_samples): the batch is drawn from
+// the trees first and src then reads through that sample, so the actor phase, given the same src, takes the same rows; the
+// critic kernel weights its losses (any src with importance weights does) and its |errors| go back to the trees once it has run
+static int sac_critic_phase(uavrl_sac *s, BatchSrc &src, int B, int Bg, const float *eps_next, cudaStream_t st)
 {
     const int grid = sac_grid(s, B);
     int rc = sac_scratch(s, B, grid, st);
     if (rc) return rc;
+    const bool per = s->replay.per_samples(src);
+    if (per) {
+        // the sample lives in the trees' scratch until the actor phase has read it
+        if (s->dp_phase != 0) return fail(UAVRL_ERR_STATE, "a prioritised-replay update while a split update waits for its next phase");
+        src = s->replay.per_source(s->cfg.seed, B, src, st, &rc);
+        if (rc) return rc;
+    }
     const dim3 tiles(grid, s->G);                        // y: trainer
     SacArgs a;
     s->adam_t += 1;
@@ -615,10 +650,15 @@ static int sac_critic_phase(uavrl_sac *s, const BatchSrc &src, int B, int Bg, co
     if (s->G > 1) sac_target_kernel<true><<<tiles, kNetThreads, smem_target(s->sh), st>>>(a);
     else sac_target_kernel<false><<<grid, kNetThreads, smem_target(s->sh), st>>>(a);
     UAVRL_LAUNCHED();
-    if (s->G > 1) sac_critic_kernel<true><<<tiles, kNetThreads, smem_critic(s->sh), st>>>(a);
-    else sac_critic_kernel<false><<<grid, kNetThreads, smem_critic(s->sh), st>>>(a);
+    if (src.is_w) {
+        if (s->G > 1) sac_critic_kernel<true, true><<<tiles, kNetThreads, smem_critic(s->sh), st>>>(a);
+        else sac_critic_kernel<false, true><<<grid, kNetThreads, smem_critic(s->sh), st>>>(a);
+    } else {
+        if (s->G > 1) sac_critic_kernel<true, false><<<tiles, kNetThreads, smem_critic(s->sh), st>>>(a);
+        else sac_critic_kernel<false, false><<<grid, kNetThreads, smem_critic(s->sh), st>>>(a);
+    }
     UAVRL_LAUNCHED();
-    return 0;
+    return per ? s->replay.per_write_back(B, st) : 0;
 }
 
 // the second half, after the critics' step: the actor's gradient partials, loss and entropy sums on the same rows
@@ -663,10 +703,11 @@ static int sac_finish(uavrl_sac *s, int grid, int Bg, bool exchanged, float *los
     return 0;
 }
 
-int uavrl::launch_sac_update(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev,
+int uavrl::launch_sac_update(uavrl_sac *s, const BatchSrc &src_in, int B, const float *eps_next, const float *eps_cur, float *losses_dev,
                              cudaStream_t st)
 {
     const int grid = sac_grid(s, B);
+    BatchSrc src = src_in;
     int rc;
     if ((rc = sac_critic_phase(s, src, B, B, eps_next, st)) || (rc = sac_reduce_adam(s, 1, grid, true, st)) ||
         (rc = sac_reduce_adam(s, 2, grid, true, st)) || (rc = sac_actor_phase(s, src, B, B, eps_cur, st)) ||
@@ -698,10 +739,11 @@ static int sac_exchange(uavrl_sac *s, bool critics, int grid, cudaStream_t st)
     return 0;
 }
 
-int uavrl::launch_sac_update_dp(uavrl_sac *s, const BatchSrc &src, int B, int global_batch, const float *eps_next, const float *eps_cur,
+int uavrl::launch_sac_update_dp(uavrl_sac *s, const BatchSrc &src_in, int B, int global_batch, const float *eps_next, const float *eps_cur,
                                 float *losses_dev, cudaStream_t st)
 {
     const int grid = sac_grid(s, B);
+    BatchSrc src = src_in;
     int rc;
     if ((rc = sac_critic_phase(s, src, B, global_batch, eps_next, st)) || (rc = sac_exchange(s, true, grid, st)) ||
         (rc = sac_actor_phase(s, src, B, global_batch, eps_cur, st)) || (rc = sac_exchange(s, false, grid, st)))
@@ -738,10 +780,11 @@ static int sac_alloc(uavrl_sac *s)
     for (size_t g = 0; g < G; ++g) init[3 * g] = logf(0.01f);          // SAC_Trainer.py:53
     UAVRL_CUDA(cudaMemcpy(s->scal, init.data(), init.size() * 4, cudaMemcpyHostToDevice));
     if (cfg->lockstep_envs > 0 && (rc = s->replay.alloc(cfg->replay_capacity, cfg->lockstep_envs, s->G, cfg->obs_dim, true))) return rc;
-    if ((rc = raise_dyn_smem(sac_target_kernel<false>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<false>, smem_critic(s->sh))) ||
+    if ((rc = raise_dyn_smem(sac_target_kernel<false>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<false, false>, smem_critic(s->sh))) ||
         (rc = raise_dyn_smem(sac_actor_kernel<false>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<false>, smem_act(s->sh))) ||
-        (rc = raise_dyn_smem(sac_target_kernel<true>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true>, smem_critic(s->sh))) ||
-        (rc = raise_dyn_smem(sac_actor_kernel<true>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<true>, smem_act(s->sh))))
+        (rc = raise_dyn_smem(sac_target_kernel<true>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true, false>, smem_critic(s->sh))) ||
+        (rc = raise_dyn_smem(sac_actor_kernel<true>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<true>, smem_act(s->sh))) ||
+        (rc = raise_dyn_smem(sac_critic_kernel<false, true>, smem_critic(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true, true>, smem_critic(s->sh))))
         return rc;
     return 0;
 }
@@ -757,7 +800,7 @@ int uavrl_sac_smem_bytes(const uavrl_sac_config *cfg, int64_t *bytes_out)
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(UAVRL_ERR_CUDA, "no CUDA device: the SAC learner has no CPU fallback");
     UAVRL_CUDA(cudaSetDevice(cfg->device));
-    size_t b[4];
+    size_t b[5];
     if ((rc = sac_smem_total(sh, b))) return rc;
     for (int i = 0; i < 4; ++i) bytes_out[i] = (int64_t)b[i];
     return 0;
@@ -774,9 +817,9 @@ int uavrl_sac_create_trainers(const uavrl_sac_config *cfg, int32_t n_trainers, u
     SacShape sh;
     int rc = sac_shape(*cfg, sh);
     if (rc || (rc = check_trainer_group(*cfg, n_trainers, "SAC learner"))) return rc;
-    size_t smem[4];
+    size_t smem[5];
     if ((rc = sac_smem_total(sh, smem))) return rc;
-    for (int i = 0; i < 4; ++i)
+    for (int i = 0; i < 5; ++i)
         if (smem[i] > kMaxBlockSmem)
             return fail(UAVRL_ERR_INVALID, "networks too large for the SMEM-resident SAC kernels: " + std::to_string(smem[i]) +
                                                " B of shared memory per block, at most " + std::to_string(kMaxBlockSmem));
@@ -896,6 +939,14 @@ int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *ep
     return launch_sac_act(s, obs_dev, n, eps_dev, actions_dev, (cudaStream_t)stream);
 }
 
+static BatchSrc sac_explicit_src(const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev, const float *d_dev)
+{
+    BatchSrc src;
+    memset(&src, 0, sizeof(src));
+    src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.act2 = a_dev; src.rew = r_dev; src.done_f32 = d_dev;
+    return src;
+}
+
 int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev,
                            const float *d_dev, const float *eps_next_dev, const float *eps_cur_dev, float *losses_dev, void *stream)
 {
@@ -903,9 +954,20 @@ int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const fl
     if (B % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_update_batch: B must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;                                             // SAC_Trainer.py:320
-    BatchSrc src;
-    memset(&src, 0, sizeof(src));
-    src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.act2 = a_dev; src.rew = r_dev; src.done_f32 = d_dev;
+    return launch_sac_update(s, sac_explicit_src(s_dev, a_dev, r_dev, s2_dev, d_dev), B / s->G, eps_next_dev, eps_cur_dev, losses_dev,
+                             (cudaStream_t)stream);
+}
+
+int uavrl_sac_update_batch_per(uavrl_sac *s, int32_t B, const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev,
+                               const float *d_dev, const float *is_weights_dev, float *abs_err_out_dev, const float *eps_next_dev,
+                               const float *eps_cur_dev, float *losses_dev, void *stream)
+{
+    if (!s || B <= 0 || !s_dev || !a_dev || !r_dev || !s2_dev || !d_dev || !is_weights_dev) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (B % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_update_batch_per: B must be a multiple of the trainer count");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    s->epoch += 1;                                             // SAC_Trainer.py:320
+    BatchSrc src = sac_explicit_src(s_dev, a_dev, r_dev, s2_dev, d_dev);
+    src.is_w = is_weights_dev; src.abs_err = abs_err_out_dev;
     return launch_sac_update(s, src, B / s->G, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
 }
 
@@ -930,6 +992,39 @@ int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const flo
     if (!s->replay.ready(s->cfg.batch_size)) return 0;         // nothing sampled yet
     return launch_sac_update(s, s->replay.source(s->cfg.seed, s->epoch, idx_tape_dev), s->cfg.batch_size, eps_next_dev, eps_cur_dev,
                              losses_dev, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------ prioritised replay: one SumTree per trainer over its slots
+// of the lockstep ring (ReplayStore::per, per.cu); the updates that sample the ring use them once enabled
+int uavrl_sac_per_enable(uavrl_sac *s, double alpha, double beta0, double beta_inc, double eps, double err_upper)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (!s->replay.frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    return s->replay.per_enable(alpha, beta0, beta_inc, eps, err_upper);
+}
+
+int uavrl_sac_per_set_priorities(uavrl_sac *s, int32_t n, const int32_t *slots_dev, const double *prio_dev, void *stream)
+{
+    return per_entry_set(s ? &s->replay : nullptr, s ? s->cfg.device : 0, n, slots_dev, prio_dev, nullptr, 0, (cudaStream_t)stream);
+}
+
+int uavrl_sac_per_set_errors(uavrl_sac *s, int32_t n, const int32_t *slots_dev, const float *abs_err_dev, int32_t clip, void *stream)
+{
+    return per_entry_set(s ? &s->replay : nullptr, s ? s->cfg.device : 0, n, slots_dev, nullptr, abs_err_dev, clip, (cudaStream_t)stream);
+}
+
+int uavrl_sac_per_sample(uavrl_sac *s, int32_t B, const double *u_tape_dev, int32_t *slots_out_dev, float *weights_out_dev, void *stream)
+{
+    // a larger B regrows the trees' scratch, which a waiting split update still reads its rows through
+    if (s && s->dp_phase != 0) return fail(UAVRL_ERR_STATE, "uavrl_sac_per_sample while a split update waits for its next phase");
+    return per_entry_sample(s ? &s->replay : nullptr, s ? s->cfg.device : 0, s ? s->cfg.seed : 0, B, u_tape_dev, slots_out_dev,
+                            weights_out_dev, (cudaStream_t)stream);
+}
+
+int uavrl_sac_per_get(uavrl_sac *s, double *leaves_host, double *total_out, double *beta_out)
+{
+    return per_entry_get(s ? &s->replay : nullptr, s ? s->cfg.device : 0, leaves_host, total_out, beta_out);
 }
 
 int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
@@ -988,10 +1083,10 @@ int uavrl_sac_update_replay_dp(uavrl_sac *s, const int32_t *idx_tape_dev, const 
 // the split form's critic phase on src: the critics' gradients and squared-error sums into the critic exchange vector
 static int sac_split_critic(uavrl_sac *s, const BatchSrc &src, int B, int global_batch, const float *eps_next, cudaStream_t st)
 {
-    s->dp_src = src; s->dp_B = B; s->dp_global = global_batch;
+    s->dp_src = src; s->dp_B = B; s->dp_global = global_batch;           // the critic phase points dp_src at a prioritised sample
     const int grid = sac_grid(s, B);
     int rc;
-    if ((rc = sac_critic_phase(s, src, B, global_batch, eps_next, st)) || (rc = sac_reduce_adam(s, 1, grid, false, st)) ||
+    if ((rc = sac_critic_phase(s, s->dp_src, B, global_batch, eps_next, st)) || (rc = sac_reduce_adam(s, 1, grid, false, st)) ||
         (rc = sac_reduce_adam(s, 2, grid, false, st)))
         return rc;
     sac_stat_sums_kernel<<<1, 32, 0, st>>>(s->stat, grid, 0, s->xc + 2 * (size_t)s->sh.critic.P);
@@ -1017,10 +1112,7 @@ int uavrl_sac_critic_grads_batch(uavrl_sac *s, int32_t B, const float *s_dev, co
     if (int rc = sac_dp_checks(s, global_batch, false, "uavrl_sac_critic_grads_batch")) return rc;
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;
-    BatchSrc src;
-    memset(&src, 0, sizeof(src));
-    src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.act2 = a_dev; src.rew = r_dev; src.done_f32 = d_dev;
-    return sac_split_critic(s, src, B, global_batch, eps_next_dev, (cudaStream_t)stream);
+    return sac_split_critic(s, sac_explicit_src(s_dev, a_dev, r_dev, s2_dev, d_dev), B, global_batch, eps_next_dev, (cudaStream_t)stream);
 }
 
 static int sac_phase_is(const uavrl_sac *s, int phase, const char *fn)

@@ -249,7 +249,47 @@ def init_draw(layout, gen):
     return torch.cat(parts).numpy()
 
 
-class Learner:
+class _PerCalls:
+    """The prioritised-replay calls a learner handle shares with the other kind (SumTree + ReplayTree of the reference,
+    BaseClass/replay_buffer.py:57-223): the C entry points named _PER + sample / set_errors / set_priorities / get, which take
+    (n,) arrays on a one-trainer learner and (G, n) arrays of trainer-local slots on a learner with G > 1 trainers."""
+    _PER = "uavrl_per_"
+
+    def _per(self, name):
+        return getattr(_lib.lib(), self._PER + name)
+
+    def _per_shape(self, n):
+        return (n,) if self.G == 1 else (self.G, n)
+
+    def per_sample(self, batch, u_tape=None):
+        """ReplayTree.sample2: (slots int32 [B], importance weights float32 [B]) on the device; (G, B) each on a grouped
+        learner, u_tape (G, B)."""
+        slots = torch.empty(self._per_shape(batch), dtype=torch.int32, device=self.device)
+        w = torch.empty(self._per_shape(batch), dtype=torch.float32, device=self.device)
+        check(self._per("sample")(self.h, int(batch), _ptr(u_tape), _ptr(slots), _ptr(w), _stream(self.device)))
+        return slots, w
+
+    def _per_n(self, slots):
+        """Slots per trainer of a (n,) or, grouped, (G, n) slot array."""
+        if self.G > 1 and (slots.dim() != 2 or slots.shape[0] != self.G):
+            raise ValueError("a learner with %d trainers takes (%d, n) slots, got %s" % (self.G, self.G, tuple(slots.shape)))
+        return int(slots.shape[-1])
+
+    def per_set_errors(self, slots, abs_err, clip=True):
+        check(self._per("set_errors")(self.h, self._per_n(slots), _ptr(slots), _ptr(abs_err), int(bool(clip)), _stream(self.device)))
+
+    def per_set_priorities(self, slots, priorities):
+        check(self._per("set_priorities")(self.h, self._per_n(slots), _ptr(slots), _ptr(priorities), _stream(self.device)))
+
+    def per_state(self, n_slots):
+        """(leaves, total, beta); grouped: n_slots per trainer, leaves (G, n_slots) and totals (G,)."""
+        leaves = np.zeros(self._per_shape(int(n_slots)), np.float64)
+        totals, beta = np.zeros(self.G, np.float64), C.c_double()
+        check(self._per("get")(self.h, _ptr(leaves), totals.ctypes.data_as(C.POINTER(C.c_double)), C.byref(beta)))
+        return leaves, (float(totals[0]) if self.G == 1 else totals), beta.value
+
+
+class Learner(_PerCalls):
     """Q-network + Adam + replay on one GPU (DQN / DDQN / DuelingDQN trainers of the reference).
 
     trainers = G > 1: G independent trainers of this network in one handle (one Trainer per UAV group, PathPlan_City.py:59-69).
@@ -412,37 +452,6 @@ class Learner:
         With G > 1 the per_* methods then take and return (G, ...) arrays of trainer-local slots."""
         check(_lib.lib().uavrl_per_enable_trainers(self.h, alpha, beta0, beta_inc, eps, err_upper))
 
-    def _per_shape(self, n):
-        return (n,) if self.G == 1 else (self.G, n)
-
-    def per_sample(self, batch, u_tape=None):
-        """ReplayTree.sample2: (slots int32 [B], importance weights float32 [B]) on the device; (G, B) each on a grouped
-        learner, u_tape (G, B)."""
-        slots = torch.empty(self._per_shape(batch), dtype=torch.int32, device=self.device)
-        w = torch.empty(self._per_shape(batch), dtype=torch.float32, device=self.device)
-        check(_lib.lib().uavrl_per_sample(self.h, int(batch), _ptr(u_tape), _ptr(slots), _ptr(w), _stream(self.device)))
-        return slots, w
-
-    def _per_n(self, slots):
-        """Slots per trainer of a (n,) or, grouped, (G, n) slot array."""
-        if self.G > 1 and (slots.dim() != 2 or slots.shape[0] != self.G):
-            raise ValueError("a learner with %d trainers takes (%d, n) slots, got %s" % (self.G, self.G, tuple(slots.shape)))
-        return int(slots.shape[-1])
-
-    def per_set_errors(self, slots, abs_err, clip=True):
-        check(_lib.lib().uavrl_per_set_errors(self.h, self._per_n(slots), _ptr(slots), _ptr(abs_err), int(bool(clip)),
-                                              _stream(self.device)))
-
-    def per_set_priorities(self, slots, priorities):
-        check(_lib.lib().uavrl_per_set_priorities(self.h, self._per_n(slots), _ptr(slots), _ptr(priorities), _stream(self.device)))
-
-    def per_state(self, n_slots):
-        """(leaves, total, beta); grouped: n_slots per trainer, leaves (G, n_slots) and totals (G,)."""
-        leaves = np.zeros(self._per_shape(int(n_slots)), np.float64)
-        totals, beta = np.zeros(self.G, np.float64), C.c_double()
-        check(_lib.lib().uavrl_per_get(self.h, _ptr(leaves), totals.ctypes.data_as(C.POINTER(C.c_double)), C.byref(beta)))
-        return leaves, (float(totals[0]) if self.G == 1 else totals), beta.value
-
     def compute_grads(self, global_batch, idx_tape=None, loss=None):
         check(_lib.lib().uavrl_learner_compute_grads(self.h, _ptr(idx_tape), int(global_batch), _ptr(loss),
                                                      _stream(self.device)))
@@ -554,7 +563,7 @@ def train_run_dp(env, learner, n_iters, eps, global_batch):
     check(_lib.lib().uavrl_train_run_dp(env.h, learner.h, int(n_iters), float(eps), int(global_batch), _stream(env.device)))
 
 
-class SacLearner:
+class SacLearner(_PerCalls):
     """SAC continuous (the reference's shipped trainer, config/Trainer.xml) on one GPU.  obs_dim must be a multiple of 4 in
     [4, 124], hidden in [1, 128], and the networks must fit the kernels' shared memory (sac_smem_bytes).  Parameter roles:
     0-4 actor, critic_1, critic_2 and their targets, 5-7 / 8-10 Adam moments, 11-13 the last reduced gradients (read-only).
@@ -692,9 +701,29 @@ class SacLearner:
 
     def update_replay(self, idx_tape=None, eps_next=None, eps_cur=None, losses=None):
         """One update sampled from the lockstep ring (idx_tape: device int32 [batch_size] logical indices, or [G][batch_size]
-        trainer-local ones; None = Philox)."""
+        trainer-local ones; None = Philox, or the trees once per_enable has run)."""
         check(_lib.lib().uavrl_sac_update_replay(self.h, _ptr(idx_tape), _ptr(eps_next), _ptr(eps_cur), self._losses(losses),
                                                  _stream(self.device)))
+
+    # -- prioritised replay (include/uavrl.h, uavrl_sac_per_enable): one SumTree per trainer over its slots of the ring
+    _PER = "uavrl_sac_per_"
+
+    def per_enable(self, alpha=-1.0, beta0=-1.0, beta_inc=-1.0, eps=-1.0, err_upper=-1.0):
+        """Every update that samples the ring then draws from the trees, weights the critic losses and writes
+        e_b = mean_j |min(Q1, Q2)_j - y_j| back; the per_* methods take (G, ...) arrays when G > 1."""
+        check(_lib.lib().uavrl_sac_per_enable(self.h, alpha, beta0, beta_inc, eps, err_upper))
+
+    def tree_slots(self):
+        """Leaves of each trainer's tree: its slots of the ring, ring_frames x lockstep_envs / G (ReplayStore::alloc)."""
+        Ng = self.cfg.lockstep_envs // self.G
+        return (max(2, -(-(self.cfg.replay_capacity // self.G) // Ng)) + 1) * Ng
+
+    def update_batch_per(self, s, a, r, s2, d, is_weights, abs_err_out=None, eps_next=None, eps_cur=None, losses=None):
+        """update_batch with importance weights is_weights [B] in the critic losses and each row's e_b written to abs_err_out
+        [B] (may be None); the trees are not touched."""
+        check(_lib.lib().uavrl_sac_update_batch_per(self.h, s.shape[0], _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d), _ptr(is_weights),
+                                                    _ptr(abs_err_out), _ptr(eps_next), _ptr(eps_cur), self._losses(losses),
+                                                    _stream(self.device)))
 
     # -- data-parallel training (include/uavrl.h, uavrl_sac_comm_init .. uavrl_sac_train_run_dp): one learner per GPU
     def _comm(self):

@@ -26,11 +26,11 @@ class SAC_Trainer_B200:
         self.save_loop = int(None2Value(param.get('save_loop'), 10))
         self.Is_Train = int(None2Value(param.get('Is_Train'), 1))
         self.IsPriority_Replay = int(None2Value(param.get('IsPriority_Replay'), 0))
-        if self.IsPriority_Replay:
-            raise ValueError("prioritised replay is not implemented (SURVEY.md section 8f-3)")
         self.IS_Continuous = 1
         self.w, self.hidden, self.act_dim = int(actor.get('w')), int(actor.get('hiden_dim')), int(actor.get('output'))
         self.lockstep_envs = int(None2Value(param.get('lockstep_envs'), 0))
+        if self.IsPriority_Replay and self.lockstep_envs == 0:
+            raise ValueError("prioritised replay with SAC needs the lockstep ring (lockstep_envs > 0): its SumTrees index the ring's slots")
         self.device_index = int(None2Value(param.get('device'), 0))
         # n_trainers = G > 1: one independent SAC trainer per block of lockstep_envs / G UAVs (the reference's SAC_Trainer per UAV,
         # PathPlan_City.py:59-69), each with its own replay_size transitions; trainer g is named UAV_<g * lockstep_envs / G>
@@ -43,6 +43,10 @@ class SAC_Trainer_B200:
             batch_size=self.Batch_Size, replay_capacity=self.replay_size * G, lockstep_envs=self.lockstep_envs,
             seed=int(None2Value(param.get('seed'), 42)), device=self.device_index, trainers=G)
         self._learner.init_params(int(None2Value(param.get('seed'), 42)))
+        if self.IsPriority_Replay:
+            # ReplayTree constants (replay_buffer.py:141-148), one tree per trainer as each reference Trainer owns its ReplayTree;
+            # the lockstep loop (engine.sac_train_run) then trains on prioritised samples
+            self._learner.per_enable()
         self._dev = self._learner.device
         self._losses = torch.zeros(4 * G, device=self._dev)
         self.loss = 0
@@ -89,7 +93,19 @@ class SAC_Trainer_B200:
         s = f(states, (-1, self.w)); s2 = f(transition_dict['next_states'], (-1, self.w))
         a = f(transition_dict['actions'], (-1, self.act_dim))
         r = f(transition_dict['rewards'], (-1,)); d = f(transition_dict['dones'], (-1,))
-        if self._world > 1:
+        wts, idx = transition_dict.get('weights'), transition_dict.get('idx')
+        if wts is not None:
+            if self._world > 1:
+                raise ValueError("a weighted (prioritised-replay) update has no split data-parallel form: train with world = 1")
+            # importance weights in the critic losses, then ReplayTree.batch_update(tree_idx, e_b) (SAC_Trainer.py:336-352)
+            w = f(wts, (-1,))
+            ae = torch.zeros(s.shape[0], dtype=torch.float32, device=dev)
+            self._learner.update_batch_per(s, a, r, s2, d, w, ae, None, None, self._losses)
+            if idx is not None:
+                slots = np.asarray(idx, np.int64).reshape(-1) - (self._learner.tree_slots() - 1)
+                shape = (-1,) if self.n_trainers == 1 else (self.n_trainers, -1)
+                self._learner.per_set_errors(torch.as_tensor(slots.astype(np.int32).reshape(shape)).to(dev), ae.reshape(shape), clip=True)
+        elif self._world > 1:
             L, dist = self._learner, self._dist
             L.critic_grads(s.shape[0] * self._world, batch=(s, a, r, s2, d))
             dist.all_reduce(self._xvec[0], op=dist.ReduceOp.SUM)

@@ -425,6 +425,41 @@ int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const flo
  * learner on different devices (UAVRL_ERR_INVALID, as uavrl_train_run); no uavrl_env_reset (UAVRL_ERR_STATE). */
 int uavrl_sac_train_run(uavrl_env *env, uavrl_sac *s, int32_t n_iters, int32_t do_update, uavrl_train_stats *stats_host, void *stream);
 
+/* Prioritised replay for SAC (IsPriority_Replay = 1; SAC_Trainer.update :336-352, BaseClass/replay_buffer.py:57-223): one
+ * SumTree per trainer over its own slots of the lockstep ring, the trees and rules of the uavrl_per_* block.  As written, the
+ * reference's branch cannot run: is_weights * critic_loss is a [B,1] tensor that .backward() refuses (not a scalar), the critics'
+ * action_dim = 2 outputs hand batch_update [B,2] errors that one SumTree leaf cannot hold, and its float tree_idx cannot index.
+ * So this port states the semantics, taking the only readings that run and agree with the Q-network learner:
+ *   - critic losses  L_k = mean over B x 2 of w_b (Q_k[b][j] - y[b][j])^2, k = 1, 2, with w_b the sample's importance weight
+ *     (ReplayTree.sample2, normalised by the batch maximum of its trainer); the reported critic losses are these;
+ *   - priority error e_b = 0.5f * (|m_0 - y_0| + |m_1 - y_1|), m_j = fminf(Q1[b][j], Q2[b][j]), float32 in that order -- the mean
+ *     over the action columns, the reference's |min(Q1, Q2) - y| for action_dim = 1 -- from the critics BEFORE this update's
+ *     step; it goes back through batch_update (clip): p = min(e + eps, err_upper)^alpha;
+ *   - the actor loss, the alpha loss, the TD target and the soft update take no weights (:361-379);
+ *   - a newly committed ring frame gets the error-less push priority (0 + eps)^alpha, the frame it drops 0.
+ * Once enabled, every update that samples the ring without an injected idx_tape_dev (uavrl_sac_update_replay, uavrl_sac_train_run,
+ * uavrl_sac_update_replay_dp, uavrl_sac_train_run_dp, uavrl_sac_critic_grads_replay) draws batch_size rows per trainer from the
+ * trees (keyed as uavrl_per_sample), runs the critic leg weighted, writes every e_b back once the critic kernel has run, and
+ * takes the actor leg on the same rows.  Trainer g of a grouped learner computes what a stand-alone learner with seed + g,
+ * replay_capacity / G and lockstep_envs / G computes, its tree and beta included; data-parallel ranks keep trees of their own.
+ *
+ * uavrl_sac_per_enable: one call for every trainer count (the ring's slot numbering is the same for any G); negative
+ * hyper-parameters take the reference's defaults.  Refused: no ring (lockstep_envs == 0; UAVRL_ERR_STATE), already enabled
+ * or a transition already stored (UAVRL_ERR_STATE), more than 4 194 304 slots per tree (UAVRL_ERR_INVALID).
+ * uavrl_sac_per_sample / _set_errors / _set_priorities / _get: the arguments, [G][...] shapes, trainer-local slots and refusals
+ * of uavrl_per_sample / _set_errors / _set_priorities / _get (UAVRL_ERR_INVALID "prioritised replay not enabled" before
+ * uavrl_sac_per_enable); uavrl_sac_per_sample is also refused (UAVRL_ERR_STATE) while a split update waits for its next phase.
+ * uavrl_sac_update_batch_per: uavrl_sac_update_batch with importance weights is_weights_dev [B] (required; block g of G B / G
+ * for trainer g) in the critic losses and e_b written to abs_err_out_dev [B] (may be NULL); it does not touch the trees. */
+int uavrl_sac_per_enable(uavrl_sac *s, double alpha, double beta0, double beta_inc, double eps, double err_upper);
+int uavrl_sac_per_sample(uavrl_sac *s, int32_t B, const double *u_tape_dev, int32_t *slots_out_dev, float *weights_out_dev, void *stream);
+int uavrl_sac_per_set_errors(uavrl_sac *s, int32_t n, const int32_t *slots_dev, const float *abs_err_dev, int32_t clip, void *stream);
+int uavrl_sac_per_set_priorities(uavrl_sac *s, int32_t n, const int32_t *slots_dev, const double *prio_dev, void *stream);
+int uavrl_sac_per_get(uavrl_sac *s, double *leaves_host, double *total_out, double *beta_out);
+int uavrl_sac_update_batch_per(uavrl_sac *s, int32_t B, const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev,
+                               const float *d_dev, const float *is_weights_dev, float *abs_err_out_dev, const float *eps_next_dev,
+                               const float *eps_cur_dev, float *losses_dev, void *stream);
+
 /* Data-parallel SAC (one learner per GPU, each rank sampling batch_size rows from its own ring shard; global_batch =
  * batch_size x world).  The actor loss is taken on the UPDATED critics, so an update makes two exchanges: both critics'
  * gradients with the two critic squared-error sums, then -- after the critics' Adam step on every rank -- the actor's

@@ -1,5 +1,7 @@
 """BASELINE configs[4]: SAC continuous (the trainer the reference ships) on 16 384 envs — env steps/s and updates/s.
-Secondary measurement (bench.py stays on configs[1]).  python tools/bench_sac.py [--envs N] [--batch B] [--steps K]"""
+Secondary measurement (bench.py stays on configs[1]).  python tools/bench_sac.py [--envs N] [--batch B] [--steps K] [--per 0|1]
+[--profile].  --per 1: prioritised replay (SumTrees over the ring, weighted critic losses, the e_b write-back); --profile: per-kernel
+device time over the timed steps from torch.profiler instead of the end-to-end rate."""
 import argparse
 import json
 import os
@@ -17,6 +19,8 @@ def main():
     ap.add_argument("--batch", type=int, default=0)
     ap.add_argument("--steps", type=int, default=500)
     ap.add_argument("--replay", type=int, default=1 << 20)
+    ap.add_argument("--per", type=int, choices=(0, 1), default=0)
+    ap.add_argument("--profile", action="store_true")
     a = ap.parse_args()
     B = a.batch or a.envs
     import uavrl_b200  # noqa: F401
@@ -32,10 +36,25 @@ def main():
     L = engine.SacLearner(100, 64, 2, 1.0, 1e-4, 1e-3, 1e-4, 1.0, 0.99, 0.05, batch_size=B, replay_capacity=a.replay,
                           lockstep_envs=a.envs, seed=7, device=0)
     L.init_params(0)
+    if a.per:
+        L.per_enable()
     frames = (a.replay + a.envs - 1) // a.envs + 1
     engine.sac_train_run(env, L, frames, False, want_stats=False)          # prefill the ring (> L2)
     engine.sac_train_run(env, L, 10, True, want_stats=False)
     torch.cuda.synchronize()
+    if a.profile:
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            engine.sac_train_run(env, L, a.steps, True, want_stats=False)
+            torch.cuda.synchronize()
+        us = {}
+        for ev in prof.events():
+            if ev.device_type.name == "CUDA":
+                us[ev.name] = us.get(ev.name, 0.0) + ev.device_time
+        print(json.dumps({"per": a.per, "steps": a.steps, "gpu": torch.cuda.get_device_name(0),
+                          "kernel_us_per_step": {k.split("(")[0][-80:]: v / a.steps for k, v in sorted(us.items(), key=lambda kv: -kv[1])}}),
+              flush=True)
+        return
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     n0 = _lib.launch_count()
     e0.record()
@@ -46,7 +65,8 @@ def main():
     sc_ = L.scalars()
     print(json.dumps({"metric": "env steps/sec (+ SAC updates/sec), 500x500x100 city", "value": a.envs * a.steps / (ms * 1e-3),
                       "unit": "env_steps/s", "updates_per_s": a.steps / (ms * 1e-3), "ms_per_step": ms / a.steps, "n_gpus": 1,
-                      "steps": a.steps, "gpu_launches": int(_lib.launch_count() - n0),
+                      "steps": a.steps, "gpu_launches": int(_lib.launch_count() - n0), "per": a.per,
+                      "gpu": torch.cuda.get_device_name(0),
                       "config": {"workload": "%d envs, continuous update_PathPlan, SAC actor 100-64-(2,2) + 2 critics 102-64-64-2, "
                                              "batch %d, replay %d (> L2), 1 update / lockstep iteration" % (a.envs, B, a.replay)},
                       "episodes_ended": int(st.episodes_ended), "last_loss": float(st.last_loss), "log_alpha": sc_["log_alpha"]},
