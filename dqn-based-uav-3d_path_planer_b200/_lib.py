@@ -76,6 +76,7 @@ SIGNATURES = {
     "uavrl_env_destroy": (C.c_int, [VP]),
     "uavrl_env_set_pool": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP, VP, VP]),
     "uavrl_env_reset": (C.c_int, [VP, C.c_int32, VP]),
+    "uavrl_env_set_reset_stride": (C.c_int, [VP, C.c_int32]),
     "uavrl_make_scenarios": (C.c_int, [C.POINTER(EnvConfig), C.c_uint64, C.c_int32, C.c_int32, VP, VP, VP, VP, VP]),
     "uavrl_set_pdl": (C.c_int, [C.c_int32]),
     "uavrl_test_fail_alloc": (C.c_int, [C.c_int32]),
@@ -108,6 +109,11 @@ SIGNATURES = {
     "uavrl_learner_create_trainers": (C.c_int, [C.POINTER(LearnerConfig), C.c_int32, C.POINTER(VP)]),
     "uavrl_learner_trainer_count": (C.c_int32, [VP]),
     "uavrl_learner_federate": (C.c_int, [VP, VP, VP, VP, VP, VP, VP]),
+    "uavrl_learner_fed_shard": (C.c_int, [VP, C.c_int32, C.c_int32]),
+    "uavrl_learner_fed_exchange_ptr": (VP, [VP, C.c_int32, C.POINTER(C.c_int64)]),
+    "uavrl_learner_fed_local": (C.c_int, [VP, VP, VP, VP, VP]),
+    "uavrl_learner_fed_columns": (C.c_int, [VP, VP]),
+    "uavrl_learner_fed_rounds": (C.c_int, [VP, VP, VP, VP]),
     "uavrl_learner_destroy": (C.c_int, [VP]),
     "uavrl_learner_param_count": (C.c_int64, [VP]),
     "uavrl_learner_set_params": (C.c_int, [VP, C.c_int32, VP]),
@@ -137,6 +143,10 @@ SIGNATURES = {
     "uavrl_sac_set_alpha": (C.c_int, [VP, VP]),
     "uavrl_sac_get_alpha": (C.c_int, [VP, VP]),
     "uavrl_sac_federate_actors": (C.c_int, [VP, VP]),
+    "uavrl_sac_fed_shard": (C.c_int, [VP, C.c_int32, C.c_int32]),
+    "uavrl_sac_fed_exchange_ptr": (VP, [VP, C.POINTER(C.c_int64)]),
+    "uavrl_sac_fed_local": (C.c_int, [VP, VP]),
+    "uavrl_sac_federate_actors_sharded": (C.c_int, [VP, VP]),
     "uavrl_sac_destroy": (C.c_int, [VP]),
     "uavrl_sac_param_count": (C.c_int64, [VP, C.c_int32]),
     "uavrl_sac_set_params": (C.c_int, [VP, C.c_int32, VP]),

@@ -189,7 +189,7 @@ static int env_init(uavrl_env *env, const uavrl_env_config *cfg)
     d.k.width = cfg->width; d.k.h = cfg->h;
     d.k.max_v = cfg->max_v; d.k.min_v = cfg->min_v; d.k.steering = cfg->steering_angle;
     d.k.climb = cfg->climb_rate; d.k.max_step = cfg->max_step; d.k.n_cyl = cfg->n_buildings;
-    d.n = cfg->n_envs; d.K = cfg->max_subgoals; d.P = 0; d.auto_reset = cfg->auto_reset;
+    d.n = cfg->n_envs; d.K = cfg->max_subgoals; d.P = 0; d.auto_reset = cfg->auto_reset; d.reset_stride = cfg->n_envs;
     d.cull_w = 20.0 + cfg->max_v + 0.5;
 
     std::vector<Cyl> cyl((size_t)(cfg->n_buildings > 0 ? cfg->n_buildings : 1));
@@ -310,6 +310,14 @@ int uavrl_env_reset(uavrl_env *env, int32_t first, void *stream)
     env_reset_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(env->d, first);
     UAVRL_LAUNCHED();
     env->reset_done = true;
+    return 0;
+}
+
+int uavrl_env_set_reset_stride(uavrl_env *env, int32_t stride)
+{
+    if (!env) return fail(UAVRL_ERR_INVALID, "null env");
+    if (stride < 1) return fail(UAVRL_ERR_INVALID, "uavrl_env_set_reset_stride: stride must be >= 1");
+    env->d.reset_stride = stride;
     return 0;
 }
 

@@ -19,7 +19,8 @@ struct EnvDev {
     EnvConst k;
     int32_t n, K, P;
     int32_t auto_reset;
-    double cull_w;                      // half-width of the probe window incl. one step of motion
+    int32_t reset_stride;               // scenario advance of an env's auto-reset: n, or the full batch's n for a shard of it
+    double cull_w;                     // half-width of the probe window incl. one step of motion
     const Cyl *cyl;
     // per-env state, structure of arrays
     double *px, *py, *pz, *vx, *vy, *V, *score, *total, *path_len, *gx, *gy, *gz, *rew64, *theta;

@@ -229,7 +229,7 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
                 n_succ = (o.info == 1); n_lose = (o.info == 2);
                 ended_flag = (uint8_t)s.done;
                 if (d.auto_reset && s.done) {                      // UAV.reset() at the episode boundary
-                    scen = (int)(((long long)scen + d.n) % d.P);
+                    scen = (int)(((long long)scen + d.reset_stride) % d.P);
                     if (EXTRAS && (d.extras & kExtraEnergy)) d.energy[e] = 0.0;
                     load_scenario(d, scen, s);
                     mask = cull_mask(d, s_cyl, s.px, s.py);

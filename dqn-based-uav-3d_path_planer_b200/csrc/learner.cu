@@ -38,10 +38,10 @@ static int build_net(const uavrl_learner_config &c, NetDev &n)
 
 // ------------------------------------------------------------------ eps-greedy action kernel
 // LOSS (federation, launch_fed_loss): grid row y evaluates weight set w = fl.w0 + y on probe rows [0, S w) (fl.tri) or
-// [S (w + 1), n) of obs = [G][S][in_dim], S = kFedProbes; a tile takes 3 whole probe groups (30 rows) and writes
-// fl.loss_out[p][w] = sum over trainer p's rows of sum_a (fl.q_ref - Q_w)^2 / (S A).  The same reduction as the tensor-core
-// loss variant (tc_forward.cu).
-struct FedLossArgs { const float *q_ref; float *loss_out; int w0, tri; };
+// [S (w + 1), n) of obs = [G][S][in_dim], S = kFedProbes, with image w - fl.img0; a tile takes 3 whole probe groups (30 rows)
+// and writes fl.loss_out[p * fl.ld + w - fl.col0] = sum over trainer p's rows of sum_a (fl.q_ref - Q_w)^2 / (S A).  The same
+// reduction as the tensor-core loss variant (tc_forward.cu).
+struct FedLossArgs { const float *q_ref; float *loss_out; int w0, tri, img0, ld, col0; };
 
 template <bool LOSS>
 __global__ void __launch_bounds__(kNetThreads)
@@ -60,7 +60,7 @@ act_kernel_t(NetDev net, const float *__restrict__ params, const float *__restri
         row0 = (size_t)lo; n_rows = hi - lo;
         n_tiles = (n_rows + kStep - 1) / kStep;
         if ((int)blockIdx.x >= n_tiles) return;
-        params += (size_t)w_set * img_floats; obs += row0 * net.in_dim;
+        params += (size_t)(w_set - fl.img0) * img_floats; obs += row0 * net.in_dim;
     } else {   // trainer blockIdx.y of a grouped learner: its weight image, its n rows and its eps-greedy key
         const int g = blockIdx.y;
         const size_t r0 = (size_t)g * (size_t)n;
@@ -102,7 +102,7 @@ act_kernel_t(NetDev net, const float *__restrict__ params, const float *__restri
             }
             __syncthreads();
             if (threadIdx.x * kFedProbes < kStep && e0 + (int)threadIdx.x * kFedProbes < n_rows)
-                fed_group_loss(sA + threadIdx.x * kFedProbes, row0 + e0 + threadIdx.x * kFedProbes, n, w_set, net.n_actions, fl.loss_out);
+                fed_group_loss(sA + threadIdx.x * kFedProbes, row0 + e0 + threadIdx.x * kFedProbes, fl.ld, w_set - fl.col0, net.n_actions, fl.loss_out);
         } else if (threadIdx.x < kTile && e0 + threadIdx.x < n) {
             const int e = e0 + threadIdx.x;
             const float *row = head + threadIdx.x * 32;
@@ -328,26 +328,28 @@ int launch_act(uavrl_learner *l, const float *obs, int n_all, float eps, int is_
     return 0;
 }
 
-int launch_fed_loss(uavrl_learner *l, const float *probes, const float *q_ref, float *loss_out, int w0, int n_weights, bool tri,
-                    cudaStream_t st)
+int launch_fed_loss(uavrl_learner *l, const FedLoss &f, int w0, int n_weights, bool tri, cudaStream_t st)
 {
-    const int n = l->G * kFedProbes;                     // every probe row; a weight set evaluates at most n - S of them
+    const int n = f.G * kFedProbes;                      // every probe row; a weight set evaluates at most n - S of them
     const int max_rows = n - kFedProbes;
     if (max_rows <= 0 || n_weights <= 0) return 0;
     const Route r = learner_route(l, max_rows);
     if (r.fwd) {
         TcArgs a;
         memset(&a, 0, sizeof(a));
-        a.img = l->tc_img_local; a.obs = probes; a.n = n; a.mode = kTcAct;
-        a.q_ref = q_ref; a.loss_out = loss_out; a.loss_w0 = w0; a.loss_tri = tri ? 1 : 0;
+        a.img = f.tc_img; a.obs = f.probes; a.n = n; a.mode = kTcAct;
+        a.q_ref = f.q_ref; a.loss_out = f.loss_out; a.loss_w0 = w0; a.loss_tri = tri ? 1 : 0;
+        a.loss_img0 = f.img0; a.loss_ld = f.ld; a.loss_col0 = f.col0;
         return launch_tc_loss(l, r, a, n_weights, max_rows, st);
     }
     constexpr int step = (kTile / kFedProbes) * kFedProbes;
     const int n_tiles = (max_rows + step - 1) / step;
     const int grid = n_tiles < 4 * num_sms() ? n_tiles : 4 * num_sms();
-    act_kernel_t<true><<<dim3(grid, n_weights), kNetThreads, act_smem_bytes(l->net), st>>>(l->net, l->img_local, probes, n, 0.f, 0, nullptr,
+    act_kernel_t<true><<<dim3(grid, n_weights), kNetThreads, act_smem_bytes(l->net), st>>>(l->net, f.img, f.probes, n, 0.f, 0, nullptr,
                                                                                           nullptr, 0, 0, nullptr, nullptr, nullptr, n_tiles,
-                                                                                          l->net.smem_w_floats, FedLossArgs{ q_ref, loss_out, w0, tri ? 1 : 0 });
+                                                                                          l->net.smem_w_floats,
+                                                                                          FedLossArgs{ f.q_ref, f.loss_out, w0, tri ? 1 : 0,
+                                                                                                       f.img0, f.ld, f.col0 });
     l->chain.launched(kChainNone);
     UAVRL_LAUNCHED();
     return 0;

@@ -74,16 +74,45 @@ __device__ __forceinline__ bool eps_greedy(float eps, int is_train, const float 
     return u > eps || !is_train;
 }
 
-// Federation: the loss entry of one probe group, M[p][w_set] = (sum of its kFedProbes rows' squared Q differences d2, in row
-// order) / (S A); first_row = the group's first row in the [G][S] probe rows.
-__device__ __forceinline__ void fed_group_loss(const float *d2, size_t first_row, int n, int w_set, int n_actions, float *loss_out)
+// Federation: the loss entry of one probe group, loss_out[p * ld + col] = (sum of its kFedProbes rows' squared Q differences
+// d2, in row order) / (S A); first_row = the group's first row in the [G][S] probe rows, p = its trainer.
+__device__ __forceinline__ void fed_group_loss(const float *d2, size_t first_row, int ld, int col, int n_actions, float *loss_out)
 {
     float s2 = 0.f;
     for (int r = 0; r < kFedProbes; ++r) s2 += d2[r];
     const size_t p = first_row / kFedProbes;
-    loss_out[p * (size_t)(n / kFedProbes) + w_set] = s2 / (float)(kFedProbes * n_actions);
+    loss_out[p * (size_t)ld + col] = s2 / (float)(kFedProbes * n_actions);
 }
 #endif
+
+// The sharded federation (federate.cu, uavrl_learner_fed_shard): this learner's G_local trainers are the global trainers
+// [rank G_local, (rank + 1) G_local) of G = G_local world.  Two buffers are exchanged by all-gathers in rank order:
+//   x0 [G][S in + S A + P]: every trainer's [probes | q_ref | q_local] (phase 0);
+//   x1 [world][G][G_local]: every rank's columns of the initial loss matrix (phase 1).
+// The rest is scratch of the rounds: the gathered rows unpacked into probes [G][S][in], q_ref [G][S][A] and the flat replica
+// rep [G][P] of every q_local, the loss matrix M [G][G], the chosen lists [G][max(1, k)], the weight images (fp32 and tensor
+// core) of the trainer a round has just averaged, and the local phase's probe rows, Q rows and actions.
+struct FedShard {
+    int32_t rank = 0, world = 0;              // world 0: no shard declared
+    int32_t phase = 0;                        // 0: ready for the local phase, 1: x0 slice written, 2: x1 slice written
+    float *x0 = nullptr, *x1 = nullptr;
+    float *probes = nullptr, *q_ref = nullptr, *rep = nullptr, *M = nullptr, *img = nullptr;
+    unsigned char *tc_img = nullptr;
+    float *l_probes = nullptr, *l_q = nullptr;
+    int32_t *chosen = nullptr, *acts = nullptr;
+    DevMem mem;
+};
+
+// One loss pass of the federation (launch_fed_loss) over the probe rows [G][kFedProbes][in_dim] of G trainers and their reference
+// Q rows [G][kFedProbes][A]: weight set w evaluates image w - img0 of img (fp32 route) or tc_img (tensor-core route) and writes
+// loss_out[p * ld + w - col0] for every probe group p it covers.
+struct FedLoss {
+    const float *probes, *q_ref;
+    float *loss_out;
+    int G, ld, col0, img0;
+    const float *img;
+    const unsigned char *tc_img;
+};
 
 }  // namespace uavrl
 
@@ -126,6 +155,7 @@ struct uavrl_learner {
     uavrl::LaunchChain chain;         // programmatic dependent launch state of the learner's stream (launch_chain.cuh)
     uint64_t act_calls = 0;
     uint64_t fed_calls = 0;           // ring-sampled federation calls: the Philox counter of their probe draws (federate.cu)
+    uavrl::FedShard fed;              // the sharded federation's rank, phase and buffers
     // data-parallel: one-shot NVLink all-reduce fused with Adam (symmetric buffers exchanged through CUDA IPC), slots of P + 1
     // words (gradient, loss share)
     uavrl::PeerComm comm;
@@ -150,10 +180,9 @@ Route learner_route(const uavrl_learner *l, int n);
 
 int launch_act(uavrl_learner *l, const float *obs, int n, float eps, int is_train, const float *u_tape,
                const int32_t *rand_tape, int32_t *actions, float *q_out, cudaStream_t st);
-// the loss variant of the act pass (federation): weight sets w0 .. w0 + n_weights - 1 on the probe rows [G][kFedProbes][in_dim]
-// (tc_forward.cuh TcArgs::loss_* for the row ranges), losses into loss_out[G][G]
-int launch_fed_loss(uavrl_learner *l, const float *probes, const float *q_ref, float *loss_out, int w0, int n_weights, bool tri,
-                    cudaStream_t st);
+// the loss variant of the act pass (federation): weight sets w0 .. w0 + n_weights - 1 on the probe rows of f (tc_forward.cuh
+// TcArgs::loss_* for the row ranges).  The route follows from f.G alone, so every entry is the same sum whichever launch makes it.
+int launch_fed_loss(uavrl_learner *l, const FedLoss &f, int w0, int n_weights, bool tri, cudaStream_t st);
 // One Trainer.update of B transitions per trainer (global_batch: the batch the loss averages over): gradient step, reduce (+ Adam
 // when apply) into loss_out ([G]), prioritised-replay write-back.  marks (profiling, may be null): events recorded after the
 // TD-target pass, the training kernel and the weight-gradient kernel; they change no launch.

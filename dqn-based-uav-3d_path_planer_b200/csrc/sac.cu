@@ -508,14 +508,15 @@ __global__ void __launch_bounds__(kNetThreads) sac_act_kernel(SacArgs a, const f
 
 // Federated_Learning_AC (Envs/PathPlan_City.py:590-601): global = deepcopy(actor_0); global[k] += actor_i[k] for i = 1 .. G-1;
 // every actor <- global.  The reference's division assigns into a temporary state_dict and is lost, so every actor becomes the
-// float32 sum theta_0 + theta_1 + ... + theta_{G-1}, added left to right in trainer order.  One thread per actor parameter.
-__global__ void sac_federate_kernel(int P, int G, float *__restrict__ actor)
+// float32 sum theta_0 + theta_1 + ... + theta_{G-1}, added left to right in trainer order.  One thread per actor parameter: the
+// sum of the G actors [G][P] in `actors` goes to the n_out actors [n_out][P] in `out` (the same G actors, or a shard's own).
+__global__ void sac_federate_kernel(int P, int G, const float *actors, int n_out, float *out)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
-    float s = actor[i];
-    for (int g = 1; g < G; ++g) s = __fadd_rn(s, actor[(size_t)g * P + i]);
-    for (int g = 0; g < G; ++g) actor[(size_t)g * P + i] = s;
+    float s = actors[i];
+    for (int g = 1; g < G; ++g) s = __fadd_rn(s, actors[(size_t)g * P + i]);
+    for (int g = 0; g < n_out; ++g) out[(size_t)g * P + i] = s;
 }
 
 }  // namespace uavrl
@@ -1033,9 +1034,57 @@ int uavrl_sac_federate_actors(uavrl_sac *s, void *stream)
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     const cudaStream_t st = (cudaStream_t)stream;
     const int P = s->sh.actor.P;
-    sac_federate_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, s->G, s->p[0]);
+    sac_federate_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, s->G, s->p[0], s->G, s->p[0]);
     UAVRL_LAUNCHED();
     return sac_pack(s, 0, st);                                 // the G actor images
+}
+
+int uavrl_sac_fed_shard(uavrl_sac *s, int32_t rank, int32_t world)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (world < 1 || rank < 0 || rank >= world) return fail(UAVRL_ERR_INVALID, "uavrl_sac_fed_shard: needs world >= 1 and rank in [0, world)");
+    const int64_t G = (int64_t)s->G * world;
+    if (G > 65535) return fail(UAVRL_ERR_INVALID, "uavrl_sac_fed_shard: the global trainer count (trainers x world) must be at most 65535");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    DevMem mem;
+    float *x = nullptr;
+    if (int rc = mem.alloc(x, (size_t)G * s->sh.actor.P, false)) return rc;
+    s->fed_mem = std::move(mem);
+    s->fed_x = x; s->fed_rank = rank; s->fed_world = world; s->fed_phase = 0;
+    return 0;
+}
+
+float *uavrl_sac_fed_exchange_ptr(uavrl_sac *s, int64_t *len_out)
+{
+    if (!s || !s->fed_world) return nullptr;
+    if (len_out) *len_out = (int64_t)s->G * s->fed_world * s->sh.actor.P;
+    return s->fed_x;
+}
+
+int uavrl_sac_fed_local(uavrl_sac *s, void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (!s->fed_world) return fail(UAVRL_ERR_STATE, "uavrl_sac_fed_local before uavrl_sac_fed_shard");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    const size_t P = s->sh.actor.P, GL = s->G;
+    UAVRL_CUDA(cudaMemcpyAsync(s->fed_x + (size_t)s->fed_rank * GL * P, s->p[0], GL * P * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    s->fed_phase = 1;
+    return 0;
+}
+
+int uavrl_sac_federate_actors_sharded(uavrl_sac *s, void *stream)
+{
+    if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (!s->fed_world) return fail(UAVRL_ERR_STATE, "uavrl_sac_federate_actors_sharded before uavrl_sac_fed_shard");
+    if (s->fed_phase != 1)
+        return fail(UAVRL_ERR_STATE, "uavrl_sac_federate_actors_sharded called out of order: it runs after uavrl_sac_fed_local and the gather");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int P = s->sh.actor.P;
+    sac_federate_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, s->G * s->fed_world, s->fed_x, s->G, s->p[0]);
+    UAVRL_LAUNCHED();
+    s->fed_phase = 0;
+    return sac_pack(s, 0, st);
 }
 
 

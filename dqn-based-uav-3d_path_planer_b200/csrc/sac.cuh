@@ -34,7 +34,11 @@ struct uavrl_sac {
     uavrl::PeerComm comm;
     int32_t dp_phase = 0, dp_B = 0, dp_global = 0;
     uavrl::BatchSrc dp_src;
-    uavrl::DevMem mem, parts_mem, td_mem;                  // owners: networks, moments, maps, scalars; partials / stat; td
+    // sharded actor aggregation (uavrl_sac_fed_shard): the trainers are global trainers [fed_rank G, (fed_rank + 1) G) of
+    // G fed_world; fed_x [G fed_world][Pa] holds every trainer's actor once gathered, fed_phase 1 once the own slice is written
+    int32_t fed_rank = 0, fed_world = 0, fed_phase = 0;
+    float *fed_x = nullptr;
+    uavrl::DevMem mem, parts_mem, td_mem, fed_mem;         // owners: networks, moments, maps, scalars; partials / stat; td; fed_x
 };
 
 namespace uavrl {

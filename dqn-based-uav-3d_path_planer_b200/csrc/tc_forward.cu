@@ -141,7 +141,7 @@ __device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a
         r0 = (size_t)lo; n_rows = hi - lo;
         tile_step = (a.rows_per_tile / kFedProbes) * kFedProbes;
         n_tiles = (n_rows + tile_step - 1) / tile_step;
-        img = a.img + (size_t)w_set * (size_t)a.img_stride;
+        img = a.img + (size_t)(w_set - a.loss_img0) * (size_t)a.img_stride;
         if ((int)blockIdx.x >= n_tiles) return;                  // nothing staged or waited for yet
     }
     // The first thread of the last warp initialises the two mbarriers and issues the weight copies while the other warps
@@ -255,7 +255,7 @@ __device__ __forceinline__ void tc_forward_body(const TcNet &tc, const TcArgs &a
             }
             __syncthreads();
             if (LOSS && tid * kFedProbes < tile_step && base + tid * kFedProbes < n_rows)   // one probe group per thread
-                fed_group_loss(s_rew + tid * kFedProbes, r0 + base + tid * kFedProbes, a.n, w_set, tc.n_actions, a.loss_out);
+                fed_group_loss(s_rew + tid * kFedProbes, r0 + base + tid * kFedProbes, a.loss_ld, w_set - a.loss_col0, tc.n_actions, a.loss_out);
         };
         forward_layers<FIXED, false>(tc, R, e, Ahi, Alo, W, acc, nullptr, false, mid, head,
                                      [&](int l, uint32_t) { stage_trace(a.trace, 7 + 3 * l); });

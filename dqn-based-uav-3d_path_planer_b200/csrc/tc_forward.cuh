@@ -28,9 +28,9 @@ struct TcArgs {
     int32_t pdl;                       // kPdlOn | kPdlEarlyWeights | kPdlEarlyRows (set by launch_tc_forward)
     long long *trace;                  // debug: CTA (0, 0) / thread 0 writes clock64() at stage boundaries (UAVRL_TC_TRACE=1)
     // loss variant of the act kernel (launch_tc_loss, federation): grid row y evaluates weight set w = loss_w0 + y on the
-    // probe rows [0, S w) (loss_tri) or [S (w + 1), n) of obs = [G][S][in_dim], S = kFedProbes, and writes
-    // loss_out[p][w] = sum over trainer p's S rows of sum_a (q_ref - Q_w)^2 / (S A), q_ref = [G][S][A]
-    const float *q_ref; float *loss_out; int32_t loss_w0, loss_tri;
+    // probe rows [0, S w) (loss_tri) or [S (w + 1), n) of obs = [G][S][in_dim], S = kFedProbes, with image w - loss_img0, and
+    // writes loss_out[p * loss_ld + w - loss_col0] = sum over trainer p's S rows of sum_a (q_ref - Q_w)^2 / (S A), q_ref = [G][S][A]
+    const float *q_ref; float *loss_out; int32_t loss_w0, loss_tri, loss_img0, loss_ld, loss_col0;
 };
 
 int tc_build(const uavrl_learner_config &c, const NetDev &net, TcNet &tc, std::vector<int32_t> &hi_map, std::vector<int32_t> &lo_map,

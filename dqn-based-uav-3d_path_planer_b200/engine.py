@@ -110,6 +110,11 @@ class EnvBatch:
     def reset(self, first_scenario=0):
         check(_lib.lib().uavrl_env_reset(self.h, int(first_scenario), _stream(self.device)))
 
+    def set_reset_stride(self, stride):
+        """Scenario advance of each env's auto-reset (default n).  A shard of N / W envs of an N-env batch, reset with
+        first + r N / W, sets N and draws exactly the scenarios of its rows of the full batch."""
+        check(_lib.lib().uavrl_env_set_reset_stride(self.h, int(stride)))
+
     # -- stepping (device buffers)
     def observe(self, out=None):
         if out is None:
@@ -411,18 +416,7 @@ class Learner(_PerCalls):
         ring; probe_tape: (G, 10) trainer-local replay indices for the ring draw, a host array (checked, then uploaded) or a
         device int32 tensor.  want_details: returns device tensors (probe_idx (G, 10), losses (G, G), chosen (G, max(1, k)))."""
         G = self.G
-        if probe_tape is not None and not isinstance(probe_tape, torch.Tensor):
-            tape = np.ascontiguousarray(probe_tape, np.int64)
-            if tape.shape != (G, 10):
-                raise ValueError("probe_tape must be (%d, 10), got %s" % (G, tape.shape))
-            if any(len(set(row.tolist())) != 10 for row in tape):
-                raise ValueError("probe_tape rows must hold 10 distinct indices")
-            n_g = self.replay_size() // G
-            if (tape < 0).any() or (tape >= n_g).any():
-                raise ValueError("probe_tape indices must lie in [0, %d) (transitions per trainer)" % n_g)
-            probe_tape = torch.from_numpy(tape.astype(np.int32)).to(self.device)
-        if probe_states is not None and tuple(probe_states.shape) != (G, 10, self.in_dim):
-            raise ValueError("probe_states must be (%d, 10, %d)" % (G, self.in_dim))
+        probe_states, probe_tape = self._probe_sources(G, probe_states, probe_tape)
         k = (G - 1) // 2
         idx = losses = chosen = None
         if want_details:
@@ -432,6 +426,82 @@ class Learner(_PerCalls):
         check(_lib.lib().uavrl_learner_federate(self.h, _ptr(probe_states), _ptr(probe_tape), _ptr(idx), _ptr(losses), _ptr(chosen),
                                                 _stream(self.device)))
         if want_details:
+            return idx, losses, chosen
+
+    def _probe_sources(self, G, probe_states, probe_tape):
+        """Checked probe sources of an aggregation over G trainers: a host tape is checked and uploaded as int32."""
+        if probe_tape is not None and not isinstance(probe_tape, torch.Tensor):
+            tape = np.ascontiguousarray(probe_tape, np.int64)
+            if tape.shape != (G, 10):
+                raise ValueError("probe_tape must be (%d, 10), got %s" % (G, tape.shape))
+            if any(len(set(row.tolist())) != 10 for row in tape):
+                raise ValueError("probe_tape rows must hold 10 distinct indices")
+            n_g = self.replay_size() // self.G
+            if (tape < 0).any() or (tape >= n_g).any():
+                raise ValueError("probe_tape indices must lie in [0, %d) (transitions per trainer)" % n_g)
+            probe_tape = torch.from_numpy(tape.astype(np.int32)).to(self.device)
+        if probe_states is not None and tuple(probe_states.shape) != (G, 10, self.in_dim):
+            raise ValueError("probe_states must be (%d, 10, %d)" % (G, self.in_dim))
+        return probe_states, probe_tape
+
+    # -- the aggregation across trainers sharded over ranks (include/uavrl.h, uavrl_learner_fed_shard)
+    def fed_shard(self, rank, world):
+        """Declare this learner's trainers as the global trainers [rank G, (rank + 1) G) of G world (create it with
+        seed + rank G).  Allocates, on the device and until the learner is closed or fed_shard runs again, the two exchange
+        buffers of fed_exchange_tensor and the rounds' scratch: about 4 Gw^2 + 2 Gw (10 in_dim + 10 A + P) floats for
+        Gw = G world trainers in all.  At Gw = 4096 and the 100-64-64-27 network that is 224 MB for exchange 0, 67 MB for
+        exchange 1, and about 0.6 GB in all."""
+        check(_lib.lib().uavrl_learner_fed_shard(self.h, int(rank), int(world)))
+        self.fed_rank, self.fed_world = int(rank), int(world)
+
+    def fed_exchange_tensor(self, phase):
+        """The buffer all-gathered after fed_local (phase 0: [Gw, 10 in_dim + 10 A + P]) or fed_columns (phase 1:
+        [world, Gw, G]), flat, as a torch view; this rank's slice is the rank-th of world equal parts."""
+        n = C.c_int64()
+        ptr = _lib.lib().uavrl_learner_fed_exchange_ptr(self.h, int(phase), C.byref(n))
+        if not ptr:
+            raise ValueError("fed_exchange_tensor needs fed_shard first and phase 0 or 1")
+        return _DevView(ptr, n.value, self.device).tensor()
+
+    def fed_local(self, probe_states=None, probe_tape=None, probe_idx=None):
+        """Phase a: this rank's probe rows (probe_states (G, 10, in_dim), probe_tape (G, 10) device int32, or the ring),
+        their Q and q_local into its slice of exchange 0.  probe_idx: optional (G, 10) int32 device output."""
+        check(_lib.lib().uavrl_learner_fed_local(self.h, _ptr(probe_states), _ptr(probe_tape), _ptr(probe_idx), _stream(self.device)))
+
+    def fed_columns(self):
+        """Phase b, after the gather of exchange 0: this rank's columns of the initial losses into its slice of exchange 1."""
+        check(_lib.lib().uavrl_learner_fed_columns(self.h, _stream(self.device)))
+
+    def fed_rounds(self, losses=None, chosen=None):
+        """Phase c, after the gather of exchange 1: every round, then this rank's q_local.  losses (Gw, Gw) float32 and chosen
+        (Gw, max(1, k)) int32 device outputs may be None."""
+        check(_lib.lib().uavrl_learner_fed_rounds(self.h, _ptr(losses), _ptr(chosen), _stream(self.device)))
+
+    def federate_sharded(self, dist, probe_states=None, probe_tape=None, want_details=False):
+        """federate() across the ranks of torch.distributed `dist` after fed_shard: every rank calls it, and every rank's
+        trainers end where the one-GPU federate() of all Gw trainers leaves them, bit for bit.  probe_states (Gw, 10, in_dim)
+        and probe_tape (Gw, 10) are global (each rank uses its own rows).  want_details: the global (probe_idx (Gw, 10),
+        losses (Gw, Gw), chosen (Gw, max(1, k))) device tensors, as federate() returns them.  The rounds run on every rank,
+        so the call costs what the one-GPU rounds cost, plus two all-gathers."""
+        r, W, G = self.fed_rank, self.fed_world, self.G
+        Gw = G * W
+        probe_states, probe_tape = self._probe_sources(Gw, probe_states, probe_tape)
+        mine = slice(r * G, (r + 1) * G)
+        own = lambda t: None if t is None else t[mine].contiguous()  # noqa: E731
+        idx = losses = chosen = None
+        if want_details:
+            idx = torch.empty((Gw, 10), dtype=torch.int32, device=self.device)
+            losses = torch.empty((Gw, Gw), dtype=torch.float32, device=self.device)
+            chosen = torch.empty((Gw, max(1, (Gw - 1) // 2)), dtype=torch.int32, device=self.device)
+        self.fed_local(own(probe_states), own(probe_tape), None if idx is None else idx[mine])
+        for phase in (0, 1):
+            x = self.fed_exchange_tensor(phase)
+            dist.all_gather_into_tensor(x, x.chunk(W)[r].clone())
+            if phase == 0:
+                self.fed_columns()
+        self.fed_rounds(losses, chosen)
+        if want_details:
+            dist.all_gather_into_tensor(idx, idx[mine].clone())
             return idx, losses, chosen
 
     def update_batch(self, s, a, r, s2, d, loss=None):
@@ -653,6 +723,37 @@ class SacLearner(_PerCalls):
         """Federated_Learning_AC (PathPlan_City.py:590-601, include/uavrl.h uavrl_sac_federate_actors): every trainer's actor
         becomes the float32 sum of all G actors (the reference's division by G is lost); nothing else changes."""
         check(_lib.lib().uavrl_sac_federate_actors(self.h, _stream(self.device)))
+
+    # -- the actor aggregation across trainers sharded over ranks (include/uavrl.h, uavrl_sac_fed_shard)
+    def fed_shard(self, rank, world):
+        """Declare this learner's trainers as the global trainers [rank G, (rank + 1) G) of G world (create it with
+        seed + rank G); allocates the exchange buffer of every global trainer's actor (G world Pa floats)."""
+        check(_lib.lib().uavrl_sac_fed_shard(self.h, int(rank), int(world)))
+        self.fed_rank, self.fed_world = int(rank), int(world)
+
+    def fed_exchange_tensor(self):
+        """The [G world, Pa] actor buffer, flat, as a torch view; this rank's slice is the rank-th of world equal parts."""
+        n = C.c_int64()
+        ptr = _lib.lib().uavrl_sac_fed_exchange_ptr(self.h, C.byref(n))
+        if not ptr:
+            raise ValueError("fed_exchange_tensor needs fed_shard first")
+        return _DevView(ptr, n.value, self.device).tensor()
+
+    def fed_local(self):
+        """This rank's actors into its slice of the exchange buffer."""
+        check(_lib.lib().uavrl_sac_fed_local(self.h, _stream(self.device)))
+
+    def fed_sum_actors(self):
+        """After the gather: every own actor becomes the sum of all G world actors in trainer order."""
+        check(_lib.lib().uavrl_sac_federate_actors_sharded(self.h, _stream(self.device)))
+
+    def federate_actors_sharded(self, dist):
+        """federate_actors() across the ranks of torch.distributed `dist` after fed_shard: every rank's actors end as the
+        one-GPU call on all trainers leaves them, bit for bit."""
+        self.fed_local()
+        x = self.fed_exchange_tensor()
+        dist.all_gather_into_tensor(x, x.chunk(self.fed_world)[self.fed_rank].clone())
+        self.fed_sum_actors()
 
     def _losses(self, losses):
         """A caller's loss tensor: an update writes 4 losses per trainer, so it must hold at least 4 G floats."""

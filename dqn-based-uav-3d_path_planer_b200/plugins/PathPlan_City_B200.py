@@ -2,6 +2,9 @@
 stepped in lockstep on a H100.  <num_trainers> (default 1) independent Q-network trainers share them: trainer g learns
 from UAVs [g num_UAV / num_trainers, (g + 1) num_UAV / num_trainers) and is named UAV_<g num_UAV / num_trainers>.
 num_trainers = num_UAV is the reference's one trainer per UAV (PathPlan_City.py:59-69); 1 is one shared trainer.
+<shard_over_ranks>1</shard_over_ranks> spreads the UAVs and the trainers over the W ranks of an initialised torch.distributed
+group (one process per GPU): rank r steps UAVs [r num_UAV / W, (r + 1) num_UAV / W) and trains trainers
+[r num_trainers / W, (r + 1) num_trainers / W), each computing what the one-GPU run's trainer of that index computes.
 
 Constructor takes the same parsed-XML dict the reference's EnvFactory passes
 (config/PathPlan_City.xml <env> ... </env>): len/width/h, num_UAV, Agent.xml_path_agent,
@@ -124,14 +127,32 @@ class PathPlan_City_B200:
         self.num_trainers = int(None2Value(param.get('num_trainers'), 1))
         if self.num_trainers < 1 or self.num_UAV % self.num_trainers != 0:
             raise ValueError("num_UAV (%d) must be a multiple of num_trainers (%d)" % (self.num_UAV, self.num_trainers))
+        # shard_over_ranks = 1: this rank's share of the UAVs and trainers.  Its env shard draws the scenarios of its rows of the
+        # whole batch (reset stride num_UAV), its trainers are seeded and named by their global index, the episode loop sums
+        # its counts over the ranks once per chunk, and the aggregations run across the ranks (federate_sharded)
+        self.shard_over_ranks = int(None2Value(param.get('shard_over_ranks'), 0))
+        self.rank, self.world, self._dist = 0, 1, None
+        if self.shard_over_ranks:
+            import torch.distributed as dist
+            if not (dist.is_available() and dist.is_initialized()):
+                raise ValueError("shard_over_ranks = 1 needs an initialised torch.distributed process group")
+            self.rank, self.world, self._dist = dist.get_rank(), dist.get_world_size(), dist
+            if self.num_UAV % self.world or self.num_trainers % self.world:
+                raise ValueError("shard_over_ranks = 1 needs num_UAV (%d) and num_trainers (%d) to be multiples of the world size "
+                                 "(%d)" % (self.num_UAV, self.num_trainers, self.world))
+            if param.get("device") is None:
+                self.device_index = torch.cuda.current_device()
+        self.n_local = self.num_UAV // self.world              # the UAVs this process steps
         agents_params = param.get('Agent')
         self.uav_dict = XML2Dict(os.path.normpath(agents_params['xml_path_agent'])).get('Agent')
         self.uav_params = uav_params_from_dict(self.uav_dict)
         self.sub_granularity = int(None2Value(self.uav_dict.get("sub_granularity"), 30))
         fn = self.uav_dict.get("update_function_name")
         self.discrete = (fn != "update_PathPlan")            # update_PathPlan27: the discrete-27 extension
-        self.batch = engine.EnvBatch(self.city, self.uav_params, self.num_UAV, max_subgoals=64,
+        self.batch = engine.EnvBatch(self.city, self.uav_params, self.n_local, max_subgoals=64,
                                      device=self.device_index, auto_reset=True)
+        if self.shard_over_ranks:
+            self.batch.set_reset_stride(self.num_UAV)
         self.pool_size = int(None2Value(param.get("scenario_pool"), max(1024, 2 * self.num_UAV)))
         sc = self.batch.make_scenarios(self.pool_size, seed=int(None2Value(param.get("seed"), 42)),
                                        rrt_step=self.sub_granularity)
@@ -159,8 +180,14 @@ class PathPlan_City_B200:
         self.host_driven = int(None2Value(param.get('host_driven'), 0))
         if self.host_driven and self.num_trainers > 1:
             raise ValueError("host_driven = 1 drives one trainer: it needs num_trainers = 1")
-        tdict['n_trainers'] = str(self.num_trainers)
-        tdict['lockstep_envs'] = '0' if self.host_driven else str(self.num_UAV)
+        if self.host_driven and self.shard_over_ranks:
+            raise ValueError("host_driven = 1 drives one process's host arrays: it cannot shard over ranks (set shard_over_ranks = 0)")
+        g_local = self.num_trainers // self.world
+        tdict['n_trainers'] = str(g_local)
+        tdict['lockstep_envs'] = '0' if self.host_driven else str(self.n_local)
+        if self.shard_over_ranks:
+            tdict['first_trainer'] = str(self.rank * g_local)
+            tdict['seed'] = str(int(None2Value(tdict.get('seed'), 42)) + self.rank * g_local)
         tdict['device'] = str(self.device_index)
         ttype = tdict.get('Trainer_Type')
         try:
@@ -190,6 +217,8 @@ class PathPlan_City_B200:
             if self.Is_AC and not isinstance(self.Trainer._learner, engine.SacLearner):
                 raise ValueError("Is_FL = 1 with Is_AC = 1 averages the trainers' actors (Federated_Learning_AC), which DQN-family "
                                  "trainers do not have: set Is_AC = 0")
+            if self.shard_over_ranks:
+                self.Trainer._learner.fed_shard(self.rank, self.world)
         self.executed_time = 0
         self.Scene_Random_Reset()
 
@@ -201,7 +230,7 @@ class PathPlan_City_B200:
     def Scene_Random_Reset(self):
         """UAV.reset() for the whole batch (a new block of the scenario pool).  Individual UAVs whose
         episode ends restart by themselves inside the step kernel."""
-        self.batch.reset(self._next_first)
+        self.batch.reset(self._next_first + self.rank * self.n_local)
         self._next_first = (self._next_first + self.num_UAV) % self.pool_size
         self.Trainer._learner_reset_lockstep()
 
@@ -296,8 +325,15 @@ class PathPlan_City_B200:
             # the device loop advances `chunk` epochs per call: save whenever a multiple of save_loop was crossed
             if save_loop > 0 and self.Trainer.epoch // save_loop != e_before // save_loop:
                 self.Trainer.save()
-            ended += st.episodes_ended; steps += st.env_steps; updates += st.updates; coll += st.collisions
-            n_s += st.n_success; n_l += st.n_lose; reward_sum += st.sum_reward; loss = st.last_loss
+            c = [st.episodes_ended, st.env_steps, st.collisions, st.n_success, st.n_lose, st.sum_reward, st.last_loss]
+            if self._dist is not None:                             # every rank stops at the chunk the one-GPU run stops at
+                t = torch.tensor(c, dtype=torch.float64, device=self.batch.device)
+                self._dist.all_reduce(t)
+                c = t.tolist()
+                c[:5] = [int(x) for x in c[:5]]
+                c[6] /= self.world                                 # the mean of the ranks' mean trainer losses
+            ended += c[0]; steps += c[1]; updates += st.updates; coll += c[2]
+            n_s += c[3]; n_l += c[4]; reward_sum += c[5]; loss = c[6]
             iters += chunk
         dt = time.time() - t0
         ag = self.Agents[0]
@@ -326,16 +362,22 @@ class PathPlan_City_B200:
         Federated_Learning (:475), which cannot run (sample2 unpacking, trainer methods the reference lacks); this plug-in runs
         the reference's selective aggregation instead.  One trainer (or the SAC trainer) has nothing to aggregate with."""
         learner = self.Trainer._learner
-        if isinstance(learner, engine.SacLearner) or learner.trainer_count() < 2:
+        if isinstance(learner, engine.SacLearner) or self.num_trainers < 2:
             return
-        learner.federate()
+        if self._dist is not None:
+            learner.federate_sharded(self._dist)
+        else:
+            learner.federate()
 
     def Federated_Learning_AC(self):
         """PathPlan_City.py:590-601 on the device (engine.SacLearner.federate_actors): every SAC trainer's actor is replaced by
         the sum of all trainers' actors.  The reference divides by the trainer count into a temporary state_dict, so the
         division is lost and the sum is what it trains on; this plug-in reproduces that.  Critics, targets, Adam moments and
         alpha are untouched; one trainer keeps its actor."""
-        self.Trainer._learner.federate_actors()
+        if self._dist is not None:
+            self.Trainer._learner.federate_actors_sharded(self._dist)
+        else:
+            self.Trainer._learner.federate_actors()
 
     def _write_path_csv(self, path="path.csv"):
         """UAV.py:461-464 / :479-482 / :505-508: at a terminal step the reference rewrites path.csv (CWD-relative) with the

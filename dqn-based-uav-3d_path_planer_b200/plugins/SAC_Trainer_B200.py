@@ -34,9 +34,10 @@ class SAC_Trainer_B200:
         self.device_index = int(None2Value(param.get('device'), 0))
         # n_trainers = G > 1: one independent SAC trainer per block of lockstep_envs / G UAVs (the reference's SAC_Trainer per UAV,
         # PathPlan_City.py:59-69), each with its own replay_size transitions; trainer g is named UAV_<g * lockstep_envs / G>
+        # (first_trainer: the global index of trainer 0 when the env plug-in shards the trainers over ranks)
         self.n_trainers = int(None2Value(param.get('n_trainers'), 1))
         G = self.n_trainers
-        self.names = [self.name] if G == 1 else ['UAV_%d' % (g * (self.lockstep_envs // G)) for g in range(G)]
+        self.names = checkpoint.trainer_names(self.name, self.lockstep_envs, G, param.get('first_trainer'))
         self._learner = engine.SacLearner(
             self.w, self.hidden, self.act_dim, float(actor.get('action_bound')), float(actor.get('lr')), float(critic.get('lr')),
             float(sp.get('alpha_lr')), float(sp.get('target_entropy')), float(sp.get('gamma')), float(sp.get('tau')),

@@ -91,9 +91,10 @@ class TrainerB200:
         self.lockstep_envs = int(None2Value(param.get('lockstep_envs'), 0))
         # n_trainers = G > 1: one independent trainer per block of lockstep_envs / G UAVs (the reference's Trainer per UAV,
         # PathPlan_City.py:59-69), each with its own replay_size transitions; trainer g is named UAV_<g * lockstep_envs / G>
+        # (first_trainer: the global index of trainer 0 when the env plug-in shards the trainers over ranks)
         self.n_trainers = int(None2Value(param.get('n_trainers'), 1))
         G = self.n_trainers
-        self.names = [self.name] if G == 1 else ['UAV_%d' % (g * (self.lockstep_envs // G)) for g in range(G)]
+        self.names = checkpoint.trainer_names(self.name, self.lockstep_envs, G, param.get('first_trainer'))
         self._learner = engine.Learner(self.w, hidden_fn(hid), self.output, dueling, self.ALGO, lr=self.LEARNING_RATE,
                                        gamma=self.gamma, batch_size=self.Batch_Size, update_loop=self.Update_loop,
                                        replay_capacity=self.replay_size * G, lockstep_envs=self.lockstep_envs,

@@ -7,6 +7,17 @@ import numpy as np
 import torch
 
 
+def trainer_names(name, lockstep_envs, n_trainers, first_trainer=None):
+    """The name each trainer's checkpoint files carry: `name` for one trainer, else UAV_<g lockstep_envs / n_trainers> for
+    global trainer g (its first UAV).  first_trainer: the global index of this handle's trainer 0 when the trainers are a
+    shard of a larger group (rank r of W holds trainers [r n_trainers, (r + 1) n_trainers)), so every shard names its
+    trainers as the one-GPU run of the whole group does, and checkpoint directories interchange."""
+    if first_trainer is None and n_trainers == 1:
+        return [name]
+    per = lockstep_envs // n_trainers
+    return ['UAV_%d' % ((int(first_trainer or 0) + g) * per) for g in range(n_trainers)]
+
+
 def flat(tensors):
     """Tensors or arrays concatenated into one flat float32 vector."""
     return np.concatenate([np.asarray(v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v, np.float32).ravel()

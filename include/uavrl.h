@@ -84,6 +84,11 @@ int uavrl_env_set_pool(uavrl_env *env, int32_t n_scenarios, const double *start_
 
 /* UAV.reset() for every env: env e takes scenario (first_scenario + e) mod P of the pool. */
 int uavrl_env_reset(uavrl_env *env, int32_t first_scenario, void *stream);
+/* The scenario an env takes at each auto-reset: its current scenario + stride (mod P).  The stride defaults to n_envs, which
+ * keeps every env of the batch on its own scenarios.  A shard of a larger batch (rank r of W, n_envs = N / W, reset with
+ * first_scenario + r N / W) sets stride N and then draws exactly the scenarios of its rows of the N-env batch.  Refused with
+ * UAVRL_ERR_INVALID for stride < 1.  Takes effect from the next step. */
+int uavrl_env_set_reset_stride(uavrl_env *env, int32_t stride);
 
 /* Host-side scenario generator (reset draws + RRT) for synthetic pools: statistical restatement of
  * UAV.py:344-360 + RRT.py:26-105 with a counter-based RNG (the reference's Python MT19937 stream is
@@ -242,6 +247,32 @@ int32_t uavrl_learner_trainer_count(const uavrl_learner *l);
 int uavrl_learner_federate(uavrl_learner *l, const float *probe_states_dev, const int32_t *probe_tape_dev,
                            int32_t *probe_idx_out_dev, float *loss_out_dev, int32_t *chosen_out_dev, void *stream);
 
+/* The same aggregation over trainers spread across ranks (one trainer group per UAV group, the groups sharded over GPUs).
+ * Rank r's learner of G_local trainers holds the global trainers [r G_local, (r + 1) G_local) of G = G_local world: create it
+ * with seed + r G_local.  uavrl_learner_fed_shard declares the shard once and allocates the buffers below (freed with the
+ * handle, replaced by a later call); refused with UAVRL_ERR_INVALID for world < 1, rank outside [0, world) or G > 65535.
+ * One aggregation is three calls with two all-gathers between them, which the caller makes in rank order into the buffers
+ * uavrl_learner_fed_exchange_ptr returns (phase 0 or 1; NULL before uavrl_learner_fed_shard; len_out = floats in all, rank r's
+ * slice is the r-th of world equal parts):
+ *   uavrl_learner_fed_local     probe states of the own trainers (from the ring as uavrl_learner_federate draws them, or the
+ *                               own rows [G_local][10][in_dim] / [G_local][10] of explicit states or a tape; probe_idx_out
+ *                               [G_local][10] as there), their Q, and q_local: [probes | q_ref | q_local] per trainer into
+ *                               exchange 0 = [G][10 in_dim + 10 A + P] (13 649 floats per trainer at 100-64-64-27);
+ *   uavrl_learner_fed_columns   after the gather of exchange 0: the initial losses of the own trainers' columns into exchange
+ *                               1 = [world][G][G_local];
+ *   uavrl_learner_fed_rounds    after the gather of exchange 1: rounds p = 0 .. G-1, run redundantly on every rank, then the
+ *                               own q_local and images.  loss_out [G][G] and chosen_out [G][max(1, k)] as uavrl_learner_federate.
+ * Every rank ends with the parameters, losses and chosen lists the one-GPU call on all G trainers produces, bit for bit.
+ * Device memory per rank: about 4 G^2 + 2 G (10 in_dim + 10 A + P) floats.  Refused with UAVRL_ERR_STATE before
+ * uavrl_learner_fed_shard or out of order (columns need local, rounds need columns; local may restart at any time), and
+ * with UAVRL_ERR_INVALID as uavrl_learner_federate refuses its probe sources; a refused call changes nothing. */
+int uavrl_learner_fed_shard(uavrl_learner *l, int32_t rank, int32_t world);
+float *uavrl_learner_fed_exchange_ptr(uavrl_learner *l, int32_t phase, int64_t *len_out);
+int uavrl_learner_fed_local(uavrl_learner *l, const float *probe_states_dev, const int32_t *probe_tape_dev,
+                            int32_t *probe_idx_out_dev, void *stream);
+int uavrl_learner_fed_columns(uavrl_learner *l, void *stream);
+int uavrl_learner_fed_rounds(uavrl_learner *l, float *loss_out_dev, int32_t *chosen_out_dev, void *stream);
+
 /* state_dict()-ordered flat fp32 parameters (fc1.weight [out][in], fc1.bias, ..., for dueling nets
  * ..., fc_A.weight, fc_A.bias, fc_V.weight, fc_V.bias) -- what torch.save({'model': ...}) holds
  * (DuelingDQN_Trainer.py:79-84).  which: 0 = q_local, 1 = q_target, 2 = Adam exp_avg,
@@ -386,6 +417,17 @@ int32_t uavrl_sac_trainer_count(const uavrl_sac *s);
  * right in trainer order (bit-reproducible).  G = 1 leaves the actor as it is.  Critics, targets, every Adam moment, alpha,
  * epoch and adam_step are untouched.  Enqueued on `stream` (two launches), with no host synchronisation. */
 int uavrl_sac_federate_actors(uavrl_sac *s, void *stream);
+/* Federated_Learning_AC over trainers spread across ranks: rank r's learner of G_local trainers holds the global trainers
+ * [r G_local, (r + 1) G_local) of G = G_local world (created with seed + r G_local).  uavrl_sac_fed_shard declares the shard and
+ * allocates the exchange [G][Pa] (6 724 floats per trainer at the shipped shape; refused with UAVRL_ERR_INVALID for world < 1,
+ * rank outside [0, world) or G > 65535); uavrl_sac_fed_exchange_ptr returns it (NULL before the shard; rank r's slice is the
+ * r-th of world parts).  uavrl_sac_fed_local copies the own actors into the own slice; after the caller's all-gather,
+ * uavrl_sac_federate_actors_sharded sums the G actors in trainer order 0 .. G-1, as uavrl_sac_federate_actors does, into every
+ * own actor and its image.  Refused with UAVRL_ERR_STATE before the shard, or the sum without a local call since the last. */
+int uavrl_sac_fed_shard(uavrl_sac *s, int32_t rank, int32_t world);
+float *uavrl_sac_fed_exchange_ptr(uavrl_sac *s, int64_t *len_out);
+int uavrl_sac_fed_local(uavrl_sac *s, void *stream);
+int uavrl_sac_federate_actors_sharded(uavrl_sac *s, void *stream);
 /* Shared memory (dynamic + static bytes) one block of each SAC kernel would take for cfg's networks: bytes_out[4] = target,
  * critic update, actor update, get_action.  uavrl_sac_create refuses cfg when any exceeds 227 KB (232 448 B). */
 int uavrl_sac_smem_bytes(const uavrl_sac_config *cfg, int64_t *bytes_out);
