@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libuavrl_b200.so")
-SOURCES = ["env.cu", "scenario.cu", "learner.cu", "tc_forward.cu", "tc_train.cu", "train.cu", "sac.cu", "per.cu", "federate.cu", "replay.cu", "optim.cu"]
+SOURCES = ["env.cu", "scenario.cu", "learner.cu", "tc_forward.cu", "tc_train.cu", "train.cu", "eval.cu", "sac.cu", "per.cu", "federate.cu", "replay.cu", "optim.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
                      "-Xcompiler", "-fPIC,-ffp-contract=off", "-Xptxas", "-v"]

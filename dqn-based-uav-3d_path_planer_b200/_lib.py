@@ -46,6 +46,15 @@ class EnvExtras(C.Structure):
                 ("track_capacity", C.c_int32)]
 
 
+class EpisodeRecord(C.Structure):
+    _fields_ = [(k, C.c_int32) for k in ("scenario", "env", "ordinal", "outcome", "steps", "subgoals", "collisions", "reserved")] + \
+               [(k, C.c_double) for k in ("total_score", "path_len", "start2goal", "planner_len", "final_dist", "energy")]
+
+
+class EvalStats(C.Structure):
+    _fields_ = [("iterations", C.c_int64), ("records", C.c_int64), ("unfinished", C.c_int64)]
+
+
 class LearnerConfig(C.Structure):
     _fields_ = [("in_dim", C.c_int32), ("n_hidden", C.c_int32), ("hidden", C.c_int32 * MAX_HIDDEN),
                 ("n_actions", C.c_int32), ("dueling", C.c_int32), ("algo", C.c_int32),
@@ -90,6 +99,12 @@ SIGNATURES = {
     "uavrl_env_get_energy_total": (C.c_int, [VP, C.POINTER(C.c_double)]),
     "uavrl_env_get_path": (C.c_int, [VP, C.c_int32, C.c_int32, C.c_int32, VP, VP]),
     "uavrl_env_get_subgoals": (C.c_int, [VP, VP]),
+    "uavrl_env_set_records": (C.c_int, [VP, C.c_int64]),
+    "uavrl_env_get_records": (C.c_int, [VP, C.c_int64, VP, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32]),
+    "uavrl_env_clear_records": (C.c_int, [VP]),
+    "uavrl_eval_run": (C.c_int, [VP, VP, C.c_int32, C.c_int32, C.c_int64, VP, C.POINTER(EvalStats), VP]),
+    "uavrl_sac_eval_run": (C.c_int, [VP, VP, C.c_int32, C.c_int32, C.c_int32, C.c_int64, VP, C.POINTER(EvalStats), VP]),
+    "uavrl_sac_act_mean": (C.c_int, [VP, VP, C.c_int32, VP, VP]),
     "uavrl_per_enable": (C.c_int, [VP, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double]),
     "uavrl_per_enable_trainers": (C.c_int, [VP, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double]),
     "uavrl_per_sample": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP]),

@@ -41,15 +41,31 @@ env_kernel(EnvDev d, int action_kind, const void *__restrict__ actions, float *_
            float *__restrict__ reward, uint8_t *__restrict__ done_out, uint8_t *__restrict__ info_out,
            uint8_t *__restrict__ coll_out, uint8_t *__restrict__ ended_out)
 {
+    static_assert(!EXTRAS, "the optional models run env_extras_kernel");
     __shared__ EnvSmem<EPB> sm;
     env_block<DO_STEP, EPB, kEnvThreads, true, (EPB < 32 ? EPB : 32), EXTRAS>(d, sm, blockIdx.x * EPB, threadIdx.x, action_kind, actions, obs,
                                                                               reward, done_out, info_out, coll_out, ended_out);
 }
 
-__global__ void env_reset_kernel(EnvDev d, int first)
+// The EXTRAS instantiation (uavrl_env_set_extras, uavrl_env_set_records): a kernel of its own, so that its records argument
+// leaves the default kernels' parameters, and with them their code, as they are
+template <bool DO_STEP, int EPB>
+__global__ void __launch_bounds__(kEnvThreads)
+env_extras_kernel(EnvDev d, int action_kind, const void *__restrict__ actions, float *__restrict__ obs,
+                  float *__restrict__ reward, uint8_t *__restrict__ done_out, uint8_t *__restrict__ info_out,
+                  uint8_t *__restrict__ coll_out, uint8_t *__restrict__ ended_out, EnvRecDev rec)
+{
+    __shared__ EnvSmem<EPB> sm;
+    env_block<DO_STEP, EPB, kEnvThreads, true, (EPB < 32 ? EPB : 32), true>(d, sm, blockIdx.x * EPB, threadIdx.x, action_kind, actions, obs,
+                                                                            reward, done_out, info_out, coll_out, ended_out, &rec);
+}
+
+// uavrl_env_reset on envs [0, n_reset): the env's first scenario first + e; with records on, its episode counters restart
+__global__ void env_reset_kernel(EnvDev d, int first, int n_reset, EnvRecDev rec)
 {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= d.n) return;
+    if (e >= d.n || e >= n_reset) return;
+    if (d.extras & kExtraRecord) { rec.steps[e] = 0; rec.coll[e] = 0; }
     const int scen = (int)(((long long)first + e) % d.P);
     EnvRegs s;
     load_scenario(d, scen, s);
@@ -85,10 +101,11 @@ __global__ void threat_kernel(EnvDev d, int n, const double *__restrict__ pts, u
     out[i] = (uint8_t)hit;
 }
 
-int launch_env_step(const EnvDev &d_in, int action_kind, const void *actions, float *obs, float *reward,
+int launch_env_step(const uavrl_env *env, int action_kind, const void *actions, float *obs, float *reward,
                     uint8_t *done, uint8_t *info, uint8_t *coll, uint8_t *ended, cudaStream_t st, bool pdl)
 {
-    EnvDev d = d_in;
+    EnvDev d = env->d;
+    const EnvRecDev &rec = env->records.dev;
     static const bool trace_on = getenv("UAVRL_ENV_TRACE") != nullptr;
     static DevMem tr_mem;
     static long long *tr = nullptr;
@@ -107,8 +124,8 @@ int launch_env_step(const EnvDev &d_in, int action_kind, const void *actions, fl
     }
     if (d.extras) {                                              // optional models: the EXTRAS instantiation (never inside a PDL chain)
         const int blocks = (d.n + kEnvsPerBlockSmall - 1) / kEnvsPerBlockSmall;
-        UAVRL_CUDA(launch_kernel(env_kernel<true, kEnvsPerBlockSmall, true>, dim3(blocks), dim3(kEnvThreads), 0, st, pdl, d, action_kind, actions, obs,
-                                 reward, done, info, coll, ended));
+        UAVRL_CUDA(launch_kernel(env_extras_kernel<true, kEnvsPerBlockSmall>, dim3(blocks), dim3(kEnvThreads), 0, st, pdl, d, action_kind, actions, obs,
+                                 reward, done, info, coll, ended, rec));
     } else if (d.n <= small_batch_envs()) {
         const int blocks = (d.n + kEnvsPerBlockSmall - 1) / kEnvsPerBlockSmall;
         UAVRL_CUDA(launch_kernel(env_kernel<true, kEnvsPerBlockSmall>, dim3(blocks), dim3(kEnvThreads), 0, st, pdl, d, action_kind, actions, obs,
@@ -122,12 +139,44 @@ int launch_env_step(const EnvDev &d_in, int action_kind, const void *actions, fl
     return 0;
 }
 
-int launch_env_observe(const EnvDev &d, float *obs, cudaStream_t st)
+int launch_env_observe(const uavrl_env *env, float *obs, cudaStream_t st)
 {
+    const EnvDev &d = env->d;
+    const EnvRecDev &rec = env->records.dev;
     const int blocks = (d.n + kEnvsPerBlockLarge - 1) / kEnvsPerBlockLarge;
-    if (d.extras) env_kernel<false, kEnvsPerBlockLarge, true><<<blocks, kEnvThreads, 0, st>>>(d, 0, nullptr, obs, nullptr, nullptr, nullptr, nullptr, nullptr);
+    if (d.extras) env_extras_kernel<false, kEnvsPerBlockLarge><<<blocks, kEnvThreads, 0, st>>>(d, 0, nullptr, obs, nullptr, nullptr, nullptr, nullptr, nullptr, rec);
     else env_kernel<false, kEnvsPerBlockLarge><<<blocks, kEnvThreads, 0, st>>>(d, 0, nullptr, obs, nullptr, nullptr, nullptr, nullptr, nullptr);
     UAVRL_LAUNCHED();
+    return 0;
+}
+
+int launch_env_reset(uavrl_env *env, int first, int n_reset, cudaStream_t st)
+{
+    const int threads = 128, blocks = (env->d.n + threads - 1) / threads;
+    env_reset_kernel<<<blocks, threads, 0, st>>>(env->d, first, n_reset, env->records.dev);
+    UAVRL_LAUNCHED();
+    env->reset_done = true;
+    return 0;
+}
+
+int records_alloc(EnvRecords &r, int n, int64_t cap)
+{
+    EnvRecDev v = { nullptr, cap, INT64_MAX, nullptr, nullptr, nullptr, nullptr };
+    int rc;
+    if ((rc = r.mem.alloc(v.rec, (size_t)cap)) || (rc = r.mem.alloc(v.ord, (size_t)n)) || (rc = r.mem.alloc(v.steps, (size_t)n)) ||
+        (rc = r.mem.alloc(v.coll, (size_t)n)) || (rc = r.mem.alloc(v.counts, 2)))
+        return rc;
+    r.dev = v;
+    r.on = true;
+    return 0;
+}
+
+// empties the slots and counts and restarts the ordinals; the episodes in progress keep their step and collision counts
+int records_clear(EnvRecords &r, int n, cudaStream_t st)
+{
+    UAVRL_CUDA(cudaMemsetAsync(r.dev.rec, 0, (size_t)r.dev.cap * sizeof(uavrl_episode_record), st));
+    UAVRL_CUDA(cudaMemsetAsync(r.dev.ord, 0, (size_t)n * 4, st));
+    UAVRL_CUDA(cudaMemsetAsync(r.dev.counts, 0, 2 * sizeof(unsigned long long), st));
     return 0;
 }
 
@@ -306,11 +355,7 @@ int uavrl_env_reset(uavrl_env *env, int32_t first, void *stream)
     if (!env) return fail(UAVRL_ERR_INVALID, "null env");
     if (!env->pool_set) return fail(UAVRL_ERR_STATE, "uavrl_env_reset before uavrl_env_set_pool");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
-    const int threads = 128, blocks = (env->d.n + threads - 1) / threads;
-    env_reset_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(env->d, first);
-    UAVRL_LAUNCHED();
-    env->reset_done = true;
-    return 0;
+    return launch_env_reset(env, first, env->d.n, (cudaStream_t)stream);
 }
 
 int uavrl_env_set_reset_stride(uavrl_env *env, int32_t stride)
@@ -326,7 +371,7 @@ int uavrl_env_observe(uavrl_env *env, float *obs_dev, void *stream)
     if (!env || !obs_dev) return fail(UAVRL_ERR_INVALID, "null argument");
     if (!env->reset_done) return fail(UAVRL_ERR_STATE, "uavrl_env_observe before uavrl_env_reset");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
-    return launch_env_observe(env->d, obs_dev, (cudaStream_t)stream);
+    return launch_env_observe(env, obs_dev, (cudaStream_t)stream);
 }
 
 int uavrl_env_step(uavrl_env *env, int32_t action_kind, const void *actions_dev, float *next_obs_dev,
@@ -337,7 +382,7 @@ int uavrl_env_step(uavrl_env *env, int32_t action_kind, const void *actions_dev,
     if (action_kind < 0 || action_kind > 3) return fail(UAVRL_ERR_INVALID, "unknown action_kind");
     if (!env->reset_done) return fail(UAVRL_ERR_STATE, "uavrl_env_step before uavrl_env_reset");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
-    return launch_env_step(env->d, action_kind, actions_dev, next_obs_dev, reward_dev, done_dev, info_dev,
+    return launch_env_step(env, action_kind, actions_dev, next_obs_dev, reward_dev, done_dev, info_dev,
                            collision_dev, ended_dev, (cudaStream_t)stream);
 }
 
@@ -357,7 +402,7 @@ int uavrl_env_step_host(uavrl_env *env, int32_t action_kind, const void *actions
     const size_t asz = (action_kind == UAVRL_ACT_CONT_F64 || action_kind == UAVRL_ACT_CONT_F32X2) ? 8 : 4;
     UAVRL_CUDA(cudaMemcpyAsync(env->h_act_dev, actions_host, n * asz, cudaMemcpyHostToDevice, st));
     uint8_t *f = env->h_flags_dev;
-    int rc = launch_env_step(env->d, action_kind, env->h_act_dev, obs_host ? env->h_obs_dev : nullptr,
+    int rc = launch_env_step(env, action_kind, env->h_act_dev, obs_host ? env->h_obs_dev : nullptr,
                              env->h_rew_dev, f, f + n, f + 2 * n, f + 3 * n, st);
     if (rc) return rc;
     if (obs_host) UAVRL_CUDA(cudaMemcpyAsync(obs_host, env->h_obs_dev, n * kObsDim * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -421,7 +466,7 @@ int uavrl_env_set_extras(uavrl_env *env, const uavrl_env_extras *x)
     EnvDev d = env->d;
     DevMem m;
     d.energy = nullptr; d.apf_obs = nullptr; d.sub_env = nullptr; d.path_buf = nullptr; d.path_n = nullptr; d.path_cur = nullptr;
-    d.extras = 0; d.track_n = 0; d.track_cap = 0;
+    d.extras = env->d.extras & kExtraRecord; d.track_n = 0; d.track_cap = 0;      // the records stay as they are
     const size_t n = (size_t)d.n;
     int rc;
     if (x->energy_enabled) {
@@ -521,6 +566,46 @@ int uavrl_env_get_subgoals(uavrl_env *env, double *sub_host)
     for (int e = 0; e < d.n; ++e)
         UAVRL_CUDA(cudaMemcpy(sub_host + (size_t)e * row, d.pool_sub + (size_t)scen[(size_t)e] * row, row * 8, cudaMemcpyDeviceToHost));
     return 0;
+}
+
+int uavrl_env_set_records(uavrl_env *env, int64_t capacity)
+{
+    if (!env) return fail(UAVRL_ERR_INVALID, "null env");
+    if (capacity < 0) return fail(UAVRL_ERR_INVALID, "uavrl_env_set_records: capacity must be >= 0");
+    UAVRL_CUDA(cudaSetDevice(env->cfg.device));
+    EnvRecords r;                                                // built beside the old records, swapped in once complete
+    if (capacity > 0)
+        if (int rc = records_alloc(r, env->d.n, capacity)) return rc;
+    UAVRL_CUDA(cudaDeviceSynchronize());                         // nothing may still write the records being replaced
+    env->records = std::move(r);
+    env->d.extras = capacity > 0 ? (env->d.extras | kExtraRecord) : (env->d.extras & ~kExtraRecord);
+    return 0;
+}
+
+int uavrl_env_get_records(uavrl_env *env, int64_t capacity, uavrl_episode_record *records_host, int64_t *n_written_out,
+                          int64_t *n_dropped_out, int32_t clear)
+{
+    if (!env || capacity < 0 || (capacity > 0 && !records_host)) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (!env->records.on) return fail(UAVRL_ERR_STATE, "episode records are not enabled (uavrl_env_set_records)");
+    UAVRL_CUDA(cudaSetDevice(env->cfg.device));
+    UAVRL_CUDA(cudaDeviceSynchronize());
+    const EnvRecDev &r = env->records.dev;
+    const int64_t m = capacity < r.cap ? capacity : r.cap;
+    if (m > 0) UAVRL_CUDA(cudaMemcpy(records_host, r.rec, (size_t)m * sizeof(uavrl_episode_record), cudaMemcpyDeviceToHost));
+    unsigned long long c[2];
+    UAVRL_CUDA(cudaMemcpy(c, r.counts, sizeof(c), cudaMemcpyDeviceToHost));
+    if (n_written_out) *n_written_out = (int64_t)c[0];
+    if (n_dropped_out) *n_dropped_out = (int64_t)c[1];
+    if (clear) {
+        if (int rc = records_clear(env->records, env->d.n, nullptr)) return rc;
+        UAVRL_CUDA(cudaDeviceSynchronize());
+    }
+    return 0;
+}
+
+int uavrl_env_clear_records(uavrl_env *env)
+{
+    return uavrl_env_get_records(env, 0, nullptr, nullptr, nullptr, 1);
 }
 
 int uavrl_env_threaten_rate(uavrl_env *env, int32_t n, const double *pts_host, uint8_t *out_host)

@@ -45,7 +45,25 @@ struct EnvDev {
     int32_t track_n, track_cap;
     long long *trace;                   // debug (UAVRL_ENV_TRACE): CTA 0 / thread 0 stage timestamps
 };
-constexpr int kExtraEnergy = 1, kExtraApf = 2, kExtraTrack = 4;
+constexpr int kExtraEnergy = 1, kExtraApf = 2, kExtraTrack = 4, kExtraRecord = 8;
+
+// Episode records (uavrl_env_set_records): the device view the EXTRAS step takes as its own kernel argument, so EnvDev and the
+// default step keep their layout.  Episode j of env e goes to slot j n + e; a slot at or beyond cap is counted as dropped.
+// limit: suite positions of an evaluation (uavrl_eval_run): an env whose next position ord n + e is >= limit is parked -- the
+// step leaves it alone; outside an evaluation limit is INT64_MAX and nothing parks.
+struct EnvRecDev {
+    uavrl_episode_record *rec;          // [cap]; outcome 0 marks a slot not written
+    int64_t cap, limit;
+    int32_t *ord, *steps, *coll;        // [n]: finished episodes since enable / clear; step calls and collisions of the episode
+    unsigned long long *counts;         // [0] records written, [1] dropped
+};
+
+// The records' owner: device memory and view; on = false leaves the step's extras as they are.
+struct EnvRecords {
+    DevMem mem;
+    EnvRecDev dev = { nullptr, 0, INT64_MAX, nullptr, nullptr, nullptr, nullptr };
+    bool on = false;
+};
 
 }  // namespace uavrl
 
@@ -63,13 +81,19 @@ struct uavrl_env {
     cudaStream_t own_stream = nullptr;
     bool extras_set = false;
     std::vector<double> base_z;          // building base heights (position.z), used by the APF distance only
+    uavrl::EnvRecords records;           // uavrl_env_set_records; swapped out for its own by an evaluation (eval.cu)
 };
 
 namespace uavrl {
-// launched by env.cu and by the fused training loop (train.cu)
-int launch_env_step(const EnvDev &d, int action_kind, const void *actions, float *obs, float *reward,
+// launched by env.cu, the fused training loops (train.cu) and the evaluation loop (eval.cu)
+int launch_env_step(const uavrl_env *env, int action_kind, const void *actions, float *obs, float *reward,
                     uint8_t *done, uint8_t *info, uint8_t *coll, uint8_t *ended, cudaStream_t st, bool pdl = false);
-int launch_env_observe(const EnvDev &d, float *obs, cudaStream_t st);
+int launch_env_observe(const uavrl_env *env, float *obs, cudaStream_t st);
+// env_reset_kernel over envs [0, n_reset) only (uavrl_env_reset: every env; an evaluation: the envs that have a suite position)
+int launch_env_reset(uavrl_env *env, int first, int n_reset, cudaStream_t st);
+// records (env.cu): allocate cap slots over the env's n rows (zeroed, stream-ordered on the env's device), and zero them again
+int records_alloc(EnvRecords &r, int n, int64_t cap);
+int records_clear(EnvRecords &r, int n, cudaStream_t st);
 // the env counters around a training loop (uavrl_train_run, uavrl_sac_train_run): begin() reads them, end() fills `out` with
 // what the loop added, all but last_loss, which each loop takes from its own losses.  Both synchronise `st`; nothing happens
 // when out is null.

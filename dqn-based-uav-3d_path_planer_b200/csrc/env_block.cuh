@@ -107,13 +107,39 @@ struct ApfDev {
     __device__ __forceinline__ P3 force(double x, double y, double z) const { return apf_force(ob, n, x, y, z); }
 };
 
+// The episode record of env e, whose episode just ended in state s on scenario scen (uavrl_env_set_records): slot j n + e for
+// its j-th finished episode, or a drop when that slot is beyond the capacity.  start2goal and planner_len are Eu_Loc_distance
+// and calculate_path_len (BaseClass/CalMod.py:133-139) in the reference's order, on the pool's copy of the scenario.
+__device__ __forceinline__ void write_record(const EnvDev &d, const EnvRecDev &rec, int e, int scen, const EnvRegs &s, int outcome,
+                                             int steps, int coll)
+{
+    const int j = rec.ord[e];
+    const long long slot = (long long)j * d.n + e;
+    if (slot >= rec.cap) { atomicAdd(&rec.counts[1], 1ull); return; }
+    const double *st = d.pool_start + (size_t)scen * 3, *gl = d.pool_goal + (size_t)scen * 3;
+    const double *q = d.pool_sub + (size_t)scen * d.K * 3;
+    double plen = 0.0;
+    for (int i = 1; i < s.n_sub; ++i) plen = dadd(plen, dist3(q[3 * i - 3], q[3 * i - 2], q[3 * i - 1], q[3 * i], q[3 * i + 1], q[3 * i + 2]));
+    uavrl_episode_record &r = rec.rec[slot];
+    r.scenario = scen; r.env = e; r.ordinal = j; r.outcome = outcome;
+    r.steps = steps; r.subgoals = s.cursor; r.collisions = coll; r.reserved = 0;
+    r.total_score = s.total; r.path_len = s.path_len;
+    r.start2goal = dist3(st[0], st[1], st[2], gl[0], gl[1], gl[2]);
+    r.planner_len = plen;
+    r.final_dist = dist3(s.px, s.py, s.pz, s.gx, s.gy, s.gz);
+    r.energy = (d.extras & kExtraEnergy) ? d.energy[e] : 0.0;
+    atomicAdd(&rec.counts[0], 1ull);
+}
+
 // EXTRAS: the optional models of uavrl_env_set_extras (energy accumulator, APF with per-env sub-goal queues, trajectory
-// recording); the default instantiation (false) is the hot path and carries none of it.
+// recording) and the episode records of uavrl_env_set_records (rec); the default instantiation (false) is the hot path and
+// carries none of it.
 template <bool DO_STEP, int EPB, int NT, bool USE_PDL, int LPW, bool EXTRAS = false>
 __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int e0, int tid, int action_kind,
                                           const void *__restrict__ actions, float *__restrict__ obs, float *__restrict__ reward,
                                           uint8_t *__restrict__ done_out, uint8_t *__restrict__ info_out,
-                                          uint8_t *__restrict__ coll_out, uint8_t *__restrict__ ended_out)
+                                          uint8_t *__restrict__ coll_out, uint8_t *__restrict__ ended_out,
+                                          const EnvRecDev *rec = nullptr)
 {
 #define ENV_TRACE(slot) do { if (d.trace && blockIdx.x == 0 && tid == 0) d.trace[slot] = clock64(); } while (0)
     ENV_TRACE(0);
@@ -139,6 +165,9 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
     StepOut o;                                               // phase 1's outputs, written back behind the phase-1 barrier
     o.reward = 0.0; o.done_ret = 0; o.info = 0; o.coll = 0;
     uint8_t ended_flag = 0;
+    // EXTRAS with records: parked = this env has no suite position left and is not stepped; park_after = its episode ended
+    // and it has none for the next one, so it keeps the finished episode's state instead of an auto-reset
+    bool parked = false, park_after = false;
     int scen = 0;
     P3 sgc[3];                                               // sub-goal queue entries cursor, cursor + 1, cursor + 2 (prefetched)
     s.px = 0.0; s.py = 0.0;
@@ -159,6 +188,7 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
             if (i < s.n_sub && i < d.K) { sgc[j].x = q[3 * i]; sgc[j].y = q[3 * i + 1]; sgc[j].z = q[3 * i + 2]; }
             else { sgc[j].x = 0.0; sgc[j].y = 0.0; sgc[j].z = 0.0; }
         }
+        if (EXTRAS && DO_STEP && (d.extras & kExtraRecord)) parked = (long long)rec->ord[e] * d.n + e >= rec->limit;
     }
     const int cur0 = s.cursor;
     for (int i = tid; i < d.k.n_cyl * 6; i += NT)
@@ -175,7 +205,7 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
         mask = cull_mask_coop<LPW>(d, s_cyl, s.px, s.py, ln);
         ENV_TRACE(2);
         if (valid) {
-            if (DO_STEP) {
+            if (DO_STEP && !(EXTRAS && parked)) {
                 if (USE_PDL) { pdl_wait(); pdl_trigger(); }
                 double act;
                 if (action_kind == UAVRL_ACT_CONT_F32) act = (double)static_cast<const float *>(actions)[e];
@@ -222,13 +252,24 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
                         d.path_n[cur * d.track_n + e] = np + 1;
                         if (s.done) { d.path_cur[e] = cur ^ 1; d.path_n[(cur ^ 1) * d.track_n + e] = 0; }     // UAV.reset: path = []
                     }
-                    if (sm_flags) sm_flags[le] = (uint8_t)((d.auto_reset && s.done) ? 2 : 1);   // 2: reload the queue, 1: shift it
+                    if (d.extras & kExtraRecord) {                  // the episode's record, before the auto-reset below
+                        const int steps = rec->steps[e] + 1, coll = rec->coll[e] + o.coll;
+                        if (s.done) {
+                            write_record(d, *rec, e, scen, s, o.info, steps, coll);
+                            const int j = rec->ord[e] + 1;
+                            rec->ord[e] = j; rec->steps[e] = 0; rec->coll[e] = 0;
+                            park_after = (long long)j * d.n + e >= rec->limit;
+                        } else {
+                            rec->steps[e] = steps; rec->coll[e] = coll;
+                        }
+                    }
+                    if (sm_flags) sm_flags[le] = (uint8_t)((d.auto_reset && s.done && !(EXTRAS && park_after)) ? 2 : 1);   // 2: reload the queue, 1: shift it
                 }
                 rew = o.reward;
                 n_stepped = 1; n_coll = o.coll; n_ended = s.done;
                 n_succ = (o.info == 1); n_lose = (o.info == 2);
                 ended_flag = (uint8_t)s.done;
-                if (d.auto_reset && s.done) {                      // UAV.reset() at the episode boundary
+                if (d.auto_reset && s.done && !(EXTRAS && park_after)) {       // UAV.reset() at the episode boundary
                     scen = (int)(((long long)scen + d.reset_stride) % d.P);
                     if (EXTRAS && (d.extras & kExtraEnergy)) d.energy[e] = 0.0;
                     load_scenario(d, scen, s);
@@ -243,11 +284,11 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
                 const bool apf_on = EXTRAS && (d.extras & kExtraApf);
                 // APF: an env that did not restart reads its own queue, whose entries phase 1b shifts right after this
                 // (same function, so the on-the-fly shift below equals what will be stored); a restarted env reads the pool
-                const bool own_q = apf_on && !(DO_STEP && d.auto_reset && n_ended);
+                const bool own_q = apf_on && !(DO_STEP && d.auto_reset && n_ended && !(EXTRAS && park_after));
                 const double *q = own_q ? d.sub_env + (size_t)e * d.K * 3 : d.pool_sub + (size_t)scen * d.K * 3;
                 const bool shift = own_q && DO_STEP;
                 const ApfObs *aob = d.apf_obs; const int an = d.k.n_cyl;
-                const bool same_q = !(DO_STEP && d.auto_reset && n_ended);       // still the queue the prefetch read
+                const bool same_q = !(DO_STEP && d.auto_reset && n_ended && !(EXTRAS && park_after));   // still the queue the prefetch read
                 auto sub = [q, shift, aob, an, same_q, cur0, &sgc](int i) {
                     P3 p;
                     const int j = i - cur0;
@@ -281,7 +322,7 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
     ENV_TRACE(8);
     // write-back of the stepped state and the step's outputs: behind the barrier, i.e. while the other warps already probe
     // (these ~25 stores per env used to sit between the step and the barrier every warp of the CTA waits at)
-    if (DO_STEP && valid) {
+    if (DO_STEP && valid && !(EXTRAS && parked)) {
         if (reward) reward[e] = (float)o.reward;
         d.rew64[e] = o.reward;
         if (done_out) done_out[e] = (uint8_t)o.done_ret;

@@ -471,7 +471,9 @@ __global__ void sac_stat_sums_kernel(const float *__restrict__ stat, int nparts,
 }
 
 // get_action (:444-448): action = actor(state)[0] with fresh noise.  Trainer blockIdx.y acts for rows [g n, (g + 1) n).
-template <bool GR>
+// MEAN: the policy's mean action instead, tanh(mu) bound -- PolicyNetContinuous_SAC.forward with zero noise (the evaluation's
+// deterministic policy, uavrl_sac_eval_run / uavrl_sac_act_mean); no noise is drawn.
+template <bool GR, bool MEAN = false>
 __global__ void __launch_bounds__(kNetThreads) sac_act_kernel(SacArgs a, const float *__restrict__ obs, int n, float *__restrict__ actions)
 {
     extern __shared__ __align__(16) float smem[];
@@ -496,7 +498,9 @@ __global__ void __launch_bounds__(kNetThreads) sac_act_kernel(SacArgs a, const f
         actor_forward_tile(an, RA, head);
         if (threadIdx.x < kTile) {
             const int b = threadIdx.x, gb = t * kTile + b;
-            if (gb < n) {
+            if (MEAN && gb < n) {
+                for (int j = 0; j < kSacA; ++j) actions[(size_t)gb * kSacA + j] = tanhf(tanhf(head[b * 32 + j])) * a.h.bound;
+            } else if (gb < n) {
                 float e[2];
                 noise2(eps, key, a.ctr, gb, e[0], e[1]);
                 for (int j = 0; j < kSacA; ++j) actions[(size_t)gb * kSacA + j] = actor_point(head[b * 32 + j], head[b * 32 + kSacA + j], e[j]).a * a.h.bound;
@@ -608,18 +612,33 @@ static int sac_scratch(uavrl_sac *s, int B, int grid, cudaStream_t st)
     return grow(s->td_mem, s->td_cap, B, st, true, buf(s->td, G * B * kSacA));
 }
 
-int uavrl::launch_sac_act(uavrl_sac *s, const float *obs, int n, const float *eps, float *actions, cudaStream_t st)
+// the act kernel of every trainer on n rows (G equal blocks) with noise counter ctr, or the mean action
+static int sac_act_launch(uavrl_sac *s, const float *obs, int n, const float *eps, uint64_t ctr, bool mean, float *actions,
+                          cudaStream_t st)
 {
     SacArgs a;
     BatchSrc none;
     memset(&none, 0, sizeof(none));
     const int ng = n / s->G;                                   // rows per trainer: block g belongs to trainer g
-    sac_fill_args(s, a, none, ng, ng, eps, 0x8000000000000000ull | s->calls++);
+    sac_fill_args(s, a, none, ng, ng, eps, ctr);
     const int grid = a.n_tiles < s->max_ctas ? a.n_tiles : s->max_ctas;
-    if (s->G > 1) sac_act_kernel<true><<<dim3(grid, s->G), kNetThreads, smem_act(s->sh), st>>>(a, obs, ng, actions);
-    else sac_act_kernel<false><<<grid, kNetThreads, smem_act(s->sh), st>>>(a, obs, ng, actions);
+    const size_t sm = smem_act(s->sh);
+    if (mean && s->G > 1) sac_act_kernel<true, true><<<dim3(grid, s->G), kNetThreads, sm, st>>>(a, obs, ng, actions);
+    else if (mean) sac_act_kernel<false, true><<<grid, kNetThreads, sm, st>>>(a, obs, ng, actions);
+    else if (s->G > 1) sac_act_kernel<true><<<dim3(grid, s->G), kNetThreads, sm, st>>>(a, obs, ng, actions);
+    else sac_act_kernel<false><<<grid, kNetThreads, sm, st>>>(a, obs, ng, actions);
     UAVRL_LAUNCHED();
     return 0;
+}
+
+int uavrl::launch_sac_act(uavrl_sac *s, const float *obs, int n, const float *eps, float *actions, cudaStream_t st)
+{
+    return sac_act_launch(s, obs, n, eps, 0x8000000000000000ull | s->calls++, false, actions, st);
+}
+
+int uavrl::launch_sac_act_eval(uavrl_sac *s, const float *obs, int n, bool mean, uint64_t ctr, float *actions, cudaStream_t st)
+{
+    return sac_act_launch(s, obs, n, nullptr, ctr, mean, actions, st);
 }
 
 static int sac_grid(const uavrl_sac *s, int B)
@@ -782,9 +801,9 @@ static int sac_alloc(uavrl_sac *s)
     UAVRL_CUDA(cudaMemcpy(s->scal, init.data(), init.size() * 4, cudaMemcpyHostToDevice));
     if (cfg->lockstep_envs > 0 && (rc = s->replay.alloc(cfg->replay_capacity, cfg->lockstep_envs, s->G, cfg->obs_dim, true))) return rc;
     if ((rc = raise_dyn_smem(sac_target_kernel<false>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<false, false>, smem_critic(s->sh))) ||
-        (rc = raise_dyn_smem(sac_actor_kernel<false>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<false>, smem_act(s->sh))) ||
+        (rc = raise_dyn_smem(sac_actor_kernel<false>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<false>, smem_act(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<false, true>, smem_act(s->sh))) ||
         (rc = raise_dyn_smem(sac_target_kernel<true>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true, false>, smem_critic(s->sh))) ||
-        (rc = raise_dyn_smem(sac_actor_kernel<true>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<true>, smem_act(s->sh))) ||
+        (rc = raise_dyn_smem(sac_actor_kernel<true>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<true>, smem_act(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<true, true>, smem_act(s->sh))) ||
         (rc = raise_dyn_smem(sac_critic_kernel<false, true>, smem_critic(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true, true>, smem_critic(s->sh))))
         return rc;
     return 0;
@@ -938,6 +957,14 @@ int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *ep
     if (n % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_act: n must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     return launch_sac_act(s, obs_dev, n, eps_dev, actions_dev, (cudaStream_t)stream);
+}
+
+int uavrl_sac_act_mean(uavrl_sac *s, const float *obs_dev, int32_t n, float *actions_dev, void *stream)
+{
+    if (!s || !obs_dev || !actions_dev || n <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (n % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_act_mean: n must be a multiple of the trainer count");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    return launch_sac_act_eval(s, obs_dev, n, true, 0, actions_dev, (cudaStream_t)stream);
 }
 
 static BatchSrc sac_explicit_src(const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev, const float *d_dev)

@@ -45,6 +45,9 @@ namespace uavrl {
 // SAC_Trainer.get_action of every trainer: n rows in G equal blocks (block g -> trainer g), actions [n][2]; eps (may be null)
 // [n][2] injects the reparameterisation noise, else Philox on the learner's act-call counter
 int launch_sac_act(uavrl_sac *s, const float *obs, int n, const float *eps, float *actions, cudaStream_t st);
+// the same pass for an evaluation (eval.cu): noise from counter ctr without advancing the act-call counter, or with mean the
+// policy's mean action tanh(mu) bound
+int launch_sac_act_eval(uavrl_sac *s, const float *obs, int n, bool mean, uint64_t ctr, float *actions, cudaStream_t st);
 // one SAC_Trainer.update of every trainer on the batch described by src (B rows per trainer); losses_dev (may be null: the
 // learner's own out) receives [G][4]
 int launch_sac_update(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev,

@@ -38,7 +38,7 @@ static int act(uavrl_sac *s, const ReplayStore::Iteration &io, int n, float, cud
 // The Q-network's step joins the learner's dependent-launch chain.
 static int env_step(uavrl_env *env, uavrl_learner *l, const ReplayStore::Iteration &io, cudaStream_t st)
 {
-    if (int rc = launch_env_step(env->d, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
+    if (int rc = launch_env_step(env, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st,
                                  l->chain.next(kChainEnv).pdl))
         return rc;
     l->chain.launched(kChainEnv);
@@ -46,7 +46,7 @@ static int env_step(uavrl_env *env, uavrl_learner *l, const ReplayStore::Iterati
 }
 static int env_step(uavrl_env *env, uavrl_sac *, const ReplayStore::Iteration &io, cudaStream_t st)
 {
-    return launch_env_step(env->d, UAVRL_ACT_CONT_F32X2, io.act2, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st);
+    return launch_env_step(env, UAVRL_ACT_CONT_F32X2, io.act2, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st);
 }
 
 // the commit's prioritised-replay priority fill launches outside the Q-network's dependent-launch chain
@@ -109,7 +109,7 @@ static int iteration(uavrl_env *env, Learner *l, float eps, int n_updates, int d
     ReplayStore &rs = l->replay;
     const ReplayStore::Iteration io = rs.begin();
     if (!rs.frame0_valid) {
-        if ((rc = launch_env_observe(env->d, io.obs_t, st))) return rc;
+        if ((rc = launch_env_observe(env, io.obs_t, st))) return rc;
         rs.frame0_valid = true;
     }
     if (ev) UAVRL_CUDA(cudaEventRecord(ev[0], st));

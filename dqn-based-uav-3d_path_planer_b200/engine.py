@@ -217,11 +217,46 @@ class EnvBatch:
         check(_lib.lib().uavrl_env_get_subgoals(self.h, _ptr(out)))
         return out
 
+    # -- episode records (include/uavrl.h, uavrl_env_set_records): one per finished episode, written by the step
+    def set_records(self, capacity):
+        """capacity > 0: record every finished episode (episode j of env e in slot j n + e; slots >= capacity are dropped);
+        0: off.  Enabling again empties them."""
+        check(_lib.lib().uavrl_env_set_records(self.h, int(capacity)))
+        self._rec_cap = int(capacity)
+
+    def records(self, clear=True):
+        """The written records in slot order as a dict of numpy columns (RECORD_FIELDS, plus 'slot'), with n_dropped; clear
+        empties them and restarts the ordinals."""
+        cap = getattr(self, "_rec_cap", 0)
+        buf = (_lib.EpisodeRecord * max(cap, 1))()
+        w, d = C.c_int64(), C.c_int64()
+        check(_lib.lib().uavrl_env_get_records(self.h, cap, buf, C.byref(w), C.byref(d), int(bool(clear))))
+        out = records_columns(buf, cap)
+        out["n_dropped"] = int(d.value)
+        return out
+
+    def clear_records(self):
+        check(_lib.lib().uavrl_env_clear_records(self.h))
+
     def threaten_rate(self, pts):
         pts = np.ascontiguousarray(pts, np.float64).reshape(-1, 3)
         out = np.zeros(pts.shape[0], np.uint8)
         check(_lib.lib().uavrl_env_threaten_rate(self.h, pts.shape[0], _ptr(pts), _ptr(out)))
         return out
+
+
+RECORD_FIELDS = ("scenario", "env", "ordinal", "outcome", "steps", "subgoals", "collisions", "total_score", "path_len",
+                 "start2goal", "planner_len", "final_dist", "energy")
+
+
+def records_columns(buf, n, written_only=True):
+    """numpy columns of the first n uavrl_episode_record entries of a ctypes array; 'slot' is each entry's index.
+    written_only keeps the entries the step wrote (outcome != 0)."""
+    arr = np.ctypeslib.as_array(buf)[:n] if n > 0 else np.zeros(0, dtype=np.ctypeslib.as_array(buf).dtype)
+    keep = arr["outcome"] != 0 if written_only else np.ones(len(arr), bool)
+    out = {k: np.array(arr[k][keep]) for k in RECORD_FIELDS}
+    out["slot"] = np.nonzero(keep)[0].astype(np.int64)
+    return out
 
 
 NET_KINDS = {                       # BaseClass/BaseCNN.py class name -> (hidden widths as f(h), dueling)
@@ -770,10 +805,19 @@ class SacLearner(_PerCalls):
     def set_scalars(self, log_alpha, la_m=0.0, la_v=0.0, epoch=0, adam_step=0):
         check(_lib.lib().uavrl_sac_set_scalars(self.h, float(log_alpha), float(la_m), float(la_v), int(epoch), int(adam_step)))
 
-    def act(self, obs, eps=None):
+    def act(self, obs, eps=None, mean=False):
+        """SAC_Trainer.get_action on n rows; mean=True: the mean action tanh(mu) bound instead (act_mean)."""
+        if mean:
+            return self.act_mean(obs)
         n = obs.shape[0]
         a = torch.empty((n, self.cfg.act_dim), dtype=torch.float32, device=self.device)
         check(_lib.lib().uavrl_sac_act(self.h, _ptr(obs), n, _ptr(eps), _ptr(a), _stream(self.device)))
+        return a
+
+    def act_mean(self, obs):
+        """The policy's mean action tanh(mu) bound (include/uavrl.h uavrl_sac_act_mean): no noise, no act-call counted."""
+        a = torch.empty((obs.shape[0], self.cfg.act_dim), dtype=torch.float32, device=self.device)
+        check(_lib.lib().uavrl_sac_act_mean(self.h, _ptr(obs), obs.shape[0], _ptr(a), _stream(self.device)))
         return a
 
     def update_batch(self, s, a, r, s2, d, eps_next=None, eps_cur=None, losses=None):
@@ -902,3 +946,34 @@ def sac_train_run_dp(env, sac, n_iters, global_batch):
     """uavrl_sac_train_run_dp: lockstep iterations whose update is the fused data-parallel SAC update (after connect_peers
     or connect_self; warm the ring up with sac_train_run first)."""
     check(_lib.lib().uavrl_sac_train_run_dp(env.h, sac.h, int(n_iters), int(global_batch), _stream(env.device)))
+
+
+def _eval_result(env, learner, n_episodes, buf, st):
+    """records in suite order (all n_episodes positions, unfinished ones with outcome 0), the trainer of each row and the stats"""
+    out = records_columns(buf, n_episodes, written_only=False)
+    del out["slot"]
+    out["trainer"] = out["env"] // (env.n // learner.G)
+    out["trainer"][out["outcome"] == 0] = -1
+    return dict(records=out, iterations=int(st.iterations), n_records=int(st.records), unfinished=int(st.unfinished))
+
+
+def eval_run(env, learner, n_episodes, first_scenario=0, max_iters=0):
+    """uavrl_eval_run: greedy episodes of a Q-network learner over pool scenarios first_scenario + k (mod P), k < n_episodes,
+    one record each.  Returns dict(records = numpy columns in suite order plus 'trainer' (-1: unfinished), iterations,
+    n_records, unfinished).  Nothing of the learner changes; the env ends in the evaluation's final state."""
+    n = int(n_episodes)
+    buf = (_lib.EpisodeRecord * max(n, 1))()
+    st = _lib.EvalStats()
+    check(_lib.lib().uavrl_eval_run(env.h, learner.h, int(first_scenario), n, int(max_iters), buf, C.byref(st), _stream(env.device)))
+    return _eval_result(env, learner, n, buf, st)
+
+
+def sac_eval_run(env, sac, n_episodes, first_scenario=0, max_iters=0, mean_action=False):
+    """uavrl_sac_eval_run: eval_run for a SAC learner; sampled actions on the evaluation's own noise stream, or with
+    mean_action the mean action tanh(mu) bound."""
+    n = int(n_episodes)
+    buf = (_lib.EpisodeRecord * max(n, 1))()
+    st = _lib.EvalStats()
+    check(_lib.lib().uavrl_sac_eval_run(env.h, sac.h, int(first_scenario), n, int(bool(mean_action)), int(max_iters), buf, C.byref(st),
+                                        _stream(env.device)))
+    return _eval_result(env, sac, n, buf, st)

@@ -10,6 +10,9 @@ Constructor takes the same parsed-XML dict the reference's EnvFactory passes
 (config/PathPlan_City.xml <env> ... </env>): len/width/h, num_UAV, Agent.xml_path_agent,
 Agent.Trainer.Trainer_path, Obstacles.buildings.  simulator.py drives it unchanged:
 env.run_eposide(eps) -> result dict; env.Agents[i].Train_time / Testing_time; env.Trainer.hard_update().
+env.run_evaluation(n) plays n held-out scenarios with the trained policy on an env of its own (<eval_seed>, <eval_episodes>,
+<eval_envs>, <eval_mean_action>) and returns its summary; <record_episodes>1</record_episodes> adds generate_train_result's
+per-episode fields to run_eposide's result.
 """
 import importlib
 import math
@@ -104,6 +107,40 @@ def buildings_from_dict(bdict: dict):
                       float(None2Value(t.get("_R"), 10)), float(None2Value(t.get("_H"), 20))] for t in th], np.float64)
 
 
+def eval_summary(rec, num_trainers=1):
+    """The summary run_evaluation returns, from evaluation records in suite order (engine.eval_run's 'records'): counts and
+    rates over the finished episodes, means of their steps / path_len / total_score / start2goal / energy, the mean
+    path_len / planner_len over successful episodes with a planner path, and with num_trainers > 1 each trainer's success
+    rate."""
+    done = rec["outcome"] != 0
+    succ = rec["outcome"] == 1
+    n = int(done.sum())
+
+    def mean(x, m):
+        return float(np.mean(x[m])) if m.any() else 0.0
+    ratio_m = succ & (rec["planner_len"] > 0)
+    out = dict(episodes=n, success=int(succ.sum()), lose=int((rec["outcome"] == 2).sum()), success_rate=float(succ.sum()) / max(n, 1),
+               collisions=int(rec["collisions"][done].sum()), steps=mean(rec["steps"], done), path_len=mean(rec["path_len"], done),
+               total_score=mean(rec["total_score"], done), start2goal=mean(rec["start2goal"], done),
+               path_ratio=mean(rec["path_len"] / np.where(ratio_m, rec["planner_len"], 1.0), ratio_m), energy=mean(rec["energy"], done))
+    if num_trainers > 1:
+        out["success_rate_per_trainer"] = [float(succ[rec["trainer"] == g].sum()) / max(int(done[rec["trainer"] == g].sum()), 1)
+                                           for g in range(num_trainers)]
+    return out
+
+
+def write_eval_csv(rec, path):
+    """One row per finished episode: its suite position, then every record field and the trainer."""
+    import csv
+    cols = list(engine.RECORD_FIELDS) + ["trainer"]
+    os.makedirs(os.path.dirname(path) or ".", exist_ok=True)
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(["position"] + cols)
+        for k in np.nonzero(rec["outcome"] != 0)[0]:
+            w.writerow([int(k)] + [rec[c][k].item() for c in cols])
+
+
 class PathPlan_City_B200:
     def __init__(self, param: dict) -> None:
         # BaseEnv.__init__ (BaseClass/BaseEnv.py:19-21,34)
@@ -167,6 +204,7 @@ class PathPlan_City_B200:
         if fp is not None:
             power = {k: float(fp[k]) for k in ("P_i", "v_0", "d_0", "rho", "s", "A", "P_b", "F_b")}
             power["xi"] = 0.8                                      # UAV.py:58 with j = 0 (one shared parameter set)
+        self._power = power
         if power is not None or self.record_csv:
             self.batch.set_extras(power=power, track_envs=(1 if self.record_csv else 0),
                                   track_capacity=(64 * self.uav_params.max_step if self.record_csv else 0))
@@ -219,6 +257,21 @@ class PathPlan_City_B200:
                                  "trainers do not have: set Is_AC = 0")
             if self.shard_over_ranks:
                 self.Trainer._learner.fed_shard(self.rank, self.world)
+        # evaluation (run_evaluation): a held-out pool drawn from eval_seed, eval_episodes suite episodes on eval_envs envs of
+        # an env of its own; record_episodes = 1: run_eposide adds generate_train_result's per-episode fields
+        seed = int(None2Value(param.get("seed"), 42))
+        self.eval_seed = int(None2Value(param.get("eval_seed"), seed + 1))
+        self.eval_episodes = int(None2Value(param.get("eval_episodes"), self.num_UAV))
+        self.eval_envs = int(None2Value(param.get("eval_envs"), self.num_UAV))
+        self.eval_mean_action = int(None2Value(param.get("eval_mean_action"), 0))
+        self.record_episodes = int(None2Value(param.get("record_episodes"), 0))
+        self._chunk = 16                                           # lockstep iterations per run_eposide chunk
+        if self.eval_envs < 1 or self.eval_envs % self.num_trainers:
+            raise ValueError("eval_envs (%d) must be a positive multiple of num_trainers (%d)" % (self.eval_envs, self.num_trainers))
+        self._eval_batch = None
+        if self.record_episodes:
+            # a chunk ends at most `chunk` episodes per UAV, and run_eposide drains the records after every chunk: nothing drops
+            self.batch.set_records(self._chunk * self.n_local)
         self.executed_time = 0
         self.Scene_Random_Reset()
 
@@ -308,7 +361,8 @@ class PathPlan_City_B200:
         t0 = time.time()
         save_loop = int(getattr(self.Trainer, "save_loop", 0) or 0)
         ended = steps = updates = coll = n_s = n_l = 0
-        reward_sum, loss, chunk, iters = 0.0, 0.0, 16, 0
+        reward_sum, loss, chunk, iters = 0.0, 0.0, self._chunk, 0
+        recs = []
         max_iters = 64 * self.uav_params.max_step
         while ended < self.num_UAV and iters < max_iters:
             e_before = self.Trainer.epoch
@@ -332,6 +386,8 @@ class PathPlan_City_B200:
                 c = t.tolist()
                 c[:5] = [int(x) for x in c[:5]]
                 c[6] /= self.world                                 # the mean of the ranks' mean trainer losses
+            if self.record_episodes:
+                recs.append(self.batch.records(clear=True))
             ended += c[0]; steps += c[1]; updates += st.updates; coll += c[2]
             n_s += c[3]; n_l += c[4]; reward_sum += c[5]; loss = c[6]
             iters += chunk
@@ -343,6 +399,13 @@ class PathPlan_City_B200:
         self.result.update(success=n_s, lose=n_l, normal=steps - n_s - n_l, loss=float(loss),
                            sum_epoch=self.Trainer.epoch, score=reward_sum, average_score=reward_sum / self.num_UAV,
                            step=iters, env_steps=steps, updates=updates, collisions=coll, episodes=ended)
+        if self.record_episodes:
+            # generate_train_result (PathPlan_City.py:479-506): path_len, start2goal, len_Astar (the planner's polyline) and
+            # ReachGoal, here the means over the episodes that ended in this call
+            cat = {k: np.concatenate([r[k] for r in recs]) for k in ("path_len", "start2goal", "planner_len", "outcome")}
+            m = (lambda x: float(np.mean(x)) if len(x) else 0.0)  # noqa: E731
+            self.result.update(path_len=m(cat["path_len"]), start2goal=m(cat["start2goal"]), len_Astar=m(cat["planner_len"]),
+                               ReachGoal=m(cat["outcome"] == 1))
         self.epoch += 1
         self.executed_time += dt
         if self.Is_FL and self.epoch % self.FL_Loop == 0:             # PathPlan_City.py:469-475
@@ -355,6 +418,45 @@ class PathPlan_City_B200:
             if self.print_loop > 0 and self.epoch % self.print_loop == 0:
                 ag.record_list()                                   # PathPlan_City.run_eposide :463-468 (every print_loop episodes)
         return self.result
+
+    # ---- policy evaluation: what the reference's Evaluation_Action / Sim stubs leave open
+    def _eval_env(self):
+        """The evaluation's own env, built once: the same city, UAV parameters and energy model, a pool from eval_seed."""
+        if self._eval_batch is None:
+            ev = engine.EnvBatch(self.city, self.uav_params, self.eval_envs, max_subgoals=64, device=self.device_index)
+            sc = ev.make_scenarios(self.eval_episodes, seed=self.eval_seed, rrt_step=self.sub_granularity)
+            ev.set_pool(sc["start"], sc["goal"], sc["heading"], sc["sub"], sc["n_sub"])
+            if self._power is not None:
+                ev.set_extras(power=self._power)
+            self._eval_batch = ev
+        return self._eval_batch
+
+    def run_evaluation(self, n_episodes=None, log_dir="logs"):
+        """The trained planner on n_episodes (default eval_episodes) held-out scenarios, each once, on the device: greedy for
+        the DQN family, SAC's sampled action (eval_mean_action = 1: its mean action).  Neither the training env nor the
+        trainer changes.  Returns eval_summary's dict plus the iterations run and the episodes left unfinished; writes one
+        CSV row per episode to <log_dir>/eval_<time>.csv (CWD-relative, like the reference's logs) and adds the wall time
+        to Agents[0].Testing_time."""
+        if self.shard_over_ranks:
+            raise ValueError("run_evaluation runs on one GPU: it is not available with shard_over_ranks = 1")
+        if self.host_driven:
+            raise ValueError("run_evaluation drives the device loop: it is not available with host_driven = 1")
+        n = self.eval_episodes if n_episodes is None else int(n_episodes)
+        if n > self.eval_episodes:
+            raise ValueError("n_episodes (%d) exceeds the evaluation pool (eval_episodes = %d)" % (n, self.eval_episodes))
+        t0 = time.time()
+        ev, learner = self._eval_env(), self.Trainer._learner
+        if isinstance(learner, engine.SacLearner):
+            res = engine.sac_eval_run(ev, learner, n, mean_action=bool(self.eval_mean_action))
+        else:
+            res = engine.eval_run(ev, learner, n)
+        out = eval_summary(res["records"], self.num_trainers)
+        out.update(iterations=res["iterations"], unfinished=res["unfinished"])
+        path = os.path.join(log_dir, "eval_%s_%06d.csv" % (time.strftime("%Y%m%d-%H%M%S"), int(time.time() % 1 * 1e6)))
+        write_eval_csv(res["records"], path)
+        out["csv"] = path
+        self.Agents[0].Testing_time += time.time() - t0
+        return out
 
     def Federated_Learning_choice(self):
         """PathPlan_City.py:644-684 on the device (engine.Learner.federate): every trainer averages itself with the half of

@@ -165,6 +165,38 @@ int uavrl_env_get_path(uavrl_env *env, int32_t e, int32_t which, int32_t capacit
 /* the per-UAV sub-goal queues [n_envs][K][3] (the scenario's queue, shifted by APF when enabled) */
 int uavrl_env_get_subgoals(uavrl_env *env, double *sub_host);
 
+/* Episode records: the per-episode statistics of the reference's UAV (Agents/UAV.py:147-153, 360-366, 443, 477, 503), which
+ * PathPlan_City.generate_train_result (Envs/PathPlan_City.py:479-506) reads for Train_info_line.  With records on, the step
+ * writes one record when an env's episode ends (UAV.done becomes true), before any auto-reset:
+ *   scenario, env, ordinal   pool index, env row, and the env's ordinal-th finished episode since records were enabled or cleared
+ *   outcome                  uavrl_info of the final step (1 success, 2 lose)
+ *   steps                    step calls of the episode, over all its sub-goal segments (UAV.Step restarts at each sub-goal)
+ *   subgoals                 sub-goals popped (the cursor's advance)
+ *   collisions               steps whose collision predicate held (UAV.py:425)
+ *   total_score, path_len    UAV.total_score and UAV.path_len at the end
+ *   start2goal               Eu_Loc_distance(start, goal) of the scenario (UAV.start2goal, UAV.py:365)
+ *   planner_len              calculate_path_len of the scenario's sub-goal queue, left to right (UAV.len_Astar, UAV.py:153,366:
+ *                            the RRT sub-goal polyline, despite the name -- RRT.getPath returns the same list twice)
+ *   final_dist               |p - goal| at the end
+ *   energy                   the episode's Calc_Fly_Power sum with the energy model on, else 0
+ * Episode j of env e goes to slot j n_envs + e; a record whose slot is at or beyond `capacity` is not written and counts as
+ * dropped.  Slots are deterministic, so identical runs return identical arrays.  Records ride on the optional-model step (as
+ * `track` does): with them off, the step is the default one.  They also work inside uavrl_train_run and uavrl_sac_train_run,
+ * whose training outputs they do not change.
+ * uavrl_env_set_records: capacity > 0 enables (or re-enables, emptied), capacity = 0 disables.  Synchronises the device.
+ * uavrl_env_get_records: copies the min(capacity, slots) first slots to records_host (outcome 0: a slot not written), the
+ * written and dropped counts, and with clear = 1 empties them (ordinals restart at 0).  uavrl_env_clear_records: the same
+ * emptying alone.  Both synchronise the device; without records enabled they are refused (UAVRL_ERR_STATE). */
+typedef struct {
+    int32_t scenario, env, ordinal, outcome;
+    int32_t steps, subgoals, collisions, reserved;
+    double total_score, path_len, start2goal, planner_len, final_dist, energy;
+} uavrl_episode_record;
+int uavrl_env_set_records(uavrl_env *env, int64_t capacity);
+int uavrl_env_get_records(uavrl_env *env, int64_t capacity, uavrl_episode_record *records_host, int64_t *n_written_out,
+                          int64_t *n_dropped_out, int32_t clear);
+int uavrl_env_clear_records(uavrl_env *env);
+
 /* PathPlan_City.Threaten_rate (Envs/PathPlan_City.py:215-223) on arbitrary points (device kernel):
  * pts_host [n][3] -> out_host [n] u8. */
 int uavrl_env_threaten_rate(uavrl_env *env, int32_t n, const double *pts_host, uint8_t *out_host);
@@ -610,6 +642,38 @@ int uavrl_per_get(uavrl_learner *l, double *leaves_host, double *total_out, doub
 int uavrl_learner_update_batch_per(uavrl_learner *l, int32_t batch, const float *obs_dev, const int32_t *act_dev,
                                    const float *rew_dev, const float *next_obs_dev, const float *done_dev,
                                    const float *is_weights_dev, float *abs_err_out_dev, float *loss_dev, void *stream);
+
+/* ---- policy evaluation (greedy episodes over a held-out scenario suite) --------------------------------------------
+ * The reference leaves its evaluation hooks as stubs (PathPlan_City.Evaluation_Action, Sim) and never advances
+ * UAV.Testing_time; it only counts successes while training, under exploration and with the replay filling.  These calls run
+ * a learner's policy on its own, one uavrl_episode_record per episode:
+ *   - the suite is pool scenarios first_scenario + k (mod P), k in [0, n_episodes); env e starts on position e and after its
+ *     j-th episode takes position (j + 1) n_envs + e; an env with no position left parks: it is not stepped again, writes no
+ *     record and adds to no statistic (envs e >= n_episodes are never reset or stepped).  The env's auto_reset, reset stride
+ *     and records are its own again afterwards; its state is the evaluation's final state;
+ *   - actions: uavrl_eval_run acts greedily (uavrl_learner_act with is_train = 0) and leaves the act-call counter as it was;
+ *     uavrl_sac_eval_run samples as SAC_Trainer.get_action does (Trainer/SAC_Trainer.py:444-448), with noise keyed by the
+ *     learner seed (trainer g: seed + g), first_scenario and the iteration, on counters no training draw uses -- or, with
+ *     mean_action = 1, takes tanh(mu) bound (uavrl_sac_act_mean).  Env block g acts with trainer g; n_envs must be a multiple
+ *     of the trainer count.  Nothing of the learner changes: parameters, moments, alpha, counters, ring and trees;
+ *   - the loop stops once every suite episode has its record, or after max_iters iterations (0: ceil(n / n_envs) K max_step,
+ *     which every suite episode ends within).  It reads the record count every 64 iterations, so iterations may run past
+ *     the last record (parked envs do nothing);
+ *   - records_host (may be NULL) receives [n_episodes] records in suite order (record k = position k; outcome 0: unfinished);
+ *     stats_host (may be NULL) the iterations run, the records written and the episodes left unfinished.
+ * Refused before anything is enqueued: n_episodes or max_iters < 0, learner input width != 100, env and learner on different
+ * devices, n_envs not a multiple of the trainer count, a Q-network without 27 actions or mean_action not 0 / 1
+ * (UAVRL_ERR_INVALID); no pool (UAVRL_ERR_STATE).  Synchronises `stream`. */
+typedef struct {
+    int64_t iterations, records, unfinished;
+} uavrl_eval_stats;
+int uavrl_eval_run(uavrl_env *env, uavrl_learner *l, int32_t first_scenario, int32_t n_episodes, int64_t max_iters,
+                   uavrl_episode_record *records_host, uavrl_eval_stats *stats_host, void *stream);
+int uavrl_sac_eval_run(uavrl_env *env, uavrl_sac *s, int32_t first_scenario, int32_t n_episodes, int32_t mean_action,
+                       int64_t max_iters, uavrl_episode_record *records_host, uavrl_eval_stats *stats_host, void *stream);
+/* The SAC policy's mean action tanh(mu) bound for n rows in G equal blocks (PolicyNetContinuous_SAC.forward without noise);
+ * draws nothing and leaves the act-call counter as it is. */
+int uavrl_sac_act_mean(uavrl_sac *s, const float *obs_dev, int32_t n, float *actions_dev, void *stream);
 
 const char *uavrl_last_error(void);
 const char *uavrl_version(void);
