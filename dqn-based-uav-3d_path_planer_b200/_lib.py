@@ -120,6 +120,8 @@ SIGNATURES = {
     "uavrl_env_get_state": (C.c_int, [VP, C.POINTER(EnvStateHost)]),
     "uavrl_env_set_state": (C.c_int, [VP, C.POINTER(EnvStateHost)]),
     "uavrl_env_threaten_rate": (C.c_int, [VP, C.c_int32, VP, VP]),
+    "uavrl_env_set_motion": (C.c_int, [VP, VP, VP]),
+    "uavrl_env_get_obstacles": (C.c_int, [VP, VP, VP, VP]),
     "uavrl_learner_create": (C.c_int, [C.POINTER(LearnerConfig), C.POINTER(VP)]),
     "uavrl_learner_create_trainers": (C.c_int, [C.POINTER(LearnerConfig), C.c_int32, C.POINTER(VP)]),
     "uavrl_learner_trainer_count": (C.c_int32, [VP]),

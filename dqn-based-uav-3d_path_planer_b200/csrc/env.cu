@@ -26,6 +26,7 @@
 
 #include <math.h>
 #include <string.h>
+#include <cmath>
 #include <vector>
 
 namespace uavrl {
@@ -53,11 +54,13 @@ template <bool DO_STEP, int EPB>
 __global__ void __launch_bounds__(kEnvThreads)
 env_extras_kernel(EnvDev d, int action_kind, const void *__restrict__ actions, float *__restrict__ obs,
                   float *__restrict__ reward, uint8_t *__restrict__ done_out, uint8_t *__restrict__ info_out,
-                  uint8_t *__restrict__ coll_out, uint8_t *__restrict__ ended_out, EnvRecDev rec)
+                  uint8_t *__restrict__ coll_out, uint8_t *__restrict__ ended_out, EnvRecDev rec, EnvMotionDev mot)
 {
     __shared__ EnvSmem<EPB> sm;
+    __shared__ MotionSmem msm;
     env_block<DO_STEP, EPB, kEnvThreads, true, (EPB < 32 ? EPB : 32), true>(d, sm, blockIdx.x * EPB, threadIdx.x, action_kind, actions, obs,
-                                                                            reward, done_out, info_out, coll_out, ended_out, &rec);
+                                                                            reward, done_out, info_out, coll_out, ended_out, &rec,
+                                                                            &mot, &msm);
 }
 
 // uavrl_env_reset on envs [0, n_reset): the env's first scenario first + e; with records on, its episode counters restart
@@ -91,17 +94,22 @@ __global__ void env_theta_kernel(EnvDev d)
     if (e < d.n) d.theta[e] = angle_xy(d.vx[e], d.vy[e]);
 }
 
-__global__ void threat_kernel(EnvDev d, int n, const double *__restrict__ pts, uint8_t *__restrict__ out)
+// moved: the current moving table (uavrl_env_set_motion), or null for the cylinders as created
+__global__ void threat_kernel(EnvDev d, int n, const double *__restrict__ pts, uint8_t *__restrict__ out, const MoveObs *moved)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const double x = pts[3 * i], y = pts[3 * i + 1], z = pts[3 * i + 2];
     int hit = out_of_bounds(d.k, x, y, z);
-    for (int c = 0; c < d.k.n_cyl && !hit; ++c) hit = cyl_hit(d.cyl[c], x, y, z);
+    for (int c = 0; c < d.k.n_cyl && !hit; ++c) {
+        Cyl cy = d.cyl[c];
+        if (moved) { cy.cx = moved[c].x; cy.cy = moved[c].y; }
+        hit = cyl_hit(cy, x, y, z);
+    }
     out[i] = (uint8_t)hit;
 }
 
-int launch_env_step(const uavrl_env *env, int action_kind, const void *actions, float *obs, float *reward,
+int launch_env_step(uavrl_env *env, int action_kind, const void *actions, float *obs, float *reward,
                     uint8_t *done, uint8_t *info, uint8_t *coll, uint8_t *ended, cudaStream_t st, bool pdl)
 {
     EnvDev d = env->d;
@@ -124,8 +132,13 @@ int launch_env_step(const uavrl_env *env, int action_kind, const void *actions, 
     }
     if (d.extras) {                                              // optional models: the EXTRAS instantiation (never inside a PDL chain)
         const int blocks = (d.n + kEnvsPerBlockSmall - 1) / kEnvsPerBlockSmall;
+        EnvMotion &mo = env->motion;
+        const EnvMotionDev mv = mo.view(true, env->cfg.len, env->cfg.width);
+        // a candidate mask must also hold every cylinder that moves into the probe window during this step
+        if (mo.on) d.cull_w += mo.reach;
         UAVRL_CUDA(launch_kernel(env_extras_kernel<true, kEnvsPerBlockSmall>, dim3(blocks), dim3(kEnvThreads), 0, st, pdl, d, action_kind, actions, obs,
-                                 reward, done, info, coll, ended, rec));
+                                 reward, done, info, coll, ended, rec, mv));
+        if (mo.on) { mo.cur ^= 1; mo.steps += 1; }             // the launch succeeded: O_{t+1} is the table from now on
     } else if (d.n <= small_batch_envs()) {
         const int blocks = (d.n + kEnvsPerBlockSmall - 1) / kEnvsPerBlockSmall;
         UAVRL_CUDA(launch_kernel(env_kernel<true, kEnvsPerBlockSmall>, dim3(blocks), dim3(kEnvThreads), 0, st, pdl, d, action_kind, actions, obs,
@@ -144,7 +157,8 @@ int launch_env_observe(const uavrl_env *env, float *obs, cudaStream_t st)
     const EnvDev &d = env->d;
     const EnvRecDev &rec = env->records.dev;
     const int blocks = (d.n + kEnvsPerBlockLarge - 1) / kEnvsPerBlockLarge;
-    if (d.extras) env_extras_kernel<false, kEnvsPerBlockLarge><<<blocks, kEnvThreads, 0, st>>>(d, 0, nullptr, obs, nullptr, nullptr, nullptr, nullptr, nullptr, rec);
+    const EnvMotionDev mv = env->motion.view(false, env->cfg.len, env->cfg.width);
+    if (d.extras) env_extras_kernel<false, kEnvsPerBlockLarge><<<blocks, kEnvThreads, 0, st>>>(d, 0, nullptr, obs, nullptr, nullptr, nullptr, nullptr, nullptr, rec, mv);
     else env_kernel<false, kEnvsPerBlockLarge><<<blocks, kEnvThreads, 0, st>>>(d, 0, nullptr, obs, nullptr, nullptr, nullptr, nullptr, nullptr);
     UAVRL_LAUNCHED();
     return 0;
@@ -461,12 +475,16 @@ int uavrl_env_set_extras(uavrl_env *env, const uavrl_env_extras *x)
     if (x->track_envs < 0 || x->track_envs > env->d.n || (x->track_envs > 0 && x->track_capacity <= 0))
         return fail(UAVRL_ERR_INVALID, "track_envs must be in [0, n_envs] with a positive track_capacity");
     if (x->energy_enabled && (!(x->v_0 > 0) || !(x->F_b > 0))) return fail(UAVRL_ERR_INVALID, "energy model: v_0 and F_b must be > 0");
+    const size_t nv = (size_t)env->cfg.n_buildings * 3;
+    // APF and motion read the same attribute of each obstacle (threaten.v): they must agree while both are on
+    if (x->apf_enabled && env->motion.on && nv > 0 && memcmp(x->obstacle_v_host, env->motion.v.data(), nv * sizeof(double)) != 0)
+        return fail(UAVRL_ERR_INVALID, "apf obstacle_v differs from the velocities of uavrl_env_set_motion");
     UAVRL_CUDA(cudaSetDevice(env->cfg.device));
     // the new extras are built beside the old ones and replace them only once complete
     EnvDev d = env->d;
     DevMem m;
     d.energy = nullptr; d.apf_obs = nullptr; d.sub_env = nullptr; d.path_buf = nullptr; d.path_n = nullptr; d.path_cur = nullptr;
-    d.extras = env->d.extras & kExtraRecord; d.track_n = 0; d.track_cap = 0;      // the records stay as they are
+    d.extras = env->d.extras & (kExtraRecord | kExtraMotion); d.track_n = 0; d.track_cap = 0;   // records and motion stay as they are
     const size_t n = (size_t)d.n;
     int rc;
     if (x->energy_enabled) {
@@ -507,6 +525,8 @@ int uavrl_env_set_extras(uavrl_env *env, const uavrl_env_extras *x)
     UAVRL_CUDA(cudaDeviceSynchronize());                         // nothing may still read the extras being replaced
     env->extras_mem = std::move(m);
     env->d = d;
+    if (x->apf_enabled) env->apf_v.assign(x->obstacle_v_host, x->obstacle_v_host + nv);
+    else env->apf_v.clear();
     env->extras_set = true;
     env->reset_done = false;                                     // the new columns are initialised by uavrl_env_reset
     return 0;
@@ -617,9 +637,106 @@ int uavrl_env_threaten_rate(uavrl_env *env, int32_t n, const double *pts_host, u
     int rc;
     if ((rc = m.alloc(dp, (size_t)n * 3, false)) || (rc = m.alloc(dout, (size_t)n, false))) return rc;
     UAVRL_CUDA(cudaMemcpy(dp, pts_host, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice));
-    threat_kernel<<<(n + 127) / 128, 128>>>(env->d, n, dp, dout);
+    threat_kernel<<<(n + 127) / 128, 128>>>(env->d, n, dp, dout, env->motion.on ? env->motion.buf[env->motion.cur] : nullptr);
     UAVRL_LAUNCHED();
     UAVRL_CUDA(cudaMemcpy(out_host, dout, (size_t)n, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int uavrl_env_set_motion(uavrl_env *env, const double *position_host, const double *velocity_host)
+{
+    if (!env) return fail(UAVRL_ERR_INVALID, "null env");
+    const int nc = env->cfg.n_buildings;
+    const double len = env->cfg.len, width = env->cfg.width;
+    if (!velocity_host && position_host)
+        return fail(UAVRL_ERR_INVALID, "uavrl_env_set_motion: positions without velocities (motion off keeps the cylinders as created)");
+    UAVRL_CUDA(cudaSetDevice(env->cfg.device));
+    if (!velocity_host) {                                        // motion off: the step reads the cylinders as created again
+        UAVRL_CUDA(cudaDeviceSynchronize());
+        env->motion = EnvMotion();
+        env->d.extras &= ~kExtraMotion;
+        return 0;
+    }
+    if (nc == 0) return fail(UAVRL_ERR_INVALID, "uavrl_env_set_motion: the city has no obstacles");
+    // the centres: the ones given, or the current ones (the moving table, else the cylinders as created)
+    std::vector<MoveObs> rows((size_t)nc);
+    if (position_host) {
+        for (int i = 0; i < nc; ++i) { rows[(size_t)i].x = position_host[3 * i]; rows[(size_t)i].y = position_host[3 * i + 1]; }
+    } else {
+        UAVRL_CUDA(cudaDeviceSynchronize());
+        if (env->motion.on) {
+            UAVRL_CUDA(cudaMemcpy(rows.data(), env->motion.buf[env->motion.cur], (size_t)nc * sizeof(MoveObs), cudaMemcpyDeviceToHost));
+        } else {
+            std::vector<Cyl> cyl((size_t)nc);
+            UAVRL_CUDA(cudaMemcpy(cyl.data(), env->d.cyl, (size_t)nc * sizeof(Cyl), cudaMemcpyDeviceToHost));
+            for (int i = 0; i < nc; ++i) { rows[(size_t)i].x = cyl[(size_t)i].cx; rows[(size_t)i].y = cyl[(size_t)i].cy; }
+        }
+    }
+    double vmax = 0.0;
+    for (int i = 0; i < nc; ++i) {
+        MoveObs &o = rows[(size_t)i];
+        o.vx = velocity_host[3 * i]; o.vy = velocity_host[3 * i + 1];
+        const double vz = velocity_host[3 * i + 2];
+        if (!std::isfinite(o.x) || !std::isfinite(o.y) || !std::isfinite(o.vx) || !std::isfinite(o.vy) || !std::isfinite(vz))
+            return fail(UAVRL_ERR_INVALID, "uavrl_env_set_motion: non-finite position or velocity");
+        if (o.x < 0.0 || o.x > len || o.y < 0.0 || o.y > width)
+            return fail(UAVRL_ERR_INVALID, "uavrl_env_set_motion: a centre lies outside [0, len] x [0, width]");
+        if (fabs(o.vx) > len || fabs(o.vy) > width)
+            return fail(UAVRL_ERR_INVALID, "uavrl_env_set_motion: |vx| must be <= len and |vy| <= width");
+        vmax = fmax(vmax, fmax(fabs(o.vx), fabs(o.vy)));
+    }
+    const size_t nv = (size_t)nc * 3;
+    if ((env->d.extras & kExtraApf) && memcmp(velocity_host, env->apf_v.data(), nv * sizeof(double)) != 0)
+        return fail(UAVRL_ERR_INVALID, "uavrl_env_set_motion: velocities differ from the APF model's obstacle_v");
+    // cos / sin of calculate_angle(0, v) for the four sign variants, with libm like uavrl_env_set_extras
+    std::vector<double> dir((size_t)nc * 8);
+    for (int i = 0; i < nc; ++i)
+        for (int v = 0; v < 4; ++v) {
+            const MoveObs &o = rows[(size_t)i];
+            const double a = angle_xy(copysign(o.vx, (v & 1) ? -1.0 : 1.0), copysign(o.vy, (v & 2) ? -1.0 : 1.0));
+            dir[(size_t)i * 8 + 2 * v] = cos(a); dir[(size_t)i * 8 + 2 * v + 1] = sin(a);
+        }
+    EnvMotion mo;                                                // built beside the old table, swapped in once complete
+    int rc;
+    if ((rc = mo.mem.alloc(mo.buf[0], (size_t)nc, false)) || (rc = mo.mem.alloc(mo.buf[1], (size_t)nc, false)) ||
+        (rc = mo.mem.alloc(mo.dir, dir.size(), false)))
+        return rc;
+    UAVRL_CUDA(cudaMemcpy(mo.buf[0], rows.data(), (size_t)nc * sizeof(MoveObs), cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(mo.buf[1], rows.data(), (size_t)nc * sizeof(MoveObs), cudaMemcpyHostToDevice));
+    UAVRL_CUDA(cudaMemcpy(mo.dir, dir.data(), dir.size() * sizeof(double), cudaMemcpyHostToDevice));
+    mo.v.assign(velocity_host, velocity_host + nv);
+    mo.reach = vmax + 1.0;                                       // a metre of margin over the rounded centre moves
+    mo.on = true;
+    UAVRL_CUDA(cudaDeviceSynchronize());                         // nothing may still read the table being replaced
+    env->motion = std::move(mo);
+    env->d.extras |= kExtraMotion;
+    return 0;
+}
+
+int uavrl_env_get_obstacles(uavrl_env *env, double *position_host, double *velocity_host, int64_t *steps_out)
+{
+    if (!env) return fail(UAVRL_ERR_INVALID, "null env");
+    const int nc = env->cfg.n_buildings;
+    UAVRL_CUDA(cudaSetDevice(env->cfg.device));
+    UAVRL_CUDA(cudaDeviceSynchronize());
+    const EnvMotion &mo = env->motion;
+    std::vector<MoveObs> rows((size_t)(nc > 0 ? nc : 1));
+    if (mo.on) {
+        UAVRL_CUDA(cudaMemcpy(rows.data(), mo.buf[mo.cur], (size_t)nc * sizeof(MoveObs), cudaMemcpyDeviceToHost));
+    } else if (nc > 0) {
+        std::vector<Cyl> cyl((size_t)nc);
+        UAVRL_CUDA(cudaMemcpy(cyl.data(), env->d.cyl, (size_t)nc * sizeof(Cyl), cudaMemcpyDeviceToHost));
+        for (int i = 0; i < nc; ++i) rows[(size_t)i] = MoveObs{ cyl[(size_t)i].cx, cyl[(size_t)i].cy, 0.0, 0.0 };
+    }
+    for (int i = 0; i < nc; ++i) {
+        const MoveObs &o = rows[(size_t)i];
+        if (position_host) { position_host[3 * i] = o.x; position_host[3 * i + 1] = o.y; position_host[3 * i + 2] = env->base_z[(size_t)i]; }
+        if (velocity_host) {
+            velocity_host[3 * i] = o.vx; velocity_host[3 * i + 1] = o.vy;
+            velocity_host[3 * i + 2] = mo.on ? mo.v[(size_t)i * 3 + 2] : 0.0;
+        }
+    }
+    if (steps_out) *steps_out = mo.on ? mo.steps : 0;
     return 0;
 }
 

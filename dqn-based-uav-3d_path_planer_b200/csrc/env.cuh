@@ -45,7 +45,38 @@ struct EnvDev {
     int32_t track_n, track_cap;
     long long *trace;                   // debug (UAVRL_ENV_TRACE): CTA 0 / thread 0 stage timestamps
 };
-constexpr int kExtraEnergy = 1, kExtraApf = 2, kExtraTrack = 4, kExtraRecord = 8;
+constexpr int kExtraEnergy = 1, kExtraApf = 2, kExtraTrack = 4, kExtraRecord = 8, kExtraMotion = 16;
+
+// Moving obstacles (uavrl_env_set_motion): the device view the EXTRAS step takes as its own kernel argument.  The step reads
+// O_t from rd and CTA 0 writes O_{t+1} to wr, the other buffer; the host flips the two after each launch.
+struct EnvMotionDev {
+    const MoveObs *rd;
+    MoveObs *wr;                        // null for an observation (nothing advances)
+    const double *dir;                  // [n_cyl][4][2]: cos, sin of calculate_angle(0, v) per motion_variant of v
+    double len, width;
+};
+
+// The table's owner: two buffers of n_cyl rows, the APF directions, and what set_motion was given
+struct EnvMotion {
+    DevMem mem;
+    MoveObs *buf[2] = { nullptr, nullptr };
+    double *dir = nullptr;
+    int cur = 0;                        // the buffer holding O_t
+    int64_t steps = 0;                  // step calls since set_motion
+    double reach = 0.0;                 // added to the cull half-width: the largest |vx|, |vy| plus a margin
+    std::vector<double> v;              // [n_cyl][3] velocities as set (vz included)
+    bool on = false;
+    EnvMotionDev view(bool advance, double len, double width) const
+    {
+        return { buf[cur], advance ? buf[cur ^ 1] : nullptr, dir, len, width };
+    }
+};
+
+// Per-CTA staging of the moving table (env_extras_kernel only): O_t as read, and the APF table at O_t
+struct MotionSmem {
+    MoveObs o[kMaxCyl];
+    ApfObs apf[kMaxCyl];
+};
 
 // Episode records (uavrl_env_set_records): the device view the EXTRAS step takes as its own kernel argument, so EnvDev and the
 // default step keep their layout.  Episode j of env e goes to slot j n + e; a slot at or beyond cap is counted as dropped.
@@ -82,11 +113,14 @@ struct uavrl_env {
     bool extras_set = false;
     std::vector<double> base_z;          // building base heights (position.z), used by the APF distance only
     uavrl::EnvRecords records;           // uavrl_env_set_records; swapped out for its own by an evaluation (eval.cu)
+    uavrl::EnvMotion motion;             // uavrl_env_set_motion
+    std::vector<double> apf_v;           // [n_cyl][3] obstacle velocities of the APF model, when it is on
 };
 
 namespace uavrl {
-// launched by env.cu, the fused training loops (train.cu) and the evaluation loop (eval.cu)
-int launch_env_step(const uavrl_env *env, int action_kind, const void *actions, float *obs, float *reward,
+// launched by env.cu, the fused training loops (train.cu) and the evaluation loop (eval.cu); with moving obstacles a launch
+// advances the table, so the handle is not const
+int launch_env_step(uavrl_env *env, int action_kind, const void *actions, float *obs, float *reward,
                     uint8_t *done, uint8_t *info, uint8_t *coll, uint8_t *ended, cudaStream_t st, bool pdl = false);
 int launch_env_observe(const uavrl_env *env, float *obs, cudaStream_t st);
 // env_reset_kernel over envs [0, n_reset) only (uavrl_env_reset: every env; an evaluation: the envs that have a suite position)

@@ -139,7 +139,8 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
                                           const void *__restrict__ actions, float *__restrict__ obs, float *__restrict__ reward,
                                           uint8_t *__restrict__ done_out, uint8_t *__restrict__ info_out,
                                           uint8_t *__restrict__ coll_out, uint8_t *__restrict__ ended_out,
-                                          const EnvRecDev *rec = nullptr)
+                                          const EnvRecDev *rec = nullptr, const EnvMotionDev *mot = nullptr,
+                                          MotionSmem *msm = nullptr)
 {
 #define ENV_TRACE(slot) do { if (d.trace && blockIdx.x == 0 && tid == 0) d.trace[slot] = clock64(); } while (0)
     ENV_TRACE(0);
@@ -191,8 +192,30 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
         if (EXTRAS && DO_STEP && (d.extras & kExtraRecord)) parked = (long long)rec->ord[e] * d.n + e >= rec->limit;
     }
     const int cur0 = s.cursor;
-    for (int i = tid; i < d.k.n_cyl * 6; i += NT)
-        reinterpret_cast<double *>(s_cyl)[i] = reinterpret_cast<const double *>(d.cyl)[i];
+    // EXTRAS with moving obstacles: every CTA stages O_t (centres into the cylinders, and the APF table at O_t with the
+    // direction of each obstacle's current velocity variant); the APF reads below all take apf_tab
+    const bool moving = EXTRAS && (d.extras & kExtraMotion);
+    const ApfObs *apf_tab = d.apf_obs;
+    if (moving) {
+        for (int c = tid; c < d.k.n_cyl; c += NT) {
+            const MoveObs o = mot->rd[c];
+            msm->o[c] = o;
+            Cyl cy = d.cyl[c];
+            cy.cx = o.x; cy.cy = o.y;
+            s_cyl[c] = cy;
+            if (d.extras & kExtraApf) {
+                ApfObs a = d.apf_obs[c];
+                const int v = motion_variant(o.vx, o.vy);
+                a.x = o.x; a.y = o.y; a.vx = o.vx; a.vy = o.vy;
+                a.cav = mot->dir[8 * c + 2 * v]; a.sav = mot->dir[8 * c + 2 * v + 1];
+                msm->apf[c] = a;
+            }
+        }
+        apf_tab = msm->apf;
+    } else {
+        for (int i = tid; i < d.k.n_cyl * 6; i += NT)
+            reinterpret_cast<double *>(s_cyl)[i] = reinterpret_cast<const double *>(d.cyl)[i];
+    }
     __syncthreads();
     ENV_TRACE(1);
     if (USE_PDL && wp >= NW1) { pdl_wait(); pdl_trigger(); }
@@ -230,8 +253,25 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
                     return threat_masked(kk, cyl, mask, x, y, z);
                 };
                 if (apf_on) {
-                    ApfDev apf; apf.ob = d.apf_obs; apf.n = d.k.n_cyl;
+                    ApfDev apf; apf.ob = apf_tab; apf.n = d.k.n_cyl;
+                    const bool alias = s.alias && s.cursor == 0;
                     step_core_apf(d.k, s, mode, act, sub, threat, apf, o);
+                    if (alias && s.cursor == 0) {
+                        // sub_goals[0] was the position object (RRT.py:69) and was not popped: the queue keeps the moved
+                        // position (a collision rebinds position, not the entry, UAV.py:427), which phase 1b and the
+                        // observation then shift.  A large APF push at the start point (a moving obstacle over it) gets here.
+                        P3 m;
+                        if (o.coll) {                        // the step restored the old position: move it again
+                            const int kk = (int)act;
+                            m.x = dadd(s.px, s.vx); m.y = dadd(s.py, s.vy);
+                            m.z = mode == 1 ? dadd(s.pz, dmul((double)((kk / 3) % 3 - 1), d.k.climb)) : s.pz;
+                        } else {
+                            m.x = s.px; m.y = s.py; m.z = s.pz;
+                        }
+                        double *q0 = d.sub_env + (size_t)e * d.K * 3;
+                        q0[0] = m.x; q0[1] = m.y; q0[2] = m.z;
+                        sgc[0] = m;
+                    }
                 } else {
                     step_core(d.k, s, mode, act, sub, threat, o);
                 }
@@ -287,7 +327,7 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
                 const bool own_q = apf_on && !(DO_STEP && d.auto_reset && n_ended && !(EXTRAS && park_after));
                 const double *q = own_q ? d.sub_env + (size_t)e * d.K * 3 : d.pool_sub + (size_t)scen * d.K * 3;
                 const bool shift = own_q && DO_STEP;
-                const ApfObs *aob = d.apf_obs; const int an = d.k.n_cyl;
+                const ApfObs *aob = apf_tab; const int an = d.k.n_cyl;
                 const bool same_q = !(DO_STEP && d.auto_reset && n_ended && !(EXTRAS && park_after));   // still the queue the prefetch read
                 auto sub = [q, shift, aob, an, same_q, cur0, &sgc](int i) {
                     P3 p;
@@ -335,6 +375,17 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
         d.step[e] = s.step; d.cursor[e] = s.cursor;
         d.done[e] = (uint8_t)s.done; d.alias[e] = (uint8_t)s.alias;
     }
+    if (moving && DO_STEP) {
+        // every obstacle runs once: O_{t+1}, the same arithmetic in every CTA, for the probes of phase 2; CTA 0 stores it into
+        // the buffer the next step reads (this launch reads the other one).  msm->apf keeps O_t for phase 1b.
+        for (int c = tid; c < d.k.n_cyl; c += NT) {
+            MoveObs o = msm->o[c];
+            obstacle_run(o, mot->len, mot->width);
+            s_cyl[c].cx = o.x; s_cyl[c].cy = o.y;
+            if (blockIdx.x == 0) mot->wr[c] = o;
+        }
+        __syncthreads();
+    }
     if (EXTRAS && DO_STEP && (d.extras & kExtraApf)) {
         // phase 1b, all threads: UAV.Adjust_subgoal (UAV.py:156-166) for the stored queues -- every entry moves by the
         // force at its (pre-step) position; an env that restarted takes its new scenario's queue instead
@@ -346,7 +397,7 @@ __device__ __forceinline__ void env_block(const EnvDev &d, EnvSmem<EPB> &sm, int
                 const double *src = d.pool_sub + ((size_t)d.scen[e] * d.K + i) * 3;
                 q[0] = src[0]; q[1] = src[1]; q[2] = src[2];
             } else if (i < d.n_sub[e]) {
-                const P3 f = apf_force(d.apf_obs, d.k.n_cyl, q[0], q[1], q[2]);
+                const P3 f = apf_force(apf_tab, d.k.n_cyl, q[0], q[1], q[2]);
                 q[0] = dadd(q[0], f.x); q[1] = dadd(q[1], f.y); q[2] = dadd(q[2], f.z);
             }
         }

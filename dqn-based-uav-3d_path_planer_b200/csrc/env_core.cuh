@@ -207,6 +207,27 @@ UAVRL_HD P3 apf_force(const ApfObs *ob, int n, double px, double py, double pz)
     return tot;
 }
 
+// Moving obstacles (uavrl_env_set_motion): a cylinder's centre and planar velocity.  z, R and H are fixed.
+struct MoveObs { double x, y, vx, vy; };
+
+// One obstacle's run() (the reference's per-obstacle hook, Obstacles/BaseThreaten.py, is `pass`; this is the port's rule):
+// x' = x + vx, reflected once at 0 and at len (y likewise at width), and the velocity component reverses at a reflection.
+// One reflection suffices because centres lie in [0, len] x [0, width] with |vx| <= len, |vy| <= width.
+UAVRL_HD void obstacle_run(MoveObs &o, double len, double width)
+{
+    double x = dadd(o.x, o.vx);
+    if (x < 0.0) { x = -x; o.vx = -o.vx; }
+    else if (x > len) { x = dsub(len, dsub(x, len)); o.vx = -o.vx; }
+    double y = dadd(o.y, o.vy);
+    if (y < 0.0) { y = -y; o.vy = -o.vy; }
+    else if (y > width) { y = dsub(width, dsub(y, width)); o.vy = -o.vy; }
+    o.x = x; o.y = y;
+}
+
+// Which of an obstacle's four sign variants (+-vx, +-vy) its velocity is in: a reflection only flips a sign bit, so the APF
+// direction of every variant is evaluated once on the host and the step selects it by the current signs.
+UAVRL_HD int motion_variant(double vx, double vy) { return (signbit(vx) ? 1 : 0) | (signbit(vy) ? 2 : 0); }
+
 struct NoApf {
     static constexpr bool enabled = false;
     UAVRL_HD P3 force(double, double, double) const { P3 z; z.x = z.y = z.z = 0.0; return z; }

@@ -244,6 +244,23 @@ class EnvBatch:
         check(_lib.lib().uavrl_env_threaten_rate(self.h, pts.shape[0], _ptr(pts), _ptr(out)))
         return out
 
+    # -- moving obstacles (include/uavrl.h, uavrl_env_set_motion): one table per batch, advanced once per step call
+    def set_motion(self, velocity, positions=None):
+        """velocity [n_buildings, 3]: every obstacle's `v` (motion on); None: motion off.  positions [n_buildings, 3] (z ignored):
+        the centres to start from; None keeps the current ones.  Takes effect from the next step."""
+        nb = self.city.buildings.shape[0]
+        v = None if velocity is None else np.ascontiguousarray(velocity, np.float64).reshape(nb, 3)
+        p = None if positions is None else np.ascontiguousarray(positions, np.float64).reshape(nb, 3)
+        check(_lib.lib().uavrl_env_set_motion(self.h, _ptr(p), _ptr(v)))
+
+    def obstacles(self):
+        """(positions [n, 3] with z the base height, velocities [n, 3], step calls since set_motion) of the current table."""
+        nb = self.city.buildings.shape[0]
+        pos = np.zeros((nb, 3), np.float64); vel = np.zeros((nb, 3), np.float64)
+        steps = C.c_int64()
+        check(_lib.lib().uavrl_env_get_obstacles(self.h, _ptr(pos), _ptr(vel), C.byref(steps)))
+        return pos, vel, int(steps.value)
+
 
 RECORD_FIELDS = ("scenario", "env", "ordinal", "outcome", "steps", "subgoals", "collisions", "total_score", "path_len",
                  "start2goal", "planner_len", "final_dist", "energy")

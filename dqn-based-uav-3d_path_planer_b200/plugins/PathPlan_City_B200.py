@@ -13,6 +13,10 @@ env.run_eposide(eps) -> result dict; env.Agents[i].Train_time / Testing_time; en
 env.run_evaluation(n) plays n held-out scenarios with the trained policy on an env of its own (<eval_seed>, <eval_episodes>,
 <eval_envs>, <eval_mean_action>) and returns its summary; <record_episodes>1</record_episodes> adds generate_train_result's
 per-episode fields to run_eposide's result.
+Moving obstacles: a <Threaten> of the buildings XML may carry the `v` attribute UAV.cal_force reads, <v><x/><y/><z/></v>
+(missing: zero).  <APF_Enabled>1</APF_Enabled> in the UAV XML turns the APF model on with those velocities, and
+<moving_obstacles>1</moving_obstacles> in the env XML moves every obstacle by its `v` once per lockstep step (include/uavrl.h,
+uavrl_env_set_motion).
 """
 import importlib
 import math
@@ -107,6 +111,17 @@ def buildings_from_dict(bdict: dict):
                       float(None2Value(t.get("_R"), 10)), float(None2Value(t.get("_H"), 20))] for t in th], np.float64)
 
 
+def obstacle_v_from_dict(bdict: dict):
+    """The `v` of every <Threaten> ([n, 3], zero where it has none) and whether any of them has one."""
+    th = bdict["Threaten"]
+    if isinstance(th, dict):
+        th = [th]
+    vs = [t.get("v") for t in th]
+    v = np.array([[float(None2Value(x.get(k), 0)) for k in ("x", "y", "z")] if isinstance(x, dict) else [0.0, 0.0, 0.0]
+                  for x in vs], np.float64).reshape(-1, 3)
+    return v, any(isinstance(x, dict) for x in vs)
+
+
 def eval_summary(rec, num_trainers=1):
     """The summary run_evaluation returns, from evaluation records in suite order (engine.eval_run's 'records'): counts and
     rates over the finished episodes, means of their steps / path_len / total_score / start2goal / energy, the mean
@@ -183,6 +198,12 @@ class PathPlan_City_B200:
         agents_params = param.get('Agent')
         self.uav_dict = XML2Dict(os.path.normpath(agents_params['xml_path_agent'])).get('Agent')
         self.uav_params = uav_params_from_dict(self.uav_dict)
+        # APF_Enabled (UAV.py:448-453) with the obstacles' `v`; moving_obstacles = 1: the obstacles move by it every step
+        self.obstacle_v, has_v = obstacle_v_from_dict(self.buildings_param)
+        self.apf_enabled = int(None2Value(self.uav_dict.get("APF_Enabled"), 0))
+        self.moving_obstacles = int(None2Value(param.get("moving_obstacles"), 0))
+        if self.apf_enabled and not has_v:
+            raise ValueError("APF_Enabled = 1 needs obstacle velocities: no <Threaten> of the buildings XML carries a <v>")
         self.sub_granularity = int(None2Value(self.uav_dict.get("sub_granularity"), 30))
         fn = self.uav_dict.get("update_function_name")
         self.discrete = (fn != "update_PathPlan")            # update_PathPlan27: the discrete-27 extension
@@ -205,9 +226,12 @@ class PathPlan_City_B200:
             power = {k: float(fp[k]) for k in ("P_i", "v_0", "d_0", "rho", "s", "A", "P_b", "F_b")}
             power["xi"] = 0.8                                      # UAV.py:58 with j = 0 (one shared parameter set)
         self._power = power
-        if power is not None or self.record_csv:
-            self.batch.set_extras(power=power, track_envs=(1 if self.record_csv else 0),
+        self._apf_v = self.obstacle_v if self.apf_enabled else None
+        if power is not None or self.record_csv or self.apf_enabled:
+            self.batch.set_extras(power=power, obstacle_v=self._apf_v, track_envs=(1 if self.record_csv else 0),
                                   track_capacity=(64 * self.uav_params.max_step if self.record_csv else 0))
+        if self.moving_obstacles:
+            self.batch.set_motion(self.obstacle_v)
         # trainer(s): one handle holding num_trainers independent trainers
         tpath = os.path.normpath(agents_params['Trainer']['Trainer_path'])
         tdict = XML2Dict(tpath).get('Trainer')
@@ -426,8 +450,8 @@ class PathPlan_City_B200:
             ev = engine.EnvBatch(self.city, self.uav_params, self.eval_envs, max_subgoals=64, device=self.device_index)
             sc = ev.make_scenarios(self.eval_episodes, seed=self.eval_seed, rrt_step=self.sub_granularity)
             ev.set_pool(sc["start"], sc["goal"], sc["heading"], sc["sub"], sc["n_sub"])
-            if self._power is not None:
-                ev.set_extras(power=self._power)
+            if self._power is not None or self._apf_v is not None:
+                ev.set_extras(power=self._power, obstacle_v=self._apf_v)
             self._eval_batch = ev
         return self._eval_batch
 
@@ -446,6 +470,8 @@ class PathPlan_City_B200:
             raise ValueError("n_episodes (%d) exceeds the evaluation pool (eval_episodes = %d)" % (n, self.eval_episodes))
         t0 = time.time()
         ev, learner = self._eval_env(), self.Trainer._learner
+        if self.moving_obstacles:                               # every evaluation starts from the XML table
+            ev.set_motion(self.obstacle_v, positions=self.buildings_table[:, :3])
         if isinstance(learner, engine.SacLearner):
             res = engine.sac_eval_run(ev, learner, n, mean_action=bool(self.eval_mean_action))
         else:

@@ -145,7 +145,8 @@ int uavrl_env_set_state(uavrl_env *env, const uavrl_env_state_host *in);
  *   apf      moving-obstacle artificial potential field (UAV.cal_force / Adjust_subgoal, UAV.py:156-210, and the reward
  *            term :448-453): obstacle_v_host [n_buildings][3] = the `v` attribute of each obstacle; obstacles with v = 0
  *            exert no force (UAV.py:180-182).  Every step shifts each remaining sub-goal by the force at its position,
- *            so sub-goal queues become per-UAV state.
+ *            so sub-goal queues become per-UAV state.  The obstacles stay where they are unless uavrl_env_set_motion moves
+ *            them; while it does, obstacle_v must equal its velocities.
  *   track    UAV.path (UAV.py:432) of the first track_envs UAVs, up to track_capacity points per episode, double
  *            buffered: the episode in progress and the last finished one (what path.csv holds, UAV.py:461-464). */
 typedef struct {
@@ -200,6 +201,35 @@ int uavrl_env_clear_records(uavrl_env *env);
 /* PathPlan_City.Threaten_rate (Envs/PathPlan_City.py:215-223) on arbitrary points (device kernel):
  * pts_host [n][3] -> out_host [n] u8. */
 int uavrl_env_threaten_rate(uavrl_env *env, int32_t n, const double *pts_host, uint8_t *out_host);
+
+/* Moving obstacles.  The reference's hooks for scene change (PathPlan_City.run(), BaseThreaten.run()) are `pass`; this is the
+ * port's rule, built from the reference's own primitives.
+ *   world    The n_envs UAVs of a batch are the UAVs of one city: one obstacle table per env handle.  It advances once per
+ *            step call (uavrl_env_step, _step_host, the training and evaluation loops), whatever each env's episode is doing;
+ *            uavrl_env_reset leaves it alone, and uavrl_env_observe / uavrl_env_threaten_rate read it without advancing it.
+ *   state    Each obstacle has a centre (x, y) and a velocity (vx, vy, vz).  Its base z, _R and _H are fixed: cylinders stand on
+ *            the ground (check_threaten tests p.z against the absolute _H), so vz moves nothing; it only adds to |v| in the APF.
+ *   run()    Per obstacle, each IEEE operation rounded, in this order: x' = x + vx; if x' < 0 then x' = -x', vx = -vx; else if
+ *            x' > len then x' = len - (x' - len), vx = -vx; then y likewise against width.  A reflection only flips signs, so
+ *            |v| is constant; the APF direction of v, cos / sin of calculate_angle(0, v), is evaluated on the host with libm
+ *            for all four sign variants (+-vx, +-vy) and the step selects one by the current signs.
+ *   order    Within step t the UAV move, the collision test (UAV.py:425), the reward (APF term included) and Adjust_subgoal use
+ *            the table O_t.  Every obstacle then runs once, giving O_{t+1}, and the observation the step writes (its probes,
+ *            and the observation of an env that auto-resets in the step) uses O_{t+1}: it is s' of transition t and s of step
+ *            t + 1.  With the table first set to the reference's positions after its first run(), the observation after k
+ *            steps is the reference loop's state_test of iteration k.  (The reference's stored next_state is computed inside
+ *            Move_Agent, before the next run(), against the old table; the port stores the observation the agent acts on.)
+ * uavrl_env_set_motion: position_host [n_buildings][3] (z ignored) or NULL to keep the current centres; velocity_host
+ *   [n_buildings][3] turns motion on, NULL turns it off (then position_host must be NULL too, and the step reads the cylinders
+ *   as uavrl_env_create was given them).  Refused with UAVRL_ERR_INVALID, changing nothing: non-finite values, a centre
+ *   outside [0, len] x [0, width], |vx| > len or |vy| > width, and velocities that differ from the APF model's obstacle_v
+ *   while APF is on (uavrl_env_set_extras likewise refuses an obstacle_v that differs from these velocities while motion is
+ *   on).  With both on, APF's force reads the moving table: current centres and current signs.  Motion rides on the
+ *   optional-model step.  Synchronises the device; takes effect from the next step.
+ * uavrl_env_get_obstacles: the current table, position_host [n][3] (z = the base height), velocity_host [n][3] (zero with
+ *   motion off), and the step calls since uavrl_env_set_motion; any pointer may be NULL.  Synchronises the device. */
+int uavrl_env_set_motion(uavrl_env *env, const double *position_host, const double *velocity_host);
+int uavrl_env_get_obstacles(uavrl_env *env, double *position_host, double *velocity_host, int64_t *steps_out);
 
 /* ------------------------------------------------------------------ learner (Q-net + replay) */
 typedef struct uavrl_learner uavrl_learner;
