@@ -20,6 +20,33 @@ def velocity_signs(tab):
     return ((tab[:, 2] < 0).astype(np.uint8) | ((tab[:, 3] < 0).astype(np.uint8) << 1))
 
 
+def wall_reflections(before, after):
+    """Reflections per wall between two tables of the same rows (any number of runs apart, one reflection per row at most):
+    at x = 0 vx turns from negative to positive, at x = len from positive to negative; likewise y at 0 and width."""
+    b, a = np.asarray(before, np.float64), np.asarray(after, np.float64)
+    return {"x0": int(((b[:, 2] < 0) & (a[:, 2] > 0)).sum()), "xlen": int(((b[:, 2] > 0) & (a[:, 2] < 0)).sum()),
+            "y0": int(((b[:, 3] < 0) & (a[:, 3] > 0)).sum()), "ywidth": int(((b[:, 3] > 0) & (a[:, 3] < 0)).sum())}
+
+
+# UAV.state_PathPlan's 80 probes (UAV.py:533-555,562-566) as the kernel takes them (env_block.cuh probe_offset): 3 planar 5 x 5
+# grids at 1 / 5 / 10 m for slots 11..85, then 1..5 m below for slots 90..94
+_G = np.array([1, 5, 10]).repeat(25)
+_IJ = np.tile(np.arange(25), 3)
+PROBE_DX = np.r_[_G * (_IJ // 5 - 2), np.zeros(5, np.int64)].astype(np.float64)
+PROBE_DY = np.r_[_G * (_IJ % 5 - 2), np.zeros(5, np.int64)].astype(np.float64)
+PROBE_SLOT = np.r_[11:86, 90:95]
+
+
+def probe_points(px, py, pz):
+    """[n, 80, 3] probe points of n UAVs in observation-slot order PROBE_SLOT, each coordinate the IEEE operation the kernel
+    performs: px + dx, py + dy at z = pz for the planar probes, px, py at pz - (k + 1) for the probes below."""
+    px, py, pz = (np.asarray(v, np.float64).reshape(-1, 1) for v in (px, py, pz))
+    x = np.concatenate([px + PROBE_DX[None, :75], np.repeat(px, 5, 1)], 1)
+    y = np.concatenate([py + PROBE_DY[None, :75], np.repeat(py, 5, 1)], 1)
+    z = np.concatenate([np.repeat(pz, 75, 1), pz - np.arange(1.0, 6.0)[None]], 1)
+    return np.stack([x, y, z], 2)
+
+
 def obstacle_run(tab, length, width):
     """One run() of every row (x, y, vx, vy) of tab, in place, each IEEE operation in the rule's order."""
     for r in tab:
@@ -41,7 +68,7 @@ class MovingCity:
     """An OracleCity whose centres follow tab [n, 4]; with apf, the oracle's APF velocities follow its signs."""
 
     def __init__(self, length, width, h, buildings, tab, vz=None, apf=False):
-        self.city = O.OracleCity(length, width, h, buildings)
+        self.city = O.OracleCity(length, width, h, np.array(buildings, np.float64))     # its own copy: the caller's stays put
         self.len, self.width = float(length), float(width)
         self.tab = np.array(tab, np.float64).reshape(-1, 4)
         self.apf = apf

@@ -83,13 +83,19 @@ def test_golden_reflects_on_every_wall(g):
     assert walls == {"x0", "xlen", "y0", "ywidth"}
 
 
-def test_host_compiled_obstacle_run_matches_golden(g, tmp_path):
-    """env_core.cuh's obstacle_run (the code the kernel runs) compiled for the host, run from each episode's first table,
-    reproduces every table the reference recorded, bit for bit."""
-    so = str(tmp_path / "libmotion_host.so")
+@pytest.fixture(scope="module")
+def shim(tmp_path_factory):
+    """env_core.cuh's obstacle_run (the code the kernel runs) compiled for the host."""
+    so = str(tmp_path_factory.mktemp("motion_host") / "libmotion_host.so")
     cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
     subprocess.check_call([cxx, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-shared", "-x", "c++", SHIM_SRC, "-o", so])
-    lib = C.CDLL(so)
+    return C.CDLL(so)
+
+
+def test_host_compiled_obstacle_run_matches_golden(g, shim):
+    """obstacle_run compiled for the host, run from each episode's first table, reproduces every table the reference
+    recorded, bit for bit."""
+    lib = shim
     dims = g["dims"]
     n = 0
     for c in range(int(g["n_cfg"])):
@@ -101,6 +107,80 @@ def test_host_compiled_obstacle_run_matches_golden(g, tmp_path):
                 assert MO.table_digest(rows) == ep["tab_digest"][t].tobytes(), (c, t)
                 n += 1
     assert n > 1000
+
+
+def edge_rows(L, W, rng):
+    """Hand rows (x, y, vx, vy) of an L x W box: centres on every wall and corner, |v| exactly L / W (wall to wall every run),
+    x + vx landing exactly on 0 or L (not a reflection), signed zeros and subnormal velocities."""
+    tiny = np.nextafter(0.0, 1.0)
+    rows = []
+    for x, y in ((0.0, W / 3), (L, W / 3), (L / 3, 0.0), (L / 3, W), (0.0, 0.0), (L, 0.0), (0.0, W), (L, W), (-0.0, -0.0)):
+        rows += [(x, y, rng.uniform(-L, L), rng.uniform(-W, W)), (x, y, L, W), (x, y, -L, -W), (x, y, L, -W), (x, y, -0.0, 0.0)]
+    rows += [(L / 2, W / 2, L, W), (L / 4, 3 * W / 4, -L, W)]
+    for x in (L / 4, L / 2, 0.375 * L):                     # dyadic fractions: x - x and x + (L - x) are exact
+        rows += [(x, W / 2, -x, 0.0), (x, W / 2, L - x, 0.0)]
+    for y in (W / 4, 0.625 * W):
+        rows += [(L / 2, y, 0.0, -y), (L / 2, y, 0.0, W - y)]
+    rows += [(0.0, 0.0, -tiny, -tiny), (L, W, tiny, tiny), (0.0, W, tiny, -tiny), (L / 2, W / 2, -0.0, -0.0),
+             (0.0, 0.0, 0.0, -0.0), (L, W / 2, -tiny, 0.0)]
+    return np.array(rows, np.float64)
+
+
+@pytest.mark.parametrize("L,W", [(300.0, 800.0), (800.0, 300.0), (1.0, 1000.0), (500.0, 500.0)])
+def test_host_compiled_obstacle_run_on_non_square_boxes(shim, L, W):
+    """obstacle_run compiled for the host against motion_oracle.obstacle_run, bit for bit after every run, on random tables
+    (|vx| <= len, |vy| <= width) and the hand edge rows; after every run the centres lie in [0, len] x [0, width] and each
+    velocity component keeps its magnitude (only its sign may flip); over the runs every wall reflects some row.  A len /
+    width swap anywhere in the rule fails the first three boxes."""
+    rng = np.random.default_rng(int(L * 7 + W))
+    n = 96
+    rnd = np.zeros((n, 4))
+    rnd[:, 0] = rng.uniform(0, L, n); rnd[:, 1] = rng.uniform(0, W, n)
+    rnd[:, 2] = rng.uniform(-L, L, n) * rng.choice([1.0, 0.1, 0.01], n)
+    rnd[:, 3] = rng.uniform(-W, W, n) * rng.choice([1.0, 0.1, 0.01], n)
+    edge = edge_rows(L, W, rng)
+    tab = np.concatenate([rnd, edge])
+    dev = np.ascontiguousarray(tab.copy())
+    mag = np.abs(tab[:, 2:]).copy()
+    walls = dict.fromkeys(("x0", "xlen", "y0", "ywidth"), 0)
+    runs = 0
+    for t in range(80):
+        before = tab.copy()
+        MO.obstacle_run(tab, L, W)
+        shim.shim_obstacle_run(C.c_int(dev.shape[0]), dev.ctypes.data_as(C.c_void_p), C.c_double(L), C.c_double(W), C.c_int(1))
+        assert MO.table_digest(dev) == MO.table_digest(tab), (L, W, t, np.nonzero((dev != tab).any(1))[0])
+        assert ((tab[:, 0] >= 0) & (tab[:, 0] <= L) & (tab[:, 1] >= 0) & (tab[:, 1] <= W)).all(), (L, W, t)
+        assert np.array_equal(np.abs(tab[:, 2:]), mag), (L, W, t)
+        for k, v in MO.wall_reflections(before, tab).items():
+            walls[k] += v
+        runs += tab.shape[0]
+    assert runs >= 10000 and min(walls.values()) > 0, walls
+    # landing exactly on a wall is not a reflection: the first run keeps those velocities
+    one = edge.copy()
+    MO.obstacle_run(one, L, W)
+    land = (edge[:, 3] == 0.0) & (edge[:, 1] == W / 2) & ((edge[:, 0] + edge[:, 2] == 0.0) | (edge[:, 0] + edge[:, 2] == L))
+    assert land.sum() >= 4 and np.array_equal(one[land, 2], edge[land, 2]) and np.isin(one[land, 0], (0.0, L)).all()
+
+
+def test_probe_points_are_the_observation_probes():
+    """motion_oracle.probe_points in slot order: the oracle's threaten_rate on them equals the occupancy bits of the oracle's
+    own observation, on a dense city with UAVs next to cylinders and the box edges."""
+    rng = np.random.default_rng(2)
+    L, W, H = 300.0, 800.0, 80.0
+    b = np.zeros((40, 5))
+    b[:, 0] = rng.uniform(0, W, 40); b[:, 1] = rng.uniform(0, W, 40)
+    b[:, 2] = 1.0; b[:, 3] = rng.uniform(4, 20, 40); b[:, 4] = rng.uniform(3, 60, 40)
+    city = O.OracleCity(L, W, H, b)
+    n = 64
+    ob = O.OracleBatch(city, O.UavParams(), n, 2)
+    start = np.stack([rng.uniform(-5, W + 5, n), rng.uniform(-5, W + 5, n), rng.uniform(0, 12, n)], 1)
+    start[:8, 0] = [0.0, 19.5, 20.0, W - 20.0, W, 10.0, 5.0, 1.0]
+    ob.reset(start, start + 50, rng.uniform(0, 6, n), np.repeat(start[:, None], 2, 1), np.full(n, 2))
+    obs = ob.state(want64=True)[1]
+    pts = MO.probe_points(ob.px, ob.py, ob.pz)
+    bits = city.threaten_rate(pts.reshape(-1, 3)).reshape(n, 80)
+    assert np.array_equal(bits, obs[:, MO.PROBE_SLOT].astype(np.uint8))
+    assert 0 < bits.sum() < bits.size
 
 
 def write_xml_variants(tmp_path):
