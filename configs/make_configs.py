@@ -104,4 +104,42 @@ for name, ttype, net, extra in (("Trainer_DQN_B200.xml", "DQN_Trainer_B200", "QV
     <save_loop>1000000000</save_loop>
 </Trainer>
 """ % (ttype, net))
+# SAC with discrete actions (SAC_Trainer's IS_Continuous = 0 branch, PolicyNet_SAC / QValueNet_SAC) on the 27-action step:
+# the shipped SAC learning rates, alpha lr, tau, gamma and target entropy (config/Trainer.xml)
+open(os.path.join(HERE, "Trainer_SAC_discrete_B200.xml"), "w").write("""<Trainer>
+    <Trainer_Type>SAC_Trainer_B200</Trainer_Type>
+    <Is_Train>1</Is_Train>
+    <IsPriority_Replay>0</IsPriority_Replay>
+    <actor>
+        <NetWork>PolicyNet_SAC</NetWork>
+        <h>1</h>
+        <w>100</w>
+        <channel>1</channel>
+        <hiden_dim>64</hiden_dim>
+        <output>27</output>
+        <lr>0.0001</lr>
+    </actor>
+    <critic>
+        <NetWork>QValueNet_SAC</NetWork>
+        <h>1</h>
+        <w>100</w>
+        <channel>1</channel>
+        <hiden_dim>64</hiden_dim>
+        <output>27</output>
+        <lr>0.001</lr>
+    </critic>
+    <SAC_param>
+        <IS_Continuous>0</IS_Continuous>
+        <alpha_lr>0.0001</alpha_lr>
+        <target_entropy>1</target_entropy>
+        <gamma>0.99</gamma>
+        <tau>0.05</tau>
+    </SAC_param>
+    <replay_size>1048576</replay_size>
+    <LEARNING_RATE>0.0005</LEARNING_RATE>
+    <Batch_Size>4096</Batch_Size>
+    <max_epoch>100</max_epoch>
+    <save_loop>1000000000</save_loop>
+</Trainer>
+""")
 print("wrote", sorted(os.listdir(HERE)))

@@ -67,7 +67,7 @@ class SacConfig(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("hidden", C.c_int32), ("act_dim", C.c_int32), ("action_bound", C.c_float),
                 ("actor_lr", C.c_float), ("critic_lr", C.c_float), ("alpha_lr", C.c_float), ("target_entropy", C.c_float),
                 ("gamma", C.c_float), ("tau", C.c_float), ("batch_size", C.c_int32), ("replay_capacity", C.c_int64),
-                ("lockstep_envs", C.c_int32), ("seed", C.c_uint64), ("device", C.c_int32), ("loss_kind", C.c_int32)]
+                ("lockstep_envs", C.c_int32), ("seed", C.c_uint64), ("device", C.c_int32), ("discrete", C.c_int32)]
 
 
 class TrainStats(C.Structure):
@@ -171,6 +171,7 @@ SIGNATURES = {
     "uavrl_sac_set_scalars": (C.c_int, [VP, C.c_float, C.c_float, C.c_float, C.c_int64, C.c_int64]),
     "uavrl_sac_get_scalars": (C.c_int, [VP, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "uavrl_sac_act": (C.c_int, [VP, VP, C.c_int32, VP, VP, VP]),
+    "uavrl_sac_act_discrete": (C.c_int, [VP, VP, C.c_int32, VP, C.c_int32, VP, VP]),
     "uavrl_sac_update_batch": (C.c_int, [VP, C.c_int32, VP, VP, VP, VP, VP, VP, VP, VP, VP]),
     "uavrl_sac_train_run": (C.c_int, [VP, VP, C.c_int32, C.c_int32, C.POINTER(TrainStats), VP]),
     "uavrl_sac_smem_bytes": (C.c_int, [C.POINTER(SacConfig), VP]),

@@ -28,7 +28,11 @@ static int obs_dim(const uavrl_learner *l) { return l->cfg.in_dim; }
 static int obs_dim(const uavrl_sac *s) { return s->cfg.obs_dim; }
 // the env step's action kind; null: the learner cannot drive it
 static const char *action_refusal(const uavrl_learner *l, int) { return l->cfg.n_actions == 27 ? nullptr : "the learner must have 27 actions (the discrete-27 step)"; }
-static const char *action_refusal(const uavrl_sac *, int mean) { return (mean == 0 || mean == 1) ? nullptr : "mean_action must be 0 or 1"; }
+static const char *action_refusal(const uavrl_sac *s, int mean)
+{
+    if (mean != 0 && mean != 1) return "mean_action must be 0 or 1";
+    return (!s->cfg.discrete || s->cfg.act_dim == 27) ? nullptr : "a discrete SAC learner must have act_dim 27 (the discrete-27 step)";
+}
 
 struct EvalBufs { DevMem mem; float *obs = nullptr, *act_f = nullptr; int32_t *act_i = nullptr; };
 
@@ -46,6 +50,10 @@ static int act_step(uavrl_env *env, uavrl_learner *l, EvalBufs &b, int, int, int
 static int act_step(uavrl_env *env, uavrl_sac *s, EvalBufs &b, int mean, int first, int64_t it, cudaStream_t st)
 {
     const uint64_t ctr = kEvalNoiseTag | ((uint64_t)(uint32_t)first << 31) | ((uint64_t)it & 0x7fffffffull);
+    if (s->cfg.discrete) {                                  // a categorical draw on the same counters, or argmax p
+        if (int rc = launch_sacd_act_eval(s, b.obs, env->d.n, mean != 0, ctr, b.act_i, st)) return rc;
+        return launch_env_step(env, UAVRL_ACT_DISCRETE27, b.act_i, b.obs, nullptr, nullptr, nullptr, nullptr, nullptr, st);
+    }
     if (int rc = launch_sac_act_eval(s, b.obs, env->d.n, mean != 0, ctr, b.act_f, st)) return rc;
     return launch_env_step(env, UAVRL_ACT_CONT_F32X2, b.act_f, b.obs, nullptr, nullptr, nullptr, nullptr, nullptr, st);
 }

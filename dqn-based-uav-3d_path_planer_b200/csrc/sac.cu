@@ -18,6 +18,8 @@
 // from blockIdx.y (gridDim.y = G) and offsets its weight images, rows, noise key, log_alpha and scratch by it (sac_g and the
 // helpers after it).
 // sac_federate_kernel is Federated_Learning_AC (Envs/PathPlan_City.py:590-601) across those trainers' actors.
+// A discrete learner (cfg.discrete, SAC_Trainer's IS_Continuous = 0 branch) shares this handle, its Adam, alpha and soft-update
+// steps and its entry points; its four tile kernels live in sac_discrete.cu.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -531,6 +533,18 @@ using namespace uavrl;
 // refuses a configuration before anything is allocated
 static int sac_shape(const uavrl_sac_config &c, SacShape &sh)
 {
+    if (c.discrete != 0 && c.discrete != 1) return fail(UAVRL_ERR_INVALID, "discrete must be 0 (continuous actions) or 1 (discrete actions)");
+    if (c.discrete) {                                          // PolicyNet_SAC / QValueNet_SAC: obs -> hidden -> hidden -> A
+        if (c.act_dim < 2 || c.act_dim > 31) return fail(UAVRL_ERR_INVALID, "a discrete SAC learner's act_dim must be in [2, 31]");
+        if (c.obs_dim <= 0 || c.obs_dim % 4 != 0 || c.obs_dim > kMaxDim)
+            return fail(UAVRL_ERR_INVALID, "a discrete SAC learner's obs_dim must be a multiple of 4 in [4, 128]");
+        if (c.hidden < 1 || c.hidden > kMaxDim) return fail(UAVRL_ERR_INVALID, "hidden must be in [1, 128]");
+        int rc;
+        const int32_t hh[2] = { c.hidden, c.hidden };
+        if ((rc = build_mlp(c.obs_dim, 2, hh, c.act_dim, 0, sh.actor)) || (rc = build_mlp(c.obs_dim, 2, hh, c.act_dim, 0, sh.critic))) return rc;
+        sh.gld = sac_gld(c.hidden);
+        return 0;
+    }
     if (c.act_dim != kSacA) return fail(UAVRL_ERR_INVALID, "act_dim must be 2 (the reference's UAV task)");
     if (c.obs_dim <= 0 || c.obs_dim % 4 != 0) return fail(UAVRL_ERR_INVALID, "obs_dim must be a multiple of 4");
     if (c.obs_dim > kMaxDim - kSacA) return fail(UAVRL_ERR_INVALID, "obs_dim must be at most 124 (the critic input obs_dim + 2 is at most 128)");
@@ -562,6 +576,13 @@ static int sac_smem_total(const SacShape &s, size_t out[5])
         out[i] = dyn[i] + fa.sharedSizeBytes;
     }
     return 0;
+}
+
+// the kernels a learner of configuration c launches: their shared memory per block, *n of them (5 continuous, 4 discrete)
+static int sac_smem_of(const uavrl_sac_config &c, const SacShape &s, size_t out[5], int *n)
+{
+    *n = c.discrete ? 4 : 5;
+    return c.discrete ? sacd_smem_total(s, out) : sac_smem_total(s, out);
 }
 
 static int sac_pack(uavrl_sac *s, int role, cudaStream_t st)
@@ -641,6 +662,39 @@ int uavrl::launch_sac_act_eval(uavrl_sac *s, const float *obs, int n, bool mean,
     return sac_act_launch(s, obs, n, nullptr, ctr, mean, actions, st);
 }
 
+// the discrete tile kernels' view of the learner: B rows per trainer, losses averaged over Bg rows
+static void sacd_fill_args(uavrl_sac *s, SacdArgs &a, const BatchSrc &src, int B, int Bg)
+{
+    memset(&a, 0, sizeof(a));
+    a.actor = s->sh.actor; a.critic = s->sh.critic; a.src = src; a.B = B; a.n_tiles = (B + kTile - 1) / kTile; a.gld = s->sh.gld;
+    a.inv_b = 1.f / (float)Bg; a.gamma = s->cfg.gamma;
+    a.img_actor = s->img[0]; a.img_c1 = s->img[1]; a.img_c2 = s->img[2]; a.img_t1 = s->img[3]; a.img_t2 = s->img[4];
+    a.log_alpha = s->scal; a.td = s->td; a.part_a = s->part[0]; a.part_c1 = s->part[1]; a.part_c2 = s->part[2]; a.stat = s->stat;
+    a.key = s->cfg.seed ^ kNoiseSalt; a.salt = kNoiseSalt;             // the continuous learner's noise stream convention
+}
+
+// the discrete act kernel of every trainer on n rows (G equal blocks) with draw counter ctr, or argmax p
+static int sacd_act_launch(uavrl_sac *s, const float *obs, int n, const float *u, uint64_t ctr, bool mean, int32_t *actions, cudaStream_t st)
+{
+    BatchSrc none;
+    memset(&none, 0, sizeof(none));
+    const int ng = n / s->G;
+    SacdArgs a;
+    sacd_fill_args(s, a, none, ng, ng);
+    a.ctr = ctr;
+    return launch_sacd_act_kernel(a, obs, ng, u, mean, actions, a.n_tiles < s->max_ctas ? a.n_tiles : s->max_ctas, s->G, st);
+}
+
+int uavrl::launch_sacd_act(uavrl_sac *s, const float *obs, int n, const float *u, int32_t *actions, cudaStream_t st)
+{
+    return sacd_act_launch(s, obs, n, u, 0x8000000000000000ull | s->calls++, false, actions, st);
+}
+
+int uavrl::launch_sacd_act_eval(uavrl_sac *s, const float *obs, int n, bool mean, uint64_t ctr, int32_t *actions, cudaStream_t st)
+{
+    return sacd_act_launch(s, obs, n, nullptr, ctr, mean, actions, st);
+}
+
 static int sac_grid(const uavrl_sac *s, int B)
 {
     const int n_tiles = (B + kTile - 1) / kTile;
@@ -712,7 +766,8 @@ static int sac_finish(uavrl_sac *s, int grid, int Bg, bool exchanged, float *los
     memset(&f, 0, sizeof(f));
     f.Pc = s->sh.critic.P; f.nparts = grid; f.img_floats = s->sh.critic.smem_w_floats;
     f.tau = s->cfg.tau; f.alpha_lr = s->cfg.alpha_lr; f.target_entropy = s->cfg.target_entropy;
-    f.inv_n = 1.f / ((float)Bg * (float)kSacA); f.do_alpha = 1;
+    // continuous: every loss is a mean over B x action_dim; discrete: over the B rows (the entropy is one per row)
+    f.inv_n = 1.f / ((float)Bg * (float)(s->cfg.discrete ? 1 : kSacA)); f.do_alpha = 1;
     AdamArgs aa;
     adam_hyper(aa, s->cfg.alpha_lr, s->adam_t);                    // the alpha step's bias corrections
     f.step_size_scale = aa.step_size; f.bc2_sqrt = aa.bc2_sqrt;
@@ -723,9 +778,27 @@ static int sac_finish(uavrl_sac *s, int grid, int Bg, bool exchanged, float *los
     return 0;
 }
 
+// The discrete update (SAC_Trainer.py:380-430): TD targets, both critics' gradients and Adam steps, then the actor on the
+// updated critics and its Adam step, then the alpha step and the soft target update
+static int sacd_update(uavrl_sac *s, const BatchSrc &src, int B, float *losses_dev, cudaStream_t st)
+{
+    const int grid = sac_grid(s, B);
+    int rc = sac_scratch(s, B, grid, st);
+    if (rc) return rc;
+    s->adam_t += 1;
+    SacdArgs a;
+    sacd_fill_args(s, a, src, B, B);
+    if ((rc = launch_sacd_phase(kSacdTarget, a, grid, s->G, st)) || (rc = launch_sacd_phase(kSacdCritic, a, grid, s->G, st)) ||
+        (rc = sac_reduce_adam(s, 1, grid, true, st)) || (rc = sac_reduce_adam(s, 2, grid, true, st)) ||
+        (rc = launch_sacd_phase(kSacdActor, a, grid, s->G, st)) || (rc = sac_reduce_adam(s, 0, grid, true, st)))
+        return rc;
+    return sac_finish(s, grid, B, false, losses_dev, st);
+}
+
 int uavrl::launch_sac_update(uavrl_sac *s, const BatchSrc &src_in, int B, const float *eps_next, const float *eps_cur, float *losses_dev,
                              cudaStream_t st)
 {
+    if (s->cfg.discrete) return sacd_update(s, src_in, B, losses_dev, st);
     const int grid = sac_grid(s, B);
     BatchSrc src = src_in;
     int rc;
@@ -799,13 +872,27 @@ static int sac_alloc(uavrl_sac *s)
     std::vector<float> init(3 * G, 0.f);
     for (size_t g = 0; g < G; ++g) init[3 * g] = logf(0.01f);          // SAC_Trainer.py:53
     UAVRL_CUDA(cudaMemcpy(s->scal, init.data(), init.size() * 4, cudaMemcpyHostToDevice));
-    if (cfg->lockstep_envs > 0 && (rc = s->replay.alloc(cfg->replay_capacity, cfg->lockstep_envs, s->G, cfg->obs_dim, true))) return rc;
+    // the ring holds float[2] actions (continuous) or int32 action indices (discrete)
+    if (cfg->lockstep_envs > 0 && (rc = s->replay.alloc(cfg->replay_capacity, cfg->lockstep_envs, s->G, cfg->obs_dim, !cfg->discrete))) return rc;
+    if (cfg->discrete) return sacd_raise_smem(s->sh);
     if ((rc = raise_dyn_smem(sac_target_kernel<false>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<false, false>, smem_critic(s->sh))) ||
         (rc = raise_dyn_smem(sac_actor_kernel<false>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<false>, smem_act(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<false, true>, smem_act(s->sh))) ||
         (rc = raise_dyn_smem(sac_target_kernel<true>, smem_target(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true, false>, smem_critic(s->sh))) ||
         (rc = raise_dyn_smem(sac_actor_kernel<true>, smem_actor(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<true>, smem_act(s->sh))) || (rc = raise_dyn_smem(sac_act_kernel<true, true>, smem_act(s->sh))) ||
         (rc = raise_dyn_smem(sac_critic_kernel<false, true>, smem_critic(s->sh))) || (rc = raise_dyn_smem(sac_critic_kernel<true, true>, smem_critic(s->sh))))
         return rc;
+    return 0;
+}
+
+// entry points of one action kind only (`what` names the call): refused before anything is enqueued or allocated
+static int refuse_discrete(const uavrl_sac *s, const std::string &what)
+{
+    if (s->cfg.discrete) return fail(UAVRL_ERR_INVALID, what + " is not available on a discrete SAC learner");
+    return 0;
+}
+static int refuse_continuous(const uavrl_sac *s, const std::string &what)
+{
+    if (!s->cfg.discrete) return fail(UAVRL_ERR_INVALID, what + " needs a discrete SAC learner (discrete = 1)");
     return 0;
 }
 
@@ -821,7 +908,8 @@ int uavrl_sac_smem_bytes(const uavrl_sac_config *cfg, int64_t *bytes_out)
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(UAVRL_ERR_CUDA, "no CUDA device: the SAC learner has no CPU fallback");
     UAVRL_CUDA(cudaSetDevice(cfg->device));
     size_t b[5];
-    if ((rc = sac_smem_total(sh, b))) return rc;
+    int nk;
+    if ((rc = sac_smem_of(*cfg, sh, b, &nk))) return rc;
     for (int i = 0; i < 4; ++i) bytes_out[i] = (int64_t)b[i];
     return 0;
 }
@@ -838,8 +926,9 @@ int uavrl_sac_create_trainers(const uavrl_sac_config *cfg, int32_t n_trainers, u
     int rc = sac_shape(*cfg, sh);
     if (rc || (rc = check_trainer_group(*cfg, n_trainers, "SAC learner"))) return rc;
     size_t smem[5];
-    if ((rc = sac_smem_total(sh, smem))) return rc;
-    for (int i = 0; i < 5; ++i)
+    int nk;
+    if ((rc = sac_smem_of(*cfg, sh, smem, &nk))) return rc;
+    for (int i = 0; i < nk; ++i)
         if (smem[i] > kMaxBlockSmem)
             return fail(UAVRL_ERR_INVALID, "networks too large for the SMEM-resident SAC kernels: " + std::to_string(smem[i]) +
                                                " B of shared memory per block, at most " + std::to_string(kMaxBlockSmem));
@@ -954,24 +1043,41 @@ int uavrl_sac_get_scalars(uavrl_sac *s, float *log_alpha, float *la_m, float *la
 int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *eps_dev, float *actions_dev, void *stream)
 {
     if (!s || !obs_dev || !actions_dev || n <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_discrete(s, "uavrl_sac_act (use uavrl_sac_act_discrete)")) return rc;
     if (n % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_act: n must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     return launch_sac_act(s, obs_dev, n, eps_dev, actions_dev, (cudaStream_t)stream);
 }
 
+int uavrl_sac_act_discrete(uavrl_sac *s, const float *obs_dev, int32_t n, const float *u_dev, int32_t mean_action, int32_t *actions_dev,
+                           void *stream)
+{
+    if (!s || !obs_dev || !actions_dev || n <= 0 || (mean_action != 0 && mean_action != 1)) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_continuous(s, "uavrl_sac_act_discrete")) return rc;
+    if (n % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_act_discrete: n must be a multiple of the trainer count");
+    UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    if (mean_action) return launch_sacd_act_eval(s, obs_dev, n, true, 0, actions_dev, (cudaStream_t)stream);
+    return launch_sacd_act(s, obs_dev, n, u_dev, actions_dev, (cudaStream_t)stream);
+}
+
 int uavrl_sac_act_mean(uavrl_sac *s, const float *obs_dev, int32_t n, float *actions_dev, void *stream)
 {
     if (!s || !obs_dev || !actions_dev || n <= 0) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_discrete(s, "uavrl_sac_act_mean (use uavrl_sac_act_discrete with mean_action = 1)")) return rc;
     if (n % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_act_mean: n must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     return launch_sac_act_eval(s, obs_dev, n, true, 0, actions_dev, (cudaStream_t)stream);
 }
 
-static BatchSrc sac_explicit_src(const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev, const float *d_dev)
+// a_dev: float [B][2] (continuous) or int32 [B] (discrete)
+static BatchSrc sac_explicit_src(const uavrl_sac *s, const float *s_dev, const float *a_dev, const float *r_dev, const float *s2_dev,
+                                 const float *d_dev)
 {
     BatchSrc src;
     memset(&src, 0, sizeof(src));
-    src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.act2 = a_dev; src.rew = r_dev; src.done_f32 = d_dev;
+    src.mode = kBatchExplicit; src.frames = s_dev; src.s2_rows = s2_dev; src.rew = r_dev; src.done_f32 = d_dev;
+    if (s->cfg.discrete) src.act = reinterpret_cast<const int32_t *>(a_dev);
+    else src.act2 = a_dev;
     return src;
 }
 
@@ -982,7 +1088,7 @@ int uavrl_sac_update_batch(uavrl_sac *s, int32_t B, const float *s_dev, const fl
     if (B % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_update_batch: B must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;                                             // SAC_Trainer.py:320
-    return launch_sac_update(s, sac_explicit_src(s_dev, a_dev, r_dev, s2_dev, d_dev), B / s->G, eps_next_dev, eps_cur_dev, losses_dev,
+    return launch_sac_update(s, sac_explicit_src(s, s_dev, a_dev, r_dev, s2_dev, d_dev), B / s->G, eps_next_dev, eps_cur_dev, losses_dev,
                              (cudaStream_t)stream);
 }
 
@@ -991,10 +1097,11 @@ int uavrl_sac_update_batch_per(uavrl_sac *s, int32_t B, const float *s_dev, cons
                                const float *eps_cur_dev, float *losses_dev, void *stream)
 {
     if (!s || B <= 0 || !s_dev || !a_dev || !r_dev || !s2_dev || !d_dev || !is_weights_dev) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_discrete(s, "uavrl_sac_update_batch_per (prioritised replay)")) return rc;
     if (B % s->G != 0) return fail(UAVRL_ERR_INVALID, "uavrl_sac_update_batch_per: B must be a multiple of the trainer count");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;                                             // SAC_Trainer.py:320
-    BatchSrc src = sac_explicit_src(s_dev, a_dev, r_dev, s2_dev, d_dev);
+    BatchSrc src = sac_explicit_src(s, s_dev, a_dev, r_dev, s2_dev, d_dev);
     src.is_w = is_weights_dev; src.abs_err = abs_err_out_dev;
     return launch_sac_update(s, src, B / s->G, eps_next_dev, eps_cur_dev, losses_dev, (cudaStream_t)stream);
 }
@@ -1007,6 +1114,7 @@ int uavrl_sac_replay_gather(uavrl_sac *s, int32_t n, const int64_t *idx, float *
     if (!s || n <= 0 || !idx) return fail(UAVRL_ERR_INVALID, "bad argument");
     if (!s->replay.frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
+    if (s->cfg.discrete) return s->replay.gather(n, idx, s_host, reinterpret_cast<int32_t *>(a_host), nullptr, r_host, s2_host, d_host);
     return s->replay.gather(n, idx, s_host, nullptr, a_host, r_host, s2_host, d_host);
 }
 
@@ -1027,6 +1135,7 @@ int uavrl_sac_update_replay(uavrl_sac *s, const int32_t *idx_tape_dev, const flo
 int uavrl_sac_per_enable(uavrl_sac *s, double alpha, double beta0, double beta_inc, double eps, double err_upper)
 {
     if (!s) return fail(UAVRL_ERR_INVALID, "null handle");
+    if (int rc = refuse_discrete(s, "uavrl_sac_per_enable (prioritised replay)")) return rc;
     if (!s->replay.frames) return fail(UAVRL_ERR_STATE, "the SAC learner has no replay ring (lockstep_envs == 0)");
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     return s->replay.per_enable(alpha, beta0, beta_inc, eps, err_upper);
@@ -1119,6 +1228,7 @@ int uavrl_sac_federate_actors_sharded(uavrl_sac *s, void *stream)
 // the refusals every data-parallel update makes before its epoch counts
 static int sac_dp_checks(const uavrl_sac *s, int32_t global_batch, bool ring, const char *fn)
 {
+    if (int rc = refuse_discrete(s, fn)) return rc;
     if (int rc = refuse_grouped(s->G, fn)) return rc;
     if (global_batch <= 0) return fail(UAVRL_ERR_INVALID, std::string(fn) + ": global_batch must be > 0");
     if (s->dp_phase != 0) return fail(UAVRL_ERR_STATE, std::string(fn) + " while a split update waits for its next phase");
@@ -1131,6 +1241,7 @@ static int sac_dp_checks(const uavrl_sac *s, int32_t global_batch, bool ring, co
 int uavrl_sac_comm_init(uavrl_sac *s, int32_t rank, int32_t world, void *handle_out)
 {
     if (!s) return fail(UAVRL_ERR_INVALID, "bad rank/world/handle pointer");
+    if (int rc = refuse_discrete(s, "uavrl_sac_comm_init")) return rc;
     if (int rc = refuse_grouped(s->G, "uavrl_sac_comm_init")) return rc;
     const size_t Pa = (size_t)s->sh.actor.P, Pc = (size_t)s->sh.critic.P;
     return comm_init(s->comm, s->cfg.device, rank, world, 2 * Pc + 2 > Pa + 2 ? 2 * Pc + 2 : Pa + 2, handle_out, true);
@@ -1139,6 +1250,7 @@ int uavrl_sac_comm_init(uavrl_sac *s, int32_t rank, int32_t world, void *handle_
 int uavrl_sac_comm_connect(uavrl_sac *s, const void *handles)
 {
     if (!s || !handles) return fail(UAVRL_ERR_INVALID, "bad argument");
+    if (int rc = refuse_discrete(s, "uavrl_sac_comm_connect")) return rc;
     if (int rc = refuse_grouped(s->G, "uavrl_sac_comm_connect")) return rc;
     if (!s->comm.recv) return fail(UAVRL_ERR_STATE, "uavrl_sac_comm_connect before uavrl_sac_comm_init");
     return comm_connect(s->comm, s->cfg.device, handles, true);
@@ -1188,11 +1300,12 @@ int uavrl_sac_critic_grads_batch(uavrl_sac *s, int32_t B, const float *s_dev, co
     if (int rc = sac_dp_checks(s, global_batch, false, "uavrl_sac_critic_grads_batch")) return rc;
     UAVRL_CUDA(cudaSetDevice(s->cfg.device));
     s->epoch += 1;
-    return sac_split_critic(s, sac_explicit_src(s_dev, a_dev, r_dev, s2_dev, d_dev), B, global_batch, eps_next_dev, (cudaStream_t)stream);
+    return sac_split_critic(s, sac_explicit_src(s, s_dev, a_dev, r_dev, s2_dev, d_dev), B, global_batch, eps_next_dev, (cudaStream_t)stream);
 }
 
 static int sac_phase_is(const uavrl_sac *s, int phase, const char *fn)
 {
+    if (int rc = refuse_discrete(s, fn)) return rc;
     if (int rc = refuse_grouped(s->G, fn)) return rc;
     static const char *want[4] = { "", "after uavrl_sac_critic_grads_*", "after uavrl_sac_apply_critic_grads", "after uavrl_sac_actor_grads" };
     if (s->dp_phase != phase) return fail(UAVRL_ERR_STATE, std::string(fn) + " called out of order: it runs " + want[phase]);

@@ -7,6 +7,35 @@
 namespace uavrl {
 // the two networks of a SAC learner and the stride of its gradient planes: everything the kernels' shared memory follows from
 struct SacShape { NetDev actor, critic; int32_t gld; };
+
+// ------------------------------------------------------------------ discrete branch (IS_Continuous = 0, sac_discrete.cu)
+// PolicyNet_SAC and QValueNet_SAC are both obs -> hidden -> hidden -> A, so the actor and the critics share one plane layout.
+// Every per-trainer array is [G][...] (G = gridDim.y), as in the continuous kernels.
+struct SacdArgs {
+    NetDev actor, critic;
+    BatchSrc src;                        // actions: src.act, int32
+    int32_t B, n_tiles, gld;             // rows per trainer, their tiles, row stride of the gradient planes (sac_gld)
+    float inv_b;                         // 1 / the rows the losses average over
+    float gamma;
+    const float *img_actor, *img_c1, *img_c2, *img_t1, *img_t2;   // [G][smem_w_floats] weight images
+    const float *log_alpha;              // [G][3]
+    float *td;                           // [G][B] TD targets y
+    float *part_a, *part_c1, *part_c2;   // gradient partials [G][grid][P]
+    float *stat;                         // [G][grid][4]: critic-1 sq-err sum, critic-2 sq-err sum, actor-loss sum, entropy sum
+    uint64_t key, ctr;                   // act: Philox key of trainer 0 (trainer g: trainer_key(key, salt, g)) and counter
+    uint64_t salt;
+};
+enum SacdKernel { kSacdTarget = 0, kSacdCritic = 1, kSacdActor = 2, kSacdAct = 3 };
+// dynamic shared memory of one CTA of kernel k for this shape; dynamic + static of all four into out[4]
+size_t sacd_smem_dyn(const SacShape &s, int k);
+int sacd_smem_total(const SacShape &s, size_t out[4]);
+// lift every discrete kernel's dynamic shared-memory limit to what this shape takes
+int sacd_raise_smem(const SacShape &s);
+// one of the update's three tile kernels (k = kSacdTarget, kSacdCritic, kSacdActor) over grid x G CTAs
+int launch_sacd_phase(int k, const SacdArgs &a, int grid, int G, cudaStream_t st);
+// get_action on n rows per trainer: categorical draws (u: [G][n] uniforms, or Philox) or, with mean, argmax p
+int launch_sacd_act_kernel(const SacdArgs &a, const float *obs, int n, const float *u, bool mean, int32_t *actions, int grid, int G,
+                           cudaStream_t st);
 }  // namespace uavrl
 
 // A grouped learner (uavrl_sac_create_trainers) holds G trainers: every per-network vector, weight image and scratch array
@@ -28,7 +57,7 @@ struct uavrl_sac {
     int32_t td_cap = 0, parts_cap = 0, max_ctas = 4 * uavrl::num_sms();
     int64_t epoch = 0, adam_t = 0;
     uint64_t calls = 0;
-    uavrl::ReplayStore replay;                             // lockstep ring (float[2] actions); none when lockstep_envs == 0
+    uavrl::ReplayStore replay;                             // lockstep ring (float[2] actions, int32 when discrete); none when lockstep_envs == 0
     // data-parallel training: the fused exchange's buffers (slots of max(2 Pc + 2, Pa + 2) words), and the split form's
     // phase (0 none, 1 critic gradients written, 2 critics stepped, 3 actor gradients written) with the batch it runs on
     uavrl::PeerComm comm;
@@ -48,6 +77,10 @@ int launch_sac_act(uavrl_sac *s, const float *obs, int n, const float *eps, floa
 // the same pass for an evaluation (eval.cu): noise from counter ctr without advancing the act-call counter, or with mean the
 // policy's mean action tanh(mu) bound
 int launch_sac_act_eval(uavrl_sac *s, const float *obs, int n, bool mean, uint64_t ctr, float *actions, cudaStream_t st);
+// the discrete learner's get_action: int32 actions [n] (u [n] injects the uniforms), on the act-call counter
+int launch_sacd_act(uavrl_sac *s, const float *obs, int n, const float *u, int32_t *actions, cudaStream_t st);
+// the same for an evaluation: draws on counter ctr without advancing the act-call counter, or with mean argmax p
+int launch_sacd_act_eval(uavrl_sac *s, const float *obs, int n, bool mean, uint64_t ctr, int32_t *actions, cudaStream_t st);
 // one SAC_Trainer.update of every trainer on the batch described by src (B rows per trainer); losses_dev (may be null: the
 // learner's own out) receives [G][4]
 int launch_sac_update(uavrl_sac *s, const BatchSrc &src, int B, const float *eps_next, const float *eps_cur, float *losses_dev,

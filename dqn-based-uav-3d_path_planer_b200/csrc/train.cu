@@ -31,6 +31,7 @@ static int act(uavrl_learner *l, const ReplayStore::Iteration &io, int n, float 
 }
 static int act(uavrl_sac *s, const ReplayStore::Iteration &io, int n, float, cudaStream_t st)
 {
+    if (s->cfg.discrete) return launch_sacd_act(s, io.obs_t, n, nullptr, io.act, st);
     return launch_sac_act(s, io.obs_t, n, nullptr, io.act2, st);
 }
 
@@ -44,8 +45,9 @@ static int env_step(uavrl_env *env, uavrl_learner *l, const ReplayStore::Iterati
     l->chain.launched(kChainEnv);
     return 0;
 }
-static int env_step(uavrl_env *env, uavrl_sac *, const ReplayStore::Iteration &io, cudaStream_t st)
+static int env_step(uavrl_env *env, uavrl_sac *s, const ReplayStore::Iteration &io, cudaStream_t st)
 {
+    if (s->cfg.discrete) return launch_env_step(env, UAVRL_ACT_DISCRETE27, io.act, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st);
     return launch_env_step(env, UAVRL_ACT_CONT_F32X2, io.act2, io.obs_next, io.rew, io.done, nullptr, nullptr, nullptr, st);
 }
 
@@ -72,6 +74,15 @@ struct Losses { const float *dev; int stride; };
 static Losses losses(const uavrl_learner *l) { return { l->loss_dev, 1 }; }
 static Losses losses(const uavrl_sac *s) { return { s->out, 4 }; }       // actor, critic 1, critic 2, alpha loss
 
+// the loop refusals of one learner kind; null: none
+static const char *learner_refusal(const uavrl_learner *, Loop) { return nullptr; }
+static const char *learner_refusal(const uavrl_sac *s, Loop loop)
+{
+    if (!s->cfg.discrete) return nullptr;
+    if (loop == kLoopDp) return "uavrl_sac_train_run_dp is not available on a discrete SAC learner";
+    return s->cfg.act_dim == 27 ? nullptr : "a discrete SAC learner in the loop must have act_dim 27 (the discrete-27 step)";
+}
+
 // ------------------------------------------------------------------ the loop
 // The refusals the loops share, each loop's in the order it reports them; nothing is enqueued before they pass.  fn: the entry
 // point, named in the reset refusal.
@@ -80,6 +91,7 @@ static int check_loop(const uavrl_env *env, const Learner *l, Loop loop, int32_t
 {
     const ReplayStore &rs = l->replay;
     const bool paired = rs.mode == kReplayLockstep && l->cfg.lockstep_envs == env->d.n;
+    if (const char *why = learner_refusal(l, loop)) return fail(UAVRL_ERR_INVALID, why);
     if (loop == kLoopDp && l->G > 1) return fail(UAVRL_ERR_INVALID, std::string(fn) + " is not available on a learner with several trainers");
     if (loop != kLoopProfile && !paired) return fail(UAVRL_ERR_INVALID, "learner.lockstep_envs must equal env.n_envs");
     // the env step writes kObsDim floats per env into the ring's frames

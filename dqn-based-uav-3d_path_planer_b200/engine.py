@@ -694,15 +694,22 @@ class SacLearner(_PerCalls):
     lockstep envs split into G blocks of lockstep_envs / G, trainer g learns from its block only and computes what a
     stand-alone SacLearner(seed=seed + g, replay_capacity=replay_capacity // G, lockstep_envs=lockstep_envs // G) computes.
     Parameters are then (G, P) arrays, alpha() is (G, 3), act / update_batch take G equal row blocks and loss tensors hold
-    [G][4] floats (include/uavrl.h, uavrl_sac_create_trainers)."""
+    [G][4] floats (include/uavrl.h, uavrl_sac_create_trainers).
+
+    discrete = True: the reference's IS_Continuous = 0 branch with PolicyNet_SAC / QValueNet_SAC (act_dim = A in [2, 31],
+    obs_dim a multiple of 4 up to 128; include/uavrl.h, "SAC, discrete actions").  act() then returns int32 actions,
+    update_batch and gather take / give int32 action indices, and prioritised replay and the data-parallel calls are
+    refused.  sac_train_run and sac_eval_run drive the 27-action step with it (act_dim 27)."""
     ROLES = ("actor", "critic_1", "critic_2", "target_critic_1", "target_critic_2")
+    discrete = False                    # the action kind, set by __init__
 
     def __init__(self, obs_dim=OBS_DIM, hidden=64, act_dim=2, action_bound=1.0, actor_lr=1e-4, critic_lr=1e-3, alpha_lr=1e-4,
                  target_entropy=1.0, gamma=0.99, tau=0.05, batch_size=64, replay_capacity=10000, lockstep_envs=0, seed=42, device=0,
-                 trainers=1):
+                 trainers=1, discrete=False):
         self.device = torch.device("cuda", device)
+        self.discrete = bool(discrete)
         c = _lib.SacConfig(obs_dim, hidden, act_dim, action_bound, actor_lr, critic_lr, alpha_lr, target_entropy, gamma, tau,
-                           batch_size, replay_capacity, lockstep_envs, seed, device)
+                           batch_size, replay_capacity, lockstep_envs, seed, device, int(self.discrete))
         self.cfg = c
         self.h = C.c_void_p()
         check(_lib.lib().uavrl_sac_create_trainers(C.byref(c), int(trainers), C.byref(self.h)))
@@ -712,8 +719,11 @@ class SacLearner(_PerCalls):
 
     def layout(self, role):
         """(state_dict key, shape) of every tensor of network `role` in flat-parameter order, named as the reference's
-        PolicyNetContinuous_SAC (role 0) and QValueNetContinuous_SAC (roles 1-4: the critics and their targets) name them."""
+        PolicyNetContinuous_SAC (role 0) and QValueNetContinuous_SAC (roles 1-4: the critics and their targets) name them --
+        or, discrete, PolicyNet_SAC and QValueNet_SAC (both fc1, fc2, fc3)."""
         o, h, a = self.cfg.obs_dim, self.cfg.hidden, self.cfg.act_dim
+        if self.discrete:
+            return _linears(("fc1", h, o), ("fc2", h, h), ("fc3", a, h))
         if role == 0:
             return _linears(("fc1", h, o), ("fc_mu", a, h), ("fc_std", a, h))
         return _linears(("fc1", h, o + a), ("fc2", h, h), ("fc_out", a, h))
@@ -822,8 +832,14 @@ class SacLearner(_PerCalls):
     def set_scalars(self, log_alpha, la_m=0.0, la_v=0.0, epoch=0, adam_step=0):
         check(_lib.lib().uavrl_sac_set_scalars(self.h, float(log_alpha), float(la_m), float(la_v), int(epoch), int(adam_step)))
 
-    def act(self, obs, eps=None, mean=False):
-        """SAC_Trainer.get_action on n rows; mean=True: the mean action tanh(mu) bound instead (act_mean)."""
+    def act(self, obs, eps=None, mean=False, u=None):
+        """SAC_Trainer.get_action on n rows; mean=True: the mean action tanh(mu) bound instead (act_mean).  Discrete: int32
+        [n] categorical draws (u: optional device float [n] uniforms), or with mean=True argmax p."""
+        if self.discrete:
+            n = obs.shape[0]
+            a = torch.empty(n, dtype=torch.int32, device=self.device)
+            check(_lib.lib().uavrl_sac_act_discrete(self.h, _ptr(obs), n, _ptr(u), int(bool(mean)), _ptr(a), _stream(self.device)))
+            return a
         if mean:
             return self.act_mean(obs)
         n = obs.shape[0]
@@ -838,6 +854,9 @@ class SacLearner(_PerCalls):
         return a
 
     def update_batch(self, s, a, r, s2, d, eps_next=None, eps_cur=None, losses=None):
+        """One SAC_Trainer.update on device tensors: a is float [B, 2], or int32 [B] action indices on a discrete learner."""
+        if self.discrete and a.dtype != torch.int32:
+            raise ValueError("a discrete SAC learner takes int32 actions, got %s" % a.dtype)
         check(_lib.lib().uavrl_sac_update_batch(self.h, s.shape[0], _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d), _ptr(eps_next),
                                                 _ptr(eps_cur), self._losses(losses), _stream(self.device)))
 
@@ -847,17 +866,18 @@ class SacLearner(_PerCalls):
 
     def smem_bytes(self):
         """Shared memory per block of the target, critic, actor and get_action kernels (see sac_smem_bytes)."""
-        return sac_smem_bytes(self.cfg.obs_dim, self.cfg.hidden, self.cfg.device)
+        return sac_smem_bytes(self.cfg.obs_dim, self.cfg.hidden, self.cfg.device, self.cfg.act_dim, self.discrete)
 
     def replay_size(self):
         return int(_lib.lib().uavrl_sac_replay_size(self.h))
 
     def gather(self, logical_idx):
-        """Transitions of the lockstep ring by logical index (0 = oldest): s, a [n, 2], r, s2, d."""
+        """Transitions of the lockstep ring by logical index (0 = oldest): s, a [n, 2] (discrete: int32 [n]), r, s2, d."""
         idx = np.ascontiguousarray(logical_idx, np.int64)
         n, o = idx.size, self.cfg.obs_dim
         s = np.zeros((n, o), np.float32); s2 = np.zeros((n, o), np.float32)
-        a = np.zeros((n, 2), np.float32); r = np.zeros(n, np.float32); d = np.zeros(n, np.uint8)
+        a = np.zeros(n, np.int32) if self.discrete else np.zeros((n, 2), np.float32)
+        r = np.zeros(n, np.float32); d = np.zeros(n, np.uint8)
         check(_lib.lib().uavrl_sac_replay_gather(self.h, n, _ptr(idx), _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d)))
         return s, a, r, s2, d
 
@@ -942,11 +962,13 @@ class SacLearner(_PerCalls):
         return _DevView(ptr, n.value, self.device).tensor()
 
 
-def sac_smem_bytes(obs_dim, hidden, device=0):
+def sac_smem_bytes(obs_dim, hidden, device=0, act_dim=None, discrete=False):
     """Shared memory (dynamic + static bytes) one block of each SAC kernel takes for these networks: [target, critic update,
-    actor update, get_action].  SacLearner refuses the shape when any exceeds 227 KB (232 448 B)."""
+    actor update, get_action] -- of the discrete kernels with discrete=True (act_dim A, default 27).  SacLearner refuses the
+    shape when any exceeds 227 KB (232 448 B)."""
     c = _lib.SacConfig()
-    c.obs_dim, c.hidden, c.act_dim, c.device = int(obs_dim), int(hidden), 2, int(device)
+    c.obs_dim, c.hidden, c.device, c.discrete = int(obs_dim), int(hidden), int(device), int(bool(discrete))
+    c.act_dim = int(act_dim) if act_dim is not None else (27 if discrete else 2)
     out = np.zeros(4, np.int64)
     check(_lib.lib().uavrl_sac_smem_bytes(C.byref(c), _ptr(out)))
     return [int(x) for x in out]
@@ -987,7 +1009,7 @@ def eval_run(env, learner, n_episodes, first_scenario=0, max_iters=0):
 
 def sac_eval_run(env, sac, n_episodes, first_scenario=0, max_iters=0, mean_action=False):
     """uavrl_sac_eval_run: eval_run for a SAC learner; sampled actions on the evaluation's own noise stream, or with
-    mean_action the mean action tanh(mu) bound."""
+    mean_action the mean action tanh(mu) bound (a discrete learner: categorical draws, or argmax p)."""
     n = int(n_episodes)
     buf = (_lib.EpisodeRecord * max(n, 1))()
     st = _lib.EvalStats()

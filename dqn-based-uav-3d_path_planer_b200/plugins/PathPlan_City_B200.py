@@ -378,8 +378,9 @@ class PathPlan_City_B200:
         self.Reset_Result(eps_rate)
         learner = self.Trainer._learner
         is_sac = isinstance(learner, engine.SacLearner)
-        if is_sac == self.discrete:
-            raise ValueError("SAC needs update_function_name = update_PathPlan (continuous); the DQN family needs update_PathPlan27")
+        if (is_sac and not learner.discrete) == self.discrete:
+            raise ValueError("continuous SAC needs update_function_name = update_PathPlan (continuous); discrete SAC and the DQN "
+                             "family need update_PathPlan27")
         if self.host_driven:
             raise ValueError("run_eposide drives the device-resident lockstep loop: construct without host_driven")
         t0 = time.time()
@@ -457,7 +458,7 @@ class PathPlan_City_B200:
 
     def run_evaluation(self, n_episodes=None, log_dir="logs"):
         """The trained planner on n_episodes (default eval_episodes) held-out scenarios, each once, on the device: greedy for
-        the DQN family, SAC's sampled action (eval_mean_action = 1: its mean action).  Neither the training env nor the
+        the DQN family, SAC's sampled action (eval_mean_action = 1: its mean action; discrete SAC: argmax p).  Neither the training env nor the
         trainer changes.  Returns eval_summary's dict plus the iterations run and the episodes left unfinished; writes one
         CSV row per episode to <log_dir>/eval_<time>.csv (CWD-relative, like the reference's logs) and adds the wall time
         to Agents[0].Testing_time."""

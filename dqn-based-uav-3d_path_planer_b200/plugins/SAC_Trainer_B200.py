@@ -1,5 +1,6 @@
-"""Trainer plug-in: SAC with continuous actions (Trainer/SAC_Trainer.py, the trainer config/Trainer.xml ships) on the
-H100 library.  Constructor takes the reference's parsed Trainer.xml dict (actor / critic / SAC_param sub-dicts)."""
+"""Trainer plug-in: SAC (Trainer/SAC_Trainer.py) on the H100 library -- continuous actions (IS_Continuous = 1, the trainer
+config/Trainer.xml ships) or discrete ones (IS_Continuous = 0 with PolicyNet_SAC / QValueNet_SAC, the 27-action step).
+Constructor takes the reference's parsed Trainer.xml dict (actor / critic / SAC_param sub-dicts)."""
 import os
 
 import numpy as np
@@ -16,17 +17,21 @@ class SAC_Trainer_B200:
 
     def __init__(self, param: dict) -> None:
         actor, critic, sp = param.get('actor'), param.get('critic'), param.get('SAC_param')
-        if int(sp.get('IS_Continuous')) != 1:
-            raise ValueError("SAC_Trainer_B200 implements the continuous-action branch (IS_Continuous = 1)")
-        if actor.get('NetWork') != 'PolicyNetContinuous_SAC' or critic.get('NetWork') != 'QValueNetContinuous_SAC':
-            raise ValueError("SAC_Trainer_B200 needs PolicyNetContinuous_SAC / QValueNetContinuous_SAC")
+        self.IS_Continuous = int(sp.get('IS_Continuous'))
+        if self.IS_Continuous not in (0, 1):
+            raise ValueError("IS_Continuous must be 1 (continuous actions) or 0 (discrete actions)")
+        nets = ('PolicyNetContinuous_SAC', 'QValueNetContinuous_SAC') if self.IS_Continuous else ('PolicyNet_SAC', 'QValueNet_SAC')
+        if (actor.get('NetWork'), critic.get('NetWork')) != nets:
+            raise ValueError("SAC_Trainer_B200 with IS_Continuous = %d needs %s / %s" % (self.IS_Continuous, nets[0], nets[1]))
         self.name = param.get('name')
         self.replay_size = int(None2Value(param.get('replay_size'), 1000))
         self.Batch_Size = int(None2Value(param.get('Batch_Size'), 128))
         self.save_loop = int(None2Value(param.get('save_loop'), 10))
         self.Is_Train = int(None2Value(param.get('Is_Train'), 1))
         self.IsPriority_Replay = int(None2Value(param.get('IsPriority_Replay'), 0))
-        self.IS_Continuous = 1
+        if self.IsPriority_Replay and not self.IS_Continuous:
+            raise ValueError("prioritised replay is not available with IS_Continuous = 0: the reference's discrete update() takes "
+                             "no importance weights")
         self.w, self.hidden, self.act_dim = int(actor.get('w')), int(actor.get('hiden_dim')), int(actor.get('output'))
         self.lockstep_envs = int(None2Value(param.get('lockstep_envs'), 0))
         if self.IsPriority_Replay and self.lockstep_envs == 0:
@@ -39,10 +44,10 @@ class SAC_Trainer_B200:
         G = self.n_trainers
         self.names = checkpoint.trainer_names(self.name, self.lockstep_envs, G, param.get('first_trainer'))
         self._learner = engine.SacLearner(
-            self.w, self.hidden, self.act_dim, float(actor.get('action_bound')), float(actor.get('lr')), float(critic.get('lr')),
-            float(sp.get('alpha_lr')), float(sp.get('target_entropy')), float(sp.get('gamma')), float(sp.get('tau')),
-            batch_size=self.Batch_Size, replay_capacity=self.replay_size * G, lockstep_envs=self.lockstep_envs,
-            seed=int(None2Value(param.get('seed'), 42)), device=self.device_index, trainers=G)
+            self.w, self.hidden, self.act_dim, float(None2Value(actor.get('action_bound'), 1.0)), float(actor.get('lr')),
+            float(critic.get('lr')), float(sp.get('alpha_lr')), float(sp.get('target_entropy')), float(sp.get('gamma')),
+            float(sp.get('tau')), batch_size=self.Batch_Size, replay_capacity=self.replay_size * G, lockstep_envs=self.lockstep_envs,
+            seed=int(None2Value(param.get('seed'), 42)), device=self.device_index, trainers=G, discrete=not self.IS_Continuous)
         self._learner.init_params(int(None2Value(param.get('seed'), 42)))
         if self.IsPriority_Replay:
             # ReplayTree constants (replay_buffer.py:141-148), one tree per trainer as each reference Trainer owns its ReplayTree;
@@ -64,13 +69,16 @@ class SAC_Trainer_B200:
         return self._learner.scalars()["log_alpha"]
 
     def get_action(self, state, eps=0.0):
-        """SAC_Trainer.get_action (:444-448): [a0, a1] for one state, or an [N, 2] array for a batch (with several trainers the
-        [num_UAV, obs] batch: row block g goes to trainer g)."""
+        """SAC_Trainer.get_action (:444-454): [a0, a1] for one state, or an [N, 2] array for a batch (with several trainers the
+        [num_UAV, obs] batch: row block g goes to trainer g).  IS_Continuous = 0: an int action index for one state, or an
+        [N] int32 array -- a draw from Categorical(actor(s)); eps is ignored, as the reference ignores it."""
         s = np.ascontiguousarray(state, np.float32)
         single = s.ndim == 1
         if single and self.n_trainers > 1:
             raise ValueError("get_action with %d trainers takes the [num_UAV, %d] batch, not one state" % (self.n_trainers, self.w))
         a = self._learner.act(torch.from_numpy(s.reshape(-1, self.w)).to(self._dev)).cpu().numpy()
+        if not self.IS_Continuous:
+            return int(a[0]) if single else a
         return a[0].tolist() if single else a
 
     def attach_dist(self, dist, rank, world):
@@ -83,7 +91,8 @@ class SAC_Trainer_B200:
             self._xvec = (self._learner.exchange_tensor(0), self._learner.exchange_tensor(1))
 
     def update(self, transition_dict):
-        """SAC_Trainer.update (:317-441), continuous branch, on the batch in transition_dict."""
+        """SAC_Trainer.update (:317-441) on the batch in transition_dict: the continuous branch, or with IS_Continuous = 0 the
+        discrete one (int action indices in 'actions')."""
         states = transition_dict['states']
         if all(len(sub) == 0 for sub in states) if isinstance(states, list) else len(states) == 0:      # :322-324
             sc = self._learner.scalars()
@@ -92,7 +101,10 @@ class SAC_Trainer_B200:
         dev = self._dev
         f = lambda x, shape: torch.as_tensor(np.asarray(x, np.float32).reshape(shape)).to(dev)  # noqa: E731
         s = f(states, (-1, self.w)); s2 = f(transition_dict['next_states'], (-1, self.w))
-        a = f(transition_dict['actions'], (-1, self.act_dim))
+        if self.IS_Continuous:
+            a = f(transition_dict['actions'], (-1, self.act_dim))
+        else:
+            a = torch.as_tensor(np.asarray(transition_dict['actions']).astype(np.int32).reshape(-1)).to(dev)
         r = f(transition_dict['rewards'], (-1,)); d = f(transition_dict['dones'], (-1,))
         wts, idx = transition_dict.get('weights'), transition_dict.get('idx')
         if wts is not None:
@@ -107,6 +119,8 @@ class SAC_Trainer_B200:
                 shape = (-1,) if self.n_trainers == 1 else (self.n_trainers, -1)
                 self._learner.per_set_errors(torch.as_tensor(slots.astype(np.int32).reshape(shape)).to(dev), ae.reshape(shape), clip=True)
         elif self._world > 1:
+            if not self.IS_Continuous:
+                raise ValueError("the data-parallel update is not available with IS_Continuous = 0: train with world = 1")
             L, dist = self._learner, self._dist
             L.critic_grads(s.shape[0] * self._world, batch=(s, a, r, s2, d))
             dist.all_reduce(self._xvec[0], op=dist.ReduceOp.SUM)

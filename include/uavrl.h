@@ -445,6 +445,7 @@ typedef struct {
     int32_t lockstep_envs;                /* > 0: frame-ring replay fed by uavrl_sac_train_run */
     uint64_t seed;
     int32_t device;
+    int32_t discrete;                     /* 0: continuous actions (IS_Continuous = 1); 1: discrete actions (IS_Continuous = 0) */
 } uavrl_sac_config;
 
 /* Limits: obs_dim a multiple of 4 in [4, 124] (the critic input obs_dim + 2 is at most 128), hidden in [1, 128], and every
@@ -507,6 +508,49 @@ int uavrl_sac_get_alpha(uavrl_sac *s, float *alpha_host);
 /* SAC_Trainer.get_action (:444-448): actions_dev [n][2] = tanh(mu + sigma*eps)*bound; eps_dev [n][2] injects the
  * reparameterisation noise (NULL = Philox Box-Muller) */
 int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *eps_dev, float *actions_dev, void *stream);
+
+/* ------------------------------------------------------------------ SAC, discrete actions (discrete = 1)
+ * SAC_Trainer with <IS_Continuous>0</IS_Continuous> (Trainer/SAC_Trainer.py:380-430, calc_target :133-141, get_action
+ * :449-454) and PolicyNet_SAC / QValueNet_SAC (BaseClass/BaseCNN.py:296-343):
+ *   actor   fc1 -> ReLU -> fc2 -> ReLU -> fc3 -> softmax over A       (obs -> hidden -> hidden -> A)
+ *   critic  fc1 -> ReLU -> fc2 -> ReLU -> fc3, the A Q-values of s      (no action input), two of them and two targets
+ * log_alpha starts at ln 0.01 with its own Adam (alpha_lr); there is no actor target.  One update on B rows (s, a in [0, A),
+ * r, s', d), every float computed in fp32:
+ *   1. reward shaping, a reference quirk kept (:390): r~ = (r + 10) / 10, inside the update only -- the ring, the env
+ *      statistics and the episode records keep raw rewards;
+ *   2. target: p' = actor(s'), H' = -sum_j p'_j log(p'_j + 1e-8) (the +1e-8 inside the log is the reference's),
+ *      m' = sum_j p'_j min(Q1t(s'), Q2t(s'))_j, y = r~ + gamma (m' + alpha H') (1 - d), alpha = exp(log_alpha) before this
+ *      update's alpha step;
+ *   3. critics: L_k = mean_b (Q_k(s)[a_b] - y_b)^2; each critic takes its own Adam step -- BEFORE the actor's leg (kept);
+ *   4. actor, on the UPDATED critics: p = actor(s), H and m as in 2 on s, L_pi = mean(-alpha H - m); gradients flow through p
+ *      only: dL/dp_j = (alpha (log(p_j + 1e-8) + p_j / (p_j + 1e-8)) - min_j) / B, then the softmax Jacobian;
+ *   5. alpha: L_alpha = mean((H - target_entropy) alpha), the gradient taken with respect to log_alpha, Adam on log_alpha;
+ *   6. both targets move by tau toward the updated critics.
+ * losses_dev receives {actor loss, critic 1 loss, critic 2 loss, d L_alpha / d log_alpha}, as the continuous learner's.
+ * get_action: Categorical(actor(s)).sample(), epsilon ignored (Choose_Action2 -> get_action ignores it).  On the device: one
+ * uniform u in [0, 1) per row -- Philox word 0 on the learner's act-call counter, the stream uavrl_sac_act draws its noise on
+ * (key seed ^ 0x5AC5, trainer g: seed + g), or an injected tape -- then the smallest k with u sum(p) < p_0 + ... + p_k
+ * (summed left to right in fp32), or, if rounding leaves none, the last k with p_k > 0.  The deterministic policy
+ * (mean_action = 1) is argmax p, the lowest index on ties.
+ * Limits: act_dim = A in [2, 31] (one 32-column head plane), obs_dim a multiple of 4 in [4, 128], hidden in [1, 128], and every
+ * kernel's shared memory at most 227 KB (the shipped 100-64-64-27 fits: uavrl_sac_smem_bytes reports the four discrete
+ * kernels, target, critic update, actor update, get_action).  Refused with UAVRL_ERR_INVALID before anything is allocated.
+ * What changes against the continuous learner:
+ *   - roles, uavrl_sac_param_count, set/get_params, alpha, scalars, grouped trainers and the actor aggregation keep their
+ *     meaning; the flat layouts are actor = fc1, fc2, fc3 and critic = fc1, fc2, fc3 (state_dict order);
+ *   - uavrl_sac_update_batch / uavrl_sac_critic_grads_batch take a_dev as int32 [B] action indices; the ring holds int32
+ *     actions and uavrl_sac_replay_gather writes a_host as int32 [n];
+ *   - uavrl_sac_act_discrete acts (below); uavrl_sac_act and uavrl_sac_act_mean are refused (UAVRL_ERR_INVALID);
+ *   - uavrl_sac_train_run acts with the discrete kernel and steps the env with UAVRL_ACT_DISCRETE27, and refuses
+ *     (UAVRL_ERR_INVALID) a learner whose act_dim is not 27; uavrl_sac_eval_run does the same, mean_action selecting argmax;
+ *   - refused with UAVRL_ERR_INVALID (the reference's discrete update() has no importance weights; a data-parallel discrete
+ *     update is not provided): prioritised replay (uavrl_sac_per_enable, uavrl_sac_update_batch_per) and every data-parallel
+ *     call (uavrl_sac_comm_init / _connect, uavrl_sac_update_replay_dp, uavrl_sac_train_run_dp, the split calls). */
+/* get_action of a discrete learner on n rows in G equal blocks: actions_dev int32 [n].  u_dev (may be NULL) [n] injects the
+ * uniforms; else Philox on the act-call counter.  Either way the call advances the counter by one, as uavrl_sac_act does.  mean_action = 1: argmax p, drawing nothing and leaving
+ * the counter as it is.  Refused on a continuous learner. */
+int uavrl_sac_act_discrete(uavrl_sac *s, const float *obs_dev, int32_t n, const float *u_dev, int32_t mean_action, int32_t *actions_dev,
+                           void *stream);
 /* SAC_Trainer.update (:317-379, continuous) on an explicit batch: s [B][obs], a [B][2], r [B], s2 [B][obs], d [B];
  * eps_next / eps_cur [B][2] = noise of the two actor evaluations (NULL = Philox); losses_dev (optional) [4] =
  * {actor_loss, critic_1_loss, critic_2_loss, d alpha_loss / d log_alpha}. */
