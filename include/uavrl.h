@@ -538,8 +538,8 @@ int uavrl_sac_act(uavrl_sac *s, const float *obs_dev, int32_t n, const float *ep
  * What changes against the continuous learner:
  *   - roles, uavrl_sac_param_count, set/get_params, alpha, scalars, grouped trainers and the actor aggregation keep their
  *     meaning; the flat layouts are actor = fc1, fc2, fc3 and critic = fc1, fc2, fc3 (state_dict order);
- *   - uavrl_sac_update_batch / uavrl_sac_critic_grads_batch take a_dev as int32 [B] action indices; the ring holds int32
- *     actions and uavrl_sac_replay_gather writes a_host as int32 [n];
+ *   - uavrl_sac_update_batch takes a_dev as int32 [B] action indices; the ring holds int32 actions and
+ *     uavrl_sac_replay_gather writes a_host as int32 [n];
  *   - uavrl_sac_act_discrete acts (below); uavrl_sac_act and uavrl_sac_act_mean are refused (UAVRL_ERR_INVALID);
  *   - uavrl_sac_train_run acts with the discrete kernel and steps the env with UAVRL_ACT_DISCRETE27, and refuses
  *     (UAVRL_ERR_INVALID) a learner whose act_dim is not 27; uavrl_sac_eval_run does the same, mean_action selecting argmax;

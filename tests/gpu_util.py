@@ -132,6 +132,28 @@ def short_episode_env(env_golden, env27_golden):
     return city, engine.UavParams(p[0], p[1], p[2], float(env27_golden["climb_rate"]), MAX_STEP)
 
 
+# ------------------------------------------------------------------ policy evaluation
+def compose(env, n, first, act):
+    """uavrl_eval_run / uavrl_sac_eval_run's suite through existing calls: auto-reset with stride N, records on, act on all N rows every iteration."""
+    env.set_reset_stride(env.n)
+    env.set_records(n)
+    env.reset(first)
+    obs = env.observe()
+    for it in range(100000):
+        a, kind = act(obs)
+        obs = env.step(a, kind=kind)["obs"]
+        if it % 16 == 15 and env.records(clear=False)["slot"].size >= n:
+            break
+    rec = env.records(clear=False)
+    assert list(rec["slot"][:n]) == list(range(n))
+    return {k: rec[k][:n] for k in engine.RECORD_FIELDS}
+
+
+def assert_records_equal(got, want, what):
+    for k in engine.RECORD_FIELDS:
+        assert_same(got[k], want[k], "%s: %s" % (what, k))
+
+
 def ring_env(city, params, n, pool, first):
     env = engine.EnvBatch(city, params, n, max_subgoals=64, auto_reset=True)
     env.set_pool(pool["start"], pool["goal"], pool["heading"], pool["sub"], pool["n_sub"])

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_util import MAX_STEP, assert_same, dev, learner, sac, short_episode_env, standalone_like
+from gpu_util import MAX_STEP, assert_records_equal, assert_same, compose, dev, learner, sac, short_episode_env, standalone_like
 from sac_restatement import actor_fwd, init_state, unpack
 from uavrl_b200 import _lib, engine
 
@@ -98,27 +98,6 @@ def test_record_fields(env_golden, env27_golden, kind, extras):
 
 
 # ------------------------------------------------------------------ 2. composition
-def compose(env, n, first, act):
-    """The suite through existing calls: auto-reset with stride N, records on, act on all N rows every iteration."""
-    env.set_reset_stride(env.n)
-    env.set_records(n)
-    env.reset(first)
-    obs = env.observe()
-    for it in range(100000):
-        a, kind = act(obs)
-        obs = env.step(a, kind=kind)["obs"]
-        if it % 16 == 15 and env.records(clear=False)["slot"].size >= n:
-            break
-    rec = env.records(clear=False)
-    assert list(rec["slot"][:n]) == list(range(n))
-    return {k: rec[k][:n] for k in FIELDS}
-
-
-def assert_records_equal(got, want, what):
-    for k in FIELDS:
-        assert_same(got[k], want[k], "%s: %s" % (what, k))
-
-
 @gpu
 @pytest.mark.parametrize("route", ["fp32", "tc"])
 def test_eval_equals_composition(env_golden, env27_golden, route):

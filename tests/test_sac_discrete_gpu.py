@@ -11,8 +11,8 @@ from scipy import stats
 import replay_restatement as R
 from conftest import GOLDEN
 from gpu_util import assert_same, city_and_params, dev
-from sac_discrete_restatement import (HP, categorical_pick, clean_batch, init_state, pick_margin, read_state, sacd_update64, softmax,
-                                      unpack, mlp_fwd, check_step)
+from sac_discrete_restatement import (HP, categorical_pick, clean_batch, init_state, pick_margin, read_state, sacd_update64, set_state,
+                                      softmax, unpack, mlp_fwd, check_step)
 
 pytestmark = pytest.mark.gpu
 SMEM_MAX = 232448
@@ -27,12 +27,6 @@ def engine():
 def sacd(obs=100, hid=64, A=27, **kw):
     kw.setdefault("batch_size", 64)
     return engine().SacLearner(obs_dim=obs, hidden=hid, act_dim=A, discrete=True, **HP, **kw)
-
-
-def set_state(S, st):
-    for role, k in enumerate(("actor", "c1", "c2", "t1", "t2", "actor_m", "c1_m", "c2_m", "actor_v", "c1_v", "c2_v")):
-        S.set_params(role, st[k].astype(np.float32))
-    S.set_scalars(st["log_alpha"], st["la_m"], st["la_v"], 0, st["step"])
 
 
 def widest_hidden(obs, A):
